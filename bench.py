@@ -1,20 +1,29 @@
 #!/usr/bin/env python
-"""bench.py -- reads/sec of the alignment hot path (150 bp reads vs the 8 bundled rRNA databases).
+"""bench.py -- reads/sec of the alignment hot path (150 bp reads vs 8 rRNA-database-shaped references).
 
-  python bench.py [--gpus N] [--steps K] [--warmup W] [--reads R] [--impl ours|reference]
+  python bench.py [--gpus N] [--steps K] [--warmup W] [--reads R] [--impl ours|reference] [--dump-outputs DIR]
 
-A "step" is one pass of the hot path over one batch of R synthetic reads per GPU (default: BASELINE.json
-config "10 M synthetic 150 bp Illumina reads vs all 8 data/rRNA_databases refs, 1xB200").
+A "step" is one pass of the hot path over one batch of R/K synthetic reads per GPU (default: BASELINE.json
+config "10 M synthetic 150 bp Illumina reads vs all 8 data/rRNA_databases refs", on one H100).  The 8 databases are the
+seeded stand-ins of tools/synth_databases.py (same sequence counts and lengths as the bundled ones), written and indexed in
+a temporary directory: the run needs nothing outside the repository and writes nothing into it.
   value  : whole-job reads/s, kernels only, batch resident in HBM (CUDA events inside the C ABI)
   e2e    : reads/s through smr_align_batch with pinned HOST buffers (H2D + kernels + D2H inside the timed region)
-  roofline: the seed-search kernel (dominant) against the measured HBM peak
-  cpu_baseline: the reference CPU build (oracle/_ref/sortmerna_ref), all host threads, bounded sample
+  roofline: the candidate kernel (dominant) against the measured DPX rate, the seed-search kernel against the HBM peak
+  cpu_baseline: the reference CPU build (oracle/_ref/sortmerna_ref, where built), all host threads, bounded sample.  It runs on the
+           index the reference's own builder makes, built afresh in the temporary directory on every run (one single-threaded
+           builder per database, all 8 in parallel: about a minute of untimed set-up on an 8-core host; reported as
+           cpu_baseline.reference_index_build_s).  --no-cpu-baseline skips both.
 --impl reference times that same reference build only (rank 0), one bounded sample per step.
+--dump-outputs DIR writes what the last timed step returned (per-read state, stored alignments, CIGARs, counters) for a
+fixed, seeded sample of its reads as float64 .npy files.
 """
 import argparse
+import atexit
 import json
 import os
 import re
+import shutil
 import subprocess
 import sys
 import tempfile
@@ -27,7 +36,7 @@ ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
 
 from sortmerna_b200 import hostio  # noqa: E402
-from tools import stage_data  # noqa: E402
+from tools import stage_data, synth_databases  # noqa: E402
 
 READ_LEN = 150
 GEN_SEED = 20260924
@@ -155,15 +164,12 @@ def write_fastq(path, reads):
 
 
 # ------------------------------------------------------------------------------------------------
-def load_databases(native_index=True):
-    stage_data.stage_inputs() if os.path.isdir(stage_data.REF_DATA) else None
-    fastas = [stage_data.db_path(n) for n in stage_data.DBS]
-    missing = [f for f in fastas if not os.path.exists(f)]
-    if missing:
-        raise SystemExit(f"missing database FASTA files {missing}: run tools/stage_data.py where /root/reference exists")
+def load_databases(work, native_index=True):
+    """The 8 seeded stand-in databases, written under `work` (a temporary directory) and indexed there."""
+    fastas = synth_databases.write(os.path.join(work, "rRNA_databases"))
     if not native_index:
         return fastas, None, None, [hostio.load_references(f) for f in fastas], None, {}
-    idx_dir, built = stage_data.ensure_indexes(fastas)   # smr_build_index (our builder), 8 databases in parallel
+    idx_dir, built = stage_data.ensure_indexes(fastas, os.path.join(work, "idx"))   # smr_build_index (our builder), 8 databases in parallel
     pre = hostio.find_index_prefixes(idx_dir)
     refs = [hostio.load_references(f) for f in fastas]
     stats = [hostio.parse_stats(pre[os.path.basename(f)]) for f in fastas]
@@ -199,10 +205,10 @@ def survey_8d_seed(fastas, prefixes, refs, ms, stats, reads03, threads, reads_pe
             "sample": f"oracle walk (reference pass schedule + pruned DFS) on the first {n} reads of the workload, 8 databases"}
 
 
-def reference_index_dir(fastas):
+def reference_index_dir(work, fastas):
     """The reference legs (cpu_baseline, --impl reference) run the unmodified binary on the index ITS OWN builder makes
-    (data_cache/idx_ref; one process per database, outside every timed region) -- never on files our builder wrote."""
-    d, _ = stage_data.ensure_indexes(fastas, os.path.join(stage_data.CACHE, "idx_ref"), builder="reference")
+    (<work>/idx_ref; one process per database, outside every timed region) -- never on files our builder wrote."""
+    d, _ = stage_data.ensure_indexes(fastas, os.path.join(work, "idx_ref"), builder="reference")
     return d
 
 
@@ -213,7 +219,7 @@ def minimal_scores(stats, fastas, nreads_total):
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (read only)."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -239,7 +245,18 @@ class ClockSampler(threading.Thread):
         for i, n in enumerate(("hw_slowdown", "hw_thermal_slowdown", "sw_thermal_slowdown", "sw_power_cap")):
             if any(len(r) > 3 + i and r[3 + i].lower().startswith("active") for r in self.rows):
                 reasons.append(n)
-        return dict(sm_mhz=float(np.median(sm)) if sm else None, sm_max_mhz=max(mx) if mx else None, reasons=reasons, samples=len(self.rows))
+        return dict(sm_mhz=float(np.median(sm)) if sm else None, sm_max_mhz=max(mx) if mx else None, reasons=reasons, samples=len(self.rows),
+                    **card(self.dev))
+
+
+def card(dev):
+    """Name and power limit of the GPU the numbers were measured on (nvidia-smi, read only)."""
+    try:
+        o = subprocess.run(["nvidia-smi", "-i", str(dev), "--query-gpu=name,power.limit", "--format=csv,noheader,nounits"],
+                           stdout=subprocess.PIPE, text=True, timeout=10).stdout.strip().split(",")
+        return dict(gpu=o[0].strip(), power_limit_w=float(o[1]))
+    except Exception:
+        return dict(gpu=None, power_limit_w=None)
 
 
 def run_reference_sample(fastas, idx_dir, reads, threads):
@@ -288,15 +305,15 @@ def host_cores():
     return eff, dict(os_cpu_count=ncpu, affinity=aff, cgroup_quota=quota, threads_used=eff, loadavg_1m=load)
 
 
-def cli_e2e(args, cores, core_info):
+def cli_e2e(args, cores, core_info, work):
     """What a user runs: the reference's host program with the binding (oracle/_ref/sortmerna_gpu -ref x8 -reads file.fq) against
     the unmodified reference binary on the same file -- 'Done alignment' seconds and total wall, flat FASTQ (and .gz with
     --cli-gz).  The CPU binary gets a bounded prefix of the same file (its cost is linear in reads)."""
     import gzip
     import shutil
     from oracle import ora
-    fastas, idx_dir, _, refs, _, _ = load_databases()
-    ref_idx = reference_index_dir(fastas)
+    fastas, idx_dir, _, refs, _, _ = load_databases(work)
+    ref_idx = reference_index_dir(work, fastas)
     pool = DbPool(refs)
     n = args.cli_reads
     gpu_bin = os.path.join(ROOT, "oracle", "_ref", "sortmerna_gpu")
@@ -351,7 +368,39 @@ def peaks():
     if os.path.exists(p):
         j = json.load(open(p))
         return float(j["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "data sheet (H100 SXM HBM3, 3.35 TB/s; not reached by any measurement here)"
+
+
+DUMP_READS = 1 << 17        # reads of the last timed step written by --dump-outputs (a fixed, seeded sample)
+
+
+def dump_outputs(d, res, n):
+    """What the last timed step returned to its caller, for DUMP_READS reads picked with a fixed seed: every field of the
+    per-read state and of the stored alignments, the CIGAR words of those alignments, and the step's counters.  float64
+    holds every integer the library returns exactly; about 25 MB in all at the default sample."""
+    os.makedirs(d, exist_ok=True)
+    pick = np.sort(np.random.default_rng(GEN_SEED).choice(n, min(n, DUMP_READS), replace=False))
+    slots = int(res["slots"])
+    out = {"read_index": pick}
+    for f in res["res"].dtype.names:
+        out["read_" + f] = res["res"][f][pick]
+    alns = res["alns"].reshape(n, slots)[pick].reshape(-1)
+    for f in alns.dtype.names:
+        if f not in ("pad", "cigar_off"):
+            out["aln_" + f] = alns[f]
+    live = alns["cigar_len"] > 0
+    cig = res["cigar"]
+    out["aln_cigar"] = np.concatenate([cig[int(o):int(o) + int(k)] for o, k in zip(alns["cigar_off"][live], alns["cigar_len"][live])]
+                                      or [np.zeros(0, np.uint32)])
+    out["counters"] = np.array([res["counters"][k] for k in DUMP_COUNTERS] + [int(x) for x in res["matched"]])
+    for k, v in out.items():
+        np.save(os.path.join(d, k + ".npy"), np.asarray(v, dtype=np.float64))
+
+
+# counters both kernel instantiations produce (the instrumented pass is checked against them)
+CHECKED_COUNTERS = ("num_aligned", "sw_calls", "sw_cells", "pos_entries", "lis_calls", "spec_calls")
+# counters that depend on the inputs alone (the speculative ones depend on the order the warps ran in), then reads aligned per database
+DUMP_COUNTERS = ("num_aligned", "num_short", "sw_calls", "sw_cells", "pos_entries", "lis_calls")
 
 
 def main():
@@ -371,7 +420,13 @@ def main():
     ap.add_argument("--cli-cpu-reads", type=int, default=100_000)
     ap.add_argument("--cli-gpus", type=int, default=1)
     ap.add_argument("--cli-gz", action="store_true")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help=f"write what the last timed step returned for {DUMP_READS} seeded-sampled reads as DIR/<name>.npy (float64)")
     args = ap.parse_args()
+    if args.steps < 1:
+        ap.error("--steps must be at least 1")
+    work = tempfile.mkdtemp(prefix="smr_bench_")      # databases, indexes, reference runs: never inside the repository
+    atexit.register(shutil.rmtree, work, True)
     # stdout carries exactly ONE JSON line: everything else that writes to fd 1 (NCCL's version banner, library chatter) goes to stderr
     sys.stdout.flush()
     json_fd = os.dup(1)
@@ -386,14 +441,14 @@ def main():
     cores, core_info = host_cores()
 
     if args.cli_e2e:
-        emit({"cli_e2e": cli_e2e(args, cores, core_info)})
+        emit({"cli_e2e": cli_e2e(args, cores, core_info, work)})
         return
 
     if args.impl == "reference":
         if rank != 0:
             return
-        fastas, _, _, refs, _, _ = load_databases(native_index=False)
-        idx_dir = reference_index_dir(fastas)
+        fastas, _, _, refs, _, _ = load_databases(work, native_index=False)
+        idx_dir = reference_index_dir(work, fastas)
         pool = DbPool(refs)
         # ~10 s of reference CPU time per step (about 230 reads/s per core on this workload): large enough that thread start-up
         # and the skew between the reference's static per-thread splits do not dominate (round 1: 300 reads per thread did)
@@ -412,7 +467,7 @@ def main():
             "metric": METRIC, "value": v, "unit": "reads/s", "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup,
             "ms_per_step": 1000.0 * float(np.mean(secs)), "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
             "dtype": "int16/u8 (SSE2)", "data": "synthetic", "impl": "reference",
-            "config": {"workload": "10 M synthetic 150 bp Illumina reads vs all 8 data/rRNA_databases refs, 1xB200",
+            "config": {"workload": "10 M synthetic 150 bp Illumina reads vs the 8 seeded stand-ins of data/rRNA_databases",
                        "sampled": "each step is a bounded sample of that workload (reads_per_step reads, same generator)",
                        "reads_per_step": sample, "read_len": READ_LEN, "databases": 8},
             "cpu_baseline": {"value": v, "unit": "reads/s", "cores": cores, "kind": "reference", "sample": desc, "host": core_info,
@@ -428,11 +483,7 @@ def main():
         torch.cuda.set_device(local_rank)
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     t_setup = time.time()
-    if world > 1:       # the index cache is built once (rank 0), the other ranks wait and then only read it
-        if rank == 0:
-            load_databases()
-        dist.barrier()
-    fastas, idx_dir, prefixes, refs, stats, built = load_databases()
+    fastas, idx_dir, prefixes, refs, stats, built = load_databases(work)
     n_job = args.reads
     n = max(1, n_job // args.steps)                   # reads per step (batch) per GPU
     ms = minimal_scores(stats, fastas, n_job * world)  # refstats totals stay GLOBAL across shards (SURVEY 8(e))
@@ -454,6 +505,7 @@ def main():
         pins.append(pin); cats.append(c)
         if s_i == 0:
             first_reads = reads
+    torch.cuda.empty_cache()      # the generator's scratch goes back to the device: the library's two contexts allocate next
     pin_off = torch.empty(n + 1, dtype=torch.int64, pin_memory=True)
     off = pin_off.numpy().view(np.uint64); off[:] = np.arange(n + 1, dtype=np.uint64) * READ_LEN
     setup_s = time.time() - t_setup
@@ -486,6 +538,8 @@ def main():
     wall_ms = (time.perf_counter() - t0) * 1000.0
     sampler.stop_flag = True; sampler.join(timeout=2)
     step_ms = float(np.sum(dev_ms))          # CUDA events on the library's stream, summed over the K steps
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, res, n)
     # ---- the same K batches once more, UNTIMED, through the instrumented instantiations of the kernels (smr_set_instrumentation):
     #      the seed-side counters (windows, lists, entries) and the cycle shares of the candidate kernel's roles come from this pass;
     #      the timed passes above run the product's kernels, which carry neither ----
@@ -499,7 +553,7 @@ def main():
             res = al.download()
             vec_s = np.array([res["counters"][k] for k in api.CNT_NAMES], dtype=np.int64)
             csum_i = vec_s if csum_i is None else csum_i + vec_s
-        for k in ("num_aligned", "sw_calls", "sw_cells", "pos_entries", "lis_calls", "spec_calls"):   # what both instantiations count must agree
+        for k in CHECKED_COUNTERS:   # what both instantiations count must agree
             i = api.CNT_NAMES.index(k)
             if int(csum[i]) != int(csum_i[i]):
                 instr_mismatch.append({"counter": k, "product": int(csum[i]), "instrumented": int(csum_i[i])})
@@ -537,6 +591,8 @@ def main():
         res_all = list(ex.map(one, range(e2e_steps)))
     barrier()
     e2e_s = time.perf_counter() - t0
+    free_b, total_b = torch.cuda.mem_get_info(local_rank)      # both contexts, their indexes and buffers still allocated
+    device_mem_used_gb = round((total_b - free_b) / 2**30, 2)
     h2d = int(cats[0].nbytes + off.nbytes)
     slots = res_all[-1][0]
     d2h = int(n * (28 + 4 + 2) + n * slots * 40 + res_all[-1][1] + 8 * 80)
@@ -573,25 +629,13 @@ def main():
     sw_kernel_rate = cells_per_rank / lis_s / 1e12 if lis_s > 0 else 0.0            # whole kernel (votes, LIS, ... included)
     sw_exec_rate = exec_cells_per_rank / lis_s / 1e12 if lis_s > 0 else 0.0
     sw_peak = dpx / 3.5 / 1e3                        # Tcell-updates/s
-    tr = {}
-    try:
-        cands = [os.path.join(ROOT, "profiles", f) for f in ("r2c_traffic.json", "r2b_traffic.json", "r2_traffic.json")]   # the newest committed capture
-        tr = json.load(open(next(f for f in cands if os.path.exists(f))))
-    except Exception:
-        pass
-    def _traffic(kernel):   # ncu DRAM bytes of the committed capture, scaled to the reads of one launch of this run
-        if kernel in tr and tr.get("reads_in_captured_launch"):
-            return int(tr[kernel]["dram_bytes"] * n / tr["reads_in_captured_launch"])
-        return None
     roof_sw = {"bound": "integer (alu pipe, DPX)", "kernel": "lis_kernel (candidates + Smith-Waterman score pass)",
                "achieved": sw_kernel_rate, "peak": sw_peak, "unit": "Tcell-updates/s", "frac": sw_kernel_rate / sw_peak if sw_peak else None,
-               "traffic": _traffic("lis_kernel"), "traffic_unit": "DRAM bytes per launch (ncu capture scaled by reads per launch)",
                "executed_incl_speculation": sw_exec_rate, "speculation_overhead": (exec_cells_per_rank / cells_per_rank - 1.0) if cells_per_rank else None,
                "planner_wait_share": counters["cyc_wait"] / max(1, counters["dbg_sum_read_cycles"]),
                "peak_source": f"measured now: {dpx:.0f} G dependent-free VIADDMNMX thread-ops/s (smr_debug_dpx_peak) / 3.5 such instructions per cell",
                "cells_per_step": int(cells_per_rank / args.steps), "kernel_ms_per_step": float(np.mean(lis_ms))}
     roof_seed = {"bound": "hbm", "kernel": "seed_kernel", "achieved": ach, "peak": peak, "unit": "GB/s", "frac": ach / peak,
-                 "traffic": _traffic("seed_kernel"), "traffic_unit": "DRAM bytes of ONE launch (index part 0 of 8; ncu capture scaled by reads per launch)",
                  "algorithmic_bytes_per_launch": int(alg_bytes / world / args.steps / max(1, info["parts"])),
                  "peak_source": peak_src, "algorithmic_bytes_per_step": int(alg_bytes / world / args.steps),
                  "kernel_ms_per_step": float(np.mean(seed_ms))}
@@ -599,11 +643,10 @@ def main():
         "metric": METRIC, "value": value, "unit": "reads/s", "n_gpus": world, "steps": args.steps, "warmup": args.warmup,
         "ms_per_step": tm[0] / args.steps, "higher_is_better": True, "scaling": "weak", "vs_baseline": None,
         "dtype": "int16x2 (DPX) / u8", "data": "synthetic",
-        "config": {"workload": "10 M synthetic 150 bp Illumina reads vs all 8 data/rRNA_databases refs, 1xB200" if (n_job == 10_000_000 and world == 1) else
-                   f"{n_job} synthetic 150 bp Illumina reads per GPU vs all 8 data/rRNA_databases refs",
+        "config": {"workload": f"{n_job} synthetic 150 bp Illumina reads per GPU vs the 8 seeded stand-ins of data/rRNA_databases (tools/synth_databases.py)",
                    "reads_per_gpu_per_step": n, "reads_per_gpu_job": n * args.steps, "read_len": READ_LEN, "databases": 8, "index_hbm_bytes": info["hbm_bytes"],
-                   "l2": "inputs larger than L2 (index 1.3 GB + reads 1.5 GB per pass)", "parallelism": f"reads sharded by record x{world}",
-                   "hit_rate": counters["num_aligned"] / total_reads_job},
+                   "l2": "inputs larger than the 50 MB L2 (index and read batch)", "parallelism": f"reads sharded by record x{world}",
+                   "hit_rate": counters["num_aligned"] / total_reads_job, "device_mem_used_gb": device_mem_used_gb},
         "e2e": {"value": e2e_value, "unit": "reads/s", "h2d_bytes_per_step": h2d, "d2h_bytes_per_step": d2h},
         "gpu_launches": int(launches),
         "roofline": roof_sw,            # the dominant kernel of the step
@@ -617,10 +660,17 @@ def main():
         "counters": counters,
         "setup_s": setup_s, "index_build_s": built, "index_source": args.index_source, "index_resident_s": round(index_resident_s, 2),
     }
-    if not args.no_cpu_baseline and world == 1:   # reported baseline: rank 0 at N = 1 only
+    from oracle import ora
+    if not args.no_cpu_baseline and world == 1 and not ora.have_reference_binary():
+        out["cpu_baseline"] = {"unavailable": "oracle/_ref/sortmerna_ref is not built (oracle/Makefile.ref needs the reference sources)"}
+    elif not args.no_cpu_baseline and world == 1:   # reported baseline: rank 0 at N = 1 only
         sample = min(n, args.cpu_sample or int(min(400_000, max(20_000, 2_300 * cores))))
-        v, t, total, _ = run_reference_sample(fastas, reference_index_dir(fastas), first_reads[:sample], cores)
+        t_ref_idx = time.time()
+        ref_idx = reference_index_dir(work, fastas)
+        t_ref_idx = time.time() - t_ref_idx
+        v, t, total, _ = run_reference_sample(fastas, ref_idx, first_reads[:sample], cores)
         out["cpu_baseline"] = {"value": v, "unit": "reads/s", "cores": cores, "kind": "reference", "host": core_info,
+                               "reference_index_build_s": round(t_ref_idx, 1),
                                "sample": f"first {sample} reads of the same synthetic workload vs the 8 databases, reference CPU build "
                                          f"(oracle/_ref/sortmerna_ref -threads {cores}), alignment loops {t:.1f} s (index loading excluded; "
                                          f"'Done alignment' incl. loading {total:.1f} s)"}

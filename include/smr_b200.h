@@ -1,5 +1,5 @@
 /*
- * include/smr_b200.h -- C ABI of the B200-native alignment hot path (libsmr_b200.so).
+ * include/smr_b200.h -- C ABI of the GPU-native (H100, sm_90a) alignment hot path (libsmr_b200.so).
  *
  * The reference (sortmerna v5.0.0) has no FFI; the seam this library replaces is the C++ call
  *     void align(Readfeed&, Readstats&, Index&, KeyValueDatabase&, Runopts&)

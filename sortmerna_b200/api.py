@@ -71,7 +71,7 @@ def load_library():
     if _lib is None:
         if not os.path.exists(LIB_PATH):
             raise RuntimeError(f"{LIB_PATH} is missing: run `python -c 'import __graft_entry__ as g; g.build()'` "
-                               "(nvcc, sm_100a). There is no CPU fallback for the alignment hot path.")
+                               "(nvcc, sm_90a). There is no CPU fallback for the alignment hot path.")
         L = C.CDLL(LIB_PATH)
         L.smr_last_error.restype = C.c_char_p
         L.smr_last_error.argtypes = [C.c_void_p]

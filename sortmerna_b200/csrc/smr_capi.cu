@@ -45,7 +45,7 @@ struct smr_ctx {
   bool have_params = false;
   std::vector<Part> parts;
   uint32_t n_index_files = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   uint32_t chunk_reads = 1u << 20;
   uint32_t need_slots = 0;       // set with SMR_ERR_CAPACITY in all-alignments mode: the stride the batch needs
   uint32_t all_slots = 16;       // stride of the result layout when num_alignments == 0 (smr_set_aln_slots)
@@ -295,7 +295,7 @@ int setup_arenas(smr_ctx* ctx) {
   ctx->lis_warps = ctx->lis_ctas * kPlannerWarps;   // planner warps (each owns an arena)
   ctx->pall_cap = 32768u * ctx->scale;
   ctx->lis_stride = lis_arena_bytes(ctx->hist_cap, ctx->cand_cap, ctx->pair_cap, ctx->task_cap, ctx->pall_cap);
-  // keep the arena total under ~16 GB (of 180): fewer persistent CTAs for huge reference sets
+  // keep the arena total under ~16 GB (of the 80 GB of an H100): fewer persistent CTAs for huge reference sets
   const size_t budget = (size_t)16 << 30;
   while (ctx->lis_ctas > 16 && ctx->lis_stride * ctx->lis_warps > budget) { ctx->lis_ctas /= 2; ctx->lis_warps = ctx->lis_ctas * kPlannerWarps; }
   if (int rc = ensure(ctx, ctx->lis_arena, ctx->lis_stride * ctx->lis_warps)) return rc;

@@ -1,4 +1,4 @@
-// Device-side data layout shared by all kernels (sm_100a).
+// Device-side data layout shared by all kernels (sm_90a).
 #pragma once
 #include <cstdint>
 #include <cuda_runtime.h>

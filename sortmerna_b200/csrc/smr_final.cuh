@@ -47,7 +47,7 @@ __host__ __device__ inline size_t final_arena_bytes(uint32_t cap_w, uint32_t cap
 
 constexpr int kFinalWarpsPerCta = 4;
 #ifndef SMR_FINAL_MIN_CTAS
-#define SMR_FINAL_MIN_CTAS 6     // resident CTAs per SM the register budget is set for (3: 167 registers, 15.3 ms finalize + traceback per 500 k reads; 4: 128, 14.4; 5: 96, 14.3; 6: 80, 13.8)
+#define SMR_FINAL_MIN_CTAS 6     // resident CTAs per SM the register budget is set for (3: 167 registers, 4: 128, 5: 96, 6: 80; more CTAs were faster)
 #endif
 constexpr int kFinalCtasPerSm = SMR_FINAL_MIN_CTAS;
 

@@ -2,7 +2,7 @@
 // Replaces the host-side inflate of the reference's read feed (src/sortmerna/readfeed.cpp:683-770 via izlib / rapidgzip) for
 // smr_upload_fastx_gz (SURVEY 8(f)(2)).
 //
-// B200 mapping: Huffman decoding is a serial bit chain, so the parallelism is ACROSS spans: one thread per span, the
+// GPU mapping: Huffman decoding is a serial bit chain, so the parallelism is ACROSS spans: one thread per span, the
 // thread's 2.5 KB of decode tables in shared memory (32 decoders per CTA, 82 KB; two CTAs per SM -> 9.4 k spans in flight), the
 // 16-bit symbols and the final bytes streamed through HBM.  A 1 GB .gz at 64 KB chunks is 16 k spans: two waves.
 #pragma once

@@ -28,11 +28,11 @@
 //     geometrically so that a perfect-score stop wastes at most what was useful.
 //   * SCORER warps drain a global multi-producer/multi-consumer queue of task PAIRS and score two tasks per pass with
 //     the packed 16-bit DPX kernel (smr_sw.cuh), whoever the read belongs to: a read with thousands of candidates is
-//     scored by the whole GPU instead of by its one warp (round 1: the heaviest read occupied one warp for 310 of the
-//     376 ms), and the integer-pipe loop never waits on the memory-latency phases of voting and grouping.
+//     scored by the whole GPU instead of by its one warp (in round 1 the heaviest read occupied one warp for most of the
+//     kernel), and the integer-pipe loop never waits on the memory-latency phases of voting and grouping.
 //   * The FETCHER warp (one lane per scorer input slot) pops the queue and stages the scorers' inputs -- reference window and query
 //     segment -- with TMA bulk copies (cp.async.bulk + mbarrier), two slots per scorer: one fills while the other is scored.
-// Hand-over without fences: __threadfence() is MEMBAR.SC.GPU + CCTL.IVALL on sm_100a -- it also invalidates the SM's whole L1.  A
+// Hand-over without fences: __threadfence() is MEMBAR.SC.GPU + CCTL.IVALL on sm_90a -- it also invalidates the SM's whole L1.  A
 // planner publishes a queue entry with a release store (MEMBAR.ALL.GPU + ST) after marking the score words of its tasks pending;
 // the fetcher reads entry and task records past L1; a scorer stores its scores and adds to the planner's counter with no fence in
 // between; the planner takes the counter as a hint and then looks at every score word itself.
@@ -43,7 +43,8 @@
 namespace smr {
 
 // One CTA of 32 warps per SM: 16 scorers + 1 fetcher (one lane per scorer slot) + 15 planners.  (Two CTAs of 8 + 1 + 7 need two
-// fetcher warps per SM: one planner fewer -- 213.1 vs 207.1 ms per 500 k reads; 14 + 1 + 17: 209.6.)
+// fetcher warps per SM, i.e. one planner fewer, and were slower, as was 14 + 1 + 17.  The split and the other tuning constants of
+// this file were chosen by A/B runs of the candidate kernel during development and have not been re-tuned on the H100.)
 #ifndef SMR_SCORER_WARPS
 #define SMR_SCORER_WARPS 16
 #endif
@@ -54,7 +55,7 @@ namespace smr {
 #define SMR_LIS_MIN_CTAS 1
 #endif
 // Phase accounting with clock64 (the cycle shares bench.py reports) is a template parameter of the kernel: the product runs the
-// instantiation without it (smr_set_instrumentation; 199.6 vs 204.9 ms per 500 k reads with it).
+// instantiation without it (smr_set_instrumentation; the accounting costs a few per cent of the kernel's time).
 template <bool kInstr> __device__ __forceinline__ long long lis_clock() { return kInstr ? clock64() : 0ll; }
 // Timeline of the instrumented instantiation (SMR_TIMELINE=1 prints it): nanoseconds per role and state in 1 ms buckets since the
 // start of the kernel -- g.dbg + kTlBase + row * kTlBuckets; rows: 0 scorers waiting for a staged pair, 1 scorers busy, 2 planners
@@ -104,20 +105,20 @@ constexpr uint32_t kNoTask = 0xFFFFFFu;
 constexpr uint32_t kPoison = 0xFFFFu;             // planner id of the shutdown entries
 constexpr uint32_t kBatchCandCap = 4096;          // candidates per batch
 #ifndef SMR_PLANNER_POLL_NS
-#define SMR_PLANNER_POLL_NS 1024                    // sleep between two looks of a planner at its score counter (256: 215.1 ms, 512: 214.2, 1024: 213.4)
+#define SMR_PLANNER_POLL_NS 1024                    // sleep between two looks of a planner at its score counter (shorter sleeps were no faster)
 #endif
 constexpr uint32_t kScorePending = 0xFFFFFFFFu;     // score word of a task that has been handed to the scorers and not been scored yet
 // Sensitivity experiments (tools/ab_round.sh; never set in the shipped build): stretch a role's own work by N per cent with sleeps
 // (no issue slots taken) -- how much the kernel slows tells which role bounds it.
 // Schedule of the reads over the planner warps.  The seed kernel bins the reads of a chunk by log2 of their voting work; index 0 of the
 // schedule is the heaviest read.  With ONE heaviest-first cursor (round 2a) every planner starts on a read whose votes take
-// milliseconds: the scorers wait for 20 ms of 205 (the kernel's role timeline, SMR_TIMELINE / tools/timeline_summary.py).  So two
+// milliseconds, and the scorers sit idle at the start of the kernel (its role timeline, SMR_TIMELINE / tools/timeline_summary.py).  So two
 // cursors: SMR_SCHED_A planners in 8 take the heaviest nwork >> SMR_SPLIT_SHIFT reads in order, the others start right behind them,
-// on reads whose few candidates reach the scorers within microseconds -- the scorers are busy 12 ms after the launch -- and go on
+// on reads whose few candidates reach the scorers within microseconds -- the scorers are busy soon after the launch -- and go on
 // towards the light end; a planner whose region is exhausted helps in the other.  SMR_SCHED_A = 0: the single cursor.
-// Measured (ms per 500 k reads, candidate kernel): single cursor 201.8; 4 in 8 planners on the heaviest 1/64: 198.1, 1/16: 195.3,
-// 1/8: 191.5 - 194.8; 2 in 8 on 1/32: 195.5; variants that also start planners at the light end (the reads without Smith-Waterman
-// work, which otherwise end the kernel with idle scorers) lost what they gained there at the start: 197 - 206.
+// Of the variants compared (single cursor; 2 or 4 in 8 planners on the heaviest 1/64 ... 1/8) 4 in 8 on the heaviest 1/8 was the
+// fastest; variants that also start planners at the light end (the reads without Smith-Waterman work, which otherwise end the
+// kernel with idle scorers) lost what they gained there at the start.
 #ifndef SMR_SCHED_A
 #define SMR_SCHED_A 4
 #endif
@@ -135,7 +136,7 @@ __device__ __forceinline__ void exp_delay(const long long t0, const int pct) {
   while (clock64() < until) __nanosleep(256);
 }
 #ifndef SMR_BATCH_CAP0
-#define SMR_BATCH_CAP0 32                         // candidates in the first batch of a call (8: 219.5 ms, 32: 216.8, 128: 216.8 per 500 k reads)
+#define SMR_BATCH_CAP0 32                         // candidates in the first batch of a call (8 was slower; 128 gained nothing over 32)
 #endif
 
 // one Smith-Waterman call the reference would make (alignment.cpp:365-381), as the scorers see it

@@ -5,7 +5,7 @@
 // (src/sortmerna/read.cpp:601-611) and the trie x Levenshtein-automaton DFS traversetrie_align
 // (src/sortmerna/traverse_bursttrie.cpp:100-298).
 //
-// B200 mapping: the index is a set of flat HBM arrays (smr_index.h); a window search is a chain of
+// GPU mapping: the index is a set of flat HBM arrays (smr_index.h); a window search is a chain of
 // dependent 8/32-byte sector reads (lookup -> root node -> child nodes -> bucket entries), so the
 // kernel is HBM/L2-latency bound and is parallelised over (read, strand, window) -- 90 windows per
 // 150-nt read -- with warp ballot/shuffle compaction of the hits into a per-read region.

@@ -452,8 +452,8 @@ __device__ __noinline__ uint32_t sw_pair_warp(const uint32_t* __restrict__ profA
     F[0] = upF;
     // vertical chain F[r+1] = max(F[r] - ge, X[r]): R dependent instructions (8.4 cycles each).  With four scorer warps per SM
     // sub-partition the pipe is full anyway (tools/ubench/dp.cu: 2 warps saturate it), so no ALU work is spent on shortening it
-    // (measured: a two-row look-ahead, F[r+2] = max(F[r] - 2 ge, max(X[r] - ge, X[r+1])), 2 more instructions per step: 227 vs 220 ms;
-    //  one-row-per-word profiles merged by IMAD instead of PRMT, 4 more shared loads per step: 238 ms -- the LSU pipe, not the ALU)
+    // (measured: a two-row look-ahead, F[r+2] = max(F[r] - 2 ge, max(X[r] - ge, X[r+1])), 2 more instructions per step: slower;
+    //  one-row-per-word profiles merged by IMAD instead of PRMT, 4 more shared loads per step: slower still -- the LSU pipe, not the ALU)
 #pragma unroll
     for (int r = 0; r < R; ++r) F[r + 1] = __viaddmax_s16x2(F[r], nge2, X[r]);
     const uint32_t hl = __viaddmax_s16x2(F[R - 1], ngo2, X[R - 1]);

@@ -1,5 +1,6 @@
 import gzip
 import json
+import lzma
 import os
 import shutil
 import sys
@@ -14,20 +15,24 @@ GOLDEN = os.path.join(ROOT, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box with -m gpu)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100; select with -m gpu)")
+
+
+def unpack_index(src, d):
+    """A stored golden index into d: .gz and .xz members decompressed (xz where gzip would exceed 1 MB), the rest copied."""
+    for fn in os.listdir(src):
+        if fn.endswith((".gz", ".xz")):
+            with (gzip.open if fn.endswith(".gz") else lzma.open)(os.path.join(src, fn), "rb") as fi, open(os.path.join(d, fn[:-3]), "wb") as fo:
+                shutil.copyfileobj(fi, fo)
+        else:
+            shutil.copy(os.path.join(src, fn), d)
 
 
 @pytest.fixture(scope="session")
 def golden_idx_dir():
     """The reference-built index of the two golden database slices, gunzipped into a temp dir."""
     d = tempfile.mkdtemp(prefix="smr_idx_")
-    src = os.path.join(GOLDEN, "idx")
-    for fn in os.listdir(src):
-        if fn.endswith(".gz"):
-            with gzip.open(os.path.join(src, fn), "rb") as fi, open(os.path.join(d, fn[:-3]), "wb") as fo:
-                shutil.copyfileobj(fi, fo)
-        else:
-            shutil.copy(os.path.join(src, fn), d)
+    unpack_index(os.path.join(GOLDEN, "idx"), d)
     yield d
     shutil.rmtree(d, ignore_errors=True)
 
@@ -84,13 +89,7 @@ def golden_t0():
     reference's own index and output (tests/golden/t0/, made by make_golden.make_t0)."""
     from sortmerna_b200 import hostio
     d = tempfile.mkdtemp(prefix="smr_idx_t0_")
-    src = os.path.join(GOLDEN, "t0", "idx")
-    for fn in os.listdir(src):
-        if fn.endswith(".gz"):
-            with gzip.open(os.path.join(src, fn), "rb") as fi, open(os.path.join(d, fn[:-3]), "wb") as fo:
-                shutil.copyfileobj(fi, fo)
-        else:
-            shutil.copy(os.path.join(src, fn), d)
+    unpack_index(os.path.join(GOLDEN, "t0", "idx"), d)
     refs = hostio.load_references(os.path.join(GOLDEN, "t0", "db_t0.fasta"))
     prefix = hostio.find_index_prefixes(d)["db_t0.fasta"]
     batch = hostio.load_reads(os.path.join(GOLDEN, "t0", "reads_t0.fasta"))

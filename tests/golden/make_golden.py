@@ -14,6 +14,7 @@ Usage: python tests/golden/make_golden.py
 """
 import gzip
 import json
+import lzma
 import os
 import shutil
 import sys
@@ -161,6 +162,16 @@ def make_reads(rng, dbs):
     return [reads[k] for k in order]
 
 
+def pack_file(src, dst):
+    """dst.gz, or dst.xz where gzip -9 would exceed 1 MB (tests/conftest.py unpack_index reads both)"""
+    data = open(src, "rb").read()
+    gz = gzip.compress(data, 9)
+    if len(gz) <= 1_000_000:
+        open(dst + ".gz", "wb").write(gz)
+    else:
+        open(dst + ".xz", "wb").write(lzma.compress(data, preset=9 | lzma.PRESET_EXTREME))
+
+
 def gz_index(src_dir, dst_dir):
     os.makedirs(dst_dir, exist_ok=True)
     for fn in sorted(os.listdir(src_dir)):
@@ -168,8 +179,7 @@ def gz_index(src_dir, dst_dir):
         if fn.endswith(".stats"):
             shutil.copy(src, os.path.join(dst_dir, fn))
         else:
-            with open(src, "rb") as fi, gzip.open(os.path.join(dst_dir, fn + ".gz"), "wb", compresslevel=9) as fo:
-                fo.write(fi.read())
+            pack_file(src, os.path.join(dst_dir, fn))
 
 
 def make_t0(tmp):
@@ -285,8 +295,7 @@ def main():
             # the .stats file embeds the absolute FASTA path; keep it as is (only lnwin/numseq/freqs are read)
             shutil.copy(src, os.path.join(idx_dir, fn))
         else:
-            with open(src, "rb") as fi, gzip.open(os.path.join(idx_dir, fn + ".gz"), "wb", compresslevel=9) as fo:
-                fo.write(fi.read())
+            pack_file(src, os.path.join(idx_dir, fn))
     make_t0(tmp)
     make_denovo()
     make_extra_index_cases()

@@ -49,11 +49,12 @@ def cases(n_reads: int = 6000):
     with gzip.GzipFile(filename="reads_file.fq", mode="wb", fileobj=bio, mtime=123) as g:
         g.write(txt[:70000])
     out.append(("header_fname", bio.getvalue(), txt[:70000]))
-    for fn in ("set4_mate_pairs_metatranscriptomics_1.fastq.gz", "set4_mate_pairs_metatranscriptomics_2.fastq.gz"):
-        p = os.path.join(ROOT, "data_cache", "sets", fn)
-        if os.path.exists(p):
-            raw = open(p, "rb").read()
-            out.append((fn[:28], raw, gzip.decompress(raw)))
+    # a stream of a few dozen deflate blocks (about 40 at the host test's size): the speculative block search must split it
+    long_txt = fastq_text(2 * n_reads, seed=2)
+    bio = io.BytesIO()
+    with gzip.GzipFile(filename="reads_long.fastq", mode="wb", fileobj=bio, compresslevel=6, mtime=456) as g:
+        g.write(long_txt)
+    out.append(("long_stream", bio.getvalue(), long_txt))
     return out
 
 

@@ -46,3 +46,22 @@ def assert_same_outputs(a, b, ref_threads=2):
                 if mp and mq and mp.group(1) == mq.group(1) and abs(float(mp.group(2)) - float(mq.group(2))) <= 1.0:
                     y[i] = p
         assert x == y, f"{fn} differs: first difference {next((p, q) for p, q in zip(x, y) if p != q)}"
+
+
+def golden_mates(d, gz=False):
+    """The reads of tests/golden/reads_mix.fq that are at least one seed (18 nt) long, split into two mate files (alternate records),
+    flat or gzip -6: the inputs of the paired-feed tests, shaped like the reference's set4_mate_pairs_metatranscriptomics_{1,2}.fastq(.gz),
+    which hold no read shorter than a seed (a shorter one triggers the reference's documented paired-feed quirk,
+    test_paired_feed_deviation_is_pinned)."""
+    import gzip
+    lines = open(os.path.join(GOLDEN, "reads_mix.fq"), "rb").read().split(b"\n")
+    recs = [b"\n".join(lines[i:i + 4]) + b"\n" for i in range(0, len(lines) - 3, 4) if lines[i].startswith(b"@") and len(lines[i + 1]) >= 18]
+    recs = recs[: len(recs) // 2 * 2]
+    paths = []
+    for k in (0, 1):
+        p = os.path.join(d, f"mates_{k + 1}.fastq" + (".gz" if gz else ""))
+        data = b"".join(recs[k::2])
+        with (gzip.open(p, "wb", compresslevel=6) if gz else open(p, "wb")) as f:
+            f.write(data)
+        paths.append(p)
+    return paths

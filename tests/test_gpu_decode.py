@@ -93,12 +93,16 @@ def test_alignment_of_decoded_batch_equals_host_parsed(aligner, golden):
     assert got["counters"]["num_aligned"] == want["counters"]["num_aligned"]
 
 
-def test_decode_bundled_set2_and_throughput(aligner):
-    p = os.path.join(ROOT, "data_cache", "sets", "set2_environmental_study_550_amplicon.fasta")
-    if not os.path.exists(p):
-        pytest.skip("data_cache/sets not staged")
-    text = open(p, "rb").read()
-    want = check_text(aligner, text, p)
+def test_decode_bundled_set2_and_throughput(aligner, tmp_path):
+    # shaped like the reference's data/set2_environmental_study_550_amplicon.fasta: 100 000 amplicons of 150-250 nt
+    rng = np.random.default_rng(550)
+    lens = rng.integers(150, 251, 100000)
+    seq = np.frombuffer(b"ACGT", np.uint8)[rng.integers(0, 4, int(lens.sum()))].tobytes()
+    ends = np.cumsum(lens)
+    text = b"".join(b">amplicon_%d sample=%d\n%s\n" % (i, i % 550, seq[e - ln:e]) for i, (ln, e) in enumerate(zip(lens.tolist(), ends.tolist())))
+    p = tmp_path / "amplicons.fasta"
+    p.write_bytes(text)
+    want = check_text(aligner, text, str(p))
     assert want.n == 100000
     # decode rate of a large text (the set repeated to ~0.5 GB), kernels only
     big = text * max(1, (1 << 29) // len(text))

@@ -58,13 +58,16 @@ def test_alignment_of_gz_batch_equals_host_parsed(aligner, golden):
     assert_same_results(got, want, "gz-decoded vs host-parsed")
 
 
-def test_bundled_gz_mates_and_throughput(aligner):
-    p = os.path.join(ROOT, "data_cache", "sets", "set4_mate_pairs_metatranscriptomics_1.fastq.gz")
-    if not os.path.exists(p):
-        pytest.skip("data_cache/sets not staged")
-    raw = open(p, "rb").read()
+def test_bundled_gz_mates_and_throughput(aligner, tmp_path):
+    # shaped like the reference's data/set4_mate_pairs_metatranscriptomics_1.fastq.gz: 5000 reads, gzip -6 with a file name
+    txt = inflate_cases.fastq_text(5000, seed=4)
+    p = tmp_path / "mates_1.fastq"
+    p.write_bytes(txt)
+    with open(str(p) + ".gz", "wb") as f, gzip.GzipFile(filename=p.name, mode="wb", fileobj=f, compresslevel=6, mtime=0) as g:
+        g.write(txt)
+    raw = open(str(p) + ".gz", "rb").read()
     n = aligner.upload_fastx_gz(raw)
-    h, s, _ = hostio.read_fastx(p[:-3])
+    h, s, _ = hostio.read_fastx(str(p))
     want = hostio.pack_reads(h, s)
     assert n == want.n == 5000
     _, off, seq = aligner.resident_layout()

@@ -1,4 +1,4 @@
-"""Parity tests proper (need a B200): the CUDA hot path, called through the C ABI, against the
+"""Parity tests proper (need an H100): the CUDA hot path, called through the C ABI, against the
 oracle on the same inputs, and against the committed golden output of the reference binary."""
 import os
 

@@ -147,17 +147,16 @@ def test_reference_t9_golden_sam_rows():
 
 
 @need
-@pytest.mark.skipif(not os.environ.get("SMR_LONG_TESTS"), reason="minutes of CPU time: set SMR_LONG_TESTS=1 (run once per round in the build container)")
 def test_reference_known_answers_t5_t11():
-    """scripts/test.jinja t5 (set4 mates vs bac-16s-id85 -max_pos 250: 6000 / 4000) and t11 (set5, 30000 simulated amplicon reads,
-    -id 0.97 -coverage 0.97 -otu_map -de_novo_otu: 19995 / 10005) through the host program with the binding: the known answers,
-    and for t11 the whole aligned.log equal to the reference's (incl. 'Total reads for de novo clustering')."""
+    """Shaped like the reference's t5 (two mate files, paired feed, 5 threads, a 16S database indexed with -max_pos 250) and t11
+    (-id 0.97 -coverage 0.97 -otu_map -de_novo_otu -blast, 3 threads), on the golden mates / reads against the golden bacterial
+    slice: the host program with the binding writes the totals of the reference binary (t5) and its whole aligned.log (t11,
+    incl. 'Total reads for de novo clustering')."""
     import re
     import subprocess
-    R = "/root/reference/data"
-    if not os.path.isdir(R):
-        pytest.skip("bundled data not available")
+    from integration_common import golden_mates
     d = tempfile.mkdtemp(prefix="smr_kat_")
+    fasta = os.path.join(GOLDEN, "db_bac.fasta")
 
     def run(binary, name, args):
         wd = os.path.join(d, name + binary)
@@ -165,14 +164,15 @@ def test_reference_known_answers_t5_t11():
         assert p.returncode == 0, p.stdout[-2000:]
         return [ln for ln in open(os.path.join(wd, "out", "aligned.log")).read().split("\n") if not re.search(r"Time|time|Command|pid|/tmp/|Date|sec|\d\d:\d\d:\d\d", ln)]
     try:
-        t5 = ["-ref", R + "/silva-bac-16s-database-id85.fasta", "-reads", R + "/set4_mate_pairs_metatranscriptomics_1.fastq.gz", "-reads",
-              R + "/set4_mate_pairs_metatranscriptomics_2.fastq.gz", "-max_pos", "250", "-fastx", "-other", "-threads", "5"]
-        log = "\n".join(run("sortmerna_gpu_mock", "t5", t5))
-        assert "passing E-value threshold = 6000" in log and "failing E-value threshold = 4000" in log
-        t11 = ["-ref", R + "/silva-bac-16s-database-id85.fasta", "-reads", R + "/set5_simulated_amplicon_silva_bac_16s.fasta", "-id", "0.97", "-coverage", "0.97",
+        m1, m2 = golden_mates(d, gz=True)
+        t5 = ["-ref", fasta, "-reads", m1, "-reads", m2, "-max_pos", "250", "-fastx", "-other", "-threads", "5"]
+        a, b = run("sortmerna_gpu_mock", "t5", t5), run("sortmerna_ref", "t5", t5)
+        totals = lambda log: [ln for ln in log if "E-value threshold" in ln or "Total reads =" in ln]
+        assert any("passing E-value threshold" in ln for ln in totals(b)) and totals(a) == totals(b)
+        t11 = ["-ref", fasta, "-reads", os.path.join(GOLDEN, "reads_mix.fq"), "-id", "0.97", "-coverage", "0.97",
                "-otu_map", "-de_novo_otu", "-blast", "1 cigar qcov", "-fastx", "-other", "-threads", "3"]
         a, b = run("sortmerna_gpu_mock", "t11", t11), run("sortmerna_ref", "t11", t11)
-        assert "passing E-value threshold = 19995" in "\n".join(a) and "failing E-value threshold = 10005" in "\n".join(a)
+        assert any("Total reads for de novo clustering" in ln for ln in b)
         assert a == b
     finally:
         shutil.rmtree(d, ignore_errors=True)

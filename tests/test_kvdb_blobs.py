@@ -108,14 +108,9 @@ if __name__ == "__main__":   # regenerate tests/golden/kvdb_blobs.json from the 
     import sys
     sys.path.insert(0, ROOT)
     import conftest
-    import tempfile, gzip, shutil
+    import tempfile
     d = tempfile.mkdtemp()
-    for fn in os.listdir(os.path.join(GOLDEN, "idx")):
-        src = os.path.join(GOLDEN, "idx", fn)
-        if fn.endswith(".gz"):
-            open(os.path.join(d, fn[:-3]), "wb").write(gzip.open(src).read())
-        else:
-            shutil.copy(src, d)
+    conftest.unpack_index(os.path.join(GOLDEN, "idx"), d)
     refs = [hostio.load_references(os.path.join(GOLDEN, n)) for n in ("db_arc.fasta", "db_bac.fasta")]
     pre = hostio.find_index_prefixes(d)
     prefixes = [pre["db_arc.fasta"], pre["db_bac.fasta"]]

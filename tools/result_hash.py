@@ -1,9 +1,10 @@
 """SHA-256 over everything smr_align_batch returns for N reads of the synthetic bench workload (8 databases, device-built
 indexes): two builds of the library (SMR_LIB_PATH) that print the same line returned bit-identical results.
-Usage: python tools/result_hash.py [N]   (GPU box)"""
+Usage: python tools/result_hash.py [N]   (needs a GPU)"""
 import hashlib
 import os
 import sys
+import tempfile
 
 import numpy as np
 
@@ -15,7 +16,8 @@ from sortmerna_b200 import api  # noqa: E402
 
 def main():
     n = int(sys.argv[1]) if len(sys.argv) > 1 else 200_000
-    fastas, idx_dir, prefixes, refs, stats, built = bench.load_databases()
+    work = tempfile.TemporaryDirectory(prefix="smr_hash_")
+    fastas, idx_dir, prefixes, refs, stats, built = bench.load_databases(work.name)
     ms = bench.minimal_scores(stats, fastas, 10_000_000)
     al = api.Aligner(0)
     al.set_params(api.default_params())

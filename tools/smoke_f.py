@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""One small pass over the 8(f) kernels for compute-sanitizer (tools/evidence.sh): index built on the device, gzip inflate + input
+"""One small pass over the 8(f) kernels for compute-sanitizer: index built on the device, gzip inflate + input
 decode on the device, then the alignment kernels on that batch."""
 import gzip
 import os

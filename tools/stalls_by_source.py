@@ -1,8 +1,8 @@
 #!/usr/bin/env python
-"""Warp-stall samples of one kernel by CUDA source line, from an ncu report (how profiles/r1_stalls_by_source.txt was made).
+"""Warp-stall samples of one kernel by CUDA source line, from an ncu report.
 
   ncu -i X.ncu-rep --page source --csv --print-source sass > src.csv
-  cuobjdump -xelf all sortmerna_b200/libsmr_b200.so && nvdisasm -g -c smr_capi.sm_100a.cubin > disasm.txt
+  cuobjdump -xelf all sortmerna_b200/libsmr_b200.so && nvdisasm -g -c smr_capi.sm_90a.cubin > disasm.txt
   python tools/stalls_by_source.py src.csv disasm.txt '.text._ZN3smr10lis_kernel'
 
 The ncu source page gives samples per SASS address; nvdisasm -g gives the source line of every SASS offset of the same cubin."""

@@ -6,7 +6,7 @@ import sys
 
 def main():
     f = sys.argv[1]
-    ns_, np_ = (int(sys.argv[2]) if len(sys.argv) > 2 else 16) * 148, (int(sys.argv[3]) if len(sys.argv) > 3 else 15) * 148
+    ns_, np_ = (int(sys.argv[2]) if len(sys.argv) > 2 else 16) * 132, (int(sys.argv[3]) if len(sys.argv) > 3 else 15) * 132
     lines = [l for l in open(f) if l.startswith("[smr timeline]")]
     rows = {}
     for l in lines[-6:]:          # the last run in the file
