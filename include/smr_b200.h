@@ -215,6 +215,48 @@ int smr_run_resident(smr_ctx*);                       /* all kernels of one pass
 int smr_download_results(smr_ctx*, smr_read_result* results, smr_aln* alns, uint32_t* cigar_pool,
                          uint64_t cigar_cap, uint64_t* cigar_used, uint64_t* counters, uint32_t n_counters);
 
+/* -- report writer on the device (sortmerna_b200/csrc/smr_report.cuh, DESIGN.md 5e): one batch's results + the FASTA / FASTQ text
+ *    of its reads -> the bytes the reference's report stage writes for that batch: aligned.sam body rows (ReportSam::append,
+ *    src/sortmerna/report_sam.cpp:64-152), tabular aligned.blast rows (ReportBlast::append, report_blast.cpp:99-346), and the records
+ *    of aligned.*, other.* and aligned_denovo.* (ReportFastx / ReportFxOther / ReportDenovo, routing of output.cpp:117-142). */
+
+/* The reference ids (BaseRecord::getId) of the loaded (index_num, part), concatenated: id k = names_cat[name_off[k] .. name_off[k+1]).
+ * Uploaded once; they stay resident with the part.  Needed for SAM and BLAST. */
+int smr_set_report_refs(smr_ctx*, uint32_t index_num, uint32_t part, const char* names_cat, const uint64_t* name_off, uint32_t nref);
+/* The E-value inputs of index index_num (Refstats: gumbel lambda / K, the corrected full_ref / full_read of refstats.cpp:236-257).
+ * The host computes the E-value and bit score of every score 0..65535 with the reference's expressions (report_blast.cpp:117-126)
+ * and uploads the tables; the device only looks them up.  Needed for BLAST. */
+int smr_set_report_scoring(smr_ctx*, uint32_t index_num, double lambda, double K, uint64_t full_ref, uint64_t full_read);
+
+enum { SMR_BLAST_COL_CIGAR = 1, SMR_BLAST_COL_QCOV = 2, SMR_BLAST_COL_QSTRAND = 3 };
+typedef struct {
+  int32_t sam;                 /* -sam */
+  int32_t blast;               /* -blast given */
+  int32_t blast_format;        /* its first field: 1 = tabular; 0 = pairwise (SMR_ERR_UNSUPPORTED) */
+  int32_t blast_cols[4];       /* the optional columns in the order given (SMR_BLAST_COL_*), 0 ends the list */
+  int32_t fastx, other;        /* -fastx, -other */
+  int32_t denovo;              /* -de_novo_otu: aligned_denovo.* */
+  double min_id, min_cov;      /* -id, -coverage (the aligned_denovo rule) */
+  int32_t paired_in, paired_out; /* the batch is interleaved mates: records 2k and 2k+1 */
+  int32_t out2, sout;          /* SMR_ERR_UNSUPPORTED */
+} smr_report_opts;
+
+/* Format one batch.  text / nbytes: the FASTA or FASTQ text of the reads, in batch order; text == nullptr means the resident text of
+ * smr_upload_fastx[_gz].  results / alns / cigar_pool (cigar_words used words) / stats: exactly what smr_align_batch or
+ * smr_download_results returned for it (stats through smr_set_stats_buffer; required for SAM, BLAST and denovo).  SEQ is taken
+ * from the text.  The number of records and every aligned read's length must agree with the results (SMR_ERR_ARG otherwise).
+ * Output: the streams one after another, in this order: SAM rows of every loaded (index, part) group in (index, part) order, BLAST
+ * rows of every group, aligned reads, other reads, aligned_denovo reads; stream k = out[stream_off[k] .. stream_off[k+1]),
+ * stream_off has 2 * groups + 4 entries.  A caller that feeds a file in several batches appends every stream to its own file and
+ * concatenates them at the end, as the reference's merge does.  If out is null or cap is below stream_off[2 * groups + 3], the call
+ * returns SMR_ERR_CAPACITY with stream_off filled. */
+int smr_format_reports(smr_ctx*, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
+                       const smr_aln* alns, const uint32_t* cigar_pool, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                       char* out, uint64_t cap, uint64_t* stream_off);
+/* of the last smr_format_reports, milliseconds (CUDA events): out[0] = H2D of text and results, [1] = device work (layout, sizes,
+ * scans, writes; includes the one read-back of the sizes), [2] = D2H of the output */
+int smr_last_report_timings(const smr_ctx*, double out[3]);
+
 /* Device-side timings of the last smr_run_resident / smr_align_batch, CUDA events on the
  * library's stream, milliseconds: out[0]=total [1]=seed kernels [2]=candidate/SW kernels
  * [3]=finalize (reverse SW + traceback) [4]=h2d [5]=d2h; out[6]=number of kernel launches */

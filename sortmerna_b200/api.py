@@ -27,7 +27,8 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_run_resident", "smr_download_results", "smr_last_timings", "smr_debug_seed_windows", "smr_debug_ssw",
            "smr_debug_dpx_peak", "smr_set_stats_buffer", "smr_build_index", "smr_upload_fastx", "smr_resident_layout", "smr_pack_kvdb_blobs",
            "smr_set_aln_slots", "smr_aln_slots", "smr_aln_slots_needed", "smr_upload_fastx_gz", "smr_resident_text", "smr_debug_inflate",
-           "smr_build_index_device", "smr_debug_index_array", "smr_set_instrumentation"]
+           "smr_build_index_device", "smr_debug_index_array", "smr_set_instrumentation", "smr_set_report_refs", "smr_set_report_scoring",
+           "smr_format_reports", "smr_last_report_timings"]
 
 CNT_NAMES = ("num_aligned", "num_short", "sw_calls", "sw_cells", "windows", "trie_nodes", "buckets",
              "bucket_entries", "pos_entries", "lis_calls", "dbg_max_read_cycles", "dbg_sum_read_cycles", "dbg_lis_kernel_cycles",
@@ -61,6 +62,30 @@ ALN_DTYPE = np.dtype([("cigar_off", "<u4"), ("cigar_len", "<u4"), ("ref_num", "<
                       ("score1", "<u2"), ("part", "<u2"), ("index_num", "<u2"), ("strand", "u1"), ("pad", "u1")])
 
 STATS_DTYPE = np.dtype([("n_miss", "<u4"), ("n_gap", "<u4"), ("n_match", "<u4"), ("n_match_denovo", "<u4")])
+
+BLAST_COLS = {"cigar": 1, "qcov": 2, "qstrand": 3}
+
+
+class ReportOpts(C.Structure):
+    """smr_report_opts (include/smr_b200.h)"""
+    _fields_ = [("sam", C.c_int32), ("blast", C.c_int32), ("blast_format", C.c_int32), ("blast_cols", C.c_int32 * 4), ("fastx", C.c_int32),
+                ("other", C.c_int32), ("denovo", C.c_int32), ("min_id", C.c_double), ("min_cov", C.c_double), ("paired_in", C.c_int32),
+                ("paired_out", C.c_int32), ("out2", C.c_int32), ("sout", C.c_int32)]
+
+
+def report_opts(sam=False, blast=None, fastx=False, other=False, denovo=None, paired_in=False, paired_out=False, out2=False, sout=False) -> ReportOpts:
+    """blast: None, or the value of the reference's -blast option ('1 cigar qcov qstrand'; '0' = pairwise, refused by the writer);
+    denovo: None, or (min_id, min_cov) = the reference's -id / -coverage."""
+    o = ReportOpts(sam=int(bool(sam)), fastx=int(bool(fastx)), other=int(bool(other)), paired_in=int(bool(paired_in)),
+                   paired_out=int(bool(paired_out)), out2=int(bool(out2)), sout=int(bool(sout)))
+    if blast is not None:
+        f = str(blast).split()
+        o.blast, o.blast_format = 1, int(f[0])
+        for k, c in enumerate(f[1:]):
+            o.blast_cols[k] = BLAST_COLS[c]
+    if denovo is not None:
+        o.denovo, o.min_id, o.min_cov = 1, float(denovo[0]), float(denovo[1])
+    return o
 
 _lib = None
 
@@ -147,6 +172,8 @@ class Aligner:
         self.params = None
         self.n_index_files = 0
         self.refs_by_index = {}
+        self.parts = []          # loaded (index_num, part)
+        self._report_refs = set()
         self._keep = []
 
     def _check(self, rc, what):
@@ -191,6 +218,7 @@ class Aligner:
         self._check(rc, f"smr_load_index_part({prefix})")
         self.n_index_files = max(self.n_index_files, index_num + 1)
         self.refs_by_index[index_num] = refs
+        self.parts.append((index_num, part))
 
     def build_index_device(self, index_num: int, fasta: str, refs=None, minimal_score: int = 0, skiplengths=(18, 9, 3), lnwin: int = 18,
                            interval: int = 1, max_pos: int = 10000, max_mb: float = 3072.0) -> int:
@@ -207,6 +235,7 @@ class Aligner:
         self.n_index_files = max(self.n_index_files, index_num + 1)
         if refs is not None:
             self.refs_by_index[index_num] = refs
+        self.parts += [(index_num, p) for p in range(int(nparts.value))]
         self.last_build_report = dict(zip(("parts", "numseq", "windows", "unique_lmers", "trie_nodes", "hbm_bytes"), (int(x) for x in rep)))
         return int(nparts.value)
 
@@ -340,17 +369,89 @@ class Aligner:
                 self._check(self.L.smr_resident_layout(self.h, C.c_void_p(0), C.c_void_p(0), _ptr(seq), C.c_uint64(seq.size)), "smr_resident_layout")
         return hdr, off, seq
 
-    def run_resident(self):
+    def run_resident(self, with_stats: bool = False):
+        """with_stats: the next download() also returns calc_miss_gap_match per stored alignment (out["stats"])"""
+        n = self._n_resident
+        self._stats = np.zeros(n * int(self.L.smr_aln_slots(self.h)), STATS_DTYPE) if with_stats else None
+        self._check(self.L.smr_set_stats_buffer(self.h, _ptr(self._stats) if with_stats else C.c_void_p(0)), "smr_set_stats_buffer")
         self._check(self.L.smr_run_resident(self.h), "smr_run_resident")
 
     def download(self):
         n = self._n_resident
         slots, res, alns, pool, cap, counters = self._outputs(n)
+        stats, self._stats = getattr(self, "_stats", None), None
         used = C.c_uint64(0)
         rc = self.L.smr_download_results(self.h, _ptr(res), _ptr(alns), _ptr(pool), C.c_uint64(cap), C.byref(used),
                                          _ptr(counters), C.c_uint32(counters.size))
+        self.L.smr_set_stats_buffer(self.h, C.c_void_p(0))
         self._check(rc, "smr_download_results")
-        return self._pack(res, alns, pool, used.value, counters, slots)
+        out = self._pack(res, alns, pool, used.value, counters, slots)
+        if stats is not None:
+            out["stats"] = stats
+        return out
+
+    # ---- report writer (smr_format_reports) ----
+    def report_groups(self) -> list:
+        """the loaded (index, part)s in the order of the SAM / BLAST streams"""
+        return sorted(set(self.parts))
+
+    def _upload_report_refs(self):
+        for (i, p) in self.report_groups():
+            if (i, p) in self._report_refs:
+                continue
+            refs = self.refs_by_index.get(i)
+            if refs is None:
+                raise SmrError(f"no reference ids for index {i}: pass refs to load_index_part / build_index_device")
+            r = refs[p] if isinstance(refs, (list, tuple)) else refs
+            names = [x.encode() for x in r.ids]
+            off = np.zeros(len(names) + 1, np.uint64)
+            np.cumsum([len(x) for x in names], out=off[1:])
+            cat = np.frombuffer(b"".join(names) or b"\0", np.uint8)
+            self._check(self.L.smr_set_report_refs(self.h, C.c_uint32(i), C.c_uint32(p), _ptr(cat), _ptr(off), C.c_uint32(len(names))),
+                        "smr_set_report_refs")
+            self._report_refs.add((i, p))
+
+    def set_report_scoring(self, index_num: int, lam: float, K: float, full_ref: int, full_read: int):
+        """smr_set_report_scoring: Gumbel lambda / K and the corrected sizes (hostio.evalue_params) the BLAST E-values of index_num use"""
+        self._check(self.L.smr_set_report_scoring(self.h, C.c_uint32(index_num), C.c_double(lam), C.c_double(K), C.c_uint64(int(full_ref)),
+                                                  C.c_uint64(int(full_read))), "smr_set_report_scoring")
+
+    def format_reports(self, out: dict, text: bytes | None = None, opts: ReportOpts | None = None, **kw) -> dict:
+        """smr_format_reports: the report streams of one batch as bytes.  out = what align(with_stats=True) / download(with_stats=True)
+        returned for it; text = the batch's FASTA / FASTQ bytes (None: the resident text of upload_fastx[_gz]); opts = report_opts(...)
+        or its keyword arguments.  Returns {"sam": [bytes per group], "blast": [...], "aligned": bytes, "other": bytes, "denovo": bytes,
+        "groups": report_groups()}."""
+        o = opts if opts is not None else report_opts(**kw)
+        if o.sam or o.blast:
+            self._upload_report_refs()
+        groups = self.report_groups()
+        G = len(groups)
+        res, alns = out["res"], out["alns"]
+        cig = np.ascontiguousarray(out["cigar"], np.uint32)
+        st = out.get("stats")
+        txt = np.frombuffer(text, np.uint8) if text is not None else None
+        so = np.zeros(2 * G + 4, np.uint64)
+        L = self.L
+        L.smr_format_reports.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                                         C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
+        args = [self.h, C.cast(C.byref(o), C.c_void_p), _ptr(txt) if txt is not None and txt.size else None, txt.size if txt is not None else 0,
+                _ptr(res), _ptr(alns), _ptr(cig) if cig.size else None, cig.size, _ptr(st) if st is not None else None, res.shape[0]]
+        buf = getattr(self, "_report_buf", None)
+        if buf is None:
+            buf = np.zeros(1 << 20, np.uint8)
+        rc = L.smr_format_reports(*args, _ptr(buf), buf.size, _ptr(so))
+        if rc == 5 and int(so[-1]) > buf.size:   # SMR_ERR_CAPACITY: so names the size; grow and run again
+            buf = np.zeros(int(so[-1]) + (int(so[-1]) >> 3), np.uint8)
+            rc = L.smr_format_reports(*args, _ptr(buf), buf.size, _ptr(so))
+        self._check(rc, "smr_format_reports")
+        self._report_buf = buf
+        b = [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(2 * G + 3)]
+        return dict(sam=b[:G], blast=b[G:2 * G], aligned=b[2 * G], other=b[2 * G + 1], denovo=b[2 * G + 2], groups=groups)
+
+    def report_timings(self):
+        out = np.zeros(3, np.float64)
+        self._check(self.L.smr_last_report_timings(self.h, _ptr(out)), "smr_last_report_timings")
+        return dict(h2d_ms=out[0], device_ms=out[1], d2h_ms=out[2])
 
     def timings(self):
         out = np.zeros(8, np.float64)
@@ -392,6 +493,72 @@ class Aligner:
                                   C.c_uint32(filters), _ptr(out), _ptr(cig), C.c_uint32(cigar_cap))
         self._check(rc, "smr_debug_ssw")
         return out.reshape(n, 6), cig.reshape(n, cigar_cap)
+
+
+class ReportWriter:
+    """The reference's report files from batches of one read file: aligned.sam (header + rows), aligned.blast, aligned.<ext>,
+    other.<ext>, aligned_denovo.<ext> under out_dir (<ext> = fq for FASTQ input, fa for FASTA, report_fx_base.cpp:94).  Every stream of
+    every batch is appended to a part file of its own; close() concatenates them in the reference's order (all SAM rows of (index, part)
+    group 0, then group 1, ...), so that feeding a file in several batches writes what one batch writes.
+    sam_header: the text before the SAM rows (hostio.sam_header); opts: report_opts(...) keyword arguments."""
+
+    def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", **opts):
+        self.dir, self.al, self.header = out_dir, aligner, sam_header
+        self.opts = report_opts(**opts)
+        self.ext = None
+        self._parts = {}
+        os.makedirs(out_dir, exist_ok=True)
+
+    def _append(self, key, data):
+        fh = self._parts.get(key)
+        if fh is None:
+            fh = self._parts[key] = open(os.path.join(self.dir, f".part_{key}"), "w+b")
+        fh.write(data)
+
+    def write(self, out: dict, text: bytes | None = None) -> dict:
+        """format one batch (see Aligner.format_reports) and append its streams; returns them"""
+        if self.ext is None:
+            first = text[:1] if text is not None else self.al.resident_text()[:1]
+            self.ext = "fq" if first == b"@" else "fa"
+        s = self.al.format_reports(out, text, opts=self.opts)
+        for g, (rows_sam, rows_blast) in enumerate(zip(s["sam"], s["blast"])):
+            self._append(f"sam_{g}", rows_sam)
+            self._append(f"blast_{g}", rows_blast)
+        for k in ("aligned", "other", "denovo"):
+            self._append(k, s[k])
+        return s
+
+    def close(self) -> list:
+        """write the files; returns their paths"""
+        o, ext, groups = self.opts, self.ext or "fq", self.al.report_groups()
+        files = []
+        if o.sam:
+            files.append(("aligned.sam", [f"sam_{g}" for g in range(len(groups))], self.header.encode()))
+        if o.blast:
+            files.append(("aligned.blast", [f"blast_{g}" for g in range(len(groups))], b""))
+        for flag, name, key in ((o.fastx, "aligned", "aligned"), (o.other, "other", "other"), (o.denovo, "aligned_denovo", "denovo")):
+            if flag:
+                files.append((f"{name}.{ext}", [key], b""))
+        paths = []
+        for name, keys, head in files:
+            path = os.path.join(self.dir, name)
+            with open(path, "wb") as f:
+                f.write(head)
+                for k in keys:
+                    fh = self._parts.get(k)
+                    if fh is not None:
+                        fh.seek(0)
+                        while True:
+                            chunk = fh.read(1 << 24)
+                            if not chunk:
+                                break
+                            f.write(chunk)
+            paths.append(path)
+        for k, fh in self._parts.items():
+            fh.close()
+            os.unlink(os.path.join(self.dir, f".part_{k}"))
+        self._parts = {}
+        return paths
 
 
 def align_files(aligner: Aligner, batch: hostio.ReadBatch):

@@ -3,6 +3,7 @@
 #include "../../include/smr_b200.h"
 
 #include <algorithm>
+#include <cmath>
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
@@ -12,6 +13,7 @@
 #include <vector>
 
 #include "smr_decode.cuh"
+#include "smr_report.cuh"
 #include "smr_inflate.cuh"
 #include "smr_build.h"
 #include "smr_build_dev.cuh"
@@ -26,6 +28,7 @@ struct Part {
   DevIndex d{};
   std::vector<void*> owned;   // device allocations
   size_t bytes = 0, n_nodes = 0, n_entries = 0, n_ids = 0, n_pos = 0, n_refseq = 0;
+  const char* rnames = nullptr; const uint64_t* rname_off = nullptr; uint32_t n_rnames = 0; bool has_rnames = false;   // smr_set_report_refs
 };
 
 struct DevBuf {
@@ -78,6 +81,12 @@ struct smr_ctx {
   uint32_t scale = 1;         // scratch scale of the current run (1 = fast path)
   bool instr = false;         // smr_set_instrumentation: seed kernel counts windows / lists / entries, candidate kernel accounts its phases (clock64)
   uint64_t flag_hist[6] = {0, 0, 0, 0, 0, 0};  // overflow causes seen so far (seed lane / seed region / pairs / trace / cigar / error)
+  // report writer (smr_report.cuh)
+  struct RptScore { bool set = false; DevBuf ev, bits; };
+  std::vector<RptScore> rpt_score;   // per index_num (smr_set_report_scoring)
+  DevBuf r_text, r_nl, r_hdr, r_sb, r_rec, r_spos, r_line, r_recs, r_res, r_aln, r_cig, r_st, r_flags, r_keys, r_keys2, r_vals, r_rows, r_first,
+         r_sz, r_off, r_bsz, r_boff, r_fxsz, r_fxoff, r_grp, r_so, r_tmp, r_out, r_scal;
+  double t_rpt[3] = {0, 0, 0};
   // timings
   std::vector<cudaEvent_t> ev;
   double t_total = 0, t_seed = 0, t_lis = 0, t_final = 0, t_h2d = 0, t_d2h = 0; uint64_t n_launch = 0;
@@ -929,6 +938,213 @@ int align_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, ui
   return rc;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// report writer (smr_report.cuh)
+// ---------------------------------------------------------------------------------------------------------------------
+template <class T>
+int upload_async(smr_ctx* ctx, DevBuf& b, const T* src, size_t n) {
+  int rc;
+  if ((rc = ensure(ctx, b, n * sizeof(T) + 16))) return rc;
+  if (n) CK(cudaMemcpyAsync(b.p, src, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+  return SMR_OK;
+}
+
+int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
+                        const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                        char* out, uint64_t cap, uint64_t* so_out) {
+  if (o->out2 || o->sout) { ctx->err = "-out2 / -sout: the report writer writes one aligned and one other file"; return SMR_ERR_UNSUPPORTED; }
+  if (o->blast && o->blast_format != 1) { ctx->err = "only tabular BLAST (-blast 1) is written on the device"; return SMR_ERR_UNSUPPORTED; }
+  if (o->paired_in && o->paired_out) { ctx->err = "paired_in and paired_out are exclusive"; return SMR_ERR_ARG; }
+  const bool paired = o->paired_in || o->paired_out;
+  if (paired && (nreads & 1u)) { ctx->err = "a paired batch holds mates 2k and 2k+1: the number of reads must be even"; return SMR_ERR_ARG; }
+  if ((o->sam || o->blast || o->denovo) && nreads && !stats) { ctx->err = "SAM, BLAST and denovo need the smr_aln_stats of the batch"; return SMR_ERR_ARG; }
+  if (nreads && (!results || !alns)) return SMR_ERR_ARG;
+  uint32_t ncols = 0, cols[4] = {0, 0, 0, 0};
+  if (o->blast)
+    for (; ncols < 4 && o->blast_cols[ncols]; ++ncols) {
+      if (o->blast_cols[ncols] < SMR_BLAST_COL_CIGAR || o->blast_cols[ncols] > SMR_BLAST_COL_QSTRAND) { ctx->err = "unknown BLAST column"; return SMR_ERR_ARG; }
+      cols[ncols] = (uint32_t)o->blast_cols[ncols];
+    }
+  // groups: the loaded (index, part)s in the reference's report order
+  std::vector<const Part*> gp;
+  for (const Part& pt : ctx->parts) gp.push_back(&pt);
+  std::sort(gp.begin(), gp.end(), [](const Part* a, const Part* b) { return a->d.index_num != b->d.index_num ? a->d.index_num < b->d.index_num : a->d.part < b->d.part; });
+  const uint32_t G = (uint32_t)gp.size(), nso = 2 * G + 4;
+  std::vector<RptGroup> hg(G);
+  for (uint32_t g = 0; g < G; ++g) {
+    const Part& pt = *gp[g];
+    if ((o->sam || o->blast) && !pt.has_rnames) {
+      ctx->err = "smr_set_report_refs was not called for index " + std::to_string(pt.d.index_num) + " part " + std::to_string(pt.d.part);
+      return SMR_ERR_ARG;
+    }
+    const bool sc = pt.d.index_num < ctx->rpt_score.size() && ctx->rpt_score[pt.d.index_num].set;
+    if (o->blast && !sc) { ctx->err = "smr_set_report_scoring was not called for index " + std::to_string(pt.d.index_num); return SMR_ERR_ARG; }
+    hg[g] = RptGroup{pt.rnames, pt.rname_off, sc ? (const double*)ctx->rpt_score[pt.d.index_num].ev.p : nullptr,
+                     sc ? (const uint32_t*)ctx->rpt_score[pt.d.index_num].bits.p : nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0};
+  }
+  const uint32_t slots = slots_of(ctx);
+  const uint64_t N = (uint64_t)nreads * slots;
+  if (N >= (1ull << 31)) { ctx->err = "batch too large for the report writer: split it"; return SMR_ERR_ARG; }
+  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
+  int rc;
+  CK(cudaEventRecord(e0, ctx->stream));
+  // the text
+  const uint8_t* dt;
+  if (text) {
+    if ((rc = upload_async(ctx, ctx->r_text, (const uint8_t*)text, nbytes))) return rc;
+    dt = (const uint8_t*)ctx->r_text.p;
+  } else {
+    if (!ctx->text_bytes) { ctx->err = "no resident text: smr_upload_fastx[_gz] was not called, or pass the text"; return SMR_ERR_ARG; }
+    nbytes = ctx->text_bytes;
+    dt = (const uint8_t*)ctx->d_text.p;
+  }
+  char c0 = 0;
+  if (nbytes) {
+    if (nbytes >= 0xF0000000ull) { ctx->err = "text batch of 2^32 bytes or more: split it"; return SMR_ERR_ARG; }
+    if (text) c0 = text[0]; else CK(cudaMemcpy(&c0, dt, 1, cudaMemcpyDeviceToHost));
+    if (c0 != '@' && c0 != '>') { ctx->err = "reads text must start with '@' (FASTQ) or '>' (FASTA)"; return SMR_ERR_ARG; }
+  }
+  const uint32_t fmt = c0 == '@' ? kFmtFastq : kFmtFasta;
+  // results
+  if ((rc = upload_async(ctx, ctx->r_res, results, nreads))) return rc;
+  if ((rc = upload_async(ctx, ctx->r_aln, alns, N))) return rc;
+  if ((rc = upload_async(ctx, ctx->r_cig, cigar, cigar ? cigar_words : 0))) return rc;
+  if ((rc = upload_async(ctx, ctx->r_st, stats, stats ? N : 0))) return rc;
+  if ((rc = upload_async(ctx, ctx->r_grp, hg.data(), G))) return rc;
+  CK(cudaEventRecord(e1, ctx->stream));
+  // record layout: the line passes of smr_decode.cuh
+  const int grid = ctx->sm_count * 8;
+  if ((rc = ensure(ctx, ctx->r_scal, 64))) return rc;
+  uint32_t* scal = (uint32_t*)ctx->r_scal.p;   // [0] nlines [1] nrec [2] total nt [3] decode err [4] report err
+  CK(cudaMemsetAsync(scal, 0, 64, ctx->stream));
+  const uint64_t nchunks = nbytes / 32 + 1;
+  if ((rc = ensure(ctx, ctx->d_cnt, nchunks * 4))) return rc;
+  count_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, nbytes, (uint32_t*)ctx->d_cnt.p, nchunks);
+  if ((rc = device_scan(ctx, (const uint32_t*)ctx->d_cnt.p, (uint32_t*)ctx->d_cnt.p, nchunks, scal + 0))) return rc;
+  uint32_t h[8];
+  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  const uint32_t nlines = nbytes ? h[0] : 0;
+  if ((rc = ensure(ctx, ctx->r_nl, ((size_t)nlines + 1) * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->r_hdr, ((size_t)nlines + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_sb, ((size_t)nlines + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_rec, ((size_t)nlines + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_spos, ((size_t)nlines + 1) * 4))) return rc;
+  uint32_t nrec = 0;
+  if (nlines) {
+    write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, nbytes, (const uint32_t*)ctx->d_cnt.p, nchunks, (uint64_t*)ctx->r_nl.p);
+    line_info_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)ctx->r_nl.p, nlines, fmt, (uint32_t*)ctx->r_hdr.p, (uint32_t*)ctx->r_sb.p, scal + 3);
+    if ((rc = device_scan(ctx, (const uint32_t*)ctx->r_hdr.p, (uint32_t*)ctx->r_rec.p, nlines, scal + 1))) return rc;
+    if ((rc = device_scan(ctx, (const uint32_t*)ctx->r_sb.p, (uint32_t*)ctx->r_spos.p, nlines, scal + 2))) return rc;
+    CK(cudaMemcpyAsync((uint32_t*)ctx->r_spos.p + nlines, scal + 2, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (h[3]) { ctx->err = h[3] & kDecBadHeader ? "reads text: a record does not start with its header character" : "reads text: FASTQ separator line '+' missing"; return SMR_ERR_ARG; }
+    nrec = h[1];
+  }
+  if (nrec != nreads) { ctx->err = "the text holds " + std::to_string(nrec) + " records, the results " + std::to_string(nreads) + " reads"; return SMR_ERR_ARG; }
+  // per record, routing, row order
+  const uint64_t fstride = (uint64_t)nreads + 1;
+  if ((rc = ensure(ctx, ctx->r_line, fstride * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_recs, fstride * sizeof(RptRec)))) return rc;
+  if ((rc = ensure(ctx, ctx->r_flags, fstride * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_keys, (N + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_keys2, (N + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_vals, (N + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_rows, (N + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->r_first, ((size_t)G + 1) * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->r_sz, (N + 1) * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->r_off, (N + 1) * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->r_bsz, (N + 1) * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->r_boff, (N + 1) * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->r_fxsz, 3 * fstride * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->r_fxoff, 3 * fstride * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->r_so, (size_t)nso * 8))) return rc;
+  RptArgs a{};
+  a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)ctx->r_nl.p; a.spos = (const uint32_t*)ctx->r_spos.p; a.nlines = nlines; a.fastq = fmt == kFmtFastq;
+  a.rec = (const RptRec*)ctx->r_recs.p; a.nreads = nreads; a.slots = slots;
+  a.res = (const smr_read_result*)ctx->r_res.p; a.aln = (const smr_aln*)ctx->r_aln.p; a.cigar = (const uint32_t*)ctx->r_cig.p;
+  a.cigar_words = cigar ? cigar_words : 0; a.st = (const smr_aln_stats*)ctx->r_st.p;
+  a.grp = (const RptGroup*)ctx->r_grp.p; a.ngroups = G;
+  for (int k = 0; k < 4; ++k) a.cols[k] = cols[k];
+  a.ncols = ncols; a.min_id = o->min_id; a.min_cov = o->min_cov;
+  a.paired_in = o->paired_in != 0; a.paired_out = o->paired_out != 0; a.denovo = o->denovo != 0; a.err = scal + 4;
+  a.fx_mask = (o->fastx ? kRptAligned : 0u) | (o->other ? kRptOther : 0u) | (o->denovo ? kRptDenovo : 0u);
+  uint32_t* flags = (uint32_t*)ctx->r_flags.p;
+  uint64_t *first = (uint64_t*)ctx->r_first.p, *sz = (uint64_t*)ctx->r_sz.p, *off = (uint64_t*)ctx->r_off.p, *bsz = (uint64_t*)ctx->r_bsz.p,
+           *boff = (uint64_t*)ctx->r_boff.p, *fxsz = (uint64_t*)ctx->r_fxsz.p, *fxoff = (uint64_t*)ctx->r_fxoff.p, *so = (uint64_t*)ctx->r_so.p;
+  CK(cudaMemsetAsync(sz, 0, (N + 1) * 8, ctx->stream));
+  CK(cudaMemsetAsync(bsz, 0, (N + 1) * 8, ctx->stream));
+  CK(cudaMemsetAsync(fxsz, 0, 3 * fstride * 8, ctx->stream));
+  CK(cudaMemsetAsync(first, 0, ((size_t)G + 1) * 8, ctx->stream));
+  const uint32_t* rows = (const uint32_t*)ctx->r_rows.p;
+  if (nreads) {
+    rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->r_hdr.p, (const uint32_t*)ctx->r_rec.p, nlines, (uint32_t*)ctx->r_line.p);
+    rpt_records_kernel<<<grid, 256, 0, ctx->stream>>>(a, (const uint32_t*)ctx->r_line.p, (RptRec*)ctx->r_recs.p);
+    rpt_route_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags);
+    rpt_row_keys_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, (uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_vals.p);
+    int nbits = 1;
+    while ((1u << nbits) <= G) ++nbits;
+    size_t tsort = 0, tscan = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, tsort, (const uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_keys2.p, (const uint32_t*)ctx->r_vals.p,
+                                       (uint32_t*)ctx->r_rows.p, (int)N, 0, nbits, ctx->stream));
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, tscan, sz, off, (int)std::max<uint64_t>(N + 1, 3 * fstride), ctx->stream));
+    size_t tbytes = std::max(tsort, tscan);
+    if ((rc = ensure(ctx, ctx->r_tmp, tbytes))) return rc;
+    CK(cub::DeviceRadixSort::SortPairs(ctx->r_tmp.p, tsort, (const uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_keys2.p, (const uint32_t*)ctx->r_vals.p,
+                                       (uint32_t*)ctx->r_rows.p, (int)N, 0, nbits, ctx->stream));
+    rpt_group_first_kernel<<<(G + 128) / 128, 128, 0, ctx->stream>>>((const uint32_t*)ctx->r_keys2.p, N, G, first);
+    if (o->sam) rpt_sam_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, sz);
+    if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz, nullptr, nullptr);
+    if (o->fastx || o->other || o->denovo) {
+      rpt_fx_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, fxsz, fstride);
+    }
+    tscan = tbytes;
+    CK(cub::DeviceScan::ExclusiveSum(ctx->r_tmp.p, tscan, sz, off, (int)(N + 1), ctx->stream));
+    tscan = tbytes;
+    CK(cub::DeviceScan::ExclusiveSum(ctx->r_tmp.p, tscan, bsz, boff, (int)(N + 1), ctx->stream));
+    tscan = tbytes;
+    CK(cub::DeviceScan::ExclusiveSum(ctx->r_tmp.p, tscan, fxsz, fxoff, (int)(3 * fstride), ctx->stream));
+  } else {
+    CK(cudaMemsetAsync(off, 0, 8, ctx->stream));
+    CK(cudaMemsetAsync(boff, 0, 8, ctx->stream));
+    CK(cudaMemsetAsync(fxoff, 0, 3 * fstride * 8, ctx->stream));
+  }
+  rpt_stream_off_kernel<<<1, 32, 0, ctx->stream>>>(first, G, off, boff, fxoff, nreads, fstride, so);
+  CK(cudaGetLastError());
+  std::vector<uint64_t> hso(nso);
+  CK(cudaMemcpyAsync(hso.data(), so, (size_t)nso * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (h[4]) {
+    ctx->err = h[4] & kRptErrLen ? "an alignment's readlen or read_end1 disagrees with the length of its read in the text"
+             : h[4] & kRptErrGroup ? "an alignment names an (index, part) that is not loaded"
+             : h[4] & kRptErrRef ? "an alignment's ref_num is beyond the reference names of its part"
+             : h[4] & kRptErrQual ? "reads text: a FASTQ record without its quality line" : "an alignment's CIGAR lies outside cigar_words";
+    return SMR_ERR_ARG;
+  }
+  memcpy(so_out, hso.data(), (size_t)nso * 8);
+  const uint64_t total = hso[nso - 1];
+  if (total && (!out || cap < total)) { ctx->err = "output buffer too small: stream_off holds the sizes"; return SMR_ERR_CAPACITY; }
+  if (total) {
+    if ((rc = ensure(ctx, ctx->r_out, total))) return rc;
+    char* dout = (char*)ctx->r_out.p;
+    if (o->sam) rpt_sam_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, off, dout);
+    if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, nullptr, boff, dout + hso[G]);
+    if (o->fastx || o->other || o->denovo) rpt_fx_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, fxoff, fstride, so + 2 * G, dout);
+    CK(cudaGetLastError());
+  }
+  CK(cudaEventRecord(e2, ctx->stream));
+  if (total) CK(cudaMemcpyAsync(out, ctx->r_out.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e3, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
+  cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
+  cudaEventElapsedTime(&ms, e2, e3); ctx->t_rpt[2] = ms;
+  return SMR_OK;
+}
+
 }  // namespace
 
 extern "C" {
@@ -973,8 +1189,12 @@ void smr_destroy(smr_ctx* ctx) {
                     &ctx->parts_dev, &ctx->lis_arena, &ctx->lis_epochs, &ctx->lis_queue, &ctx->lis_done, &ctx->lis_rows, &ctx->lis_dbg, &ctx->final_arena, &ctx->lane_hits, &ctx->tb_arena, &ctx->tb_jobs, &ctx->aln_stats,
                     &ctx->d_text, &ctx->d_cnt, &ctx->d_scal, &ctx->d_nl, &ctx->d_hdr, &ctx->d_sb, &ctx->d_rec, &ctx->d_spos, &ctx->d_hdroff, &ctx->scan_sums,
                     &ctx->d_gz, &ctx->d_cand, &ctx->d_res, &ctx->d_sym, &ctx->d_win, &ctx->d_ids, &ctx->d_off, &ctx->d_cnt64,
-                    &ctx->d_moff, &ctx->d_mem, &ctx->d_poff, &ctx->d_plen, &ctx->d_pcrc, &ctx->seed_ctr};
+                    &ctx->d_moff, &ctx->d_mem, &ctx->d_poff, &ctx->d_plen, &ctx->d_pcrc, &ctx->seed_ctr,
+                    &ctx->r_text, &ctx->r_nl, &ctx->r_hdr, &ctx->r_sb, &ctx->r_rec, &ctx->r_spos, &ctx->r_line, &ctx->r_recs, &ctx->r_res, &ctx->r_aln,
+                    &ctx->r_cig, &ctx->r_st, &ctx->r_flags, &ctx->r_keys, &ctx->r_keys2, &ctx->r_vals, &ctx->r_rows, &ctx->r_first, &ctx->r_sz, &ctx->r_off,
+                    &ctx->r_bsz, &ctx->r_boff, &ctx->r_fxsz, &ctx->r_fxoff, &ctx->r_grp, &ctx->r_so, &ctx->r_tmp, &ctx->r_out, &ctx->r_scal};
   for (DevBuf* b : bufs) release(*b);
+  for (auto& sc : ctx->rpt_score) { release(sc.ev); release(sc.bits); }
   PinBuf* pins[] = {&ctx->h_state, &ctx->h_flags, &ctx->h_hitdb, &ctx->h_outaln, &ctx->h_stats, &ctx->h_cigar, &ctx->h_off32, &ctx->h_pkoff};
   for (PinBuf* b : pins) release(*b);
   for (cudaEvent_t e : ctx->ev) cudaEventDestroy(e);
@@ -1257,6 +1477,59 @@ int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, 
   if (cigar_used) *cigar_used = out.cigar_used;
   return rc;
 } SMR_CATCH(ctx)
+
+int smr_set_report_refs(smr_ctx* ctx, uint32_t index_num, uint32_t part, const char* names_cat, const uint64_t* name_off, uint32_t nref) try {
+  if (!ctx || !name_off || (!names_cat && name_off[nref])) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  for (Part& pt : ctx->parts) {
+    if (pt.d.index_num != index_num || pt.d.part != part) continue;
+    if (nref != pt.d.nref) { ctx->err = "smr_set_report_refs: " + std::to_string(nref) + " names for a part of " + std::to_string(pt.d.nref) + " references"; return SMR_ERR_ARG; }
+    std::vector<char> names(names_cat, names_cat + name_off[nref]);
+    std::vector<uint64_t> off(name_off, name_off + nref + 1);
+    int rc;
+    if ((rc = upload_vec(ctx, pt, names, &pt.rnames))) return rc;
+    if ((rc = upload_vec(ctx, pt, off, &pt.rname_off))) return rc;
+    pt.n_rnames = nref; pt.has_rnames = true;
+    return SMR_OK;
+  }
+  ctx->err = "smr_set_report_refs: index " + std::to_string(index_num) + " part " + std::to_string(part) + " is not loaded";
+  return SMR_ERR_ARG;
+} SMR_CATCH(ctx)
+
+int smr_set_report_scoring(smr_ctx* ctx, uint32_t index_num, double lambda, double K, uint64_t full_ref, uint64_t full_read) try {
+  if (!ctx || !(K > 0)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  if (ctx->rpt_score.size() <= index_num) ctx->rpt_score.resize(index_num + 1);
+  auto& sc = ctx->rpt_score[index_num];
+  std::vector<double> ev(65536);
+  std::vector<uint32_t> bits(65536);
+  for (uint32_t s = 0; s < 65536; ++s) {   // report_blast.cpp:117-126, operand order kept
+    const float b = (float)(lambda * s - std::log(K)) / (float)std::log(2);
+    bits[s] = b > 0 ? (uint32_t)b : 0u;
+    ev[s] = (double)K * full_ref * full_read * std::exp(-lambda * s);
+  }
+  int rc;
+  if ((rc = ensure(ctx, sc.ev, ev.size() * 8))) return rc;
+  if ((rc = ensure(ctx, sc.bits, bits.size() * 4))) return rc;
+  CK(cudaMemcpy(sc.ev.p, ev.data(), ev.size() * 8, cudaMemcpyHostToDevice));
+  CK(cudaMemcpy(sc.bits.p, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice));
+  sc.set = true;
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_format_reports(smr_ctx* ctx, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
+                       const smr_aln* alns, const uint32_t* cigar_pool, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                       char* out, uint64_t cap, uint64_t* stream_off) try {
+  if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  return format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off);
+} SMR_CATCH(ctx)
+
+int smr_last_report_timings(const smr_ctx* ctx, double out[3]) {
+  if (!ctx || !out) return SMR_ERR_ARG;
+  for (int k = 0; k < 3; ++k) out[k] = ctx->t_rpt[k];
+  return SMR_OK;
+}
 
 int smr_last_timings(const smr_ctx* ctx, double out[8]) {
   if (!ctx || !out) return SMR_ERR_ARG;

@@ -1,0 +1,392 @@
+// Report writer on the device: one batch's alignment results + the FASTA / FASTQ text of its reads -> the bytes the reference's
+// report stage writes for that batch (aligned.sam body rows, tabular aligned.blast rows, aligned / other / aligned_denovo reads).
+//   SAM rows      ReportSam::append (src/sortmerna/report_sam.cpp:64-152)
+//   BLAST rows    ReportBlast::append, tabular (report_blast.cpp:99-126, 260-346)
+//   read files    ReportFastx / ReportFxOther / ReportDenovo::append + ReportFxBase::write_a_read (report_fastx.cpp:56-140,
+//                 report_fx_other.cpp:50-120, report_denovo.cpp:57-130, report_fx_base.cpp:176-181), routing of output.cpp:117-142
+// Layout of the text: the newline index / line classification / scans of smr_decode.cuh, then one thread per record (rpt_records_kernel).
+// Every output is made in two passes: a size pass (bytes of every row / record), an exclusive scan (cub) into offsets, a write pass.
+// SAM and BLAST rows are ordered (index, part) group first, then read, then alignment slot (output.cpp:196-237) by a stable radix sort
+// of the live alignment slots on their group.  SEQ and QUAL of a SAM row and the records of the read files are copied by a whole warp,
+// so a 30 kb read is not serialised on one thread; the short fields are printed by one lane with smr_fmt.h.
+#pragma once
+#include <cstdint>
+
+#include <cub/cub.cuh>
+
+#include "../../include/smr_b200.h"
+#include "smr_decode.cuh"
+#include "smr_fmt.h"
+
+namespace smr {
+
+// one record of the reads text
+struct RptRec {
+  uint64_t hdr;          // offset of the header line
+  uint64_t qual;         // FASTQ: offset of the quality line
+  uint32_t hdr_len;      // header without trailing white space (Readfeed right-trims every line, readfeed.cpp:579-582)
+  uint32_t name_beg, name_len;   // Read::getSeqId (read.cpp:371-377): up to the first space, leading '>' / '@' removed
+  uint32_t line, next;   // line of the header; line of the next record's header (or the number of lines)
+  uint32_t seq_len, qual_len;
+  uint32_t verbatim;     // FASTQ record already in output form (header\nseq\n+\nqual\n): written as one copy
+};
+
+// one loaded (index, part): what its rows print
+struct RptGroup {
+  const char* names;          // reference ids, concatenated
+  const uint64_t* name_off;   // [nref + 1]
+  const double* evalue;       // [65536] E-value of each score1 (host-computed, report_blast.cpp:121-126)
+  const uint32_t* bits;       // [65536] bit score of each score1 (report_blast.cpp:117-119)
+  uint32_t nref, index_num, part, pad;
+};
+
+enum : uint32_t { kRptAligned = 1, kRptOther = 2, kRptDenovo = 4, kRptSkip = 8 };
+enum : uint32_t { kRptErrLen = 1, kRptErrGroup = 2, kRptErrRef = 4, kRptErrQual = 8, kRptErrCigar = 16 };
+enum : uint32_t { kColCigar = 1, kColQcov = 2, kColQstrand = 3 };
+
+struct RptArgs {
+  const uint8_t* text; uint64_t nbytes;
+  const uint64_t* nl; const uint32_t* spos; uint32_t nlines, fastq;
+  const RptRec* rec; uint32_t nreads, slots;
+  const smr_read_result* res; const smr_aln* aln; const uint32_t* cigar; uint64_t cigar_words; const smr_aln_stats* st;
+  const RptGroup* grp; uint32_t ngroups;
+  uint32_t cols[4], ncols;
+  double min_id, min_cov;
+  uint32_t paired_in, paired_out, denovo;
+  uint32_t fx_mask;   // the read files asked for (kRptAligned | kRptOther | kRptDenovo)
+  uint32_t* err;
+};
+
+__device__ __forceinline__ uint64_t rpt_line_beg(const uint64_t* nl, uint32_t i) { return i ? nl[i - 1] + 1 : 0; }
+__device__ __forceinline__ bool rpt_space(uint8_t c) { return c == ' ' || (c >= '\t' && c <= '\r'); }
+
+// headers: rec_line[rec_idx[i]] = i
+__global__ void rpt_header_lines_kernel(const uint32_t* __restrict__ is_hdr, const uint32_t* __restrict__ rec_idx, uint32_t nlines,
+                                        uint32_t* __restrict__ rec_line) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < nlines; i += gridDim.x * blockDim.x)
+    if (is_hdr[i]) rec_line[rec_idx[i]] = i;
+}
+
+__global__ void rpt_records_kernel(RptArgs a, const uint32_t* __restrict__ rec_line, RptRec* __restrict__ out) {
+  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.nreads; r += gridDim.x * blockDim.x) {
+    RptRec o{};
+    o.line = rec_line[r];
+    o.next = r + 1 < a.nreads ? rec_line[r + 1] : a.nlines;
+    const uint64_t s = rpt_line_beg(a.nl, o.line);
+    uint64_t e = a.nl[o.line];
+    while (e > s && rpt_space(a.text[e - 1])) --e;
+    o.hdr = s; o.hdr_len = (uint32_t)(e - s);
+    uint32_t sp = 0;
+    while (sp < o.hdr_len && a.text[s + sp] != ' ') ++sp;
+    uint32_t nb = 0;
+    while (nb < sp && (a.text[s + nb] == '>' || a.text[s + nb] == '@')) ++nb;
+    o.name_beg = nb; o.name_len = sp - nb;
+    o.seq_len = a.spos[o.next] - a.spos[o.line];
+    if (a.fastq) {
+      if (o.line + 3 >= a.nlines) { atomicOr(a.err, kRptErrQual); out[r] = o; continue; }
+      const uint64_t qs = rpt_line_beg(a.nl, o.line + 3);
+      uint64_t qe = a.nl[o.line + 3];
+      while (qe > qs && rpt_space(a.text[qe - 1])) --qe;
+      o.qual = qs; o.qual_len = (uint32_t)(qe - qs);
+      const uint64_t out_len = (uint64_t)o.hdr_len + o.seq_len + o.qual_len + 5;
+      o.verbatim = a.nl[o.line + 3] < a.nbytes && a.nl[o.line + 3] + 1 - s == out_len;   // no CR, no trailing blanks, bare '+'
+    }
+    out[r] = o;
+  }
+}
+
+// counting / writing output cursor: p == nullptr counts only
+struct RptSink {
+  char* p; uint64_t n;
+  __device__ void c(char x) { if (p) p[n] = x; ++n; }
+  __device__ void s(const char* x, uint32_t k) { if (p) for (uint32_t i = 0; i < k; ++i) p[n + i] = x[i]; n += k; }
+  __device__ void u(uint64_t v) { char t[24]; s(t, (uint32_t)fmt::put_u64(t, v)); }
+  __device__ void i(int64_t v) { char t[24]; s(t, (uint32_t)fmt::put_i64(t, v)); }
+  __device__ void g3(double v) { char t[24]; s(t, (uint32_t)fmt::fmt_g3(v, t)); }
+};
+
+__device__ __forceinline__ uint32_t rpt_group_of(const RptArgs& a, const smr_aln& al) {
+  for (uint32_t g = 0; g < a.ngroups; ++g)
+    if (a.grp[g].index_num == al.index_num && a.grp[g].part == al.part) return g;
+  return a.ngroups;
+}
+
+// CIGAR with the soft clips of report_sam.cpp:99-116 / report_blast.cpp:318-337
+__device__ void rpt_cigar(RptSink& o, const RptArgs& a, const smr_aln& al, uint32_t read_len) {
+  if (al.read_begin1 != 0) { o.i(al.read_begin1); o.c('S'); }
+  if ((uint64_t)al.cigar_off + al.cigar_len > a.cigar_words) { atomicOr(a.err, kRptErrCigar); return; }
+  for (uint32_t c = 0; c < al.cigar_len; ++c) {
+    const uint32_t w = a.cigar[al.cigar_off + c], op = w & 0xF;
+    o.u(w >> 4);
+    o.c(op == 0 ? 'M' : op == 1 ? 'I' : 'D');
+  }
+  const int64_t end_mask = (int64_t)read_len - al.read_end1 - 1;
+  if (end_mask > 0) { o.i(end_mask); o.c('S'); }
+}
+
+__device__ __forceinline__ void rpt_ref_name(RptSink& o, const RptArgs& a, const RptGroup& g, uint32_t ref_num) {
+  if (ref_num >= g.nref) { atomicOr(a.err, kRptErrRef); return; }
+  const uint64_t b = g.name_off[ref_num];
+  o.s(g.names + b, (uint32_t)(g.name_off[ref_num + 1] - b));
+}
+
+// per read: routing to aligned / other / aligned_denovo and the skip of empty reads (output.cpp:117-142)
+__device__ bool rpt_is_denovo(const RptArgs& a, uint32_t r) {   // denovo_stats_run (processor.cpp:329-357), as hostio.denovo_classes
+  const uint32_t n = a.res[r].n_align;
+  if (n == 0) return false;
+  for (uint32_t k = 0; k < n; ++k) {
+    const smr_aln& al = a.aln[(size_t)r * a.slots + k];
+    const smr_aln_stats& st = a.st[(size_t)r * a.slots + k];
+    const double id = (double)st.n_match_denovo / (double)(st.n_miss + st.n_gap + st.n_match);
+    const int32_t span = al.read_end1 - al.read_begin1 + 1;
+    const double cov = (double)(span < 0 ? -span : span) / (double)al.readlen;
+    const bool is_id = floor(__dadd_rn(__dmul_rn(id, 1000.0), 0.5)) / 1000.0 >= a.min_id;   // no FMA: the host rounds twice
+    const bool is_cov = floor(__dadd_rn(__dmul_rn(cov, 1000.0), 0.5)) / 1000.0 >= a.min_cov;
+    if (is_id || is_cov) return false;
+  }
+  return true;
+}
+
+__global__ void rpt_route_kernel(RptArgs a, uint32_t* __restrict__ flags) {
+  const bool paired = a.paired_in || a.paired_out;
+  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.nreads; r += gridDim.x * blockDim.x) {
+    const uint32_t m = paired ? (r ^ 1u) : r;
+    const bool empty = a.rec[paired ? (r | 1u) : r].seq_len == 0;   // Readfeed pairs: only the second read is checked (output.cpp:120)
+    if (empty) { flags[r] = kRptSkip; continue; }
+    const bool h = a.res[r].is_hit, hm = a.res[m].is_hit;
+    uint32_t f = 0;
+    if (!paired) {
+      f |= h ? kRptAligned : kRptOther;
+    } else {
+      const bool h0 = (r & 1u) ? hm : h, h1 = (r & 1u) ? h : hm;
+      if (a.paired_out ? (h0 && h1) : (h0 || h1)) f |= kRptAligned;
+      if (!(h0 && h1) && (a.paired_out || !(h0 || h1))) f |= kRptOther;
+    }
+    if (a.denovo) {
+      const bool d = rpt_is_denovo(a, r);
+      if (!paired) { if (d) f |= kRptDenovo; }
+      else if ((d || rpt_is_denovo(a, m)) && (a.paired_in || d)) f |= kRptDenovo;
+    }
+    flags[r] = f & a.fx_mask;
+  }
+}
+
+// live alignment slots: key = group (ngroups = not written), value = slot
+__global__ void rpt_row_keys_kernel(RptArgs a, const uint32_t* __restrict__ flags, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
+  const uint64_t n = (uint64_t)a.nreads * a.slots;
+  for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t r = (uint32_t)(i / a.slots), k = (uint32_t)(i % a.slots);
+    uint32_t key = a.ngroups;
+    if (k < a.res[r].n_align && !(flags[r] & kRptSkip)) {
+      const smr_aln& al = a.aln[i];
+      key = rpt_group_of(a, al);
+      if (key == a.ngroups) atomicOr(a.err, kRptErrGroup);
+      if (al.readlen != a.rec[r].seq_len || al.read_end1 >= (int32_t)a.rec[r].seq_len) atomicOr(a.err, kRptErrLen);
+    }
+    keys[i] = key; vals[i] = (uint32_t)i;
+  }
+}
+
+// first[g] = first sorted row of group g (lower bound); first[ngroups] = number of rows
+__global__ void rpt_group_first_kernel(const uint32_t* __restrict__ keys, uint64_t n, uint32_t ngroups, uint64_t* __restrict__ first) {
+  const uint32_t g = blockIdx.x * blockDim.x + threadIdx.x;
+  if (g > ngroups) return;
+  uint64_t lo = 0, hi = n;
+  while (lo < hi) { const uint64_t mid = (lo + hi) / 2; if (keys[mid] < g) lo = mid + 1; else hi = mid; }
+  first[g] = lo;
+}
+
+// ---- SAM ----
+// QUAL of a row: ReportSam::append reverses read.quality IN PLACE for every minus-strand alignment (report_sam.cpp:125-129), and the
+// read object lives for one (index, part) pass: the quality is printed reversed iff an odd number of this read's minus-strand
+// alignments of the same (index, part), up to this one, came before in alignv order.
+__device__ bool rpt_qual_reversed(const RptArgs& a, uint32_t r, uint32_t k) {
+  const smr_aln& al = a.aln[(size_t)r * a.slots + k];
+  uint32_t flips = 0;
+  for (uint32_t j = 0; j <= k; ++j) {
+    const smr_aln& b = a.aln[(size_t)r * a.slots + j];
+    flips += b.index_num == al.index_num && b.part == al.part && !b.strand;
+  }
+  return flips & 1u;
+}
+
+__device__ void rpt_sam_prefix(RptSink& o, const RptArgs& a, const RptRec& rc, const smr_aln& al, uint32_t g) {
+  o.s((const char*)a.text + rc.hdr + rc.name_beg, rc.name_len);
+  o.s(al.strand ? "\t0\t" : "\t16\t", al.strand ? 3 : 4);
+  rpt_ref_name(o, a, a.grp[g], al.ref_num);
+  o.c('\t'); o.i((int64_t)al.ref_begin1 + 1);
+  o.s("\t255\t", 5);
+  rpt_cigar(o, a, al, rc.seq_len);
+  o.s("\t*\t0\t0\t", 7);
+}
+__device__ void rpt_sam_suffix(RptSink& o, const RptArgs& a, const smr_aln& al, const smr_aln_stats& st) {
+  o.s("\tAS:i:", 6); o.u(al.score1);
+  o.s("\tNM:i:", 6); o.u((uint64_t)st.n_miss + st.n_gap);
+  o.c('\n');
+}
+
+__global__ void rpt_sam_size_kernel(RptArgs a, const uint32_t* __restrict__ rows, const uint64_t* __restrict__ first, uint64_t* __restrict__ size) {
+  const uint64_t n = first[a.ngroups];
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t i = rows[j], r = i / a.slots;
+    const smr_aln& al = a.aln[i];
+    const RptRec& rc = a.rec[r];
+    RptSink o{nullptr, 0};
+    rpt_sam_prefix(o, a, rc, al, rpt_group_of(a, al));
+    rpt_sam_suffix(o, a, al, a.st[i]);
+    size[j] = o.n + rc.seq_len + 1 + (a.fastq ? rc.qual_len : 1);
+  }
+}
+
+// byte p of a record's sequence (FASTA sequences may span several lines)
+struct RptSeqLines {
+  const RptArgs& a; const RptRec& rc;
+  // calls f(text offset, offset in the sequence, count) for every sequence line, by lane: lanes share the work of each line
+  template <class F> __device__ void each(F f) const {
+    for (uint32_t l = rc.line + 1; l < (a.fastq ? rc.line + 2 : rc.next); ++l) {
+      const uint32_t off = a.spos[l] - a.spos[rc.line], cnt = a.spos[l + 1] - a.spos[l];
+      if (cnt) f(rpt_line_beg(a.nl, l), off, cnt);
+    }
+  }
+};
+
+__device__ __forceinline__ char rpt_nt(uint8_t c, bool rc) {   // nt_table (common.hpp:68-77) then ACGTN, complemented for the minus strand
+  c &= 0xDF;
+  const int v = c == 'A' ? 0 : c == 'C' ? 1 : c == 'G' ? 2 : (c == 'T' || c == 'U') ? 3 : 4;
+  return "ACGTN"[rc && v < 4 ? 3 - v : v];
+}
+
+__global__ void __launch_bounds__(256) rpt_sam_write_kernel(RptArgs a, const uint32_t* __restrict__ rows, const uint64_t* __restrict__ first,
+                                                            const uint64_t* __restrict__ off, char* __restrict__ out) {
+  const uint64_t n = first[a.ngroups];
+  const unsigned lane = lane_id();
+  for (uint64_t j = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n; j += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
+    const uint32_t i = rows[j], r = i / a.slots;
+    const smr_aln al = a.aln[i];
+    const RptRec rc = a.rec[r];
+    char* dst = out + off[j];
+    uint64_t plen = 0;
+    if (lane == 0) {
+      RptSink o{dst, 0};
+      rpt_sam_prefix(o, a, rc, al, rpt_group_of(a, al));
+      plen = o.n;
+    }
+    plen = __shfl_sync(kFull, plen, 0);
+    const bool minus = !al.strand;
+    const uint32_t L = rc.seq_len;
+    char* seq = dst + plen;
+    RptSeqLines{a, rc}.each([&](uint64_t src, uint32_t so, uint32_t cnt) {
+      for (uint32_t k = lane; k < cnt; k += 32) {
+        const uint32_t p = so + k;
+        seq[minus ? L - 1 - p : p] = rpt_nt(a.text[src + k], minus);
+      }
+    });
+    char* q = seq + L;
+    if (lane == 0) q[0] = '\t';
+    ++q;
+    uint32_t qlen = 1;
+    if (a.fastq) {
+      qlen = rc.qual_len;
+      const bool rev = rpt_qual_reversed(a, r, i % a.slots);
+      for (uint32_t k = lane; k < qlen; k += 32) q[rev ? qlen - 1 - k : k] = (char)a.text[rc.qual + k];
+    } else if (lane == 0) {
+      q[0] = '*';
+    }
+    if (lane == 0) {
+      RptSink o{q + qlen, 0};
+      rpt_sam_suffix(o, a, al, a.st[i]);
+    }
+  }
+}
+
+// ---- tabular BLAST (one thread per row) ----
+__device__ void rpt_blast_row(RptSink& o, const RptArgs& a, const RptRec& rc, const smr_aln& al, const smr_aln_stats& st, uint32_t g) {
+  const RptGroup& G = a.grp[g];
+  o.s((const char*)a.text + rc.hdr + rc.name_beg, rc.name_len); o.c('\t');
+  rpt_ref_name(o, a, G, al.ref_num); o.c('\t');
+  o.g3((double)st.n_match / (double)(st.n_miss + st.n_gap + st.n_match) * 100); o.c('\t');
+  o.i((int64_t)al.read_end1 - al.read_begin1 + 1); o.c('\t');
+  o.u(st.n_miss); o.c('\t');
+  o.u(st.n_gap); o.c('\t');
+  o.i((int64_t)al.read_begin1 + 1); o.c('\t');
+  o.i((int64_t)al.read_end1 + 1); o.c('\t');
+  o.i((int64_t)al.ref_begin1 + 1); o.c('\t');
+  o.i((int64_t)al.ref_end1 + 1); o.c('\t');
+  o.g3(G.evalue[al.score1]); o.c('\t');
+  o.u(G.bits[al.score1]);
+  for (uint32_t c = 0; c < a.ncols; ++c) {
+    o.c('\t');
+    if (a.cols[c] == kColCigar) {
+      rpt_cigar(o, a, al, rc.seq_len);
+    } else if (a.cols[c] == kColQcov) {
+      const int32_t span = al.read_end1 - al.read_begin1 + 1;
+      o.g3((double)(span < 0 ? -span : span) / (double)al.readlen * 100);
+    } else {
+      o.c(al.strand ? '+' : '-');
+    }
+  }
+  o.c('\n');
+}
+
+__global__ void rpt_blast_kernel(RptArgs a, const uint32_t* __restrict__ rows, const uint64_t* __restrict__ first, uint64_t* __restrict__ size,
+                                 const uint64_t* __restrict__ off, char* __restrict__ out) {
+  const uint64_t n = first[a.ngroups];
+  for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
+    const uint32_t i = rows[j];
+    const smr_aln& al = a.aln[i];
+    RptSink o{out ? out + off[j] : nullptr, 0};
+    rpt_blast_row(o, a, a.rec[i / a.slots], al, a.st[i], rpt_group_of(a, al));
+    if (size) size[j] = o.n;
+  }
+}
+
+// ---- aligned / other / aligned_denovo reads: write_a_read (report_fx_base.cpp:176-181) ----
+__global__ void rpt_fx_size_kernel(RptArgs a, const uint32_t* __restrict__ flags, uint64_t* __restrict__ size, uint64_t stride) {
+  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.nreads; r += gridDim.x * blockDim.x) {
+    const RptRec& rc = a.rec[r];
+    const uint64_t len = (uint64_t)rc.hdr_len + rc.seq_len + 2 + (a.fastq ? rc.qual_len + 3 : 0);
+    const uint32_t f = flags[r];
+    size[r] = f & kRptAligned ? len : 0;   // route masked the files not asked for
+    size[stride + r] = f & kRptOther ? len : 0;
+    size[2 * stride + r] = f & kRptDenovo ? len : 0;
+  }
+}
+
+__device__ __forceinline__ void rpt_warp_copy(char* dst, const uint8_t* src, uint64_t n, unsigned lane) {
+  for (uint64_t k = lane; k < n; k += 32) dst[k] = (char)src[k];
+}
+
+// off: one exclusive scan over the sizes of the three files (stride nreads + 1), so off already includes the files before; *base = start of
+// the first read file in the output
+__global__ void __launch_bounds__(256) rpt_fx_write_kernel(RptArgs a, const uint32_t* __restrict__ flags, const uint64_t* __restrict__ off,
+                                                           uint64_t stride, const uint64_t* __restrict__ base, char* __restrict__ out) {
+  const unsigned lane = lane_id();
+  for (uint32_t r = (blockIdx.x * blockDim.x + threadIdx.x) >> 5; r < a.nreads; r += (gridDim.x * blockDim.x) >> 5) {
+    const uint32_t f = flags[r];
+    const RptRec rc = a.rec[r];
+    for (uint32_t s = 0; s < 3; ++s) {
+      if (!(f & (1u << s))) continue;
+      char* dst = out + base[0] + off[s * stride + r];
+      if (rc.verbatim) { rpt_warp_copy(dst, a.text + rc.hdr, (uint64_t)rc.hdr_len + rc.seq_len + rc.qual_len + 5, lane); continue; }
+      rpt_warp_copy(dst, a.text + rc.hdr, rc.hdr_len, lane);
+      char* seq = dst + rc.hdr_len + 1;
+      RptSeqLines{a, rc}.each([&](uint64_t src, uint32_t so, uint32_t cnt) { rpt_warp_copy(seq + so, a.text + src, cnt, lane); });
+      char* q = seq + rc.seq_len;
+      if (lane == 0) { dst[rc.hdr_len] = '\n'; q[0] = '\n'; if (a.fastq) { q[1] = '+'; q[2] = '\n'; q[3 + rc.qual_len] = '\n'; } }
+      if (a.fastq) rpt_warp_copy(q + 3, a.text + rc.qual, rc.qual_len, lane);
+    }
+  }
+}
+
+// stream offsets: SAM groups, BLAST groups, aligned, other, denovo (2 * ngroups + 4 entries)
+__global__ void rpt_stream_off_kernel(const uint64_t* __restrict__ first, uint32_t ngroups, const uint64_t* __restrict__ sam_off,
+                                      const uint64_t* __restrict__ blast_off, const uint64_t* __restrict__ fx_off, uint32_t nreads, uint64_t stride,
+                                      uint64_t* __restrict__ so) {
+  if (threadIdx.x != 0 || blockIdx.x != 0) return;
+  const uint64_t sam_total = sam_off[first[ngroups]];
+  for (uint32_t g = 0; g <= ngroups; ++g) so[g] = sam_off[first[g]];
+  for (uint32_t g = 0; g <= ngroups; ++g) so[ngroups + g] = sam_total + blast_off[first[g]];
+  for (uint32_t s = 0; s < 3; ++s) so[2 * ngroups + 1 + s] = so[2 * ngroups] + fx_off[s * stride + nreads];   // fx_off: one scan over the three
+}
+
+}  // namespace smr

@@ -177,6 +177,28 @@ def parse_stats(prefix: str) -> IndexStats:
     return IndexStats(prefix, fsize, name, freq, full_ref, lnwin, numseq, nparts, parts)
 
 
+def sam_header(prefixes: list, cmdline: str, sq: bool = False) -> str:
+    """The header of aligned.sam (ReportSam::write_header, report_sam.cpp:154-205): @HD, with sq (-SQ) one @SQ line per reference
+    sequence of every index in --ref order (read from the sequence table after the part table of <prefix>.stats), and @PG with the
+    command line."""
+    out = ["@HD\tVN:1.0\tSO:unsorted\n"]
+    for prefix in prefixes:
+        with open(prefix + ".stats", "rb") as fh:
+            b = fh.read()
+        o = 8
+        (nlen,) = struct.unpack_from("<I", b, o); o += 4 + nlen + 32 + 8 + 4 + 8
+        (nparts,) = struct.unpack_from("<H", b, o); o += 2 + 24 * nparts
+        (num_sq,) = struct.unpack_from("<I", b, o); o += 4
+        for _ in range(num_sq):
+            (lid,) = struct.unpack_from("<I", b, o); o += 4
+            sid = b[o:o + lid].decode(); o += lid
+            (lseq,) = struct.unpack_from("<I", b, o); o += 4
+            if sq:
+                out.append(f"@SQ\tSN:{sid}\tLN:{lseq}\n")
+    out.append(f"@PG\tID:sortmerna\tVN:1.0\tCL:{cmdline}\n")
+    return "".join(out)
+
+
 def find_index_prefixes(idx_dir: str) -> dict:
     """Map reference FASTA basename -> index prefix for every *.stats in idx_dir."""
     out = {}
