@@ -1,5 +1,5 @@
 // Index builder on the device: reference sequences (2-bit codes) -> the resident arrays the kernels read (DevIndex: flookup,
-// flist, pos_off, pos), without the on-disk files in between.  Stands in for build_index + Index::load
+// ftext, fid, pos_off, pos), without the on-disk files in between.  Stands in for build_index + Index::load
 // (src/sortmerna/indexdb.cpp:1119-2095, src/sortmerna/index.cpp:143-357) (SURVEY 8(f)(3)); the host builder smr_build.cpp writes
 // the files, this one makes the same index content where it is used.
 //
@@ -155,14 +155,15 @@ __global__ void bld_level_kernel(const uint64_t* __restrict__ key, const uint32_
   }
 }
 
-// flist in final order + the lookup rows
+// the entry texts and ids in final order + the lookup rows
 __global__ void bld_flist_kernel(const uint32_t* __restrict__ perm, const uint32_t* __restrict__ e_list, const uint32_t* __restrict__ e_text,
-                                 const uint32_t* __restrict__ e_id, uint32_t n, uint2* flist, uint32_t* flookup /*4 words per kmer*/, int pass) {
+                                 const uint32_t* __restrict__ e_id, uint32_t n, uint32_t* ftext, uint32_t* fid, uint32_t* flookup /*4 words per kmer*/, int pass) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const uint32_t e = perm[i], l = e_list[e];
   if (pass == 0) {
-    flist[i] = make_uint2(e_text[e], e_id[e]);
+    ftext[i] = e_text[e];
+    fid[i] = e_id[e];
     if (i == 0 || e_list[perm[i - 1]] != l) flookup[(size_t)(l >> 1) * 4 + 2 * (l & 1u)] = i;
   } else if (i == n - 1 || e_list[perm[i + 1]] != l) {
     const size_t at = (size_t)(l >> 1) * 4 + 2 * (l & 1u);

@@ -128,7 +128,7 @@ void release(PinBuf& b) { if (b.p) cudaFreeHost(b.p); b.p = nullptr; b.cap = 0; 
 template <class T>
 int upload_vec(smr_ctx* ctx, Part& pt, const std::vector<T>& v, const T** out) {
   void* d = nullptr;
-  size_t bytes = v.size() * sizeof(T) + 64;   // the seed kernel reads whole aligned groups of four list entries
+  size_t bytes = v.size() * sizeof(T) + 64;   // 64 zero bytes of slack past the end of every array
   CK(cudaMalloc(&d, bytes));
   CK(cudaMemset(d, 0, bytes));
   if (!v.empty()) CK(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
@@ -225,7 +225,7 @@ int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const st
   uint32_t npos = 0;
   CK(cudaMemcpyAsync(&npos, u3 + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  void *p_posoff = nullptr, *p_pos = nullptr, *p_flist = nullptr, *p_flookup = nullptr, *p_ref = nullptr, *p_roff = nullptr;
+  void *p_posoff = nullptr, *p_pos = nullptr, *p_ftext = nullptr, *p_fid = nullptr, *p_flookup = nullptr, *p_ref = nullptr, *p_roff = nullptr;
   CK(keep_alloc(&p_posoff, ((size_t)nids + 1) * 4)); CK(keep_alloc(&p_pos, (size_t)npos * 8));
   bld_poswrite_kernel<<<gw, tb, 0, st>>>(keyB, u1, u2, u3, d_wstart, g, nids, (uint32_t*)p_posoff, (uint2*)p_pos);
   CK(cudaGetLastError());
@@ -244,9 +244,9 @@ int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const st
   }
   // 5. the lists and their lookup rows
   const size_t nk = (size_t)1 << (2 * g.half);
-  CK(keep_alloc(&p_flist, (size_t)E * 8)); CK(keep_alloc(&p_flookup, nk * 16));
-  bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, (uint2*)p_flist, (uint32_t*)p_flookup, 0);
-  bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, (uint2*)p_flist, (uint32_t*)p_flookup, 1);
+  CK(keep_alloc(&p_ftext, ftext_words(E) * 4)); CK(keep_alloc(&p_fid, (size_t)E * 4)); CK(keep_alloc(&p_flookup, nk * 16));
+  bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, (uint32_t*)p_ftext, (uint32_t*)p_fid, (uint32_t*)p_flookup, 0);
+  bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, (uint32_t*)p_ftext, (uint32_t*)p_fid, (uint32_t*)p_flookup, 1);
   CK(cudaGetLastError());
   // 6. references for the Smith-Waterman side
   CK(keep_alloc(&p_ref, c04.size())); CK(keep_alloc(&p_roff, roff.size() * 4));
@@ -254,7 +254,7 @@ int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const st
   CK(cudaMemcpyAsync(p_roff, roff.data(), roff.size() * 4, cudaMemcpyHostToDevice, st));
   CK(cudaStreamSynchronize(st));
   pt.d.lnwin = g.L; pt.d.partialwin = g.half; pt.d.nref = g.nseq; pt.d.nids = nids;
-  pt.d.flookup = (const uint4*)p_flookup; pt.d.flist = (const uint2*)p_flist; pt.d.pos_off = (const uint32_t*)p_posoff; pt.d.pos = (const uint2*)p_pos;
+  pt.d.flookup = (const uint4*)p_flookup; pt.d.ftext = (const uint32_t*)p_ftext; pt.d.fid = (const uint32_t*)p_fid; pt.d.pos_off = (const uint32_t*)p_posoff; pt.d.pos = (const uint2*)p_pos;
   pt.d.refseq = (const uint8_t*)p_ref; pt.d.ref_off = (const uint32_t*)p_roff;
   pt.n_entries = E; pt.n_ids = nids; pt.n_pos = npos; pt.n_refseq = c04.size();
   return SMR_OK;
@@ -1228,16 +1228,19 @@ int smr_load_index_part(smr_ctx* ctx, uint32_t index_num, uint32_t part, const v
   for (uint32_t i = 0; i <= nref; ++i) roff[i] = (uint32_t)(ref_off[i] - ref_off[0]);
   std::vector<uint8_t> rseq(refseq_cat + ref_off[0], refseq_cat + ref_off[nref]);
   rseq.resize(rseq.size() + 64, 4);
+  std::vector<uint32_t> ftext(ftext_words(fx.flist.size()), 0), fid(fx.flist.size());
+  for (size_t i = 0; i < fx.flist.size(); ++i) { ftext[i] = fx.flist[i].tail; fid[i] = fx.flist[i].id; }   // an flist item's tail holds the full text
   int rc;
-  const uint32_t* lk = nullptr; const Entry* en = nullptr; const uint32_t* po = nullptr; const SeqPos* ps = nullptr;
+  const uint32_t *lk = nullptr, *ft = nullptr, *fi = nullptr, *po = nullptr; const SeqPos* ps = nullptr;
   const uint8_t* rs = nullptr; const uint32_t* ro = nullptr;
   if ((rc = upload_vec(ctx, pt, fx.flookup, &lk))) return rc;
-  if ((rc = upload_vec(ctx, pt, fx.flist, &en))) return rc;
+  if ((rc = upload_vec(ctx, pt, ftext, &ft))) return rc;
+  if ((rc = upload_vec(ctx, pt, fid, &fi))) return rc;
   if ((rc = upload_vec(ctx, pt, fx.pos_off, &po))) return rc;
   if ((rc = upload_vec(ctx, pt, fx.pos, &ps))) return rc;
   if ((rc = upload_vec(ctx, pt, rseq, &rs))) return rc;
   if ((rc = upload_vec(ctx, pt, roff, &ro))) return rc;
-  pt.d.flookup = (const uint4*)lk; pt.d.flist = (const uint2*)en; pt.d.pos_off = po; pt.d.pos = (const uint2*)ps;
+  pt.d.flookup = (const uint4*)lk; pt.d.ftext = ft; pt.d.fid = fi; pt.d.pos_off = po; pt.d.pos = (const uint2*)ps;
   pt.d.refseq = rs; pt.d.ref_off = ro;
   pt.n_refseq = rseq.size();
   pt.n_nodes = fx.nodes.size(); pt.n_entries = fx.entries.size(); pt.n_ids = pt.d.nids; pt.n_pos = fx.pos.size();
@@ -1294,7 +1297,7 @@ int smr_debug_index_array(smr_ctx* ctx, uint32_t slot, uint32_t which, void* out
   const void* src = nullptr; uint64_t n = 0;
   switch (which) {
     case 0: src = pt.d.flookup; n = ((uint64_t)16) << (2 * pt.d.partialwin); break;
-    case 1: src = pt.d.flist; n = (uint64_t)pt.n_entries * 8; break;
+    case 1: n = (uint64_t)pt.n_entries * 8; break;   // {text, id} pairs, interleaved below
     case 2: src = pt.d.pos_off; n = ((uint64_t)pt.n_ids + 1) * 4; break;
     case 3: src = pt.d.pos; n = (uint64_t)pt.n_pos * 8; break;
     case 4: src = pt.d.refseq; n = pt.n_refseq; break;
@@ -1304,6 +1307,14 @@ int smr_debug_index_array(smr_ctx* ctx, uint32_t slot, uint32_t which, void* out
   *nbytes = n;
   if (!out) return SMR_OK;
   if (cap_bytes < n) { ctx->err = "buffer too small"; return SMR_ERR_CAPACITY; }
+  if (which == 1) {
+    std::vector<uint32_t> text(pt.n_entries), id(pt.n_entries), pairs(2 * pt.n_entries);
+    if (n) CK(cudaMemcpy(text.data(), pt.d.ftext, n / 2, cudaMemcpyDeviceToHost));
+    if (n) CK(cudaMemcpy(id.data(), pt.d.fid, n / 2, cudaMemcpyDeviceToHost));
+    for (size_t i = 0; i < pt.n_entries; ++i) { pairs[2 * i] = text[i]; pairs[2 * i + 1] = id[i]; }
+    if (n) memcpy(out, pairs.data(), n);
+    return SMR_OK;
+  }
   if (n) CK(cudaMemcpy(out, src, n, cudaMemcpyDeviceToHost));
   return SMR_OK;
 }

@@ -17,13 +17,17 @@ struct DevIndex {
   uint32_t nref, nids;
   uint32_t is_last;          // last (index,part) in --ref order (paralleltraversal.cpp:294)
   uint32_t slot;             // ordinal of this part in the context
-  const uint4* flookup;      // [4^partialwin] {offF, cntF, offR, cntR} into flist
-  const uint2* flist;        // {text (path + tail, partialwin+1 chars, first char lowest), id}, DFS order per (9-mer, direction)
+  const uint4* flookup;      // [4^partialwin] {offF, cntF, offR, cntR}: entry indices into ftext and fid
+  const uint32_t* ftext;     // entry texts (path + tail, partialwin+1 chars, first char lowest), DFS order per (9-mer, direction);
+                             // zero-padded to a multiple of 8 entries (the seed kernel reads whole aligned 32-byte chunks)
+  const uint32_t* fid;       // entry ids, same order
   const uint32_t* pos_off;   // [nids+1]
   const uint2* pos;          // {pos, seq}, each id's list sorted by (seq,pos)
   const uint8_t* refseq;     // 0..4
   const uint32_t* ref_off;   // [nref+1]
 };
+// words allocated for the texts of n entries
+__host__ __device__ inline size_t ftext_words(size_t n) { return (n + 7) & ~(size_t)7; }
 
 struct DevParams {
   int32_t match, mismatch, score_N, gap_open, gap_ext;

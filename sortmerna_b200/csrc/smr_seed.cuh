@@ -32,8 +32,8 @@ namespace smr {
 //   * a window search classifies EVERY entry of the list of its 9-mer with three bit-parallel predicates
 //     (smr_levbits.h) -- entries in sub-tries the reference would have pruned simply classify as "no match",
 //     so the outcome is the same, and the ~2.4x more entries cost less than the pruning did;
-//   * the 32 windows of a round are searched together: their lists form one entry stream, one entry per lane
-//     per step (coalesced 8-byte loads, no divergence); the few matching entries are compacted with
+//   * the 32 windows of a round are searched together: their lists form one entry stream, eight entry texts per
+//     lane per step (one aligned 32-byte sector, no divergence); the few matching entries are compacted with
 //     ballot/popc into a shared list and each lane then replays the reference's order-dependent rules
 //     (0-error exit, per-window de-duplication, traverse_bursttrie.cpp:249-281) over its own matches.
 // ---------------------------------------------------------------------------------------------
@@ -93,11 +93,12 @@ __device__ __forceinline__ uint32_t pass_class(uint32_t p, uint32_t s0, uint32_t
   return 3;
 }
 
-constexpr int kAccCap = 256;   // matching entries buffered per flush (a step adds at most 128)
+constexpr int kAccStep = 256;  // matching entries one step can add (32 lanes x 8 entries)
+constexpr int kAccCap = 384;   // matching entries buffered: a step that leaves more than kAccCap - kAccStep flushes, so the next one fits
 
 struct CoopSmem {              // per warp
-  uint4 tab[64];               // the non-empty lists of a round in stream order: {first group - first chunk, pattern, first entry, end entry}
-  uint32_t id[kAccCap];        // matching entries in stream order: id, text, owner
+  uint4 tab[64];               // the non-empty lists of a round in stream order: {first chunk - first stream chunk, pattern, first entry, end entry}
+  uint32_t id[kAccCap];        // matching entries in stream order: entry index (its id once the flush has loaded it), text, owner
   uint32_t text[kAccCap];
   uint8_t meta[kAccCap];       // owner lane | 32 for a mirror list
   uint8_t own[64];             // the same for list k
@@ -110,12 +111,13 @@ struct CoopSmem {              // per warp
 //   (b) mirror: trie_R list of the second half, pattern = first half (:188-240) -- the reference runs (b) only without a
 //       0-error hit in (a); here every (a) list precedes every (b) list in the stream and a lane stops replaying its matches
 //       at its 0-error hit, so streaming (b) regardless changes nothing but the entries read (~5 % of the windows).
-// The unit of work is a CHUNK = one aligned group of four 8-byte entries (one 32-byte sector, two 16-byte loads): a lane
-// finds the list of its chunk once (REDUX.OR of the lists that start in this step + popc, one shared-memory row) and tests
-// four entries with within_one_edit().  Matching entries (text, id, owner) are compacted in stream order; at a flush every lane
+// The unit of work is a CHUNK = the texts of one aligned group of eight entries (one 32-byte sector of ix.ftext, two 16-byte
+// loads): a lane finds the list of its chunk once (REDUX.OR of the lists that start in this step + popc, one shared-memory row)
+// and tests eight texts with within_one_edit().  The ids are not streamed: matching entries (text, entry index, owner) are
+// compacted in stream order, and at a flush the lanes first load the ids of all buffered matches from ix.fid, then every lane
 // finds the (at most two) runs of its own matches and replays them -- exact classification and the reference's order-dependent
 // rules (0-error exit, per-window de-duplication, traverse_bursttrie.cpp:249-281) -- all lanes in parallel.
-// offF/cntF/PF, offR/cntR/PR: the lane's two lists in ix.flist (cnt == 0: none).  Appends to lh; sets zero.
+// offF/cntF/PF, offR/cntR/PR: the lane's two lists, entry indices into ix.ftext / ix.fid (cnt == 0: none).  Appends to lh; sets zero.
 template <bool INSTR>
 __device__ void coop_stream(const DevIndex& ix, CoopSmem& sm, const uint32_t offF, const uint32_t cntF, const uint32_t PF,
                             const uint32_t offR, const uint32_t cntR, const uint32_t PR, const bool full_search,
@@ -123,12 +125,12 @@ __device__ void coop_stream(const DevIndex& ix, CoopSmem& sm, const uint32_t off
   const unsigned lane = lane_id();
   const uint32_t pw = ix.partialwin;
   const LevMasks km = lev_masks(pw);
-  const uint4* __restrict__ fl4 = reinterpret_cast<const uint4*>(ix.flist);   // group g = fl4[2g], fl4[2g+1]
-  const uint32_t gF = offF >> 2, nF = cntF ? ((offF + cntF + 3u) >> 2) - gF : 0u;
-  const uint32_t gR = offR >> 2, nR = cntR ? ((offR + cntR + 3u) >> 2) - gR : 0u;
+  const uint4* __restrict__ ft4 = reinterpret_cast<const uint4*>(ix.ftext);   // chunk g = ft4[2g], ft4[2g+1]
+  const uint32_t gF = offF >> 3, nF = cntF ? ((offF + cntF + 7u) >> 3) - gF : 0u;
+  const uint32_t gR = offR >> 3, nR = cntR ? ((offR + cntR + 7u) >> 3) - gR : 0u;
   const uint32_t inF = warp_incl_scan_u32(nF), inR = warp_incl_scan_u32(nR);
   const uint32_t totF = __shfl_sync(kFull, inF, 31), E = totF + __shfl_sync(kFull, inR, 31);
-  const uint32_t exF = inF - nF, exR = totF + inR - nR;
+  const uint32_t exF = nF ? inF - nF : kNoneDev, exR = nR ? totF + inR - nR : kNoneDev;   // first stream chunk of each list (none: never starts)
   if (INSTR) { st.entries += cntF + cntR; st.lists += (cntF ? 1u : 0u) + (cntR ? 1u : 0u); }
   if (E == 0) return;
   const uint32_t lt = (1u << lane) - 1u, le = lt | (1u << lane);
@@ -139,56 +141,61 @@ __device__ void coop_stream(const DevIndex& ix, CoopSmem& sm, const uint32_t off
   }
   __syncwarp();
   uint32_t cum = 0, nacc = 0;
-  // the chunk of a lane in step e0: its list (row k of the table) and its two 16-byte loads -- issued one step ahead of their use
-  uint32_t kn; uint4 tn, q0n, q1n; bool inn;
+  // the chunk of a lane in step e0: its list (row k of the table), its chunk g, the list's pattern and its two 16-byte loads --
+  // issued one step ahead of their use (the list's bounds are read from the table only when the chunk has a match)
+  uint32_t kn, gn, Pn; uint4 q0n, q1n;
   auto fetch = [&](const uint32_t e0) {
     const uint32_t dF = exF - e0, dR = exR - e0;   // a list that began in an earlier step wraps to a huge value
-    const uint32_t bit = ((nF && dF < 32u) ? (1u << dF) : 0u) | ((nR && dR < 32u) ? (1u << dR) : 0u);
+    const uint32_t bit = (dF < 32u ? (1u << dF) : 0u) | (dR < 32u ? (1u << dR) : 0u);
     const uint32_t starts = __reduce_or_sync(kFull, bit);
     const uint32_t e = e0 + lane;
     kn = cum + __popc(starts & le) - 1u;      // the list of chunk e (step 0 always has a list starting at chunk 0)
     cum += __popc(starts);
-    inn = e < E;
-    tn = sm.tab[kn];
-    const uint32_t g = tn.x + e;
+    const uint2 t = *reinterpret_cast<const uint2*>(&sm.tab[kn]);
+    gn = t.x + e; Pn = t.y;
     q0n = make_uint4(0, 0, 0, 0); q1n = q0n;
-    if (inn) { q0n = __ldg(fl4 + 2 * (size_t)g); q1n = __ldg(fl4 + 2 * (size_t)g + 1); }
-    tn.x = g;
+    if (e < E) { q0n = __ldg(ft4 + 2 * (size_t)gn); q1n = __ldg(ft4 + 2 * (size_t)gn + 1); }
   };
   fetch(0);
   for (uint32_t e0 = 0; e0 < E; e0 += 32) {
-    const uint32_t k = kn; const uint4 t = tn, q0 = q0n, q1 = q1n; const bool in = inn;
-    const uint32_t g = t.x;
+    const uint32_t k = kn, g = gn, P = Pn; const uint4 q0 = q0n, q1 = q1n;
     if (e0 + 32 < E) fetch(e0 + 32);
-    const bool m0 = within_one_edit(t.y, q0.x, km), m1 = within_one_edit(t.y, q0.z, km);
-    const bool m2 = within_one_edit(t.y, q1.x, km), m3 = within_one_edit(t.y, q1.z, km);
-    const bool any = in && (m0 | m1 | m2 | m3);
+    const uint32_t hit8 = (within_one_edit(P, q0.x, km) ? 1u : 0u) | (within_one_edit(P, q0.y, km) ? 2u : 0u) |
+                          (within_one_edit(P, q0.z, km) ? 4u : 0u) | (within_one_edit(P, q0.w, km) ? 8u : 0u) |
+                          (within_one_edit(P, q1.x, km) ? 16u : 0u) | (within_one_edit(P, q1.y, km) ? 32u : 0u) |
+                          (within_one_edit(P, q1.z, km) ? 64u : 0u) | (within_one_edit(P, q1.w, km) ? 128u : 0u);
+    const bool any = e0 + lane < E && hit8;
     const unsigned am = __ballot_sync(kFull, any);
     if (am) {   // entries outside [first, end) of the list dropped, matches compacted in stream order (lane-major, then entry)
       uint32_t mk = 0;
+      const uint32_t i0 = 8u * g;
       if (any) {
-        const uint32_t i0 = 4u * g;
-        const uint32_t lo = t.z > i0 ? min(t.z - i0, 4u) : 0u, hi = min(t.w - i0, 4u);
-        mk = ((m0 ? 1u : 0u) | (m1 ? 2u : 0u) | (m2 ? 4u : 0u) | (m3 ? 8u : 0u)) & ((1u << hi) - 1u) & ~((1u << lo) - 1u);
+        const uint2 t = *reinterpret_cast<const uint2*>(&sm.tab[k].z);
+        const uint32_t lo = t.x > i0 ? min(t.x - i0, 8u) : 0u, hi = min(t.y - i0, 8u);
+        mk = hit8 & ((1u << hi) - 1u) & ~((1u << lo) - 1u);
       }
       const uint32_t nm = __popc(mk);
-      const unsigned b0 = __ballot_sync(kFull, nm & 1u), b1 = __ballot_sync(kFull, nm & 2u), b2 = __ballot_sync(kFull, nm & 4u);
-      uint32_t slot = nacc + __popc(b0 & lt) + 2u * __popc(b1 & lt) + 4u * __popc(b2 & lt);
+      const unsigned b0 = __ballot_sync(kFull, nm & 1u), b1 = __ballot_sync(kFull, nm & 2u), b2 = __ballot_sync(kFull, nm & 4u),
+                     b3 = __ballot_sync(kFull, nm & 8u);
+      uint32_t slot = nacc + __popc(b0 & lt) + 2u * __popc(b1 & lt) + 4u * __popc(b2 & lt) + 8u * __popc(b3 & lt);
       const uint8_t own = sm.own[k];
       while (mk) {
         const uint32_t j = (uint32_t)__ffs((int)mk) - 1u;
         mk &= mk - 1u;
-        sm.text[slot] = j == 0 ? q0.x : (j == 1 ? q0.z : (j == 2 ? q1.x : q1.z));
-        sm.id[slot] = j == 0 ? q0.y : (j == 1 ? q0.w : (j == 2 ? q1.y : q1.w));
+        const uint4 q = j < 4 ? q0 : q1;
+        const uint32_t jj = j & 3u;
+        sm.text[slot] = jj == 0 ? q.x : (jj == 1 ? q.y : (jj == 2 ? q.z : q.w));
+        sm.id[slot] = i0 + j;
         sm.meta[slot] = own;
         ++slot;
       }
-      nacc += __popc(b0) + 2u * __popc(b1) + 4u * __popc(b2);
+      nacc += __popc(b0) + 2u * __popc(b1) + 4u * __popc(b2) + 8u * __popc(b3);
     }
-    if (nacc && (nacc > (uint32_t)kAccCap - 128u || e0 + 32 >= E)) {   // flush
+    if (nacc && (nacc > (uint32_t)(kAccCap - kAccStep) || e0 + 32 >= E)) {   // flush
       sm.run[0][0][lane] = 0; sm.run[0][1][lane] = 0; sm.run[1][0][lane] = 0; sm.run[1][1][lane] = 0;
       __syncwarp();
       for (uint32_t i = lane; i < nacc; i += 32) {   // a list's matches are contiguous: mark where each (owner, direction) run begins and ends
+        sm.id[i] = __ldg(ix.fid + sm.id[i]);
         const uint32_t m = sm.meta[i];
         const uint32_t prev = i ? sm.meta[i - 1] : 0xFFu, next = i + 1 < nacc ? sm.meta[i + 1] : 0xFFu;
         if (m != prev) sm.run[m >> 5][0][m & 31u] = (uint16_t)i;
@@ -433,10 +440,10 @@ seed_debug_kernel(DevIndex ix, const uint8_t* seq03, const uint32_t* seq_off, co
     coop_stream<false>(ix, sm, lf.x, lf.y, Pf, lr.z, lr.w, Pr, full, lh, z, st);
   } else if (active) {
     const uint4 lf = __ldg(&ix.flookup[keyf]);
-    for (uint32_t i = 0; i < lf.y && !z; ++i) { const uint2 en = __ldg(ix.flist + lf.x + i); z = apply_entry(classify_bits(Pf, en.x, pw), en.y, full, lh); }
+    for (uint32_t i = lf.x; i < lf.x + lf.y && !z; ++i) z = apply_entry(classify_bits(Pf, __ldg(ix.ftext + i), pw), __ldg(ix.fid + i), full, lh);
     if (!z) {
       const uint4 lr = __ldg(&ix.flookup[keyr]);
-      for (uint32_t i = 0; i < lr.w && !z; ++i) { const uint2 en = __ldg(ix.flist + lr.z + i); z = apply_entry(classify_bits(Pr, en.x, pw), en.y, full, lh); }
+      for (uint32_t i = lr.z; i < lr.z + lr.w && !z; ++i) z = apply_entry(classify_bits(Pr, __ldg(ix.ftext + i), pw), __ldg(ix.fid + i), full, lh);
     }
   }
   if (active) {
