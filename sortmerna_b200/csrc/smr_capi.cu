@@ -61,7 +61,7 @@ struct smr_ctx {
   DevBuf seq04, seq_off, pk03, pk03alt, pk_off, has_n, hit_cnt, flags, state, hit_db, aln_work, out_aln;
   DevBuf hits, cost, bins, scalars, counters, cigar_pool, parts_dev;
   size_t hits_stride = 0; uint32_t cnt_stride = 0;
-  DevBuf lis_arena, lis_epochs, lis_queue, lis_done, lis_rows, lis_dbg, final_arena, lane_hits, tb_arena, tb_jobs, aln_stats;
+  DevBuf lis_arena, lis_epochs, lis_queue, lis_done, lis_rows, lis_dbg, final_arena, lane_hits, tb_arena, tb_jobs, fin_list, aln_stats;
   smr_aln_stats* host_stats = nullptr;   // optional output of the report arithmetic
   PinBuf h_state, h_flags, h_hitdb, h_outaln, h_stats, h_cigar, h_off32, h_pkoff;
   std::vector<uint64_t> h_coff;
@@ -277,11 +277,12 @@ cudaEvent_t get_event(smr_ctx* ctx, size_t i) {
   return ctx->ev[i];
 }
 
-// scalars block layout (u32): [0]=work_n [1]=lis work_next [2]=final work_next [3]=lis work_next of the second cursor ; cigar_used (u64) at byte 16 ; task queue cursors at 128..
-struct Scalars { uint32_t* work_n; uint32_t* lis_next; uint32_t* fin_next; uint32_t* lis_next_b; unsigned long long* cigar_used; uint32_t* q_head; uint32_t* q_tail; uint32_t* planners_done; };
+// scalars block layout (u32): [0]=work_n [1]=lis work_next [2]=final work_next [3]=lis work_next of the second cursor ; cigar_used (u64) at byte 16 ;
+// finalize job count (u32) at byte 24 ; task queue cursors at 128..
+struct Scalars { uint32_t* work_n; uint32_t* lis_next; uint32_t* fin_next; uint32_t* lis_next_b; unsigned long long* cigar_used; uint32_t* fin_jobs; uint32_t* q_head; uint32_t* q_tail; uint32_t* planners_done; };
 Scalars scalars_of(smr_ctx* ctx) {
   uint8_t* p = (uint8_t*)ctx->scalars.p;
-  return Scalars{(uint32_t*)p, (uint32_t*)(p + 4), (uint32_t*)(p + 8), (uint32_t*)(p + 12), (unsigned long long*)(p + 16), (uint32_t*)(p + 128), (uint32_t*)(p + 256), (uint32_t*)(p + 384)};
+  return Scalars{(uint32_t*)p, (uint32_t*)(p + 4), (uint32_t*)(p + 8), (uint32_t*)(p + 12), (unsigned long long*)(p + 16), (uint32_t*)(p + 24), (uint32_t*)(p + 128), (uint32_t*)(p + 256), (uint32_t*)(p + 384)};
 }
 
 int setup_arenas(smr_ctx* ctx) {
@@ -744,6 +745,7 @@ int run_impl(smr_ctx* ctx) {
     }
     // finalize this chunk
     CK(cudaMemsetAsync(sc.fin_next, 0, 4, ctx->stream));
+    CK(cudaMemsetAsync(sc.fin_jobs, 0, 4, ctx->stream));
     cudaEvent_t f0 = get_event(ctx, evi), f1 = get_event(ctx, evi + 1); evi += 2;
     CK(cudaEventRecord(f0, ctx->stream));
     FinalGlobals fg{};
@@ -753,6 +755,8 @@ int run_impl(smr_ctx* ctx) {
     fg.slots = slots; fg.cigar_pool = (uint32_t*)ctx->cigar_pool.p; fg.cigar_cap = ctx->cigar_cap_dev; fg.cigar_used = sc.cigar_used;
     fg.work_next = sc.fin_next;
     if ((rc = ensure(ctx, ctx->tb_jobs, (size_t)n * slots * sizeof(TraceJob)))) return rc;
+    if ((rc = ensure(ctx, ctx->fin_list, (size_t)n * slots * 4))) return rc;
+    fg.job_list = (uint32_t*)ctx->fin_list.p; fg.job_count = sc.fin_jobs;
     fg.jobs = (TraceJob*)ctx->tb_jobs.p; fg.tb_arena = (uint8_t*)ctx->tb_arena.p; fg.tb_stride = ctx->tb_stride;
     fg.tb_cap_w = ctx->tb_cap_w; fg.tb_cap_cig = ctx->tb_cap_cig; fg.tb_cap_dir = ctx->tb_cap_dir;
     fg.stats = nullptr;
@@ -760,11 +764,13 @@ int run_impl(smr_ctx* ctx) {
       if ((rc = ensure(ctx, ctx->aln_stats, (size_t)nreads * slots * sizeof(AlnStats)))) return rc;
       fg.stats = (AlnStats*)ctx->aln_stats.p;
     }
+    final_jobs_kernel<<<std::min<uint32_t>((n * slots + 255) / 256, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(b, fg);
+    CK(cudaGetLastError());
     finalize_kernel<<<ctx->final_warps / kFinalWarpsPerCta, kFinalWarpsPerCta * 32, 0, ctx->stream>>>(b, dp, fg);
     CK(cudaGetLastError());
     traceback_kernel<<<ctx->tb_threads / 128, 128, 0, ctx->stream>>>(b, dp, fg);
     CK(cudaGetLastError());
-    ctx->n_launch += 1;
+    ctx->n_launch += 2;
     CK(cudaEventRecord(f1, ctx->stream));
     spans.push_back({evi - 2, 1});
     ctx->n_launch += 1;
@@ -1186,7 +1192,7 @@ void smr_destroy(smr_ctx* ctx) {
   for (auto& pt : ctx->parts) for (void* p : pt.owned) cudaFree(p);
   DevBuf* bufs[] = {&ctx->seq04, &ctx->seq_off, &ctx->pk03, &ctx->pk03alt, &ctx->pk_off, &ctx->has_n, &ctx->hit_cnt, &ctx->flags, &ctx->state,
                     &ctx->hit_db, &ctx->aln_work, &ctx->out_aln, &ctx->hits, &ctx->cost, &ctx->bins, &ctx->scalars, &ctx->counters, &ctx->cigar_pool,
-                    &ctx->parts_dev, &ctx->lis_arena, &ctx->lis_epochs, &ctx->lis_queue, &ctx->lis_done, &ctx->lis_rows, &ctx->lis_dbg, &ctx->final_arena, &ctx->lane_hits, &ctx->tb_arena, &ctx->tb_jobs, &ctx->aln_stats,
+                    &ctx->parts_dev, &ctx->lis_arena, &ctx->lis_epochs, &ctx->lis_queue, &ctx->lis_done, &ctx->lis_rows, &ctx->lis_dbg, &ctx->final_arena, &ctx->lane_hits, &ctx->tb_arena, &ctx->tb_jobs, &ctx->fin_list, &ctx->aln_stats,
                     &ctx->d_text, &ctx->d_cnt, &ctx->d_scal, &ctx->d_nl, &ctx->d_hdr, &ctx->d_sb, &ctx->d_rec, &ctx->d_spos, &ctx->d_hdroff, &ctx->scan_sums,
                     &ctx->d_gz, &ctx->d_cand, &ctx->d_res, &ctx->d_sym, &ctx->d_win, &ctx->d_ids, &ctx->d_off, &ctx->d_cnt64,
                     &ctx->d_moff, &ctx->d_mem, &ctx->d_poff, &ctx->d_plen, &ctx->d_pcrc, &ctx->seed_ctr,

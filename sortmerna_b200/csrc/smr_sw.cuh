@@ -398,16 +398,28 @@ __device__ __forceinline__ bool sw_pair_ok(const int32_t m, const int32_t n, con
 __device__ __forceinline__ uint32_t pack16(const int32_t lo, const int32_t hi) { return ((uint32_t)lo & 0xFFFFu) | ((uint32_t)hi << 16); }
 
 constexpr int kPairRP = 4;   // row pairs per lane in the profile layout (fixed: one layout for every R <= 8)
+constexpr uint32_t kPairNoHit = 0x7FFFFFFFu;
+constexpr uint32_t kPairNoTarget = 0x7FFFu;          // a target no 15-bit score reaches: the half is not searched
 
-template <int R>
-__device__ __noinline__ uint32_t sw_pair_warp(const uint32_t* __restrict__ profA, const uint32_t* __restrict__ profB, const uint8_t* __restrict__ refA,
-                                              const uint8_t* __restrict__ refB, const int32_t nmax, const SwScore sc) {
+// FIND = false: returns the packed best scores (A low, B high).
+// FIND = true: `tgt2` packs the (known) best score of each problem; returns, per problem, the first cell holding it in the reference's
+// order (smallest column, then smallest row: ssw.c:310-336) as column<<16 | row, or kPairNoHit.  Every cell is <= its problem's
+// maximum, so "a cell of this column holds the target" is "the lane's running maximum reached the target in this step": the
+// running maximum of the score pass is compared with the target once per step, and a lane's rows are only searched in the
+// step where one of its halves first reaches it -- that column is the lane's first hit column, and the smallest row holding the
+// target there is its hit.  Sentinel columns and dead rows stay strictly below any positive target (see sw_score_warp).
+template <int R, bool FIND = false>
+__device__ __noinline__ auto sw_pair_warp(const uint32_t* __restrict__ profA, const uint32_t* __restrict__ profB, const uint8_t* __restrict__ refA,
+                                          const uint8_t* __restrict__ refB, const int32_t nmax, const SwScore sc, const uint32_t tgt2 = 0) {
   constexpr int RP = (R + 1) / 2;
   const int lane = (int)lane_id();
   uint32_t Hp[R], E[R];
 #pragma unroll
   for (int r = 0; r < R; ++r) { Hp[r] = 0; E[r] = 0; }
   uint32_t diagH = 0, upH = 0, upF = 0, best = 0;
+  // FIND: need1 = target - 1 per half still searched (0x7FFE once found): the sign bit of need1 - best is set where best >= target
+  uint32_t need1 = __vsub2(tgt2, 0x00010001u), foundA = kPairNoHit, foundB = kPairNoHit;
+  (void)need1; (void)foundA; (void)foundB;
   const uint8_t* cpA = refA + 32 - lane;
   const uint8_t* cpB = refB + 32 - lane;
   const uint32_t* pA = profA + lane;
@@ -470,12 +482,38 @@ __device__ __noinline__ uint32_t sw_pair_warp(const uint32_t* __restrict__ profA
 #pragma unroll
     for (int r = 0; r + 1 < R; r += 2) best = __vimax3_s16x2(best, Hp[r], Hp[r + 1]);
     if (R & 1) best = __vmaxs2(best, Hp[R - 1]);
+    if constexpr (FIND) {
+      const uint32_t reached = __vsub2(need1, best) & 0x80008000u;
+      if (reached) {   // once per half and lane at most
+        const uint32_t col = (uint32_t)(ts - lane) << 16;
+        if (reached & 0x8000u) {
+          int rr = R;
+#pragma unroll
+          for (int r = R - 1; r >= 0; --r) if (((Hp[r] ^ tgt2) & 0xFFFFu) == 0u) rr = r;
+          if (rr < R) foundA = col | (uint32_t)(lane * R + rr);
+          need1 = (need1 & 0xFFFF0000u) | (kPairNoTarget - 1u);
+        }
+        if (reached & 0x80000000u) {
+          int rr = R;
+#pragma unroll
+          for (int r = R - 1; r >= 0; --r) if (((Hp[r] ^ tgt2) >> 16) == 0u) rr = r;
+          if (rr < R) foundB = col | (uint32_t)(lane * R + rr);
+          need1 = (need1 & 0xFFFFu) | ((kPairNoTarget - 1u) << 16);
+        }
+      }
+    }
 #pragma unroll
     for (int r = 0; r < R; ++r) sc_cur[r] = sc_next[r];
   }
+  if constexpr (FIND) {
 #pragma unroll
-  for (int o = 16; o > 0; o >>= 1) best = __vmaxs2(best, __shfl_xor_sync(kFull, best, o));
-  return best;
+    for (int o = 16; o > 0; o >>= 1) { foundA = min(foundA, __shfl_xor_sync(kFull, foundA, o)); foundB = min(foundB, __shfl_xor_sync(kFull, foundB, o)); }
+    return make_uint2(foundA, foundB);
+  } else {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) best = __vmaxs2(best, __shfl_xor_sync(kFull, best, o));
+    return best;
+  }
 }
 
 // query profile of one problem for the packed pass: R rows per lane (run-time), m real rows; one copy of this code serves every R.
@@ -519,6 +557,61 @@ __device__ __forceinline__ uint32_t sw_pair_dispatch(const int R, const uint32_t
     case 6: return sw_pair_warp<6>(pa, pb, ra, rb, nmax, sc);
     default: return sw_pair_warp<8>(pa, pb, ra, rb, nmax, sc);
   }
+}
+
+__device__ __forceinline__ uint2 sw_pair_find_dispatch(const int R, const uint32_t* pa, const uint32_t* pb, const uint8_t* wa, const uint8_t* wb, const int32_t nmax,
+                                                       const SwScore sc, const uint32_t tgt2) {
+  const uint8_t* ra = wa - 32; const uint8_t* rb = wb - 32;
+  switch (R) {
+    case 1: return sw_pair_warp<1, true>(pa, pb, ra, rb, nmax, sc, tgt2);
+    case 2: return sw_pair_warp<2, true>(pa, pb, ra, rb, nmax, sc, tgt2);
+    case 3: return sw_pair_warp<3, true>(pa, pb, ra, rb, nmax, sc, tgt2);
+    case 4: return sw_pair_warp<4, true>(pa, pb, ra, rb, nmax, sc, tgt2);
+    case 5: return sw_pair_warp<5, true>(pa, pb, ra, rb, nmax, sc, tgt2);
+    case 6: return sw_pair_warp<6, true>(pa, pb, ra, rb, nmax, sc, tgt2);
+    default: return sw_pair_warp<8, true>(pa, pb, ra, rb, nmax, sc, tgt2);
+  }
+}
+
+// Packed locate: the window of one problem, staged from global memory at w[0 .. n) (letters 0..4) with the sentinel letter in the
+// 32 columns before it and from column n up to column nstage + 32 (w has kRefStage + 33 bytes after it and 32 before it).  All loads
+// of a lane are issued before its first store.
+constexpr int kPairWinBytes = kRefStage + 72;   // per window: 32 leading sentinels, kRefStage columns, 33 trailing, padding
+__device__ __forceinline__ void pair_stage(const SeqView t, const int32_t n, const int32_t nstage, uint8_t* __restrict__ w) {
+  constexpr int K = (kRefStage + 65 + 31) / 32;
+  const int lane = (int)lane_id();
+  uint32_t v[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const int32_t j = lane + 32 * k - 32;
+    v[k] = (j >= 0 && j < n) ? min(t.at(j), 4u) : 5u;
+  }
+#pragma unroll
+  for (int k = 0; k < K; ++k) {
+    const int32_t j = lane + 32 * k - 32;
+    if (j <= nstage + 32) w[j] = (uint8_t)v[k];
+  }
+}
+
+// One half of a packed locate: query q (m rows), window t (n columns), known best score target > 0.  m == 0: no problem.
+struct PairLoc { SeqView q; int32_t m; SeqView t; int32_t n, target; };
+
+// The end points (column<<16 | row, or kPairNoHit) of both problems' first cells holding their targets, in one packed pass.
+// prof: 2 * kPairProfWords words, wa / wb: kPairWinBytes bytes each, all shared memory owned by this warp.  Both halves must pass
+// sw_pair_ok (or be empty).
+__device__ __noinline__ uint2 sw_pair_locate(const PairLoc A, const PairLoc B, const SwScore sc, uint32_t* prof, uint8_t* wa, uint8_t* wb) {
+  const int R = pair_rows(max(A.m, B.m));
+  const int32_t nmax = max(A.m ? A.n : 0, B.m ? B.n : 0);   // (an empty half's window is not looked at)
+  __syncwarp();
+  uint8_t* a = wa + 32; uint8_t* b = wb + 32;
+  pair_stage(A.t, A.m ? A.n : 0, nmax, a);
+  pair_stage(B.t, B.m ? B.n : 0, nmax, b);
+  pair_profile(A.q.base + A.q.start, A.q.step, A.q.comp, A.m, R, sc, prof);
+  const uint32_t* pb = prof;
+  if (B.m) { pair_profile(B.q.base + B.q.start, B.q.step, B.q.comp, B.m, R, sc, prof + kPairProfWords); pb = prof + kPairProfWords; }
+  __syncwarp();
+  const uint32_t tgt2 = pack16(A.m ? A.target : (int32_t)kPairNoTarget, B.m ? B.target : (int32_t)kPairNoTarget);
+  return sw_pair_find_dispatch(R, prof, pb, a, b, nmax, sc, tgt2);
 }
 
 // ---- TMA bulk copy + mbarrier (cp.async.bulk; SASS: UBLKCP / SYNCS) ----
@@ -571,13 +664,13 @@ __device__ int32_t banded_traceback_lane(const SeqView t, const SeqView q, const
     for (int32_t i = 0; i < readLen; ++i) {
       const int32_t beg = max(0, i - band_width), end = min(refLen - 1, i + band_width);
       const int32_t edge = end + 1 < width - 1 ? end + 1 : width - 1;
-      int32_t f = 0, u = 0;
+      int32_t f = 0, u = 0, hleft = 0;   // hleft: H of the left neighbour, hc[u - 1] (hc[0] = 0 at the row's first cell)
       A.hb[0] = 0; A.eb[0] = 0; A.hb[edge * S] = 0; A.eb[edge * S] = 0; A.hc[0] = 0;
       int8_t* dl = A.dir + (size_t)width_d * i * 3 * S;
       const uint32_t qi = q.at(i);
       for (int32_t j = beg; j <= end; ++j) {
         u = band_u(band_width, i, j);
-        const int32_t up = band_u(band_width, i - 1, j), lf = band_u(band_width, i, j - 1), dg = band_u(band_width, i - 1, j - 1);
+        const int32_t up = band_u(band_width, i - 1, j), dg = band_u(band_width, i - 1, j - 1);
         const int32_t de = band_d(band_width, i, j, 0), df = de + 1, dh = de + 2;
         int32_t t1 = i == 0 ? -sc.go : A.hb[up * S] - sc.go;
         int32_t t2 = i == 0 ? -sc.ge : A.eb[up * S] - sc.ge;
@@ -585,7 +678,7 @@ __device__ int32_t banded_traceback_lane(const SeqView t, const SeqView q, const
         A.eb[u * S] = ev;
         const int8_t cde = t1 > t2 ? 3 : 2;
         dl[de * S] = cde;
-        t1 = A.hc[lf * S] - sc.go; t2 = f - sc.ge;
+        t1 = hleft - sc.go; t2 = f - sc.ge;
         f = t1 > t2 ? t1 : t2;
         const int8_t cdf = t1 > t2 ? 5 : 4;
         dl[df * S] = cdf;
@@ -595,7 +688,7 @@ __device__ int32_t banded_traceback_lane(const SeqView t, const SeqView q, const
         const int32_t s = (tj >= 4u || qi >= 4u) ? sc.sN : (tj == qi ? sc.match : sc.mismatch);
         t2 = A.hb[dg * S] + s;
         const int32_t hv = t1 > t2 ? t1 : t2;
-        A.hc[u * S] = hv;
+        A.hc[u * S] = hv; hleft = hv;
         if (hv > maxv) maxv = hv;
         dl[dh * S] = (t1 <= t2) ? (int8_t)1 : (e1 > f1 ? cde : cdf);
       }
