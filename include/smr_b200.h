@@ -257,6 +257,32 @@ int smr_format_reports(smr_ctx*, const smr_report_opts* opts, const char* text, 
  * scans, writes; includes the one read-back of the sizes), [2] = D2H of the output */
 int smr_last_report_timings(const smr_ctx*, double out[3]);
 
+/* -- OTU map on the device (sortmerna_b200/csrc/smr_otu.cuh, DESIGN.md 5e): the reference's otu_map.txt (fill_otu_map /
+ *    fill_otu_map2 / OtuMap::write, src/sortmerna/otumap.cpp:84-281) at -threads 1, accumulated over the batches of one read file.
+ *    A stored alignment of a read is an entry of the line of its reference id when the read counts as c_yid_ycov > 0 (one of its
+ *    alignments passes -id and -coverage with floor(x * 1000 + 0.5) / 1000.0, processor.cpp:334-342) and the alignment itself passes
+ *    them with floor(x * 1000 + 0.5) * 0.001 (otumap.cpp:160-163).  %id is taken from n_match_denovo.  Lines: one per reference id in
+ *    unsigned byte order of the id, "id\tread\tread...\n"; within a line the (index, part) groups in order, reads in the order added. */
+typedef struct {
+  double min_id, min_cov;         /* -id, -coverage (the reference's default under -otu_map: 0.97, 0.97) */
+  int32_t paired_in, paired_out;  /* a paired batch: SMR_ERR_UNSUPPORTED (DESIGN.md 5e) */
+} smr_otu_opts;
+/* Open (or reset) the accumulator of this context.  SMR_ERR_ARG if params.is_best == 0 (the reference refuses -otu_map with
+ * -no-best) or a loaded part has no smr_set_report_refs.  Loading a part or setting report ids afterwards makes the next
+ * smr_otu_add / smr_otu_finish fail with SMR_ERR_ARG. */
+int smr_otu_begin(smr_ctx*, const smr_otu_opts* opts);
+/* Add one batch: text / nbytes / results / alns / stats as for smr_format_reports (text == nullptr: the resident text).
+ * *n_added = entries it added (optional). */
+int smr_otu_add(smr_ctx*, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
+                uint32_t nreads, uint64_t* n_added);
+/* The map: counts[0] = bytes, [1] = lines ("Total OTUs"), [2] = entries ("passing %id and %coverage" of aligned.log).  The reference
+ * writes no file when counts[2] == 0.  If out is null or cap < counts[0]: SMR_ERR_CAPACITY with counts filled and the accumulator
+ * kept; a successful call closes it (smr_otu_begin opens the next). */
+int smr_otu_finish(smr_ctx*, char* out, uint64_t cap, uint64_t counts[3]);
+/* milliseconds (CUDA events): out[0] = H2D of the smr_otu_add calls since smr_otu_begin, [1] = their device work (includes the one
+ * read-back of the sizes per call), [2] = the last smr_otu_finish (sort, sizes, write, D2H) */
+int smr_last_otu_timings(const smr_ctx*, double out[3]);
+
 /* Device-side timings of the last smr_run_resident / smr_align_batch, CUDA events on the
  * library's stream, milliseconds: out[0]=total [1]=seed kernels [2]=candidate/SW kernels
  * [3]=finalize (reverse SW + traceback) [4]=h2d [5]=d2h; out[6]=number of kernel launches */

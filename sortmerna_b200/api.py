@@ -28,7 +28,7 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_debug_dpx_peak", "smr_set_stats_buffer", "smr_build_index", "smr_upload_fastx", "smr_resident_layout", "smr_pack_kvdb_blobs",
            "smr_set_aln_slots", "smr_aln_slots", "smr_aln_slots_needed", "smr_upload_fastx_gz", "smr_resident_text", "smr_debug_inflate",
            "smr_build_index_device", "smr_debug_index_array", "smr_set_instrumentation", "smr_set_report_refs", "smr_set_report_scoring",
-           "smr_format_reports", "smr_last_report_timings"]
+           "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings"]
 
 CNT_NAMES = ("num_aligned", "num_short", "sw_calls", "sw_cells", "windows", "trie_nodes", "buckets",
              "bucket_entries", "pos_entries", "lis_calls", "dbg_max_read_cycles", "dbg_sum_read_cycles", "dbg_lis_kernel_cycles",
@@ -86,6 +86,12 @@ def report_opts(sam=False, blast=None, fastx=False, other=False, denovo=None, pa
     if denovo is not None:
         o.denovo, o.min_id, o.min_cov = 1, float(denovo[0]), float(denovo[1])
     return o
+
+
+class OtuOpts(C.Structure):
+    """smr_otu_opts (include/smr_b200.h)"""
+    _fields_ = [("min_id", C.c_double), ("min_cov", C.c_double), ("paired_in", C.c_int32), ("paired_out", C.c_int32)]
+
 
 _lib = None
 
@@ -448,6 +454,43 @@ class Aligner:
         b = [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(2 * G + 3)]
         return dict(sam=b[:G], blast=b[G:2 * G], aligned=b[2 * G], other=b[2 * G + 1], denovo=b[2 * G + 2], groups=groups)
 
+    # ---- OTU map (smr_otu_begin / smr_otu_add / smr_otu_finish) ----
+    def otu_begin(self, min_id: float = 0.97, min_cov: float = 0.97, paired_in: bool = False, paired_out: bool = False):
+        """smr_otu_begin: open (or reset) the OTU map of this context; -id / -coverage as the reference's -otu_map defaults them"""
+        self._upload_report_refs()
+        o = OtuOpts(float(min_id), float(min_cov), int(bool(paired_in)), int(bool(paired_out)))
+        self._check(self.L.smr_otu_begin(self.h, C.byref(o)), "smr_otu_begin")
+
+    def otu_add(self, out: dict, text: bytes | None = None) -> int:
+        """smr_otu_add: one batch (out and text as for format_reports; out needs "stats"); returns the entries it added"""
+        res, alns, st = out["res"], out["alns"], out.get("stats")
+        txt = np.frombuffer(text, np.uint8) if text is not None else None
+        n = C.c_uint64(0)
+        self.L.smr_otu_add.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
+        rc = self.L.smr_otu_add(self.h, _ptr(txt) if txt is not None and txt.size else None, txt.size if txt is not None else 0, _ptr(res), _ptr(alns),
+                                _ptr(st) if st is not None else None, res.shape[0], C.cast(C.byref(n), C.c_void_p))
+        self._check(rc, "smr_otu_add")
+        return int(n.value)
+
+    def otu_finish(self) -> dict:
+        """smr_otu_finish: {"text": the bytes of otu_map.txt, "total_otu": lines, "n_yid_ycov": entries}"""
+        counts = np.zeros(3, np.uint64)
+        buf = getattr(self, "_otu_buf", None)
+        if buf is None:
+            buf = np.zeros(1 << 16, np.uint8)
+        rc = self.L.smr_otu_finish(self.h, _ptr(buf), C.c_uint64(buf.size), _ptr(counts))
+        if rc == 5 and int(counts[0]) > buf.size:   # SMR_ERR_CAPACITY: counts[0] names the size; grow and run again
+            buf = np.zeros(int(counts[0]) + (int(counts[0]) >> 3), np.uint8)
+            rc = self.L.smr_otu_finish(self.h, _ptr(buf), C.c_uint64(buf.size), _ptr(counts))
+        self._check(rc, "smr_otu_finish")
+        self._otu_buf = buf
+        return dict(text=bytes(buf[:int(counts[0])]), total_otu=int(counts[1]), n_yid_ycov=int(counts[2]))
+
+    def otu_timings(self):
+        out = np.zeros(3, np.float64)
+        self._check(self.L.smr_last_otu_timings(self.h, _ptr(out)), "smr_last_otu_timings")
+        return dict(add_h2d_ms=out[0], add_device_ms=out[1], finish_ms=out[2])
+
     def report_timings(self):
         out = np.zeros(3, np.float64)
         self._check(self.L.smr_last_report_timings(self.h, _ptr(out)), "smr_last_report_timings")
@@ -500,11 +543,16 @@ class ReportWriter:
     other.<ext>, aligned_denovo.<ext> under out_dir (<ext> = fq for FASTQ input, fa for FASTA, report_fx_base.cpp:94).  Every stream of
     every batch is appended to a part file of its own; close() concatenates them in the reference's order (all SAM rows of (index, part)
     group 0, then group 1, ...), so that feeding a file in several batches writes what one batch writes.
-    sam_header: the text before the SAM rows (hostio.sam_header); opts: report_opts(...) keyword arguments."""
+    sam_header: the text before the SAM rows (hostio.sam_header); opts: report_opts(...) keyword arguments.
+    otu_map: (min_id, min_cov) = the reference's -otu_map -id -coverage: close() also writes otu_map.txt (none when no alignment
+    passes, as the reference) and sets total_otu and n_yid_ycov, the two OTU numbers of aligned.log."""
 
-    def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", **opts):
+    def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", otu_map=None, **opts):
         self.dir, self.al, self.header = out_dir, aligner, sam_header
         self.opts = report_opts(**opts)
+        self.otu_map, self.total_otu, self.n_yid_ycov = otu_map, None, None
+        if otu_map is not None:
+            aligner.otu_begin(otu_map[0], otu_map[1], paired_in=self.opts.paired_in, paired_out=self.opts.paired_out)
         self.ext = None
         self._parts = {}
         os.makedirs(out_dir, exist_ok=True)
@@ -526,6 +574,8 @@ class ReportWriter:
             self._append(f"blast_{g}", rows_blast)
         for k in ("aligned", "other", "denovo"):
             self._append(k, s[k])
+        if self.otu_map is not None:
+            self.al.otu_add(out, text)
         return s
 
     def close(self) -> list:
@@ -554,6 +604,14 @@ class ReportWriter:
                                 break
                             f.write(chunk)
             paths.append(path)
+        if self.otu_map is not None:
+            m = self.al.otu_finish()
+            self.total_otu, self.n_yid_ycov = m["total_otu"], m["n_yid_ycov"]
+            if m["n_yid_ycov"] > 0:
+                path = os.path.join(self.dir, "otu_map.txt")
+                with open(path, "wb") as f:
+                    f.write(m["text"])
+                paths.append(path)
         for k, fh in self._parts.items():
             fh.close()
             os.unlink(os.path.join(self.dir, f".part_{k}"))

@@ -14,6 +14,7 @@
 
 #include "smr_decode.cuh"
 #include "smr_report.cuh"
+#include "smr_otu.cuh"
 #include "smr_inflate.cuh"
 #include "smr_build.h"
 #include "smr_build_dev.cuh"
@@ -29,6 +30,7 @@ struct Part {
   std::vector<void*> owned;   // device allocations
   size_t bytes = 0, n_nodes = 0, n_entries = 0, n_ids = 0, n_pos = 0, n_refseq = 0;
   const char* rnames = nullptr; const uint64_t* rname_off = nullptr; uint32_t n_rnames = 0; bool has_rnames = false;   // smr_set_report_refs
+  std::vector<std::string> h_rnames;   // host copy of the same ids: the OTU map ranks them (smr_otu_begin)
 };
 
 struct DevBuf {
@@ -87,6 +89,15 @@ struct smr_ctx {
   DevBuf r_text, r_nl, r_hdr, r_sb, r_rec, r_spos, r_line, r_recs, r_res, r_aln, r_cig, r_st, r_flags, r_keys, r_keys2, r_vals, r_rows, r_first,
          r_sz, r_off, r_bsz, r_boff, r_fxsz, r_fxoff, r_grp, r_so, r_tmp, r_out, r_scal;
   double t_rpt[3] = {0, 0, 0};
+  uint64_t parts_gen = 0;   // bumped whenever a part is loaded or its report ids are set: an open OTU map refuses to go on after that
+  // OTU map accumulator (smr_otu.cuh), smr_otu_begin .. smr_otu_finish
+  struct Otu {
+    bool active = false; uint64_t gen = 0; double min_id = 0, min_cov = 0;
+    std::vector<RptGroup> groups; uint32_t gbits = 0, kbits = 0;
+    DevBuf rank, rank_off, grp, key, ent, pool, flag, pos, nsz, noff, vals, skey, sidx, size, off, out, tmp, scal;
+    uint64_t n = 0, pool_bytes = 0;
+    double t[3] = {0, 0, 0};
+  } otu;
   // timings
   std::vector<cudaEvent_t> ev;
   double t_total = 0, t_seed = 0, t_lis = 0, t_final = 0, t_h2d = 0, t_d2h = 0; uint64_t n_launch = 0;
@@ -955,45 +966,22 @@ int upload_async(smr_ctx* ctx, DevBuf& b, const T* src, size_t n) {
   return SMR_OK;
 }
 
-int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
-                        const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
-                        char* out, uint64_t cap, uint64_t* so_out) {
-  if (o->out2 || o->sout) { ctx->err = "-out2 / -sout: the report writer writes one aligned and one other file"; return SMR_ERR_UNSUPPORTED; }
-  if (o->blast && o->blast_format != 1) { ctx->err = "only tabular BLAST (-blast 1) is written on the device"; return SMR_ERR_UNSUPPORTED; }
-  if (o->paired_in && o->paired_out) { ctx->err = "paired_in and paired_out are exclusive"; return SMR_ERR_ARG; }
-  const bool paired = o->paired_in || o->paired_out;
-  if (paired && (nreads & 1u)) { ctx->err = "a paired batch holds mates 2k and 2k+1: the number of reads must be even"; return SMR_ERR_ARG; }
-  if ((o->sam || o->blast || o->denovo) && nreads && !stats) { ctx->err = "SAM, BLAST and denovo need the smr_aln_stats of the batch"; return SMR_ERR_ARG; }
-  if (nreads && (!results || !alns)) return SMR_ERR_ARG;
-  uint32_t ncols = 0, cols[4] = {0, 0, 0, 0};
-  if (o->blast)
-    for (; ncols < 4 && o->blast_cols[ncols]; ++ncols) {
-      if (o->blast_cols[ncols] < SMR_BLAST_COL_CIGAR || o->blast_cols[ncols] > SMR_BLAST_COL_QSTRAND) { ctx->err = "unknown BLAST column"; return SMR_ERR_ARG; }
-      cols[ncols] = (uint32_t)o->blast_cols[ncols];
-    }
-  // groups: the loaded (index, part)s in the reference's report order
-  std::vector<const Part*> gp;
-  for (const Part& pt : ctx->parts) gp.push_back(&pt);
-  std::sort(gp.begin(), gp.end(), [](const Part* a, const Part* b) { return a->d.index_num != b->d.index_num ? a->d.index_num < b->d.index_num : a->d.part < b->d.part; });
-  const uint32_t G = (uint32_t)gp.size(), nso = 2 * G + 4;
-  std::vector<RptGroup> hg(G);
-  for (uint32_t g = 0; g < G; ++g) {
-    const Part& pt = *gp[g];
-    if ((o->sam || o->blast) && !pt.has_rnames) {
-      ctx->err = "smr_set_report_refs was not called for index " + std::to_string(pt.d.index_num) + " part " + std::to_string(pt.d.part);
-      return SMR_ERR_ARG;
-    }
-    const bool sc = pt.d.index_num < ctx->rpt_score.size() && ctx->rpt_score[pt.d.index_num].set;
-    if (o->blast && !sc) { ctx->err = "smr_set_report_scoring was not called for index " + std::to_string(pt.d.index_num); return SMR_ERR_ARG; }
-    hg[g] = RptGroup{pt.rnames, pt.rname_off, sc ? (const double*)ctx->rpt_score[pt.d.index_num].ev.p : nullptr,
-                     sc ? (const uint32_t*)ctx->rpt_score[pt.d.index_num].bits.p : nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0};
-  }
-  const uint32_t slots = slots_of(ctx);
+int rpt_error(smr_ctx* ctx, uint32_t e) {
+  ctx->err = e & kRptErrLen ? "an alignment's readlen or read_end1 disagrees with the length of its read in the text"
+           : e & kRptErrGroup ? "an alignment names an (index, part) that is not loaded"
+           : e & kRptErrRef ? "an alignment's ref_num is beyond the reference names of its part"
+           : e & kRptErrQual ? "reads text: a FASTQ record without its quality line" : "an alignment's CIGAR lies outside cigar_words";
+  return SMR_ERR_ARG;
+}
+
+// The first half of smr_format_reports and smr_otu_add: text, results and groups on the device (e1 recorded after the copies), the
+// record layout of the text (the line passes of smr_decode.cuh, then rpt_records_kernel) and the fields of `a` that describe them.
+// The report error word is scal[4] of ctx->r_scal.
+int rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar,
+                 uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads, const std::vector<RptGroup>& hg, cudaEvent_t e1, RptArgs& a) {
+  const uint32_t slots = slots_of(ctx), G = (uint32_t)hg.size();
   const uint64_t N = (uint64_t)nreads * slots;
-  if (N >= (1ull << 31)) { ctx->err = "batch too large for the report writer: split it"; return SMR_ERR_ARG; }
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
   int rc;
-  CK(cudaEventRecord(e0, ctx->stream));
   // the text
   const uint8_t* dt;
   if (text) {
@@ -1049,10 +1037,73 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
     nrec = h[1];
   }
   if (nrec != nreads) { ctx->err = "the text holds " + std::to_string(nrec) + " records, the results " + std::to_string(nreads) + " reads"; return SMR_ERR_ARG; }
-  // per record, routing, row order
+  // per record
   const uint64_t fstride = (uint64_t)nreads + 1;
   if ((rc = ensure(ctx, ctx->r_line, fstride * 4))) return rc;
   if ((rc = ensure(ctx, ctx->r_recs, fstride * sizeof(RptRec)))) return rc;
+  a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)ctx->r_nl.p; a.spos = (const uint32_t*)ctx->r_spos.p; a.nlines = nlines; a.fastq = fmt == kFmtFastq;
+  a.rec = (const RptRec*)ctx->r_recs.p; a.nreads = nreads; a.slots = slots;
+  a.res = (const smr_read_result*)ctx->r_res.p; a.aln = (const smr_aln*)ctx->r_aln.p; a.cigar = (const uint32_t*)ctx->r_cig.p;
+  a.cigar_words = cigar ? cigar_words : 0; a.st = (const smr_aln_stats*)ctx->r_st.p;
+  a.grp = (const RptGroup*)ctx->r_grp.p; a.ngroups = G; a.err = scal + 4;
+  if (nreads) {
+    rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->r_hdr.p, (const uint32_t*)ctx->r_rec.p, nlines, (uint32_t*)ctx->r_line.p);
+    rpt_records_kernel<<<grid, 256, 0, ctx->stream>>>(a, (const uint32_t*)ctx->r_line.p, (RptRec*)ctx->r_recs.p);
+  }
+  return SMR_OK;
+}
+
+// the loaded (index, part)s in the reference's report order (index, then part)
+std::vector<const Part*> report_groups(const smr_ctx* ctx) {
+  std::vector<const Part*> gp;
+  for (const Part& pt : ctx->parts) gp.push_back(&pt);
+  std::sort(gp.begin(), gp.end(), [](const Part* a, const Part* b) { return a->d.index_num != b->d.index_num ? a->d.index_num < b->d.index_num : a->d.part < b->d.part; });
+  return gp;
+}
+
+int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
+                        const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                        char* out, uint64_t cap, uint64_t* so_out) {
+  if (o->out2 || o->sout) { ctx->err = "-out2 / -sout: the report writer writes one aligned and one other file"; return SMR_ERR_UNSUPPORTED; }
+  if (o->blast && o->blast_format != 1) { ctx->err = "only tabular BLAST (-blast 1) is written on the device"; return SMR_ERR_UNSUPPORTED; }
+  if (o->paired_in && o->paired_out) { ctx->err = "paired_in and paired_out are exclusive"; return SMR_ERR_ARG; }
+  const bool paired = o->paired_in || o->paired_out;
+  if (paired && (nreads & 1u)) { ctx->err = "a paired batch holds mates 2k and 2k+1: the number of reads must be even"; return SMR_ERR_ARG; }
+  if ((o->sam || o->blast || o->denovo) && nreads && !stats) { ctx->err = "SAM, BLAST and denovo need the smr_aln_stats of the batch"; return SMR_ERR_ARG; }
+  if (nreads && (!results || !alns)) return SMR_ERR_ARG;
+  uint32_t ncols = 0, cols[4] = {0, 0, 0, 0};
+  if (o->blast)
+    for (; ncols < 4 && o->blast_cols[ncols]; ++ncols) {
+      if (o->blast_cols[ncols] < SMR_BLAST_COL_CIGAR || o->blast_cols[ncols] > SMR_BLAST_COL_QSTRAND) { ctx->err = "unknown BLAST column"; return SMR_ERR_ARG; }
+      cols[ncols] = (uint32_t)o->blast_cols[ncols];
+    }
+  const std::vector<const Part*> gp = report_groups(ctx);
+  const uint32_t G = (uint32_t)gp.size(), nso = 2 * G + 4;
+  std::vector<RptGroup> hg(G);
+  for (uint32_t g = 0; g < G; ++g) {
+    const Part& pt = *gp[g];
+    if ((o->sam || o->blast) && !pt.has_rnames) {
+      ctx->err = "smr_set_report_refs was not called for index " + std::to_string(pt.d.index_num) + " part " + std::to_string(pt.d.part);
+      return SMR_ERR_ARG;
+    }
+    const bool sc = pt.d.index_num < ctx->rpt_score.size() && ctx->rpt_score[pt.d.index_num].set;
+    if (o->blast && !sc) { ctx->err = "smr_set_report_scoring was not called for index " + std::to_string(pt.d.index_num); return SMR_ERR_ARG; }
+    hg[g] = RptGroup{pt.rnames, pt.rname_off, sc ? (const double*)ctx->rpt_score[pt.d.index_num].ev.p : nullptr,
+                     sc ? (const uint32_t*)ctx->rpt_score[pt.d.index_num].bits.p : nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0};
+  }
+  const uint32_t slots = slots_of(ctx);
+  const uint64_t N = (uint64_t)nreads * slots;
+  if (N >= (1ull << 31)) { ctx->err = "batch too large for the report writer: split it"; return SMR_ERR_ARG; }
+  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
+  int rc;
+  CK(cudaEventRecord(e0, ctx->stream));
+  RptArgs a{};
+  if ((rc = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e1, a))) return rc;
+  const int grid = ctx->sm_count * 8;
+  uint32_t* scal = (uint32_t*)ctx->r_scal.p;
+  uint32_t h[8];
+  // per record, routing, row order
+  const uint64_t fstride = (uint64_t)nreads + 1;
   if ((rc = ensure(ctx, ctx->r_flags, fstride * 4))) return rc;
   if ((rc = ensure(ctx, ctx->r_keys, (N + 1) * 4))) return rc;
   if ((rc = ensure(ctx, ctx->r_keys2, (N + 1) * 4))) return rc;
@@ -1066,15 +1117,9 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   if ((rc = ensure(ctx, ctx->r_fxsz, 3 * fstride * 8))) return rc;
   if ((rc = ensure(ctx, ctx->r_fxoff, 3 * fstride * 8))) return rc;
   if ((rc = ensure(ctx, ctx->r_so, (size_t)nso * 8))) return rc;
-  RptArgs a{};
-  a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)ctx->r_nl.p; a.spos = (const uint32_t*)ctx->r_spos.p; a.nlines = nlines; a.fastq = fmt == kFmtFastq;
-  a.rec = (const RptRec*)ctx->r_recs.p; a.nreads = nreads; a.slots = slots;
-  a.res = (const smr_read_result*)ctx->r_res.p; a.aln = (const smr_aln*)ctx->r_aln.p; a.cigar = (const uint32_t*)ctx->r_cig.p;
-  a.cigar_words = cigar ? cigar_words : 0; a.st = (const smr_aln_stats*)ctx->r_st.p;
-  a.grp = (const RptGroup*)ctx->r_grp.p; a.ngroups = G;
   for (int k = 0; k < 4; ++k) a.cols[k] = cols[k];
   a.ncols = ncols; a.min_id = o->min_id; a.min_cov = o->min_cov;
-  a.paired_in = o->paired_in != 0; a.paired_out = o->paired_out != 0; a.denovo = o->denovo != 0; a.err = scal + 4;
+  a.paired_in = o->paired_in != 0; a.paired_out = o->paired_out != 0; a.denovo = o->denovo != 0;
   a.fx_mask = (o->fastx ? kRptAligned : 0u) | (o->other ? kRptOther : 0u) | (o->denovo ? kRptDenovo : 0u);
   uint32_t* flags = (uint32_t*)ctx->r_flags.p;
   uint64_t *first = (uint64_t*)ctx->r_first.p, *sz = (uint64_t*)ctx->r_sz.p, *off = (uint64_t*)ctx->r_off.p, *bsz = (uint64_t*)ctx->r_bsz.p,
@@ -1085,8 +1130,6 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   CK(cudaMemsetAsync(first, 0, ((size_t)G + 1) * 8, ctx->stream));
   const uint32_t* rows = (const uint32_t*)ctx->r_rows.p;
   if (nreads) {
-    rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->r_hdr.p, (const uint32_t*)ctx->r_rec.p, nlines, (uint32_t*)ctx->r_line.p);
-    rpt_records_kernel<<<grid, 256, 0, ctx->stream>>>(a, (const uint32_t*)ctx->r_line.p, (RptRec*)ctx->r_recs.p);
     rpt_route_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags);
     rpt_row_keys_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, (uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_vals.p);
     int nbits = 1;
@@ -1122,13 +1165,7 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   CK(cudaMemcpyAsync(hso.data(), so, (size_t)nso * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (h[4]) {
-    ctx->err = h[4] & kRptErrLen ? "an alignment's readlen or read_end1 disagrees with the length of its read in the text"
-             : h[4] & kRptErrGroup ? "an alignment names an (index, part) that is not loaded"
-             : h[4] & kRptErrRef ? "an alignment's ref_num is beyond the reference names of its part"
-             : h[4] & kRptErrQual ? "reads text: a FASTQ record without its quality line" : "an alignment's CIGAR lies outside cigar_words";
-    return SMR_ERR_ARG;
-  }
+  if (h[4]) return rpt_error(ctx, h[4]);
   memcpy(so_out, hso.data(), (size_t)nso * 8);
   const uint64_t total = hso[nso - 1];
   if (total && (!out || cap < total)) { ctx->err = "output buffer too small: stream_off holds the sizes"; return SMR_ERR_CAPACITY; }
@@ -1148,6 +1185,187 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
   cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
   cudaEventElapsedTime(&ms, e2, e3); ctx->t_rpt[2] = ms;
+  return SMR_OK;
+}
+// ---------------------------------------------------------------------------------------------------------------------
+// OTU map (smr_otu.cuh)
+// ---------------------------------------------------------------------------------------------------------------------
+// device buffer grown to at least `need` bytes by doubling, keeping its first `used` bytes
+int grow_keep(smr_ctx* ctx, DevBuf& b, size_t used, size_t need) {
+  if (need <= b.cap && b.p) return SMR_OK;
+  const size_t want = std::max<size_t>({need, 2 * b.cap, 4096});
+  void* p = nullptr;
+  CK(cudaMalloc(&p, want));
+  if (used) {
+    const cudaError_t e = cudaMemcpyAsync(p, b.p, used, cudaMemcpyDeviceToDevice, ctx->stream);
+    if (e != cudaSuccess) { cudaFree(p); ctx->err = std::string("cudaMemcpyAsync: ") + cudaGetErrorString(e); return SMR_ERR_CUDA; }
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  release(b);
+  b.p = p; b.cap = want;
+  return SMR_OK;
+}
+
+int otu_open(smr_ctx* ctx) {
+  if (!ctx->otu.active) { ctx->err = "no open OTU map: call smr_otu_begin first"; return SMR_ERR_ARG; }
+  if (ctx->otu.gen != ctx->parts_gen) {
+    ctx->err = "an index part was loaded or its report ids were set after smr_otu_begin: begin the OTU map again";
+    return SMR_ERR_ARG;
+  }
+  return SMR_OK;
+}
+
+int otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
+  auto& U = ctx->otu;
+  U.active = false;
+  if (!ctx->have_params || !ctx->prm.is_best) {
+    ctx->err = "the OTU map is made from the best alignments: params.is_best must be 1 (-otu_map cannot be set with -no-best)";
+    return SMR_ERR_ARG;
+  }
+  if (o->paired_in && o->paired_out) { ctx->err = "paired_in and paired_out are exclusive"; return SMR_ERR_ARG; }
+  if (o->paired_in || o->paired_out) {
+    ctx->err = "paired reads: the reference's OTU pass reads only the first mate file of two, but every record of one interleaved file, "
+               "so a paired batch does not say which map is meant";
+    return SMR_ERR_UNSUPPORTED;
+  }
+  const std::vector<const Part*> gp = report_groups(ctx);
+  const uint32_t G = (uint32_t)gp.size();
+  for (const Part* pt : gp)
+    if (!pt->has_rnames) {
+      ctx->err = "smr_set_report_refs was not called for index " + std::to_string(pt->d.index_num) + " part " + std::to_string(pt->d.part);
+      return SMR_ERR_ARG;
+    }
+  // ranks of the reference ids in unsigned byte order (std::string compares as unsigned char)
+  std::vector<const std::string*> ids;
+  for (const Part* pt : gp) for (const std::string& s : pt->h_rnames) ids.push_back(&s);
+  std::sort(ids.begin(), ids.end(), [](const std::string* a, const std::string* b) { return *a < *b; });
+  ids.erase(std::unique(ids.begin(), ids.end(), [](const std::string* a, const std::string* b) { return *a == *b; }), ids.end());
+  std::vector<uint32_t> rank, rank_off(std::max(G, 1u), 0);
+  U.groups.assign(G, RptGroup{});
+  for (uint32_t g = 0; g < G; ++g) {
+    const Part& pt = *gp[g];
+    rank_off[g] = (uint32_t)rank.size();
+    for (const std::string& s : pt.h_rnames)
+      rank.push_back((uint32_t)(std::lower_bound(ids.begin(), ids.end(), &s, [](const std::string* a, const std::string* b) { return *a < *b; }) - ids.begin()));
+    U.groups[g] = RptGroup{pt.rnames, pt.rname_off, nullptr, nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0};
+  }
+  uint32_t gbits = 1, rbits = 1;
+  while ((1ull << gbits) <= G) ++gbits;
+  while ((1ull << rbits) <= ids.size()) ++rbits;
+  int rc;
+  if ((rc = upload_async(ctx, U.rank, rank.data(), rank.size()))) return rc;
+  if ((rc = upload_async(ctx, U.rank_off, rank_off.data(), rank_off.size()))) return rc;
+  if ((rc = upload_async(ctx, U.grp, U.groups.data(), G))) return rc;
+  CK(cudaStreamSynchronize(ctx->stream));
+  U.gbits = gbits; U.kbits = gbits + rbits;
+  U.min_id = o->min_id; U.min_cov = o->min_cov;
+  U.n = 0; U.pool_bytes = 0;
+  for (double& t : U.t) t = 0;
+  U.gen = ctx->parts_gen;
+  U.active = true;
+  return SMR_OK;
+}
+
+int otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
+                 uint32_t nreads, uint64_t* n_added) {
+  auto& U = ctx->otu;
+  int rc;
+  if ((rc = otu_open(ctx))) return rc;
+  if (nreads && (!results || !alns || !stats)) { ctx->err = "the OTU map needs the results, alignments and smr_aln_stats of the batch"; return SMR_ERR_ARG; }
+  const uint32_t slots = slots_of(ctx);
+  const uint64_t N = (uint64_t)nreads * slots;
+  if (N >= (1ull << 31)) { ctx->err = "batch too large for the OTU map: split it"; return SMR_ERR_ARG; }
+  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
+  CK(cudaEventRecord(e0, ctx->stream));
+  RptArgs a{};
+  if ((rc = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e1, a))) return rc;
+  const OtuArgs oa{(const uint32_t*)U.rank.p, (const uint32_t*)U.rank_off.p, U.gbits, U.min_id, U.min_cov};
+  if ((rc = ensure(ctx, U.flag, (N + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, U.pos, (N + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, U.nsz, (N + 1) * 8))) return rc;
+  if ((rc = ensure(ctx, U.noff, (N + 1) * 8))) return rc;
+  uint32_t *flag = (uint32_t*)U.flag.p, *pos = (uint32_t*)U.pos.p;
+  uint64_t *nsz = (uint64_t*)U.nsz.p, *noff = (uint64_t*)U.noff.p;
+  const int grid = ctx->sm_count * 8;
+  CK(cudaMemsetAsync(flag + N, 0, 4, ctx->stream));
+  CK(cudaMemsetAsync(nsz + N, 0, 8, ctx->stream));
+  otu_flag_kernel<<<grid, 256, 0, ctx->stream>>>(a, oa, flag, nsz);
+  size_t t1 = 0, t2 = 0;
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, t1, flag, pos, (int)(N + 1), ctx->stream));
+  CK(cub::DeviceScan::ExclusiveSum(nullptr, t2, nsz, noff, (int)(N + 1), ctx->stream));
+  if ((rc = ensure(ctx, U.tmp, std::max(t1, t2)))) return rc;
+  CK(cub::DeviceScan::ExclusiveSum(U.tmp.p, t1, flag, pos, (int)(N + 1), ctx->stream));
+  CK(cub::DeviceScan::ExclusiveSum(U.tmp.p, t2, nsz, noff, (int)(N + 1), ctx->stream));
+  CK(cudaGetLastError());
+  uint32_t m = 0, err = 0; uint64_t bytes = 0;
+  CK(cudaMemcpyAsync(&m, pos + N, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&bytes, noff + N, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&err, (uint32_t*)ctx->r_scal.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (err) return rpt_error(ctx, err);
+  if (U.n + m >= (1ull << 31)) { ctx->err = "OTU map of 2^31 entries or more"; return SMR_ERR_CAPACITY; }
+  if ((rc = grow_keep(ctx, U.key, U.n * 8, (U.n + m) * 8))) return rc;
+  if ((rc = grow_keep(ctx, U.ent, U.n * sizeof(OtuEnt), (U.n + m) * sizeof(OtuEnt)))) return rc;
+  if ((rc = grow_keep(ctx, U.pool, U.pool_bytes, U.pool_bytes + bytes))) return rc;
+  if (m) otu_append_kernel<<<grid, 256, 0, ctx->stream>>>(a, oa, flag, pos, noff, U.n, U.pool_bytes, (uint64_t*)U.key.p, (OtuEnt*)U.ent.p, (char*)U.pool.p);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e2, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  U.n += m; U.pool_bytes += bytes;
+  if (n_added) *n_added = m;
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e0, e1); U.t[0] += ms;
+  cudaEventElapsedTime(&ms, e1, e2); U.t[1] += ms;
+  return SMR_OK;
+}
+
+int otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) {
+  auto& U = ctx->otu;
+  int rc;
+  if ((rc = otu_open(ctx))) return rc;
+  const uint64_t m = U.n;
+  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
+  CK(cudaEventRecord(e0, ctx->stream));
+  uint64_t bytes = 0; uint32_t runs = 0;
+  const int grid = ctx->sm_count * 8;
+  if (m) {
+    if ((rc = ensure(ctx, U.vals, m * 4))) return rc;
+    if ((rc = ensure(ctx, U.sidx, m * 4))) return rc;
+    if ((rc = ensure(ctx, U.skey, m * 8))) return rc;
+    if ((rc = ensure(ctx, U.size, (m + 1) * 8))) return rc;
+    if ((rc = ensure(ctx, U.off, (m + 1) * 8))) return rc;
+    if ((rc = ensure(ctx, U.scal, 16))) return rc;
+    uint64_t *skey = (uint64_t*)U.skey.p, *size = (uint64_t*)U.size.p, *off = (uint64_t*)U.off.p;
+    uint32_t *sidx = (uint32_t*)U.sidx.p, *scal = (uint32_t*)U.scal.p;
+    otu_iota_kernel<<<grid, 256, 0, ctx->stream>>>((uint32_t*)U.vals.p, m);
+    size_t t1 = 0, t2 = 0;
+    CK(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint64_t*)U.key.p, skey, (const uint32_t*)U.vals.p, sidx, (int)m, 0, (int)U.kbits, ctx->stream));
+    CK(cub::DeviceScan::ExclusiveSum(nullptr, t2, size, off, (int)(m + 1), ctx->stream));
+    if ((rc = ensure(ctx, U.tmp, std::max(t1, t2)))) return rc;
+    CK(cub::DeviceRadixSort::SortPairs(U.tmp.p, t1, (const uint64_t*)U.key.p, skey, (const uint32_t*)U.vals.p, sidx, (int)m, 0, (int)U.kbits, ctx->stream));
+    CK(cudaMemsetAsync(scal, 0, 16, ctx->stream));
+    CK(cudaMemsetAsync(size + m, 0, 8, ctx->stream));
+    otu_size_kernel<<<grid, 256, 0, ctx->stream>>>(skey, sidx, (const OtuEnt*)U.ent.p, m, U.gbits, (const RptGroup*)U.grp.p, size, scal);
+    CK(cub::DeviceScan::ExclusiveSum(U.tmp.p, t2, size, off, (int)(m + 1), ctx->stream));
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(&bytes, off + m, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(&runs, scal, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  counts[0] = bytes; counts[1] = runs; counts[2] = m;
+  if (bytes && (!out || cap < bytes)) { ctx->err = "output buffer too small: counts[0] holds the size"; return SMR_ERR_CAPACITY; }
+  if (bytes) {
+    if ((rc = ensure(ctx, U.out, bytes))) return rc;
+    otu_write_kernel<<<grid, 256, 0, ctx->stream>>>((const uint64_t*)U.skey.p, (const uint32_t*)U.sidx.p, (const OtuEnt*)U.ent.p, m, U.gbits,
+                                                    (const RptGroup*)U.grp.p, (const char*)U.pool.p, (const uint64_t*)U.off.p, (char*)U.out.p);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(out, U.out.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  CK(cudaEventRecord(e1, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e0, e1); U.t[2] = ms;
+  U.active = false;
   return SMR_OK;
 }
 
@@ -1201,6 +1419,10 @@ void smr_destroy(smr_ctx* ctx) {
                     &ctx->r_bsz, &ctx->r_boff, &ctx->r_fxsz, &ctx->r_fxoff, &ctx->r_grp, &ctx->r_so, &ctx->r_tmp, &ctx->r_out, &ctx->r_scal};
   for (DevBuf* b : bufs) release(*b);
   for (auto& sc : ctx->rpt_score) { release(sc.ev); release(sc.bits); }
+  DevBuf* obufs[] = {&ctx->otu.rank, &ctx->otu.rank_off, &ctx->otu.grp, &ctx->otu.key, &ctx->otu.ent, &ctx->otu.pool, &ctx->otu.flag, &ctx->otu.pos,
+                     &ctx->otu.nsz, &ctx->otu.noff, &ctx->otu.vals, &ctx->otu.skey, &ctx->otu.sidx, &ctx->otu.size, &ctx->otu.off, &ctx->otu.out,
+                     &ctx->otu.tmp, &ctx->otu.scal};
+  for (DevBuf* b : obufs) release(*b);
   PinBuf* pins[] = {&ctx->h_state, &ctx->h_flags, &ctx->h_hitdb, &ctx->h_outaln, &ctx->h_stats, &ctx->h_cigar, &ctx->h_off32, &ctx->h_pkoff};
   for (PinBuf* b : pins) release(*b);
   for (cudaEvent_t e : ctx->ev) cudaEventDestroy(e);
@@ -1252,6 +1474,7 @@ int smr_load_index_part(smr_ctx* ctx, uint32_t index_num, uint32_t part, const v
   pt.n_nodes = fx.nodes.size(); pt.n_entries = fx.entries.size(); pt.n_ids = pt.d.nids; pt.n_pos = fx.pos.size();
   ctx->parts.push_back(std::move(pt));
   ctx->n_index_files = std::max(ctx->n_index_files, index_num + 1);
+  ++ctx->parts_gen;
   return SMR_OK;
 }
 
@@ -1287,6 +1510,7 @@ int smr_build_index_device(smr_ctx* ctx, uint32_t index_num, const char* fasta_p
     rep[3] += pt.n_ids; rep[5] += pt.bytes;
     ctx->parts.push_back(std::move(pt));
     ctx->n_index_files = std::max(ctx->n_index_files, index_num + 1);
+    ++ctx->parts_gen;
     ++part; first = next;
   }
   if (part == 0) { ctx->err = "no index was created"; return SMR_ERR_INDEX; }
@@ -1507,6 +1731,9 @@ int smr_set_report_refs(smr_ctx* ctx, uint32_t index_num, uint32_t part, const c
     if ((rc = upload_vec(ctx, pt, names, &pt.rnames))) return rc;
     if ((rc = upload_vec(ctx, pt, off, &pt.rname_off))) return rc;
     pt.n_rnames = nref; pt.has_rnames = true;
+    pt.h_rnames.resize(nref);
+    for (uint32_t k = 0; k < nref; ++k) if (name_off[k + 1] > name_off[k]) pt.h_rnames[k].assign(names_cat + name_off[k], name_off[k + 1] - name_off[k]);
+    ++ctx->parts_gen;
     return SMR_OK;
   }
   ctx->err = "smr_set_report_refs: index " + std::to_string(index_num) + " part " + std::to_string(part) + " is not loaded";
@@ -1637,6 +1864,32 @@ int smr_debug_ssw(smr_ctx* ctx, const uint8_t* q_cat, const uint64_t* q_off, con
   CK(cudaMemcpy(out, dout, (size_t)npairs * 6 * 4, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(cigars, dc, (size_t)npairs * cigar_cap * 4, cudaMemcpyDeviceToHost));
   cudaFree(dq); cudaFree(dt); cudaFree(dqo); cudaFree(dto); cudaFree(dc); cudaFree(dout); cudaFree(arena);
+  return SMR_OK;
+}
+
+int smr_otu_begin(smr_ctx* ctx, const smr_otu_opts* opts) try {
+  if (!ctx || !opts) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  return otu_begin_impl(ctx, opts);
+} SMR_CATCH(ctx)
+
+int smr_otu_add(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
+                uint32_t nreads, uint64_t* n_added) try {
+  if (!ctx || (!text && nbytes)) return SMR_ERR_ARG;
+  if (n_added) *n_added = 0;
+  CK(cudaSetDevice(ctx->device));
+  return otu_add_impl(ctx, text, nbytes, results, alns, stats, nreads, n_added);
+} SMR_CATCH(ctx)
+
+int smr_otu_finish(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) try {
+  if (!ctx || !counts) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  return otu_finish_impl(ctx, out, cap, counts);
+} SMR_CATCH(ctx)
+
+int smr_last_otu_timings(const smr_ctx* ctx, double out[3]) {
+  if (!ctx || !out) return SMR_ERR_ARG;
+  for (int k = 0; k < 3; ++k) out[k] = ctx->otu.t[k];
   return SMR_OK;
 }
 

@@ -310,6 +310,47 @@ def denovo_classes(results, alns, slots: int, stats, min_id: float, min_cov: flo
     return out
 
 
+def _round3(x: float) -> float:
+    """denovo_stats_run's rounding to 3 decimals (processor.cpp:334-335)"""
+    return math.floor(x * 1000.0 + 0.5) / 1000.0
+
+
+def _round3_otu(x: float) -> float:
+    """fill_otu_map2's rounding (otumap.cpp:160-161): scaled back with * 0.001, one ulp above / 1000.0 for 144 of the k in 0..1000"""
+    return math.floor(x * 1000.0 + 0.5) * 0.001
+
+
+def otu_map(refs_by_index, headers, results, alns, slots: int, stats, min_id: float, min_cov: float) -> dict:
+    """fill_otu_map / fill_otu_map2 / OtuMap::write (otumap.cpp:84-281) at -threads 1, single-end: the bytes of otu_map.txt,
+    the number of its lines (Total OTUs) and of its entries (n_yid_ycov of aligned.log).  A read is looked at when one of its
+    alignments passes -id and -coverage under denovo_stats_run's rounding (its c_yid_ycov > 0); each of its alignments that passes
+    them under fill_otu_map2's rounding appends the read's QNAME to the line of its reference id.  (index, part) groups are walked in
+    order, reads in order, alignments in slot order; lines come out in unsigned byte order of the id."""
+    n = results.shape[0]
+    per_read = []
+    for r in range(n):
+        rows = []
+        for a in range(int(results["n_align"][r])):
+            al, st = alns[r * slots + a], stats[r * slots + a]
+            tot = int(st["n_miss"]) + int(st["n_gap"]) + int(st["n_match"])
+            idv = int(st["n_match_denovo"]) / tot
+            cov = abs(int(al["read_end1"]) - int(al["read_begin1"]) + 1) / int(al["readlen"])
+            rows.append((al, idv, cov))
+        counts = any(_round3(i) >= min_id and _round3(c) >= min_cov for _, i, c in rows)
+        per_read.append(rows if counts else [])
+    groups = sorted({(int(al["index_num"]), int(al["part"])) for rows in per_read for al, _, _ in rows})
+    lines = {}
+    for g in groups:
+        for r, rows in enumerate(per_read):
+            for al, idv, cov in rows:
+                if (int(al["index_num"]), int(al["part"])) != g or not (_round3_otu(idv) >= min_id and _round3_otu(cov) >= min_cov):
+                    continue
+                ref = _refs_of(refs_by_index, al).ids[int(al["ref_num"])].encode()
+                lines.setdefault(ref, []).append(seq_id(headers[r]).encode())
+    text = b"".join(k + b"\t" + b"\t".join(v) + b"\n" for k, v in sorted(lines.items()))
+    return dict(text=text, total_otu=len(lines), n_yid_ycov=sum(len(v) for v in lines.values()))
+
+
 def is_denovo_read(classes: np.ndarray) -> np.ndarray:
     """output.cpp:130-141 (single-end): the read goes to aligned_denovo.* when n_denovo > 0 and the other three are 0"""
     return (classes[:, 3] > 0) & (classes[:, 0] == 0) & (classes[:, 1] == 0) & (classes[:, 2] == 0)
