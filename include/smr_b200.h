@@ -253,8 +253,19 @@ typedef struct {
 int smr_format_reports(smr_ctx*, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
                        const smr_aln* alns, const uint32_t* cigar_pool, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
                        char* out, uint64_t cap, uint64_t* stream_off);
-/* of the last smr_format_reports, milliseconds (CUDA events): out[0] = H2D of text and results, [1] = device work (layout, sizes,
- * scans, writes; includes the one read-back of the sizes), [2] = D2H of the output */
+/* The same streams, each non-empty one compressed on the device to one gzip member (RFC 1952) before the D2H: the reference's
+ * -zip-out output (its report writers go through zlib's gzip wrapper, izlib.cpp).  An empty stream stays 0 bytes.  Arguments and
+ * stream_off as for smr_format_reports, with the sizes of the members: if out is null or cap is below stream_off[2 * groups + 3], the
+ * call returns SMR_ERR_CAPACITY with the exact compressed sizes in stream_off, and a retry gives the same bytes.  The members are not
+ * zlib's bytes (sortmerna_b200/csrc/smr_deflate.h) but the same input always gives the same bytes. */
+int smr_format_reports_gz(smr_ctx*, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
+                          const smr_aln* alns, const uint32_t* cigar_pool, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                          char* out, uint64_t cap, uint64_t* stream_off);
+/* n host bytes compressed on the device into one gzip member (n == 0: an empty member).  *out_bytes = its size; if out is null or
+ * cap is smaller, SMR_ERR_CAPACITY. */
+int smr_gzip(smr_ctx*, const void* in, uint64_t n, void* out, uint64_t cap, uint64_t* out_bytes);
+/* of the last smr_format_reports[_gz] or smr_gzip, milliseconds (CUDA events): out[0] = H2D of the input (text and results), [1] =
+ * device work (layout, sizes, scans, writes, compression; includes the read-backs of the sizes), [2] = D2H of the output */
 int smr_last_report_timings(const smr_ctx*, double out[3]);
 
 /* -- OTU map on the device (sortmerna_b200/csrc/smr_otu.cuh, DESIGN.md 5e): the reference's otu_map.txt (fill_otu_map /

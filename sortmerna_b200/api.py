@@ -28,7 +28,8 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_debug_dpx_peak", "smr_set_stats_buffer", "smr_build_index", "smr_upload_fastx", "smr_resident_layout", "smr_pack_kvdb_blobs",
            "smr_set_aln_slots", "smr_aln_slots", "smr_aln_slots_needed", "smr_upload_fastx_gz", "smr_resident_text", "smr_debug_inflate",
            "smr_build_index_device", "smr_debug_index_array", "smr_set_instrumentation", "smr_set_report_refs", "smr_set_report_scoring",
-           "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings"]
+           "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings",
+           "smr_format_reports_gz", "smr_gzip"]
 
 CNT_NAMES = ("num_aligned", "num_short", "sw_calls", "sw_cells", "windows", "trie_nodes", "buckets",
              "bucket_entries", "pos_entries", "lis_calls", "dbg_max_read_cycles", "dbg_sum_read_cycles", "dbg_lis_kernel_cycles",
@@ -422,11 +423,21 @@ class Aligner:
         self._check(self.L.smr_set_report_scoring(self.h, C.c_uint32(index_num), C.c_double(lam), C.c_double(K), C.c_uint64(int(full_ref)),
                                                   C.c_uint64(int(full_read))), "smr_set_report_scoring")
 
-    def format_reports(self, out: dict, text: bytes | None = None, opts: ReportOpts | None = None, **kw) -> dict:
+    def gzip(self, data: bytes) -> bytes:
+        """smr_gzip: `data` compressed on the device into one gzip member (an empty member for empty data)"""
+        buf = np.frombuffer(data, np.uint8)
+        cap = buf.size + (buf.size >> 6) + 1024   # the stored fallback bounds a member: 10 bytes per 32 KB chunk, 18 around
+        o = np.zeros(cap, np.uint8)
+        nb = C.c_uint64(0)
+        self.L.smr_gzip.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
+        self._check(self.L.smr_gzip(self.h, _ptr(buf) if buf.size else None, buf.size, _ptr(o), o.size, C.cast(C.byref(nb), C.c_void_p)), "smr_gzip")
+        return o[:nb.value].tobytes()
+
+    def format_reports(self, out: dict, text: bytes | None = None, opts: ReportOpts | None = None, gzip: bool = False, **kw) -> dict:
         """smr_format_reports: the report streams of one batch as bytes.  out = what align(with_stats=True) / download(with_stats=True)
         returned for it; text = the batch's FASTA / FASTQ bytes (None: the resident text of upload_fastx[_gz]); opts = report_opts(...)
         or its keyword arguments.  Returns {"sam": [bytes per group], "blast": [...], "aligned": bytes, "other": bytes, "denovo": bytes,
-        "groups": report_groups()}."""
+        "groups": report_groups()}.  gzip: smr_format_reports_gz, every non-empty stream as one gzip member (empty ones stay b"")."""
         o = opts if opts is not None else report_opts(**kw)
         if o.sam or o.blast:
             self._upload_report_refs()
@@ -437,19 +448,19 @@ class Aligner:
         st = out.get("stats")
         txt = np.frombuffer(text, np.uint8) if text is not None else None
         so = np.zeros(2 * G + 4, np.uint64)
-        L = self.L
-        L.smr_format_reports.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
-                                         C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
+        fn = self.L.smr_format_reports_gz if gzip else self.L.smr_format_reports
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                       C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
         args = [self.h, C.cast(C.byref(o), C.c_void_p), _ptr(txt) if txt is not None and txt.size else None, txt.size if txt is not None else 0,
                 _ptr(res), _ptr(alns), _ptr(cig) if cig.size else None, cig.size, _ptr(st) if st is not None else None, res.shape[0]]
         buf = getattr(self, "_report_buf", None)
         if buf is None:
             buf = np.zeros(1 << 20, np.uint8)
-        rc = L.smr_format_reports(*args, _ptr(buf), buf.size, _ptr(so))
+        rc = fn(*args, _ptr(buf), buf.size, _ptr(so))
         if rc == 5 and int(so[-1]) > buf.size:   # SMR_ERR_CAPACITY: so names the size; grow and run again
             buf = np.zeros(int(so[-1]) + (int(so[-1]) >> 3), np.uint8)
-            rc = L.smr_format_reports(*args, _ptr(buf), buf.size, _ptr(so))
-        self._check(rc, "smr_format_reports")
+            rc = fn(*args, _ptr(buf), buf.size, _ptr(so))
+        self._check(rc, "smr_format_reports_gz" if gzip else "smr_format_reports")
         self._report_buf = buf
         b = [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(2 * G + 3)]
         return dict(sam=b[:G], blast=b[G:2 * G], aligned=b[2 * G], other=b[2 * G + 1], denovo=b[2 * G + 2], groups=groups)
@@ -545,10 +556,13 @@ class ReportWriter:
     group 0, then group 1, ...), so that feeding a file in several batches writes what one batch writes.
     sam_header: the text before the SAM rows (hostio.sam_header); opts: report_opts(...) keyword arguments.
     otu_map: (min_id, min_cov) = the reference's -otu_map -id -coverage: close() also writes otu_map.txt (none when no alignment
-    passes, as the reference) and sets total_otu and n_yid_ycov, the two OTU numbers of aligned.log."""
+    passes, as the reference) and sets total_otu and n_yid_ycov, the two OTU numbers of aligned.log.
+    zip_out: the reference's -zip-out (its default for gzip input): every report file is written gzip-compressed on the device under
+    its name with ".gz" appended, as members appended batch by batch (a multi-member file, as the reference's merge makes); a file
+    with no member gets one empty member.  otu_map.txt stays plain, as the reference writes it."""
 
-    def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", otu_map=None, **opts):
-        self.dir, self.al, self.header = out_dir, aligner, sam_header
+    def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", otu_map=None, zip_out: bool = False, **opts):
+        self.dir, self.al, self.header, self.zip_out = out_dir, aligner, sam_header, zip_out
         self.opts = report_opts(**opts)
         self.otu_map, self.total_otu, self.n_yid_ycov = otu_map, None, None
         if otu_map is not None:
@@ -568,7 +582,7 @@ class ReportWriter:
         if self.ext is None:
             first = text[:1] if text is not None else self.al.resident_text()[:1]
             self.ext = "fq" if first == b"@" else "fa"
-        s = self.al.format_reports(out, text, opts=self.opts)
+        s = self.al.format_reports(out, text, opts=self.opts, gzip=self.zip_out)
         for g, (rows_sam, rows_blast) in enumerate(zip(s["sam"], s["blast"])):
             self._append(f"sam_{g}", rows_sam)
             self._append(f"blast_{g}", rows_blast)
@@ -582,8 +596,9 @@ class ReportWriter:
         """write the files; returns their paths"""
         o, ext, groups = self.opts, self.ext or "fq", self.al.report_groups()
         files = []
+        head = self.header.encode()
         if o.sam:
-            files.append(("aligned.sam", [f"sam_{g}" for g in range(len(groups))], self.header.encode()))
+            files.append(("aligned.sam", [f"sam_{g}" for g in range(len(groups))], self.al.gzip(head) if self.zip_out and head else head))
         if o.blast:
             files.append(("aligned.blast", [f"blast_{g}" for g in range(len(groups))], b""))
         for flag, name, key in ((o.fastx, "aligned", "aligned"), (o.other, "other", "other"), (o.denovo, "aligned_denovo", "denovo")):
@@ -591,7 +606,7 @@ class ReportWriter:
                 files.append((f"{name}.{ext}", [key], b""))
         paths = []
         for name, keys, head in files:
-            path = os.path.join(self.dir, name)
+            path = os.path.join(self.dir, name + (".gz" if self.zip_out else ""))
             with open(path, "wb") as f:
                 f.write(head)
                 for k in keys:
@@ -603,6 +618,8 @@ class ReportWriter:
                             if not chunk:
                                 break
                             f.write(chunk)
+                if self.zip_out and f.tell() == 0:
+                    f.write(self.al.gzip(b""))
             paths.append(path)
         if self.otu_map is not None:
             m = self.al.otu_finish()

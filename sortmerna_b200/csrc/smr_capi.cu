@@ -16,6 +16,7 @@
 #include "smr_report.cuh"
 #include "smr_otu.cuh"
 #include "smr_inflate.cuh"
+#include "smr_deflate.cuh"
 #include "smr_build.h"
 #include "smr_build_dev.cuh"
 #include "smr_final.cuh"
@@ -89,6 +90,7 @@ struct smr_ctx {
   DevBuf r_text, r_nl, r_hdr, r_sb, r_rec, r_spos, r_line, r_recs, r_res, r_aln, r_cig, r_st, r_flags, r_keys, r_keys2, r_vals, r_rows, r_first,
          r_sz, r_off, r_bsz, r_boff, r_fxsz, r_fxoff, r_grp, r_so, r_tmp, r_out, r_scal;
   double t_rpt[3] = {0, 0, 0};
+  DevBuf z_in, z_chunk, z_m, z_freq, z_codes, z_hdr, z_info, z_scratch, z_poff, z_plen, z_crc, z_dst, z_trl, z_out;   // gzip deflate (smr_deflate.cuh)
   uint64_t parts_gen = 0;   // bumped whenever a part is loaded or its report ids are set: an open OTU map refuses to go on after that
   // OTU map accumulator (smr_otu.cuh), smr_otu_begin .. smr_otu_finish
   struct Otu {
@@ -1061,9 +1063,86 @@ std::vector<const Part*> report_groups(const smr_ctx* ctx) {
   return gp;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// gzip deflate (smr_deflate.cuh)
+// ---------------------------------------------------------------------------------------------------------------------
+// The streams [sb[k], se[k]) of the device bytes `in` (padded by >= 8 readable bytes), each non-empty one compressed to one gzip
+// member, into the host buffer `out` one after another; so[0 .. ns] = their offsets.  If the members do not fit in cap, returns
+// SMR_ERR_CAPACITY with so filled (a retry gives the same bytes).  e_dev is recorded before the D2H, e_end after it.
+int gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& sb, const std::vector<uint64_t>& se, char* out, uint64_t cap,
+                 uint64_t* so, cudaEvent_t e_dev, cudaEvent_t e_end) {
+  const uint32_t ns = (uint32_t)sb.size();
+  std::vector<DefChunk> ch;
+  def_plan(sb.data(), se.data(), ns, ch);
+  const uint32_t nch = (uint32_t)ch.size();
+  int rc;
+  std::vector<DefInfo> info(nch);
+  std::vector<uint32_t> crcs(nch);
+  if (nch) {
+    const uint64_t end = se[ns - 1];
+    std::vector<uint64_t> poff(nch); std::vector<uint32_t> plen(nch);
+    for (uint32_t c = 0; c < nch; ++c) { poff[c] = ch[c].b; plen[c] = (uint32_t)(ch[c].e - ch[c].b); }
+    if ((rc = upload_async(ctx, ctx->z_chunk, ch.data(), nch))) return rc;
+    if ((rc = upload_async(ctx, ctx->z_poff, poff.data(), nch))) return rc;
+    if ((rc = upload_async(ctx, ctx->z_plen, plen.data(), nch))) return rc;
+    if ((rc = ensure(ctx, ctx->z_m, (end + 1) * 4))) return rc;
+    if ((rc = ensure(ctx, ctx->z_freq, (size_t)nch * kDefFreqStride * 4))) return rc;
+    if ((rc = ensure(ctx, ctx->z_codes, (size_t)nch * sizeof(DefCodes)))) return rc;
+    if ((rc = ensure(ctx, ctx->z_hdr, (size_t)nch * kDefHdrWords * 4))) return rc;
+    if ((rc = ensure(ctx, ctx->z_info, (size_t)nch * sizeof(DefInfo)))) return rc;
+    if ((rc = ensure(ctx, ctx->z_scratch, (size_t)nch * kDefScratch))) return rc;
+    if ((rc = ensure(ctx, ctx->z_crc, (size_t)nch * 4))) return rc;
+    CK(cudaMemsetAsync(ctx->z_freq.p, 0, (size_t)nch * kDefFreqStride * 4, ctx->stream));
+    CK(cudaMemsetAsync(ctx->z_hdr.p, 0, (size_t)nch * kDefHdrWords * 4, ctx->stream));
+    CK(cudaMemsetAsync(ctx->z_scratch.p, 0, (size_t)nch * kDefScratch, ctx->stream));
+    const DefChunk* dch = (const DefChunk*)ctx->z_chunk.p;
+    uint32_t* m = (uint32_t*)ctx->z_m.p;
+    DefInfo* dinfo = (DefInfo*)ctx->z_info.p;
+    def_match_kernel<<<nch, 32, 0, ctx->stream>>>(in, dch, m);
+    def_parse_kernel<<<(nch + 127) / 128, 128, 0, ctx->stream>>>(in, dch, nch, m, (uint32_t*)ctx->z_freq.p, dinfo);
+    def_code_kernel<<<(nch + 1) / 2, 64, 0, ctx->stream>>>(dch, nch, (const uint32_t*)ctx->z_freq.p, (DefCodes*)ctx->z_codes.p, (uint32_t*)ctx->z_hdr.p, dinfo);
+    def_write_kernel<<<(nch + 3) / 4, 128, 0, ctx->stream>>>(in, dch, nch, m, (const DefCodes*)ctx->z_codes.p, (const uint32_t*)ctx->z_hdr.p, dinfo,
+                                                             (uint8_t*)ctx->z_scratch.p);
+    inf_crc_kernel<<<(nch + 127) / 128, 128, 0, ctx->stream>>>(in, (const uint64_t*)ctx->z_poff.p, (const uint32_t*)ctx->z_plen.p, nch, (uint32_t*)ctx->z_crc.p);
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(info.data(), ctx->z_info.p, (size_t)nch * sizeof(DefInfo), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(crcs.data(), ctx->z_crc.p, (size_t)nch * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  // the byte-size scan: chunk c goes to dst[c]; every member is header, its chunks, trailer
+  std::vector<uint64_t> dst(nch);
+  std::vector<uint32_t> trl(2 * (size_t)ns + 2, 0);
+  uint64_t at = 0;
+  uint32_t c = 0;
+  for (uint32_t k = 0; k < ns; ++k) {
+    so[k] = at;
+    if (se[k] == sb[k]) continue;
+    at += 10;
+    uint32_t crc = 0;
+    for (; c < nch && ch[c].stream == k; ++c) { dst[c] = at; at += info[c].bytes; crc = crc_concat(crc, crcs[c], ch[c].e - ch[c].b); }
+    trl[2 * k] = crc; trl[2 * k + 1] = (uint32_t)(se[k] - sb[k]);
+    at += 8;
+  }
+  so[ns] = at;
+  if (at && (!out || cap < at)) { ctx->err = "output buffer too small: stream_off holds the compressed sizes"; return SMR_ERR_CAPACITY; }
+  if (nch) {
+    if ((rc = upload_async(ctx, ctx->z_dst, dst.data(), nch))) return rc;
+    if ((rc = upload_async(ctx, ctx->z_trl, trl.data(), trl.size()))) return rc;
+    if ((rc = ensure(ctx, ctx->z_out, at))) return rc;
+    def_place_kernel<<<nch, 256, 0, ctx->stream>>>((const DefChunk*)ctx->z_chunk.p, (const DefInfo*)ctx->z_info.p, (const uint8_t*)ctx->z_scratch.p,
+                                                   (const uint64_t*)ctx->z_dst.p, (const uint32_t*)ctx->z_trl.p, (uint8_t*)ctx->z_out.p);
+    CK(cudaGetLastError());
+  }
+  CK(cudaEventRecord(e_dev, ctx->stream));
+  if (at) CK(cudaMemcpyAsync(out, ctx->z_out.p, at, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e_end, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return SMR_OK;
+}
+
 int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
                         const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
-                        char* out, uint64_t cap, uint64_t* so_out) {
+                        char* out, uint64_t cap, uint64_t* so_out, bool gz) {
   if (o->out2 || o->sout) { ctx->err = "-out2 / -sout: the report writer writes one aligned and one other file"; return SMR_ERR_UNSUPPORTED; }
   if (o->blast && o->blast_format != 1) { ctx->err = "only tabular BLAST (-blast 1) is written on the device"; return SMR_ERR_UNSUPPORTED; }
   if (o->paired_in && o->paired_out) { ctx->err = "paired_in and paired_out are exclusive"; return SMR_ERR_ARG; }
@@ -1166,21 +1245,29 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   if (h[4]) return rpt_error(ctx, h[4]);
-  memcpy(so_out, hso.data(), (size_t)nso * 8);
+  if (!gz) memcpy(so_out, hso.data(), (size_t)nso * 8);
   const uint64_t total = hso[nso - 1];
-  if (total && (!out || cap < total)) { ctx->err = "output buffer too small: stream_off holds the sizes"; return SMR_ERR_CAPACITY; }
+  if (!gz && total && (!out || cap < total)) { ctx->err = "output buffer too small: stream_off holds the sizes"; return SMR_ERR_CAPACITY; }
+  // the encoder reads up to 8 bytes past a stream's end (def_load32): the padding is part of the one allocation before the writes,
+  // since ensure() does not keep what a buffer held
+  if ((total || gz) && (rc = ensure(ctx, ctx->r_out, total + (gz ? 8 : 0)))) return rc;
   if (total) {
-    if ((rc = ensure(ctx, ctx->r_out, total))) return rc;
     char* dout = (char*)ctx->r_out.p;
     if (o->sam) rpt_sam_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, off, dout);
     if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, nullptr, boff, dout + hso[G]);
     if (o->fastx || o->other || o->denovo) rpt_fx_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, fxoff, fstride, so + 2 * G, dout);
     CK(cudaGetLastError());
   }
-  CK(cudaEventRecord(e2, ctx->stream));
-  if (total) CK(cudaMemcpyAsync(out, ctx->r_out.p, total, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaEventRecord(e3, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
+  if (gz) {   // every non-empty stream to one gzip member, before the D2H
+    std::vector<uint64_t> sb(hso.begin(), hso.end() - 1), se(hso.begin() + 1, hso.end());
+    rc = gzip_streams(ctx, (const uint8_t*)ctx->r_out.p, sb, se, out, cap, so_out, e2, e3);
+    if (rc) return rc;
+  } else {
+    CK(cudaEventRecord(e2, ctx->stream));
+    if (total) CK(cudaMemcpyAsync(out, ctx->r_out.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(e3, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
   cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
@@ -1416,7 +1503,9 @@ void smr_destroy(smr_ctx* ctx) {
                     &ctx->d_moff, &ctx->d_mem, &ctx->d_poff, &ctx->d_plen, &ctx->d_pcrc, &ctx->seed_ctr,
                     &ctx->r_text, &ctx->r_nl, &ctx->r_hdr, &ctx->r_sb, &ctx->r_rec, &ctx->r_spos, &ctx->r_line, &ctx->r_recs, &ctx->r_res, &ctx->r_aln,
                     &ctx->r_cig, &ctx->r_st, &ctx->r_flags, &ctx->r_keys, &ctx->r_keys2, &ctx->r_vals, &ctx->r_rows, &ctx->r_first, &ctx->r_sz, &ctx->r_off,
-                    &ctx->r_bsz, &ctx->r_boff, &ctx->r_fxsz, &ctx->r_fxoff, &ctx->r_grp, &ctx->r_so, &ctx->r_tmp, &ctx->r_out, &ctx->r_scal};
+                    &ctx->r_bsz, &ctx->r_boff, &ctx->r_fxsz, &ctx->r_fxoff, &ctx->r_grp, &ctx->r_so, &ctx->r_tmp, &ctx->r_out, &ctx->r_scal,
+                    &ctx->z_in, &ctx->z_chunk, &ctx->z_m, &ctx->z_freq, &ctx->z_codes, &ctx->z_hdr, &ctx->z_info, &ctx->z_scratch, &ctx->z_poff,
+                    &ctx->z_plen, &ctx->z_crc, &ctx->z_dst, &ctx->z_trl, &ctx->z_out};
   for (DevBuf* b : bufs) release(*b);
   for (auto& sc : ctx->rpt_score) { release(sc.ev); release(sc.bits); }
   DevBuf* obufs[] = {&ctx->otu.rank, &ctx->otu.rank_off, &ctx->otu.grp, &ctx->otu.key, &ctx->otu.ent, &ctx->otu.pool, &ctx->otu.flag, &ctx->otu.pos,
@@ -1766,7 +1855,44 @@ int smr_format_reports(smr_ctx* ctx, const smr_report_opts* opts, const char* te
                        char* out, uint64_t cap, uint64_t* stream_off) try {
   if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  return format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off);
+  return format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, false);
+} SMR_CATCH(ctx)
+
+int smr_format_reports_gz(smr_ctx* ctx, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
+                          const smr_aln* alns, const uint32_t* cigar_pool, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                          char* out, uint64_t cap, uint64_t* stream_off) try {
+  if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  return format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, true);
+} SMR_CATCH(ctx)
+
+int smr_gzip(smr_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t cap, uint64_t* out_bytes) try {
+  if (!ctx || !out_bytes || (!in && n)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  *out_bytes = 0;
+  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
+  CK(cudaEventRecord(e0, ctx->stream));
+  if (n == 0) {   // one empty member
+    *out_bytes = sizeof kGzEmpty;
+    if (!out || cap < sizeof kGzEmpty) { ctx->err = "output buffer too small: out_bytes holds the size"; return SMR_ERR_CAPACITY; }
+    memcpy(out, kGzEmpty, sizeof kGzEmpty);
+    ctx->t_rpt[0] = ctx->t_rpt[1] = ctx->t_rpt[2] = 0;
+    return SMR_OK;
+  }
+  int rc;
+  if ((rc = ensure(ctx, ctx->z_in, n + 64))) return rc;
+  CK(cudaMemsetAsync((uint8_t*)ctx->z_in.p + n, 0, 64, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->z_in.p, in, n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaEventRecord(e1, ctx->stream));
+  uint64_t so[2];
+  rc = gzip_streams(ctx, (const uint8_t*)ctx->z_in.p, {0}, {n}, (char*)out, cap, so, e2, e3);
+  *out_bytes = so[1];
+  if (rc) return rc;
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
+  cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
+  cudaEventElapsedTime(&ms, e2, e3); ctx->t_rpt[2] = ms;
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_last_report_timings(const smr_ctx* ctx, double out[3]) {

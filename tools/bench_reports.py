@@ -3,8 +3,13 @@ databases, aligned once on the GPU, then formatted per output kind.  Prints one 
   * per format (sam, blast, fastx+other, denovo, all): device time of the call (CUDA events: layout, size pass, scans, write pass),
     the H2D of text + results and the D2H of the output, the call's wall time, output MB/s and reads/s;
   * the host formatters of hostio (format_sam_rows / format_blast_rows, one Python row at a time) on a subset;
-  * with --reference, the reference binary's report stage ("done Reports in" of its log) on a subset of the same reads.
-Run on the GPU:  python tools/bench_reports.py --reads 1000000"""
+  * with --reference, the reference binary's report stage ("done Reports in" of its log) on a subset of the same reads;
+  * with --gzip, per format the gzip call (smr_format_reports_gz, the -zip-out output) next to the plain call on the same reads: the
+    compressed bytes, the call wall times, the sizes Python's zlib makes of the same streams at levels 1 and 6, and the gz call's
+    device span minus the plain call's (compress_span_ms: the encoder's kernels plus the host work inside the span -- chunk plan,
+    the read-back of the chunk sizes, the byte-size scan, the uploads).  For "all", the encoder's kernels alone under torch.profiler
+    (one run of its own): device time per kernel, their sum and its input GB/s.
+Run on the GPU:  python tools/bench_reports.py --reads 1000000 [--gzip]"""
 import argparse
 import json
 import os
@@ -12,6 +17,7 @@ import re
 import sys
 import tempfile
 import time
+import zlib
 
 import numpy as np
 
@@ -32,6 +38,7 @@ def main():
     ap.add_argument("--reps", type=int, default=5)
     ap.add_argument("--host-reads", type=int, default=20_000, help="subset for the Python hostio formatters")
     ap.add_argument("--reference", type=int, default=0, help="reads of the subset the reference binary formats (0: skip)")
+    ap.add_argument("--gzip", action="store_true", help="also time the gzip (-zip-out) call of every format")
     args = ap.parse_args()
     out = dict(card=bench.card(0), reads=args.reads)
     with tempfile.TemporaryDirectory(prefix="smr_bench_rpt_") as work:
@@ -56,21 +63,56 @@ def main():
         res = al.download()
         out["aligned"] = int(res["res"]["is_hit"].sum())
         out["text_mb"] = len(text) / 1e6
-        fm = {}
-        for name, kw in FORMATS.items():
-            al.format_reports(res, None, **kw)   # warm-up: buffers, module load
+        def timed(kw, gz):
+            al.format_reports(res, None, gzip=gz, **kw)   # warm-up: buffers, module load
             dev, wall = [], []
             for _ in range(args.reps):
                 t0 = time.perf_counter()
-                s = al.format_reports(res, None, **kw)
+                s = al.format_reports(res, None, gzip=gz, **kw)
                 wall.append(time.perf_counter() - t0)
                 dev.append(al.report_timings())
-            nb = sum(len(x) for x in s["sam"] + s["blast"]) + len(s["aligned"]) + len(s["other"]) + len(s["denovo"])
-            dms = float(np.median([t["device_ms"] for t in dev]))
-            w = float(np.median(wall))
-            fm[name] = dict(out_mb=nb / 1e6, device_ms=dms, h2d_ms=float(np.median([t["h2d_ms"] for t in dev])),
-                            d2h_ms=float(np.median([t["d2h_ms"] for t in dev])), call_wall_ms=w * 1e3,
-                            device_mb_s=nb / 1e6 / (dms / 1e3), wall_mb_s=nb / 1e6 / w, wall_reads_s=n / w)
+            med = {k: float(np.median([t[k] for t in dev])) for k in ("device_ms", "h2d_ms", "d2h_ms")}
+            return s, med, float(np.median(wall))
+
+        def streams(s):
+            return dict(sam=b"".join(s["sam"]), blast=b"".join(s["blast"]), aligned=s["aligned"], other=s["other"], denovo=s["denovo"])
+
+        fm, zl = {}, {}
+        for name, kw in FORMATS.items():
+            s, med, w = timed(kw, False)
+            nb = sum(len(x) for x in streams(s).values())
+            fm[name] = dict(out_mb=nb / 1e6, device_ms=med["device_ms"], h2d_ms=med["h2d_ms"], d2h_ms=med["d2h_ms"], call_wall_ms=w * 1e3,
+                            device_mb_s=nb / 1e6 / (med["device_ms"] / 1e3), wall_mb_s=nb / 1e6 / w, wall_reads_s=n / w)
+            if args.gzip:
+                if name == "all":   # zlib of every stream kind once; a format's size is the sum over the kinds it writes
+                    for k, v in streams(s).items():
+                        zl[k] = (len(zlib.compress(v, 1)), len(zlib.compress(v, 6)))
+                g, gmed, gw = timed(kw, True)
+                gb = sum(len(x) for x in g["sam"] + g["blast"]) + len(g["aligned"]) + len(g["other"]) + len(g["denovo"])
+                comp = gmed["device_ms"] - med["device_ms"]
+                fm[name]["gzip"] = dict(out_mb=gb / 1e6, ratio=gb / nb if nb else None, device_ms=gmed["device_ms"], compress_span_ms=comp,
+                                        compress_span_in_gb_s=nb / 1e9 / (comp / 1e3) if comp > 0 else None, h2d_ms=gmed["h2d_ms"],
+                                        d2h_ms=gmed["d2h_ms"], call_wall_ms=gw * 1e3, plain_call_wall_ms=w * 1e3)
+        if args.gzip:
+            for name in fm:
+                kinds = [k for k, v in streams(al.format_reports(res, None, **FORMATS[name])).items() if v]
+                fm[name]["gzip"]["zlib1_mb"] = sum(zl[k][0] for k in kinds) / 1e6
+                fm[name]["gzip"]["zlib6_mb"] = sum(zl[k][1] for k in kinds) / 1e6
+        if args.gzip:   # the encoder's kernels alone, in a profiled run of their own
+            import torch
+            from torch.profiler import ProfilerActivity, profile
+            torch.cuda.synchronize()
+            with profile(activities=[ProfilerActivity.CUDA]) as prof:
+                al.format_reports(res, None, gzip=True, **FORMATS["all"])
+                torch.cuda.synchronize()
+            kern = {}
+            for ev in prof.key_averages():
+                if "def_" in ev.key or "inf_crc" in ev.key:
+                    t_us = getattr(ev, "device_time_total", None)
+                    kern[ev.key.split("(")[0].replace("smr::", "")] = (t_us if t_us is not None else ev.cuda_time_total) / 1e3
+            tot = sum(kern.values())
+            fm["all"]["gzip"].update(kernels_ms=kern, compress_kernels_ms=tot,
+                                     compress_kernels_in_gb_s=fm["all"]["out_mb"] / 1e3 / (tot / 1e3) if tot > 0 else None)
         out["writer"] = fm
         # Python host formatters on a subset
         m = args.host_reads
