@@ -26,19 +26,35 @@ using namespace smr;
 
 namespace {
 
+// Device memory (DevBuf) or page-locked host memory (PinBuf), freed by its destructor.  Move-only: the buffers live in vectors.
+template <bool kPinned>
+struct Buf {
+  void* p = nullptr; size_t cap = 0;
+  Buf() = default;
+  Buf(Buf&& o) noexcept : p(o.p), cap(o.cap) { o.p = nullptr; o.cap = 0; }
+  Buf& operator=(Buf&& o) noexcept { std::swap(p, o.p); std::swap(cap, o.cap); return *this; }   // o frees what this held
+  ~Buf() { reset(); }
+  void reset() {
+    if (p) { if (kPinned) cudaFreeHost(p); else cudaFree(p); }
+    p = nullptr; cap = 0;
+  }
+  // exactly `bytes`, contents undefined; what the buffer held is freed first
+  cudaError_t alloc(size_t bytes) {
+    reset();
+    const cudaError_t e = kPinned ? cudaHostAlloc(&p, bytes, cudaHostAllocDefault) : cudaMalloc(&p, bytes);
+    if (e == cudaSuccess) cap = bytes; else p = nullptr;
+    return e;
+  }
+};
+using DevBuf = Buf<false>;
+using PinBuf = Buf<true>;   // host staging (page-locked once; pageable vectors cost a page-fault pass + a bounce copy per batch)
+
 struct Part {
   DevIndex d{};
-  std::vector<void*> owned;   // device allocations
+  std::vector<DevBuf> owned;   // the device arrays behind d and rnames (part_array)
   size_t bytes = 0, n_nodes = 0, n_entries = 0, n_ids = 0, n_pos = 0, n_refseq = 0;
   const char* rnames = nullptr; const uint64_t* rname_off = nullptr; uint32_t n_rnames = 0; bool has_rnames = false;   // smr_set_report_refs
   std::vector<std::string> h_rnames;   // host copy of the same ids: the OTU map ranks them (smr_otu_begin)
-};
-
-struct DevBuf {
-  void* p = nullptr; size_t cap = 0;
-};
-struct PinBuf {   // grow-only pinned host staging (page-locked once; pageable vectors cost a page-fault pass + a bounce copy per batch)
-  void* p = nullptr; size_t cap = 0;
 };
 
 }  // namespace
@@ -68,7 +84,9 @@ struct smr_ctx {
   smr_aln_stats* host_stats = nullptr;   // optional output of the report arithmetic
   PinBuf h_state, h_flags, h_hitdb, h_outaln, h_stats, h_cigar, h_off32, h_pkoff;
   std::vector<uint64_t> h_coff;
-  DevBuf d_text, d_cnt, d_scal, d_nl, d_hdr, d_sb, d_rec, d_spos, d_hdroff, scan_sums;   // input decode (smr_decode.cuh)
+  DevBuf d_text, d_hdroff;   // input decode (smr_decode.cuh)
+  DevBuf d_cnt, d_scal, d_nl, d_hdr, d_sb, d_rec, d_spos;   // line layout of a text (text_layout), for the decode and the report writer
+  DevBuf cub_tmp;   // cub scratch of the text layout, the report writer and the OTU map
   DevBuf seed_ctr, d_gz, d_cand, d_res, d_sym, d_win, d_ids, d_off, d_cnt64, d_moff, d_mem, d_poff, d_plen, d_pcrc;   // gz inflate (smr_inflate.cuh)
   uint64_t text_bytes = 0;          // size of the text behind the resident batch (smr_upload_fastx / _gz)
   uint32_t inf_spans = 0, inf_candidates = 0; double t_inflate = 0;
@@ -87,8 +105,8 @@ struct smr_ctx {
   // report writer (smr_report.cuh)
   struct RptScore { bool set = false; DevBuf ev, bits; };
   std::vector<RptScore> rpt_score;   // per index_num (smr_set_report_scoring)
-  DevBuf r_text, r_nl, r_hdr, r_sb, r_rec, r_spos, r_line, r_recs, r_res, r_aln, r_cig, r_st, r_flags, r_keys, r_keys2, r_vals, r_rows, r_first,
-         r_sz, r_off, r_bsz, r_boff, r_fxsz, r_fxoff, r_grp, r_so, r_tmp, r_out, r_scal;
+  DevBuf r_text, r_line, r_recs, r_res, r_aln, r_cig, r_st, r_flags, r_keys, r_keys2, r_vals, r_rows, r_first,
+         r_sz, r_off, r_bsz, r_boff, r_fxsz, r_fxoff, r_grp, r_so, r_out;
   double t_rpt[3] = {0, 0, 0};
   DevBuf z_in, z_chunk, z_m, z_freq, z_codes, z_hdr, z_info, z_scratch, z_poff, z_plen, z_crc, z_dst, z_trl, z_out;   // gzip deflate (smr_deflate.cuh)
   uint64_t parts_gen = 0;   // bumped whenever a part is loaded or its report ids are set: an open OTU map refuses to go on after that
@@ -96,7 +114,7 @@ struct smr_ctx {
   struct Otu {
     bool active = false; uint64_t gen = 0; double min_id = 0, min_cov = 0;
     std::vector<RptGroup> groups; uint32_t gbits = 0, kbits = 0;
-    DevBuf rank, rank_off, grp, key, ent, pool, flag, pos, nsz, noff, vals, skey, sidx, size, off, out, tmp, scal;
+    DevBuf rank, rank_off, grp, key, ent, pool, flag, pos, nsz, noff, vals, skey, sidx, size, off, out, scal;
     uint64_t n = 0, pool_bytes = 0;
     double t[3] = {0, 0, 0};
   } otu;
@@ -119,46 +137,50 @@ namespace {
 // alignment slots per read in every flat result array: num_alignments, or the stride set for "all alignments" (0)
 uint32_t slots_of(const smr_ctx* ctx) { return ctx->prm.num_alignments > 0 ? (uint32_t)ctx->prm.num_alignments : std::max(1u, ctx->all_slots); }
 
-int ensure(smr_ctx* ctx, DevBuf& b, size_t bytes) {
+// grow-only: at least `bytes`; what the buffer held is not kept
+template <bool kPinned>
+int ensure(smr_ctx* ctx, Buf<kPinned>& b, size_t bytes) {
   if (bytes <= b.cap && b.p) return SMR_OK;
-  if (b.p) { cudaFree(b.p); b.p = nullptr; b.cap = 0; }
-  size_t want = bytes + bytes / 8 + 256;
-  CK(cudaMalloc(&b.p, want));
-  b.cap = want;
+  CK(b.alloc(bytes + bytes / 8 + 256));
   return SMR_OK;
 }
-void release(DevBuf& b) { if (b.p) cudaFree(b.p); b.p = nullptr; b.cap = 0; }
-int ensure_pinned(smr_ctx* ctx, PinBuf& b, size_t bytes) {
-  if (bytes <= b.cap && b.p) return SMR_OK;
-  if (b.p) { cudaFreeHost(b.p); b.p = nullptr; b.cap = 0; }
-  const size_t want = bytes + bytes / 8 + 256;
-  CK(cudaHostAlloc(&b.p, want, cudaHostAllocDefault));
-  b.cap = want;
-  return SMR_OK;
-}
-void release(PinBuf& b) { if (b.p) cudaFreeHost(b.p); b.p = nullptr; b.cap = 0; }
 
+// a device array of the part: n items, copied from src (host) or else zero, and 64 zero bytes of slack past the end; counted in pt.bytes
 template <class T>
-int upload_vec(smr_ctx* ctx, Part& pt, const std::vector<T>& v, const T** out) {
-  void* d = nullptr;
-  size_t bytes = v.size() * sizeof(T) + 64;   // 64 zero bytes of slack past the end of every array
-  CK(cudaMalloc(&d, bytes));
-  CK(cudaMemset(d, 0, bytes));
-  if (!v.empty()) CK(cudaMemcpy(d, v.data(), v.size() * sizeof(T), cudaMemcpyHostToDevice));
-  pt.owned.push_back(d); pt.bytes += bytes;
-  *out = (const T*)d;
+int part_array(smr_ctx* ctx, Part& pt, size_t n, const void* src, T** out) {
+  const size_t bytes = n * sizeof(T);
+  DevBuf b;
+  CK(b.alloc(bytes + 64));
+  CK(cudaMemsetAsync(b.p, 0, bytes + 64, ctx->stream));
+  if (src && bytes) CK(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
+  *out = (T*)b.p;
+  pt.bytes += bytes + 64;
+  pt.owned.push_back(std::move(b));
   return SMR_OK;
 }
 
+// device scratch of one call: n items of T (at least one) in a new buffer of `pool`, freed with it
+template <class T>
+cudaError_t scratch(std::vector<DevBuf>& pool, size_t n, T** out) {
+  pool.emplace_back();
+  const cudaError_t e = pool.back().alloc(std::max<size_t>(n, 1) * sizeof(T));
+  *out = (T*)pool.back().p;
+  return e;
+}
+
+// one cub device call, run twice: with no scratch to size it, then in `tmp` (grown as needed).  call(void* tmp, size_t& bytes).
+template <class F>
+int cub_run(smr_ctx* ctx, DevBuf& tmp, F&& call) {
+  size_t bytes = 0;
+  CK(call(nullptr, bytes));
+  if (int rc = ensure(ctx, tmp, bytes)) return rc;
+  CK(call(tmp.p, bytes));
+  return SMR_OK;
+}
 
 // ---------------------------------------------------------------------------------------------------------------------
 // index build on the device (smr_build_dev.cuh): orchestration of one part
 // ---------------------------------------------------------------------------------------------------------------------
-struct TempPool {   // device scratch of one build, freed on return
-  std::vector<void*> v;
-  ~TempPool() { for (void* p : v) cudaFree(p); }
-  template <class T> cudaError_t get(T** out, size_t n) { void* p = nullptr; cudaError_t e = cudaMalloc(&p, std::max<size_t>(n, 1) * sizeof(T)); if (e == cudaSuccess) v.push_back(p); *out = (T*)p; return e; }
-};
 
 int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const std::vector<size_t>& members, const BuildOptions& opt, Part& pt) {
   BuildGeom g{};
@@ -187,88 +209,89 @@ int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const st
   }
   std::vector<uint32_t> roff(g.nseq + 1);
   for (uint32_t k = 0; k <= g.nseq; ++k) roff[k] = (uint32_t)soff[k];
-  TempPool tp;
+  std::vector<DevBuf> tmp;   // scratch of this build, freed on return
   cudaStream_t st = ctx->stream;
   const uint32_t n = g.nwin;
   const unsigned tb = 256, gw = (n + tb - 1) / tb;
+  int rc;
   uint8_t* d_codes; uint64_t* d_soff; uint32_t* d_wstart;
-  CK(tp.get(&d_codes, codes.size() + 64)); CK(tp.get(&d_soff, soff.size())); CK(tp.get(&d_wstart, wstart.size()));
+  CK(scratch(tmp, codes.size() + 64, &d_codes)); CK(scratch(tmp, soff.size(), &d_soff)); CK(scratch(tmp, wstart.size(), &d_wstart));
   CK(cudaMemcpyAsync(d_codes, codes.data(), codes.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_soff, soff.data(), soff.size() * 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_wstart, wstart.data(), wstart.size() * 4, cudaMemcpyHostToDevice, st));
   uint64_t *keyA, *keyB; uint32_t *valA, *valB, *u0, *u1, *u2, *u3, *win_id;
-  CK(tp.get(&keyA, n)); CK(tp.get(&keyB, n)); CK(tp.get(&valA, n)); CK(tp.get(&valB, n));
-  CK(tp.get(&u0, n)); CK(tp.get(&u1, n)); CK(tp.get(&u2, n)); CK(tp.get(&u3, n)); CK(tp.get(&win_id, n));
-  // cub scratch, sized for the largest call (entries: at most 2n)
+  CK(scratch(tmp, n, &keyA)); CK(scratch(tmp, n, &keyB)); CK(scratch(tmp, n, &valA)); CK(scratch(tmp, n, &valB));
+  CK(scratch(tmp, n, &u0)); CK(scratch(tmp, n, &u1)); CK(scratch(tmp, n, &u2)); CK(scratch(tmp, n, &u3)); CK(scratch(tmp, n, &win_id));
+  // cub scratch, sized exactly for the largest call (entries: at most 2n), so that cub_run never grows it
   size_t cub_bytes = 0, need = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, need, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, 2 * (size_t)n, 0, 64, st); cub_bytes = std::max(cub_bytes, need);
   cub::DeviceScan::InclusiveSum(nullptr, need, (uint32_t*)nullptr, (uint32_t*)nullptr, 2 * (size_t)n, st); cub_bytes = std::max(cub_bytes, need);
   cub::DeviceScan::InclusiveScan(nullptr, need, (uint32_t*)nullptr, (uint32_t*)nullptr, cuda::maximum<uint32_t>{}, 2 * (size_t)n, st); cub_bytes = std::max(cub_bytes, need);
-  uint8_t* d_cub; CK(tp.get(&d_cub, cub_bytes + 256));
+  DevBuf d_cub;
+  CK(d_cub.alloc(cub_bytes + 256));
   // 1. windows sorted by value (stable: equal values keep scan order)
   bld_windows_kernel<<<gw, tb, 0, st>>>(d_codes, d_soff, d_wstart, g, keyA, valA);
   CK(cudaGetLastError());
-  need = cub_bytes; CK(cub::DeviceRadixSort::SortPairs(d_cub, need, keyA, keyB, valA, valB, (size_t)n, 0, (int)(2 * g.pread), st));
+  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, keyA, keyB, valA, valB, (size_t)n, 0, (int)(2 * g.pread), st); }))) return rc;
   // 2. distinct (L+1)-mers, ids of the L-mers
   bld_heads_kernel<<<gw, tb, 0, st>>>(keyB, n, u0, u1);
   CK(cudaGetLastError());
-  need = cub_bytes; CK(cub::DeviceScan::InclusiveSum(d_cub, need, u0, u2, (size_t)n, st));
-  need = cub_bytes; CK(cub::DeviceScan::InclusiveSum(d_cub, need, u1, u3, (size_t)n, st));
+  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u0, u2, (size_t)n, st); }))) return rc;
+  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u1, u3, (size_t)n, st); }))) return rc;
   uint32_t nent = 0, nids = 0;
   CK(cudaMemcpyAsync(&nent, u2 + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(&nids, u3 + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   const uint32_t E = 2 * nent;
   uint32_t *e_list, *e_pref, *e_text, *e_id, *e_arr, *e_tpar; uint8_t* e_leaf;
-  CK(tp.get(&e_list, E)); CK(tp.get(&e_pref, E)); CK(tp.get(&e_text, E)); CK(tp.get(&e_id, E)); CK(tp.get(&e_arr, E)); CK(tp.get(&e_tpar, E)); CK(tp.get(&e_leaf, E));
+  CK(scratch(tmp, E, &e_list)); CK(scratch(tmp, E, &e_pref)); CK(scratch(tmp, E, &e_text)); CK(scratch(tmp, E, &e_id)); CK(scratch(tmp, E, &e_arr)); CK(scratch(tmp, E, &e_tpar)); CK(scratch(tmp, E, &e_leaf));
   CK(cudaMemsetAsync(e_tpar, 0, (size_t)E * 4, st)); CK(cudaMemsetAsync(e_leaf, 0, E, st));
   bld_entries_kernel<<<gw, tb, 0, st>>>(keyB, valB, u0, u2, u3, g, nent, win_id, e_list, e_pref, e_text, e_id, e_arr);
   CK(cudaGetLastError());
   // 3. positions (persistent arrays)
-  auto keep_alloc = [&](void** out, size_t bytes) -> cudaError_t { cudaError_t e = cudaMalloc(out, bytes + 64); if (e == cudaSuccess) { pt.owned.push_back(*out); pt.bytes += bytes + 64; e = cudaMemsetAsync(*out, 0, bytes + 64, st); } return e; };
   bld_poskeys_kernel<<<gw, tb, 0, st>>>(win_id, n, keyA);
   CK(cudaGetLastError());
-  need = cub_bytes; CK(cub::DeviceRadixSort::SortKeys(d_cub, need, keyA, keyB, (size_t)n, 0, 64, st));
+  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, keyA, keyB, (size_t)n, 0, 64, st); }))) return rc;
   bld_posflag_kernel<<<gw, tb, 0, st>>>(keyB, n, u0);
   CK(cudaGetLastError());
-  need = cub_bytes; CK(cub::DeviceScan::InclusiveScan(d_cub, need, u0, u1, cuda::maximum<uint32_t>{}, (size_t)n, st));
+  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveScan(t, b, u0, u1, cuda::maximum<uint32_t>{}, (size_t)n, st); }))) return rc;
   bld_poskeep_kernel<<<gw, tb, 0, st>>>(u1, n, g.max_pos, u2);
   CK(cudaGetLastError());
-  need = cub_bytes; CK(cub::DeviceScan::InclusiveSum(d_cub, need, u2, u3, (size_t)n, st));
+  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u2, u3, (size_t)n, st); }))) return rc;
   uint32_t npos = 0;
   CK(cudaMemcpyAsync(&npos, u3 + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  void *p_posoff = nullptr, *p_pos = nullptr, *p_ftext = nullptr, *p_fid = nullptr, *p_flookup = nullptr, *p_ref = nullptr, *p_roff = nullptr;
-  CK(keep_alloc(&p_posoff, ((size_t)nids + 1) * 4)); CK(keep_alloc(&p_pos, (size_t)npos * 8));
-  bld_poswrite_kernel<<<gw, tb, 0, st>>>(keyB, u1, u2, u3, d_wstart, g, nids, (uint32_t*)p_posoff, (uint2*)p_pos);
+  uint32_t *p_posoff, *p_ftext, *p_fid, *p_roff; uint2* p_pos; uint4* p_flookup; uint8_t* p_ref;
+  if ((rc = part_array(ctx, pt, (size_t)nids + 1, nullptr, &p_posoff)) || (rc = part_array(ctx, pt, npos, nullptr, &p_pos))) return rc;
+  bld_poswrite_kernel<<<gw, tb, 0, st>>>(keyB, u1, u2, u3, d_wstart, g, nids, p_posoff, p_pos);
   CK(cudaGetLastError());
   // 4. burst-trie order of the entries: first occurrence order, then one stable sort + one decision pass per level
   const unsigned ge = (E + tb - 1) / tb;
   uint64_t *ekA, *ekB; uint32_t *pA, *pB;
-  CK(tp.get(&ekA, E)); CK(tp.get(&ekB, E)); CK(tp.get(&pA, E)); CK(tp.get(&pB, E));
+  CK(scratch(tmp, E, &ekA)); CK(scratch(tmp, E, &ekB)); CK(scratch(tmp, E, &pA)); CK(scratch(tmp, E, &pB));
   bld_arrkey_kernel<<<ge, tb, 0, st>>>(e_arr, E, ekA, pA);
   CK(cudaGetLastError());
-  need = cub_bytes; CK(cub::DeviceRadixSort::SortPairs(d_cub, need, ekA, ekB, pA, pB, (size_t)E, 0, 32, st));
+  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, ekA, ekB, pA, pB, (size_t)E, 0, 32, st); }))) return rc;
   for (uint32_t d = 1; d <= g.burst_depth; ++d) {
     bld_levelkey_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_pref, e_leaf, E, d, g.burst_depth, ekA, pA);
     CK(cudaGetLastError());
-    need = cub_bytes; CK(cub::DeviceRadixSort::SortPairs(d_cub, need, ekA, ekB, pA, pB, (size_t)E, 0, (int)key_bits, st));
+    if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, ekA, ekB, pA, pB, (size_t)E, 0, (int)key_bits, st); }))) return rc;
     if (d < g.burst_depth) { bld_level_kernel<<<ge, tb, 0, st>>>(ekB, pB, E, d, e_arr, e_tpar, e_leaf); CK(cudaGetLastError()); }
   }
   // 5. the lists and their lookup rows
   const size_t nk = (size_t)1 << (2 * g.half);
-  CK(keep_alloc(&p_ftext, ftext_words(E) * 4)); CK(keep_alloc(&p_fid, (size_t)E * 4)); CK(keep_alloc(&p_flookup, nk * 16));
-  bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, (uint32_t*)p_ftext, (uint32_t*)p_fid, (uint32_t*)p_flookup, 0);
-  bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, (uint32_t*)p_ftext, (uint32_t*)p_fid, (uint32_t*)p_flookup, 1);
+  if ((rc = part_array(ctx, pt, ftext_words(E), nullptr, &p_ftext)) || (rc = part_array(ctx, pt, E, nullptr, &p_fid)) ||
+      (rc = part_array(ctx, pt, nk, nullptr, &p_flookup)))
+    return rc;
+  bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, p_ftext, p_fid, (uint32_t*)p_flookup, 0);
+  bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, p_ftext, p_fid, (uint32_t*)p_flookup, 1);
   CK(cudaGetLastError());
   // 6. references for the Smith-Waterman side
-  CK(keep_alloc(&p_ref, c04.size())); CK(keep_alloc(&p_roff, roff.size() * 4));
-  CK(cudaMemcpyAsync(p_ref, c04.data(), c04.size(), cudaMemcpyHostToDevice, st));
-  CK(cudaMemcpyAsync(p_roff, roff.data(), roff.size() * 4, cudaMemcpyHostToDevice, st));
+  if ((rc = part_array(ctx, pt, c04.size(), c04.data(), &p_ref)) || (rc = part_array(ctx, pt, roff.size(), roff.data(), &p_roff))) return rc;
   CK(cudaStreamSynchronize(st));
   pt.d.lnwin = g.L; pt.d.partialwin = g.half; pt.d.nref = g.nseq; pt.d.nids = nids;
-  pt.d.flookup = (const uint4*)p_flookup; pt.d.ftext = (const uint32_t*)p_ftext; pt.d.fid = (const uint32_t*)p_fid; pt.d.pos_off = (const uint32_t*)p_posoff; pt.d.pos = (const uint2*)p_pos;
-  pt.d.refseq = (const uint8_t*)p_ref; pt.d.ref_off = (const uint32_t*)p_roff;
+  pt.d.flookup = p_flookup; pt.d.ftext = p_ftext; pt.d.fid = p_fid; pt.d.pos_off = p_posoff; pt.d.pos = p_pos;
+  pt.d.refseq = p_ref; pt.d.ref_off = p_roff;
   pt.n_entries = E; pt.n_ids = nids; pt.n_pos = npos; pt.n_refseq = c04.size();
   return SMR_OK;
 }
@@ -362,7 +385,7 @@ int upload_batch_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
   CK(cudaEventRecord(e0, ctx->stream));
   std::vector<uint32_t>& off32 = ctx->off32; off32.resize(nreads + 1);
-  { int prc; if ((prc = ensure_pinned(ctx, ctx->h_pkoff, (size_t)(nreads + 1) * 4))) return prc; if ((prc = ensure_pinned(ctx, ctx->h_off32, (size_t)(nreads + 1) * 4))) return prc; }
+  { int prc; if ((prc = ensure(ctx, ctx->h_pkoff, (size_t)(nreads + 1) * 4))) return prc; if ((prc = ensure(ctx, ctx->h_off32, (size_t)(nreads + 1) * 4))) return prc; }
   uint32_t* pkoff = (uint32_t*)ctx->h_pkoff.p;
   uint32_t max_len = 0; uint64_t w = 0;
   for (uint32_t r = 0; r <= nreads; ++r) {
@@ -439,16 +462,58 @@ int finish_upload(smr_ctx* ctx, uint32_t nreads, uint64_t w) {
   return SMR_OK;
 }
 
-// exclusive scan of n u32 on the device (out may alias in); total (optional, device pointer) receives the sum
-int device_scan(smr_ctx* ctx, const uint32_t* in, uint32_t* out, uint64_t n, uint32_t* total_dev) {
-  const uint32_t ntiles = (uint32_t)((n + kScanTile - 1) / kScanTile);
+// exclusive sum of n u32 (out may equal in) in the context's cub scratch
+int exclusive_sum(smr_ctx* ctx, const uint32_t* in, uint32_t* out, uint32_t n) {
+  return cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, n, ctx->stream); });
+}
+
+struct TextLayout { uint32_t nlines = 0, nrec = 0, total_nt = 0; uint32_t fmt = kFmtFasta; };
+
+// The line layout of a FASTA / FASTQ text on the device (the line passes of smr_decode.cuh), for the decode and the report writer.
+// first_byte is text[0] and names the format.  Leaves, for each of the L.nlines lines, its newline position (d_nl), header flag
+// (d_hdr), sequence bytes (d_sb), record index (d_rec) and the offset of its sequence bytes (d_spos); the arrays hold nlines + 1
+// items, d_rec and d_spos the totals at [nlines].  d_scal is zeroed; its words from [4] on are the caller's.
+int text_layout(smr_ctx* ctx, const uint8_t* text, uint64_t nbytes, char first_byte, TextLayout& L) {
+  L = TextLayout{};
+  if (nbytes >= 0xF0000000ull) { ctx->err = "text batch of 2^32 bytes or more: split it (line counts and sequence offsets are 32-bit on the device)"; return SMR_ERR_ARG; }
+  if (nbytes && first_byte != '@' && first_byte != '>') { ctx->err = "reads text must start with '@' (FASTQ) or '>' (FASTA)"; return SMR_ERR_ARG; }
+  L.fmt = first_byte == '@' ? kFmtFastq : kFmtFasta;
   int rc;
-  if ((rc = ensure(ctx, ctx->scan_sums, (size_t)std::max<uint32_t>(ntiles, 1) * 4))) return rc;
-  if (ntiles == 0) { if (total_dev) CK(cudaMemsetAsync(total_dev, 0, 4, ctx->stream)); return SMR_OK; }
-  scan_tile_sums_kernel<<<ntiles, kScanThreads, 0, ctx->stream>>>(in, n, (uint32_t*)ctx->scan_sums.p);
-  scan_sums_kernel<<<1, 1024, 0, ctx->stream>>>((uint32_t*)ctx->scan_sums.p, ntiles, total_dev);
-  scan_apply_kernel<<<ntiles, kScanThreads, 0, ctx->stream>>>(in, n, (const uint32_t*)ctx->scan_sums.p, out);
-  CK(cudaGetLastError());
+  if ((rc = ensure(ctx, ctx->d_scal, 64))) return rc;
+  uint32_t* scal = (uint32_t*)ctx->d_scal.p;   // [1] records [2] sequence bytes [3] decode error
+  CK(cudaMemsetAsync(scal, 0, 64, ctx->stream));
+  // newlines: count per 32-byte chunk, scan (the total lands at [nchunks]), positions
+  const int grid = ctx->sm_count * 8;
+  const uint64_t nchunks = nbytes / 32 + 1;
+  if ((rc = ensure(ctx, ctx->d_cnt, (nchunks + 1) * 4))) return rc;
+  uint32_t* cnt = (uint32_t*)ctx->d_cnt.p;
+  count_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks);
+  CK(cudaMemsetAsync(cnt + nchunks, 0, 4, ctx->stream));
+  if ((rc = exclusive_sum(ctx, cnt, cnt, (uint32_t)nchunks + 1))) return rc;
+  CK(cudaMemcpyAsync(&L.nlines, cnt + nchunks, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  const uint32_t n = L.nlines;
+  if ((rc = ensure(ctx, ctx->d_nl, ((size_t)n + 1) * 8))) return rc;
+  if ((rc = ensure(ctx, ctx->d_hdr, ((size_t)n + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->d_sb, ((size_t)n + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->d_rec, ((size_t)n + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->d_spos, ((size_t)n + 1) * 4))) return rc;
+  if (n == 0) return SMR_OK;
+  uint32_t *hdr = (uint32_t*)ctx->d_hdr.p, *sb = (uint32_t*)ctx->d_sb.p, *rec = (uint32_t*)ctx->d_rec.p, *spos = (uint32_t*)ctx->d_spos.p;
+  write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks, (uint64_t*)ctx->d_nl.p);
+  // per line: header flag and sequence bytes; their scans give the record of every line and the offset of its bytes
+  line_info_kernel<<<grid, 256, 0, ctx->stream>>>(text, (const uint64_t*)ctx->d_nl.p, n, L.fmt, hdr, sb, scal + 3);
+  CK(cudaMemsetAsync(hdr + n, 0, 4, ctx->stream));
+  CK(cudaMemsetAsync(sb + n, 0, 4, ctx->stream));
+  if ((rc = exclusive_sum(ctx, hdr, rec, n + 1))) return rc;
+  if ((rc = exclusive_sum(ctx, sb, spos, n + 1))) return rc;
+  CK(cudaMemcpyAsync(scal + 1, rec + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(scal + 2, spos + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  uint32_t h[8];
+  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (h[3]) { ctx->err = h[3] & kDecBadHeader ? "reads text: a record does not start with its header character" : "reads text: FASTQ separator line '+' missing"; return SMR_ERR_ARG; }
+  L.nrec = h[1]; L.total_nt = h[2];
   return SMR_OK;
 }
 
@@ -459,10 +524,6 @@ int upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t*
   ctx->nreads = 0;
   ctx->text_bytes = nbytes;
   if (nbytes == 0) return SMR_OK;
-  if (nbytes >= 0xF0000000ull) { ctx->err = "text batch of 2^32 bytes or more: split it (line counts and sequence offsets are 32-bit on the device)"; return SMR_ERR_ARG; }
-  const char c0 = text ? text[0] : first_byte;
-  const uint32_t fmt = c0 == '@' ? kFmtFastq : kFmtFasta;
-  if (c0 != '@' && c0 != '>') { ctx->err = "reads text must start with '@' (FASTQ) or '>' (FASTA)"; return SMR_ERR_ARG; }
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
   int rc;
   CK(cudaEventRecord(e0, ctx->stream));
@@ -472,49 +533,31 @@ int upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t*
   }
   CK(cudaEventRecord(e1, ctx->stream));
   const uint8_t* dt = (const uint8_t*)ctx->d_text.p;
-  const uint64_t nchunks = nbytes / 32 + 1;
-  if ((rc = ensure(ctx, ctx->d_cnt, nchunks * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->d_scal, 64))) return rc;
-  uint32_t* scal = (uint32_t*)ctx->d_scal.p;   // [0] nlines [1] nrec [2] total nt [3] err [4] words [5] max_len
-  CK(cudaMemsetAsync(scal, 0, 64, ctx->stream));
-  const int grid = ctx->sm_count * 8;
-  count_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, nbytes, (uint32_t*)ctx->d_cnt.p, nchunks);
-  if ((rc = device_scan(ctx, (const uint32_t*)ctx->d_cnt.p, (uint32_t*)ctx->d_cnt.p, nchunks, scal + 0))) return rc;
-  uint32_t h[8];
-  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  const uint32_t nlines = h[0];
-  if (nlines == 0) return SMR_OK;
-  if ((rc = ensure(ctx, ctx->d_nl, (size_t)nlines * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->d_hdr, (size_t)nlines * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->d_sb, (size_t)nlines * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->d_rec, (size_t)nlines * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->d_spos, (size_t)nlines * 4))) return rc;
-  write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, nbytes, (const uint32_t*)ctx->d_cnt.p, nchunks, (uint64_t*)ctx->d_nl.p);
-  line_info_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)ctx->d_nl.p, nlines, fmt, (uint32_t*)ctx->d_hdr.p, (uint32_t*)ctx->d_sb.p, scal + 3);
-  if ((rc = device_scan(ctx, (const uint32_t*)ctx->d_hdr.p, (uint32_t*)ctx->d_rec.p, nlines, scal + 1))) return rc;
-  if ((rc = device_scan(ctx, (const uint32_t*)ctx->d_sb.p, (uint32_t*)ctx->d_spos.p, nlines, scal + 2))) return rc;
-  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  const uint32_t nreads = h[1], total = h[2], err = h[3];
-  if (err) { ctx->err = err & kDecBadHeader ? "reads text: a record does not start with its header character" : "reads text: FASTQ separator line '+' missing"; return SMR_ERR_ARG; }
+  TextLayout L;
+  if ((rc = text_layout(ctx, dt, nbytes, text ? text[0] : first_byte, L))) return rc;
+  const uint32_t nreads = L.nrec, total = L.total_nt;
   if (total >= 0xF0000000u) { ctx->err = "batch larger than 2^32 nucleotides: split it"; return SMR_ERR_ARG; }
   if (nreads == 0) return SMR_OK;
+  const int grid = ctx->sm_count * 8;
+  uint32_t* scal = (uint32_t*)ctx->d_scal.p;   // of text_layout; here [4] packed words [5] max_len
   if ((rc = ensure(ctx, ctx->seq04, (size_t)total + 64))) return rc;
   if ((rc = ensure(ctx, ctx->seq_off, (size_t)(nreads + 1) * 4))) return rc;
   if ((rc = ensure(ctx, ctx->pk_off, (size_t)(nreads + 1) * 4))) return rc;
   if ((rc = ensure(ctx, ctx->d_hdroff, (size_t)nreads * 8))) return rc;
-  scatter_lines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)ctx->d_nl.p, nlines, (const uint32_t*)ctx->d_hdr.p, (const uint32_t*)ctx->d_rec.p,
+  scatter_lines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)ctx->d_nl.p, L.nlines, (const uint32_t*)ctx->d_hdr.p, (const uint32_t*)ctx->d_rec.p,
                                                        (const uint32_t*)ctx->d_sb.p, (const uint32_t*)ctx->d_spos.p, (uint8_t*)ctx->seq04.p,
                                                        (uint32_t*)ctx->seq_off.p, (uint64_t*)ctx->d_hdroff.p);
   CK(cudaMemcpyAsync((uint32_t*)ctx->seq_off.p + nreads, scal + 2, 4, cudaMemcpyDeviceToDevice, ctx->stream));
-  // packed-word offsets and the longest read (what upload_batch_impl computes on the host)
+  // packed-word offsets and the longest read (what upload_batch_impl computes on the host); words[nreads] = 0, so pk_off[nreads] is the total
   if ((rc = ensure(ctx, ctx->d_cnt, (size_t)(nreads + 1) * 4))) return rc;
+  uint32_t* pk_off = (uint32_t*)ctx->pk_off.p;
   record_words_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->seq_off.p, nreads, (uint32_t*)ctx->d_cnt.p, scal + 5);
-  if ((rc = device_scan(ctx, (const uint32_t*)ctx->d_cnt.p, (uint32_t*)ctx->pk_off.p, (uint64_t)nreads + 1, scal + 4))) return rc;
+  if ((rc = exclusive_sum(ctx, (const uint32_t*)ctx->d_cnt.p, pk_off, nreads + 1))) return rc;
+  CK(cudaMemcpyAsync(scal + 4, pk_off + nreads, 4, cudaMemcpyDeviceToDevice, ctx->stream));
   ctx->off32.resize((size_t)nreads + 1);
-  if ((rc = ensure_pinned(ctx, ctx->h_off32, (size_t)(nreads + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, ctx->h_off32, (size_t)(nreads + 1) * 4))) return rc;
   CK(cudaMemcpyAsync(ctx->h_off32.p, ctx->seq_off.p, (size_t)(nreads + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  uint32_t h[8];
   CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(e2, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
@@ -830,15 +873,15 @@ int download_impl(smr_ctx* ctx, HostOut& out, std::vector<uint32_t>& flagged, co
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
   CK(cudaEventRecord(e0, ctx->stream));
   int prc;
-  if ((prc = ensure_pinned(ctx, ctx->h_state, (size_t)n * sizeof(ReadState)))) return prc;
-  if ((prc = ensure_pinned(ctx, ctx->h_flags, (size_t)n * 4))) return prc;
-  if ((prc = ensure_pinned(ctx, ctx->h_hitdb, (size_t)n * 2))) return prc;
-  if ((prc = ensure_pinned(ctx, ctx->h_outaln, (size_t)n * slots * sizeof(OutAln)))) return prc;
+  if ((prc = ensure(ctx, ctx->h_state, (size_t)n * sizeof(ReadState)))) return prc;
+  if ((prc = ensure(ctx, ctx->h_flags, (size_t)n * 4))) return prc;
+  if ((prc = ensure(ctx, ctx->h_hitdb, (size_t)n * 2))) return prc;
+  if ((prc = ensure(ctx, ctx->h_outaln, (size_t)n * slots * sizeof(OutAln)))) return prc;
   const ReadState* st = (const ReadState*)ctx->h_state.p; const uint32_t* fl = (const uint32_t*)ctx->h_flags.p;
   const uint16_t* hdb = (const uint16_t*)ctx->h_hitdb.p; const OutAln* oa = (const OutAln*)ctx->h_outaln.p;
   const AlnStats* ast = nullptr;
   if (ctx->host_stats) {
-    if ((prc = ensure_pinned(ctx, ctx->h_stats, (size_t)n * slots * sizeof(AlnStats)))) return prc;
+    if ((prc = ensure(ctx, ctx->h_stats, (size_t)n * slots * sizeof(AlnStats)))) return prc;
     ast = (const AlnStats*)ctx->h_stats.p;
     CK(cudaMemcpyAsync(ctx->h_stats.p, ctx->aln_stats.p, (size_t)n * slots * sizeof(AlnStats), cudaMemcpyDeviceToHost, ctx->stream));
   }
@@ -852,7 +895,7 @@ int download_impl(smr_ctx* ctx, HostOut& out, std::vector<uint32_t>& flagged, co
   CK(cudaMemcpyAsync(cnt.data(), ctx->counters.p, cnt.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   used = std::min<unsigned long long>(used, ctx->cigar_cap_dev);
-  if ((prc = ensure_pinned(ctx, ctx->h_cigar, (size_t)used * 4 + 16))) return prc;
+  if ((prc = ensure(ctx, ctx->h_cigar, (size_t)used * 4 + 16))) return prc;
   const uint32_t* cig = (const uint32_t*)ctx->h_cigar.p;
   if (used) CK(cudaMemcpyAsync(ctx->h_cigar.p, ctx->cigar_pool.p, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(e1, ctx->stream));
@@ -977,8 +1020,8 @@ int rpt_error(smr_ctx* ctx, uint32_t e) {
 }
 
 // The first half of smr_format_reports and smr_otu_add: text, results and groups on the device (e1 recorded after the copies), the
-// record layout of the text (the line passes of smr_decode.cuh, then rpt_records_kernel) and the fields of `a` that describe them.
-// The report error word is scal[4] of ctx->r_scal.
+// record layout of the text (text_layout, then rpt_records_kernel) and the fields of `a` that describe them.
+// The report error word is [4] of ctx->d_scal.
 int rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar,
                  uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads, const std::vector<RptGroup>& hg, cudaEvent_t e1, RptArgs& a) {
   const uint32_t slots = slots_of(ctx), G = (uint32_t)hg.size();
@@ -995,12 +1038,7 @@ int rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read
     dt = (const uint8_t*)ctx->d_text.p;
   }
   char c0 = 0;
-  if (nbytes) {
-    if (nbytes >= 0xF0000000ull) { ctx->err = "text batch of 2^32 bytes or more: split it"; return SMR_ERR_ARG; }
-    if (text) c0 = text[0]; else CK(cudaMemcpy(&c0, dt, 1, cudaMemcpyDeviceToHost));
-    if (c0 != '@' && c0 != '>') { ctx->err = "reads text must start with '@' (FASTQ) or '>' (FASTA)"; return SMR_ERR_ARG; }
-  }
-  const uint32_t fmt = c0 == '@' ? kFmtFastq : kFmtFasta;
+  if (nbytes) { if (text) c0 = text[0]; else CK(cudaMemcpy(&c0, dt, 1, cudaMemcpyDeviceToHost)); }
   // results
   if ((rc = upload_async(ctx, ctx->r_res, results, nreads))) return rc;
   if ((rc = upload_async(ctx, ctx->r_aln, alns, N))) return rc;
@@ -1008,48 +1046,21 @@ int rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read
   if ((rc = upload_async(ctx, ctx->r_st, stats, stats ? N : 0))) return rc;
   if ((rc = upload_async(ctx, ctx->r_grp, hg.data(), G))) return rc;
   CK(cudaEventRecord(e1, ctx->stream));
-  // record layout: the line passes of smr_decode.cuh
-  const int grid = ctx->sm_count * 8;
-  if ((rc = ensure(ctx, ctx->r_scal, 64))) return rc;
-  uint32_t* scal = (uint32_t*)ctx->r_scal.p;   // [0] nlines [1] nrec [2] total nt [3] decode err [4] report err
-  CK(cudaMemsetAsync(scal, 0, 64, ctx->stream));
-  const uint64_t nchunks = nbytes / 32 + 1;
-  if ((rc = ensure(ctx, ctx->d_cnt, nchunks * 4))) return rc;
-  count_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, nbytes, (uint32_t*)ctx->d_cnt.p, nchunks);
-  if ((rc = device_scan(ctx, (const uint32_t*)ctx->d_cnt.p, (uint32_t*)ctx->d_cnt.p, nchunks, scal + 0))) return rc;
-  uint32_t h[8];
-  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  const uint32_t nlines = nbytes ? h[0] : 0;
-  if ((rc = ensure(ctx, ctx->r_nl, ((size_t)nlines + 1) * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->r_hdr, ((size_t)nlines + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_sb, ((size_t)nlines + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_rec, ((size_t)nlines + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_spos, ((size_t)nlines + 1) * 4))) return rc;
-  uint32_t nrec = 0;
-  if (nlines) {
-    write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, nbytes, (const uint32_t*)ctx->d_cnt.p, nchunks, (uint64_t*)ctx->r_nl.p);
-    line_info_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)ctx->r_nl.p, nlines, fmt, (uint32_t*)ctx->r_hdr.p, (uint32_t*)ctx->r_sb.p, scal + 3);
-    if ((rc = device_scan(ctx, (const uint32_t*)ctx->r_hdr.p, (uint32_t*)ctx->r_rec.p, nlines, scal + 1))) return rc;
-    if ((rc = device_scan(ctx, (const uint32_t*)ctx->r_sb.p, (uint32_t*)ctx->r_spos.p, nlines, scal + 2))) return rc;
-    CK(cudaMemcpyAsync((uint32_t*)ctx->r_spos.p + nlines, scal + 2, 4, cudaMemcpyDeviceToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    if (h[3]) { ctx->err = h[3] & kDecBadHeader ? "reads text: a record does not start with its header character" : "reads text: FASTQ separator line '+' missing"; return SMR_ERR_ARG; }
-    nrec = h[1];
-  }
-  if (nrec != nreads) { ctx->err = "the text holds " + std::to_string(nrec) + " records, the results " + std::to_string(nreads) + " reads"; return SMR_ERR_ARG; }
+  TextLayout L;
+  if ((rc = text_layout(ctx, dt, nbytes, c0, L))) return rc;
+  if (L.nrec != nreads) { ctx->err = "the text holds " + std::to_string(L.nrec) + " records, the results " + std::to_string(nreads) + " reads"; return SMR_ERR_ARG; }
   // per record
   const uint64_t fstride = (uint64_t)nreads + 1;
   if ((rc = ensure(ctx, ctx->r_line, fstride * 4))) return rc;
   if ((rc = ensure(ctx, ctx->r_recs, fstride * sizeof(RptRec)))) return rc;
-  a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)ctx->r_nl.p; a.spos = (const uint32_t*)ctx->r_spos.p; a.nlines = nlines; a.fastq = fmt == kFmtFastq;
+  a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)ctx->d_nl.p; a.spos = (const uint32_t*)ctx->d_spos.p; a.nlines = L.nlines; a.fastq = L.fmt == kFmtFastq;
   a.rec = (const RptRec*)ctx->r_recs.p; a.nreads = nreads; a.slots = slots;
   a.res = (const smr_read_result*)ctx->r_res.p; a.aln = (const smr_aln*)ctx->r_aln.p; a.cigar = (const uint32_t*)ctx->r_cig.p;
   a.cigar_words = cigar ? cigar_words : 0; a.st = (const smr_aln_stats*)ctx->r_st.p;
-  a.grp = (const RptGroup*)ctx->r_grp.p; a.ngroups = G; a.err = scal + 4;
+  a.grp = (const RptGroup*)ctx->r_grp.p; a.ngroups = G; a.err = (uint32_t*)ctx->d_scal.p + 4;
   if (nreads) {
-    rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->r_hdr.p, (const uint32_t*)ctx->r_rec.p, nlines, (uint32_t*)ctx->r_line.p);
+    const int grid = ctx->sm_count * 8;
+    rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->d_hdr.p, (const uint32_t*)ctx->d_rec.p, L.nlines, (uint32_t*)ctx->r_line.p);
     rpt_records_kernel<<<grid, 256, 0, ctx->stream>>>(a, (const uint32_t*)ctx->r_line.p, (RptRec*)ctx->r_recs.p);
   }
   return SMR_OK;
@@ -1179,7 +1190,7 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   RptArgs a{};
   if ((rc = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e1, a))) return rc;
   const int grid = ctx->sm_count * 8;
-  uint32_t* scal = (uint32_t*)ctx->r_scal.p;
+  uint32_t* scal = (uint32_t*)ctx->d_scal.p;
   uint32_t h[8];
   // per record, routing, row order
   const uint64_t fstride = (uint64_t)nreads + 1;
@@ -1213,26 +1224,20 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
     rpt_row_keys_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, (uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_vals.p);
     int nbits = 1;
     while ((1u << nbits) <= G) ++nbits;
-    size_t tsort = 0, tscan = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, tsort, (const uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_keys2.p, (const uint32_t*)ctx->r_vals.p,
-                                       (uint32_t*)ctx->r_rows.p, (int)N, 0, nbits, ctx->stream));
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, tscan, sz, off, (int)std::max<uint64_t>(N + 1, 3 * fstride), ctx->stream));
-    size_t tbytes = std::max(tsort, tscan);
-    if ((rc = ensure(ctx, ctx->r_tmp, tbytes))) return rc;
-    CK(cub::DeviceRadixSort::SortPairs(ctx->r_tmp.p, tsort, (const uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_keys2.p, (const uint32_t*)ctx->r_vals.p,
-                                       (uint32_t*)ctx->r_rows.p, (int)N, 0, nbits, ctx->stream));
+    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) {
+           return cub::DeviceRadixSort::SortPairs(t, b, (const uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_keys2.p, (const uint32_t*)ctx->r_vals.p,
+                                                  (uint32_t*)ctx->r_rows.p, (int)N, 0, nbits, ctx->stream);
+         })))
+      return rc;
     rpt_group_first_kernel<<<(G + 128) / 128, 128, 0, ctx->stream>>>((const uint32_t*)ctx->r_keys2.p, N, G, first);
     if (o->sam) rpt_sam_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, sz);
     if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz, nullptr, nullptr);
     if (o->fastx || o->other || o->denovo) {
       rpt_fx_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, fxsz, fstride);
     }
-    tscan = tbytes;
-    CK(cub::DeviceScan::ExclusiveSum(ctx->r_tmp.p, tscan, sz, off, (int)(N + 1), ctx->stream));
-    tscan = tbytes;
-    CK(cub::DeviceScan::ExclusiveSum(ctx->r_tmp.p, tscan, bsz, boff, (int)(N + 1), ctx->stream));
-    tscan = tbytes;
-    CK(cub::DeviceScan::ExclusiveSum(ctx->r_tmp.p, tscan, fxsz, fxoff, (int)(3 * fstride), ctx->stream));
+    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, sz, off, (int)(N + 1), ctx->stream); }))) return rc;
+    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, bsz, boff, (int)(N + 1), ctx->stream); }))) return rc;
+    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fxsz, fxoff, (int)(3 * fstride), ctx->stream); }))) return rc;
   } else {
     CK(cudaMemsetAsync(off, 0, 8, ctx->stream));
     CK(cudaMemsetAsync(boff, 0, 8, ctx->stream));
@@ -1280,16 +1285,13 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
 // device buffer grown to at least `need` bytes by doubling, keeping its first `used` bytes
 int grow_keep(smr_ctx* ctx, DevBuf& b, size_t used, size_t need) {
   if (need <= b.cap && b.p) return SMR_OK;
-  const size_t want = std::max<size_t>({need, 2 * b.cap, 4096});
-  void* p = nullptr;
-  CK(cudaMalloc(&p, want));
+  DevBuf nb;
+  CK(nb.alloc(std::max<size_t>({need, 2 * b.cap, 4096})));
   if (used) {
-    const cudaError_t e = cudaMemcpyAsync(p, b.p, used, cudaMemcpyDeviceToDevice, ctx->stream);
-    if (e != cudaSuccess) { cudaFree(p); ctx->err = std::string("cudaMemcpyAsync: ") + cudaGetErrorString(e); return SMR_ERR_CUDA; }
+    CK(cudaMemcpyAsync(nb.p, b.p, used, cudaMemcpyDeviceToDevice, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
-  release(b);
-  b.p = p; b.cap = want;
+  b = std::move(nb);   // nb frees the old buffer
   return SMR_OK;
 }
 
@@ -1377,17 +1379,13 @@ int otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read
   CK(cudaMemsetAsync(flag + N, 0, 4, ctx->stream));
   CK(cudaMemsetAsync(nsz + N, 0, 8, ctx->stream));
   otu_flag_kernel<<<grid, 256, 0, ctx->stream>>>(a, oa, flag, nsz);
-  size_t t1 = 0, t2 = 0;
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, t1, flag, pos, (int)(N + 1), ctx->stream));
-  CK(cub::DeviceScan::ExclusiveSum(nullptr, t2, nsz, noff, (int)(N + 1), ctx->stream));
-  if ((rc = ensure(ctx, U.tmp, std::max(t1, t2)))) return rc;
-  CK(cub::DeviceScan::ExclusiveSum(U.tmp.p, t1, flag, pos, (int)(N + 1), ctx->stream));
-  CK(cub::DeviceScan::ExclusiveSum(U.tmp.p, t2, nsz, noff, (int)(N + 1), ctx->stream));
+  if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, flag, pos, (int)(N + 1), ctx->stream); }))) return rc;
+  if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, nsz, noff, (int)(N + 1), ctx->stream); }))) return rc;
   CK(cudaGetLastError());
   uint32_t m = 0, err = 0; uint64_t bytes = 0;
   CK(cudaMemcpyAsync(&m, pos + N, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(&bytes, noff + N, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(&err, (uint32_t*)ctx->r_scal.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&err, (uint32_t*)ctx->d_scal.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   if (err) return rpt_error(ctx, err);
   if (U.n + m >= (1ull << 31)) { ctx->err = "OTU map of 2^31 entries or more"; return SMR_ERR_CAPACITY; }
@@ -1425,15 +1423,14 @@ int otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) {
     uint64_t *skey = (uint64_t*)U.skey.p, *size = (uint64_t*)U.size.p, *off = (uint64_t*)U.off.p;
     uint32_t *sidx = (uint32_t*)U.sidx.p, *scal = (uint32_t*)U.scal.p;
     otu_iota_kernel<<<grid, 256, 0, ctx->stream>>>((uint32_t*)U.vals.p, m);
-    size_t t1 = 0, t2 = 0;
-    CK(cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint64_t*)U.key.p, skey, (const uint32_t*)U.vals.p, sidx, (int)m, 0, (int)U.kbits, ctx->stream));
-    CK(cub::DeviceScan::ExclusiveSum(nullptr, t2, size, off, (int)(m + 1), ctx->stream));
-    if ((rc = ensure(ctx, U.tmp, std::max(t1, t2)))) return rc;
-    CK(cub::DeviceRadixSort::SortPairs(U.tmp.p, t1, (const uint64_t*)U.key.p, skey, (const uint32_t*)U.vals.p, sidx, (int)m, 0, (int)U.kbits, ctx->stream));
+    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) {
+           return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)U.key.p, skey, (const uint32_t*)U.vals.p, sidx, (int)m, 0, (int)U.kbits, ctx->stream);
+         })))
+      return rc;
     CK(cudaMemsetAsync(scal, 0, 16, ctx->stream));
     CK(cudaMemsetAsync(size + m, 0, 8, ctx->stream));
     otu_size_kernel<<<grid, 256, 0, ctx->stream>>>(skey, sidx, (const OtuEnt*)U.ent.p, m, U.gbits, (const RptGroup*)U.grp.p, size, scal);
-    CK(cub::DeviceScan::ExclusiveSum(U.tmp.p, t2, size, off, (int)(m + 1), ctx->stream));
+    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, size, off, (int)(m + 1), ctx->stream); }))) return rc;
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(&bytes, off + m, 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(&runs, scal, 4, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1494,29 +1491,9 @@ int smr_init(int device, smr_ctx** out) {
 void smr_destroy(smr_ctx* ctx) {
   if (!ctx) return;
   cudaSetDevice(ctx->device);
-  for (auto& pt : ctx->parts) for (void* p : pt.owned) cudaFree(p);
-  DevBuf* bufs[] = {&ctx->seq04, &ctx->seq_off, &ctx->pk03, &ctx->pk03alt, &ctx->pk_off, &ctx->has_n, &ctx->hit_cnt, &ctx->flags, &ctx->state,
-                    &ctx->hit_db, &ctx->aln_work, &ctx->out_aln, &ctx->hits, &ctx->cost, &ctx->bins, &ctx->scalars, &ctx->counters, &ctx->cigar_pool,
-                    &ctx->parts_dev, &ctx->lis_arena, &ctx->lis_epochs, &ctx->lis_queue, &ctx->lis_done, &ctx->lis_rows, &ctx->lis_dbg, &ctx->final_arena, &ctx->lane_hits, &ctx->tb_arena, &ctx->tb_jobs, &ctx->fin_list, &ctx->aln_stats,
-                    &ctx->d_text, &ctx->d_cnt, &ctx->d_scal, &ctx->d_nl, &ctx->d_hdr, &ctx->d_sb, &ctx->d_rec, &ctx->d_spos, &ctx->d_hdroff, &ctx->scan_sums,
-                    &ctx->d_gz, &ctx->d_cand, &ctx->d_res, &ctx->d_sym, &ctx->d_win, &ctx->d_ids, &ctx->d_off, &ctx->d_cnt64,
-                    &ctx->d_moff, &ctx->d_mem, &ctx->d_poff, &ctx->d_plen, &ctx->d_pcrc, &ctx->seed_ctr,
-                    &ctx->r_text, &ctx->r_nl, &ctx->r_hdr, &ctx->r_sb, &ctx->r_rec, &ctx->r_spos, &ctx->r_line, &ctx->r_recs, &ctx->r_res, &ctx->r_aln,
-                    &ctx->r_cig, &ctx->r_st, &ctx->r_flags, &ctx->r_keys, &ctx->r_keys2, &ctx->r_vals, &ctx->r_rows, &ctx->r_first, &ctx->r_sz, &ctx->r_off,
-                    &ctx->r_bsz, &ctx->r_boff, &ctx->r_fxsz, &ctx->r_fxoff, &ctx->r_grp, &ctx->r_so, &ctx->r_tmp, &ctx->r_out, &ctx->r_scal,
-                    &ctx->z_in, &ctx->z_chunk, &ctx->z_m, &ctx->z_freq, &ctx->z_codes, &ctx->z_hdr, &ctx->z_info, &ctx->z_scratch, &ctx->z_poff,
-                    &ctx->z_plen, &ctx->z_crc, &ctx->z_dst, &ctx->z_trl, &ctx->z_out};
-  for (DevBuf* b : bufs) release(*b);
-  for (auto& sc : ctx->rpt_score) { release(sc.ev); release(sc.bits); }
-  DevBuf* obufs[] = {&ctx->otu.rank, &ctx->otu.rank_off, &ctx->otu.grp, &ctx->otu.key, &ctx->otu.ent, &ctx->otu.pool, &ctx->otu.flag, &ctx->otu.pos,
-                     &ctx->otu.nsz, &ctx->otu.noff, &ctx->otu.vals, &ctx->otu.skey, &ctx->otu.sidx, &ctx->otu.size, &ctx->otu.off, &ctx->otu.out,
-                     &ctx->otu.tmp, &ctx->otu.scal};
-  for (DevBuf* b : obufs) release(*b);
-  PinBuf* pins[] = {&ctx->h_state, &ctx->h_flags, &ctx->h_hitdb, &ctx->h_outaln, &ctx->h_stats, &ctx->h_cigar, &ctx->h_off32, &ctx->h_pkoff};
-  for (PinBuf* b : pins) release(*b);
   for (cudaEvent_t e : ctx->ev) cudaEventDestroy(e);
   if (ctx->stream) cudaStreamDestroy(ctx->stream);
-  delete ctx;
+  delete ctx;   // the buffers free themselves
 }
 
 const char* smr_last_error(const smr_ctx* ctx) { return ctx ? ctx->err.c_str() : "null context"; }
@@ -1550,13 +1527,14 @@ int smr_load_index_part(smr_ctx* ctx, uint32_t index_num, uint32_t part, const v
   int rc;
   const uint32_t *lk = nullptr, *ft = nullptr, *fi = nullptr, *po = nullptr; const SeqPos* ps = nullptr;
   const uint8_t* rs = nullptr; const uint32_t* ro = nullptr;
-  if ((rc = upload_vec(ctx, pt, fx.flookup, &lk))) return rc;
-  if ((rc = upload_vec(ctx, pt, ftext, &ft))) return rc;
-  if ((rc = upload_vec(ctx, pt, fid, &fi))) return rc;
-  if ((rc = upload_vec(ctx, pt, fx.pos_off, &po))) return rc;
-  if ((rc = upload_vec(ctx, pt, fx.pos, &ps))) return rc;
-  if ((rc = upload_vec(ctx, pt, rseq, &rs))) return rc;
-  if ((rc = upload_vec(ctx, pt, roff, &ro))) return rc;
+  if ((rc = part_array(ctx, pt, fx.flookup.size(), fx.flookup.data(), &lk))) return rc;
+  if ((rc = part_array(ctx, pt, ftext.size(), ftext.data(), &ft))) return rc;
+  if ((rc = part_array(ctx, pt, fid.size(), fid.data(), &fi))) return rc;
+  if ((rc = part_array(ctx, pt, fx.pos_off.size(), fx.pos_off.data(), &po))) return rc;
+  if ((rc = part_array(ctx, pt, fx.pos.size(), fx.pos.data(), &ps))) return rc;
+  if ((rc = part_array(ctx, pt, rseq.size(), rseq.data(), &rs))) return rc;
+  if ((rc = part_array(ctx, pt, roff.size(), roff.data(), &ro))) return rc;
+  CK(cudaStreamSynchronize(ctx->stream));
   pt.d.flookup = (const uint4*)lk; pt.d.ftext = ft; pt.d.fid = fi; pt.d.pos_off = po; pt.d.pos = (const uint2*)ps;
   pt.d.refseq = rs; pt.d.ref_off = ro;
   pt.n_refseq = rseq.size();
@@ -1592,8 +1570,7 @@ int smr_build_index_device(smr_ctx* ctx, uint32_t index_num, const char* fasta_p
     if (!e.empty()) { ctx->err = e; return SMR_ERR_INDEX; }
     if (members.empty()) break;
     Part pt;
-    int rc = build_part_device(ctx, recs, members, opt, pt);
-    if (rc) { for (void* p : pt.owned) cudaFree(p); return rc; }
+    if (int rc = build_part_device(ctx, recs, members, opt, pt)) return rc;
     pt.d.index_num = index_num; pt.d.part = part; pt.d.minimal_score = minimal_score;
     for (int i = 0; i < 3; ++i) pt.d.skip[i] = skiplengths[i];
     rep[3] += pt.n_ids; rep[5] += pt.bytes;
@@ -1817,8 +1794,9 @@ int smr_set_report_refs(smr_ctx* ctx, uint32_t index_num, uint32_t part, const c
     std::vector<char> names(names_cat, names_cat + name_off[nref]);
     std::vector<uint64_t> off(name_off, name_off + nref + 1);
     int rc;
-    if ((rc = upload_vec(ctx, pt, names, &pt.rnames))) return rc;
-    if ((rc = upload_vec(ctx, pt, off, &pt.rname_off))) return rc;
+    if ((rc = part_array(ctx, pt, names.size(), names.data(), &pt.rnames))) return rc;
+    if ((rc = part_array(ctx, pt, off.size(), off.data(), &pt.rname_off))) return rc;
+    CK(cudaStreamSynchronize(ctx->stream));
     pt.n_rnames = nref; pt.has_rnames = true;
     pt.h_rnames.resize(nref);
     for (uint32_t k = 0; k < nref; ++k) if (name_off[k + 1] > name_off[k]) pt.h_rnames[k].assign(names_cat + name_off[k], name_off[k + 1] - name_off[k]);
@@ -1911,14 +1889,14 @@ int smr_last_timings(const smr_ctx* ctx, double out[8]) {
 int smr_debug_dpx_peak(smr_ctx* ctx, double* giga_ops_per_s) {
   if (!ctx || !giga_ops_per_s) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  int32_t* d = nullptr;
-  CK(cudaMalloc(&d, 64));
+  DevBuf d;
+  CK(d.alloc(64));
   const int iters = 1 << 14, ctas = ctx->sm_count * 8, thr = 256;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
   double best = 0;
   for (int rep = 0; rep < 4; ++rep) {
     CK(cudaEventRecord(e0, ctx->stream));
-    dpx_peak_kernel<<<ctas, thr, 0, ctx->stream>>>(d, iters, -2, -1000000);
+    dpx_peak_kernel<<<ctas, thr, 0, ctx->stream>>>((int32_t*)d.p, iters, -2, -1000000);
     CK(cudaGetLastError());
     CK(cudaEventRecord(e1, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1926,7 +1904,6 @@ int smr_debug_dpx_peak(smr_ctx* ctx, double* giga_ops_per_s) {
     const double ops = (double)ctas * thr * iters * 8.0;
     if (rep > 0) best = std::max(best, ops / (ms * 1e-3) / 1e9);
   }
-  cudaFree(d);
   *giga_ops_per_s = best;
   return SMR_OK;
 }
@@ -1941,10 +1918,11 @@ int smr_debug_seed_windows(smr_ctx* ctx, uint32_t part_slot, const uint8_t* seq_
   const uint64_t total = seq_off[nreads] - seq_off[0];
   std::vector<uint32_t> off32(nreads + 1);
   for (uint32_t r = 0; r <= nreads; ++r) off32[r] = (uint32_t)(seq_off[r] - seq_off[0]);
-  uint8_t *d_seq = nullptr, *d_zero = nullptr; uint32_t *d_off = nullptr, *d_wr = nullptr, *d_wp = nullptr, *d_ids = nullptr, *d_cnt = nullptr;
-  CK(cudaMalloc(&d_seq, total + 64)); CK(cudaMalloc(&d_off, (size_t)(nreads + 1) * 4)); CK(cudaMalloc(&d_wr, (size_t)nwin * 4 + 4));
-  CK(cudaMalloc(&d_wp, (size_t)nwin * 4 + 4)); CK(cudaMalloc(&d_ids, (size_t)nwin * cap * 4 + 4)); CK(cudaMalloc(&d_cnt, (size_t)nwin * 4 + 4));
-  CK(cudaMalloc(&d_zero, nwin + 4));
+  std::vector<DevBuf> tmp;
+  uint8_t *d_seq, *d_zero; uint32_t *d_off, *d_wr, *d_wp, *d_ids, *d_cnt;
+  CK(scratch(tmp, total + 64, &d_seq)); CK(scratch(tmp, (size_t)nreads + 1, &d_off)); CK(scratch(tmp, (size_t)nwin + 1, &d_wr));
+  CK(scratch(tmp, (size_t)nwin + 1, &d_wp)); CK(scratch(tmp, (size_t)nwin * cap + 1, &d_ids)); CK(scratch(tmp, (size_t)nwin + 1, &d_cnt));
+  CK(scratch(tmp, (size_t)nwin + 4, &d_zero));
   CK(cudaMemcpy(d_seq, seq_cat + seq_off[0], total, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(d_off, off32.data(), (size_t)(nreads + 1) * 4, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(d_wr, win_read, (size_t)nwin * 4, cudaMemcpyHostToDevice));
@@ -1959,7 +1937,6 @@ int smr_debug_seed_windows(smr_ctx* ctx, uint32_t part_slot, const uint8_t* seq_
   CK(cudaMemcpy(ids, d_ids, (size_t)nwin * cap * 4, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(counts, d_cnt, (size_t)nwin * 4, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(zero, d_zero, nwin, cudaMemcpyDeviceToHost));
-  cudaFree(d_seq); cudaFree(d_off); cudaFree(d_wr); cudaFree(d_wp); cudaFree(d_ids); cudaFree(d_cnt); cudaFree(d_zero);
   return SMR_OK;
 }
 
@@ -1972,14 +1949,15 @@ int smr_debug_ssw(smr_ctx* ctx, const uint8_t* q_cat, const uint64_t* q_off, con
   uint32_t maxlen = 0;
   for (uint32_t i = 0; i <= npairs; ++i) { qo[i] = (uint32_t)(q_off[i] - q_off[0]); to[i] = (uint32_t)(t_off[i] - t_off[0]); }
   for (uint32_t i = 0; i < npairs; ++i) maxlen = std::max(maxlen, std::max(qo[i + 1] - qo[i], to[i + 1] - to[i]));
-  uint8_t *dq = nullptr, *dt = nullptr, *arena = nullptr; uint32_t *dqo = nullptr, *dto = nullptr, *dc = nullptr; int32_t* dout = nullptr;
+  std::vector<DevBuf> tmp;
+  uint8_t *dq, *dt, *arena; uint32_t *dqo, *dto, *dc; int32_t* dout;
   FinalGlobals g{};
   g.cap_w = 2 * 2048 + 8; g.cap_cig = 2 * (maxlen + 64) + 16; g.row_cap = maxlen + 128; g.cap_dir = (size_t)(2 * 64 + 1) * (maxlen + 8) * 3 + 65536;
   const uint32_t nwarps = 512;
   g.arena_stride = final_arena_bytes(g.cap_w, g.cap_cig, g.row_cap, g.cap_dir);
-  CK(cudaMalloc(&arena, g.arena_stride * nwarps)); g.arena_base = arena;
-  CK(cudaMalloc(&dq, qt + 64)); CK(cudaMalloc(&dt, tt + 64)); CK(cudaMalloc(&dqo, (size_t)(npairs + 1) * 4)); CK(cudaMalloc(&dto, (size_t)(npairs + 1) * 4));
-  CK(cudaMalloc(&dc, (size_t)npairs * cigar_cap * 4 + 4)); CK(cudaMalloc(&dout, (size_t)npairs * 6 * 4 + 4));
+  CK(scratch(tmp, g.arena_stride * nwarps, &arena)); g.arena_base = arena;
+  CK(scratch(tmp, qt + 64, &dq)); CK(scratch(tmp, tt + 64, &dt)); CK(scratch(tmp, (size_t)npairs + 1, &dqo)); CK(scratch(tmp, (size_t)npairs + 1, &dto));
+  CK(scratch(tmp, (size_t)npairs * cigar_cap + 1, &dc)); CK(scratch(tmp, (size_t)npairs * 6 + 1, &dout));
   CK(cudaMemcpy(dq, q_cat + q_off[0], qt, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dt, t_cat + t_off[0], tt, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(dqo, qo.data(), (size_t)(npairs + 1) * 4, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dto, to.data(), (size_t)(npairs + 1) * 4, cudaMemcpyHostToDevice));
   CK(cudaMemset(dc, 0, (size_t)npairs * cigar_cap * 4));
@@ -1989,7 +1967,6 @@ int smr_debug_ssw(smr_ctx* ctx, const uint8_t* q_cat, const uint64_t* q_off, con
   CK(cudaStreamSynchronize(ctx->stream));
   CK(cudaMemcpy(out, dout, (size_t)npairs * 6 * 4, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(cigars, dc, (size_t)npairs * cigar_cap * 4, cudaMemcpyDeviceToHost));
-  cudaFree(dq); cudaFree(dt); cudaFree(dqo); cudaFree(dto); cudaFree(dc); cudaFree(dout); cudaFree(arena);
   return SMR_OK;
 }
 

@@ -4,80 +4,16 @@
 // lines up to the next header), Read::Read(readstr) (read.cpp:141-176) and the alphabet of Read::init / seqToIntStr via
 // nt_table (include/common.hpp:68-77: ACGTU in either case -> 0..3, everything else 4).
 //
-// All passes are streaming and HBM-bound: (1) newline count per 32-byte chunk, (2) exclusive scan, (3) newline positions,
-// (4) per line: header flag + sequence bytes, (5) two scans over the lines give the record index of every line and the
-// offset of every sequence line in the concatenated read buffer, (6) one warp per sequence line encodes its bytes.
+// All passes are streaming and HBM-bound: (1) newline count per 32-byte chunk, (3) newline positions, (4) per line: header flag +
+// sequence bytes, (6) one warp per sequence line encodes its bytes.  The host (text_layout in smr_capi.cu) runs the scans between
+// them with cub: (2) over the chunk counts, (5) over the lines, giving the record index of every line and the offset of every
+// sequence line in the concatenated read buffer.
 #pragma once
 #include <cstdint>
 
 #include "smr_dev.cuh"
 
 namespace smr {
-
-constexpr int kScanItems = 4;        // items per thread
-constexpr int kScanThreads = 256;
-constexpr int kScanTile = kScanItems * kScanThreads;
-
-// ---- exclusive scan of u32 (n up to 2^32-1 items, totals < 2^32): tile sums, scan of the sums, tile-local scan + base ----
-__global__ void __launch_bounds__(kScanThreads) scan_tile_sums_kernel(const uint32_t* __restrict__ in, uint64_t n, uint32_t* __restrict__ sums) {
-  __shared__ uint32_t s_w[kScanThreads / 32];
-  const uint64_t base = (uint64_t)blockIdx.x * kScanTile + (uint64_t)threadIdx.x * kScanItems;
-  uint32_t v = 0;
-#pragma unroll
-  for (int k = 0; k < kScanItems; ++k) if (base + k < n) v += in[base + k];
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(kFull, v, o);
-  if ((threadIdx.x & 31) == 0) s_w[threadIdx.x >> 5] = v;
-  __syncthreads();
-  if (threadIdx.x == 0) { uint32_t t = 0; for (int w = 0; w < kScanThreads / 32; ++w) t += s_w[w]; sums[blockIdx.x] = t; }
-}
-// one block: exclusive scan of `sums` in place (ntiles arbitrary), total written to *total
-__global__ void __launch_bounds__(1024) scan_sums_kernel(uint32_t* __restrict__ sums, uint32_t ntiles, uint32_t* __restrict__ total) {
-  __shared__ uint32_t s_w[32];
-  __shared__ uint32_t s_carry;
-  if (threadIdx.x == 0) s_carry = 0;
-  __syncthreads();
-  for (uint32_t b0 = 0; b0 < ntiles; b0 += 1024) {
-    const uint32_t i = b0 + threadIdx.x;
-    const uint32_t v = i < ntiles ? sums[i] : 0u;
-    uint32_t incl = v;
-#pragma unroll
-    for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(kFull, incl, o); if ((threadIdx.x & 31) >= (unsigned)o) incl += t; }
-    if ((threadIdx.x & 31) == 31) s_w[threadIdx.x >> 5] = incl;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-      uint32_t w = s_w[threadIdx.x], wi = w;
-#pragma unroll
-      for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(kFull, wi, o); if (threadIdx.x >= (unsigned)o) wi += t; }
-      s_w[threadIdx.x] = wi - w;   // exclusive prefix of the warp totals
-    }
-    __syncthreads();
-    const uint32_t carry = s_carry;
-    if (i < ntiles) sums[i] = carry + s_w[threadIdx.x >> 5] + incl - v;
-    __syncthreads();
-    if (threadIdx.x == 1023) s_carry = carry + s_w[31] + incl;
-    __syncthreads();
-  }
-  if (threadIdx.x == 0 && total) *total = s_carry;
-}
-__global__ void __launch_bounds__(kScanThreads) scan_apply_kernel(const uint32_t* __restrict__ in, uint64_t n, const uint32_t* __restrict__ sums,
-                                                                   uint32_t* __restrict__ out) {
-  __shared__ uint32_t s_w[kScanThreads / 32];
-  const uint64_t base = (uint64_t)blockIdx.x * kScanTile + (uint64_t)threadIdx.x * kScanItems;
-  uint32_t x[kScanItems], v = 0;
-#pragma unroll
-  for (int k = 0; k < kScanItems; ++k) { x[k] = base + k < n ? in[base + k] : 0u; v += x[k]; }
-  uint32_t incl = v;
-#pragma unroll
-  for (int o = 1; o < 32; o <<= 1) { const uint32_t t = __shfl_up_sync(kFull, incl, o); if ((threadIdx.x & 31) >= (unsigned)o) incl += t; }
-  if ((threadIdx.x & 31) == 31) s_w[threadIdx.x >> 5] = incl;
-  __syncthreads();
-  uint32_t wbase = 0;
-  for (unsigned w = 0; w < (threadIdx.x >> 5); ++w) wbase += s_w[w];
-  uint32_t run = sums[blockIdx.x] + wbase + incl - v;
-#pragma unroll
-  for (int k = 0; k < kScanItems; ++k) { if (base + k < n) out[base + k] = run; run += x[k]; }
-}
 
 // ---- (1) newlines per 32-byte chunk; a text that does not end in '\n' gets a virtual one at position n ----
 __global__ void count_newlines_kernel(const uint8_t* __restrict__ text, uint64_t n, uint32_t* __restrict__ counts, uint64_t nchunks) {
