@@ -16,7 +16,7 @@
 //   * ssw_align's reverse pass and CIGAR are deferred to the finalize kernel: accept / replace / stop
 //     decisions only need score1 (:388-469).
 //
-// Warp specialisation.  One persistent CTA of 32 warps per SM; its warps have three roles (16 scorers, 1 fetcher, 15 planners):
+// Warp specialisation.  One persistent CTA of 32 warps per SM; its warps have three roles (12 scorers, 1 fetcher, 19 planners):
 //   * PLANNER warps own reads.  For each compute_lis_alignment call they vote, order and group as above, then walk the
 //     candidates in the reference's order WITHOUT scoring: every (candidate, sliding-window step) that would reach
 //     ssw_align becomes a task record (window, query segment).  Which steps reach it is score-independent -- the
@@ -42,14 +42,19 @@
 
 namespace smr {
 
-// One CTA of 32 warps per SM: 16 scorers + 1 fetcher (one lane per scorer slot) + 15 planners.  (Two CTAs of 8 + 1 + 7 need two
-// fetcher warps per SM, i.e. one planner fewer, and were slower, as was 14 + 1 + 17.  The split and the other tuning constants of
-// this file were chosen by A/B runs of the candidate kernel during development and have not been re-tuned on the H100.)
+// One CTA of 32 warps per SM: 12 scorers + 1 fetcher (one lane per scorer slot) + 19 planners.  The split trades two regimes.
+// bench.py's reads make ~3 Smith-Waterman calls each, and there the planners bound the kernel: 16 scorers waited for work 66 % of
+// their cycles.  Reads from conserved regions make dozens of calls, and there the scorers bound it.  Candidate-kernel time per
+// step on an H100 80GB HBM3 at 700 W (1980 MHz), bench.py with 0.5 M reads per step / tools/bench_heavy.py (430 k cells per read):
+// 16 + 1 + 15: 44.9 / 40.5 ms; 12 + 1 + 19: 38.7 / 42.5; 10 + 1 + 21: 37.7 / 45.2; 8 + 1 + 23: 38.4 / 49.1; 6 + 1 + 25: 41.4 / -;
+// 4 + 1 + 27: 45.0 / -.  12 + 1 + 19 takes most of the gain on the first at +5 % on the second.  (Two CTAs of 8 + 1 + 7 need two
+// fetcher warps per SM, i.e. one planner fewer, and were slower.  The other tuning constants of this file were chosen by A/B runs
+// during development and have not been re-tuned on the H100.)
 #ifndef SMR_SCORER_WARPS
-#define SMR_SCORER_WARPS 16
+#define SMR_SCORER_WARPS 12
 #endif
 #ifndef SMR_PLANNER_WARPS
-#define SMR_PLANNER_WARPS 15
+#define SMR_PLANNER_WARPS 19
 #endif
 #ifndef SMR_LIS_MIN_CTAS
 #define SMR_LIS_MIN_CTAS 1
