@@ -74,13 +74,11 @@ final_jobs_kernel(DevBatch b, FinalGlobals g) {
   }
 }
 
-// Per warp shared memory of the finalize kernels: the packed locate's two query profiles and two windows; the s32 locate (shapes
-// outside the packed kernel) uses the first window as its staged window and the profile words as its own profile.
+// Per warp shared memory of the finalize kernels: the packed passes' two query profiles and two windows.
 struct FinalSmem {
   uint32_t prof[2 * kPairProfWords];
   __align__(16) uint8_t win[2][kPairWinBytes];
 };
-static_assert(2 * kPairProfWords == kProfWords && kPairWinBytes >= kRefStage + 64, "the s32 locate's staging must fit the packed locate's");
 
 __device__ __forceinline__ TraceArena final_arena(const FinalGlobals& g, const uint32_t warp, int32_t*& rowH, int32_t*& rowF) {
   uint8_t* p = g.arena_base + (size_t)warp * g.arena_stride;
@@ -117,8 +115,9 @@ __device__ __forceinline__ PairLoc reverse_loc(const PairLoc& L, const uint32_t 
 }
 
 // The rest of one job after the packed passes: packed = both end points came from them (kPairNoHit: no cell held the score);
-// otherwise the s32 locate passes run here.  Then the output row and the traceback job.
-__device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, const FinalGlobals& g, FinalSmem& S, int32_t* rowH, int32_t* rowF,
+// otherwise sw_forward runs here, forward and on the reversed prefixes ending at its end point.  Then the output row and the
+// traceback job.
+__device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, const FinalGlobals& g, int32_t* rowH, int32_t* rowF,
                                           const uint32_t ji, const uint32_t wi, const bool packed, const uint32_t ef, const uint32_t er) {
   const unsigned lane = lane_id();
   const PairLoc L = final_loc(b, g, wi);
@@ -127,9 +126,8 @@ __device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, c
     if (ef != kPairNoHit) fwd = SwEnd{L.target, (int32_t)(ef >> 16), (int32_t)(ef & 0xFFFFu)};
     if (er != kPairNoHit) rev = SwEnd{L.target, (int32_t)(er >> 16), (int32_t)(er & 0xFFFFu)};
   } else {
-    fwd = sw_locate(L.q, L.m, L.t, L.n, sc, L.target, S.win[0], (int32_t*)S.prof, rowH, rowF);
-    if ((fwd.score & 0xFFFF) == L.target)
-      rev = sw_locate(L.q.reversed_prefix(fwd.read), fwd.read + 1, L.t.reversed_prefix(fwd.ref), fwd.ref + 1, sc, L.target, S.win[0], (int32_t*)S.prof, rowH, rowF);
+    fwd = sw_forward(L.q, L.m, L.t, L.n, sc, rowH, rowF);
+    if ((fwd.score & 0xFFFF) == L.target) rev = sw_forward(L.q.reversed_prefix(fwd.read), fwd.read + 1, L.t.reversed_prefix(fwd.ref), fwd.ref + 1, sc, rowH, rowF);
   }
   if (lane != 0) return;
   const uint32_t r = b.r0 + wi / g.slots, k = wi % g.slots;
@@ -158,8 +156,8 @@ __device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, c
 }
 
 // Forward pass again, now with the end-point tie-breaks (ssw.c:310-336), then the reverse pass over the prefixes that end at the
-// forward optimum, for the jobs job_list[2i], job_list[2i + 1] of a warp: both in one packed pass (sw_pair_locate) where their
-// shapes and the scores allow it (sw_pair_ok), the s32 kernels otherwise; a lone last job runs with an empty second half.
+// forward optimum, for the jobs job_list[2i], job_list[2i + 1] of a warp: both in one packed pass (sw_pair_run) where their
+// shapes and the scores allow it (sw_pair_ok), sw_forward otherwise; a lone last job runs with an empty second half.
 __global__ void __launch_bounds__(kFinalWarpsPerCta * 32, kFinalCtasPerSm)
 finalize_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
   __shared__ FinalSmem s_fin[kFinalWarpsPerCta];
@@ -182,15 +180,15 @@ finalize_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
     {
       const PairLoc L0 = final_loc(b, g, w0), L1 = two ? final_loc(b, g, w1) : no_loc();
       p0 = final_packed(L0, sc); p1 = two && final_packed(L1, sc);
-      if (p0 || p1) ef = sw_pair_locate(p0 ? L0 : no_loc(), p1 ? L1 : no_loc(), sc, S.prof, S.win[0], S.win[1]);
+      if (p0 || p1) ef = sw_pair_run<true>(p0 ? L0 : no_loc(), p1 ? L1 : no_loc(), sc, S.prof, S.win[0], S.win[1]);
     }
     const bool r0 = p0 && ef.x != kPairNoHit, r1 = p1 && ef.y != kPairNoHit;
     if (r0 || r1) {
       const PairLoc R0 = r0 ? reverse_loc(final_loc(b, g, w0), ef.x) : no_loc(), R1 = r1 ? reverse_loc(final_loc(b, g, w1), ef.y) : no_loc();
-      er = sw_pair_locate(R0, R1, sc, S.prof, S.win[0], S.win[1]);
+      er = sw_pair_run<true>(R0, R1, sc, S.prof, S.win[0], S.win[1]);
     }
-    final_finish(b, sc, g, S, rowH, rowF, j0, w0, p0, ef.x, er.x);
-    if (two) final_finish(b, sc, g, S, rowH, rowF, j0 + 1, w1, p1, ef.y, er.y);
+    final_finish(b, sc, g, rowH, rowF, j0, w0, p0, ef.x, er.x);
+    if (two) final_finish(b, sc, g, rowH, rowF, j0 + 1, w1, p1, ef.y, er.y);
     __syncwarp();
   }
 }
@@ -250,10 +248,10 @@ traceback_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
   }
 }
 
-// unit-test kernel: full ssw_align(flag=2) equivalent on explicit pairs, one warp per pair (smr_debug_ssw).  Every kernel that
-// computes part of it is checked against the s32 arg-max kernel sw_forward; a disagreement replaces the score with a marker:
-// -12345 the score-only kernel, -12346 the s32 locate, -12347 the packed locate of the finalize kernel, which runs the pairs
-// (2i, 2i + 1) together, forward and on the reversed prefixes.
+// unit-test kernel: full ssw_align(flag=2) equivalent on explicit pairs, one warp per pair (smr_debug_ssw).  The packed kernel is
+// checked against the s32 arg-max kernel sw_forward, the pairs (2i, 2i + 1) in one pass as the candidate and finalize kernels run
+// them; a pair outside sw_pair_ok is left out.  A disagreement replaces the score with a marker: -12345 the packed score pass (the
+// candidate kernel's), -12347 the packed locate (the finalize kernel's), forward and on the reversed prefixes.
 __global__ void __launch_bounds__(kFinalWarpsPerCta * 32)
 ssw_debug_kernel(const uint8_t* qcat, const uint32_t* qoff, const uint8_t* tcat, const uint32_t* toff, uint32_t npairs, uint32_t filters,
                  DevParams prm, int32_t* out, uint32_t* cigars, uint32_t cigar_cap, FinalGlobals g) {
@@ -263,31 +261,27 @@ ssw_debug_kernel(const uint8_t* qcat, const uint32_t* qoff, const uint8_t* tcat,
   int32_t *rowH, *rowF;
   TraceArena A = final_arena(g, warp, rowH, rowF);
   FinalSmem& S = s_fin[threadIdx.x >> 5];
-  uint8_t* s_ref = S.win[0]; int32_t* s_prof = (int32_t*)S.prof;
   const SwScore sc{prm.match, prm.mismatch, prm.score_N, prm.gap_open, prm.gap_ext, prm.one};
   for (uint32_t k0 = 2 * warp; k0 < npairs; k0 += 2 * nwarps) {
-    PairLoc L[2], RL[2];
+    PairLoc P[2], L[2], RL[2];
     SwEnd fe[2], re[2];
 #pragma unroll 1
     for (uint32_t h = 0; h < 2; ++h) {
-      L[h] = no_loc(); RL[h] = no_loc();
+      P[h] = no_loc(); L[h] = no_loc(); RL[h] = no_loc();
       const uint32_t k = k0 + h;
       if (k >= npairs) break;
       const int32_t m = (int32_t)(qoff[k + 1] - qoff[k]), n = (int32_t)(toff[k + 1] - toff[k]);
       const SeqView q{qcat + qoff[k], 0, 1, false}, t{tcat + toff[k], 0, 1, false};
       int32_t* o = out + (size_t)k * 6;
-      SwEnd f = sw_forward(q, m, t, n, sc, rowH, rowF);
-      // the score-only kernel of the candidate loop must agree with the arg-max kernel
-      if (sw_score(q, m, t, n, sc, s_ref, s_prof, rowH, rowF) != f.score) f.score = -12345;
-      if (f.score > 0) {   // the score-known locate kernel (finalize) must agree with the arg-max kernel on the end point
-        const SwEnd l = sw_locate(q, m, t, n, sc, f.score, s_ref, s_prof, rowH, rowF);
-        if (l.ref != f.ref || l.read != f.read) f.score = -12346;
-      }
-      if (f.score > 0 && m > 0 && sw_pair_ok(m, n, sc)) {
-        L[h] = PairLoc{q, m, t, n, f.score};
-        fe[h] = f;
-        RL[h] = PairLoc{q.reversed_prefix(f.read), f.read + 1, t.reversed_prefix(f.ref), f.ref + 1, f.score};
-        re[h] = sw_forward(RL[h].q, RL[h].m, RL[h].t, RL[h].n, sc, rowH, rowF);
+      const SwEnd f = sw_forward(q, m, t, n, sc, rowH, rowF);
+      if (m > 0 && sw_pair_ok(m, n, sc)) {
+        P[h] = PairLoc{q, m, t, n, f.score};
+        if (f.score > 0) {
+          L[h] = P[h];
+          fe[h] = f;
+          RL[h] = PairLoc{q.reversed_prefix(f.read), f.read + 1, t.reversed_prefix(f.ref), f.ref + 1, f.score};
+          re[h] = sw_forward(RL[h].q, RL[h].m, RL[h].t, RL[h].n, sc, rowH, rowF);
+        }
       }
       int32_t rb = -1, qb = -1, nc = 0;
       if ((uint32_t)(f.score & 0xFFFF) >= filters && f.score > 0) {
@@ -304,10 +298,18 @@ ssw_debug_kernel(const uint8_t* qcat, const uint32_t* qoff, const uint8_t* tcat,
       if (lane == 0) { o[0] = f.score; o[1] = rb; o[2] = f.ref; o[3] = qb; o[4] = f.read; o[5] = nc; }
       __syncwarp();
     }
+    // the packed score pass of both pairs at once, best scores of 0 included
+    if (P[0].m || P[1].m) {
+      const uint32_t s2 = sw_pair_run<false>(P[0], P[1], sc, S.prof, S.win[0], S.win[1]);
+#pragma unroll
+      for (int h = 0; h < 2; ++h)
+        if (P[h].m && (h ? s2 >> 16 : s2 & 0xFFFFu) != (uint32_t)P[h].target && lane == 0) out[(size_t)(k0 + h) * 6] = -12345;
+      __syncwarp();
+    }
     // the packed locate of both pairs at once, forward and on the reversed prefixes ending at each pair's own end point
     if (L[0].m || L[1].m) {
-      const uint2 ef = sw_pair_locate(L[0], L[1], sc, S.prof, S.win[0], S.win[1]);
-      const uint2 er = sw_pair_locate(RL[0], RL[1], sc, S.prof, S.win[0], S.win[1]);
+      const uint2 ef = sw_pair_run<true>(L[0], L[1], sc, S.prof, S.win[0], S.win[1]);
+      const uint2 er = sw_pair_run<true>(RL[0], RL[1], sc, S.prof, S.win[0], S.win[1]);
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
         if (!L[h].m) continue;

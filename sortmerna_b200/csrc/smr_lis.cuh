@@ -1200,7 +1200,7 @@ __device__ void scorer_loop(const DevBatch& b, const DevParams& prm, const LisGl
       }
       __syncwarp();
       { const long long t2 = lis_clock<kInstr>(); cy_load += (unsigned long long)(t2 - tq); tq = t2; }
-      const uint32_t r2 = sw_pair_dispatch(R, s_prof, profB, wa, wb, nmax, sc);
+      const uint32_t r2 = sw_pair_dispatch<false>(R, s_prof, profB, wa - 32, wb - 32, nmax, sc);
       sa = r2 & 0xFFFFu; sb = r2 >> 16;
     } else {
       // shapes or scoring schemes outside the 16-bit kernel: the s32 wavefront (row blocks for long queries), from global memory

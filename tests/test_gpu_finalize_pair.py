@@ -1,6 +1,7 @@
-"""The finalize stage locates stored alignments two per warp pass (packed 16-bit locate) over a dense job list.  These tests
-check it against the oracle: through smr_debug_ssw, which runs consecutive pairs (2i, 2i + 1) through the packed locate and
-marks any disagreement with the s32 kernels, and end to end through smr_align_batch."""
+"""The candidate kernel scores alignments, and the finalize stage locates stored ones over a dense job list, two per warp pass
+with the packed 16-bit kernel.  These tests check it against the oracle: through smr_debug_ssw, which runs consecutive pairs
+(2i, 2i + 1) through the packed score pass and the packed locate and marks any disagreement with the s32 kernel, and end to
+end through smr_align_batch."""
 import os
 
 import numpy as np
@@ -51,7 +52,7 @@ def _check_pairs(aligner, ora, pairs, scores, filters=0):
     for k, (q, t) in enumerate(zip(qs, ts)):
         rc, eo, ec = ora.ssw_align(q.astype(np.int8), t.astype(np.int8), mat, go, ge, filters)
         assert rc == 0
-        assert out[k, 0] not in (-12345, -12346, -12347), (k, out[k])
+        assert out[k, 0] not in (-12345, -12347), (k, out[k])
         assert out[k, 0] == eo[0] and out[k, 2] == eo[2] and out[k, 4] == eo[4], (k, out[k], eo)
         if eo[0] >= filters and eo[0] > 0:
             assert out[k, 1] == eo[1] and out[k, 3] == eo[3] and out[k, 5] == eo[5], (k, out[k], eo)
