@@ -101,6 +101,8 @@ typedef struct {
 enum {
   SMR_CNT_NUM_ALIGNED = 0,   /* readstats.num_aligned (alignment.cpp:414) */
   SMR_CNT_NUM_SHORT = 1,     /* readstats.num_short of the LAST index pass (processor.cpp:109-114,228) */
+  /* SW_CALLS, SW_CELLS, POS_ENTRIES and LIS_CALLS count the work done, so they also count the first (failed) pass of a read
+   * that overflowed its scratch and was run again (smr_align_batch). */
   SMR_CNT_SW_CALLS = 2,      /* ssw_align-equivalent calls */
   SMR_CNT_SW_CELLS = 3,      /* sum refLen*readLen over those calls (forward pass only) */
   SMR_CNT_WINDOWS = 4,       /* seed windows searched (speculative windows included) */
@@ -156,7 +158,12 @@ int smr_index_info(const smr_ctx*, uint64_t out[6]);
  *    seq_cat: reads in 0..4 (4 = ambiguous, as nt_table yields), concatenated; seq_off[nreads+1].
  *    Host buffers; the call copies host->device, runs, and copies the results back.
  *    results[nreads]; alns[nreads * smr_aln_slots()] (= num_alignments per read; see smr_set_aln_slots for 0); cigar_pool[cigar_cap] u32 words;
- *    counters[SMR_CNT_FIXED + n_index_files] are ADDED to (caller zeroes them). */
+ *    counters[SMR_CNT_FIXED + n_index_files] are ADDED to (caller zeroes them).
+ *    *cigar_used = words of cigar_pool used.  If cigar_cap is too small the call fails with SMR_ERR_CAPACITY and *cigar_used names
+ *    the words the batch needs (more than cigar_cap): call again with a pool at least that large.
+ *    Scratch overflow: every read first runs with fixed scratch; a read that outgrows it (many seed hits, a wide traceback band,
+ *    many CIGAR operations, a full device CIGAR pool) is run again on its own with 8x the scratch, then 64x and 512x; after that
+ *    the call fails with SMR_ERR_CAPACITY.  Results do not depend on it. */
 int smr_align_batch(smr_ctx*, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads,
                     smr_read_result* results, smr_aln* alns,
                     uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used,
@@ -209,7 +216,14 @@ int smr_debug_inflate(smr_ctx*, const void* gz, uint64_t nbytes, uint64_t chunk_
  * offsets into the concatenated 0-4 codes, seq04 (optional) = those codes (seq_cap bytes available). */
 int smr_resident_layout(smr_ctx*, uint64_t* header_text_off, uint64_t* read_off, uint8_t* seq04, uint64_t seq_cap);
 
-/* Same work with the batch already resident: upload once, run many times (bench `value` leg). */
+/* Same work with the batch already resident: upload once, run many times (bench `value` leg).
+ * smr_download_results takes the arguments of smr_align_batch and behaves the same way: reads that overflowed their scratch are run
+ * again from a host copy of the resident reads, and a cigar pool too small gives SMR_ERR_CAPACITY with *cigar_used = the words
+ * needed (smr_run_resident again, then download into a larger pool).  The resident batch stays the one uploaded either way:
+ * smr_resident_layout, smr_resident_text and further smr_run_resident calls see it unchanged (a download that retried uploads the
+ * resident reads again).  The retry's own run replaces the device results, so after a download that retried, the next
+ * smr_download_results fails with SMR_ERR_ARG until smr_run_resident has run again (without a retry, downloading twice gives the
+ * same results twice). */
 int smr_upload_batch(smr_ctx*, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads);
 int smr_run_resident(smr_ctx*);                       /* all kernels of one pass over the resident batch */
 int smr_download_results(smr_ctx*, smr_read_result* results, smr_aln* alns, uint32_t* cigar_pool,

@@ -267,18 +267,19 @@ class Aligner:
         self._check(self.L.smr_index_info(self.h, _ptr(out)), "smr_index_info")
         return dict(zip(("parts", "hbm_bytes", "nodes", "entries", "ids", "positions"), map(int, out)))
 
-    def _outputs(self, n, reuse=False):
+    def _outputs(self, n, reuse=False, cigar_words=0):
+        """result buffers of n reads; the CIGAR pool holds 48 words per alignment slot, or cigar_words if that is more"""
         slots = int(self.L.smr_aln_slots(self.h))   # num_alignments, or the stride of the all-alignments mode (0)
         if reuse:   # the same host buffers for every call of this shape (a streaming caller consumes a batch before the next)
-            key = (n, slots, self.n_index_files)
+            key = (n, slots, self.n_index_files, cigar_words)
             if getattr(self, "_out_key", None) != key:
-                self._out_key, self._out_bufs = key, self._outputs(n)
+                self._out_key, self._out_bufs = key, self._outputs(n, cigar_words=cigar_words)
             bufs = self._out_bufs
             bufs[5][:] = 0
             return bufs
         res = np.zeros(n, RESULT_DTYPE)
         alns = np.zeros(n * slots, ALN_DTYPE)
-        cap = 48 * n * slots + 4096
+        cap = max(48 * n * slots + 4096, cigar_words)
         pool = np.zeros(cap, np.uint32)
         counters = np.zeros(CNT_FIXED + max(1, self.n_index_files), np.uint64)
         return slots, res, alns, pool, cap, counters
@@ -296,8 +297,9 @@ class Aligner:
         cat = np.ascontiguousarray(cat, np.uint8)
         off = np.ascontiguousarray(off, np.uint64)
         n = off.size - 1
+        words = 0
         while True:
-            slots, res, alns, pool, cap, counters = self._outputs(n, reuse_outputs)
+            slots, res, alns, pool, cap, counters = self._outputs(n, reuse_outputs, words)
             stats = np.zeros(n * slots, STATS_DTYPE) if with_stats else None
             self._check(self.L.smr_set_stats_buffer(self.h, _ptr(stats) if with_stats else C.c_void_p(0)), "smr_set_stats_buffer")
             used = C.c_uint64(0)
@@ -306,6 +308,9 @@ class Aligner:
             need = int(self.L.smr_aln_slots_needed(self.h)) if rc == 5 and self.params.num_alignments == 0 else 0
             if need > slots:   # all-alignments mode: the library names the stride this batch needs; allocate and run again
                 self.set_aln_slots(need)
+                continue
+            if rc == 5 and used.value > cap:   # the CIGAR pool: the library names the words this batch needs
+                words = used.value
                 continue
             break
         self._check(rc, "smr_align_batch")
@@ -385,11 +390,18 @@ class Aligner:
 
     def download(self):
         n = self._n_resident
-        slots, res, alns, pool, cap, counters = self._outputs(n)
         stats, self._stats = getattr(self, "_stats", None), None
-        used = C.c_uint64(0)
-        rc = self.L.smr_download_results(self.h, _ptr(res), _ptr(alns), _ptr(pool), C.c_uint64(cap), C.byref(used),
-                                         _ptr(counters), C.c_uint32(counters.size))
+        words = 0
+        while True:
+            slots, res, alns, pool, cap, counters = self._outputs(n, cigar_words=words)
+            used = C.c_uint64(0)
+            rc = self.L.smr_download_results(self.h, _ptr(res), _ptr(alns), _ptr(pool), C.c_uint64(cap), C.byref(used),
+                                             _ptr(counters), C.c_uint32(counters.size))
+            if rc == 5 and used.value > cap:   # the CIGAR pool: the library names the words needed; run the batch again into a larger one
+                words = used.value
+                self._check(self.L.smr_run_resident(self.h), "smr_run_resident")
+                continue
+            break
         self.L.smr_set_stats_buffer(self.h, C.c_void_p(0))
         self._check(rc, "smr_download_results")
         out = self._pack(res, alns, pool, used.value, counters, slots)

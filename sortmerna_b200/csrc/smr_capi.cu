@@ -91,6 +91,7 @@ struct smr_ctx {
   uint64_t text_bytes = 0;          // size of the text behind the resident batch (smr_upload_fastx / _gz)
   uint32_t inf_spans = 0, inf_candidates = 0; double t_inflate = 0;
   bool device_only_reads = false;   // the resident batch was decoded on the device: no host copy of the sequences yet
+  bool results_spent = false;       // a download retried reads: the device results are those of the retry, not of the resident batch
   double t_decode = 0;
   uint32_t tb_threads = 0, tb_cap_w = 0, tb_cap_cig = 0; size_t tb_cap_dir = 0, tb_stride = 0;
   uint32_t lis_warps = 0, final_warps = 0;
@@ -730,6 +731,7 @@ int run_impl(smr_ctx* ctx) {
   if (ctx->prm.num_alignments < 0) { ctx->err = "num_alignments < 0"; return SMR_ERR_ARG; }
   if (ctx->prm.minoccur != 0) { ctx->err = "minoccur != 0 is not supported"; return SMR_ERR_UNSUPPORTED; }
   ctx->t_seed = ctx->t_lis = ctx->t_final = ctx->t_total = 0; ctx->n_launch = 0;
+  ctx->results_spent = false;
   const uint32_t nreads = ctx->nreads;
   if (nreads == 0) return SMR_OK;
   const uint32_t slots = slots_of(ctx);
@@ -862,7 +864,14 @@ int run_impl(smr_ctx* ctx) {
 struct HostOut {
   smr_read_result* results; smr_aln* alns; uint32_t* cigar_pool; uint64_t cigar_cap; uint64_t cigar_used;
   uint64_t* counters; uint32_t n_counters;
+  bool pool_short = false;   // cigar_cap was exceeded: nothing more is written, cigar_used goes on counting the words the batch needs
 };
+
+// the caller's CIGAR pool was too small: *cigar_used names the words the batch needs
+int pool_short_error(smr_ctx* ctx, const HostOut& out) {
+  ctx->err = "cigar pool too small: the batch needs " + std::to_string(out.cigar_used) + " words, cigar_cap is " + std::to_string(out.cigar_cap);
+  return SMR_ERR_CAPACITY;
+}
 
 // copies results of the resident batch to the host; returns the indices of reads whose scratch overflowed
 int download_impl(smr_ctx* ctx, HostOut& out, std::vector<uint32_t>& flagged, const uint32_t* map /*local->caller index or null*/) {
@@ -926,9 +935,12 @@ int download_impl(smr_ctx* ctx, HostOut& out, std::vector<uint32_t>& flagged, co
     ctx->need_slots = need_slots;
     return SMR_ERR_CAPACITY;
   }
-  if (run > out.cigar_cap) { ctx->err = "cigar pool too small"; return SMR_ERR_CAPACITY; }
   if (run >= 0xFFFFFFFFull) { ctx->err = "CIGAR pool offset passes 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches"; return SMR_ERR_CAPACITY; }
   out.cigar_used = run;
+  // a pool too small fails the call only at its end (pool_short_error): the flagged reads are still retried, so that
+  // cigar_used names every word the batch needs and one larger pool is enough
+  if (run > out.cigar_cap) out.pool_short = true;
+  if (out.pool_short) return rc;
   // pass 2: results, alignments and cigars of disjoint read ranges, by a few host threads for large batches
   auto pack = [&](uint32_t lo, uint32_t hi) {
     for (uint32_t r = lo; r < hi; ++r) {
@@ -1657,6 +1669,7 @@ int smr_align_batch(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_of
   HostOut out{results, alns, cigar_pool, cigar_cap, 0, counters, n_counters};
   ctx->scale = 1;
   int rc = align_impl(ctx, seq_cat, seq_off, nreads, out, nullptr, 0);
+  if (rc == SMR_OK && out.pool_short) rc = pool_short_error(ctx, out);
   if (cigar_used) *cigar_used = out.cigar_used;
   return rc;
 } SMR_CATCH(ctx)
@@ -1755,6 +1768,7 @@ int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, 
                          uint64_t* counters, uint32_t n_counters) try {
   if (!ctx || !results || !alns) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
+  if (ctx->results_spent) { ctx->err = "the results of the last run were replaced by the retry of a download: smr_run_resident again"; return SMR_ERR_ARG; }
   const uint32_t slots = slots_of(ctx);
   const uint32_t n = ctx->nreads;
   memset(results, 0, (size_t)n * sizeof(smr_read_result));
@@ -1766,7 +1780,8 @@ int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, 
     if (getenv("SMR_VERBOSE")) fprintf(stderr, "[smr] %zu reads overflowed their scratch (resident batch): retrying with scale 8 (causes so far: lane %llu region %llu pairs %llu trace %llu cigar %llu err %llu)\n", flagged.size(),
       (unsigned long long)ctx->flag_hist[0], (unsigned long long)ctx->flag_hist[1], (unsigned long long)ctx->flag_hist[2], (unsigned long long)ctx->flag_hist[3], (unsigned long long)ctx->flag_hist[4], (unsigned long long)ctx->flag_hist[5]);
     // redo the overflowed reads from the retained host copy with larger scratch
-    if (ctx->device_only_reads) {   // decoded on the device: fetch the sequences now (only when a retry is needed)
+    const bool device_only = ctx->device_only_reads;
+    if (device_only) {   // decoded on the device: fetch the sequences now (only when a retry is needed)
       ctx->h_seq.resize(ctx->total_nt);
       CK(cudaMemcpy(ctx->h_seq.data(), ctx->seq04.p, ctx->total_nt, cudaMemcpyDeviceToHost));
       ctx->h_off.assign(ctx->off32.begin(), ctx->off32.end());
@@ -1778,9 +1793,17 @@ int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, 
     ctx->scale = 8;
     rc = align_impl(ctx, sseq.data(), soff.data(), (uint32_t)flagged.size(), out, flagged.data(), 1);
     ctx->scale = 1;
-    // the resident batch was replaced by the retry batch: upload again before the next smr_run_resident
-    ctx->nreads = 0;
+    // the retry made its sub-batch the resident batch: upload the original reads again, so that the resident batch is the one
+    // uploaded (read offsets, sequences; the text, header offsets and host copy stay as the upload left them) and the next
+    // smr_run_resident / smr_resident_layout see it.  Only a download that retried pays for this copy.
+    const double h2d = ctx->t_h2d;
+    const int up = upload_batch_impl(ctx, hs.data(), ho.data(), n, !device_only);
+    ctx->t_h2d = h2d;
+    ctx->device_only_reads = device_only;
+    if (rc == SMR_OK) rc = up;
+    ctx->results_spent = true;   // (the retry's run overwrote the device results: a second download needs a new run)
   }
+  if (rc == SMR_OK && out.pool_short) rc = pool_short_error(ctx, out);
   if (cigar_used) *cigar_used = out.cigar_used;
   return rc;
 } SMR_CATCH(ctx)
