@@ -102,7 +102,7 @@ enum {
   SMR_CNT_NUM_ALIGNED = 0,   /* readstats.num_aligned (alignment.cpp:414) */
   SMR_CNT_NUM_SHORT = 1,     /* readstats.num_short of the LAST index pass (processor.cpp:109-114,228) */
   /* SW_CALLS, SW_CELLS, POS_ENTRIES and LIS_CALLS count the work done, so they also count the first (failed) pass of a read
-   * that overflowed its scratch and was run again (smr_align_batch). */
+   * that overflowed its scratch and was run again (smr_align_batch, smr_download_results). */
   SMR_CNT_SW_CALLS = 2,      /* ssw_align-equivalent calls */
   SMR_CNT_SW_CELLS = 3,      /* sum refLen*readLen over those calls (forward pass only) */
   SMR_CNT_WINDOWS = 4,       /* seed windows searched (speculative windows included) */
@@ -162,8 +162,10 @@ int smr_index_info(const smr_ctx*, uint64_t out[6]);
  *    *cigar_used = words of cigar_pool used.  If cigar_cap is too small the call fails with SMR_ERR_CAPACITY and *cigar_used names
  *    the words the batch needs (more than cigar_cap): call again with a pool at least that large.
  *    Scratch overflow: every read first runs with fixed scratch; a read that outgrows it (many seed hits, a wide traceback band,
- *    many CIGAR operations, a full device CIGAR pool) is run again on its own with 8x the scratch, then 64x and 512x; after that
- *    the call fails with SMR_ERR_CAPACITY.  Results do not depend on it. */
+ *    many CIGAR operations, a full device CIGAR pool) is run again with 8x the scratch, then 64x and 512x, in a batch of the
+ *    flagged reads gathered on the device; after that the call fails with SMR_ERR_CAPACITY.  Results do not depend on it; the
+ *    CIGARs of retried reads follow those of the others in cigar_pool.  smr_last_timings sums the kernel and D2H times of the first
+ *    run and its retries.  Uploads the batch as the resident batch, with no text behind it (as smr_upload_batch). */
 int smr_align_batch(smr_ctx*, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads,
                     smr_read_result* results, smr_aln* alns,
                     uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used,
@@ -205,7 +207,8 @@ int smr_upload_fastx(smr_ctx*, const char* text, uint64_t nbytes, uint32_t* nrea
  * truncated file fails with SMR_ERR_ARG. */
 int smr_upload_fastx_gz(smr_ctx*, const void* gz, uint64_t nbytes, uint32_t* nreads);
 /* The text behind the resident batch (what smr_upload_fastx was given / what smr_upload_fastx_gz inflated): *nbytes = its size;
- * copied to `text` when that is not null (cap bytes available).  header_text_off of smr_resident_layout indexes it. */
+ * copied to `text` when that is not null (cap bytes available).  header_text_off of smr_resident_layout indexes it.  A batch
+ * uploaded by smr_upload_batch or smr_align_batch has no text: *nbytes = 0. */
 int smr_resident_text(smr_ctx*, char* text, uint64_t cap, uint64_t* nbytes);
 /* Test hook: inflate only.  chunk_bytes = distance of the speculative block searches (>= 1024; 0 = the default of smr_upload_fastx_gz); info = {spans decoded,
  * candidates found, device time in us, H2D time in us}. */
@@ -218,12 +221,10 @@ int smr_resident_layout(smr_ctx*, uint64_t* header_text_off, uint64_t* read_off,
 
 /* Same work with the batch already resident: upload once, run many times (bench `value` leg).
  * smr_download_results takes the arguments of smr_align_batch and behaves the same way: reads that overflowed their scratch are run
- * again from a host copy of the resident reads, and a cigar pool too small gives SMR_ERR_CAPACITY with *cigar_used = the words
- * needed (smr_run_resident again, then download into a larger pool).  The resident batch stays the one uploaded either way:
- * smr_resident_layout, smr_resident_text and further smr_run_resident calls see it unchanged (a download that retried uploads the
- * resident reads again).  The retry's own run replaces the device results, so after a download that retried, the next
- * smr_download_results fails with SMR_ERR_ARG until smr_run_resident has run again (without a retry, downloading twice gives the
- * same results twice). */
+ * again in a batch of their own, and a cigar pool too small gives SMR_ERR_CAPACITY with *cigar_used = the words needed (download
+ * again into a larger pool).  It never changes the resident batch or the device results of its run: it may be called any number
+ * of times after one smr_run_resident, and a download that needs retries runs them again each time.  smr_upload_batch leaves no
+ * text behind the resident batch (smr_resident_text: 0 bytes; smr_format_reports needs the text passed in). */
 int smr_upload_batch(smr_ctx*, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads);
 int smr_run_resident(smr_ctx*);                       /* all kernels of one pass over the resident batch */
 int smr_download_results(smr_ctx*, smr_read_result* results, smr_aln* alns, uint32_t* cigar_pool,

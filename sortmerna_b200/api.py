@@ -382,24 +382,26 @@ class Aligner:
         return hdr, off, seq
 
     def run_resident(self, with_stats: bool = False):
-        """with_stats: the next download() also returns calc_miss_gap_match per stored alignment (out["stats"])"""
+        """with_stats: download() also returns calc_miss_gap_match per stored alignment (out["stats"])"""
         n = self._n_resident
         self._stats = np.zeros(n * int(self.L.smr_aln_slots(self.h)), STATS_DTYPE) if with_stats else None
         self._check(self.L.smr_set_stats_buffer(self.h, _ptr(self._stats) if with_stats else C.c_void_p(0)), "smr_set_stats_buffer")
         self._check(self.L.smr_run_resident(self.h), "smr_run_resident")
 
     def download(self):
+        """smr_download_results: the results of the last run_resident(); may be called again without running again"""
         n = self._n_resident
-        stats, self._stats = getattr(self, "_stats", None), None
+        stats = getattr(self, "_stats", None)
+        stats = np.zeros_like(stats) if stats is not None else None
+        self._check(self.L.smr_set_stats_buffer(self.h, _ptr(stats) if stats is not None else C.c_void_p(0)), "smr_set_stats_buffer")
         words = 0
         while True:
             slots, res, alns, pool, cap, counters = self._outputs(n, cigar_words=words)
             used = C.c_uint64(0)
             rc = self.L.smr_download_results(self.h, _ptr(res), _ptr(alns), _ptr(pool), C.c_uint64(cap), C.byref(used),
                                              _ptr(counters), C.c_uint32(counters.size))
-            if rc == 5 and used.value > cap:   # the CIGAR pool: the library names the words needed; run the batch again into a larger one
+            if rc == 5 and used.value > cap:   # the CIGAR pool: the library names the words needed; download again into a larger one
                 words = used.value
-                self._check(self.L.smr_run_resident(self.h), "smr_run_resident")
                 continue
             break
         self.L.smr_set_stats_buffer(self.h, C.c_void_p(0))

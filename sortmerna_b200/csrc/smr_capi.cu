@@ -57,6 +57,25 @@ struct Part {
   std::vector<std::string> h_rnames;   // host copy of the same ids: the OTU map ranks them (smr_otu_begin)
 };
 
+// device times of one run (CUDA events, ms) and its kernel launches (smr_last_timings)
+struct RunTimes {
+  double total = 0, seed = 0, lis = 0, final = 0; uint64_t launches = 0;
+  RunTimes& operator+=(const RunTimes& o) { total += o.total; seed += o.seed; lis += o.lis; final += o.final; launches += o.launches; return *this; }
+};
+
+// One batch of reads on the device, the seed scratch sized from it, and what a run of it leaves for a download.  The context's
+// resident batch is one; a scratch-overflow retry runs the flagged reads as another.  Move-only: the buffers free themselves.
+struct Batch {
+  uint32_t nreads = 0, max_len = 0; uint64_t total_nt = 0;
+  uint32_t scale = 1;                // scratch scale (1 = fast path; 8x per retry)
+  bool from_text = false;            // decoded from text on the device (smr_upload_fastx[_gz]): its header offsets are known
+  std::vector<uint32_t> off32;       // host copy of seq_off
+  DevBuf seq04, seq_off, pk_off, pk03, pk03alt, has_n;
+  DevBuf hits, hit_cnt, cost, bins; size_t hits_stride = 0; uint32_t cnt_stride = 0;
+  DevBuf state, flags, hit_db, aln_work, out_aln, aln_stats, cigar_pool, scalars, counters; uint64_t cigar_cap_dev = 0;
+  RunTimes run;
+};
+
 }  // namespace
 
 struct smr_ctx {
@@ -73,14 +92,9 @@ struct smr_ctx {
   uint32_t all_slots = 16;       // stride of the result layout when num_alignments == 0 (smr_set_aln_slots)
   uint32_t lis_ctas_per_sm = kLisMinCtas;   // persistent CTAs of the candidate kernel per SM (matches its __launch_bounds__)
 
-  // resident batch
-  uint32_t nreads = 0; uint64_t total_nt = 0; uint32_t max_len = 0;
-  std::vector<uint8_t> h_seq; std::vector<uint64_t> h_off;    // host copy (scratch-overflow retries)
-  std::vector<uint32_t> off32;                                // 32-bit read offsets of the resident batch
-  DevBuf seq04, seq_off, pk03, pk03alt, pk_off, has_n, hit_cnt, flags, state, hit_db, aln_work, out_aln;
-  DevBuf hits, cost, bins, scalars, counters, cigar_pool, parts_dev;
-  size_t hits_stride = 0; uint32_t cnt_stride = 0;
-  DevBuf lis_arena, lis_epochs, lis_queue, lis_done, lis_rows, lis_dbg, final_arena, lane_hits, tb_arena, tb_jobs, fin_list, aln_stats;
+  Batch resident;
+  // scratch of a run that no later call reads, sized by the scale of the run
+  DevBuf parts_dev, lis_arena, lis_epochs, lis_queue, lis_done, lis_rows, lis_dbg, final_arena, lane_hits, tb_arena, tb_jobs, fin_list;
   smr_aln_stats* host_stats = nullptr;   // optional output of the report arithmetic
   PinBuf h_state, h_flags, h_hitdb, h_outaln, h_stats, h_cigar, h_off32, h_pkoff;
   std::vector<uint64_t> h_coff;
@@ -90,8 +104,6 @@ struct smr_ctx {
   DevBuf seed_ctr, d_gz, d_cand, d_res, d_sym, d_win, d_ids, d_off, d_cnt64, d_moff, d_mem, d_poff, d_plen, d_pcrc;   // gz inflate (smr_inflate.cuh)
   uint64_t text_bytes = 0;          // size of the text behind the resident batch (smr_upload_fastx / _gz)
   uint32_t inf_spans = 0, inf_candidates = 0; double t_inflate = 0;
-  bool device_only_reads = false;   // the resident batch was decoded on the device: no host copy of the sequences yet
-  bool results_spent = false;       // a download retried reads: the device results are those of the retry, not of the resident batch
   double t_decode = 0;
   uint32_t tb_threads = 0, tb_cap_w = 0, tb_cap_cig = 0; size_t tb_cap_dir = 0, tb_stride = 0;
   uint32_t lis_warps = 0, final_warps = 0;
@@ -99,8 +111,6 @@ struct smr_ctx {
   uint32_t hist_cap = 0, cand_cap = 0, pair_cap = 0, row_cap = 0, pall_cap = 0, task_cap = 0, cap_w = 0, cap_cig = 0; size_t cap_dir = 0;
   uint32_t lis_ctas = 0;
   uint32_t lane_hits_cap = 0, lane_hits_warps = 0;
-  uint64_t cigar_cap_dev = 0;
-  uint32_t scale = 1;         // scratch scale of the current run (1 = fast path)
   bool instr = false;         // smr_set_instrumentation: seed kernel counts windows / lists / entries, candidate kernel accounts its phases (clock64)
   uint64_t flag_hist[6] = {0, 0, 0, 0, 0, 0};  // overflow causes seen so far (seed lane / seed region / pairs / trace / cigar / error)
   // report writer (smr_report.cuh)
@@ -121,7 +131,8 @@ struct smr_ctx {
   } otu;
   // timings
   std::vector<cudaEvent_t> ev;
-  double t_total = 0, t_seed = 0, t_lis = 0, t_final = 0, t_h2d = 0, t_d2h = 0; uint64_t n_launch = 0;
+  RunTimes t_run;   // the last run, and the retries of its download
+  double t_h2d = 0, t_d2h = 0;
 };
 
 namespace {
@@ -317,21 +328,21 @@ cudaEvent_t get_event(smr_ctx* ctx, size_t i) {
 // scalars block layout (u32): [0]=work_n [1]=lis work_next [2]=final work_next [3]=lis work_next of the second cursor ; cigar_used (u64) at byte 16 ;
 // finalize job count (u32) at byte 24 ; task queue cursors at 128..
 struct Scalars { uint32_t* work_n; uint32_t* lis_next; uint32_t* fin_next; uint32_t* lis_next_b; unsigned long long* cigar_used; uint32_t* fin_jobs; uint32_t* q_head; uint32_t* q_tail; uint32_t* planners_done; };
-Scalars scalars_of(smr_ctx* ctx) {
-  uint8_t* p = (uint8_t*)ctx->scalars.p;
+Scalars scalars_of(const Batch& b) {
+  uint8_t* p = (uint8_t*)b.scalars.p;
   return Scalars{(uint32_t*)p, (uint32_t*)(p + 4), (uint32_t*)(p + 8), (uint32_t*)(p + 12), (unsigned long long*)(p + 16), (uint32_t*)(p + 24), (uint32_t*)(p + 128), (uint32_t*)(p + 256), (uint32_t*)(p + 384)};
 }
 
-int setup_arenas(smr_ctx* ctx) {
+int setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
   uint32_t max_nref = 1;
   for (auto& pt : ctx->parts) max_nref = std::max(max_nref, pt.d.nref);
   ctx->hist_cap = max_nref;
   ctx->cand_cap = std::max(64u, max_nref);
-  ctx->pair_cap = pow2_ge(4096u * ctx->scale);
+  ctx->pair_cap = pow2_ge(4096u * scale);
   ctx->task_cap = 2 * ctx->pair_cap;
   // SW windows are at most read length + 2 * edges columns (alignment.cpp:272-357; edges may be a percentage of the read)
-  const uint32_t edges = ctx->prm.edges_is_percent ? (uint32_t)((ctx->prm.edges / 100.0) * (double)ctx->max_len) : (uint32_t)std::max(0, ctx->prm.edges);
-  ctx->row_cap = ctx->max_len + 2 * edges + 2 * 64 + 64;
+  const uint32_t edges = ctx->prm.edges_is_percent ? (uint32_t)((ctx->prm.edges / 100.0) * (double)max_len) : (uint32_t)std::max(0, ctx->prm.edges);
+  ctx->row_cap = max_len + 2 * edges + 2 * 64 + 64;
   // planner and scorer warps wait for each other: EVERY CTA of the grid must be resident at once
   int occ = 0;
   CK(cudaFuncSetAttribute(lis_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLisSmemBytes));
@@ -340,7 +351,7 @@ int setup_arenas(smr_ctx* ctx) {
   if (occ < 1) { ctx->err = "lis_kernel does not fit on an SM"; return SMR_ERR_CUDA; }
   ctx->lis_ctas = (uint32_t)ctx->sm_count * std::min<uint32_t>(ctx->lis_ctas_per_sm, (uint32_t)occ);
   ctx->lis_warps = ctx->lis_ctas * kPlannerWarps;   // planner warps (each owns an arena)
-  ctx->pall_cap = 32768u * ctx->scale;
+  ctx->pall_cap = 32768u * scale;
   ctx->lis_stride = lis_arena_bytes(ctx->hist_cap, ctx->cand_cap, ctx->pair_cap, ctx->task_cap, ctx->pall_cap);
   // keep the arena total under ~16 GB (of the 80 GB of an H100): fewer persistent CTAs for huge reference sets
   const size_t budget = (size_t)16 << 30;
@@ -356,110 +367,124 @@ int setup_arenas(smr_ctx* ctx) {
   // histogram epochs start at 0 over a zeroed histogram (every run: the arena layout depends on the scale of the run)
   CK(cudaMemset2DAsync(ctx->lis_arena.p, ctx->lis_stride, 0, lis_arena_zero_bytes(ctx->hist_cap), ctx->lis_warps, ctx->stream));   // votes + bitmaps only
   CK(cudaMemsetAsync(ctx->lis_epochs.p, 0, (size_t)ctx->lis_warps * 4, ctx->stream));
-  ctx->cap_w = 2 * 256 * ctx->scale + 8;          // band widths up to 256*scale
-  ctx->cap_cig = 2 * (ctx->max_len + 64) + 16;
-  ctx->cap_dir = (size_t)65536 * ctx->scale + (size_t)ctx->max_len * 9 * 3 + 64;
+  ctx->cap_w = 2 * 256 * scale + 8;          // band widths up to 256*scale
+  ctx->cap_cig = 2 * (max_len + 64) + 16;
+  ctx->cap_dir = (size_t)65536 * scale + (size_t)max_len * 9 * 3 + 64;
   ctx->final_warps = (uint32_t)ctx->sm_count * kFinalCtasPerSm * kFinalWarpsPerCta;
   ctx->final_stride = final_arena_bytes(ctx->cap_w, ctx->cap_cig, ctx->row_cap, ctx->cap_dir);
   while (ctx->final_warps > 64 && ctx->final_stride * ctx->final_warps > budget) ctx->final_warps /= 2;
   if (int rc = ensure(ctx, ctx->final_arena, ctx->final_stride * ctx->final_warps)) return rc;
   // traceback stage: one thread per alignment, 1024 threads per SM
   ctx->tb_threads = (uint32_t)ctx->sm_count * 1024u;
-  ctx->tb_cap_w = 2 * 32 * ctx->scale + 8;                       // band widths up to 32*scale
-  ctx->tb_cap_cig = 128 * ctx->scale;
-  ctx->tb_cap_dir = (size_t)32768 * ctx->scale;                  // (2*band+1) * readLen * 3 bytes: band 32 at 150 nt
+  ctx->tb_cap_w = 2 * 32 * scale + 8;                       // band widths up to 32*scale
+  ctx->tb_cap_cig = 128 * scale;
+  ctx->tb_cap_dir = (size_t)32768 * scale;                  // (2*band+1) * readLen * 3 bytes: band 32 at 150 nt
   ctx->tb_stride = ((size_t)ctx->tb_cap_w * 12 + (size_t)ctx->tb_cap_cig * 4 + ctx->tb_cap_dir + 255) & ~(size_t)255;
   while (ctx->tb_threads > 4096 && ctx->tb_stride * ctx->tb_threads > budget) ctx->tb_threads /= 2;
   if (int rc = ensure(ctx, ctx->tb_arena, ctx->tb_stride * ctx->tb_threads)) return rc;
-  ctx->lane_hits_cap = kLaneHitCap * ctx->scale;
-  ctx->lane_hits_warps = ctx->scale == 1 ? (uint32_t)ctx->sm_count * kSeedCtasPerSm * kSeedWarpsPerCta : 1024u;
+  ctx->lane_hits_cap = kLaneHitCap * scale;
+  ctx->lane_hits_warps = scale == 1 ? (uint32_t)ctx->sm_count * kSeedCtasPerSm * kSeedWarpsPerCta : 1024u;
   if (int rc = ensure(ctx, ctx->lane_hits, (size_t)ctx->lane_hits_warps * ctx->lane_hits_cap * 32 * 4)) return rc;
   return SMR_OK;
 }
 
-int finish_upload(smr_ctx* ctx, uint32_t nreads, uint64_t w);
+// the reads c0 .. c0 + n of a batch as the kernels see them
+DevBatch make_batch(const Batch& s, uint32_t c0, uint32_t n) {
+  DevBatch b{};
+  b.nreads = n; b.r0 = c0; b.seq_base0 = s.off32[c0];
+  b.seq04 = (const uint8_t*)s.seq04.p; b.seq_off = (const uint32_t*)s.seq_off.p;
+  b.pk03 = (const uint32_t*)s.pk03.p; b.pk03alt = (const uint32_t*)s.pk03alt.p; b.pk_off = (const uint32_t*)s.pk_off.p;
+  b.has_n = (const uint8_t*)s.has_n.p; b.hit_scale = s.scale; b.hits = (uint2*)s.hits.p;
+  b.hit_cnt = (uint32_t*)s.hit_cnt.p; b.flags = (uint32_t*)s.flags.p; b.state = (ReadState*)s.state.p;
+  b.hit_db = (uint16_t*)s.hit_db.p; b.counters = (unsigned long long*)s.counters.p;
+  b.hits_stride = s.hits_stride; b.cnt_stride = s.cnt_stride; b.cost = (uint32_t*)s.cost.p;
+  b.bins = (uint32_t*)s.bins.p; b.bin_count = (uint32_t*)s.bins.p + (size_t)s.cnt_stride * kCostBins;
+  return b;
+}
 
-int upload_batch_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads, bool keep_host) {
-  if (nreads == 0) { ctx->nreads = 0; return SMR_OK; }
-  const uint64_t total = seq_off[nreads] - seq_off[0];
-  if (total >= 0xF0000000ull) { ctx->err = "batch larger than 2^32 nucleotides: split it"; return SMR_ERR_ARG; }
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
-  CK(cudaEventRecord(e0, ctx->stream));
-  std::vector<uint32_t>& off32 = ctx->off32; off32.resize(nreads + 1);
-  { int prc; if ((prc = ensure(ctx, ctx->h_pkoff, (size_t)(nreads + 1) * 4))) return prc; if ((prc = ensure(ctx, ctx->h_off32, (size_t)(nreads + 1) * 4))) return prc; }
-  uint32_t* pkoff = (uint32_t*)ctx->h_pkoff.p;
-  uint32_t max_len = 0; uint64_t w = 0;
-  for (uint32_t r = 0; r <= nreads; ++r) {
-    off32[r] = (uint32_t)(seq_off[r] - seq_off[0]);
+// The layout of n reads of lengths len(r) in b: read offsets (b.off32, b.seq_off), packed-word offsets (b.pk_off: (len + 15) / 16 + 2
+// words per read, the layout of pack_reads_kernel), nreads, total_nt and max_len.  *words = the packed-word total.  The device copies
+// are staged in the context's pinned buffers: the caller synchronizes before the next layout.
+template <class Len>
+int read_layout(smr_ctx* ctx, Batch& b, uint32_t n, Len len, uint64_t* words) {
+  int rc;
+  if ((rc = ensure(ctx, ctx->h_pkoff, (size_t)(n + 1) * 4)) || (rc = ensure(ctx, ctx->h_off32, (size_t)(n + 1) * 4))) return rc;
+  uint32_t *off32 = (uint32_t*)ctx->h_off32.p, *pkoff = (uint32_t*)ctx->h_pkoff.p;
+  uint64_t total = 0, w = 0; uint32_t max_len = 0;
+  for (uint32_t r = 0; r <= n; ++r) {
+    off32[r] = (uint32_t)total;
     pkoff[r] = (uint32_t)w;
-    if (r < nreads) {
-      const uint64_t len = seq_off[r + 1] - seq_off[r];
-      max_len = std::max<uint32_t>(max_len, (uint32_t)len);
-      w += (len + 15) / 16 + 2;     // +2 padding words: window_fwd reads three consecutive words
+    if (r < n) {
+      const uint64_t l = len(r);
+      max_len = std::max<uint32_t>(max_len, (uint32_t)l);
+      total += l;
+      w += (l + 15) / 16 + 2;     // +2 padding words: window_fwd reads three consecutive words
     }
   }
+  if (total >= 0xF0000000ull) { ctx->err = "batch larger than 2^32 nucleotides: split it"; return SMR_ERR_ARG; }
   if (w >= 0xFFFFFFFFull) { ctx->err = "batch too large"; return SMR_ERR_ARG; }
-  ctx->nreads = nreads; ctx->total_nt = total; ctx->max_len = max_len;
-  if (keep_host) {
-    ctx->h_seq.assign(seq_cat + seq_off[0], seq_cat + seq_off[nreads]);
-    ctx->h_off.resize(nreads + 1);
-    for (uint32_t r = 0; r <= nreads; ++r) ctx->h_off[r] = seq_off[r] - seq_off[0];
-  }
-  const uint32_t slots = slots_of(ctx);
-  int rc;
-  if ((rc = ensure(ctx, ctx->seq04, total + 64))) return rc;
-  if ((rc = ensure(ctx, ctx->seq_off, (size_t)(nreads + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->pk_off, (size_t)(nreads + 1) * 4))) return rc;
-  CK(cudaMemcpyAsync(ctx->seq04.p, seq_cat + seq_off[0], total, cudaMemcpyHostToDevice, ctx->stream));
-  memcpy(ctx->h_off32.p, off32.data(), (size_t)(nreads + 1) * 4);
-  CK(cudaMemcpyAsync(ctx->seq_off.p, ctx->h_off32.p, (size_t)(nreads + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->pk_off.p, pkoff, (size_t)(nreads + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-  ctx->device_only_reads = false;
-  if ((rc = finish_upload(ctx, nreads, w))) return rc;
-  CK(cudaEventRecord(e1, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));   // off32/pkoff are stack-owned
-  float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_h2d = ms;
+  if ((rc = ensure(ctx, b.seq_off, (size_t)(n + 1) * 4)) || (rc = ensure(ctx, b.pk_off, (size_t)(n + 1) * 4))) return rc;
+  CK(cudaMemcpyAsync(b.seq_off.p, off32, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(b.pk_off.p, pkoff, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+  b.off32.assign(off32, off32 + n + 1);
+  b.nreads = n; b.total_nt = total; b.max_len = max_len;
+  *words = w;
   return SMR_OK;
 }
 
-// the part of an upload that does not depend on where the reads came from: seq04 / seq_off / pk_off are on the device,
-// ctx->off32 (host) holds the offsets; sizes the per-batch buffers and 2-bit packs the reads
-int finish_upload(smr_ctx* ctx, uint32_t nreads, uint64_t w) {
-  const uint32_t slots = slots_of(ctx);
-  const std::vector<uint32_t>& off32 = ctx->off32;
+// The part of an upload that does not depend on where the reads came from: b's reads and offsets are on the device and b.off32 on the
+// host; sizes the batch's other buffers for its scale and 2-bit packs the reads.
+int finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
+  const uint32_t slots = slots_of(ctx), nreads = b.nreads;
   int rc;
-  if ((rc = ensure(ctx, ctx->pk03, (size_t)(w + 4) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->pk03alt, (size_t)(w + 4) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->has_n, nreads))) return rc;
-  if ((rc = ensure(ctx, ctx->flags, (size_t)nreads * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->state, (size_t)nreads * sizeof(ReadState)))) return rc;
-  if ((rc = ensure(ctx, ctx->hit_db, (size_t)nreads * 2))) return rc;
-  if ((rc = ensure(ctx, ctx->aln_work, (size_t)nreads * slots * sizeof(AlnWork)))) return rc;
-  if ((rc = ensure(ctx, ctx->out_aln, (size_t)nreads * slots * sizeof(OutAln)))) return rc;
-  if ((rc = ensure(ctx, ctx->scalars, 512))) return rc;
-  if ((rc = ensure(ctx, ctx->counters, (size_t)(dcCount + 64) * 8))) return rc;
-  CK(cudaMemsetAsync(ctx->pk03.p, 0, (size_t)(w + 4) * 4, ctx->stream));
-  CK(cudaMemsetAsync(ctx->pk03alt.p, 0, (size_t)(w + 4) * 4, ctx->stream));
+  if ((rc = ensure(ctx, b.pk03, (size_t)(w + 4) * 4))) return rc;
+  if ((rc = ensure(ctx, b.pk03alt, (size_t)(w + 4) * 4))) return rc;
+  if ((rc = ensure(ctx, b.has_n, nreads))) return rc;
+  if ((rc = ensure(ctx, b.flags, (size_t)nreads * 4))) return rc;
+  if ((rc = ensure(ctx, b.state, (size_t)nreads * sizeof(ReadState)))) return rc;
+  if ((rc = ensure(ctx, b.hit_db, (size_t)nreads * 2))) return rc;
+  if ((rc = ensure(ctx, b.aln_work, (size_t)nreads * slots * sizeof(AlnWork)))) return rc;
+  if ((rc = ensure(ctx, b.out_aln, (size_t)nreads * slots * sizeof(OutAln)))) return rc;
+  if ((rc = ensure(ctx, b.scalars, 512))) return rc;
+  if ((rc = ensure(ctx, b.counters, (size_t)(dcCount + 64) * 8))) return rc;
+  CK(cudaMemsetAsync(b.pk03.p, 0, (size_t)(w + 4) * 4, ctx->stream));
+  CK(cudaMemsetAsync(b.pk03alt.p, 0, (size_t)(w + 4) * 4, ctx->stream));
   // hit regions are per chunk
   uint64_t max_chunk_nt = 0;
   for (uint32_t c0 = 0; c0 < nreads; c0 += ctx->chunk_reads) {
     const uint32_t c1 = std::min(nreads, c0 + ctx->chunk_reads);
-    max_chunk_nt = std::max<uint64_t>(max_chunk_nt, off32[c1] - off32[c0]);
+    max_chunk_nt = std::max<uint64_t>(max_chunk_nt, b.off32[c1] - b.off32[c0]);
   }
   // one hit-region set per loaded (index,part): all parts are seeded before the candidate kernel runs read-major
   const uint32_t nparts = (uint32_t)std::max<size_t>(1, ctx->parts.size());
-  ctx->cnt_stride = std::min(nreads, ctx->chunk_reads);
-  ctx->hits_stride = (size_t)((uint64_t)ctx->scale * (2 * max_chunk_nt + 32ull * ctx->cnt_stride) + 64);
-  if ((rc = ensure(ctx, ctx->hits, ctx->hits_stride * nparts * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->hit_cnt, (size_t)ctx->cnt_stride * nparts * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->cost, (size_t)ctx->cnt_stride * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->bins, (size_t)ctx->cnt_stride * kCostBins * 4 + (size_t)kCostBins * 4))) return rc;
+  b.cnt_stride = std::min(nreads, ctx->chunk_reads);
+  b.hits_stride = (size_t)((uint64_t)b.scale * (2 * max_chunk_nt + 32ull * b.cnt_stride) + 64);
+  if ((rc = ensure(ctx, b.hits, b.hits_stride * nparts * 8))) return rc;
+  if ((rc = ensure(ctx, b.hit_cnt, (size_t)b.cnt_stride * nparts * 4))) return rc;
+  if ((rc = ensure(ctx, b.cost, (size_t)b.cnt_stride * 4))) return rc;
+  if ((rc = ensure(ctx, b.bins, (size_t)b.cnt_stride * kCostBins * 4 + (size_t)kCostBins * 4))) return rc;
   // 2-bit packing + N detection
-  DevBatch b{};
-  b.nreads = nreads; b.r0 = 0; b.seq04 = (const uint8_t*)ctx->seq04.p; b.seq_off = (const uint32_t*)ctx->seq_off.p;
-  b.pk_off = (const uint32_t*)ctx->pk_off.p;
-  pack_reads_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(b, (uint32_t*)ctx->pk03.p, (uint32_t*)ctx->pk03alt.p, (uint8_t*)ctx->has_n.p);
+  pack_reads_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(make_batch(b, 0, nreads), (uint32_t*)b.pk03.p, (uint32_t*)b.pk03alt.p, (uint8_t*)b.has_n.p);
   CK(cudaGetLastError());
+  return SMR_OK;
+}
+
+// host reads -> the resident batch (no text behind it)
+int upload_batch_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads) {
+  Batch& b = ctx->resident;
+  b.nreads = 0; b.from_text = false; ctx->text_bytes = 0;
+  if (nreads == 0) return SMR_OK;
+  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
+  CK(cudaEventRecord(e0, ctx->stream));
+  uint64_t w = 0;
+  int rc;
+  if ((rc = read_layout(ctx, b, nreads, [&](uint32_t r) { return seq_off[r + 1] - seq_off[r]; }, &w))) return rc;
+  if ((rc = ensure(ctx, b.seq04, b.total_nt + 64))) return rc;
+  CK(cudaMemcpyAsync(b.seq04.p, seq_cat + seq_off[0], b.total_nt, cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = finish_upload(ctx, b, w))) return rc;
+  CK(cudaEventRecord(e1, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_h2d = ms;
   return SMR_OK;
 }
 
@@ -522,7 +547,8 @@ int text_layout(smr_ctx* ctx, const uint8_t* text, uint64_t nbytes, char first_b
 // text == nullptr: the text is already in ctx->d_text (inflated on the device), first byte given
 int upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t* nreads_out, char first_byte = 0) {
   *nreads_out = 0;
-  ctx->nreads = 0;
+  Batch& b = ctx->resident;
+  b.nreads = 0; b.from_text = true;
   ctx->text_bytes = nbytes;
   if (nbytes == 0) return SMR_OK;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
@@ -541,31 +567,30 @@ int upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t*
   if (nreads == 0) return SMR_OK;
   const int grid = ctx->sm_count * 8;
   uint32_t* scal = (uint32_t*)ctx->d_scal.p;   // of text_layout; here [4] packed words [5] max_len
-  if ((rc = ensure(ctx, ctx->seq04, (size_t)total + 64))) return rc;
-  if ((rc = ensure(ctx, ctx->seq_off, (size_t)(nreads + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->pk_off, (size_t)(nreads + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, b.seq04, (size_t)total + 64))) return rc;
+  if ((rc = ensure(ctx, b.seq_off, (size_t)(nreads + 1) * 4))) return rc;
+  if ((rc = ensure(ctx, b.pk_off, (size_t)(nreads + 1) * 4))) return rc;
   if ((rc = ensure(ctx, ctx->d_hdroff, (size_t)nreads * 8))) return rc;
   scatter_lines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)ctx->d_nl.p, L.nlines, (const uint32_t*)ctx->d_hdr.p, (const uint32_t*)ctx->d_rec.p,
-                                                       (const uint32_t*)ctx->d_sb.p, (const uint32_t*)ctx->d_spos.p, (uint8_t*)ctx->seq04.p,
-                                                       (uint32_t*)ctx->seq_off.p, (uint64_t*)ctx->d_hdroff.p);
-  CK(cudaMemcpyAsync((uint32_t*)ctx->seq_off.p + nreads, scal + 2, 4, cudaMemcpyDeviceToDevice, ctx->stream));
-  // packed-word offsets and the longest read (what upload_batch_impl computes on the host); words[nreads] = 0, so pk_off[nreads] is the total
+                                                       (const uint32_t*)ctx->d_sb.p, (const uint32_t*)ctx->d_spos.p, (uint8_t*)b.seq04.p,
+                                                       (uint32_t*)b.seq_off.p, (uint64_t*)ctx->d_hdroff.p);
+  CK(cudaMemcpyAsync((uint32_t*)b.seq_off.p + nreads, scal + 2, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  // packed-word offsets and the longest read (what read_layout computes on the host); words[nreads] = 0, so pk_off[nreads] is the total
   if ((rc = ensure(ctx, ctx->d_cnt, (size_t)(nreads + 1) * 4))) return rc;
-  uint32_t* pk_off = (uint32_t*)ctx->pk_off.p;
-  record_words_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->seq_off.p, nreads, (uint32_t*)ctx->d_cnt.p, scal + 5);
+  uint32_t* pk_off = (uint32_t*)b.pk_off.p;
+  record_words_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)b.seq_off.p, nreads, (uint32_t*)ctx->d_cnt.p, scal + 5);
   if ((rc = exclusive_sum(ctx, (const uint32_t*)ctx->d_cnt.p, pk_off, nreads + 1))) return rc;
   CK(cudaMemcpyAsync(scal + 4, pk_off + nreads, 4, cudaMemcpyDeviceToDevice, ctx->stream));
-  ctx->off32.resize((size_t)nreads + 1);
   if ((rc = ensure(ctx, ctx->h_off32, (size_t)(nreads + 1) * 4))) return rc;
-  CK(cudaMemcpyAsync(ctx->h_off32.p, ctx->seq_off.p, (size_t)(nreads + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h_off32.p, b.seq_off.p, (size_t)(nreads + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream));
   uint32_t h[8];
   CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(e2, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  memcpy(ctx->off32.data(), ctx->h_off32.p, (size_t)(nreads + 1) * 4);
-  ctx->nreads = nreads; ctx->total_nt = total; ctx->max_len = h[5];
-  ctx->h_seq.clear(); ctx->h_off.clear(); ctx->device_only_reads = true;
-  if ((rc = finish_upload(ctx, nreads, h[4]))) return rc;
+  const uint32_t* off32 = (const uint32_t*)ctx->h_off32.p;
+  b.off32.assign(off32, off32 + nreads + 1);
+  b.nreads = nreads; b.total_nt = total; b.max_len = h[5];
+  if ((rc = finish_upload(ctx, b, h[4]))) return rc;
   CK(cudaStreamSynchronize(ctx->stream));
   float ms = 0; cudaEventElapsedTime(&ms, e0, e1); if (text) ctx->t_h2d = ms;
   cudaEventElapsedTime(&ms, e1, e2); ctx->t_decode = ms;
@@ -703,19 +728,6 @@ int inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_b
   return SMR_OK;
 }
 
-DevBatch make_batch(smr_ctx* ctx, uint32_t c0, uint32_t n) {
-  DevBatch b{};
-  b.nreads = n; b.r0 = c0;
-  b.seq04 = (const uint8_t*)ctx->seq04.p; b.seq_off = (const uint32_t*)ctx->seq_off.p;
-  b.pk03 = (const uint32_t*)ctx->pk03.p; b.pk03alt = (const uint32_t*)ctx->pk03alt.p; b.pk_off = (const uint32_t*)ctx->pk_off.p;
-  b.has_n = (const uint8_t*)ctx->has_n.p; b.hit_scale = ctx->scale; b.hits = (uint2*)ctx->hits.p;
-  b.hit_cnt = (uint32_t*)ctx->hit_cnt.p; b.flags = (uint32_t*)ctx->flags.p; b.state = (ReadState*)ctx->state.p;
-  b.hit_db = (uint16_t*)ctx->hit_db.p; b.counters = (unsigned long long*)ctx->counters.p;
-  b.hits_stride = ctx->hits_stride; b.cnt_stride = ctx->cnt_stride; b.cost = (uint32_t*)ctx->cost.p;
-  b.bins = (uint32_t*)ctx->bins.p; b.bin_count = (uint32_t*)ctx->bins.p + (size_t)ctx->cnt_stride * kCostBins;
-  return b;
-}
-
 // Several contexts may share a device (two per GPU let the copies and the host-side result packing of one batch run under the
 // kernels of the other).  Their KERNEL sections are serialised: the candidate kernel is persistent and needs every one of its CTAs
 // resident at once (planner and scorer warps wait for each other), which two such kernels sharing the SMs could not guarantee.
@@ -724,20 +736,20 @@ std::mutex& device_kernel_mutex(int device) {
   return m[device & 63];
 }
 
-// all kernels of one pass over the resident batch
-int run_impl(smr_ctx* ctx) {
+// all kernels of one pass over a batch; its results and times stay in the batch
+int run_impl(smr_ctx* ctx, Batch& bt) {
   if (!ctx->have_params) { ctx->err = "smr_set_params not called"; return SMR_ERR_ARG; }
   if (ctx->parts.empty()) { ctx->err = "no index loaded"; return SMR_ERR_ARG; }
   if (ctx->prm.num_alignments < 0) { ctx->err = "num_alignments < 0"; return SMR_ERR_ARG; }
   if (ctx->prm.minoccur != 0) { ctx->err = "minoccur != 0 is not supported"; return SMR_ERR_UNSUPPORTED; }
-  ctx->t_seed = ctx->t_lis = ctx->t_final = ctx->t_total = 0; ctx->n_launch = 0;
-  ctx->results_spent = false;
-  const uint32_t nreads = ctx->nreads;
+  RunTimes& t = bt.run;
+  t = RunTimes{};
+  const uint32_t nreads = bt.nreads;
   if (nreads == 0) return SMR_OK;
   const uint32_t slots = slots_of(ctx);
   std::lock_guard<std::mutex> dev_lock(device_kernel_mutex(ctx->device));   // held until the stream has drained
   int rc;
-  if ((rc = setup_arenas(ctx))) return rc;
+  if ((rc = setup_arenas(ctx, bt.scale, bt.max_len))) return rc;
   // device copy of the part table (finalize looks parts up by slot)
   std::vector<DevIndex> hp;
   for (size_t i = 0; i < ctx->parts.size(); ++i) {
@@ -747,23 +759,22 @@ int run_impl(smr_ctx* ctx) {
   if ((rc = ensure(ctx, ctx->parts_dev, hp.size() * sizeof(DevIndex)))) return rc;
   CK(cudaMemcpyAsync(ctx->parts_dev.p, hp.data(), hp.size() * sizeof(DevIndex), cudaMemcpyHostToDevice, ctx->stream));
   // cigar pool on the device: generous fixed share per alignment slot
-  ctx->cigar_cap_dev = (uint64_t)nreads * slots * 24 * ctx->scale + 4096;
-  if (ctx->cigar_cap_dev >= 0xFFFFFFFFull) { ctx->err = "CIGAR pool of this batch would pass 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches"; return SMR_ERR_CAPACITY; }
-  if ((rc = ensure(ctx, ctx->cigar_pool, ctx->cigar_cap_dev * 4))) return rc;
-  const Scalars sc = scalars_of(ctx);
-  CK(cudaMemsetAsync(ctx->scalars.p, 0, 512, ctx->stream));
-  CK(cudaMemsetAsync(ctx->counters.p, 0, (size_t)(dcCount + 64) * 8, ctx->stream));
-  CK(cudaMemsetAsync(ctx->state.p, 0, (size_t)nreads * sizeof(ReadState), ctx->stream));
-  CK(cudaMemsetAsync(ctx->flags.p, 0, (size_t)nreads * 4, ctx->stream));
-  CK(cudaMemsetAsync(ctx->hit_db.p, 0xFF, (size_t)nreads * 2, ctx->stream));
+  bt.cigar_cap_dev = (uint64_t)nreads * slots * 24 * bt.scale + 4096;
+  if (bt.cigar_cap_dev >= 0xFFFFFFFFull) { ctx->err = "CIGAR pool of this batch would pass 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches"; return SMR_ERR_CAPACITY; }
+  if ((rc = ensure(ctx, bt.cigar_pool, bt.cigar_cap_dev * 4))) return rc;
+  const Scalars sc = scalars_of(bt);
+  CK(cudaMemsetAsync(bt.scalars.p, 0, 512, ctx->stream));
+  CK(cudaMemsetAsync(bt.counters.p, 0, (size_t)(dcCount + 64) * 8, ctx->stream));
+  CK(cudaMemsetAsync(bt.state.p, 0, (size_t)nreads * sizeof(ReadState), ctx->stream));
+  CK(cudaMemsetAsync(bt.flags.p, 0, (size_t)nreads * 4, ctx->stream));
+  CK(cudaMemsetAsync(bt.hit_db.p, 0xFF, (size_t)nreads * 2, ctx->stream));
   const DevParams dp = to_dev(ctx->prm);
   size_t evi = 2;
   std::vector<std::pair<size_t, int>> spans;   // (event index of start, kind) ; end = start+1
   cudaEvent_t eb = get_event(ctx, evi++); CK(cudaEventRecord(eb, ctx->stream));
   for (uint32_t c0 = 0; c0 < nreads; c0 += ctx->chunk_reads) {
     const uint32_t n = std::min(ctx->chunk_reads, nreads - c0);
-    DevBatch b = make_batch(ctx, c0, n);
-    b.seq_base0 = ctx->off32[c0];
+    DevBatch b = make_batch(bt, c0, n);
     CK(cudaMemsetAsync(sc.work_n, 0, 16, ctx->stream));  // (unused word), the two cursors of the candidate kernel's read schedule, finalize's cursor (zeroed again before it runs)
     CK(cudaMemsetAsync(b.cost, 0, (size_t)n * 4, ctx->stream));
     CK(cudaMemsetAsync(b.bin_count, 0, (size_t)kCostBins * 4, ctx->stream));
@@ -777,7 +788,7 @@ int run_impl(smr_ctx* ctx) {
       if (ctx->instr) seed_kernel<true><<<ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[pi], b, dp, (uint32_t*)ctx->lane_hits.p, ctx->lane_hits_cap, next_read);
       else seed_kernel<false><<<ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[pi], b, dp, (uint32_t*)ctx->lane_hits.p, ctx->lane_hits_cap, next_read);
       CK(cudaGetLastError());
-      ctx->n_launch += 1;
+      t.launches += 1;
     }
     bin_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(b);
     CK(cudaGetLastError());
@@ -787,7 +798,7 @@ int run_impl(smr_ctx* ctx) {
       lg.arena_base = (uint8_t*)ctx->lis_arena.p; lg.arena_stride = ctx->lis_stride;
       lg.hist_cap = ctx->hist_cap; lg.cand_cap = ctx->cand_cap; lg.pair_cap = ctx->pair_cap; lg.row_cap = ctx->row_cap; lg.pall_cap = ctx->pall_cap;
       lg.task_cap = ctx->task_cap;
-      lg.epochs = (uint32_t*)ctx->lis_epochs.p; lg.aln_work = (AlnWork*)ctx->aln_work.p; lg.slots = slots; lg.work_next = sc.lis_next; lg.work_next_b = sc.lis_next_b;
+      lg.epochs = (uint32_t*)ctx->lis_epochs.p; lg.aln_work = (AlnWork*)bt.aln_work.p; lg.slots = slots; lg.work_next = sc.lis_next; lg.work_next_b = sc.lis_next_b;
       lg.parts = (const DevIndex*)ctx->parts_dev.p; lg.nparts = (uint32_t)hp.size();
       lg.ring = (QSlot*)ctx->lis_queue.p; lg.done = (uint32_t*)ctx->lis_done.p; lg.score_rows = (int32_t*)ctx->lis_rows.p;
       lg.dbg = (getenv("SMR_TIMELINE") || getenv("SMR_VERBOSE")) ? (unsigned long long*)ctx->lis_dbg.p : nullptr;   // (the timeline costs the instrumented kernel an atomic per scored pair)
@@ -799,7 +810,7 @@ int run_impl(smr_ctx* ctx) {
       CK(cudaGetLastError());
       CK(cudaEventRecord(s2, ctx->stream));
       spans.push_back({evi - 3, 0});
-      ctx->n_launch += 2;
+      t.launches += 2;
     }
     // finalize this chunk
     CK(cudaMemsetAsync(sc.fin_next, 0, 4, ctx->stream));
@@ -809,8 +820,8 @@ int run_impl(smr_ctx* ctx) {
     FinalGlobals fg{};
     fg.arena_base = (uint8_t*)ctx->final_arena.p; fg.arena_stride = ctx->final_stride;
     fg.cap_w = ctx->cap_w; fg.cap_cig = ctx->cap_cig; fg.row_cap = ctx->row_cap; fg.cap_dir = ctx->cap_dir;
-    fg.parts = (const DevIndex*)ctx->parts_dev.p; fg.aln_work = (const AlnWork*)ctx->aln_work.p; fg.out = (OutAln*)ctx->out_aln.p;
-    fg.slots = slots; fg.cigar_pool = (uint32_t*)ctx->cigar_pool.p; fg.cigar_cap = ctx->cigar_cap_dev; fg.cigar_used = sc.cigar_used;
+    fg.parts = (const DevIndex*)ctx->parts_dev.p; fg.aln_work = (const AlnWork*)bt.aln_work.p; fg.out = (OutAln*)bt.out_aln.p;
+    fg.slots = slots; fg.cigar_pool = (uint32_t*)bt.cigar_pool.p; fg.cigar_cap = bt.cigar_cap_dev; fg.cigar_used = sc.cigar_used;
     fg.work_next = sc.fin_next;
     if ((rc = ensure(ctx, ctx->tb_jobs, (size_t)n * slots * sizeof(TraceJob)))) return rc;
     if ((rc = ensure(ctx, ctx->fin_list, (size_t)n * slots * 4))) return rc;
@@ -819,8 +830,8 @@ int run_impl(smr_ctx* ctx) {
     fg.tb_cap_w = ctx->tb_cap_w; fg.tb_cap_cig = ctx->tb_cap_cig; fg.tb_cap_dir = ctx->tb_cap_dir;
     fg.stats = nullptr;
     if (ctx->host_stats) {
-      if ((rc = ensure(ctx, ctx->aln_stats, (size_t)nreads * slots * sizeof(AlnStats)))) return rc;
-      fg.stats = (AlnStats*)ctx->aln_stats.p;
+      if ((rc = ensure(ctx, bt.aln_stats, (size_t)nreads * slots * sizeof(AlnStats)))) return rc;
+      fg.stats = (AlnStats*)bt.aln_stats.p;
     }
     final_jobs_kernel<<<std::min<uint32_t>((n * slots + 255) / 256, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(b, fg);
     CK(cudaGetLastError());
@@ -828,15 +839,15 @@ int run_impl(smr_ctx* ctx) {
     CK(cudaGetLastError());
     traceback_kernel<<<ctx->tb_threads / 128, 128, 0, ctx->stream>>>(b, dp, fg);
     CK(cudaGetLastError());
-    ctx->n_launch += 2;
+    t.launches += 2;
     CK(cudaEventRecord(f1, ctx->stream));
     spans.push_back({evi - 2, 1});
-    ctx->n_launch += 1;
+    t.launches += 1;
   }
   cudaEvent_t ee = get_event(ctx, evi++); CK(cudaEventRecord(ee, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   float ms = 0;
-  cudaEventElapsedTime(&ms, eb, ee); ctx->t_total = ms;
+  cudaEventElapsedTime(&ms, eb, ee); t.total = ms;
   if (getenv("SMR_VERBOSE")) {
     unsigned long long d[16]; cudaMemcpy(d, ctx->lis_dbg.p, 128, cudaMemcpyDeviceToHost);
     fprintf(stderr, "[smr] slowest read %llu: %.2f ms; cycles vote %llu order %llu group %llu plan %llu wait %llu replay %llu; sw calls %llu, tasks scored %llu, rounds %llu\n", d[10], d[0] / 1.965e6, d[1], d[2], d[3], d[4], d[5], d[6], d[7], d[8], d[9]);
@@ -854,9 +865,9 @@ int run_impl(smr_ctx* ctx) {
   }
   for (auto& s : spans) {
     if (s.second == 0) {
-      cudaEventElapsedTime(&ms, ctx->ev[s.first], ctx->ev[s.first + 1]); ctx->t_seed += ms;
-      cudaEventElapsedTime(&ms, ctx->ev[s.first + 1], ctx->ev[s.first + 2]); ctx->t_lis += ms;
-    } else { cudaEventElapsedTime(&ms, ctx->ev[s.first], ctx->ev[s.first + 1]); ctx->t_final += ms; }
+      cudaEventElapsedTime(&ms, ctx->ev[s.first], ctx->ev[s.first + 1]); t.seed += ms;
+      cudaEventElapsedTime(&ms, ctx->ev[s.first + 1], ctx->ev[s.first + 2]); t.lis += ms;
+    } else { cudaEventElapsedTime(&ms, ctx->ev[s.first], ctx->ev[s.first + 1]); t.final += ms; }
   }
   return SMR_OK;
 }
@@ -873,9 +884,9 @@ int pool_short_error(smr_ctx* ctx, const HostOut& out) {
   return SMR_ERR_CAPACITY;
 }
 
-// copies results of the resident batch to the host; returns the indices of reads whose scratch overflowed
-int download_impl(smr_ctx* ctx, HostOut& out, std::vector<uint32_t>& flagged, const uint32_t* map /*local->caller index or null*/) {
-  const uint32_t n = ctx->nreads;
+// copies the results of a batch's run to the host; returns the indices of reads whose scratch overflowed
+int download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint32_t>& flagged, const uint32_t* map /*local->caller index or null*/) {
+  const uint32_t n = b.nreads;
   flagged.clear();
   if (n == 0) return SMR_OK;
   const uint32_t slots = slots_of(ctx);
@@ -892,21 +903,21 @@ int download_impl(smr_ctx* ctx, HostOut& out, std::vector<uint32_t>& flagged, co
   if (ctx->host_stats) {
     if ((prc = ensure(ctx, ctx->h_stats, (size_t)n * slots * sizeof(AlnStats)))) return prc;
     ast = (const AlnStats*)ctx->h_stats.p;
-    CK(cudaMemcpyAsync(ctx->h_stats.p, ctx->aln_stats.p, (size_t)n * slots * sizeof(AlnStats), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->h_stats.p, b.aln_stats.p, (size_t)n * slots * sizeof(AlnStats), cudaMemcpyDeviceToHost, ctx->stream));
   }
   unsigned long long used = 0;
   std::vector<unsigned long long> cnt(dcCount + 64);
-  CK(cudaMemcpyAsync(ctx->h_state.p, ctx->state.p, (size_t)n * sizeof(ReadState), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->h_flags.p, ctx->flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->h_hitdb.p, ctx->hit_db.p, (size_t)n * 2, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->h_outaln.p, ctx->out_aln.p, (size_t)n * slots * sizeof(OutAln), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(&used, scalars_of(ctx).cigar_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(cnt.data(), ctx->counters.p, cnt.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h_state.p, b.state.p, (size_t)n * sizeof(ReadState), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h_flags.p, b.flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h_hitdb.p, b.hit_db.p, (size_t)n * 2, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h_outaln.p, b.out_aln.p, (size_t)n * slots * sizeof(OutAln), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&used, scalars_of(b).cigar_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(cnt.data(), b.counters.p, cnt.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  used = std::min<unsigned long long>(used, ctx->cigar_cap_dev);
+  used = std::min<unsigned long long>(used, b.cigar_cap_dev);
   if ((prc = ensure(ctx, ctx->h_cigar, (size_t)used * 4 + 16))) return prc;
   const uint32_t* cig = (const uint32_t*)ctx->h_cigar.p;
-  if (used) CK(cudaMemcpyAsync(ctx->h_cigar.p, ctx->cigar_pool.p, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  if (used) CK(cudaMemcpyAsync(ctx->h_cigar.p, b.cigar_pool.p, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(e1, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_d2h = ms;
@@ -983,32 +994,49 @@ int download_impl(smr_ctx* ctx, HostOut& out, std::vector<uint32_t>& flagged, co
   return rc;
 }
 
-// align a host batch, retrying reads whose scratch overflowed with a larger scale
-int align_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads, HostOut& out, const uint32_t* map, int depth) {
-  int rc = upload_batch_impl(ctx, seq_cat, seq_off, nreads, false);
-  if (rc) return rc;
-  const double h2d = ctx->t_h2d;
-  if ((rc = run_impl(ctx))) return rc;
-  std::vector<uint32_t> flagged;
-  if ((rc = download_impl(ctx, out, flagged, map))) return rc;
-  ctx->t_h2d = h2d;
-  if (flagged.empty()) return SMR_OK;
-  if (getenv("SMR_VERBOSE")) fprintf(stderr, "[smr] %zu reads overflowed their scratch at scale %u: retrying with scale %u (causes so far: lane %llu region %llu pairs %llu trace %llu cigar %llu err %llu)\n", flagged.size(), ctx->scale, ctx->scale * 8,
+// Runs the flagged reads of a failed batch again as a batch of their own with 8x its scratch, gathered from its reads on the device,
+// and downloads them into the caller's arrays after what is there (map: index in `failed` -> the caller's index; null = the same).
+// Reads that overflow again go on to 64x and 512x.  The batch frees itself on return.
+int retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t>& flagged, const uint32_t* map, HostOut& out, int depth) {
+  if (getenv("SMR_VERBOSE")) fprintf(stderr, "[smr] %zu reads overflowed their scratch at scale %u: retrying with scale %u (causes so far: lane %llu region %llu pairs %llu trace %llu cigar %llu err %llu)\n", flagged.size(), failed.scale, failed.scale * 8,
       (unsigned long long)ctx->flag_hist[0], (unsigned long long)ctx->flag_hist[1], (unsigned long long)ctx->flag_hist[2], (unsigned long long)ctx->flag_hist[3], (unsigned long long)ctx->flag_hist[4], (unsigned long long)ctx->flag_hist[5]);
   if (depth >= 3) { ctx->err = "scratch overflow persists after 3 retries (" + std::to_string(flagged.size()) + " reads)"; return SMR_ERR_CAPACITY; }
-  // sub-batch of the flagged reads, 8x the scratch
-  std::vector<uint8_t> sseq; std::vector<uint64_t> soff(1, 0); std::vector<uint32_t> smap;
-  for (uint32_t r : flagged) {
-    sseq.insert(sseq.end(), seq_cat + seq_off[r], seq_cat + seq_off[r + 1]);
-    soff.push_back(sseq.size());
-    smap.push_back(map ? map[r] : r);
+  const uint32_t n = (uint32_t)flagged.size();
+  std::vector<uint32_t> src(n), smap(n);
+  for (uint32_t k = 0; k < n; ++k) { src[k] = failed.off32[flagged[k]]; smap[k] = map ? map[flagged[k]] : flagged[k]; }
+  Batch b;
+  b.scale = failed.scale * 8;
+  uint64_t w = 0;
+  int rc;
+  if ((rc = read_layout(ctx, b, n, [&](uint32_t k) { return failed.off32[flagged[k] + 1] - src[k]; }, &w))) return rc;
+  DevBuf d_src;
+  CK(d_src.alloc((size_t)n * 4));
+  CK(cudaMemcpyAsync(d_src.p, src.data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+  if ((rc = ensure(ctx, b.seq04, b.total_nt + 64))) return rc;
+  gather_reads_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
+      (const uint8_t*)failed.seq04.p, (const uint32_t*)d_src.p, n, (const uint32_t*)b.seq_off.p, (uint8_t*)b.seq04.p);
+  CK(cudaGetLastError());
+  if ((rc = finish_upload(ctx, b, w)) || (rc = run_impl(ctx, b))) return rc;
+  const double d2h = ctx->t_d2h;
+  std::vector<uint32_t> again;
+  rc = download_impl(ctx, b, out, again, smap.data());
+  ctx->t_run += b.run; ctx->t_d2h += d2h;
+  if (rc || again.empty()) return rc;
+  return retry_flagged(ctx, b, again, smap.data(), out, depth + 1);
+}
+
+// the results of the resident batch's last run into the caller's arrays, its flagged reads retried; the resident batch and its
+// device results stay as they are
+int download_resident(smr_ctx* ctx, HostOut& out) {
+  ctx->t_run = ctx->resident.run;
+  std::vector<uint32_t> flagged;
+  int rc = download_impl(ctx, ctx->resident, out, flagged, nullptr);
+  if (rc == SMR_OK && !flagged.empty()) {
+    rc = retry_flagged(ctx, ctx->resident, flagged, nullptr, out, 0);
+    // the arenas grew with the retry's scale (after 64x, tens of GB): the next run allocates them again at its own
+    for (DevBuf* s : {&ctx->lis_arena, &ctx->final_arena, &ctx->tb_arena, &ctx->lane_hits}) s->reset();
   }
-  const uint32_t old_scale = ctx->scale;
-  const double tt = ctx->t_total, ts = ctx->t_seed, tl = ctx->t_lis, tf = ctx->t_final, td = ctx->t_d2h; const uint64_t nl = ctx->n_launch;
-  ctx->scale = old_scale * 8;
-  rc = align_impl(ctx, sseq.data(), soff.data(), (uint32_t)flagged.size(), out, smap.data(), depth + 1);
-  ctx->scale = old_scale;
-  ctx->t_total += tt; ctx->t_seed += ts; ctx->t_lis += tl; ctx->t_final += tf; ctx->t_d2h += td; ctx->t_h2d += h2d; ctx->n_launch += nl;
+  if (rc == SMR_OK && out.pool_short) rc = pool_short_error(ctx, out);
   return rc;
 }
 
@@ -1667,9 +1695,9 @@ int smr_align_batch(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_of
   memset(results, 0, (size_t)nreads * sizeof(smr_read_result));
   memset(alns, 0, (size_t)nreads * slots * sizeof(smr_aln));
   HostOut out{results, alns, cigar_pool, cigar_cap, 0, counters, n_counters};
-  ctx->scale = 1;
-  int rc = align_impl(ctx, seq_cat, seq_off, nreads, out, nullptr, 0);
-  if (rc == SMR_OK && out.pool_short) rc = pool_short_error(ctx, out);
+  int rc = upload_batch_impl(ctx, seq_cat, seq_off, nreads);
+  if (rc == SMR_OK) rc = run_impl(ctx, ctx->resident);
+  if (rc == SMR_OK) rc = download_resident(ctx, out);
   if (cigar_used) *cigar_used = out.cigar_used;
   return rc;
 } SMR_CATCH(ctx)
@@ -1689,22 +1717,19 @@ int smr_set_stats_buffer(smr_ctx* ctx, smr_aln_stats* stats) {
 int smr_upload_batch(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads) try {
   if (!ctx || !seq_cat || !seq_off) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  ctx->scale = 1;
-  return upload_batch_impl(ctx, seq_cat, seq_off, nreads, true);
+  return upload_batch_impl(ctx, seq_cat, seq_off, nreads);
 } SMR_CATCH(ctx)
 
 int smr_upload_fastx(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t* nreads) try {
   if (!ctx || (!text && nbytes) || !nreads) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  ctx->scale = 1;
   return upload_fastx_impl(ctx, text, nbytes, nreads);
 } SMR_CATCH(ctx)
 
 int smr_upload_fastx_gz(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint32_t* nreads) try {
   if (!ctx || !gz || !nreads) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  ctx->scale = 1;
-  *nreads = 0; ctx->nreads = 0; ctx->text_bytes = 0;
+  *nreads = 0; ctx->resident.nreads = 0; ctx->text_bytes = 0;
   uint64_t total = 0;
   const char* e = getenv("SMR_INFLATE_CHUNK");
   // distance of the speculative block searches: 64 KB for large files, down to 8 KB so that a small file still makes thousands of spans
@@ -1730,7 +1755,7 @@ int smr_resident_text(smr_ctx* ctx, char* text, uint64_t cap, uint64_t* nbytes) 
 int smr_debug_inflate(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_bytes, uint32_t info[4]) try {
   if (!ctx || !gz || !out_bytes) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  ctx->nreads = 0; ctx->text_bytes = 0;
+  ctx->resident.nreads = 0; ctx->text_bytes = 0;
   if (chunk_bytes == 0) chunk_bytes = std::min<uint64_t>(65536, std::max<uint64_t>(8192, nbytes / 8192));   // as smr_upload_fastx_gz
   int rc = inflate_impl(ctx, gz, nbytes, chunk_bytes, out_bytes);
   if (rc) return rc;
@@ -1745,15 +1770,16 @@ int smr_debug_inflate(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t ch
 int smr_resident_layout(smr_ctx* ctx, uint64_t* header_text_off, uint64_t* read_off, uint8_t* seq04, uint64_t seq_cap) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  const uint32_t n = ctx->nreads;
-  if (read_off) for (uint32_t r = 0; r <= n; ++r) read_off[r] = n ? ctx->off32[r] : 0;
+  const Batch& b = ctx->resident;
+  const uint32_t n = b.nreads;
+  if (read_off) for (uint32_t r = 0; r <= n; ++r) read_off[r] = n ? b.off32[r] : 0;
   if (header_text_off && n) {
-    if (!ctx->device_only_reads) { ctx->err = "the resident batch was not uploaded as text"; return SMR_ERR_ARG; }
+    if (!b.from_text) { ctx->err = "the resident batch was not uploaded as text"; return SMR_ERR_ARG; }
     CK(cudaMemcpy(header_text_off, ctx->d_hdroff.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
   }
   if (seq04 && n) {
-    if (seq_cap < ctx->total_nt) { ctx->err = "sequence buffer too small"; return SMR_ERR_CAPACITY; }
-    CK(cudaMemcpy(seq04, ctx->seq04.p, ctx->total_nt, cudaMemcpyDeviceToHost));
+    if (seq_cap < b.total_nt) { ctx->err = "sequence buffer too small"; return SMR_ERR_CAPACITY; }
+    CK(cudaMemcpy(seq04, b.seq04.p, b.total_nt, cudaMemcpyDeviceToHost));
   }
   return SMR_OK;
 } SMR_CATCH(ctx)
@@ -1761,49 +1787,21 @@ int smr_resident_layout(smr_ctx* ctx, uint64_t* header_text_off, uint64_t* read_
 int smr_run_resident(smr_ctx* ctx) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  return run_impl(ctx);
+  const int rc = run_impl(ctx, ctx->resident);
+  ctx->t_run = ctx->resident.run;
+  return rc;
 } SMR_CATCH(ctx)
 
 int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used,
                          uint64_t* counters, uint32_t n_counters) try {
   if (!ctx || !results || !alns) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  if (ctx->results_spent) { ctx->err = "the results of the last run were replaced by the retry of a download: smr_run_resident again"; return SMR_ERR_ARG; }
   const uint32_t slots = slots_of(ctx);
-  const uint32_t n = ctx->nreads;
+  const uint32_t n = ctx->resident.nreads;
   memset(results, 0, (size_t)n * sizeof(smr_read_result));
   memset(alns, 0, (size_t)n * slots * sizeof(smr_aln));
   HostOut out{results, alns, cigar_pool, cigar_cap, 0, counters, n_counters};
-  std::vector<uint32_t> flagged;
-  int rc = download_impl(ctx, out, flagged, nullptr);
-  if (rc == SMR_OK && !flagged.empty()) {
-    if (getenv("SMR_VERBOSE")) fprintf(stderr, "[smr] %zu reads overflowed their scratch (resident batch): retrying with scale 8 (causes so far: lane %llu region %llu pairs %llu trace %llu cigar %llu err %llu)\n", flagged.size(),
-      (unsigned long long)ctx->flag_hist[0], (unsigned long long)ctx->flag_hist[1], (unsigned long long)ctx->flag_hist[2], (unsigned long long)ctx->flag_hist[3], (unsigned long long)ctx->flag_hist[4], (unsigned long long)ctx->flag_hist[5]);
-    // redo the overflowed reads from the retained host copy with larger scratch
-    const bool device_only = ctx->device_only_reads;
-    if (device_only) {   // decoded on the device: fetch the sequences now (only when a retry is needed)
-      ctx->h_seq.resize(ctx->total_nt);
-      CK(cudaMemcpy(ctx->h_seq.data(), ctx->seq04.p, ctx->total_nt, cudaMemcpyDeviceToHost));
-      ctx->h_off.assign(ctx->off32.begin(), ctx->off32.end());
-    }
-    std::vector<uint8_t> hs; std::vector<uint64_t> ho;
-    hs.swap(ctx->h_seq); ho.swap(ctx->h_off);
-    std::vector<uint8_t> sseq; std::vector<uint64_t> soff(1, 0);
-    for (uint32_t r : flagged) { sseq.insert(sseq.end(), hs.begin() + ho[r], hs.begin() + ho[r + 1]); soff.push_back(sseq.size()); }
-    ctx->scale = 8;
-    rc = align_impl(ctx, sseq.data(), soff.data(), (uint32_t)flagged.size(), out, flagged.data(), 1);
-    ctx->scale = 1;
-    // the retry made its sub-batch the resident batch: upload the original reads again, so that the resident batch is the one
-    // uploaded (read offsets, sequences; the text, header offsets and host copy stay as the upload left them) and the next
-    // smr_run_resident / smr_resident_layout see it.  Only a download that retried pays for this copy.
-    const double h2d = ctx->t_h2d;
-    const int up = upload_batch_impl(ctx, hs.data(), ho.data(), n, !device_only);
-    ctx->t_h2d = h2d;
-    ctx->device_only_reads = device_only;
-    if (rc == SMR_OK) rc = up;
-    ctx->results_spent = true;   // (the retry's run overwrote the device results: a second download needs a new run)
-  }
-  if (rc == SMR_OK && out.pool_short) rc = pool_short_error(ctx, out);
+  const int rc = download_resident(ctx, out);
   if (cigar_used) *cigar_used = out.cigar_used;
   return rc;
 } SMR_CATCH(ctx)
@@ -1904,8 +1902,8 @@ int smr_last_report_timings(const smr_ctx* ctx, double out[3]) {
 
 int smr_last_timings(const smr_ctx* ctx, double out[8]) {
   if (!ctx || !out) return SMR_ERR_ARG;
-  out[0] = ctx->t_total; out[1] = ctx->t_seed; out[2] = ctx->t_lis; out[3] = ctx->t_final; out[4] = ctx->t_h2d; out[5] = ctx->t_d2h;
-  out[6] = (double)ctx->n_launch; out[7] = ctx->t_decode;
+  out[0] = ctx->t_run.total; out[1] = ctx->t_run.seed; out[2] = ctx->t_run.lis; out[3] = ctx->t_run.final; out[4] = ctx->t_h2d; out[5] = ctx->t_d2h;
+  out[6] = (double)ctx->t_run.launches; out[7] = ctx->t_decode;
   return SMR_OK;
 }
 

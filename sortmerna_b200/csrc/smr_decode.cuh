@@ -124,4 +124,15 @@ __global__ void record_words_kernel(const uint32_t* __restrict__ seq_off, uint32
   if ((threadIdx.x & 31) == 0 && m) atomicMax(max_len, m);
 }
 
+// one warp per read: n reads of the 0-4 codes `src`, read k starting at src_off[k], copied to dst at dst_off[k] (dst_off[k + 1] -
+// dst_off[k] codes each); gathers the flagged reads of a batch into the batch of their scratch-overflow retry
+__global__ void __launch_bounds__(256) gather_reads_kernel(const uint8_t* __restrict__ src, const uint32_t* __restrict__ src_off, uint32_t n,
+                                                           const uint32_t* __restrict__ dst_off, uint8_t* __restrict__ dst) {
+  const uint32_t warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
+  for (uint32_t k = warp; k < n; k += nwarps) {
+    const uint32_t s = src_off[k], o = dst_off[k], len = dst_off[k + 1] - o;
+    for (uint32_t i = lane_id(); i < len; i += 32) dst[o + i] = src[s + i];
+  }
+}
+
 }  // namespace smr

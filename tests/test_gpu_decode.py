@@ -93,6 +93,18 @@ def test_alignment_of_decoded_batch_equals_host_parsed(aligner, golden):
     assert got["counters"]["num_aligned"] == want["counters"]["num_aligned"]
 
 
+def test_upload_clears_the_resident_text(aligner, golden):
+    """reads uploaded from host arrays have no text behind them: the text of an earlier upload_fastx is gone, so reports of the
+    new batch cannot be formatted against it"""
+    b = golden["batch"]
+    aligner.upload_fastx(open(os.path.join(GOLDEN, "reads_mix.fq"), "rb").read())
+    aligner.upload(b.cat, b.off)
+    assert aligner.resident_text() == b""
+    res = aligner.align(b.cat, b.off, with_stats=True)
+    with pytest.raises(api.SmrError, match="no resident text"):
+        aligner.format_reports(res, None, sam=True)
+
+
 def test_decode_bundled_set2_and_throughput(aligner, tmp_path):
     # shaped like the reference's data/set2_environmental_study_550_amplicon.fasta: 100 000 amplicons of 150-250 nt
     rng = np.random.default_rng(550)

@@ -341,7 +341,8 @@ def test_heavy_batch_needs_a_larger_host_pool(inputs):
 # -------------------------------------------------------------------------------------------------------------------------
 
 CAUSES = ("lane", "region", "pairs", "trace", "cigar", "err")
-_LOG = re.compile(r"\[smr\] (\d+) reads overflowed their scratch (?:at scale (\d+)|\(resident batch\)): retrying with scale (\d+) "
+WORK_COUNTERS = ("num_aligned", "num_short", "sw_calls", "sw_cells", "pos_entries", "lis_calls")   # the counters the reference reports
+_LOG = re.compile(r"\[smr\] (\d+) reads overflowed their scratch at scale (\d+): retrying with scale (\d+) "
                   r"\(causes so far: lane (\d+) region (\d+) pairs (\d+) trace (\d+) cigar (\d+) err (\d+)\)")
 
 
@@ -437,9 +438,10 @@ def test_retry_with_one_index_file_each(inputs, monkeypatch, capfd):
 
 @pytest.mark.gpu
 @pytest.mark.parametrize("source", ["batch", "fastx", "fastx_gz"])
-def test_resident_path_retry_keeps_the_batch(inputs, source, monkeypatch, capfd):
+def test_resident_path_retry_keeps_the_batch_and_its_results(inputs, source, monkeypatch, capfd):
     """upload / upload_fastx / upload_fastx_gz, run_resident + download == the host path; then, without uploading again, the
-    resident batch is the one uploaded (layout, report text) and a second run + download gives the same answer"""
+    resident batch is the one uploaded (layout, report text), a second download with no run between gives the same answer, and
+    so does a second run + download"""
     names = ["swarm", "neigh"]
     monkeypatch.setenv("SMR_VERBOSE", "1")
     capfd.readouterr()
@@ -466,8 +468,11 @@ def test_resident_path_retry_keeps_the_batch(inputs, source, monkeypatch, capfd)
     if source != "batch":
         assert a.resident_text() == text
         assert a.format_reports(first, None, sam=True, fastx=True, other=True) == a.format_reports(first, text, sam=True, fastx=True, other=True)
-    with pytest.raises(api.SmrError, match="smr_run_resident again"):   # the retry's run replaced the device results
-        a.download()
+    again = a.download()   # the retry ran in a batch of its own: the device results of the run are still there
+    assert_same_results(again, first, source + " download again")
+    assert np.array_equal(again["stats"], first["stats"]) and again["matched"].tolist() == first["matched"].tolist()
+    assert np.array_equal(again["cigar"], first["cigar"])
+    assert {k: again["counters"][k] for k in WORK_COUNTERS} == {k: first["counters"][k] for k in WORK_COUNTERS}
     a.run_resident(with_stats=True)
     second = a.download()
     assert_same_results(second, first, source + " second download")
@@ -534,4 +539,39 @@ def test_host_pool_too_small_names_the_size(inputs, monkeypatch, capfd):
     assert res["cigar"].size == need
     assert_same_results(res, got, "heavy, download")
     assert np.array_equal(res["stats"], got["stats"]) and res["matched"].tolist() == got["matched"].tolist()
+    a.close()
+
+
+def _download_raw(a, n, cap):
+    """smr_download_results of the resident batch into a host pool of `cap` words: ((status, *cigar_used), the result dict)"""
+    slots, res, alns, _, _, counters = a._outputs(n)
+    pool = np.zeros(max(cap, 1), np.uint32)
+    used = api.C.c_uint64(0)
+    rc = a.L.smr_download_results(a.h, api._ptr(res), api._ptr(alns), api._ptr(pool), api.C.c_uint64(cap), api.C.byref(used),
+                                  api._ptr(counters), api.C.c_uint32(counters.size))
+    return (rc, int(used.value)), a._pack(res, alns, pool, int(used.value), counters, slots)
+
+
+@pytest.mark.gpu
+def test_download_again_into_a_larger_pool(inputs, monkeypatch, capfd):
+    """One run of the CIGAR-heavy batch, then three downloads with no run between: a host pool too small names the words needed
+    (counted across the retry, which every download runs again), and the download into a pool of that size equals align()."""
+    names = ["neigh"]
+    monkeypatch.setenv("SMR_VERBOSE", "1")
+    b = inputs["heavy_batch"]
+    a = _aligner(inputs, names)
+    want = a.align(b.cat, b.off)
+    need = want["cigar"].size
+    a.upload(b.cat, b.off)
+    a.run_resident()
+    capfd.readouterr()
+    assert _download_raw(a, b.n, 1000)[0] == (5, need)
+    assert _download_raw(a, b.n, need - 1)[0] == (5, need)
+    status, got = _download_raw(a, b.n, need)
+    causes, scales = _collect(capfd)
+    assert status == (0, need)
+    assert causes["trace"] > 0 and 8 in scales, causes
+    assert_same_results(got, want, "heavy, third download")   # (which reads fill the device CIGAR pool first, and so are retried,
+    assert got["matched"].tolist() == want["matched"].tolist()   # varies from run to run: so does the order of the host pool)
+    assert got["counters"]["num_aligned"] == want["counters"]["num_aligned"]
     a.close()
