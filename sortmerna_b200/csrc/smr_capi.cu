@@ -137,69 +137,74 @@ struct smr_ctx {
 
 namespace {
 
+// A failed call inside the library: the status and the smr_last_error text its entry point returns (SMR_CATCH).  Not a
+// std::exception, so that only its own catch clause takes it.
+struct Failure { int code; std::string msg; };
+[[noreturn]] void fail(int code, std::string msg) { throw Failure{code, std::move(msg)}; }
+
 #define CK(call)                                                                                   \
   do {                                                                                             \
     cudaError_t e_ = (call);                                                                       \
-    if (e_ != cudaSuccess) {                                                                       \
-      ctx->err = std::string(#call) + ": " + cudaGetErrorString(e_);                               \
-      return SMR_ERR_CUDA;                                                                         \
-    }                                                                                              \
+    if (e_ != cudaSuccess) fail(SMR_ERR_CUDA, std::string(#call) + ": " + cudaGetErrorString(e_)); \
   } while (0)
+
+// runs f when it leaves its scope, by return or by a throw
+template <class F>
+struct OnExit { F f; ~OnExit() { f(); } };
+template <class F>
+OnExit<F> on_exit(F f) { return OnExit<F>{f}; }
 
 // alignment slots per read in every flat result array: num_alignments, or the stride set for "all alignments" (0)
 uint32_t slots_of(const smr_ctx* ctx) { return ctx->prm.num_alignments > 0 ? (uint32_t)ctx->prm.num_alignments : std::max(1u, ctx->all_slots); }
 
 // grow-only: at least `bytes`; what the buffer held is not kept
-template <bool kPinned>
-int ensure(smr_ctx* ctx, Buf<kPinned>& b, size_t bytes) {
-  if (bytes <= b.cap && b.p) return SMR_OK;
-  CK(b.alloc(bytes + bytes / 8 + 256));
-  return SMR_OK;
+template <class T = void, bool kPinned>
+T* ensure(Buf<kPinned>& b, size_t bytes) {
+  if (bytes > b.cap || !b.p) CK(b.alloc(bytes + bytes / 8 + 256));
+  return (T*)b.p;
 }
 
 // a device array of the part: n items, copied from src (host) or else zero, and 64 zero bytes of slack past the end; counted in pt.bytes
 template <class T>
-int part_array(smr_ctx* ctx, Part& pt, size_t n, const void* src, T** out) {
+T* part_array(smr_ctx* ctx, Part& pt, size_t n, const void* src) {
   const size_t bytes = n * sizeof(T);
   DevBuf b;
   CK(b.alloc(bytes + 64));
   CK(cudaMemsetAsync(b.p, 0, bytes + 64, ctx->stream));
   if (src && bytes) CK(cudaMemcpyAsync(b.p, src, bytes, cudaMemcpyHostToDevice, ctx->stream));
-  *out = (T*)b.p;
+  T* out = (T*)b.p;
   pt.bytes += bytes + 64;
   pt.owned.push_back(std::move(b));
-  return SMR_OK;
+  return out;
 }
 
 // device scratch of one call: n items of T (at least one) in a new buffer of `pool`, freed with it
 template <class T>
-cudaError_t scratch(std::vector<DevBuf>& pool, size_t n, T** out) {
+T* scratch(std::vector<DevBuf>& pool, size_t n) {
   pool.emplace_back();
-  const cudaError_t e = pool.back().alloc(std::max<size_t>(n, 1) * sizeof(T));
-  *out = (T*)pool.back().p;
-  return e;
+  CK(pool.back().alloc(std::max<size_t>(n, 1) * sizeof(T)));
+  return (T*)pool.back().p;
 }
 
 // one cub device call, run twice: with no scratch to size it, then in `tmp` (grown as needed).  call(void* tmp, size_t& bytes).
 template <class F>
-int cub_run(smr_ctx* ctx, DevBuf& tmp, F&& call) {
+void cub_run(DevBuf& tmp, F&& call) {
   size_t bytes = 0;
   CK(call(nullptr, bytes));
-  if (int rc = ensure(ctx, tmp, bytes)) return rc;
+  ensure(tmp, bytes);
   CK(call(tmp.p, bytes));
-  return SMR_OK;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // index build on the device (smr_build_dev.cuh): orchestration of one part
 // ---------------------------------------------------------------------------------------------------------------------
 
-int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const std::vector<size_t>& members, const BuildOptions& opt, Part& pt) {
+Part build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const std::vector<size_t>& members, const BuildOptions& opt) {
   BuildGeom g{};
   g.L = opt.lnwin; g.half = g.L / 2; g.pread = g.L + 1; g.interval = opt.interval; g.max_pos = opt.max_pos; g.burst_depth = g.pread - g.half - 3;
   g.nseq = (uint32_t)members.size();
   const uint32_t list_bits = 2 * g.half + 1, key_bits = list_bits + 2 * g.burst_depth;
-  if (key_bits > 64 || 2 * g.pread > 62 || 2 * (g.half + 1) > 32) { ctx->err = "seed length too large for the device builder"; return SMR_ERR_UNSUPPORTED; }
+  if (key_bits > 64 || 2 * g.pread > 62 || 2 * (g.half + 1) > 32) fail(SMR_ERR_UNSUPPORTED, "seed length too large for the device builder");
   // host: concatenated builder codes + 0..4 codes, offsets, first window of every sequence
   std::vector<uint64_t> soff(g.nseq + 1, 0);
   std::vector<uint32_t> wstart(g.nseq + 1, 0);
@@ -208,10 +213,10 @@ int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const st
     const size_t len = recs[members[k]].seq.size();
     soff[k + 1] = soff[k] + len;
     total_win += (len - g.pread + g.interval) / g.interval;
-    if (total_win >= (1ull << 31)) { ctx->err = "more than 2^31 windows in one index part"; return SMR_ERR_UNSUPPORTED; }
+    if (total_win >= (1ull << 31)) fail(SMR_ERR_UNSUPPORTED, "more than 2^31 windows in one index part");
     wstart[k + 1] = (uint32_t)total_win;
   }
-  if (soff[g.nseq] >= 0xFFFFFFFFull) { ctx->err = "reference part larger than 4 GB"; return SMR_ERR_UNSUPPORTED; }
+  if (soff[g.nseq] >= 0xFFFFFFFFull) fail(SMR_ERR_UNSUPPORTED, "reference part larger than 4 GB");
   g.nwin = (uint32_t)total_win;
   std::vector<uint8_t> codes(soff[g.nseq]), c04(soff[g.nseq] + 64, 4);
   for (uint32_t k = 0; k < g.nseq; ++k) {
@@ -225,15 +230,15 @@ int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const st
   cudaStream_t st = ctx->stream;
   const uint32_t n = g.nwin;
   const unsigned tb = 256, gw = (n + tb - 1) / tb;
-  int rc;
-  uint8_t* d_codes; uint64_t* d_soff; uint32_t* d_wstart;
-  CK(scratch(tmp, codes.size() + 64, &d_codes)); CK(scratch(tmp, soff.size(), &d_soff)); CK(scratch(tmp, wstart.size(), &d_wstart));
+  uint8_t* d_codes = scratch<uint8_t>(tmp, codes.size() + 64);
+  uint64_t* d_soff = scratch<uint64_t>(tmp, soff.size());
+  uint32_t* d_wstart = scratch<uint32_t>(tmp, wstart.size());
   CK(cudaMemcpyAsync(d_codes, codes.data(), codes.size(), cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_soff, soff.data(), soff.size() * 8, cudaMemcpyHostToDevice, st));
   CK(cudaMemcpyAsync(d_wstart, wstart.data(), wstart.size() * 4, cudaMemcpyHostToDevice, st));
-  uint64_t *keyA, *keyB; uint32_t *valA, *valB, *u0, *u1, *u2, *u3, *win_id;
-  CK(scratch(tmp, n, &keyA)); CK(scratch(tmp, n, &keyB)); CK(scratch(tmp, n, &valA)); CK(scratch(tmp, n, &valB));
-  CK(scratch(tmp, n, &u0)); CK(scratch(tmp, n, &u1)); CK(scratch(tmp, n, &u2)); CK(scratch(tmp, n, &u3)); CK(scratch(tmp, n, &win_id));
+  uint64_t *keyA = scratch<uint64_t>(tmp, n), *keyB = scratch<uint64_t>(tmp, n);
+  uint32_t *valA = scratch<uint32_t>(tmp, n), *valB = scratch<uint32_t>(tmp, n), *u0 = scratch<uint32_t>(tmp, n), *u1 = scratch<uint32_t>(tmp, n),
+           *u2 = scratch<uint32_t>(tmp, n), *u3 = scratch<uint32_t>(tmp, n), *win_id = scratch<uint32_t>(tmp, n);
   // cub scratch, sized exactly for the largest call (entries: at most 2n), so that cub_run never grows it
   size_t cub_bytes = 0, need = 0;
   cub::DeviceRadixSort::SortPairs(nullptr, need, (uint64_t*)nullptr, (uint64_t*)nullptr, (uint32_t*)nullptr, (uint32_t*)nullptr, 2 * (size_t)n, 0, 64, st); cub_bytes = std::max(cub_bytes, need);
@@ -244,68 +249,71 @@ int build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const st
   // 1. windows sorted by value (stable: equal values keep scan order)
   bld_windows_kernel<<<gw, tb, 0, st>>>(d_codes, d_soff, d_wstart, g, keyA, valA);
   CK(cudaGetLastError());
-  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, keyA, keyB, valA, valB, (size_t)n, 0, (int)(2 * g.pread), st); }))) return rc;
+  cub_run(d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, keyA, keyB, valA, valB, (size_t)n, 0, (int)(2 * g.pread), st); });
   // 2. distinct (L+1)-mers, ids of the L-mers
   bld_heads_kernel<<<gw, tb, 0, st>>>(keyB, n, u0, u1);
   CK(cudaGetLastError());
-  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u0, u2, (size_t)n, st); }))) return rc;
-  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u1, u3, (size_t)n, st); }))) return rc;
+  cub_run(d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u0, u2, (size_t)n, st); });
+  cub_run(d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u1, u3, (size_t)n, st); });
   uint32_t nent = 0, nids = 0;
   CK(cudaMemcpyAsync(&nent, u2 + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   CK(cudaMemcpyAsync(&nids, u3 + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   const uint32_t E = 2 * nent;
-  uint32_t *e_list, *e_pref, *e_text, *e_id, *e_arr, *e_tpar; uint8_t* e_leaf;
-  CK(scratch(tmp, E, &e_list)); CK(scratch(tmp, E, &e_pref)); CK(scratch(tmp, E, &e_text)); CK(scratch(tmp, E, &e_id)); CK(scratch(tmp, E, &e_arr)); CK(scratch(tmp, E, &e_tpar)); CK(scratch(tmp, E, &e_leaf));
+  uint32_t *e_list = scratch<uint32_t>(tmp, E), *e_pref = scratch<uint32_t>(tmp, E), *e_text = scratch<uint32_t>(tmp, E), *e_id = scratch<uint32_t>(tmp, E),
+           *e_arr = scratch<uint32_t>(tmp, E), *e_tpar = scratch<uint32_t>(tmp, E);
+  uint8_t* e_leaf = scratch<uint8_t>(tmp, E);
   CK(cudaMemsetAsync(e_tpar, 0, (size_t)E * 4, st)); CK(cudaMemsetAsync(e_leaf, 0, E, st));
   bld_entries_kernel<<<gw, tb, 0, st>>>(keyB, valB, u0, u2, u3, g, nent, win_id, e_list, e_pref, e_text, e_id, e_arr);
   CK(cudaGetLastError());
   // 3. positions (persistent arrays)
   bld_poskeys_kernel<<<gw, tb, 0, st>>>(win_id, n, keyA);
   CK(cudaGetLastError());
-  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, keyA, keyB, (size_t)n, 0, 64, st); }))) return rc;
+  cub_run(d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortKeys(t, b, keyA, keyB, (size_t)n, 0, 64, st); });
   bld_posflag_kernel<<<gw, tb, 0, st>>>(keyB, n, u0);
   CK(cudaGetLastError());
-  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveScan(t, b, u0, u1, cuda::maximum<uint32_t>{}, (size_t)n, st); }))) return rc;
+  cub_run(d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveScan(t, b, u0, u1, cuda::maximum<uint32_t>{}, (size_t)n, st); });
   bld_poskeep_kernel<<<gw, tb, 0, st>>>(u1, n, g.max_pos, u2);
   CK(cudaGetLastError());
-  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u2, u3, (size_t)n, st); }))) return rc;
+  cub_run(d_cub, [&](void* t, size_t& b) { return cub::DeviceScan::InclusiveSum(t, b, u2, u3, (size_t)n, st); });
   uint32_t npos = 0;
   CK(cudaMemcpyAsync(&npos, u3 + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
-  uint32_t *p_posoff, *p_ftext, *p_fid, *p_roff; uint2* p_pos; uint4* p_flookup; uint8_t* p_ref;
-  if ((rc = part_array(ctx, pt, (size_t)nids + 1, nullptr, &p_posoff)) || (rc = part_array(ctx, pt, npos, nullptr, &p_pos))) return rc;
+  Part pt;
+  uint32_t* p_posoff = part_array<uint32_t>(ctx, pt, (size_t)nids + 1, nullptr);
+  uint2* p_pos = part_array<uint2>(ctx, pt, npos, nullptr);
   bld_poswrite_kernel<<<gw, tb, 0, st>>>(keyB, u1, u2, u3, d_wstart, g, nids, p_posoff, p_pos);
   CK(cudaGetLastError());
   // 4. burst-trie order of the entries: first occurrence order, then one stable sort + one decision pass per level
   const unsigned ge = (E + tb - 1) / tb;
-  uint64_t *ekA, *ekB; uint32_t *pA, *pB;
-  CK(scratch(tmp, E, &ekA)); CK(scratch(tmp, E, &ekB)); CK(scratch(tmp, E, &pA)); CK(scratch(tmp, E, &pB));
+  uint64_t *ekA = scratch<uint64_t>(tmp, E), *ekB = scratch<uint64_t>(tmp, E);
+  uint32_t *pA = scratch<uint32_t>(tmp, E), *pB = scratch<uint32_t>(tmp, E);
   bld_arrkey_kernel<<<ge, tb, 0, st>>>(e_arr, E, ekA, pA);
   CK(cudaGetLastError());
-  if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, ekA, ekB, pA, pB, (size_t)E, 0, 32, st); }))) return rc;
+  cub_run(d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, ekA, ekB, pA, pB, (size_t)E, 0, 32, st); });
   for (uint32_t d = 1; d <= g.burst_depth; ++d) {
     bld_levelkey_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_pref, e_leaf, E, d, g.burst_depth, ekA, pA);
     CK(cudaGetLastError());
-    if ((rc = cub_run(ctx, d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, ekA, ekB, pA, pB, (size_t)E, 0, (int)key_bits, st); }))) return rc;
+    cub_run(d_cub, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, ekA, ekB, pA, pB, (size_t)E, 0, (int)key_bits, st); });
     if (d < g.burst_depth) { bld_level_kernel<<<ge, tb, 0, st>>>(ekB, pB, E, d, e_arr, e_tpar, e_leaf); CK(cudaGetLastError()); }
   }
   // 5. the lists and their lookup rows
   const size_t nk = (size_t)1 << (2 * g.half);
-  if ((rc = part_array(ctx, pt, ftext_words(E), nullptr, &p_ftext)) || (rc = part_array(ctx, pt, E, nullptr, &p_fid)) ||
-      (rc = part_array(ctx, pt, nk, nullptr, &p_flookup)))
-    return rc;
+  uint32_t* p_ftext = part_array<uint32_t>(ctx, pt, ftext_words(E), nullptr);
+  uint32_t* p_fid = part_array<uint32_t>(ctx, pt, E, nullptr);
+  uint4* p_flookup = part_array<uint4>(ctx, pt, nk, nullptr);
   bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, p_ftext, p_fid, (uint32_t*)p_flookup, 0);
   bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, p_ftext, p_fid, (uint32_t*)p_flookup, 1);
   CK(cudaGetLastError());
   // 6. references for the Smith-Waterman side
-  if ((rc = part_array(ctx, pt, c04.size(), c04.data(), &p_ref)) || (rc = part_array(ctx, pt, roff.size(), roff.data(), &p_roff))) return rc;
+  uint8_t* p_ref = part_array<uint8_t>(ctx, pt, c04.size(), c04.data());
+  uint32_t* p_roff = part_array<uint32_t>(ctx, pt, roff.size(), roff.data());
   CK(cudaStreamSynchronize(st));
   pt.d.lnwin = g.L; pt.d.partialwin = g.half; pt.d.nref = g.nseq; pt.d.nids = nids;
   pt.d.flookup = p_flookup; pt.d.ftext = p_ftext; pt.d.fid = p_fid; pt.d.pos_off = p_posoff; pt.d.pos = p_pos;
   pt.d.refseq = p_ref; pt.d.ref_off = p_roff;
   pt.n_entries = E; pt.n_ids = nids; pt.n_pos = npos; pt.n_refseq = c04.size();
-  return SMR_OK;
+  return pt;
 }
 
 DevParams to_dev(const smr_params& p) {
@@ -333,7 +341,7 @@ Scalars scalars_of(const Batch& b) {
   return Scalars{(uint32_t*)p, (uint32_t*)(p + 4), (uint32_t*)(p + 8), (uint32_t*)(p + 12), (unsigned long long*)(p + 16), (uint32_t*)(p + 24), (uint32_t*)(p + 128), (uint32_t*)(p + 256), (uint32_t*)(p + 384)};
 }
 
-int setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
+void setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
   uint32_t max_nref = 1;
   for (auto& pt : ctx->parts) max_nref = std::max(max_nref, pt.d.nref);
   ctx->hist_cap = max_nref;
@@ -348,7 +356,7 @@ int setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
   CK(cudaFuncSetAttribute(lis_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLisSmemBytes));
   CK(cudaFuncSetAttribute(lis_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLisSmemBytes));
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lis_kernel<true>, kLisWarpsPerCta * 32, kLisSmemBytes));   // (same launch bounds and shared memory for both)
-  if (occ < 1) { ctx->err = "lis_kernel does not fit on an SM"; return SMR_ERR_CUDA; }
+  if (occ < 1) fail(SMR_ERR_CUDA, "lis_kernel does not fit on an SM");
   ctx->lis_ctas = (uint32_t)ctx->sm_count * std::min<uint32_t>(ctx->lis_ctas_per_sm, (uint32_t)occ);
   ctx->lis_warps = ctx->lis_ctas * kPlannerWarps;   // planner warps (each owns an arena)
   ctx->pall_cap = 32768u * scale;
@@ -356,14 +364,14 @@ int setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
   // keep the arena total under ~16 GB (of the 80 GB of an H100): fewer persistent CTAs for huge reference sets
   const size_t budget = (size_t)16 << 30;
   while (ctx->lis_ctas > 16 && ctx->lis_stride * ctx->lis_warps > budget) { ctx->lis_ctas /= 2; ctx->lis_warps = ctx->lis_ctas * kPlannerWarps; }
-  if (int rc = ensure(ctx, ctx->lis_arena, ctx->lis_stride * ctx->lis_warps)) return rc;
-  if (int rc = ensure(ctx, ctx->lis_epochs, (size_t)ctx->lis_warps * 4)) return rc;
-  if (int rc = ensure(ctx, ctx->lis_queue, (size_t)2 * kQueueCap * sizeof(QSlot) + 64)) return rc;
-  if (int rc = ensure(ctx, ctx->lis_done, (size_t)ctx->lis_warps * 4 + 64)) return rc;
+  ensure(ctx->lis_arena, ctx->lis_stride * ctx->lis_warps);
+  ensure(ctx->lis_epochs, (size_t)ctx->lis_warps * 4);
+  ensure(ctx->lis_queue, (size_t)2 * kQueueCap * sizeof(QSlot) + 64);
+  ensure(ctx->lis_done, (size_t)ctx->lis_warps * 4 + 64);
   const size_t dbg_bytes = (size_t)(kTlBase + kTlRows * kTlBuckets) * 8;
-  if (int rc = ensure(ctx, ctx->lis_dbg, dbg_bytes)) return rc;
+  ensure(ctx->lis_dbg, dbg_bytes);
   CK(cudaMemsetAsync(ctx->lis_dbg.p, 0, dbg_bytes, ctx->stream));
-  if (int rc = ensure(ctx, ctx->lis_rows, (size_t)ctx->lis_ctas * kScorerWarps * 2 * ctx->row_cap * 4)) return rc;
+  ensure(ctx->lis_rows, (size_t)ctx->lis_ctas * kScorerWarps * 2 * ctx->row_cap * 4);
   // histogram epochs start at 0 over a zeroed histogram (every run: the arena layout depends on the scale of the run)
   CK(cudaMemset2DAsync(ctx->lis_arena.p, ctx->lis_stride, 0, lis_arena_zero_bytes(ctx->hist_cap), ctx->lis_warps, ctx->stream));   // votes + bitmaps only
   CK(cudaMemsetAsync(ctx->lis_epochs.p, 0, (size_t)ctx->lis_warps * 4, ctx->stream));
@@ -373,7 +381,7 @@ int setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
   ctx->final_warps = (uint32_t)ctx->sm_count * kFinalCtasPerSm * kFinalWarpsPerCta;
   ctx->final_stride = final_arena_bytes(ctx->cap_w, ctx->cap_cig, ctx->row_cap, ctx->cap_dir);
   while (ctx->final_warps > 64 && ctx->final_stride * ctx->final_warps > budget) ctx->final_warps /= 2;
-  if (int rc = ensure(ctx, ctx->final_arena, ctx->final_stride * ctx->final_warps)) return rc;
+  ensure(ctx->final_arena, ctx->final_stride * ctx->final_warps);
   // traceback stage: one thread per alignment, 1024 threads per SM
   ctx->tb_threads = (uint32_t)ctx->sm_count * 1024u;
   ctx->tb_cap_w = 2 * 32 * scale + 8;                       // band widths up to 32*scale
@@ -381,11 +389,10 @@ int setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
   ctx->tb_cap_dir = (size_t)32768 * scale;                  // (2*band+1) * readLen * 3 bytes: band 32 at 150 nt
   ctx->tb_stride = ((size_t)ctx->tb_cap_w * 12 + (size_t)ctx->tb_cap_cig * 4 + ctx->tb_cap_dir + 255) & ~(size_t)255;
   while (ctx->tb_threads > 4096 && ctx->tb_stride * ctx->tb_threads > budget) ctx->tb_threads /= 2;
-  if (int rc = ensure(ctx, ctx->tb_arena, ctx->tb_stride * ctx->tb_threads)) return rc;
+  ensure(ctx->tb_arena, ctx->tb_stride * ctx->tb_threads);
   ctx->lane_hits_cap = kLaneHitCap * scale;
   ctx->lane_hits_warps = scale == 1 ? (uint32_t)ctx->sm_count * kSeedCtasPerSm * kSeedWarpsPerCta : 1024u;
-  if (int rc = ensure(ctx, ctx->lane_hits, (size_t)ctx->lane_hits_warps * ctx->lane_hits_cap * 32 * 4)) return rc;
-  return SMR_OK;
+  ensure(ctx->lane_hits, (size_t)ctx->lane_hits_warps * ctx->lane_hits_cap * 32 * 4);
 }
 
 // the reads c0 .. c0 + n of a batch as the kernels see them
@@ -403,13 +410,12 @@ DevBatch make_batch(const Batch& s, uint32_t c0, uint32_t n) {
 }
 
 // The layout of n reads of lengths len(r) in b: read offsets (b.off32, b.seq_off), packed-word offsets (b.pk_off: (len + 15) / 16 + 2
-// words per read, the layout of pack_reads_kernel), nreads, total_nt and max_len.  *words = the packed-word total.  The device copies
+// words per read, the layout of pack_reads_kernel), nreads, total_nt and max_len.  Returns the packed-word total.  The device copies
 // are staged in the context's pinned buffers: the caller synchronizes before the next layout.
 template <class Len>
-int read_layout(smr_ctx* ctx, Batch& b, uint32_t n, Len len, uint64_t* words) {
-  int rc;
-  if ((rc = ensure(ctx, ctx->h_pkoff, (size_t)(n + 1) * 4)) || (rc = ensure(ctx, ctx->h_off32, (size_t)(n + 1) * 4))) return rc;
-  uint32_t *off32 = (uint32_t*)ctx->h_off32.p, *pkoff = (uint32_t*)ctx->h_pkoff.p;
+uint64_t read_layout(smr_ctx* ctx, Batch& b, uint32_t n, Len len) {
+  uint32_t* pkoff = ensure<uint32_t>(ctx->h_pkoff, (size_t)(n + 1) * 4);
+  uint32_t* off32 = ensure<uint32_t>(ctx->h_off32, (size_t)(n + 1) * 4);
   uint64_t total = 0, w = 0; uint32_t max_len = 0;
   for (uint32_t r = 0; r <= n; ++r) {
     off32[r] = (uint32_t)total;
@@ -421,32 +427,31 @@ int read_layout(smr_ctx* ctx, Batch& b, uint32_t n, Len len, uint64_t* words) {
       w += (l + 15) / 16 + 2;     // +2 padding words: window_fwd reads three consecutive words
     }
   }
-  if (total >= 0xF0000000ull) { ctx->err = "batch larger than 2^32 nucleotides: split it"; return SMR_ERR_ARG; }
-  if (w >= 0xFFFFFFFFull) { ctx->err = "batch too large"; return SMR_ERR_ARG; }
-  if ((rc = ensure(ctx, b.seq_off, (size_t)(n + 1) * 4)) || (rc = ensure(ctx, b.pk_off, (size_t)(n + 1) * 4))) return rc;
+  if (total >= 0xF0000000ull) fail(SMR_ERR_ARG, "batch larger than 2^32 nucleotides: split it");
+  if (w >= 0xFFFFFFFFull) fail(SMR_ERR_ARG, "batch too large");
+  ensure(b.seq_off, (size_t)(n + 1) * 4);
+  ensure(b.pk_off, (size_t)(n + 1) * 4);
   CK(cudaMemcpyAsync(b.seq_off.p, off32, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaMemcpyAsync(b.pk_off.p, pkoff, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
   b.off32.assign(off32, off32 + n + 1);
   b.nreads = n; b.total_nt = total; b.max_len = max_len;
-  *words = w;
-  return SMR_OK;
+  return w;
 }
 
 // The part of an upload that does not depend on where the reads came from: b's reads and offsets are on the device and b.off32 on the
 // host; sizes the batch's other buffers for its scale and 2-bit packs the reads.
-int finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
+void finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
   const uint32_t slots = slots_of(ctx), nreads = b.nreads;
-  int rc;
-  if ((rc = ensure(ctx, b.pk03, (size_t)(w + 4) * 4))) return rc;
-  if ((rc = ensure(ctx, b.pk03alt, (size_t)(w + 4) * 4))) return rc;
-  if ((rc = ensure(ctx, b.has_n, nreads))) return rc;
-  if ((rc = ensure(ctx, b.flags, (size_t)nreads * 4))) return rc;
-  if ((rc = ensure(ctx, b.state, (size_t)nreads * sizeof(ReadState)))) return rc;
-  if ((rc = ensure(ctx, b.hit_db, (size_t)nreads * 2))) return rc;
-  if ((rc = ensure(ctx, b.aln_work, (size_t)nreads * slots * sizeof(AlnWork)))) return rc;
-  if ((rc = ensure(ctx, b.out_aln, (size_t)nreads * slots * sizeof(OutAln)))) return rc;
-  if ((rc = ensure(ctx, b.scalars, 512))) return rc;
-  if ((rc = ensure(ctx, b.counters, (size_t)(dcCount + 64) * 8))) return rc;
+  ensure(b.pk03, (size_t)(w + 4) * 4);
+  ensure(b.pk03alt, (size_t)(w + 4) * 4);
+  ensure(b.has_n, nreads);
+  ensure(b.flags, (size_t)nreads * 4);
+  ensure(b.state, (size_t)nreads * sizeof(ReadState));
+  ensure(b.hit_db, (size_t)nreads * 2);
+  ensure(b.aln_work, (size_t)nreads * slots * sizeof(AlnWork));
+  ensure(b.out_aln, (size_t)nreads * slots * sizeof(OutAln));
+  ensure(b.scalars, 512);
+  ensure(b.counters, (size_t)(dcCount + 64) * 8);
   CK(cudaMemsetAsync(b.pk03.p, 0, (size_t)(w + 4) * 4, ctx->stream));
   CK(cudaMemsetAsync(b.pk03alt.p, 0, (size_t)(w + 4) * 4, ctx->stream));
   // hit regions are per chunk
@@ -459,129 +464,119 @@ int finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
   const uint32_t nparts = (uint32_t)std::max<size_t>(1, ctx->parts.size());
   b.cnt_stride = std::min(nreads, ctx->chunk_reads);
   b.hits_stride = (size_t)((uint64_t)b.scale * (2 * max_chunk_nt + 32ull * b.cnt_stride) + 64);
-  if ((rc = ensure(ctx, b.hits, b.hits_stride * nparts * 8))) return rc;
-  if ((rc = ensure(ctx, b.hit_cnt, (size_t)b.cnt_stride * nparts * 4))) return rc;
-  if ((rc = ensure(ctx, b.cost, (size_t)b.cnt_stride * 4))) return rc;
-  if ((rc = ensure(ctx, b.bins, (size_t)b.cnt_stride * kCostBins * 4 + (size_t)kCostBins * 4))) return rc;
+  ensure(b.hits, b.hits_stride * nparts * 8);
+  ensure(b.hit_cnt, (size_t)b.cnt_stride * nparts * 4);
+  ensure(b.cost, (size_t)b.cnt_stride * 4);
+  ensure(b.bins, (size_t)b.cnt_stride * kCostBins * 4 + (size_t)kCostBins * 4);
   // 2-bit packing + N detection
   pack_reads_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(make_batch(b, 0, nreads), (uint32_t*)b.pk03.p, (uint32_t*)b.pk03alt.p, (uint8_t*)b.has_n.p);
   CK(cudaGetLastError());
-  return SMR_OK;
 }
 
 // host reads -> the resident batch (no text behind it)
-int upload_batch_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads) {
+void upload_batch_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads) {
   Batch& b = ctx->resident;
   b.nreads = 0; b.from_text = false; ctx->text_bytes = 0;
-  if (nreads == 0) return SMR_OK;
+  if (nreads == 0) return;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
   CK(cudaEventRecord(e0, ctx->stream));
-  uint64_t w = 0;
-  int rc;
-  if ((rc = read_layout(ctx, b, nreads, [&](uint32_t r) { return seq_off[r + 1] - seq_off[r]; }, &w))) return rc;
-  if ((rc = ensure(ctx, b.seq04, b.total_nt + 64))) return rc;
+  const uint64_t w = read_layout(ctx, b, nreads, [&](uint32_t r) { return seq_off[r + 1] - seq_off[r]; });
+  ensure(b.seq04, b.total_nt + 64);
   CK(cudaMemcpyAsync(b.seq04.p, seq_cat + seq_off[0], b.total_nt, cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = finish_upload(ctx, b, w))) return rc;
+  finish_upload(ctx, b, w);
   CK(cudaEventRecord(e1, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_h2d = ms;
-  return SMR_OK;
 }
 
 // exclusive sum of n u32 (out may equal in) in the context's cub scratch
-int exclusive_sum(smr_ctx* ctx, const uint32_t* in, uint32_t* out, uint32_t n) {
-  return cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, n, ctx->stream); });
+void exclusive_sum(smr_ctx* ctx, const uint32_t* in, uint32_t* out, uint32_t n) {
+  cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, n, ctx->stream); });
 }
 
 struct TextLayout { uint32_t nlines = 0, nrec = 0, total_nt = 0; uint32_t fmt = kFmtFasta; };
 
 // The line layout of a FASTA / FASTQ text on the device (the line passes of smr_decode.cuh), for the decode and the report writer.
-// first_byte is text[0] and names the format.  Leaves, for each of the L.nlines lines, its newline position (d_nl), header flag
+// first_byte is text[0] and names the format.  Leaves, for each of the nlines lines, its newline position (d_nl), header flag
 // (d_hdr), sequence bytes (d_sb), record index (d_rec) and the offset of its sequence bytes (d_spos); the arrays hold nlines + 1
 // items, d_rec and d_spos the totals at [nlines].  d_scal is zeroed; its words from [4] on are the caller's.
-int text_layout(smr_ctx* ctx, const uint8_t* text, uint64_t nbytes, char first_byte, TextLayout& L) {
-  L = TextLayout{};
-  if (nbytes >= 0xF0000000ull) { ctx->err = "text batch of 2^32 bytes or more: split it (line counts and sequence offsets are 32-bit on the device)"; return SMR_ERR_ARG; }
-  if (nbytes && first_byte != '@' && first_byte != '>') { ctx->err = "reads text must start with '@' (FASTQ) or '>' (FASTA)"; return SMR_ERR_ARG; }
+TextLayout text_layout(smr_ctx* ctx, const uint8_t* text, uint64_t nbytes, char first_byte) {
+  TextLayout L;
+  if (nbytes >= 0xF0000000ull) fail(SMR_ERR_ARG, "text batch of 2^32 bytes or more: split it (line counts and sequence offsets are 32-bit on the device)");
+  if (nbytes && first_byte != '@' && first_byte != '>') fail(SMR_ERR_ARG, "reads text must start with '@' (FASTQ) or '>' (FASTA)");
   L.fmt = first_byte == '@' ? kFmtFastq : kFmtFasta;
-  int rc;
-  if ((rc = ensure(ctx, ctx->d_scal, 64))) return rc;
-  uint32_t* scal = (uint32_t*)ctx->d_scal.p;   // [1] records [2] sequence bytes [3] decode error
+  uint32_t* scal = ensure<uint32_t>(ctx->d_scal, 64);   // [1] records [2] sequence bytes [3] decode error
   CK(cudaMemsetAsync(scal, 0, 64, ctx->stream));
   // newlines: count per 32-byte chunk, scan (the total lands at [nchunks]), positions
   const int grid = ctx->sm_count * 8;
   const uint64_t nchunks = nbytes / 32 + 1;
-  if ((rc = ensure(ctx, ctx->d_cnt, (nchunks + 1) * 4))) return rc;
-  uint32_t* cnt = (uint32_t*)ctx->d_cnt.p;
+  uint32_t* cnt = ensure<uint32_t>(ctx->d_cnt, (nchunks + 1) * 4);
   count_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks);
   CK(cudaMemsetAsync(cnt + nchunks, 0, 4, ctx->stream));
-  if ((rc = exclusive_sum(ctx, cnt, cnt, (uint32_t)nchunks + 1))) return rc;
+  exclusive_sum(ctx, cnt, cnt, (uint32_t)nchunks + 1);
   CK(cudaMemcpyAsync(&L.nlines, cnt + nchunks, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   const uint32_t n = L.nlines;
-  if ((rc = ensure(ctx, ctx->d_nl, ((size_t)n + 1) * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->d_hdr, ((size_t)n + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->d_sb, ((size_t)n + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->d_rec, ((size_t)n + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->d_spos, ((size_t)n + 1) * 4))) return rc;
-  if (n == 0) return SMR_OK;
+  ensure(ctx->d_nl, ((size_t)n + 1) * 8);
+  ensure(ctx->d_hdr, ((size_t)n + 1) * 4);
+  ensure(ctx->d_sb, ((size_t)n + 1) * 4);
+  ensure(ctx->d_rec, ((size_t)n + 1) * 4);
+  ensure(ctx->d_spos, ((size_t)n + 1) * 4);
+  if (n == 0) return L;
   uint32_t *hdr = (uint32_t*)ctx->d_hdr.p, *sb = (uint32_t*)ctx->d_sb.p, *rec = (uint32_t*)ctx->d_rec.p, *spos = (uint32_t*)ctx->d_spos.p;
   write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks, (uint64_t*)ctx->d_nl.p);
   // per line: header flag and sequence bytes; their scans give the record of every line and the offset of its bytes
   line_info_kernel<<<grid, 256, 0, ctx->stream>>>(text, (const uint64_t*)ctx->d_nl.p, n, L.fmt, hdr, sb, scal + 3);
   CK(cudaMemsetAsync(hdr + n, 0, 4, ctx->stream));
   CK(cudaMemsetAsync(sb + n, 0, 4, ctx->stream));
-  if ((rc = exclusive_sum(ctx, hdr, rec, n + 1))) return rc;
-  if ((rc = exclusive_sum(ctx, sb, spos, n + 1))) return rc;
+  exclusive_sum(ctx, hdr, rec, n + 1);
+  exclusive_sum(ctx, sb, spos, n + 1);
   CK(cudaMemcpyAsync(scal + 1, rec + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
   CK(cudaMemcpyAsync(scal + 2, spos + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
   uint32_t h[8];
   CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (h[3]) { ctx->err = h[3] & kDecBadHeader ? "reads text: a record does not start with its header character" : "reads text: FASTQ separator line '+' missing"; return SMR_ERR_ARG; }
+  if (h[3]) fail(SMR_ERR_ARG, h[3] & kDecBadHeader ? "reads text: a record does not start with its header character" : "reads text: FASTQ separator line '+' missing");
   L.nrec = h[1]; L.total_nt = h[2];
-  return SMR_OK;
+  return L;
 }
 
 // FASTA / FASTQ text -> resident batch (smr_decode.cuh)
-// text == nullptr: the text is already in ctx->d_text (inflated on the device), first byte given
-int upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t* nreads_out, char first_byte = 0) {
-  *nreads_out = 0;
+// text == nullptr: the text is already in ctx->d_text (inflated on the device), first byte given.  Returns the number of reads.
+uint32_t upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, char first_byte = 0) {
   Batch& b = ctx->resident;
   b.nreads = 0; b.from_text = true;
   ctx->text_bytes = nbytes;
-  if (nbytes == 0) return SMR_OK;
+  if (nbytes == 0) return 0;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
-  int rc;
   CK(cudaEventRecord(e0, ctx->stream));
   if (text) {
-    if ((rc = ensure(ctx, ctx->d_text, nbytes + 64))) return rc;
+    ensure(ctx->d_text, nbytes + 64);
     CK(cudaMemcpyAsync(ctx->d_text.p, text, nbytes, cudaMemcpyHostToDevice, ctx->stream));
   }
   CK(cudaEventRecord(e1, ctx->stream));
   const uint8_t* dt = (const uint8_t*)ctx->d_text.p;
-  TextLayout L;
-  if ((rc = text_layout(ctx, dt, nbytes, text ? text[0] : first_byte, L))) return rc;
+  const TextLayout L = text_layout(ctx, dt, nbytes, text ? text[0] : first_byte);
   const uint32_t nreads = L.nrec, total = L.total_nt;
-  if (total >= 0xF0000000u) { ctx->err = "batch larger than 2^32 nucleotides: split it"; return SMR_ERR_ARG; }
-  if (nreads == 0) return SMR_OK;
+  if (total >= 0xF0000000u) fail(SMR_ERR_ARG, "batch larger than 2^32 nucleotides: split it");
+  if (nreads == 0) return 0;
   const int grid = ctx->sm_count * 8;
   uint32_t* scal = (uint32_t*)ctx->d_scal.p;   // of text_layout; here [4] packed words [5] max_len
-  if ((rc = ensure(ctx, b.seq04, (size_t)total + 64))) return rc;
-  if ((rc = ensure(ctx, b.seq_off, (size_t)(nreads + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, b.pk_off, (size_t)(nreads + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->d_hdroff, (size_t)nreads * 8))) return rc;
+  ensure(b.seq04, (size_t)total + 64);
+  ensure(b.seq_off, (size_t)(nreads + 1) * 4);
+  ensure(b.pk_off, (size_t)(nreads + 1) * 4);
+  ensure(ctx->d_hdroff, (size_t)nreads * 8);
   scatter_lines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)ctx->d_nl.p, L.nlines, (const uint32_t*)ctx->d_hdr.p, (const uint32_t*)ctx->d_rec.p,
                                                        (const uint32_t*)ctx->d_sb.p, (const uint32_t*)ctx->d_spos.p, (uint8_t*)b.seq04.p,
                                                        (uint32_t*)b.seq_off.p, (uint64_t*)ctx->d_hdroff.p);
   CK(cudaMemcpyAsync((uint32_t*)b.seq_off.p + nreads, scal + 2, 4, cudaMemcpyDeviceToDevice, ctx->stream));
   // packed-word offsets and the longest read (what read_layout computes on the host); words[nreads] = 0, so pk_off[nreads] is the total
-  if ((rc = ensure(ctx, ctx->d_cnt, (size_t)(nreads + 1) * 4))) return rc;
+  uint32_t* words = ensure<uint32_t>(ctx->d_cnt, (size_t)(nreads + 1) * 4);
   uint32_t* pk_off = (uint32_t*)b.pk_off.p;
-  record_words_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)b.seq_off.p, nreads, (uint32_t*)ctx->d_cnt.p, scal + 5);
-  if ((rc = exclusive_sum(ctx, (const uint32_t*)ctx->d_cnt.p, pk_off, nreads + 1))) return rc;
+  record_words_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)b.seq_off.p, nreads, words, scal + 5);
+  exclusive_sum(ctx, words, pk_off, nreads + 1);
   CK(cudaMemcpyAsync(scal + 4, pk_off + nreads, 4, cudaMemcpyDeviceToDevice, ctx->stream));
-  if ((rc = ensure(ctx, ctx->h_off32, (size_t)(nreads + 1) * 4))) return rc;
+  ensure(ctx->h_off32, (size_t)(nreads + 1) * 4);
   CK(cudaMemcpyAsync(ctx->h_off32.p, b.seq_off.p, (size_t)(nreads + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream));
   uint32_t h[8];
   CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
@@ -590,12 +585,11 @@ int upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t*
   const uint32_t* off32 = (const uint32_t*)ctx->h_off32.p;
   b.off32.assign(off32, off32 + nreads + 1);
   b.nreads = nreads; b.total_nt = total; b.max_len = h[5];
-  if ((rc = finish_upload(ctx, b, h[4]))) return rc;
+  finish_upload(ctx, b, h[4]);
   CK(cudaStreamSynchronize(ctx->stream));
   float ms = 0; cudaEventElapsedTime(&ms, e0, e1); if (text) ctx->t_h2d = ms;
   cudaEventElapsedTime(&ms, e1, e2); ctx->t_decode = ms;
-  *nreads_out = nreads;
-  return SMR_OK;
+  return nreads;
 }
 
 const char* inf_status_text(uint32_t st) {
@@ -612,28 +606,26 @@ const char* inf_status_text(uint32_t st) {
   }
 }
 
-// gzip file (host bytes) -> inflated bytes in ctx->d_text.  The five steps of smr_inflate.h; the host only walks the list of
-// spans (a few thousand entries) between the COUNT and the WRITE pass.
-int inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes, uint64_t* out_bytes) {
-  *out_bytes = 0;
+// gzip file (host bytes) -> inflated bytes in ctx->d_text; returns their number.  The five steps of smr_inflate.h; the host only
+// walks the list of spans (a few thousand entries) between the COUNT and the WRITE pass.
+uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes) {
   ctx->inf_spans = ctx->inf_candidates = 0;
-  if (nbytes < 18) { ctx->err = "gz input: shorter than a gzip header and trailer"; return SMR_ERR_ARG; }
+  if (nbytes < 18) fail(SMR_ERR_ARG, "gz input: shorter than a gzip header and trailer");
   if (chunk_bytes < 1024) chunk_bytes = 1024;
-  int rc;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
   CK(cudaEventRecord(e0, ctx->stream));
   const size_t padded = (nbytes + 3) / 4 * 4 + 128;
-  if ((rc = ensure(ctx, ctx->d_gz, padded))) return rc;
+  ensure(ctx->d_gz, padded);
   CK(cudaMemsetAsync((uint8_t*)ctx->d_gz.p + nbytes / 4 * 4, 0, padded - nbytes / 4 * 4, ctx->stream));
   CK(cudaMemcpyAsync(ctx->d_gz.p, gz, nbytes, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaEventRecord(e1, ctx->stream));
   const uint32_t* w = (const uint32_t*)ctx->d_gz.p;
   // FIND
   const uint64_t nchunks = (nbytes + chunk_bytes - 1) / chunk_bytes;
-  if (nchunks > (1u << 24)) { ctx->err = "gz input: too many chunks"; return SMR_ERR_ARG; }
+  if (nchunks > (1u << 24)) fail(SMR_ERR_ARG, "gz input: too many chunks");
   std::vector<uint64_t> cand;
   if (nchunks > 1) {
-    if ((rc = ensure(ctx, ctx->d_cand, nchunks * 8))) return rc;
+    ensure(ctx->d_cand, nchunks * 8);
     inf_find_kernel<<<(unsigned)(nchunks - 1), 256, 0, ctx->stream>>>(w, nbytes, chunk_bytes, (uint64_t*)ctx->d_cand.p);
     CK(cudaGetLastError());
     std::vector<uint64_t> raw(nchunks - 1);
@@ -641,12 +633,12 @@ int inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_b
     CK(cudaStreamSynchronize(ctx->stream));
     for (uint64_t p : raw) if (p != kInfNone) cand.push_back(p);   // chunk order = position order
     if (!cand.empty()) CK(cudaMemcpyAsync(ctx->d_cand.p, cand.data(), cand.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-  } else if ((rc = ensure(ctx, ctx->d_cand, 8))) return rc;
+  } else ensure(ctx->d_cand, 8);
   const uint32_t ncand = (uint32_t)cand.size(), ns = ncand + 1;
   // COUNT
   CK(cudaFuncSetAttribute(inf_span_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kInfSpanSmem));   // per device
   CK(cudaFuncSetAttribute(inf_span_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kInfSpanSmem));
-  if ((rc = ensure(ctx, ctx->d_res, (size_t)ns * sizeof(SpanResult)))) return rc;
+  ensure(ctx->d_res, (size_t)ns * sizeof(SpanResult));
   const unsigned ctas = (ns + kInfSpanThreads - 1) / kInfSpanThreads;
   inf_span_kernel<false><<<ctas, kInfSpanThreads, kInfSpanSmem, ctx->stream>>>(w, nbytes, (const uint64_t*)ctx->d_cand.p, ncand, nullptr, nullptr, nullptr, nullptr, nullptr, ns,
                                                                                nullptr, (SpanResult*)ctx->d_res.p);
@@ -657,24 +649,24 @@ int inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_b
   std::vector<uint32_t> real(ns); std::vector<uint64_t> off(ns), cnt(ns);
   uint32_t nreal = 0, why = 0;
   const uint64_t total = inf_chain(cand.data(), ncand, res.data(), real.data(), off.data(), nreal, &why);
-  if (total == kInfNone) { ctx->err = std::string("gz input: ") + inf_status_text(why); return SMR_ERR_ARG; }
+  if (total == kInfNone) fail(SMR_ERR_ARG, std::string("gz input: ") + inf_status_text(why));
   std::vector<uint32_t> moff(nreal + 1, 0);
   for (uint32_t k = 0; k < nreal; ++k) { cnt[k] = res[real[k]].out_n; moff[k + 1] = moff[k] + res[real[k]].members; }
   const uint32_t nmembers = moff[nreal];
   ctx->inf_spans = nreal; ctx->inf_candidates = ncand;
-  if ((rc = ensure(ctx, ctx->d_text, total + 64))) return rc;
+  ensure(ctx->d_text, total + 64);
   if (total) {
     // WRITE
-    if ((rc = ensure(ctx, ctx->d_ids, (size_t)nreal * 4))) return rc;
-    if ((rc = ensure(ctx, ctx->d_off, (size_t)nreal * 8))) return rc;
-    if ((rc = ensure(ctx, ctx->d_cnt64, (size_t)nreal * 8))) return rc;
-    if ((rc = ensure(ctx, ctx->d_sym, (total + 8) * 2))) return rc;
-    if ((rc = ensure(ctx, ctx->d_win, (size_t)(nreal + 1) * kInfWindow))) return rc;
+    ensure(ctx->d_ids, (size_t)nreal * 4);
+    ensure(ctx->d_off, (size_t)nreal * 8);
+    ensure(ctx->d_cnt64, (size_t)nreal * 8);
+    ensure(ctx->d_sym, (total + 8) * 2);
+    ensure(ctx->d_win, (size_t)(nreal + 1) * kInfWindow);
     CK(cudaMemcpyAsync(ctx->d_ids.p, real.data(), (size_t)nreal * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_off.p, off.data(), (size_t)nreal * 8, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_cnt64.p, cnt.data(), (size_t)nreal * 8, cudaMemcpyHostToDevice, ctx->stream));
-    if ((rc = ensure(ctx, ctx->d_moff, (size_t)(nreal + 1) * 4))) return rc;
-    if ((rc = ensure(ctx, ctx->d_mem, (size_t)(nmembers + 1) * sizeof(MemberEnd)))) return rc;
+    ensure(ctx->d_moff, (size_t)(nreal + 1) * 4);
+    ensure(ctx->d_mem, (size_t)(nmembers + 1) * sizeof(MemberEnd));
     CK(cudaMemcpyAsync(ctx->d_moff.p, moff.data(), (size_t)(nreal + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
     inf_span_kernel<true><<<(nreal + kInfSpanThreads - 1) / kInfSpanThreads, kInfSpanThreads, kInfSpanSmem, ctx->stream>>>(
         w, nbytes, (const uint64_t*)ctx->d_cand.p, ncand, (const uint32_t*)ctx->d_ids.p, (const uint64_t*)ctx->d_off.p, (const uint64_t*)ctx->d_cnt64.p,
@@ -694,9 +686,8 @@ int inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_b
     if (nmembers) CK(cudaMemcpyAsync(ends.data(), ctx->d_mem.p, (size_t)nmembers * sizeof(MemberEnd), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     for (uint32_t k = 0; k < nreal; ++k) {
-      if (res2[k].status != res[real[k]].status || res2[k].out_n != cnt[k] || res2[k].end_bit != res[real[k]].end_bit || res2[k].members != res[real[k]].members) {
-        ctx->err = "gz inflate: the write pass disagrees with the count pass"; return SMR_ERR_CUDA;
-      }
+      if (res2[k].status != res[real[k]].status || res2[k].out_n != cnt[k] || res2[k].end_bit != res[real[k]].end_bit || res2[k].members != res[real[k]].members)
+        fail(SMR_ERR_CUDA, "gz inflate: the write pass disagrees with the count pass");
       for (uint32_t m = moff[k]; m < moff[k + 1]; ++m) ends[m].out_end += off[k];
     }
     // CRC-32 + ISIZE of every member (RFC 1952 2.3.1): pieces on the device, joined here
@@ -705,9 +696,9 @@ int inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_b
     const uint32_t npieces = (uint32_t)poff.size();
     std::vector<uint32_t> crcs(npieces);
     if (npieces) {
-      if ((rc = ensure(ctx, ctx->d_poff, (size_t)npieces * 8))) return rc;
-      if ((rc = ensure(ctx, ctx->d_plen, (size_t)npieces * 4))) return rc;
-      if ((rc = ensure(ctx, ctx->d_pcrc, (size_t)npieces * 4))) return rc;
+      ensure(ctx->d_poff, (size_t)npieces * 8);
+      ensure(ctx->d_plen, (size_t)npieces * 4);
+      ensure(ctx->d_pcrc, (size_t)npieces * 4);
       CK(cudaMemcpyAsync(ctx->d_poff.p, poff.data(), (size_t)npieces * 8, cudaMemcpyHostToDevice, ctx->stream));
       CK(cudaMemcpyAsync(ctx->d_plen.p, plen.data(), (size_t)npieces * 4, cudaMemcpyHostToDevice, ctx->stream));
       inf_crc_kernel<<<(npieces + 127) / 128, 128, 0, ctx->stream>>>((const uint8_t*)ctx->d_text.p, (const uint64_t*)ctx->d_poff.p, (const uint32_t*)ctx->d_plen.p, npieces,
@@ -717,15 +708,14 @@ int inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_b
     }
     CK(cudaEventRecord(e2, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    if (const uint32_t bad = inf_crc_verify(ends, plen, first, crcs.data())) { ctx->err = std::string("gz input: ") + inf_status_text(bad); return SMR_ERR_ARG; }
+    if (const uint32_t bad = inf_crc_verify(ends, plen, first, crcs.data())) fail(SMR_ERR_ARG, std::string("gz input: ") + inf_status_text(bad));
   } else {
     CK(cudaEventRecord(e2, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
   float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_h2d = ms;
   cudaEventElapsedTime(&ms, e1, e2); ctx->t_inflate = ms;
-  *out_bytes = total;
-  return SMR_OK;
+  return total;
 }
 
 // Several contexts may share a device (two per GPU let the copies and the host-side result packing of one batch run under the
@@ -737,31 +727,30 @@ std::mutex& device_kernel_mutex(int device) {
 }
 
 // all kernels of one pass over a batch; its results and times stay in the batch
-int run_impl(smr_ctx* ctx, Batch& bt) {
-  if (!ctx->have_params) { ctx->err = "smr_set_params not called"; return SMR_ERR_ARG; }
-  if (ctx->parts.empty()) { ctx->err = "no index loaded"; return SMR_ERR_ARG; }
-  if (ctx->prm.num_alignments < 0) { ctx->err = "num_alignments < 0"; return SMR_ERR_ARG; }
-  if (ctx->prm.minoccur != 0) { ctx->err = "minoccur != 0 is not supported"; return SMR_ERR_UNSUPPORTED; }
+void run_impl(smr_ctx* ctx, Batch& bt) {
+  if (!ctx->have_params) fail(SMR_ERR_ARG, "smr_set_params not called");
+  if (ctx->parts.empty()) fail(SMR_ERR_ARG, "no index loaded");
+  if (ctx->prm.num_alignments < 0) fail(SMR_ERR_ARG, "num_alignments < 0");
+  if (ctx->prm.minoccur != 0) fail(SMR_ERR_UNSUPPORTED, "minoccur != 0 is not supported");
   RunTimes& t = bt.run;
   t = RunTimes{};
   const uint32_t nreads = bt.nreads;
-  if (nreads == 0) return SMR_OK;
+  if (nreads == 0) return;
   const uint32_t slots = slots_of(ctx);
   std::lock_guard<std::mutex> dev_lock(device_kernel_mutex(ctx->device));   // held until the stream has drained
-  int rc;
-  if ((rc = setup_arenas(ctx, bt.scale, bt.max_len))) return rc;
+  setup_arenas(ctx, bt.scale, bt.max_len);
   // device copy of the part table (finalize looks parts up by slot)
   std::vector<DevIndex> hp;
   for (size_t i = 0; i < ctx->parts.size(); ++i) {
     DevIndex d = ctx->parts[i].d; d.slot = (uint32_t)i; d.is_last = (i + 1 == ctx->parts.size()) ? 1u : 0u;
     hp.push_back(d);
   }
-  if ((rc = ensure(ctx, ctx->parts_dev, hp.size() * sizeof(DevIndex)))) return rc;
+  ensure(ctx->parts_dev, hp.size() * sizeof(DevIndex));
   CK(cudaMemcpyAsync(ctx->parts_dev.p, hp.data(), hp.size() * sizeof(DevIndex), cudaMemcpyHostToDevice, ctx->stream));
   // cigar pool on the device: generous fixed share per alignment slot
   bt.cigar_cap_dev = (uint64_t)nreads * slots * 24 * bt.scale + 4096;
-  if (bt.cigar_cap_dev >= 0xFFFFFFFFull) { ctx->err = "CIGAR pool of this batch would pass 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches"; return SMR_ERR_CAPACITY; }
-  if ((rc = ensure(ctx, bt.cigar_pool, bt.cigar_cap_dev * 4))) return rc;
+  if (bt.cigar_cap_dev >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, "CIGAR pool of this batch would pass 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches");
+  ensure(bt.cigar_pool, bt.cigar_cap_dev * 4);
   const Scalars sc = scalars_of(bt);
   CK(cudaMemsetAsync(bt.scalars.p, 0, 512, ctx->stream));
   CK(cudaMemsetAsync(bt.counters.p, 0, (size_t)(dcCount + 64) * 8, ctx->stream));
@@ -780,7 +769,7 @@ int run_impl(smr_ctx* ctx, Batch& bt) {
     CK(cudaMemsetAsync(b.bin_count, 0, (size_t)kCostBins * 4, ctx->stream));
     cudaEvent_t s0 = get_event(ctx, evi), s1 = get_event(ctx, evi + 1), s2 = get_event(ctx, evi + 2); evi += 3;
     CK(cudaEventRecord(s0, ctx->stream));
-    if ((rc = ensure(ctx, ctx->seed_ctr, hp.size() * 4))) return rc;
+    ensure(ctx->seed_ctr, hp.size() * 4);
     CK(cudaMemsetAsync(ctx->seed_ctr.p, 0, hp.size() * 4, ctx->stream));   // one work counter per seed launch
     for (size_t pi = 0; pi < hp.size(); ++pi) {
       const int ctas = (int)(ctx->lane_hits_warps / kSeedWarpsPerCta);
@@ -823,14 +812,14 @@ int run_impl(smr_ctx* ctx, Batch& bt) {
     fg.parts = (const DevIndex*)ctx->parts_dev.p; fg.aln_work = (const AlnWork*)bt.aln_work.p; fg.out = (OutAln*)bt.out_aln.p;
     fg.slots = slots; fg.cigar_pool = (uint32_t*)bt.cigar_pool.p; fg.cigar_cap = bt.cigar_cap_dev; fg.cigar_used = sc.cigar_used;
     fg.work_next = sc.fin_next;
-    if ((rc = ensure(ctx, ctx->tb_jobs, (size_t)n * slots * sizeof(TraceJob)))) return rc;
-    if ((rc = ensure(ctx, ctx->fin_list, (size_t)n * slots * 4))) return rc;
+    ensure(ctx->tb_jobs, (size_t)n * slots * sizeof(TraceJob));
+    ensure(ctx->fin_list, (size_t)n * slots * 4);
     fg.job_list = (uint32_t*)ctx->fin_list.p; fg.job_count = sc.fin_jobs;
     fg.jobs = (TraceJob*)ctx->tb_jobs.p; fg.tb_arena = (uint8_t*)ctx->tb_arena.p; fg.tb_stride = ctx->tb_stride;
     fg.tb_cap_w = ctx->tb_cap_w; fg.tb_cap_cig = ctx->tb_cap_cig; fg.tb_cap_dir = ctx->tb_cap_dir;
     fg.stats = nullptr;
     if (ctx->host_stats) {
-      if ((rc = ensure(ctx, bt.aln_stats, (size_t)nreads * slots * sizeof(AlnStats)))) return rc;
+      ensure(bt.aln_stats, (size_t)nreads * slots * sizeof(AlnStats));
       fg.stats = (AlnStats*)bt.aln_stats.p;
     }
     final_jobs_kernel<<<std::min<uint32_t>((n * slots + 255) / 256, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(b, fg);
@@ -869,7 +858,6 @@ int run_impl(smr_ctx* ctx, Batch& bt) {
       cudaEventElapsedTime(&ms, ctx->ev[s.first + 1], ctx->ev[s.first + 2]); t.lis += ms;
     } else { cudaEventElapsedTime(&ms, ctx->ev[s.first], ctx->ev[s.first + 1]); t.final += ms; }
   }
-  return SMR_OK;
 }
 
 struct HostOut {
@@ -878,31 +866,21 @@ struct HostOut {
   bool pool_short = false;   // cigar_cap was exceeded: nothing more is written, cigar_used goes on counting the words the batch needs
 };
 
-// the caller's CIGAR pool was too small: *cigar_used names the words the batch needs
-int pool_short_error(smr_ctx* ctx, const HostOut& out) {
-  ctx->err = "cigar pool too small: the batch needs " + std::to_string(out.cigar_used) + " words, cigar_cap is " + std::to_string(out.cigar_cap);
-  return SMR_ERR_CAPACITY;
-}
-
 // copies the results of a batch's run to the host; returns the indices of reads whose scratch overflowed
-int download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint32_t>& flagged, const uint32_t* map /*local->caller index or null*/) {
+void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint32_t>& flagged, const uint32_t* map /*local->caller index or null*/) {
   const uint32_t n = b.nreads;
   flagged.clear();
-  if (n == 0) return SMR_OK;
+  if (n == 0) return;
   const uint32_t slots = slots_of(ctx);
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
   CK(cudaEventRecord(e0, ctx->stream));
-  int prc;
-  if ((prc = ensure(ctx, ctx->h_state, (size_t)n * sizeof(ReadState)))) return prc;
-  if ((prc = ensure(ctx, ctx->h_flags, (size_t)n * 4))) return prc;
-  if ((prc = ensure(ctx, ctx->h_hitdb, (size_t)n * 2))) return prc;
-  if ((prc = ensure(ctx, ctx->h_outaln, (size_t)n * slots * sizeof(OutAln)))) return prc;
-  const ReadState* st = (const ReadState*)ctx->h_state.p; const uint32_t* fl = (const uint32_t*)ctx->h_flags.p;
-  const uint16_t* hdb = (const uint16_t*)ctx->h_hitdb.p; const OutAln* oa = (const OutAln*)ctx->h_outaln.p;
+  const ReadState* st = ensure<ReadState>(ctx->h_state, (size_t)n * sizeof(ReadState));
+  const uint32_t* fl = ensure<uint32_t>(ctx->h_flags, (size_t)n * 4);
+  const uint16_t* hdb = ensure<uint16_t>(ctx->h_hitdb, (size_t)n * 2);
+  const OutAln* oa = ensure<OutAln>(ctx->h_outaln, (size_t)n * slots * sizeof(OutAln));
   const AlnStats* ast = nullptr;
   if (ctx->host_stats) {
-    if ((prc = ensure(ctx, ctx->h_stats, (size_t)n * slots * sizeof(AlnStats)))) return prc;
-    ast = (const AlnStats*)ctx->h_stats.p;
+    ast = ensure<AlnStats>(ctx->h_stats, (size_t)n * slots * sizeof(AlnStats));
     CK(cudaMemcpyAsync(ctx->h_stats.p, b.aln_stats.p, (size_t)n * slots * sizeof(AlnStats), cudaMemcpyDeviceToHost, ctx->stream));
   }
   unsigned long long used = 0;
@@ -915,20 +893,21 @@ int download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint32
   CK(cudaMemcpyAsync(cnt.data(), b.counters.p, cnt.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   used = std::min<unsigned long long>(used, b.cigar_cap_dev);
-  if ((prc = ensure(ctx, ctx->h_cigar, (size_t)used * 4 + 16))) return prc;
-  const uint32_t* cig = (const uint32_t*)ctx->h_cigar.p;
+  const uint32_t* cig = ensure<uint32_t>(ctx->h_cigar, (size_t)used * 4 + 16);
   if (used) CK(cudaMemcpyAsync(ctx->h_cigar.p, b.cigar_pool.p, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(e1, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_d2h = ms;
-  int rc = SMR_OK;
+  // a trace back error fails the call after what it can still write; the capacity errors below take precedence
+  bool trace_error = false;
+  auto fail_on_trace_error = [&] { if (trace_error) fail(SMR_ERR_INDEX, "trace back error (ssw.c:707 is fatal in the reference too)"); };
   // pass 1 (sequential, cheap): flagged reads, cigar offsets in the caller's pool (running sum in read order), counters
   std::vector<uint64_t>& coff = ctx->h_coff; coff.resize((size_t)n + 1);
   uint64_t run = out.cigar_used;
   uint32_t need_slots = 0;
   for (uint32_t r = 0; r < n; ++r) {
     coff[r] = run;
-    if (fl[r] & kErrTrace) { ctx->err = "trace back error (ssw.c:707 is fatal in the reference too)"; rc = SMR_ERR_INDEX; }
+    if (fl[r] & kErrTrace) trace_error = true;
     if (fl[r] & kOvfSlots) { need_slots = std::max(need_slots, st[r].n_align); continue; }   // not retried: the stride is the caller's
     if (fl[r]) { flagged.push_back(r); for (int bit = 0; bit < 6; ++bit) if (fl[r] & (1u << bit)) ctx->flag_hist[bit]++; continue; }
     const ReadState& s = st[r];
@@ -941,17 +920,16 @@ int download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint32
   }
   coff[n] = run;
   if (need_slots) {
-    ctx->err = "all-alignments mode: a read stored " + std::to_string(need_slots) + " alignments, the result stride is " + std::to_string(slots) +
-               " (smr_set_aln_slots(" + std::to_string(need_slots) + ") or more, then call again)";
     ctx->need_slots = need_slots;
-    return SMR_ERR_CAPACITY;
+    fail(SMR_ERR_CAPACITY, "all-alignments mode: a read stored " + std::to_string(need_slots) + " alignments, the result stride is " +
+                               std::to_string(slots) + " (smr_set_aln_slots(" + std::to_string(need_slots) + ") or more, then call again)");
   }
-  if (run >= 0xFFFFFFFFull) { ctx->err = "CIGAR pool offset passes 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches"; return SMR_ERR_CAPACITY; }
+  if (run >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, "CIGAR pool offset passes 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches");
   out.cigar_used = run;
-  // a pool too small fails the call only at its end (pool_short_error): the flagged reads are still retried, so that
+  // a pool too small fails the call only at its end (download_resident): the flagged reads are still retried, so that
   // cigar_used names every word the batch needs and one larger pool is enough
   if (run > out.cigar_cap) out.pool_short = true;
-  if (out.pool_short) return rc;
+  if (out.pool_short) { fail_on_trace_error(); return; }
   // pass 2: results, alignments and cigars of disjoint read ranges, by a few host threads for large batches
   auto pack = [&](uint32_t lo, uint32_t hi) {
     for (uint32_t r = lo; r < hi; ++r) {
@@ -991,108 +969,104 @@ int download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint32
                                   {20, dcSpecCells}, {21, dcSpecPairs}, {22, dcSlowPairs}, {23, dcScWait}, {24, dcScLoad}, {25, dcScSw}, {26, dcScPub}, {27, dcRoundsA}, {28, dcRoundsB}, {29, dcW1Cyc}, {30, dcW1Cnt}, {31, dcMaxReadBusy}};
     for (auto& m : mapc) if ((uint32_t)m[0] < out.n_counters) out.counters[m[0]] += cnt[m[1]];
   }
-  return rc;
+  fail_on_trace_error();
 }
 
 // Runs the flagged reads of a failed batch again as a batch of their own with 8x its scratch, gathered from its reads on the device,
 // and downloads them into the caller's arrays after what is there (map: index in `failed` -> the caller's index; null = the same).
 // Reads that overflow again go on to 64x and 512x.  The batch frees itself on return.
-int retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t>& flagged, const uint32_t* map, HostOut& out, int depth) {
+void retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t>& flagged, const uint32_t* map, HostOut& out, int depth) {
   if (getenv("SMR_VERBOSE")) fprintf(stderr, "[smr] %zu reads overflowed their scratch at scale %u: retrying with scale %u (causes so far: lane %llu region %llu pairs %llu trace %llu cigar %llu err %llu)\n", flagged.size(), failed.scale, failed.scale * 8,
       (unsigned long long)ctx->flag_hist[0], (unsigned long long)ctx->flag_hist[1], (unsigned long long)ctx->flag_hist[2], (unsigned long long)ctx->flag_hist[3], (unsigned long long)ctx->flag_hist[4], (unsigned long long)ctx->flag_hist[5]);
-  if (depth >= 3) { ctx->err = "scratch overflow persists after 3 retries (" + std::to_string(flagged.size()) + " reads)"; return SMR_ERR_CAPACITY; }
+  if (depth >= 3) fail(SMR_ERR_CAPACITY, "scratch overflow persists after 3 retries (" + std::to_string(flagged.size()) + " reads)");
   const uint32_t n = (uint32_t)flagged.size();
   std::vector<uint32_t> src(n), smap(n);
   for (uint32_t k = 0; k < n; ++k) { src[k] = failed.off32[flagged[k]]; smap[k] = map ? map[flagged[k]] : flagged[k]; }
   Batch b;
   b.scale = failed.scale * 8;
-  uint64_t w = 0;
-  int rc;
-  if ((rc = read_layout(ctx, b, n, [&](uint32_t k) { return failed.off32[flagged[k] + 1] - src[k]; }, &w))) return rc;
+  const uint64_t w = read_layout(ctx, b, n, [&](uint32_t k) { return failed.off32[flagged[k] + 1] - src[k]; });
   DevBuf d_src;
   CK(d_src.alloc((size_t)n * 4));
   CK(cudaMemcpyAsync(d_src.p, src.data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
-  if ((rc = ensure(ctx, b.seq04, b.total_nt + 64))) return rc;
+  ensure(b.seq04, b.total_nt + 64);
   gather_reads_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
       (const uint8_t*)failed.seq04.p, (const uint32_t*)d_src.p, n, (const uint32_t*)b.seq_off.p, (uint8_t*)b.seq04.p);
   CK(cudaGetLastError());
-  if ((rc = finish_upload(ctx, b, w)) || (rc = run_impl(ctx, b))) return rc;
+  finish_upload(ctx, b, w);
+  run_impl(ctx, b);
   const double d2h = ctx->t_d2h;
   std::vector<uint32_t> again;
-  rc = download_impl(ctx, b, out, again, smap.data());
+  download_impl(ctx, b, out, again, smap.data());
   ctx->t_run += b.run; ctx->t_d2h += d2h;
-  if (rc || again.empty()) return rc;
-  return retry_flagged(ctx, b, again, smap.data(), out, depth + 1);
+  if (!again.empty()) retry_flagged(ctx, b, again, smap.data(), out, depth + 1);
 }
 
 // the results of the resident batch's last run into the caller's arrays, its flagged reads retried; the resident batch and its
 // device results stay as they are
-int download_resident(smr_ctx* ctx, HostOut& out) {
+void download_resident(smr_ctx* ctx, HostOut& out) {
   ctx->t_run = ctx->resident.run;
   std::vector<uint32_t> flagged;
-  int rc = download_impl(ctx, ctx->resident, out, flagged, nullptr);
-  if (rc == SMR_OK && !flagged.empty()) {
-    rc = retry_flagged(ctx, ctx->resident, flagged, nullptr, out, 0);
-    // the arenas grew with the retry's scale (after 64x, tens of GB): the next run allocates them again at its own
-    for (DevBuf* s : {&ctx->lis_arena, &ctx->final_arena, &ctx->tb_arena, &ctx->lane_hits}) s->reset();
+  download_impl(ctx, ctx->resident, out, flagged, nullptr);
+  if (!flagged.empty()) {
+    // the arenas grow with the retry's scale (after 64x, tens of GB): the next run allocates them again at its own, whether the
+    // retry succeeds or not
+    const auto release = on_exit([ctx] { for (DevBuf* s : {&ctx->lis_arena, &ctx->final_arena, &ctx->tb_arena, &ctx->lane_hits}) s->reset(); });
+    retry_flagged(ctx, ctx->resident, flagged, nullptr, out, 0);
   }
-  if (rc == SMR_OK && out.pool_short) rc = pool_short_error(ctx, out);
-  return rc;
+  // the caller's CIGAR pool was too small: *cigar_used names the words the batch needs
+  if (out.pool_short)
+    fail(SMR_ERR_CAPACITY, "cigar pool too small: the batch needs " + std::to_string(out.cigar_used) + " words, cigar_cap is " + std::to_string(out.cigar_cap));
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // report writer (smr_report.cuh)
 // ---------------------------------------------------------------------------------------------------------------------
 template <class T>
-int upload_async(smr_ctx* ctx, DevBuf& b, const T* src, size_t n) {
-  int rc;
-  if ((rc = ensure(ctx, b, n * sizeof(T) + 16))) return rc;
+void upload_async(smr_ctx* ctx, DevBuf& b, const T* src, size_t n) {
+  ensure(b, n * sizeof(T) + 16);
   if (n) CK(cudaMemcpyAsync(b.p, src, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-  return SMR_OK;
 }
 
-int rpt_error(smr_ctx* ctx, uint32_t e) {
-  ctx->err = e & kRptErrLen ? "an alignment's readlen or read_end1 disagrees with the length of its read in the text"
-           : e & kRptErrGroup ? "an alignment names an (index, part) that is not loaded"
-           : e & kRptErrRef ? "an alignment's ref_num is beyond the reference names of its part"
-           : e & kRptErrQual ? "reads text: a FASTQ record without its quality line" : "an alignment's CIGAR lies outside cigar_words";
-  return SMR_ERR_ARG;
+[[noreturn]] void rpt_error(uint32_t e) {
+  fail(SMR_ERR_ARG, e & kRptErrLen ? "an alignment's readlen or read_end1 disagrees with the length of its read in the text"
+                    : e & kRptErrGroup ? "an alignment names an (index, part) that is not loaded"
+                    : e & kRptErrRef ? "an alignment's ref_num is beyond the reference names of its part"
+                    : e & kRptErrQual ? "reads text: a FASTQ record without its quality line" : "an alignment's CIGAR lies outside cigar_words");
 }
 
 // The first half of smr_format_reports and smr_otu_add: text, results and groups on the device (e1 recorded after the copies), the
-// record layout of the text (text_layout, then rpt_records_kernel) and the fields of `a` that describe them.
+// record layout of the text (text_layout, then rpt_records_kernel); returns the report arguments that describe them.
 // The report error word is [4] of ctx->d_scal.
-int rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar,
-                 uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads, const std::vector<RptGroup>& hg, cudaEvent_t e1, RptArgs& a) {
+RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar,
+                     uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads, const std::vector<RptGroup>& hg, cudaEvent_t e1) {
   const uint32_t slots = slots_of(ctx), G = (uint32_t)hg.size();
   const uint64_t N = (uint64_t)nreads * slots;
-  int rc;
   // the text
   const uint8_t* dt;
   if (text) {
-    if ((rc = upload_async(ctx, ctx->r_text, (const uint8_t*)text, nbytes))) return rc;
+    upload_async(ctx, ctx->r_text, (const uint8_t*)text, nbytes);
     dt = (const uint8_t*)ctx->r_text.p;
   } else {
-    if (!ctx->text_bytes) { ctx->err = "no resident text: smr_upload_fastx[_gz] was not called, or pass the text"; return SMR_ERR_ARG; }
+    if (!ctx->text_bytes) fail(SMR_ERR_ARG, "no resident text: smr_upload_fastx[_gz] was not called, or pass the text");
     nbytes = ctx->text_bytes;
     dt = (const uint8_t*)ctx->d_text.p;
   }
   char c0 = 0;
   if (nbytes) { if (text) c0 = text[0]; else CK(cudaMemcpy(&c0, dt, 1, cudaMemcpyDeviceToHost)); }
   // results
-  if ((rc = upload_async(ctx, ctx->r_res, results, nreads))) return rc;
-  if ((rc = upload_async(ctx, ctx->r_aln, alns, N))) return rc;
-  if ((rc = upload_async(ctx, ctx->r_cig, cigar, cigar ? cigar_words : 0))) return rc;
-  if ((rc = upload_async(ctx, ctx->r_st, stats, stats ? N : 0))) return rc;
-  if ((rc = upload_async(ctx, ctx->r_grp, hg.data(), G))) return rc;
+  upload_async(ctx, ctx->r_res, results, nreads);
+  upload_async(ctx, ctx->r_aln, alns, N);
+  upload_async(ctx, ctx->r_cig, cigar, cigar ? cigar_words : 0);
+  upload_async(ctx, ctx->r_st, stats, stats ? N : 0);
+  upload_async(ctx, ctx->r_grp, hg.data(), G);
   CK(cudaEventRecord(e1, ctx->stream));
-  TextLayout L;
-  if ((rc = text_layout(ctx, dt, nbytes, c0, L))) return rc;
-  if (L.nrec != nreads) { ctx->err = "the text holds " + std::to_string(L.nrec) + " records, the results " + std::to_string(nreads) + " reads"; return SMR_ERR_ARG; }
+  const TextLayout L = text_layout(ctx, dt, nbytes, c0);
+  if (L.nrec != nreads) fail(SMR_ERR_ARG, "the text holds " + std::to_string(L.nrec) + " records, the results " + std::to_string(nreads) + " reads");
   // per record
   const uint64_t fstride = (uint64_t)nreads + 1;
-  if ((rc = ensure(ctx, ctx->r_line, fstride * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_recs, fstride * sizeof(RptRec)))) return rc;
+  ensure(ctx->r_line, fstride * 4);
+  ensure(ctx->r_recs, fstride * sizeof(RptRec));
+  RptArgs a{};
   a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)ctx->d_nl.p; a.spos = (const uint32_t*)ctx->d_spos.p; a.nlines = L.nlines; a.fastq = L.fmt == kFmtFastq;
   a.rec = (const RptRec*)ctx->r_recs.p; a.nreads = nreads; a.slots = slots;
   a.res = (const smr_read_result*)ctx->r_res.p; a.aln = (const smr_aln*)ctx->r_aln.p; a.cigar = (const uint32_t*)ctx->r_cig.p;
@@ -1103,7 +1077,7 @@ int rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read
     rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->d_hdr.p, (const uint32_t*)ctx->d_rec.p, L.nlines, (uint32_t*)ctx->r_line.p);
     rpt_records_kernel<<<grid, 256, 0, ctx->stream>>>(a, (const uint32_t*)ctx->r_line.p, (RptRec*)ctx->r_recs.p);
   }
-  return SMR_OK;
+  return a;
 }
 
 // the loaded (index, part)s in the reference's report order (index, then part)
@@ -1118,31 +1092,30 @@ std::vector<const Part*> report_groups(const smr_ctx* ctx) {
 // gzip deflate (smr_deflate.cuh)
 // ---------------------------------------------------------------------------------------------------------------------
 // The streams [sb[k], se[k]) of the device bytes `in` (padded by >= 8 readable bytes), each non-empty one compressed to one gzip
-// member, into the host buffer `out` one after another; so[0 .. ns] = their offsets.  If the members do not fit in cap, returns
+// member, into the host buffer `out` one after another; so[0 .. ns] = their offsets.  If the members do not fit in cap, fails with
 // SMR_ERR_CAPACITY with so filled (a retry gives the same bytes).  e_dev is recorded before the D2H, e_end after it.
-int gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& sb, const std::vector<uint64_t>& se, char* out, uint64_t cap,
-                 uint64_t* so, cudaEvent_t e_dev, cudaEvent_t e_end) {
+void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& sb, const std::vector<uint64_t>& se, char* out, uint64_t cap,
+                  uint64_t* so, cudaEvent_t e_dev, cudaEvent_t e_end) {
   const uint32_t ns = (uint32_t)sb.size();
   std::vector<DefChunk> ch;
   def_plan(sb.data(), se.data(), ns, ch);
   const uint32_t nch = (uint32_t)ch.size();
-  int rc;
   std::vector<DefInfo> info(nch);
   std::vector<uint32_t> crcs(nch);
   if (nch) {
     const uint64_t end = se[ns - 1];
     std::vector<uint64_t> poff(nch); std::vector<uint32_t> plen(nch);
     for (uint32_t c = 0; c < nch; ++c) { poff[c] = ch[c].b; plen[c] = (uint32_t)(ch[c].e - ch[c].b); }
-    if ((rc = upload_async(ctx, ctx->z_chunk, ch.data(), nch))) return rc;
-    if ((rc = upload_async(ctx, ctx->z_poff, poff.data(), nch))) return rc;
-    if ((rc = upload_async(ctx, ctx->z_plen, plen.data(), nch))) return rc;
-    if ((rc = ensure(ctx, ctx->z_m, (end + 1) * 4))) return rc;
-    if ((rc = ensure(ctx, ctx->z_freq, (size_t)nch * kDefFreqStride * 4))) return rc;
-    if ((rc = ensure(ctx, ctx->z_codes, (size_t)nch * sizeof(DefCodes)))) return rc;
-    if ((rc = ensure(ctx, ctx->z_hdr, (size_t)nch * kDefHdrWords * 4))) return rc;
-    if ((rc = ensure(ctx, ctx->z_info, (size_t)nch * sizeof(DefInfo)))) return rc;
-    if ((rc = ensure(ctx, ctx->z_scratch, (size_t)nch * kDefScratch))) return rc;
-    if ((rc = ensure(ctx, ctx->z_crc, (size_t)nch * 4))) return rc;
+    upload_async(ctx, ctx->z_chunk, ch.data(), nch);
+    upload_async(ctx, ctx->z_poff, poff.data(), nch);
+    upload_async(ctx, ctx->z_plen, plen.data(), nch);
+    ensure(ctx->z_m, (end + 1) * 4);
+    ensure(ctx->z_freq, (size_t)nch * kDefFreqStride * 4);
+    ensure(ctx->z_codes, (size_t)nch * sizeof(DefCodes));
+    ensure(ctx->z_hdr, (size_t)nch * kDefHdrWords * 4);
+    ensure(ctx->z_info, (size_t)nch * sizeof(DefInfo));
+    ensure(ctx->z_scratch, (size_t)nch * kDefScratch);
+    ensure(ctx->z_crc, (size_t)nch * 4);
     CK(cudaMemsetAsync(ctx->z_freq.p, 0, (size_t)nch * kDefFreqStride * 4, ctx->stream));
     CK(cudaMemsetAsync(ctx->z_hdr.p, 0, (size_t)nch * kDefHdrWords * 4, ctx->stream));
     CK(cudaMemsetAsync(ctx->z_scratch.p, 0, (size_t)nch * kDefScratch, ctx->stream));
@@ -1175,11 +1148,11 @@ int gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& s
     at += 8;
   }
   so[ns] = at;
-  if (at && (!out || cap < at)) { ctx->err = "output buffer too small: stream_off holds the compressed sizes"; return SMR_ERR_CAPACITY; }
+  if (at && (!out || cap < at)) fail(SMR_ERR_CAPACITY, "output buffer too small: stream_off holds the compressed sizes");
   if (nch) {
-    if ((rc = upload_async(ctx, ctx->z_dst, dst.data(), nch))) return rc;
-    if ((rc = upload_async(ctx, ctx->z_trl, trl.data(), trl.size()))) return rc;
-    if ((rc = ensure(ctx, ctx->z_out, at))) return rc;
+    upload_async(ctx, ctx->z_dst, dst.data(), nch);
+    upload_async(ctx, ctx->z_trl, trl.data(), trl.size());
+    ensure(ctx->z_out, at);
     def_place_kernel<<<nch, 256, 0, ctx->stream>>>((const DefChunk*)ctx->z_chunk.p, (const DefInfo*)ctx->z_info.p, (const uint8_t*)ctx->z_scratch.p,
                                                    (const uint64_t*)ctx->z_dst.p, (const uint32_t*)ctx->z_trl.p, (uint8_t*)ctx->z_out.p);
     CK(cudaGetLastError());
@@ -1188,23 +1161,22 @@ int gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& s
   if (at) CK(cudaMemcpyAsync(out, ctx->z_out.p, at, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(e_end, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  return SMR_OK;
 }
 
-int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
-                        const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
-                        char* out, uint64_t cap, uint64_t* so_out, bool gz) {
-  if (o->out2 || o->sout) { ctx->err = "-out2 / -sout: the report writer writes one aligned and one other file"; return SMR_ERR_UNSUPPORTED; }
-  if (o->blast && o->blast_format != 1) { ctx->err = "only tabular BLAST (-blast 1) is written on the device"; return SMR_ERR_UNSUPPORTED; }
-  if (o->paired_in && o->paired_out) { ctx->err = "paired_in and paired_out are exclusive"; return SMR_ERR_ARG; }
+void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
+                         const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                         char* out, uint64_t cap, uint64_t* so_out, bool gz) {
+  if (o->out2 || o->sout) fail(SMR_ERR_UNSUPPORTED, "-out2 / -sout: the report writer writes one aligned and one other file");
+  if (o->blast && o->blast_format != 1) fail(SMR_ERR_UNSUPPORTED, "only tabular BLAST (-blast 1) is written on the device");
+  if (o->paired_in && o->paired_out) fail(SMR_ERR_ARG, "paired_in and paired_out are exclusive");
   const bool paired = o->paired_in || o->paired_out;
-  if (paired && (nreads & 1u)) { ctx->err = "a paired batch holds mates 2k and 2k+1: the number of reads must be even"; return SMR_ERR_ARG; }
-  if ((o->sam || o->blast || o->denovo) && nreads && !stats) { ctx->err = "SAM, BLAST and denovo need the smr_aln_stats of the batch"; return SMR_ERR_ARG; }
-  if (nreads && (!results || !alns)) return SMR_ERR_ARG;
+  if (paired && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
+  if ((o->sam || o->blast || o->denovo) && nreads && !stats) fail(SMR_ERR_ARG, "SAM, BLAST and denovo need the smr_aln_stats of the batch");
+  if (nreads && (!results || !alns)) fail(SMR_ERR_ARG, ctx->err);   // a null array: no text of its own, the last one stays
   uint32_t ncols = 0, cols[4] = {0, 0, 0, 0};
   if (o->blast)
     for (; ncols < 4 && o->blast_cols[ncols]; ++ncols) {
-      if (o->blast_cols[ncols] < SMR_BLAST_COL_CIGAR || o->blast_cols[ncols] > SMR_BLAST_COL_QSTRAND) { ctx->err = "unknown BLAST column"; return SMR_ERR_ARG; }
+      if (o->blast_cols[ncols] < SMR_BLAST_COL_CIGAR || o->blast_cols[ncols] > SMR_BLAST_COL_QSTRAND) fail(SMR_ERR_ARG, "unknown BLAST column");
       cols[ncols] = (uint32_t)o->blast_cols[ncols];
     }
   const std::vector<const Part*> gp = report_groups(ctx);
@@ -1212,72 +1184,63 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   std::vector<RptGroup> hg(G);
   for (uint32_t g = 0; g < G; ++g) {
     const Part& pt = *gp[g];
-    if ((o->sam || o->blast) && !pt.has_rnames) {
-      ctx->err = "smr_set_report_refs was not called for index " + std::to_string(pt.d.index_num) + " part " + std::to_string(pt.d.part);
-      return SMR_ERR_ARG;
-    }
+    if ((o->sam || o->blast) && !pt.has_rnames)
+      fail(SMR_ERR_ARG, "smr_set_report_refs was not called for index " + std::to_string(pt.d.index_num) + " part " + std::to_string(pt.d.part));
     const bool sc = pt.d.index_num < ctx->rpt_score.size() && ctx->rpt_score[pt.d.index_num].set;
-    if (o->blast && !sc) { ctx->err = "smr_set_report_scoring was not called for index " + std::to_string(pt.d.index_num); return SMR_ERR_ARG; }
+    if (o->blast && !sc) fail(SMR_ERR_ARG, "smr_set_report_scoring was not called for index " + std::to_string(pt.d.index_num));
     hg[g] = RptGroup{pt.rnames, pt.rname_off, sc ? (const double*)ctx->rpt_score[pt.d.index_num].ev.p : nullptr,
                      sc ? (const uint32_t*)ctx->rpt_score[pt.d.index_num].bits.p : nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0};
   }
   const uint32_t slots = slots_of(ctx);
   const uint64_t N = (uint64_t)nreads * slots;
-  if (N >= (1ull << 31)) { ctx->err = "batch too large for the report writer: split it"; return SMR_ERR_ARG; }
+  if (N >= (1ull << 31)) fail(SMR_ERR_ARG, "batch too large for the report writer: split it");
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
-  int rc;
   CK(cudaEventRecord(e0, ctx->stream));
-  RptArgs a{};
-  if ((rc = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e1, a))) return rc;
+  RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e1);
   const int grid = ctx->sm_count * 8;
   uint32_t* scal = (uint32_t*)ctx->d_scal.p;
   uint32_t h[8];
   // per record, routing, row order
   const uint64_t fstride = (uint64_t)nreads + 1;
-  if ((rc = ensure(ctx, ctx->r_flags, fstride * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_keys, (N + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_keys2, (N + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_vals, (N + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_rows, (N + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, ctx->r_first, ((size_t)G + 1) * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->r_sz, (N + 1) * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->r_off, (N + 1) * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->r_bsz, (N + 1) * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->r_boff, (N + 1) * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->r_fxsz, 3 * fstride * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->r_fxoff, 3 * fstride * 8))) return rc;
-  if ((rc = ensure(ctx, ctx->r_so, (size_t)nso * 8))) return rc;
+  uint32_t* flags = ensure<uint32_t>(ctx->r_flags, fstride * 4);
+  ensure(ctx->r_keys, (N + 1) * 4);
+  ensure(ctx->r_keys2, (N + 1) * 4);
+  ensure(ctx->r_vals, (N + 1) * 4);
+  const uint32_t* rows = ensure<uint32_t>(ctx->r_rows, (N + 1) * 4);
+  uint64_t* first = ensure<uint64_t>(ctx->r_first, ((size_t)G + 1) * 8);
+  uint64_t* sz = ensure<uint64_t>(ctx->r_sz, (N + 1) * 8);
+  uint64_t* off = ensure<uint64_t>(ctx->r_off, (N + 1) * 8);
+  uint64_t* bsz = ensure<uint64_t>(ctx->r_bsz, (N + 1) * 8);
+  uint64_t* boff = ensure<uint64_t>(ctx->r_boff, (N + 1) * 8);
+  uint64_t* fxsz = ensure<uint64_t>(ctx->r_fxsz, 3 * fstride * 8);
+  uint64_t* fxoff = ensure<uint64_t>(ctx->r_fxoff, 3 * fstride * 8);
+  uint64_t* so = ensure<uint64_t>(ctx->r_so, (size_t)nso * 8);
   for (int k = 0; k < 4; ++k) a.cols[k] = cols[k];
   a.ncols = ncols; a.min_id = o->min_id; a.min_cov = o->min_cov;
   a.paired_in = o->paired_in != 0; a.paired_out = o->paired_out != 0; a.denovo = o->denovo != 0;
   a.fx_mask = (o->fastx ? kRptAligned : 0u) | (o->other ? kRptOther : 0u) | (o->denovo ? kRptDenovo : 0u);
-  uint32_t* flags = (uint32_t*)ctx->r_flags.p;
-  uint64_t *first = (uint64_t*)ctx->r_first.p, *sz = (uint64_t*)ctx->r_sz.p, *off = (uint64_t*)ctx->r_off.p, *bsz = (uint64_t*)ctx->r_bsz.p,
-           *boff = (uint64_t*)ctx->r_boff.p, *fxsz = (uint64_t*)ctx->r_fxsz.p, *fxoff = (uint64_t*)ctx->r_fxoff.p, *so = (uint64_t*)ctx->r_so.p;
   CK(cudaMemsetAsync(sz, 0, (N + 1) * 8, ctx->stream));
   CK(cudaMemsetAsync(bsz, 0, (N + 1) * 8, ctx->stream));
   CK(cudaMemsetAsync(fxsz, 0, 3 * fstride * 8, ctx->stream));
   CK(cudaMemsetAsync(first, 0, ((size_t)G + 1) * 8, ctx->stream));
-  const uint32_t* rows = (const uint32_t*)ctx->r_rows.p;
   if (nreads) {
     rpt_route_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags);
     rpt_row_keys_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, (uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_vals.p);
     int nbits = 1;
     while ((1u << nbits) <= G) ++nbits;
-    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) {
-           return cub::DeviceRadixSort::SortPairs(t, b, (const uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_keys2.p, (const uint32_t*)ctx->r_vals.p,
-                                                  (uint32_t*)ctx->r_rows.p, (int)N, 0, nbits, ctx->stream);
-         })))
-      return rc;
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, (const uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_keys2.p, (const uint32_t*)ctx->r_vals.p,
+                                             (uint32_t*)ctx->r_rows.p, (int)N, 0, nbits, ctx->stream);
+    });
     rpt_group_first_kernel<<<(G + 128) / 128, 128, 0, ctx->stream>>>((const uint32_t*)ctx->r_keys2.p, N, G, first);
     if (o->sam) rpt_sam_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, sz);
     if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz, nullptr, nullptr);
     if (o->fastx || o->other || o->denovo) {
       rpt_fx_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, fxsz, fstride);
     }
-    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, sz, off, (int)(N + 1), ctx->stream); }))) return rc;
-    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, bsz, boff, (int)(N + 1), ctx->stream); }))) return rc;
-    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fxsz, fxoff, (int)(3 * fstride), ctx->stream); }))) return rc;
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, sz, off, (int)(N + 1), ctx->stream); });
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, bsz, boff, (int)(N + 1), ctx->stream); });
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fxsz, fxoff, (int)(3 * fstride), ctx->stream); });
   } else {
     CK(cudaMemsetAsync(off, 0, 8, ctx->stream));
     CK(cudaMemsetAsync(boff, 0, 8, ctx->stream));
@@ -1289,13 +1252,13 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   CK(cudaMemcpyAsync(hso.data(), so, (size_t)nso * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (h[4]) return rpt_error(ctx, h[4]);
+  if (h[4]) rpt_error(h[4]);
   if (!gz) memcpy(so_out, hso.data(), (size_t)nso * 8);
   const uint64_t total = hso[nso - 1];
-  if (!gz && total && (!out || cap < total)) { ctx->err = "output buffer too small: stream_off holds the sizes"; return SMR_ERR_CAPACITY; }
+  if (!gz && total && (!out || cap < total)) fail(SMR_ERR_CAPACITY, "output buffer too small: stream_off holds the sizes");
   // the encoder reads up to 8 bytes past a stream's end (def_load32): the padding is part of the one allocation before the writes,
   // since ensure() does not keep what a buffer held
-  if ((total || gz) && (rc = ensure(ctx, ctx->r_out, total + (gz ? 8 : 0)))) return rc;
+  if (total || gz) ensure(ctx->r_out, total + (gz ? 8 : 0));
   if (total) {
     char* dout = (char*)ctx->r_out.p;
     if (o->sam) rpt_sam_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, off, dout);
@@ -1305,8 +1268,7 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   }
   if (gz) {   // every non-empty stream to one gzip member, before the D2H
     std::vector<uint64_t> sb(hso.begin(), hso.end() - 1), se(hso.begin() + 1, hso.end());
-    rc = gzip_streams(ctx, (const uint8_t*)ctx->r_out.p, sb, se, out, cap, so_out, e2, e3);
-    if (rc) return rc;
+    gzip_streams(ctx, (const uint8_t*)ctx->r_out.p, sb, se, out, cap, so_out, e2, e3);
   } else {
     CK(cudaEventRecord(e2, ctx->stream));
     if (total) CK(cudaMemcpyAsync(out, ctx->r_out.p, total, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1317,14 +1279,13 @@ int format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text
   cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
   cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
   cudaEventElapsedTime(&ms, e2, e3); ctx->t_rpt[2] = ms;
-  return SMR_OK;
 }
 // ---------------------------------------------------------------------------------------------------------------------
 // OTU map (smr_otu.cuh)
 // ---------------------------------------------------------------------------------------------------------------------
 // device buffer grown to at least `need` bytes by doubling, keeping its first `used` bytes
-int grow_keep(smr_ctx* ctx, DevBuf& b, size_t used, size_t need) {
-  if (need <= b.cap && b.p) return SMR_OK;
+void grow_keep(smr_ctx* ctx, DevBuf& b, size_t used, size_t need) {
+  if (need <= b.cap && b.p) return;
   DevBuf nb;
   CK(nb.alloc(std::max<size_t>({need, 2 * b.cap, 4096})));
   if (used) {
@@ -1332,38 +1293,28 @@ int grow_keep(smr_ctx* ctx, DevBuf& b, size_t used, size_t need) {
     CK(cudaStreamSynchronize(ctx->stream));
   }
   b = std::move(nb);   // nb frees the old buffer
-  return SMR_OK;
 }
 
-int otu_open(smr_ctx* ctx) {
-  if (!ctx->otu.active) { ctx->err = "no open OTU map: call smr_otu_begin first"; return SMR_ERR_ARG; }
-  if (ctx->otu.gen != ctx->parts_gen) {
-    ctx->err = "an index part was loaded or its report ids were set after smr_otu_begin: begin the OTU map again";
-    return SMR_ERR_ARG;
-  }
-  return SMR_OK;
+void otu_open(smr_ctx* ctx) {
+  if (!ctx->otu.active) fail(SMR_ERR_ARG, "no open OTU map: call smr_otu_begin first");
+  if (ctx->otu.gen != ctx->parts_gen)
+    fail(SMR_ERR_ARG, "an index part was loaded or its report ids were set after smr_otu_begin: begin the OTU map again");
 }
 
-int otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
+void otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
   auto& U = ctx->otu;
   U.active = false;
-  if (!ctx->have_params || !ctx->prm.is_best) {
-    ctx->err = "the OTU map is made from the best alignments: params.is_best must be 1 (-otu_map cannot be set with -no-best)";
-    return SMR_ERR_ARG;
-  }
-  if (o->paired_in && o->paired_out) { ctx->err = "paired_in and paired_out are exclusive"; return SMR_ERR_ARG; }
-  if (o->paired_in || o->paired_out) {
-    ctx->err = "paired reads: the reference's OTU pass reads only the first mate file of two, but every record of one interleaved file, "
-               "so a paired batch does not say which map is meant";
-    return SMR_ERR_UNSUPPORTED;
-  }
+  if (!ctx->have_params || !ctx->prm.is_best)
+    fail(SMR_ERR_ARG, "the OTU map is made from the best alignments: params.is_best must be 1 (-otu_map cannot be set with -no-best)");
+  if (o->paired_in && o->paired_out) fail(SMR_ERR_ARG, "paired_in and paired_out are exclusive");
+  if (o->paired_in || o->paired_out)
+    fail(SMR_ERR_UNSUPPORTED, "paired reads: the reference's OTU pass reads only the first mate file of two, but every record of one interleaved file, "
+                              "so a paired batch does not say which map is meant");
   const std::vector<const Part*> gp = report_groups(ctx);
   const uint32_t G = (uint32_t)gp.size();
   for (const Part* pt : gp)
-    if (!pt->has_rnames) {
-      ctx->err = "smr_set_report_refs was not called for index " + std::to_string(pt->d.index_num) + " part " + std::to_string(pt->d.part);
-      return SMR_ERR_ARG;
-    }
+    if (!pt->has_rnames)
+      fail(SMR_ERR_ARG, "smr_set_report_refs was not called for index " + std::to_string(pt->d.index_num) + " part " + std::to_string(pt->d.part));
   // ranks of the reference ids in unsigned byte order (std::string compares as unsigned char)
   std::vector<const std::string*> ids;
   for (const Part* pt : gp) for (const std::string& s : pt->h_rnames) ids.push_back(&s);
@@ -1381,10 +1332,9 @@ int otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
   uint32_t gbits = 1, rbits = 1;
   while ((1ull << gbits) <= G) ++gbits;
   while ((1ull << rbits) <= ids.size()) ++rbits;
-  int rc;
-  if ((rc = upload_async(ctx, U.rank, rank.data(), rank.size()))) return rc;
-  if ((rc = upload_async(ctx, U.rank_off, rank_off.data(), rank_off.size()))) return rc;
-  if ((rc = upload_async(ctx, U.grp, U.groups.data(), G))) return rc;
+  upload_async(ctx, U.rank, rank.data(), rank.size());
+  upload_async(ctx, U.rank_off, rank_off.data(), rank_off.size());
+  upload_async(ctx, U.grp, U.groups.data(), G);
   CK(cudaStreamSynchronize(ctx->stream));
   U.gbits = gbits; U.kbits = gbits + rbits;
   U.min_id = o->min_id; U.min_cov = o->min_cov;
@@ -1392,94 +1342,85 @@ int otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
   for (double& t : U.t) t = 0;
   U.gen = ctx->parts_gen;
   U.active = true;
-  return SMR_OK;
 }
 
-int otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
-                 uint32_t nreads, uint64_t* n_added) {
+// returns the number of entries added
+uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
+                      uint32_t nreads) {
   auto& U = ctx->otu;
-  int rc;
-  if ((rc = otu_open(ctx))) return rc;
-  if (nreads && (!results || !alns || !stats)) { ctx->err = "the OTU map needs the results, alignments and smr_aln_stats of the batch"; return SMR_ERR_ARG; }
+  otu_open(ctx);
+  if (nreads && (!results || !alns || !stats)) fail(SMR_ERR_ARG, "the OTU map needs the results, alignments and smr_aln_stats of the batch");
   const uint32_t slots = slots_of(ctx);
   const uint64_t N = (uint64_t)nreads * slots;
-  if (N >= (1ull << 31)) { ctx->err = "batch too large for the OTU map: split it"; return SMR_ERR_ARG; }
+  if (N >= (1ull << 31)) fail(SMR_ERR_ARG, "batch too large for the OTU map: split it");
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
   CK(cudaEventRecord(e0, ctx->stream));
-  RptArgs a{};
-  if ((rc = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e1, a))) return rc;
+  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e1);
   const OtuArgs oa{(const uint32_t*)U.rank.p, (const uint32_t*)U.rank_off.p, U.gbits, U.min_id, U.min_cov};
-  if ((rc = ensure(ctx, U.flag, (N + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, U.pos, (N + 1) * 4))) return rc;
-  if ((rc = ensure(ctx, U.nsz, (N + 1) * 8))) return rc;
-  if ((rc = ensure(ctx, U.noff, (N + 1) * 8))) return rc;
-  uint32_t *flag = (uint32_t*)U.flag.p, *pos = (uint32_t*)U.pos.p;
-  uint64_t *nsz = (uint64_t*)U.nsz.p, *noff = (uint64_t*)U.noff.p;
+  uint32_t* flag = ensure<uint32_t>(U.flag, (N + 1) * 4);
+  uint32_t* pos = ensure<uint32_t>(U.pos, (N + 1) * 4);
+  uint64_t* nsz = ensure<uint64_t>(U.nsz, (N + 1) * 8);
+  uint64_t* noff = ensure<uint64_t>(U.noff, (N + 1) * 8);
   const int grid = ctx->sm_count * 8;
   CK(cudaMemsetAsync(flag + N, 0, 4, ctx->stream));
   CK(cudaMemsetAsync(nsz + N, 0, 8, ctx->stream));
   otu_flag_kernel<<<grid, 256, 0, ctx->stream>>>(a, oa, flag, nsz);
-  if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, flag, pos, (int)(N + 1), ctx->stream); }))) return rc;
-  if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, nsz, noff, (int)(N + 1), ctx->stream); }))) return rc;
+  cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, flag, pos, (int)(N + 1), ctx->stream); });
+  cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, nsz, noff, (int)(N + 1), ctx->stream); });
   CK(cudaGetLastError());
   uint32_t m = 0, err = 0; uint64_t bytes = 0;
   CK(cudaMemcpyAsync(&m, pos + N, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(&bytes, noff + N, 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(&err, (uint32_t*)ctx->d_scal.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (err) return rpt_error(ctx, err);
-  if (U.n + m >= (1ull << 31)) { ctx->err = "OTU map of 2^31 entries or more"; return SMR_ERR_CAPACITY; }
-  if ((rc = grow_keep(ctx, U.key, U.n * 8, (U.n + m) * 8))) return rc;
-  if ((rc = grow_keep(ctx, U.ent, U.n * sizeof(OtuEnt), (U.n + m) * sizeof(OtuEnt)))) return rc;
-  if ((rc = grow_keep(ctx, U.pool, U.pool_bytes, U.pool_bytes + bytes))) return rc;
+  if (err) rpt_error(err);
+  if (U.n + m >= (1ull << 31)) fail(SMR_ERR_CAPACITY, "OTU map of 2^31 entries or more");
+  grow_keep(ctx, U.key, U.n * 8, (U.n + m) * 8);
+  grow_keep(ctx, U.ent, U.n * sizeof(OtuEnt), (U.n + m) * sizeof(OtuEnt));
+  grow_keep(ctx, U.pool, U.pool_bytes, U.pool_bytes + bytes);
   if (m) otu_append_kernel<<<grid, 256, 0, ctx->stream>>>(a, oa, flag, pos, noff, U.n, U.pool_bytes, (uint64_t*)U.key.p, (OtuEnt*)U.ent.p, (char*)U.pool.p);
   CK(cudaGetLastError());
   CK(cudaEventRecord(e2, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   U.n += m; U.pool_bytes += bytes;
-  if (n_added) *n_added = m;
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1); U.t[0] += ms;
   cudaEventElapsedTime(&ms, e1, e2); U.t[1] += ms;
-  return SMR_OK;
+  return m;
 }
 
-int otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) {
+void otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) {
   auto& U = ctx->otu;
-  int rc;
-  if ((rc = otu_open(ctx))) return rc;
+  otu_open(ctx);
   const uint64_t m = U.n;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
   CK(cudaEventRecord(e0, ctx->stream));
   uint64_t bytes = 0; uint32_t runs = 0;
   const int grid = ctx->sm_count * 8;
   if (m) {
-    if ((rc = ensure(ctx, U.vals, m * 4))) return rc;
-    if ((rc = ensure(ctx, U.sidx, m * 4))) return rc;
-    if ((rc = ensure(ctx, U.skey, m * 8))) return rc;
-    if ((rc = ensure(ctx, U.size, (m + 1) * 8))) return rc;
-    if ((rc = ensure(ctx, U.off, (m + 1) * 8))) return rc;
-    if ((rc = ensure(ctx, U.scal, 16))) return rc;
-    uint64_t *skey = (uint64_t*)U.skey.p, *size = (uint64_t*)U.size.p, *off = (uint64_t*)U.off.p;
-    uint32_t *sidx = (uint32_t*)U.sidx.p, *scal = (uint32_t*)U.scal.p;
-    otu_iota_kernel<<<grid, 256, 0, ctx->stream>>>((uint32_t*)U.vals.p, m);
-    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) {
-           return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)U.key.p, skey, (const uint32_t*)U.vals.p, sidx, (int)m, 0, (int)U.kbits, ctx->stream);
-         })))
-      return rc;
+    uint32_t* vals = ensure<uint32_t>(U.vals, m * 4);
+    uint32_t* sidx = ensure<uint32_t>(U.sidx, m * 4);
+    uint64_t* skey = ensure<uint64_t>(U.skey, m * 8);
+    uint64_t* size = ensure<uint64_t>(U.size, (m + 1) * 8);
+    uint64_t* off = ensure<uint64_t>(U.off, (m + 1) * 8);
+    uint32_t* scal = ensure<uint32_t>(U.scal, 16);
+    otu_iota_kernel<<<grid, 256, 0, ctx->stream>>>(vals, m);
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) {
+      return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)U.key.p, skey, (const uint32_t*)vals, sidx, (int)m, 0, (int)U.kbits, ctx->stream);
+    });
     CK(cudaMemsetAsync(scal, 0, 16, ctx->stream));
     CK(cudaMemsetAsync(size + m, 0, 8, ctx->stream));
     otu_size_kernel<<<grid, 256, 0, ctx->stream>>>(skey, sidx, (const OtuEnt*)U.ent.p, m, U.gbits, (const RptGroup*)U.grp.p, size, scal);
-    if ((rc = cub_run(ctx, ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, size, off, (int)(m + 1), ctx->stream); }))) return rc;
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, size, off, (int)(m + 1), ctx->stream); });
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(&bytes, off + m, 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaMemcpyAsync(&runs, scal, 4, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
   counts[0] = bytes; counts[1] = runs; counts[2] = m;
-  if (bytes && (!out || cap < bytes)) { ctx->err = "output buffer too small: counts[0] holds the size"; return SMR_ERR_CAPACITY; }
+  if (bytes && (!out || cap < bytes)) fail(SMR_ERR_CAPACITY, "output buffer too small: counts[0] holds the size");
   if (bytes) {
-    if ((rc = ensure(ctx, U.out, bytes))) return rc;
+    ensure(U.out, bytes);
     otu_write_kernel<<<grid, 256, 0, ctx->stream>>>((const uint64_t*)U.skey.p, (const uint32_t*)U.sidx.p, (const OtuEnt*)U.ent.p, m, U.gbits,
                                                     (const RptGroup*)U.grp.p, (const char*)U.pool.p, (const uint64_t*)U.off.p, (char*)U.out.p);
     CK(cudaGetLastError());
@@ -1490,16 +1431,15 @@ int otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) {
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1); U.t[2] = ms;
   U.active = false;
-  return SMR_OK;
 }
 
 }  // namespace
 
 extern "C" {
 
-// No exception crosses the C ABI: the batch entry points below are function-try-blocks that turn a failed host allocation (the result
-// vectors of a 2^32-nt batch, the retry copies) or any other std::exception into a status and an error text.
+// Internal code throws; every entry point that can fail is a function-try-block that turns the failure into a status and an error text here.
 #define SMR_CATCH(ctx) \
+  catch (const Failure& f) { (ctx)->err = f.msg; return f.code; } \
   catch (const std::bad_alloc&) { if (ctx) (ctx)->err = "out of host memory"; return SMR_ERR_CAPACITY; } \
   catch (const std::exception& ex) { if (ctx) (ctx)->err = std::string("internal error: ") + ex.what(); return SMR_ERR_CUDA; }
 
@@ -1509,7 +1449,7 @@ int smr_device_count(void) {
   return n;
 }
 
-int smr_init(int device, smr_ctx** out) {
+int smr_init(int device, smr_ctx** out) try {
   if (!out) return SMR_ERR_ARG;
   *out = nullptr;
   int n = 0;
@@ -1526,7 +1466,7 @@ int smr_init(int device, smr_ctx** out) {
   if (const char* e = getenv("SMR_LIS_CTAS_PER_SM")) { const int v = atoi(e); if (v >= 1 && v <= 16) ctx->lis_ctas_per_sm = (uint32_t)v; }
   *out = ctx;
   return SMR_OK;
-}
+} catch (const std::bad_alloc&) { return SMR_ERR_CAPACITY; } catch (const std::exception&) { return SMR_ERR_CUDA; }
 
 void smr_destroy(smr_ctx* ctx) {
   if (!ctx) return;
@@ -1541,7 +1481,7 @@ const char* smr_last_error(const smr_ctx* ctx) { return ctx ? ctx->err.c_str() :
 int smr_load_index_part(smr_ctx* ctx, uint32_t index_num, uint32_t part, const void* kmer_file, size_t kmer_bytes,
                         const void* bursttrie_file, size_t bursttrie_bytes, const void* pos_file, size_t pos_bytes,
                         const uint8_t* refseq_cat, const uint64_t* ref_off, uint32_t nref, uint32_t lnwin, uint32_t minimal_score,
-                        const uint32_t skiplengths[3]) {
+                        const uint32_t skiplengths[3]) try {
   if (!ctx || !kmer_file || !bursttrie_file || !pos_file || !refseq_cat || !ref_off || !skiplengths) return SMR_ERR_ARG;
   if (skiplengths[0] == 0 || skiplengths[1] == 0 || skiplengths[2] == 0) { ctx->err = "skiplengths must be positive"; return SMR_ERR_ARG; }
   CK(cudaSetDevice(ctx->device));
@@ -1564,29 +1504,24 @@ int smr_load_index_part(smr_ctx* ctx, uint32_t index_num, uint32_t part, const v
   rseq.resize(rseq.size() + 64, 4);
   std::vector<uint32_t> ftext(ftext_words(fx.flist.size()), 0), fid(fx.flist.size());
   for (size_t i = 0; i < fx.flist.size(); ++i) { ftext[i] = fx.flist[i].tail; fid[i] = fx.flist[i].id; }   // an flist item's tail holds the full text
-  int rc;
-  const uint32_t *lk = nullptr, *ft = nullptr, *fi = nullptr, *po = nullptr; const SeqPos* ps = nullptr;
-  const uint8_t* rs = nullptr; const uint32_t* ro = nullptr;
-  if ((rc = part_array(ctx, pt, fx.flookup.size(), fx.flookup.data(), &lk))) return rc;
-  if ((rc = part_array(ctx, pt, ftext.size(), ftext.data(), &ft))) return rc;
-  if ((rc = part_array(ctx, pt, fid.size(), fid.data(), &fi))) return rc;
-  if ((rc = part_array(ctx, pt, fx.pos_off.size(), fx.pos_off.data(), &po))) return rc;
-  if ((rc = part_array(ctx, pt, fx.pos.size(), fx.pos.data(), &ps))) return rc;
-  if ((rc = part_array(ctx, pt, rseq.size(), rseq.data(), &rs))) return rc;
-  if ((rc = part_array(ctx, pt, roff.size(), roff.data(), &ro))) return rc;
+  pt.d.flookup = (const uint4*)part_array<uint32_t>(ctx, pt, fx.flookup.size(), fx.flookup.data());
+  pt.d.ftext = part_array<uint32_t>(ctx, pt, ftext.size(), ftext.data());
+  pt.d.fid = part_array<uint32_t>(ctx, pt, fid.size(), fid.data());
+  pt.d.pos_off = part_array<uint32_t>(ctx, pt, fx.pos_off.size(), fx.pos_off.data());
+  pt.d.pos = (const uint2*)part_array<SeqPos>(ctx, pt, fx.pos.size(), fx.pos.data());
+  pt.d.refseq = part_array<uint8_t>(ctx, pt, rseq.size(), rseq.data());
+  pt.d.ref_off = part_array<uint32_t>(ctx, pt, roff.size(), roff.data());
   CK(cudaStreamSynchronize(ctx->stream));
-  pt.d.flookup = (const uint4*)lk; pt.d.ftext = ft; pt.d.fid = fi; pt.d.pos_off = po; pt.d.pos = (const uint2*)ps;
-  pt.d.refseq = rs; pt.d.ref_off = ro;
   pt.n_refseq = rseq.size();
   pt.n_nodes = fx.nodes.size(); pt.n_entries = fx.entries.size(); pt.n_ids = pt.d.nids; pt.n_pos = fx.pos.size();
   ctx->parts.push_back(std::move(pt));
   ctx->n_index_files = std::max(ctx->n_index_files, index_num + 1);
   ++ctx->parts_gen;
   return SMR_OK;
-}
+} SMR_CATCH(ctx)
 
 int smr_build_index_device(smr_ctx* ctx, uint32_t index_num, const char* fasta_path, uint32_t lnwin, uint32_t interval, uint32_t max_pos, double max_mb,
-                           const uint32_t skiplengths[3], uint32_t minimal_score, uint32_t* nparts, uint64_t report6[6]) {
+                           const uint32_t skiplengths[3], uint32_t minimal_score, uint32_t* nparts, uint64_t report6[6]) try {
   if (!ctx || !fasta_path || !skiplengths) return SMR_ERR_ARG;
   if (skiplengths[0] == 0 || skiplengths[1] == 0 || skiplengths[2] == 0) { ctx->err = "skiplengths must be positive"; return SMR_ERR_ARG; }
   if (lnwin < 8 || lnwin > 26 || (lnwin & 1)) { ctx->err = "unsupported seed length"; return SMR_ERR_ARG; }
@@ -1609,8 +1544,7 @@ int smr_build_index_device(smr_ctx* ctx, uint32_t index_num, const char* fasta_p
     e = next_index_part(recs, first, lnwin + 1, max_mb, members, next, start_part, seq_part_size);
     if (!e.empty()) { ctx->err = e; return SMR_ERR_INDEX; }
     if (members.empty()) break;
-    Part pt;
-    if (int rc = build_part_device(ctx, recs, members, opt, pt)) return rc;
+    Part pt = build_part_device(ctx, recs, members, opt);
     pt.d.index_num = index_num; pt.d.part = part; pt.d.minimal_score = minimal_score;
     for (int i = 0; i < 3; ++i) pt.d.skip[i] = skiplengths[i];
     rep[3] += pt.n_ids; rep[5] += pt.bytes;
@@ -1624,9 +1558,9 @@ int smr_build_index_device(smr_ctx* ctx, uint32_t index_num, const char* fasta_p
   if (nparts) *nparts = part;
   if (report6) memcpy(report6, rep, sizeof(rep));
   return SMR_OK;
-}
+} SMR_CATCH(ctx)
 
-int smr_debug_index_array(smr_ctx* ctx, uint32_t slot, uint32_t which, void* out, uint64_t cap_bytes, uint64_t* nbytes) {
+int smr_debug_index_array(smr_ctx* ctx, uint32_t slot, uint32_t which, void* out, uint64_t cap_bytes, uint64_t* nbytes) try {
   if (!ctx || !nbytes || slot >= ctx->parts.size()) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   const Part& pt = ctx->parts[slot];
@@ -1653,7 +1587,7 @@ int smr_debug_index_array(smr_ctx* ctx, uint32_t slot, uint32_t which, void* out
   }
   if (n) CK(cudaMemcpy(out, src, n, cudaMemcpyDeviceToHost));
   return SMR_OK;
-}
+} SMR_CATCH(ctx)
 
 int smr_set_minimal_score(smr_ctx* ctx, uint32_t index_num, uint32_t minimal_score) {
   if (!ctx) return SMR_ERR_ARG;
@@ -1695,11 +1629,11 @@ int smr_align_batch(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_of
   memset(results, 0, (size_t)nreads * sizeof(smr_read_result));
   memset(alns, 0, (size_t)nreads * slots * sizeof(smr_aln));
   HostOut out{results, alns, cigar_pool, cigar_cap, 0, counters, n_counters};
-  int rc = upload_batch_impl(ctx, seq_cat, seq_off, nreads);
-  if (rc == SMR_OK) rc = run_impl(ctx, ctx->resident);
-  if (rc == SMR_OK) rc = download_resident(ctx, out);
-  if (cigar_used) *cigar_used = out.cigar_used;
-  return rc;
+  const auto put_used = on_exit([&] { if (cigar_used) *cigar_used = out.cigar_used; });   // a pool too small fails, and names the words needed
+  upload_batch_impl(ctx, seq_cat, seq_off, nreads);
+  run_impl(ctx, ctx->resident);
+  download_resident(ctx, out);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_set_instrumentation(smr_ctx* ctx, int on) {
@@ -1717,32 +1651,34 @@ int smr_set_stats_buffer(smr_ctx* ctx, smr_aln_stats* stats) {
 int smr_upload_batch(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads) try {
   if (!ctx || !seq_cat || !seq_off) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  return upload_batch_impl(ctx, seq_cat, seq_off, nreads);
+  upload_batch_impl(ctx, seq_cat, seq_off, nreads);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_upload_fastx(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t* nreads) try {
   if (!ctx || (!text && nbytes) || !nreads) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  return upload_fastx_impl(ctx, text, nbytes, nreads);
+  *nreads = 0;   // as it stays if the upload fails
+  *nreads = upload_fastx_impl(ctx, text, nbytes);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_upload_fastx_gz(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint32_t* nreads) try {
   if (!ctx || !gz || !nreads) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   *nreads = 0; ctx->resident.nreads = 0; ctx->text_bytes = 0;
-  uint64_t total = 0;
   const char* e = getenv("SMR_INFLATE_CHUNK");
   // distance of the speculative block searches: 64 KB for large files, down to 8 KB so that a small file still makes thousands of spans
   const uint64_t chunk = e ? strtoull(e, nullptr, 10) : std::min<uint64_t>(65536, std::max<uint64_t>(8192, nbytes / 8192));
-  int rc = inflate_impl(ctx, gz, nbytes, chunk, &total);
-  if (rc) return rc;
+  const uint64_t total = inflate_impl(ctx, gz, nbytes, chunk);
   if (total == 0) return SMR_OK;
   char c0 = 0;
   CK(cudaMemcpy(&c0, ctx->d_text.p, 1, cudaMemcpyDeviceToHost));
-  return upload_fastx_impl(ctx, nullptr, total, nreads, c0);
+  *nreads = upload_fastx_impl(ctx, nullptr, total, c0);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
-int smr_resident_text(smr_ctx* ctx, char* text, uint64_t cap, uint64_t* nbytes) {
+int smr_resident_text(smr_ctx* ctx, char* text, uint64_t cap, uint64_t* nbytes) try {
   if (!ctx || !nbytes) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   *nbytes = ctx->text_bytes;
@@ -1750,15 +1686,15 @@ int smr_resident_text(smr_ctx* ctx, char* text, uint64_t cap, uint64_t* nbytes) 
   if (cap < ctx->text_bytes) { ctx->err = "text buffer too small"; return SMR_ERR_CAPACITY; }
   CK(cudaMemcpy(text, ctx->d_text.p, ctx->text_bytes, cudaMemcpyDeviceToHost));
   return SMR_OK;
-}
+} SMR_CATCH(ctx)
 
 int smr_debug_inflate(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_bytes, uint32_t info[4]) try {
   if (!ctx || !gz || !out_bytes) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   ctx->resident.nreads = 0; ctx->text_bytes = 0;
   if (chunk_bytes == 0) chunk_bytes = std::min<uint64_t>(65536, std::max<uint64_t>(8192, nbytes / 8192));   // as smr_upload_fastx_gz
-  int rc = inflate_impl(ctx, gz, nbytes, chunk_bytes, out_bytes);
-  if (rc) return rc;
+  *out_bytes = 0;   // as it stays if the inflate fails
+  *out_bytes = inflate_impl(ctx, gz, nbytes, chunk_bytes);
   if (info) { info[0] = ctx->inf_spans; info[1] = ctx->inf_candidates; info[2] = (uint32_t)(ctx->t_inflate * 1000.0); info[3] = (uint32_t)(ctx->t_h2d * 1000.0); }
   if (out && *out_bytes) {
     if (out_cap < *out_bytes) { ctx->err = "output buffer too small"; return SMR_ERR_CAPACITY; }
@@ -1787,9 +1723,9 @@ int smr_resident_layout(smr_ctx* ctx, uint64_t* header_text_off, uint64_t* read_
 int smr_run_resident(smr_ctx* ctx) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  const int rc = run_impl(ctx, ctx->resident);
+  run_impl(ctx, ctx->resident);
   ctx->t_run = ctx->resident.run;
-  return rc;
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used,
@@ -1801,9 +1737,9 @@ int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, 
   memset(results, 0, (size_t)n * sizeof(smr_read_result));
   memset(alns, 0, (size_t)n * slots * sizeof(smr_aln));
   HostOut out{results, alns, cigar_pool, cigar_cap, 0, counters, n_counters};
-  const int rc = download_resident(ctx, out);
-  if (cigar_used) *cigar_used = out.cigar_used;
-  return rc;
+  const auto put_used = on_exit([&] { if (cigar_used) *cigar_used = out.cigar_used; });   // a pool too small fails, and names the words needed
+  download_resident(ctx, out);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_set_report_refs(smr_ctx* ctx, uint32_t index_num, uint32_t part, const char* names_cat, const uint64_t* name_off, uint32_t nref) try {
@@ -1814,9 +1750,8 @@ int smr_set_report_refs(smr_ctx* ctx, uint32_t index_num, uint32_t part, const c
     if (nref != pt.d.nref) { ctx->err = "smr_set_report_refs: " + std::to_string(nref) + " names for a part of " + std::to_string(pt.d.nref) + " references"; return SMR_ERR_ARG; }
     std::vector<char> names(names_cat, names_cat + name_off[nref]);
     std::vector<uint64_t> off(name_off, name_off + nref + 1);
-    int rc;
-    if ((rc = part_array(ctx, pt, names.size(), names.data(), &pt.rnames))) return rc;
-    if ((rc = part_array(ctx, pt, off.size(), off.data(), &pt.rname_off))) return rc;
+    pt.rnames = part_array<char>(ctx, pt, names.size(), names.data());
+    pt.rname_off = part_array<uint64_t>(ctx, pt, off.size(), off.data());
     CK(cudaStreamSynchronize(ctx->stream));
     pt.n_rnames = nref; pt.has_rnames = true;
     pt.h_rnames.resize(nref);
@@ -1840,9 +1775,8 @@ int smr_set_report_scoring(smr_ctx* ctx, uint32_t index_num, double lambda, doub
     bits[s] = b > 0 ? (uint32_t)b : 0u;
     ev[s] = (double)K * full_ref * full_read * std::exp(-lambda * s);
   }
-  int rc;
-  if ((rc = ensure(ctx, sc.ev, ev.size() * 8))) return rc;
-  if ((rc = ensure(ctx, sc.bits, bits.size() * 4))) return rc;
+  ensure(sc.ev, ev.size() * 8);
+  ensure(sc.bits, bits.size() * 4);
   CK(cudaMemcpy(sc.ev.p, ev.data(), ev.size() * 8, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(sc.bits.p, bits.data(), bits.size() * 4, cudaMemcpyHostToDevice));
   sc.set = true;
@@ -1854,7 +1788,8 @@ int smr_format_reports(smr_ctx* ctx, const smr_report_opts* opts, const char* te
                        char* out, uint64_t cap, uint64_t* stream_off) try {
   if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  return format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, false);
+  format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, false);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_format_reports_gz(smr_ctx* ctx, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
@@ -1862,7 +1797,8 @@ int smr_format_reports_gz(smr_ctx* ctx, const smr_report_opts* opts, const char*
                           char* out, uint64_t cap, uint64_t* stream_off) try {
   if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  return format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, true);
+  format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, true);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_gzip(smr_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t cap, uint64_t* out_bytes) try {
@@ -1878,15 +1814,15 @@ int smr_gzip(smr_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t cap, 
     ctx->t_rpt[0] = ctx->t_rpt[1] = ctx->t_rpt[2] = 0;
     return SMR_OK;
   }
-  int rc;
-  if ((rc = ensure(ctx, ctx->z_in, n + 64))) return rc;
+  ensure(ctx->z_in, n + 64);
   CK(cudaMemsetAsync((uint8_t*)ctx->z_in.p + n, 0, 64, ctx->stream));
   CK(cudaMemcpyAsync(ctx->z_in.p, in, n, cudaMemcpyHostToDevice, ctx->stream));
   CK(cudaEventRecord(e1, ctx->stream));
-  uint64_t so[2];
-  rc = gzip_streams(ctx, (const uint8_t*)ctx->z_in.p, {0}, {n}, (char*)out, cap, so, e2, e3);
-  *out_bytes = so[1];
-  if (rc) return rc;
+  uint64_t so[2] = {0, 0};
+  {
+    const auto put_size = on_exit([&] { *out_bytes = so[1]; });   // a buffer too small fails, and names the size needed
+    gzip_streams(ctx, (const uint8_t*)ctx->z_in.p, {0}, {n}, (char*)out, cap, so, e2, e3);
+  }
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
   cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
@@ -1907,7 +1843,7 @@ int smr_last_timings(const smr_ctx* ctx, double out[8]) {
   return SMR_OK;
 }
 
-int smr_debug_dpx_peak(smr_ctx* ctx, double* giga_ops_per_s) {
+int smr_debug_dpx_peak(smr_ctx* ctx, double* giga_ops_per_s) try {
   if (!ctx || !giga_ops_per_s) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   DevBuf d;
@@ -1927,11 +1863,11 @@ int smr_debug_dpx_peak(smr_ctx* ctx, double* giga_ops_per_s) {
   }
   *giga_ops_per_s = best;
   return SMR_OK;
-}
+} SMR_CATCH(ctx)
 
 int smr_debug_seed_windows(smr_ctx* ctx, uint32_t part_slot, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads,
                            const uint32_t* win_read, const uint32_t* win_pos, uint32_t nwin, uint32_t* ids, uint32_t cap, uint32_t* counts,
-                           uint8_t* zero) {
+                           uint8_t* zero) try {
   if (!ctx || part_slot >= ctx->parts.size() || !seq_cat || !seq_off || !win_read || !win_pos || !ids || !counts || !zero) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   const uint32_t cap_arg = cap;
@@ -1940,10 +1876,10 @@ int smr_debug_seed_windows(smr_ctx* ctx, uint32_t part_slot, const uint8_t* seq_
   std::vector<uint32_t> off32(nreads + 1);
   for (uint32_t r = 0; r <= nreads; ++r) off32[r] = (uint32_t)(seq_off[r] - seq_off[0]);
   std::vector<DevBuf> tmp;
-  uint8_t *d_seq, *d_zero; uint32_t *d_off, *d_wr, *d_wp, *d_ids, *d_cnt;
-  CK(scratch(tmp, total + 64, &d_seq)); CK(scratch(tmp, (size_t)nreads + 1, &d_off)); CK(scratch(tmp, (size_t)nwin + 1, &d_wr));
-  CK(scratch(tmp, (size_t)nwin + 1, &d_wp)); CK(scratch(tmp, (size_t)nwin * cap + 1, &d_ids)); CK(scratch(tmp, (size_t)nwin + 1, &d_cnt));
-  CK(scratch(tmp, (size_t)nwin + 4, &d_zero));
+  uint8_t* d_seq = scratch<uint8_t>(tmp, total + 64);
+  uint32_t *d_off = scratch<uint32_t>(tmp, (size_t)nreads + 1), *d_wr = scratch<uint32_t>(tmp, (size_t)nwin + 1), *d_wp = scratch<uint32_t>(tmp, (size_t)nwin + 1),
+           *d_ids = scratch<uint32_t>(tmp, (size_t)nwin * cap + 1), *d_cnt = scratch<uint32_t>(tmp, (size_t)nwin + 1);
+  uint8_t* d_zero = scratch<uint8_t>(tmp, (size_t)nwin + 4);
   CK(cudaMemcpy(d_seq, seq_cat + seq_off[0], total, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(d_off, off32.data(), (size_t)(nreads + 1) * 4, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(d_wr, win_read, (size_t)nwin * 4, cudaMemcpyHostToDevice));
@@ -1959,10 +1895,10 @@ int smr_debug_seed_windows(smr_ctx* ctx, uint32_t part_slot, const uint8_t* seq_
   CK(cudaMemcpy(counts, d_cnt, (size_t)nwin * 4, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(zero, d_zero, nwin, cudaMemcpyDeviceToHost));
   return SMR_OK;
-}
+} SMR_CATCH(ctx)
 
 int smr_debug_ssw(smr_ctx* ctx, const uint8_t* q_cat, const uint64_t* q_off, const uint8_t* t_cat, const uint64_t* t_off, uint32_t npairs,
-                  uint32_t filters, int32_t* out, uint32_t* cigars, uint32_t cigar_cap) {
+                  uint32_t filters, int32_t* out, uint32_t* cigars, uint32_t cigar_cap) try {
   if (!ctx || !q_cat || !q_off || !t_cat || !t_off || !out || !cigars || !ctx->have_params) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   const uint64_t qt = q_off[npairs] - q_off[0], tt = t_off[npairs] - t_off[0];
@@ -1971,14 +1907,14 @@ int smr_debug_ssw(smr_ctx* ctx, const uint8_t* q_cat, const uint64_t* q_off, con
   for (uint32_t i = 0; i <= npairs; ++i) { qo[i] = (uint32_t)(q_off[i] - q_off[0]); to[i] = (uint32_t)(t_off[i] - t_off[0]); }
   for (uint32_t i = 0; i < npairs; ++i) maxlen = std::max(maxlen, std::max(qo[i + 1] - qo[i], to[i + 1] - to[i]));
   std::vector<DevBuf> tmp;
-  uint8_t *dq, *dt, *arena; uint32_t *dqo, *dto, *dc; int32_t* dout;
   FinalGlobals g{};
   g.cap_w = 2 * 2048 + 8; g.cap_cig = 2 * (maxlen + 64) + 16; g.row_cap = maxlen + 128; g.cap_dir = (size_t)(2 * 64 + 1) * (maxlen + 8) * 3 + 65536;
   const uint32_t nwarps = 512;
   g.arena_stride = final_arena_bytes(g.cap_w, g.cap_cig, g.row_cap, g.cap_dir);
-  CK(scratch(tmp, g.arena_stride * nwarps, &arena)); g.arena_base = arena;
-  CK(scratch(tmp, qt + 64, &dq)); CK(scratch(tmp, tt + 64, &dt)); CK(scratch(tmp, (size_t)npairs + 1, &dqo)); CK(scratch(tmp, (size_t)npairs + 1, &dto));
-  CK(scratch(tmp, (size_t)npairs * cigar_cap + 1, &dc)); CK(scratch(tmp, (size_t)npairs * 6 + 1, &dout));
+  g.arena_base = scratch<uint8_t>(tmp, g.arena_stride * nwarps);
+  uint8_t *dq = scratch<uint8_t>(tmp, qt + 64), *dt = scratch<uint8_t>(tmp, tt + 64);
+  uint32_t *dqo = scratch<uint32_t>(tmp, (size_t)npairs + 1), *dto = scratch<uint32_t>(tmp, (size_t)npairs + 1), *dc = scratch<uint32_t>(tmp, (size_t)npairs * cigar_cap + 1);
+  int32_t* dout = scratch<int32_t>(tmp, (size_t)npairs * 6 + 1);
   CK(cudaMemcpy(dq, q_cat + q_off[0], qt, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dt, t_cat + t_off[0], tt, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(dqo, qo.data(), (size_t)(npairs + 1) * 4, cudaMemcpyHostToDevice)); CK(cudaMemcpy(dto, to.data(), (size_t)(npairs + 1) * 4, cudaMemcpyHostToDevice));
   CK(cudaMemset(dc, 0, (size_t)npairs * cigar_cap * 4));
@@ -1989,12 +1925,13 @@ int smr_debug_ssw(smr_ctx* ctx, const uint8_t* q_cat, const uint64_t* q_off, con
   CK(cudaMemcpy(out, dout, (size_t)npairs * 6 * 4, cudaMemcpyDeviceToHost));
   CK(cudaMemcpy(cigars, dc, (size_t)npairs * cigar_cap * 4, cudaMemcpyDeviceToHost));
   return SMR_OK;
-}
+} SMR_CATCH(ctx)
 
 int smr_otu_begin(smr_ctx* ctx, const smr_otu_opts* opts) try {
   if (!ctx || !opts) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  return otu_begin_impl(ctx, opts);
+  otu_begin_impl(ctx, opts);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_otu_add(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
@@ -2002,13 +1939,16 @@ int smr_otu_add(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_
   if (!ctx || (!text && nbytes)) return SMR_ERR_ARG;
   if (n_added) *n_added = 0;
   CK(cudaSetDevice(ctx->device));
-  return otu_add_impl(ctx, text, nbytes, results, alns, stats, nreads, n_added);
+  const uint64_t m = otu_add_impl(ctx, text, nbytes, results, alns, stats, nreads);
+  if (n_added) *n_added = m;
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_otu_finish(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) try {
   if (!ctx || !counts) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  return otu_finish_impl(ctx, out, cap, counts);
+  otu_finish_impl(ctx, out, cap, counts);
+  return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_last_otu_timings(const smr_ctx* ctx, double out[3]) {
