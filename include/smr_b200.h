@@ -214,6 +214,41 @@ int smr_resident_text(smr_ctx*, char* text, uint64_t cap, uint64_t* nbytes);
  * candidates found, device time in us, H2D time in us}. */
 int smr_debug_inflate(smr_ctx*, const void* gz, uint64_t nbytes, uint64_t chunk_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_bytes, uint32_t info[4]);
 
+/* -- read stream: a reads file of any size, pushed piece by piece (sortmerna_b200/csrc/smr_stream.cuh) --
+ * The caller pushes the file's bytes (compressed bytes with SMR_STREAM_GZ) in pieces of any size, such as 64-512 MB read from disk;
+ * the library inflates them on the device as they arrive (one round of smr_upload_fastx_gz's inflate per push, resumed at the last
+ * block boundary the pushed bytes reach; the CRC-32 and ISIZE of every member are checked as members complete) and hands back
+ * record-aligned batches: each one is made resident as by smr_upload_fastx, so smr_run_resident, smr_download_results,
+ * smr_resident_text and smr_format_reports[_gz] / smr_otu_add with text == nullptr work on it unchanged.  A batch holds the whole
+ * records that fit in batch_bytes of text (FASTQ: 4 lines each; FASTA: a header line and the lines up to the next one), or one
+ * record alone when that record is longer; the batches of a file, one after another, decode to exactly the reads of the whole file.
+ * The stream's buffers (compressed bytes not yet inflated, text not yet in a batch) belong to the stream; opening a new stream
+ * drops them.  A corrupt, truncated or non-gzip SMR_STREAM_GZ input (bad data, CRC-32 or ISIZE, EOF inside a header, block or
+ * trailer) fails with SMR_ERR_ARG, at the push that shows it, and closes the stream; text that is neither FASTA nor FASTQ fails in
+ * smr_stream_next with the refusals of smr_upload_fastx.
+ *
+ * Separately, every pushed byte of text is counted as the reference's Readfeed::count_reads_parallel counts a reads file
+ * (src/sortmerna/readfeed.cpp:1486-1663; rule in sortmerna_b200/csrc/smr_stream.h): a fixed cycle of 4 lines (first byte '@') or 2
+ * lines per record, every byte of a cycle-position-1 line before its '\n' counted ('\r' included), a last sequence line without
+ * '\n' not counted, multi-line FASTA taken as 2-line records.  For a flat multi-line FASTA the reference's figures depend on its
+ * -threads (each split restarts the cycle at a '>' line); these are the single-split figures, which -threads 1 and gzip input give.
+ * They are what Refstats::minimal_score and the E-value read length are computed from.  SMR_STREAM_COUNT_ONLY counts and keeps no
+ * text: the cheap first pass over a file. */
+enum { SMR_STREAM_GZ = 1, SMR_STREAM_COUNT_ONLY = 2, SMR_STREAM_NEXT_FILE = 4 };
+/* open (or reset) the context's read stream; batch_bytes = text bytes per batch, in [1, 0xF0000000) (ignored with COUNT_ONLY).  Every
+ * batch but the file's last holds the whole records that fit in batch_bytes; before the end of the file, pending text that fits in
+ * one batch waits for the next push.  SMR_STREAM_NEXT_FILE: the counts go on from the previous stream's, as the reference counts
+ * the -reads files of one run (mates): totals add up, the line cycle of the first file holds, a gzip file updates the minimum read
+ * by read and a flat file's own minimum is merged at its end (readfeed.cpp:1497-1662). */
+int smr_stream_begin(smr_ctx*, uint32_t flags, uint64_t batch_bytes);
+/* the next n bytes of the file; eof = 1 with the last piece (n may be 0) */
+int smr_stream_push(smr_ctx*, const void* bytes, uint64_t n, int eof);
+/* make the next batch resident: *nreads > 0 = a batch is resident (as after smr_upload_fastx); *nreads == 0 and *done == 0 = push
+ * more; *done == 1 = the file is exhausted */
+int smr_stream_next(smr_ctx*, uint32_t* nreads, int* done);
+/* count_reads_parallel over everything pushed so far: {num_reads_tot, length_all, min_read_len, max_read_len} */
+int smr_stream_counts(smr_ctx*, uint64_t out[4]);
+
 /* Where the resident reads are: header_text_off[r] = offset of record r's header line in the text given to
  * smr_upload_fastx (for Read::getSeqId / report writers; nullptr = skip; only after smr_upload_fastx), read_off[0..nreads] =
  * offsets into the concatenated 0-4 codes, seq04 (optional) = those codes (seq_cap bytes available). */

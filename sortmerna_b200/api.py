@@ -29,7 +29,7 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_set_aln_slots", "smr_aln_slots", "smr_aln_slots_needed", "smr_upload_fastx_gz", "smr_resident_text", "smr_debug_inflate",
            "smr_build_index_device", "smr_debug_index_array", "smr_set_instrumentation", "smr_set_report_refs", "smr_set_report_scoring",
            "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings",
-           "smr_format_reports_gz", "smr_gzip"]
+           "smr_format_reports_gz", "smr_gzip", "smr_stream_begin", "smr_stream_push", "smr_stream_next", "smr_stream_counts"]
 
 CNT_NAMES = ("num_aligned", "num_short", "sw_calls", "sw_cells", "windows", "trie_nodes", "buckets",
              "bucket_entries", "pos_entries", "lis_calls", "dbg_max_read_cycles", "dbg_sum_read_cycles", "dbg_lis_kernel_cycles",
@@ -116,6 +116,10 @@ def load_library():
         L.smr_aln_slots_needed.argtypes = [C.c_void_p]
         L.smr_set_aln_slots.argtypes = [C.c_void_p, C.c_uint32]
         L.smr_set_instrumentation.argtypes = [C.c_void_p, C.c_int]
+        L.smr_stream_begin.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64]
+        L.smr_stream_push.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int]
+        L.smr_stream_next.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
+        L.smr_stream_counts.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
         for name in SYMBOLS:
             getattr(L, name)  # AttributeError if the build is stale
         _lib = L
@@ -366,6 +370,68 @@ class Aligner:
             self._check(self.L.smr_debug_inflate(self.h, _ptr(buf), C.c_uint64(buf.size), C.c_uint64(chunk_bytes), _ptr(out), C.c_uint64(out.size), C.byref(nb2), info),
                         "smr_debug_inflate")
         return out.tobytes(), {"spans": info[0], "candidates": info[1], "device_us": info[2], "h2d_us": info[3]}
+
+    # -- read stream (smr_stream_*): files of any size, pushed from disk piece by piece --
+    STREAM_GZ, STREAM_COUNT_ONLY, STREAM_NEXT_FILE = 1, 2, 4
+
+    def _push_file(self, path: str, piece_bytes: int):
+        """Pushes the file at `path` into the open stream, piece by piece; yields after every push."""
+        with open(path, "rb") as f:
+            piece = f.read(piece_bytes)
+            while True:
+                nxt = f.read(piece_bytes) if piece else b""
+                buf = np.frombuffer(piece, dtype=np.uint8)
+                self._check(self.L.smr_stream_push(self.h, _ptr(buf) if buf.size else C.c_void_p(0), C.c_uint64(buf.size), C.c_int(0 if nxt else 1)),
+                            "smr_stream_push")
+                yield
+                if not nxt:
+                    return
+                piece = nxt
+
+    @staticmethod
+    def _is_gz(path: str) -> bool:
+        with open(path, "rb") as f:
+            return f.read(2) == b"\x1f\x8b"
+
+    def read_counts(self, path_or_paths, piece_bytes: int = 256 << 20) -> dict:
+        """The reference's first pass over the reads files (Readfeed::count_reads_parallel, readfeed.cpp:1486-1663) on the device:
+        {"reads", "length", "min_len", "max_len"} = num_reads_tot, length_all, min_read_len, max_read_len -- the figures
+        hostio.minimal_score and hostio.evalue_params take.  gzip files are recognised by their magic bytes; several files (mates)
+        are counted one after another as the reference counts the -reads files of one run (SMR_STREAM_NEXT_FILE)."""
+        paths = [path_or_paths] if isinstance(path_or_paths, (str, os.PathLike)) else list(path_or_paths)
+        for k, p in enumerate(paths):
+            flags = self.STREAM_COUNT_ONLY | (self.STREAM_GZ if self._is_gz(p) else 0) | (self.STREAM_NEXT_FILE if k else 0)
+            self._check(self.L.smr_stream_begin(self.h, C.c_uint32(flags), C.c_uint64(0)), "smr_stream_begin")
+            for _ in self._push_file(p, piece_bytes):
+                pass
+        return self.stream_counts()
+
+    def stream_fastx(self, path: str, batch_bytes: int = 256 << 20, piece_bytes: int = 256 << 20):
+        """Streams a FASTA / FASTQ file (plain or gzip, by its magic bytes) through the device in record-aligned batches of at
+        most batch_bytes of text (one longer record makes a batch alone).  Yields the read count of each batch once it is
+        resident: run run_resident() / download() / ReportWriter.write(out) inside the loop.  The file is read piece_bytes at a
+        time and is never held whole in host memory."""
+        flags = self.STREAM_GZ if self._is_gz(path) else 0
+        self._check(self.L.smr_stream_begin(self.h, C.c_uint32(flags), C.c_uint64(batch_bytes)), "smr_stream_begin")
+        n, done = C.c_uint32(0), C.c_int(0)
+
+        def drain():
+            while True:
+                self._check(self.L.smr_stream_next(self.h, C.byref(n), C.byref(done)), "smr_stream_next")
+                if n.value == 0:
+                    return
+                self._n_resident = int(n.value)
+                yield int(n.value)
+
+        for _ in self._push_file(path, piece_bytes):
+            yield from drain()
+        yield from drain()
+
+    def stream_counts(self) -> dict:
+        """smr_stream_counts of the open stream: the count_reads_parallel figures of what was pushed so far."""
+        out = (C.c_uint64 * 4)()
+        self._check(self.L.smr_stream_counts(self.h, out), "smr_stream_counts")
+        return dict(zip(("reads", "length", "min_len", "max_len"), (int(v) for v in out)))
 
     def resident_layout(self, with_headers: bool = True, with_seq: bool = True):
         """smr_resident_layout: (header offsets in the uploaded text, read offsets, concatenated 0-4 codes) of the resident batch."""

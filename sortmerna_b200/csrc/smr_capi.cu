@@ -16,6 +16,7 @@
 #include "smr_report.cuh"
 #include "smr_otu.cuh"
 #include "smr_inflate.cuh"
+#include "smr_stream.cuh"
 #include "smr_deflate.cuh"
 #include "smr_build.h"
 #include "smr_build_dev.cuh"
@@ -76,6 +77,24 @@ struct Batch {
   RunTimes run;
 };
 
+// What a read stream's inflate carries from one round to the next (smr_inflate.h): where to resume, the open member's CRC-32 and
+// length, the members seen so far; the last 32 KB of output are in smr_ctx::d_infwin.
+struct InfStream { InfResume at; InfCarry carry; uint32_t members = 0; bool have_window = false; };
+
+// The read stream of a context (smr_stream_begin .. smr_stream_next): the compressed bytes not inflated yet (gz) and the text not
+// made into a batch yet belong to it.
+struct ReadStream {
+  bool open = false, gz = false, count_only = false, eof = false;
+  uint64_t batch_bytes = 0;
+  std::vector<uint8_t> tail;   // gz: the pushed bytes from the byte of the resume point on (inf.at.bit counts from tail[0])
+  InfStream inf;
+  DevBuf text;                 // pending text: [off, n) is not in a batch yet
+  uint64_t off = 0, n = 0, pushed = 0;
+  char first = 0;              // the file's first byte: '@' = FASTQ
+  bool have_first = false;
+  CountState counts;
+};
+
 }  // namespace
 
 struct smr_ctx {
@@ -103,6 +122,8 @@ struct smr_ctx {
   DevBuf cub_tmp;   // cub scratch of the text layout, the report writer and the OTU map
   DevBuf seed_ctr, d_gz, d_cand, d_res, d_sym, d_win, d_ids, d_off, d_cnt64, d_moff, d_mem, d_poff, d_plen, d_pcrc;   // gz inflate (smr_inflate.cuh)
   uint64_t text_bytes = 0;          // size of the text behind the resident batch (smr_upload_fastx / _gz)
+  DevBuf d_infwin, d_infwin2, d_rc, d_cut;   // read stream: carried inflate window, count-pass partials, batch cut
+  ReadStream rs;
   uint32_t inf_spans = 0, inf_candidates = 0; double t_inflate = 0;
   double t_decode = 0;
   uint32_t tb_threads = 0, tb_cap_w = 0, tb_cap_cig = 0; size_t tb_cap_dir = 0, tb_stride = 0;
@@ -494,6 +515,24 @@ void exclusive_sum(smr_ctx* ctx, const uint32_t* in, uint32_t* out, uint32_t n) 
   cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, n, ctx->stream); });
 }
 
+// Newline positions of a text (smr_decode.cuh (1)-(3)) in d_nl: count per 32-byte chunk, scan (the total lands at [nchunks]),
+// positions.  A text that does not end in '\n' gets a virtual one at nbytes.  Returns their number.
+uint32_t newline_index(smr_ctx* ctx, const uint8_t* text, uint64_t nbytes) {
+  const int grid = ctx->sm_count * 8;
+  const uint64_t nchunks = nbytes / 32 + 1;
+  uint32_t* cnt = ensure<uint32_t>(ctx->d_cnt, (nchunks + 1) * 4);
+  count_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks);
+  CK(cudaMemsetAsync(cnt + nchunks, 0, 4, ctx->stream));
+  exclusive_sum(ctx, cnt, cnt, (uint32_t)nchunks + 1);
+  uint32_t n = 0;
+  CK(cudaMemcpyAsync(&n, cnt + nchunks, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  ensure(ctx->d_nl, ((size_t)n + 1) * 8);
+  if (n) write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks, (uint64_t*)ctx->d_nl.p);
+  CK(cudaGetLastError());
+  return n;
+}
+
 struct TextLayout { uint32_t nlines = 0, nrec = 0, total_nt = 0; uint32_t fmt = kFmtFasta; };
 
 // The line layout of a FASTA / FASTQ text on the device (the line passes of smr_decode.cuh), for the decode and the report writer.
@@ -507,24 +546,15 @@ TextLayout text_layout(smr_ctx* ctx, const uint8_t* text, uint64_t nbytes, char 
   L.fmt = first_byte == '@' ? kFmtFastq : kFmtFasta;
   uint32_t* scal = ensure<uint32_t>(ctx->d_scal, 64);   // [1] records [2] sequence bytes [3] decode error
   CK(cudaMemsetAsync(scal, 0, 64, ctx->stream));
-  // newlines: count per 32-byte chunk, scan (the total lands at [nchunks]), positions
   const int grid = ctx->sm_count * 8;
-  const uint64_t nchunks = nbytes / 32 + 1;
-  uint32_t* cnt = ensure<uint32_t>(ctx->d_cnt, (nchunks + 1) * 4);
-  count_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks);
-  CK(cudaMemsetAsync(cnt + nchunks, 0, 4, ctx->stream));
-  exclusive_sum(ctx, cnt, cnt, (uint32_t)nchunks + 1);
-  CK(cudaMemcpyAsync(&L.nlines, cnt + nchunks, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
+  L.nlines = newline_index(ctx, text, nbytes);
   const uint32_t n = L.nlines;
-  ensure(ctx->d_nl, ((size_t)n + 1) * 8);
   ensure(ctx->d_hdr, ((size_t)n + 1) * 4);
   ensure(ctx->d_sb, ((size_t)n + 1) * 4);
   ensure(ctx->d_rec, ((size_t)n + 1) * 4);
   ensure(ctx->d_spos, ((size_t)n + 1) * 4);
   if (n == 0) return L;
   uint32_t *hdr = (uint32_t*)ctx->d_hdr.p, *sb = (uint32_t*)ctx->d_sb.p, *rec = (uint32_t*)ctx->d_rec.p, *spos = (uint32_t*)ctx->d_spos.p;
-  write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks, (uint64_t*)ctx->d_nl.p);
   // per line: header flag and sequence bytes; their scans give the record of every line and the offset of its bytes
   line_info_kernel<<<grid, 256, 0, ctx->stream>>>(text, (const uint64_t*)ctx->d_nl.p, n, L.fmt, hdr, sb, scal + 3);
   CK(cudaMemsetAsync(hdr + n, 0, 4, ctx->stream));
@@ -606,11 +636,22 @@ const char* inf_status_text(uint32_t st) {
   }
 }
 
-// gzip file (host bytes) -> inflated bytes in ctx->d_text; returns their number.  The five steps of smr_inflate.h; the host only
-// walks the list of spans (a few thousand entries) between the COUNT and the WRITE pass.
-uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes) {
+// grow-only, keeping the first `keep` bytes
+void ensure_keep(smr_ctx* ctx, DevBuf& b, size_t bytes, size_t keep) {
+  if (bytes <= b.cap && b.p) return;
+  DevBuf n;
+  CK(n.alloc(bytes + bytes / 8 + 256));
+  if (keep) CK(cudaMemcpyAsync(n.p, b.p, keep, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  b = std::move(n);
+}
+
+// One round of the inflate (the five steps of smr_inflate.h) over the compressed bytes gz[0 .. nbytes) (host), from st.at on: the
+// output goes to out + at (grown as needed, its first `at` bytes kept).  eof: these bytes end the file; otherwise the round keeps
+// what it inflated up to the last block boundary it could reach and st says where the next round resumes.  Returns the bytes
+// kept.  The host only walks the list of spans (a few thousand entries) between the COUNT and the WRITE pass.
+uint64_t inflate_round(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes, bool eof, InfStream& st, DevBuf& out, uint64_t at) {
   ctx->inf_spans = ctx->inf_candidates = 0;
-  if (nbytes < 18) fail(SMR_ERR_ARG, "gz input: shorter than a gzip header and trailer");
   if (chunk_bytes < 1024) chunk_bytes = 1024;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
   CK(cudaEventRecord(e0, ctx->stream));
@@ -631,7 +672,7 @@ uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t ch
     std::vector<uint64_t> raw(nchunks - 1);
     CK(cudaMemcpyAsync(raw.data(), ctx->d_cand.p, (nchunks - 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    for (uint64_t p : raw) if (p != kInfNone) cand.push_back(p);   // chunk order = position order
+    for (uint64_t p : raw) if (p != kInfNone && p > st.at.bit) cand.push_back(p);   // chunk order = position order
     if (!cand.empty()) CK(cudaMemcpyAsync(ctx->d_cand.p, cand.data(), cand.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
   } else ensure(ctx->d_cand, 8);
   const uint32_t ncand = (uint32_t)cand.size(), ns = ncand + 1;
@@ -640,27 +681,38 @@ uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t ch
   CK(cudaFuncSetAttribute(inf_span_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kInfSpanSmem));
   ensure(ctx->d_res, (size_t)ns * sizeof(SpanResult));
   const unsigned ctas = (ns + kInfSpanThreads - 1) / kInfSpanThreads;
-  inf_span_kernel<false><<<ctas, kInfSpanThreads, kInfSpanSmem, ctx->stream>>>(w, nbytes, (const uint64_t*)ctx->d_cand.p, ncand, nullptr, nullptr, nullptr, nullptr, nullptr, ns,
-                                                                               nullptr, (SpanResult*)ctx->d_res.p);
+  const uint64_t start = st.at.bit, prior = st.carry.len;
+  const bool at_member = st.at.at_member;
+  inf_span_kernel<false><<<ctas, kInfSpanThreads, kInfSpanSmem, ctx->stream>>>(w, nbytes, start, at_member, prior, (const uint64_t*)ctx->d_cand.p, ncand, nullptr, nullptr,
+                                                                               nullptr, nullptr, nullptr, ns, nullptr, (SpanResult*)ctx->d_res.p);
   CK(cudaGetLastError());
   std::vector<SpanResult> res(ns);
   CK(cudaMemcpyAsync(res.data(), ctx->d_res.p, (size_t)ns * sizeof(SpanResult), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  std::vector<uint32_t> real(ns); std::vector<uint64_t> off(ns), cnt(ns);
+  std::vector<uint32_t> real(ns); std::vector<uint64_t> off(ns), cnt(ns), keep(ns);
   uint32_t nreal = 0, why = 0;
-  const uint64_t total = inf_chain(cand.data(), ncand, res.data(), real.data(), off.data(), nreal, &why);
-  if (total == kInfNone) fail(SMR_ERR_ARG, std::string("gz input: ") + inf_status_text(why));
+  InfResume next;
+  const uint64_t total = inf_chain(cand.data(), ncand, res.data(), real.data(), off.data(), nreal, &why, eof, nbytes * 8, at_member, &next);
+  if (total == kInfNone) {
+    // bytes after the last member that are no member are ignored, as gzip does (a round that resumed at a member's end sees them alone)
+    if (at_member && st.members && res[0].status == kInfErrMember) { st.at.eos = true; return 0; }
+    fail(SMR_ERR_ARG, std::string("gz input: ") + inf_status_text(why));
+  }
   std::vector<uint32_t> moff(nreal + 1, 0);
-  for (uint32_t k = 0; k < nreal; ++k) { cnt[k] = res[real[k]].out_n; moff[k + 1] = moff[k] + res[real[k]].members; }
+  for (uint32_t k = 0; k < nreal; ++k) { cnt[k] = res[real[k]].out_n; keep[k] = cnt[k]; moff[k + 1] = moff[k] + res[real[k]].members; }
+  keep[nreal - 1] = next.keep_last;
   const uint32_t nmembers = moff[nreal];
   ctx->inf_spans = nreal; ctx->inf_candidates = ncand;
-  ensure(ctx->d_text, total + 64);
-  if (total) {
+  ensure_keep(ctx, out, at + total + 64, at);
+  uint8_t* dst = (uint8_t*)out.p + at;
+  if (total || (nmembers && st.carry.len)) {
     // WRITE
     ensure(ctx->d_ids, (size_t)nreal * 4);
     ensure(ctx->d_off, (size_t)nreal * 8);
     ensure(ctx->d_cnt64, (size_t)nreal * 8);
-    ensure(ctx->d_sym, (total + 8) * 2);
+    uint64_t nsym = 0;
+    for (uint32_t k = 0; k < nreal; ++k) nsym = std::max(nsym, off[k] + cnt[k]);
+    ensure(ctx->d_sym, (nsym + 8) * 2);
     ensure(ctx->d_win, (size_t)(nreal + 1) * kInfWindow);
     CK(cudaMemcpyAsync(ctx->d_ids.p, real.data(), (size_t)nreal * 4, cudaMemcpyHostToDevice, ctx->stream));
     CK(cudaMemcpyAsync(ctx->d_off.p, off.data(), (size_t)nreal * 8, cudaMemcpyHostToDevice, ctx->stream));
@@ -669,16 +721,19 @@ uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t ch
     ensure(ctx->d_mem, (size_t)(nmembers + 1) * sizeof(MemberEnd));
     CK(cudaMemcpyAsync(ctx->d_moff.p, moff.data(), (size_t)(nreal + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
     inf_span_kernel<true><<<(nreal + kInfSpanThreads - 1) / kInfSpanThreads, kInfSpanThreads, kInfSpanSmem, ctx->stream>>>(
-        w, nbytes, (const uint64_t*)ctx->d_cand.p, ncand, (const uint32_t*)ctx->d_ids.p, (const uint64_t*)ctx->d_off.p, (const uint64_t*)ctx->d_cnt64.p,
-        (const uint32_t*)ctx->d_moff.p, (MemberEnd*)ctx->d_mem.p, nreal, (uint16_t*)ctx->d_sym.p, (SpanResult*)ctx->d_res.p);
+        w, nbytes, start, at_member, prior, (const uint64_t*)ctx->d_cand.p, ncand, (const uint32_t*)ctx->d_ids.p, (const uint64_t*)ctx->d_off.p,
+        (const uint64_t*)ctx->d_cnt64.p, (const uint32_t*)ctx->d_moff.p, (MemberEnd*)ctx->d_mem.p, nreal, (uint16_t*)ctx->d_sym.p, (SpanResult*)ctx->d_res.p);
     CK(cudaGetLastError());
-    // WINDOW, RESOLVE
+    // WINDOW (seeded with the last 32 KB of the previous round), RESOLVE of the bytes kept
+    if (st.have_window) CK(cudaMemcpyAsync(ctx->d_win.p, ctx->d_infwin.p, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
+    else CK(cudaMemsetAsync(ctx->d_win.p, 0, kInfWindow, ctx->stream));
     inf_window_kernel<<<1, 1024, 0, ctx->stream>>>((const uint16_t*)ctx->d_sym.p, (const uint64_t*)ctx->d_off.p, (const uint64_t*)ctx->d_cnt64.p, nreal, (uint8_t*)ctx->d_win.p);
     CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(ctx->d_cnt64.p, keep.data(), (size_t)nreal * 8, cudaMemcpyHostToDevice, ctx->stream));
     const uint64_t avg = total / nreal + 1;
     const unsigned pieces = (unsigned)std::min<uint64_t>(64, std::max<uint64_t>(1, avg / 8192));
     inf_resolve_kernel<<<dim3(pieces, nreal), 256, 0, ctx->stream>>>((const uint16_t*)ctx->d_sym.p, (const uint64_t*)ctx->d_off.p, (const uint64_t*)ctx->d_cnt64.p,
-                                                                     (const uint8_t*)ctx->d_win.p, (uint8_t*)ctx->d_text.p);
+                                                                     (const uint8_t*)ctx->d_win.p, dst);
     CK(cudaGetLastError());
     std::vector<SpanResult> res2(nreal);
     std::vector<MemberEnd> ends(nmembers);
@@ -690,9 +745,9 @@ uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t ch
         fail(SMR_ERR_CUDA, "gz inflate: the write pass disagrees with the count pass");
       for (uint32_t m = moff[k]; m < moff[k + 1]; ++m) ends[m].out_end += off[k];
     }
-    // CRC-32 + ISIZE of every member (RFC 1952 2.3.1): pieces on the device, joined here
+    // CRC-32 + ISIZE of every member (RFC 1952 2.3.1): pieces on the device, joined here; the open member's part is carried
     std::vector<uint64_t> poff; std::vector<uint32_t> plen, first;
-    inf_crc_plan(ends, 32768, poff, plen, first);
+    inf_crc_plan(ends, 32768, poff, plen, first, total);
     const uint32_t npieces = (uint32_t)poff.size();
     std::vector<uint32_t> crcs(npieces);
     if (npieces) {
@@ -701,21 +756,170 @@ uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t ch
       ensure(ctx->d_pcrc, (size_t)npieces * 4);
       CK(cudaMemcpyAsync(ctx->d_poff.p, poff.data(), (size_t)npieces * 8, cudaMemcpyHostToDevice, ctx->stream));
       CK(cudaMemcpyAsync(ctx->d_plen.p, plen.data(), (size_t)npieces * 4, cudaMemcpyHostToDevice, ctx->stream));
-      inf_crc_kernel<<<(npieces + 127) / 128, 128, 0, ctx->stream>>>((const uint8_t*)ctx->d_text.p, (const uint64_t*)ctx->d_poff.p, (const uint32_t*)ctx->d_plen.p, npieces,
+      inf_crc_kernel<<<(npieces + 127) / 128, 128, 0, ctx->stream>>>(dst, (const uint64_t*)ctx->d_poff.p, (const uint32_t*)ctx->d_plen.p, npieces,
                                                                        (uint32_t*)ctx->d_pcrc.p);
       CK(cudaGetLastError());
       CK(cudaMemcpyAsync(crcs.data(), ctx->d_pcrc.p, (size_t)npieces * 4, cudaMemcpyDeviceToHost, ctx->stream));
     }
+    // the window the next round starts from: the last 32 KB of (previous window, this round's output)
+    if (!next.eos) {
+      ensure(ctx->d_infwin, kInfWindow);
+      ensure(ctx->d_infwin2, kInfWindow);
+      if (total >= kInfWindow) CK(cudaMemcpyAsync(ctx->d_infwin.p, dst + total - kInfWindow, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
+      else if (total) {
+        CK(cudaMemcpyAsync(ctx->d_infwin2.p, (uint8_t*)ctx->d_win.p + total, kInfWindow - total, cudaMemcpyDeviceToDevice, ctx->stream));
+        CK(cudaMemcpyAsync((uint8_t*)ctx->d_infwin2.p + kInfWindow - total, dst, total, cudaMemcpyDeviceToDevice, ctx->stream));
+        std::swap(ctx->d_infwin, ctx->d_infwin2);
+      }
+      if (total) st.have_window = true;
+    }
     CK(cudaEventRecord(e2, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    if (const uint32_t bad = inf_crc_verify(ends, plen, first, crcs.data())) fail(SMR_ERR_ARG, std::string("gz input: ") + inf_status_text(bad));
+    if (const uint32_t bad = inf_crc_verify(ends, plen, first, crcs.data(), &st.carry)) fail(SMR_ERR_ARG, std::string("gz input: ") + inf_status_text(bad));
   } else {
     CK(cudaEventRecord(e2, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
+  st.members += nmembers;
+  st.at = next;
   float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_h2d = ms;
   cudaEventElapsedTime(&ms, e1, e2); ctx->t_inflate = ms;
   return total;
+}
+
+// gzip file (host bytes) -> inflated bytes in ctx->d_text; returns their number.  The whole file is one round.
+uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes) {
+  ctx->inf_spans = ctx->inf_candidates = 0;
+  if (nbytes < 18) fail(SMR_ERR_ARG, "gz input: shorter than a gzip header and trailer");
+  InfStream st;
+  return inflate_round(ctx, gz, nbytes, chunk_bytes, true, st, ctx->d_text, 0);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// read stream (smr_stream_*): a file pushed piece by piece, counted as the reference counts it and cut into record-aligned batches
+// ---------------------------------------------------------------------------------------------------------------------
+
+// the count pass (smr_stream.h) over n bytes of new text at t (device)
+void count_text(smr_ctx* ctx, const uint8_t* t, uint64_t n, CountState& s) {
+  if (n == 0) return;
+  const uint32_t nlines = newline_index(ctx, t, n);
+  const uint32_t parts = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->sm_count * 8, (nlines + 255) / 256));
+  const uint32_t per = (uint32_t)(((uint64_t)nlines + parts - 1) / parts + 255) / 256 * 256;
+  uint8_t* rc = ensure<uint8_t>(ctx->d_rc, (size_t)(parts + 1) * sizeof(ReadCounts) + 16);
+  ReadCounts* part = (ReadCounts*)rc;
+  uint64_t* info = (uint64_t*)(rc + (size_t)(parts + 1) * sizeof(ReadCounts));
+  count_lines_kernel<<<parts, 256, 0, ctx->stream>>>((const uint64_t*)ctx->d_nl.p, nlines, n, s, per, part);
+  CK(cudaGetLastError());
+  count_fold_kernel<<<1, 1, 0, ctx->stream>>>(part, parts, (const uint64_t*)ctx->d_nl.p, nlines, n, part + parts, info);
+  CK(cudaGetLastError());
+  struct { ReadCounts r; uint64_t nl[2]; } h;
+  CK(cudaMemcpyAsync(&h.r, part + parts, sizeof(ReadCounts), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h.nl, info, 16, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  rc_fold(s, h.r);
+  rc_advance(s, n, h.nl[0], h.nl[1]);
+}
+
+// the pending text from [off, n) on, with room for `extra` more bytes after n
+void compact_pending(smr_ctx* ctx, ReadStream& rs, uint64_t extra) {
+  const uint64_t live = rs.n - rs.off;
+  if (rs.off == 0 && rs.text.p && rs.text.cap >= rs.n + extra + 64) return;
+  DevBuf nb;
+  const uint64_t want = live + extra + 64;
+  CK(nb.alloc(want + want / 8 + 256));
+  if (live) CK(cudaMemcpyAsync(nb.p, (uint8_t*)rs.text.p + rs.off, live, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  rs.text = std::move(nb);
+  rs.off = 0; rs.n = live;
+}
+
+// new text at [from, rs.n): the file's first byte, the count pass; a count-only stream keeps none of it
+void took_text(smr_ctx* ctx, ReadStream& rs, uint64_t from) {
+  const uint8_t* t = (const uint8_t*)rs.text.p;
+  if (rs.n > from && !rs.have_first) {
+    CK(cudaMemcpyAsync(&rs.first, t + from, 1, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    rs.have_first = true;
+    if (!rs.counts.period) rs.counts.period = rs.first == '@' ? 4 : 2;   // the line cycle of a run's first file holds for all
+  }
+  count_text(ctx, t + from, rs.n - from, rs.counts);
+  if (rs.count_only) rs.off = rs.n = 0;
+}
+
+void stream_push_impl(smr_ctx* ctx, const uint8_t* bytes, uint64_t n, bool eof) {
+  ReadStream& rs = ctx->rs;
+  if (!rs.open) fail(SMR_ERR_ARG, "no open read stream: call smr_stream_begin");
+  if (rs.eof) fail(SMR_ERR_ARG, "read stream: the file has ended (eof was pushed)");
+  rs.eof = eof;
+  if (!rs.gz) {
+    compact_pending(ctx, rs, n);
+    if (n) CK(cudaMemcpyAsync((uint8_t*)rs.text.p + rs.n, bytes, n, cudaMemcpyHostToDevice, ctx->stream));
+    const uint64_t from = rs.n;
+    rs.n += n;
+    took_text(ctx, rs, from);
+    return;
+  }
+  rs.tail.insert(rs.tail.end(), bytes, bytes + n);
+  if (rs.inf.at.eos) { rs.tail.clear(); return; }   // bytes after the gzip stream are ignored
+  rs.pushed += n;
+  if (eof && rs.pushed < 18) fail(SMR_ERR_ARG, "gz input: shorter than a gzip header and trailer");
+  if (rs.tail.empty() && !eof) return;
+  compact_pending(ctx, rs, 0);
+  const uint64_t nb = rs.tail.size();
+  const uint64_t chunk = std::min<uint64_t>(65536, std::max<uint64_t>(8192, nb / 8192));   // as smr_upload_fastx_gz
+  const uint64_t from = rs.n;
+  rs.n += inflate_round(ctx, rs.tail.data(), nb, chunk, eof, rs.inf, rs.text, rs.n);
+  if (rs.inf.at.eos) rs.tail.clear();
+  else {
+    const uint64_t drop = rs.inf.at.bit / 8;
+    rs.tail.erase(rs.tail.begin(), rs.tail.begin() + drop);
+    rs.inf.at.bit -= drop * 8;
+  }
+  took_text(ctx, rs, from);
+}
+
+// where the next batch ends in the pending text (bytes from rs.off), or 0 when more text must be pushed first
+uint64_t stream_cut(smr_ctx* ctx, ReadStream& rs) {
+  const uint64_t avail = rs.n - rs.off, limit = rs.batch_bytes;
+  if (avail == 0) return 0;
+  if (avail <= limit) return rs.eof ? avail : 0;   // a batch takes whole records up to batch_bytes: wait for more text
+  const uint8_t* t = (const uint8_t*)rs.text.p + rs.off;
+  unsigned long long* cut = ensure<unsigned long long>(ctx->d_cut, 16);
+  uint64_t w = std::min(avail, limit + 1);   // a record end at <= limit is a '\n' before it or a header line starting at it
+  for (;;) {
+    const uint32_t nl = newline_index(ctx, t, w);
+    const unsigned long long init[2] = {0ull, ~0ull};
+    CK(cudaMemcpyAsync(cut, init, 16, cudaMemcpyHostToDevice, ctx->stream));
+    stream_cut_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(t, (const uint64_t*)ctx->d_nl.p, nl, w, limit, rs.first == '@' ? kFmtFastq : kFmtFasta, cut);
+    CK(cudaGetLastError());
+    unsigned long long h[2];
+    CK(cudaMemcpyAsync(h, cut, 16, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (h[0]) return h[0];
+    if (h[1] != ~0ull) return h[1];   // the first record is longer than a batch: it is the batch
+    if (w == avail) return rs.eof ? avail : 0;
+    w = std::min(avail, 2 * w);
+  }
+}
+
+uint32_t stream_next_impl(smr_ctx* ctx, int* done) {
+  ReadStream& rs = ctx->rs;
+  if (!rs.open) fail(SMR_ERR_ARG, "no open read stream: call smr_stream_begin");
+  if (rs.count_only) fail(SMR_ERR_ARG, "read stream opened with SMR_STREAM_COUNT_ONLY: it makes no batches");
+  for (;;) {
+    *done = rs.eof && rs.n == rs.off;
+    const uint64_t cut = stream_cut(ctx, rs);
+    if (cut == 0) return 0;
+    if (cut >= 0xF0000000ull) fail(SMR_ERR_ARG, "read stream: one record of 2^32 bytes or more");
+    ensure(ctx->d_text, cut + 64);
+    CK(cudaMemcpyAsync(ctx->d_text.p, (const uint8_t*)rs.text.p + rs.off, cut, cudaMemcpyDeviceToDevice, ctx->stream));
+    char c0 = 0;
+    CK(cudaMemcpyAsync(&c0, (const uint8_t*)rs.text.p + rs.off, 1, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    rs.off += cut;
+    const uint32_t nreads = upload_fastx_impl(ctx, nullptr, cut, c0);
+    if (nreads) { *done = 0; return nreads; }
+  }
 }
 
 // Several contexts may share a device (two per GPU let the copies and the host-side result packing of one batch run under the
@@ -1702,6 +1906,52 @@ int smr_debug_inflate(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t ch
   }
   return SMR_OK;
 } SMR_CATCH(ctx)
+
+int smr_stream_begin(smr_ctx* ctx, uint32_t flags, uint64_t batch_bytes) try {
+  if (!ctx) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  const CountState before = ctx->rs.counts;
+  ctx->rs = ReadStream{};
+  if (flags & ~(uint32_t)(SMR_STREAM_GZ | SMR_STREAM_COUNT_ONLY | SMR_STREAM_NEXT_FILE)) fail(SMR_ERR_ARG, "smr_stream_begin: unknown flags");
+  if (flags & SMR_STREAM_NEXT_FILE) ctx->rs.counts = rc_next_file(before, flags & SMR_STREAM_GZ);
+  if (!(flags & SMR_STREAM_COUNT_ONLY) && (batch_bytes == 0 || batch_bytes >= 0xF0000000ull)) fail(SMR_ERR_ARG, "smr_stream_begin: batch_bytes must be in [1, 0xF0000000)");
+  ReadStream& rs = ctx->rs;
+  rs.gz = flags & SMR_STREAM_GZ; rs.count_only = flags & SMR_STREAM_COUNT_ONLY; rs.batch_bytes = batch_bytes;
+  rs.open = true;
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_stream_push(smr_ctx* ctx, const void* bytes, uint64_t n, int eof) try {
+  if (!ctx || (!bytes && n)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  try {
+    stream_push_impl(ctx, (const uint8_t*)bytes, n, eof != 0);
+  } catch (...) {
+    ctx->rs = ReadStream{};   // a stream that failed is closed
+    throw;
+  }
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_stream_next(smr_ctx* ctx, uint32_t* nreads, int* done) try {
+  if (!ctx || !nreads || !done) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  *nreads = 0; *done = 0;
+  try {
+    *nreads = stream_next_impl(ctx, done);
+  } catch (...) {
+    ctx->rs = ReadStream{};
+    throw;
+  }
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_stream_counts(smr_ctx* ctx, uint64_t out[4]) {
+  if (!ctx || !out) return SMR_ERR_ARG;
+  const CountState& c = ctx->rs.counts;
+  out[0] = c.reads; out[1] = c.length; out[2] = rc_min(c); out[3] = c.max_len;
+  return SMR_OK;
+}
 
 int smr_resident_layout(smr_ctx* ctx, uint64_t* header_text_off, uint64_t* read_off, uint8_t* seq04, uint64_t seq_cap) try {
   if (!ctx) return SMR_ERR_ARG;

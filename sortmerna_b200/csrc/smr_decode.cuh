@@ -16,11 +16,13 @@
 namespace smr {
 
 // ---- (1) newlines per 32-byte chunk; a text that does not end in '\n' gets a virtual one at position n ----
+// A text that does not start on a 16-byte boundary (a piece of a read stream) is read byte by byte.
 __global__ void count_newlines_kernel(const uint8_t* __restrict__ text, uint64_t n, uint32_t* __restrict__ counts, uint64_t nchunks) {
+  const bool aligned = ((uintptr_t)text & 15u) == 0;
   for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nchunks; c += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t b0 = c * 32;
     uint32_t k = 0;
-    if (b0 + 32 <= n) {
+    if (b0 + 32 <= n && aligned) {
       const uint4 a = __ldg((const uint4*)(text + b0)), b = __ldg((const uint4*)(text + b0 + 16));
       const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 #pragma unroll
@@ -30,7 +32,7 @@ __global__ void count_newlines_kernel(const uint8_t* __restrict__ text, uint64_t
         k += __popc(~(t | x | 0x7F7F7F7Fu));
       }
     } else {
-      for (uint64_t i = b0; i < n; ++i) k += text[i] == '\n';
+      for (uint64_t i = b0; i < n && i < b0 + 32; ++i) k += text[i] == '\n';
       if (n > 0 && text[n - 1] != '\n' && b0 + 32 > n && b0 <= n) k += 1;   // the virtual final newline lives in the last chunk
     }
     counts[c] = k;
@@ -39,10 +41,11 @@ __global__ void count_newlines_kernel(const uint8_t* __restrict__ text, uint64_t
 // (3) positions of the newlines, in order
 __global__ void write_newlines_kernel(const uint8_t* __restrict__ text, uint64_t n, const uint32_t* __restrict__ first, uint64_t nchunks,
                                       uint64_t* __restrict__ nl_pos) {
+  const bool aligned = ((uintptr_t)text & 15u) == 0;
   for (uint64_t c = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; c < nchunks; c += (uint64_t)gridDim.x * blockDim.x) {
     const uint64_t b0 = c * 32;
     uint32_t k = first[c];
-    if (b0 + 32 <= n) {
+    if (b0 + 32 <= n && aligned) {
       const uint4 a = __ldg((const uint4*)(text + b0)), b = __ldg((const uint4*)(text + b0 + 16));
       const uint32_t w[8] = {a.x, a.y, a.z, a.w, b.x, b.y, b.z, b.w};
 #pragma unroll
@@ -52,8 +55,8 @@ __global__ void write_newlines_kernel(const uint8_t* __restrict__ text, uint64_t
         while (z) { const uint32_t bit = __ffs(z) - 1; z &= z - 1; nl_pos[k++] = b0 + 4 * i + (bit >> 3); }
       }
     } else {
-      for (uint64_t i = b0; i < n; ++i) if (text[i] == '\n') nl_pos[k++] = i;
-      if (n > 0 && text[n - 1] != '\n') nl_pos[k] = n;
+      for (uint64_t i = b0; i < n && i < b0 + 32; ++i) if (text[i] == '\n') nl_pos[k++] = i;
+      if (n > 0 && text[n - 1] != '\n' && b0 + 32 > n) nl_pos[k] = n;
     }
   }
 }

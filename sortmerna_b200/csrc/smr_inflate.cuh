@@ -32,9 +32,11 @@ __global__ void __launch_bounds__(256) inf_find_kernel(const uint32_t* __restric
   if (threadIdx.x == 0) cand[blockIdx.x] = best;
 }
 
-// COUNT / WRITE: thread t decodes span ids[t] (COUNT: ids == nullptr, span t).  Span 0 starts at the gzip header, span i at cand[i-1].
+// COUNT / WRITE: thread t decodes span ids[t] (COUNT: ids == nullptr, span t).  Span 0 starts at bit start0 (a gzip header when
+// at_member0; else a block of a member of which prior0 bytes came before), span i at cand[i-1].
 template <bool WRITE>
-__global__ void __launch_bounds__(kInfSpanThreads) inf_span_kernel(const uint32_t* __restrict__ w, uint64_t nbytes, const uint64_t* __restrict__ cand, uint32_t ncand,
+__global__ void __launch_bounds__(kInfSpanThreads) inf_span_kernel(const uint32_t* __restrict__ w, uint64_t nbytes, uint64_t start0, bool at_member0, uint64_t prior0,
+                                                                    const uint64_t* __restrict__ cand, uint32_t ncand,
                                                                     const uint32_t* __restrict__ ids, const uint64_t* __restrict__ off, const uint64_t* __restrict__ cap,
                                                                     const uint32_t* __restrict__ mem_off, MemberEnd* mem, uint32_t nspans, uint16_t* sym, SpanResult* res) {
   extern __shared__ __align__(16) unsigned char inf_smem[];
@@ -43,16 +45,17 @@ __global__ void __launch_bounds__(kInfSpanThreads) inf_span_kernel(const uint32_
   if (t >= nspans) return;
   const uint32_t i = WRITE ? ids[t] : t;
   SpanResult r;
-  inflate_span<WRITE>(w, nbytes, i ? cand[i - 1] : 0ull, i == 0, cand, ncand, i, tabs[threadIdx.x].t, WRITE ? sym + off[t] : nullptr, WRITE ? cap[t] : 0ull,
-                      WRITE ? mem + mem_off[t] : nullptr, r);
+  inflate_span<WRITE>(w, nbytes, i ? cand[i - 1] : start0, i == 0 && at_member0, cand, ncand, i, tabs[threadIdx.x].t, WRITE ? sym + off[t] : nullptr, WRITE ? cap[t] : 0ull,
+                      WRITE ? mem + mem_off[t] : nullptr, r, i == 0 && !at_member0 ? prior0 : kInfNone);
   res[t] = r;
 }
 
-// WINDOW: the 32 KB every real span leaves behind, resolved front to back by ONE CTA (span k needs only window k); window 0 is empty.
+// WINDOW: the 32 KB every real span leaves behind, resolved front to back by ONE CTA (span k needs only window k); window 0 is the
+// caller's: zeros at the start of a file, the last 32 KB of the previous round's output when a round resumes.
 __global__ void __launch_bounds__(1024) inf_window_kernel(const uint16_t* __restrict__ sym, const uint64_t* __restrict__ off, const uint64_t* __restrict__ cnt,
                                                            uint32_t nreal, uint8_t* win) {
   __shared__ uint8_t prev[kInfWindow];
-  for (uint32_t j = threadIdx.x; j < kInfWindow; j += blockDim.x) { prev[j] = 0; win[j] = 0; }
+  for (uint32_t j = threadIdx.x; j < kInfWindow; j += blockDim.x) prev[j] = win[j];
   __syncthreads();
   for (uint32_t k = 0; k < nreal; ++k) {
     const uint16_t* s = sym + off[k];

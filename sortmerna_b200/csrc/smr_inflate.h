@@ -18,6 +18,12 @@
 //             byte, or 256 + k for "byte k of the 32 KB that precede this span" (a MARKER).
 //   4. WINDOW the last 32 KB of every span are resolved front to back (each needs only the previous span's window);
 //   5. RESOLVE every symbol becomes a byte, all spans in parallel.
+//
+// The five steps run in ROUNDS over whatever part of the file is held, so a file can be inflated as it arrives (the read stream
+// of smr_stream_push).  A round that is not the file's last lets its last span decode until the input runs out and resumes the
+// next round at the last block boundary that span crossed (InfResume): the output up to there is kept, the 32 KB before it seed
+// the window of the next round's first span, and the CRC-32 / length of the member still open carry over (InfCarry).  A whole
+// file in memory is the one-round case.
 #pragma once
 #include <cstddef>
 #include <cstdint>
@@ -218,38 +224,57 @@ SMR_HD uint64_t gz_member_header(const uint8_t* p, uint64_t nbytes, uint64_t at)
   return q + 8 <= nbytes ? q : kInfNone;
 }
 
+// Could the bytes at `at` still become a gzip member header once more bytes arrive?  (what is there matches ID1 ID2 CM FLG)
+SMR_HD bool gz_member_short(const uint8_t* p, uint64_t nbytes, uint64_t at) {
+  const uint8_t id[3] = {0x1f, 0x8b, 8};
+  for (uint64_t k = 0; k < 3; ++k) if (at + k < nbytes && p[at + k] != id[k]) return false;
+  return !(at + 3 < nbytes && (p[at + 3] & 0xE0u));
+}
+
 struct SpanResult {
   uint64_t end_bit;     // landed: the candidate position; eos: first bit after the last trailer
   uint64_t out_n;       // bytes produced
   uint32_t status;      // InfStatus
   uint32_t isize_sum;   // sum of the ISIZE fields of the members that ended in this span (mod 2^32)
-  uint64_t member_out;  // bytes produced since the last member start seen in this span (kInfNone: no member start seen)
   uint32_t members;     // gzip members that ended in this span
   uint32_t pad;
+  uint64_t blk_bit;     // start of the last block the span began to decode (a round that ran out of input resumes there)
+  uint64_t blk_out;     // bytes produced before that block
+  uint64_t stop_bit;    // how far the decoder had read when it stopped (an error this close to the end of a partial input may be the cut);
+                        // a member header that failed: nbits if more bytes may still complete it, else its start
 };
 struct MemberEnd { uint64_t out_end; uint32_t crc, isize; };   // trailer of a member (RFC 1952 2.3.1); out_end counts from the span's first byte
 
 // One span: decode from `start_bit` (a block start; or a member header when `at_member` is set) until a block boundary that is one of
 // the sorted candidate positions cand[first_cand ..ncand) or the end of the gzip stream.  WRITE: 16-bit symbols to out[0 .. out_cap).
+// member_prior: bytes of the open member produced before start_bit, when they are known (the first span of a resumed round);
+// kInfNone otherwise.
 template <bool WRITE>
 SMR_HD void inflate_span(const uint32_t* w, uint64_t nbytes, uint64_t start_bit, bool at_member, const uint64_t* cand, uint32_t ncand,
-                         uint32_t first_cand, HuffTabs& T, uint16_t* out, uint64_t out_cap, MemberEnd* mem, SpanResult& res) {
+                         uint32_t first_cand, HuffTabs& T, uint16_t* out, uint64_t out_cap, MemberEnd* mem, SpanResult& res,
+                         uint64_t member_prior = kInfNone) {
   const uint8_t* bytes = reinterpret_cast<const uint8_t*>(w);
   const uint64_t nbits = nbytes * 8, wlimit = (nbits >> 5) + 3;   // a decoder that has loaded this many words ran past the end
-  uint64_t n = 0, member_base = kInfNone;
+  bool member_known = member_prior != kInfNone;
+  uint64_t n = 0, member_base = 0 - member_prior, blk_bit = start_bit, blk_out = 0;   // member_base wraps: n - member_base = bytes of the member
   uint32_t nextc = first_cand, isize_sum = 0, members = 0;
   BitIn b; b.w = w;
-  auto finish = [&](uint32_t st, uint64_t endb) { res.end_bit = endb; res.out_n = n; res.status = st; res.isize_sum = isize_sum; res.members = members; res.pad = 0; res.member_out = member_base == kInfNone ? kInfNone : n - member_base; };
+  bool seeked = false;
+  auto finish = [&](uint32_t st, uint64_t endb) {
+    res.end_bit = endb; res.out_n = n; res.status = st; res.isize_sum = isize_sum; res.members = members; res.pad = 0;
+    res.blk_bit = blk_bit; res.blk_out = blk_out; res.stop_bit = seeked ? bi_pos(b) : endb;
+  };
   uint64_t pos = start_bit;
   if (at_member) {
     const uint64_t q = gz_member_header(bytes, nbytes, pos >> 3);
-    if (q == kInfNone) { finish(kInfErrMember, pos); return; }
-    pos = q * 8; member_base = 0;
+    if (q == kInfNone) { finish(kInfErrMember, pos); if (gz_member_short(bytes, nbytes, pos >> 3)) res.stop_bit = nbits; return; }
+    pos = q * 8; member_base = 0; member_known = true;
   }
-  bi_seek(b, pos);
+  bi_seek(b, pos); seeked = true;
   bool first_block = true;
   for (;;) {
     pos = bi_pos(b);
+    blk_bit = pos; blk_out = n;
     if (pos + 3 > nbits) { finish(kInfErrOverrun, pos); return; }
     if (!first_block || at_member) {   // a block boundary reached by decoding: is it another span's start?
       while (nextc < ncand && cand[nextc] < pos) ++nextc;
@@ -304,7 +329,7 @@ SMR_HD void inflate_span(const uint32_t* w, uint64_t nbytes, uint64_t start_bit,
         if (ds > 29) { finish(kInfErrCode, bi_pos(b)); return; }
         inf_dist_sym(ds, dbase, dextra);
         const uint32_t dist = dbase + bi_get(b, dextra);    // <= 13 bits after <= 15 of the code
-        if (member_base != kInfNone && dist > n - member_base) { finish(kInfErrDistance, bi_pos(b)); return; }   // zlib: "invalid distance too far back"
+        if (member_known && dist > n - member_base) { finish(kInfErrDistance, bi_pos(b)); return; }   // zlib: "invalid distance too far back"
         if (WRITE) {
           if (n + len > out_cap) { finish(kInfErrCapacity, pos); return; }
           // the copy (3.2.3): up to `dist` symbols never overlap what they produce, so they are loaded together before they are
@@ -341,7 +366,7 @@ SMR_HD void inflate_span(const uint32_t* w, uint64_t nbytes, uint64_t start_bit,
       q += 8;
       const uint64_t h = gz_member_header(bytes, nbytes, q);
       if (h == kInfNone) { finish(kInfEos, q * 8); return; }   // gzip: trailing bytes that are no member are ignored
-      member_base = n;
+      member_base = n; member_known = true;
       bi_seek(b, h * 8);
     }
   }
@@ -374,8 +399,10 @@ inline uint32_t crc_concat(uint32_t crc_a, uint32_t crc_b, uint64_t len_b) {   /
 }
 
 // Host side of the CRC / ISIZE check: the members (trailers in stream order, out_end = offset in the whole output) are cut into
-// pieces that end at multiples of `piece` bytes; `first[m]` = first piece of member m.
-inline void inf_crc_plan(const std::vector<MemberEnd>& ends, uint32_t piece, std::vector<uint64_t>& poff, std::vector<uint32_t>& plen, std::vector<uint32_t>& first) {
+// pieces that end at multiples of `piece` bytes; `first[m]` = first piece of member m.  Output past the last trailer, up to
+// `total`, belongs to the member still open at the end of a round: its pieces follow, from first[ends.size()] to first[ends.size() + 1].
+inline void inf_crc_plan(const std::vector<MemberEnd>& ends, uint32_t piece, std::vector<uint64_t>& poff, std::vector<uint32_t>& plen, std::vector<uint32_t>& first,
+                         uint64_t total = 0) {
   poff.clear(); plen.clear(); first.clear();
   uint64_t a = 0;
   for (const MemberEnd& m : ends) {
@@ -387,16 +414,30 @@ inline void inf_crc_plan(const std::vector<MemberEnd>& ends, uint32_t piece, std
     }
   }
   first.push_back((uint32_t)poff.size());
+  while (a < total) {
+    const uint64_t stop = std::min<uint64_t>(total, (a / piece + 1) * piece);
+    poff.push_back(a); plen.push_back((uint32_t)(stop - a));
+    a = stop;
+  }
+  first.push_back((uint32_t)poff.size());
 }
-inline uint32_t inf_crc_verify(const std::vector<MemberEnd>& ends, const std::vector<uint32_t>& plen, const std::vector<uint32_t>& first, const uint32_t* crcs) {
-  uint64_t a = 0;
+// CRC-32 and length of the member that is open where a round ends; the next round's first member starts with them
+struct InfCarry { uint32_t crc = 0; uint64_t len = 0; };   // 0 = CRC of the empty string
+inline uint32_t inf_crc_verify(const std::vector<MemberEnd>& ends, const std::vector<uint32_t>& plen, const std::vector<uint32_t>& first, const uint32_t* crcs,
+                               InfCarry* carry = nullptr) {
+  InfCarry c0;
+  InfCarry& cy = carry ? *carry : c0;
+  uint64_t a = 0 - cy.len;   // wraps: out_end - a = the member's whole length
   for (size_t m = 0; m < ends.size(); ++m) {
     if ((uint32_t)(ends[m].out_end - a) != ends[m].isize) return kInfErrSize;
-    uint32_t c = 0;   // CRC of the empty string
+    uint32_t c = m ? 0u : cy.crc;
     for (uint32_t k = first[m]; k < first[m + 1]; ++k) c = crc_concat(c, crcs[k], plen[k]);
     if (c != ends[m].crc) return kInfErrCrc;
     a = ends[m].out_end;
   }
+  if (!ends.empty()) cy = InfCarry{};
+  if (first.size() > ends.size() + 1)
+    for (uint32_t k = first[ends.size()]; k < first[ends.size() + 1]; ++k) { cy.crc = crc_concat(cy.crc, crcs[k], plen[k]); cy.len += plen[k]; }
   return 0;
 }
 
@@ -408,9 +449,18 @@ SMR_HD uint8_t inf_window_byte(const uint16_t* syms, uint64_t n, const uint8_t* 
   return v >= 0 ? inf_resolve(syms[v], prev_window) : prev_window[kInfWindow + v];
 }
 
-// The walk over the COUNT results (host side): span 0 is the start of the stream, span i >= 1 starts at cand[i - 1].  Fills
-// `real` with the spans that are reached and `off` with their output offsets; returns the total size or kInfNone with *why set.
-inline uint64_t inf_chain(const uint64_t* cand, uint32_t ncand, const SpanResult* res, uint32_t* real, uint64_t* off, uint32_t& nreal, uint32_t* why) {
+// Where a round of the inflate ends.  bit: where the next round starts (in the round's input); at_member: a gzip member header is
+// due there; keep_last: the bytes of the chain's last span that are kept (its output up to `bit`); eos: the stream ended.
+struct InfResume { uint64_t bit = 0; bool at_member = true; bool eos = false; uint64_t keep_last = 0; };
+
+// The walk over the COUNT results (host side): span 0 is the start of the round, span i >= 1 starts at cand[i - 1].  Fills
+// `real` with the spans that are reached and `off` with their output offsets; returns the bytes the round keeps or kInfNone
+// with *why set.  A round over the whole rest of the file (eof) must end in the end of the gzip stream.  Otherwise (next != null,
+// eof false) the chain may end in a span that ran out of input: the round keeps the output up to that span's last block boundary
+// and *next says where to resume.  The sum of the ISIZE fields is checked here when the round covers whole members (isize_check);
+// every member is checked again, with its CRC, after the write pass.
+inline uint64_t inf_chain(const uint64_t* cand, uint32_t ncand, const SpanResult* res, uint32_t* real, uint64_t* off, uint32_t& nreal, uint32_t* why,
+                          bool eof = true, uint64_t nbits = 0, bool isize_check = true, InfResume* next = nullptr) {
   uint64_t total = 0;
   uint32_t isize = 0;
   nreal = 0;
@@ -418,14 +468,32 @@ inline uint64_t inf_chain(const uint64_t* cand, uint32_t ncand, const SpanResult
   for (;;) {
     real[nreal] = i; off[nreal] = total; ++nreal;
     total += res[i].out_n; isize += res[i].isize_sum;
-    if (res[i].status == kInfEos) break;
-    if (res[i].status != kInfLanded) { *why = res[i].status; return kInfNone; }
+    if (next) next->keep_last = res[i].out_n;
+    if (res[i].status == kInfEos) {
+      if (next) { next->bit = res[i].end_bit; next->at_member = true; next->eos = eof; }
+      break;
+    }
+    if (res[i].status != kInfLanded) {
+      // before the end of the file: the last span stopped because the input ran out -- or it met an error close enough to the end
+      // that the missing bytes may be the cause (a decode error reads at most 64 bits past what it consumed), or a member header
+      // that has not fully arrived
+      const bool cut = res[i].status == kInfErrMember ? res[i].stop_bit >= nbits : (res[i].status == kInfErrOverrun || res[i].stop_bit + 128 > nbits);
+      if (!eof && next && cut) {
+        total -= res[i].out_n - res[i].blk_out;
+        next->keep_last = res[i].blk_out;
+        if (res[i].status == kInfErrMember) next->bit = res[i].end_bit;
+        else { next->bit = res[i].blk_bit; next->at_member = false; }
+        next->eos = false;
+        return total;
+      }
+      *why = res[i].status; return kInfNone;
+    }
     uint32_t lo = i, hi = ncand;   // the candidate it landed on: cand[] is sorted, and it lies after span i's own start
     while (lo < hi) { const uint32_t mid = (lo + hi) / 2; if (cand[mid] < res[i].end_bit) lo = mid + 1; else hi = mid; }
     if (lo >= ncand || cand[lo] != res[i].end_bit) { *why = kInfErrMember; return kInfNone; }
     i = lo + 1;
   }
-  if ((uint32_t)total != isize) { *why = kInfErrSize; return kInfNone; }   // RFC 1952 ISIZE: sizes mod 2^32 (per member again after the write pass)
+  if (isize_check && (uint32_t)total != isize) { *why = kInfErrSize; return kInfNone; }   // RFC 1952 ISIZE: sizes mod 2^32 (per member again after the write pass)
   return total;
 }
 
