@@ -234,15 +234,28 @@ int smr_debug_inflate(smr_ctx*, const void* gz, uint64_t nbytes, uint64_t chunk_
  * -threads (each split restarts the cycle at a '>' line); these are the single-split figures, which -threads 1 and gzip input give.
  * They are what Refstats::minimal_score and the E-value read length are computed from.  SMR_STREAM_COUNT_ONLY counts and keeps no
  * text: the cheap first pass over a file. */
-enum { SMR_STREAM_GZ = 1, SMR_STREAM_COUNT_ONLY = 2, SMR_STREAM_NEXT_FILE = 4 };
+enum { SMR_STREAM_GZ = 1, SMR_STREAM_COUNT_ONLY = 2, SMR_STREAM_NEXT_FILE = 4, SMR_STREAM_MATES = 8 };
 /* open (or reset) the context's read stream; batch_bytes = text bytes per batch, in [1, 0xF0000000) (ignored with COUNT_ONLY).  Every
  * batch but the file's last holds the whole records that fit in batch_bytes; before the end of the file, pending text that fits in
  * one batch waits for the next push.  SMR_STREAM_NEXT_FILE: the counts go on from the previous stream's, as the reference counts
  * the -reads files of one run (mates): totals add up, the line cycle of the first file holds, a gzip file updates the minimum read
  * by read and a flat file's own minimum is merged at its end (readfeed.cpp:1497-1662). */
 int smr_stream_begin(smr_ctx*, uint32_t flags, uint64_t batch_bytes);
-/* the next n bytes of the file; eof = 1 with the last piece (n may be 0) */
+/* the next n bytes of the file; eof = 1 with the last piece (n may be 0).  SMR_ERR_ARG on a mate stream. */
 int smr_stream_push(smr_ctx*, const void* bytes, uint64_t n, int eof);
+/* SMR_STREAM_MATES: a stream of two mate files (-reads R1 -reads R2), records k of both files paired (sortmerna_b200/csrc/smr_stream.cuh,
+ * DESIGN.md 5c).  Each mate is pushed on its own, mate = 1 or 2, in pieces of any size; SMR_STREAM_GZ applies to both, and each is
+ * inflated and indexed as a single stream's file.  smr_stream_next makes a batch of k pairs resident: record k of mate 1 and then
+ * record k of mate 2, as one interleaved text (records 2k and 2k+1), a last line without '
+' given one.  k is the largest number
+ * of pairs both files hold whose interleaved text fits in batch_bytes, or 1 when the first pair alone is longer; before both files
+ * have ended, pairs that fit wait for more pushes.  The batch is then used as any resident batch; smr_format_reports[_gz] with text
+ * == nullptr treats it as mates (smr_report_opts.mates).  SMR_ERR_ARG, closing the stream, for: one mate FASTQ and the other FASTA;
+ * files that differ in record count (at the smr_stream_next that finds one file ended while the other holds a record); a corrupt
+ * gzip input of either mate (the message names the mate); smr_stream_push_mate on a stream without SMR_STREAM_MATES.  A mate
+ * stream counts nothing (smr_stream_counts stays 0): count the mate files one after another with SMR_STREAM_NEXT_FILE.  MATES with
+ * COUNT_ONLY or NEXT_FILE is SMR_ERR_ARG. */
+int smr_stream_push_mate(smr_ctx*, uint32_t mate, const void* bytes, uint64_t n, int eof);
 /* make the next batch resident: *nreads > 0 = a batch is resident (as after smr_upload_fastx); *nreads == 0 and *done == 0 = push
  * more; *done == 1 = the file is exhausted */
 int smr_stream_next(smr_ctx*, uint32_t* nreads, int* done);
@@ -288,7 +301,10 @@ typedef struct {
   int32_t denovo;              /* -de_novo_otu: aligned_denovo.* */
   double min_id, min_cov;      /* -id, -coverage (the aligned_denovo rule) */
   int32_t paired_in, paired_out; /* the batch is interleaved mates: records 2k and 2k+1 */
-  int32_t out2, sout;          /* SMR_ERR_UNSUPPORTED */
+  int32_t out2, sout;          /* -out2, -sout: aligned / other / aligned_denovo each split into 2 files (4 with both), for a paired
+                                  batch only (SMR_ERR_UNSUPPORTED otherwise); -sout with paired_in / paired_out is SMR_ERR_ARG */
+  int32_t mates;               /* records 2k and 2k+1 are mates from two files (-reads R1 -reads R2): paired, as the reference
+                                  makes every two-file run (options.cpp:1590-1592); forced on for the resident batch of a mate stream */
 } smr_report_opts;
 
 /* Format one batch.  text / nbytes: the FASTA or FASTQ text of the reads, in batch order; text == nullptr means the resident text of
@@ -297,15 +313,17 @@ typedef struct {
  * from the text.  The number of records and every aligned read's length must agree with the results (SMR_ERR_ARG otherwise).
  * Output: the streams one after another, in this order: SAM rows of every loaded (index, part) group in (index, part) order, BLAST
  * rows of every group, aligned reads, other reads, aligned_denovo reads; stream k = out[stream_off[k] .. stream_off[k+1]),
- * stream_off has 2 * groups + 4 entries.  A caller that feeds a file in several batches appends every stream to its own file and
- * concatenates them at the end, as the reference's merge does.  If out is null or cap is below stream_off[2 * groups + 3], the call
+ * stream_off has 2 * groups + 3 * num_out + 1 entries.  num_out = 1, or 2 with -out2 (_fwd, _rev) or -sout (_paired, _singleton),
+ * or 4 with both (_paired_fwd, _paired_rev, _singleton_fwd, _singleton_rev): each of the three read files is num_out streams in
+ * that order (report_fx_base.cpp:73-90), routed as ReportFastx / ReportFxOther / ReportDenovo::append at -threads 1.  A caller that feeds a file in several batches appends every stream to its own file and
+ * concatenates them at the end, as the reference's merge does.  If out is null or cap is below the last entry of stream_off, the call
  * returns SMR_ERR_CAPACITY with stream_off filled. */
 int smr_format_reports(smr_ctx*, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
                        const smr_aln* alns, const uint32_t* cigar_pool, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
                        char* out, uint64_t cap, uint64_t* stream_off);
 /* The same streams, each non-empty one compressed on the device to one gzip member (RFC 1952) before the D2H: the reference's
  * -zip-out output (its report writers go through zlib's gzip wrapper, izlib.cpp).  An empty stream stays 0 bytes.  Arguments and
- * stream_off as for smr_format_reports, with the sizes of the members: if out is null or cap is below stream_off[2 * groups + 3], the
+ * stream_off as for smr_format_reports, with the sizes of the members: if out is null or cap is below the last entry of stream_off, the
  * call returns SMR_ERR_CAPACITY with the exact compressed sizes in stream_off, and a retry gives the same bytes.  The members are not
  * zlib's bytes (sortmerna_b200/csrc/smr_deflate.h) but the same input always gives the same bytes. */
 int smr_format_reports_gz(smr_ctx*, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,

@@ -29,7 +29,8 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_set_aln_slots", "smr_aln_slots", "smr_aln_slots_needed", "smr_upload_fastx_gz", "smr_resident_text", "smr_debug_inflate",
            "smr_build_index_device", "smr_debug_index_array", "smr_set_instrumentation", "smr_set_report_refs", "smr_set_report_scoring",
            "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings",
-           "smr_format_reports_gz", "smr_gzip", "smr_stream_begin", "smr_stream_push", "smr_stream_next", "smr_stream_counts"]
+           "smr_format_reports_gz", "smr_gzip", "smr_stream_begin", "smr_stream_push", "smr_stream_next", "smr_stream_counts",
+           "smr_stream_push_mate"]
 
 CNT_NAMES = ("num_aligned", "num_short", "sw_calls", "sw_cells", "windows", "trie_nodes", "buckets",
              "bucket_entries", "pos_entries", "lis_calls", "dbg_max_read_cycles", "dbg_sum_read_cycles", "dbg_lis_kernel_cycles",
@@ -71,14 +72,16 @@ class ReportOpts(C.Structure):
     """smr_report_opts (include/smr_b200.h)"""
     _fields_ = [("sam", C.c_int32), ("blast", C.c_int32), ("blast_format", C.c_int32), ("blast_cols", C.c_int32 * 4), ("fastx", C.c_int32),
                 ("other", C.c_int32), ("denovo", C.c_int32), ("min_id", C.c_double), ("min_cov", C.c_double), ("paired_in", C.c_int32),
-                ("paired_out", C.c_int32), ("out2", C.c_int32), ("sout", C.c_int32)]
+                ("paired_out", C.c_int32), ("out2", C.c_int32), ("sout", C.c_int32), ("mates", C.c_int32)]
 
 
-def report_opts(sam=False, blast=None, fastx=False, other=False, denovo=None, paired_in=False, paired_out=False, out2=False, sout=False) -> ReportOpts:
+def report_opts(sam=False, blast=None, fastx=False, other=False, denovo=None, paired_in=False, paired_out=False, out2=False, sout=False,
+                mates=False) -> ReportOpts:
     """blast: None, or the value of the reference's -blast option ('1 cigar qcov qstrand'; '0' = pairwise, refused by the writer);
-    denovo: None, or (min_id, min_cov) = the reference's -id / -coverage."""
+    denovo: None, or (min_id, min_cov) = the reference's -id / -coverage; mates: records 2k and 2k+1 come from two mate files
+    (implied for the resident batch of stream_mates)."""
     o = ReportOpts(sam=int(bool(sam)), fastx=int(bool(fastx)), other=int(bool(other)), paired_in=int(bool(paired_in)),
-                   paired_out=int(bool(paired_out)), out2=int(bool(out2)), sout=int(bool(sout)))
+                   paired_out=int(bool(paired_out)), out2=int(bool(out2)), sout=int(bool(sout)), mates=int(bool(mates)))
     if blast is not None:
         f = str(blast).split()
         o.blast, o.blast_format = 1, int(f[0])
@@ -92,6 +95,21 @@ def report_opts(sam=False, blast=None, fastx=False, other=False, denovo=None, pa
 class OtuOpts(C.Structure):
     """smr_otu_opts (include/smr_b200.h)"""
     _fields_ = [("min_id", C.c_double), ("min_cov", C.c_double), ("paired_in", C.c_int32), ("paired_out", C.c_int32)]
+
+
+def num_out_of(o: ReportOpts) -> int:
+    """files per kind of read file (ReportFxBase::set_num_out, report_fx_base.cpp:165-171)"""
+    return 4 if o.out2 and o.sout else 2 if o.out2 or o.sout else 1
+
+
+def fx_suffixes(o: ReportOpts) -> list:
+    """the name suffixes of a kind's num_out files, in stream order (report_fx_base.cpp:73-90)"""
+    n = num_out_of(o)
+    if n == 4:
+        return ["_paired_fwd", "_paired_rev", "_singleton_fwd", "_singleton_rev"]
+    if n == 2:
+        return ["_fwd", "_rev"] if o.out2 else ["_paired", "_singleton"]
+    return [""]
 
 
 _lib = None
@@ -120,6 +138,7 @@ def load_library():
         L.smr_stream_push.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_int]
         L.smr_stream_next.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
         L.smr_stream_counts.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
+        L.smr_stream_push_mate.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_int]
         for name in SYMBOLS:
             getattr(L, name)  # AttributeError if the build is stale
         _lib = L
@@ -372,17 +391,21 @@ class Aligner:
         return out.tobytes(), {"spans": info[0], "candidates": info[1], "device_us": info[2], "h2d_us": info[3]}
 
     # -- read stream (smr_stream_*): files of any size, pushed from disk piece by piece --
-    STREAM_GZ, STREAM_COUNT_ONLY, STREAM_NEXT_FILE = 1, 2, 4
+    STREAM_GZ, STREAM_COUNT_ONLY, STREAM_NEXT_FILE, STREAM_MATES = 1, 2, 4, 8
 
-    def _push_file(self, path: str, piece_bytes: int):
-        """Pushes the file at `path` into the open stream, piece by piece; yields after every push."""
+    def _push_file(self, path: str, piece_bytes: int, mate: int = 0):
+        """Pushes the file at `path` into the open stream, piece by piece (mate 1 / 2 of a mate stream: smr_stream_push_mate);
+        yields after every push."""
         with open(path, "rb") as f:
             piece = f.read(piece_bytes)
             while True:
                 nxt = f.read(piece_bytes) if piece else b""
                 buf = np.frombuffer(piece, dtype=np.uint8)
-                self._check(self.L.smr_stream_push(self.h, _ptr(buf) if buf.size else C.c_void_p(0), C.c_uint64(buf.size), C.c_int(0 if nxt else 1)),
-                            "smr_stream_push")
+                args = (_ptr(buf) if buf.size else C.c_void_p(0), C.c_uint64(buf.size), C.c_int(0 if nxt else 1))
+                if mate:
+                    self._check(self.L.smr_stream_push_mate(self.h, C.c_uint32(mate), *args), "smr_stream_push_mate")
+                else:
+                    self._check(self.L.smr_stream_push(self.h, *args), "smr_stream_push")
                 yield
                 if not nxt:
                     return
@@ -413,19 +436,35 @@ class Aligner:
         time and is never held whole in host memory."""
         flags = self.STREAM_GZ if self._is_gz(path) else 0
         self._check(self.L.smr_stream_begin(self.h, C.c_uint32(flags), C.c_uint64(batch_bytes)), "smr_stream_begin")
-        n, done = C.c_uint32(0), C.c_int(0)
-
-        def drain():
-            while True:
-                self._check(self.L.smr_stream_next(self.h, C.byref(n), C.byref(done)), "smr_stream_next")
-                if n.value == 0:
-                    return
-                self._n_resident = int(n.value)
-                yield int(n.value)
-
         for _ in self._push_file(path, piece_bytes):
-            yield from drain()
-        yield from drain()
+            yield from self._drain()
+        yield from self._drain()
+
+    def _drain(self):
+        """the batches the open stream can make now: yields the read count of each once it is resident"""
+        n, done = C.c_uint32(0), C.c_int(0)
+        while True:
+            self._check(self.L.smr_stream_next(self.h, C.byref(n), C.byref(done)), "smr_stream_next")
+            if n.value == 0:
+                return
+            self._n_resident = int(n.value)
+            yield int(n.value)
+
+    def stream_mates(self, path1: str, path2: str, batch_bytes: int = 256 << 20, piece_bytes: int = 256 << 20):
+        """Streams two mate files (the reference's -reads R1 -reads R2; plain or gzip by their magic bytes, both alike) through the
+        device as pairs: every batch is k whole pairs interleaved (records 2k and 2k+1 are record k of each file) in at most
+        batch_bytes of text, or one longer pair alone.  Yields the read count (2k) of each batch once it is resident, as
+        stream_fastx; format_reports / ReportWriter.write(out) route it as mates.  Each round pushes one piece of each file that
+        has not ended, then takes the batches that are ready.  Files that differ in record count or format raise SmrError."""
+        gz = [self._is_gz(p) for p in (path1, path2)]
+        if gz[0] != gz[1]:
+            raise SmrError(f"stream_mates: {path1 if gz[0] else path2} is gzip and {path2 if gz[0] else path1} is not")
+        flags = self.STREAM_MATES | (self.STREAM_GZ if gz[0] else 0)
+        self._check(self.L.smr_stream_begin(self.h, C.c_uint32(flags), C.c_uint64(batch_bytes)), "smr_stream_begin")
+        feeds = [self._push_file(path1, piece_bytes, 1), self._push_file(path2, piece_bytes, 2)]
+        while feeds:
+            feeds = [f for f in feeds if next(f, StopIteration) is not StopIteration]
+            yield from self._drain()
 
     def stream_counts(self) -> dict:
         """smr_stream_counts of the open stream: the count_reads_parallel figures of what was pushed so far."""
@@ -517,7 +556,9 @@ class Aligner:
         """smr_format_reports: the report streams of one batch as bytes.  out = what align(with_stats=True) / download(with_stats=True)
         returned for it; text = the batch's FASTA / FASTQ bytes (None: the resident text of upload_fastx[_gz]); opts = report_opts(...)
         or its keyword arguments.  Returns {"sam": [bytes per group], "blast": [...], "aligned": bytes, "other": bytes, "denovo": bytes,
-        "groups": report_groups()}.  gzip: smr_format_reports_gz, every non-empty stream as one gzip member (empty ones stay b"")."""
+        "groups": report_groups()}; with out2 or sout, "aligned" / "other" / "denovo" are tuples of the num_out files (2, or 4 with
+        both) in the reference's order (_fwd, _rev | _paired, _singleton | _paired_fwd, _paired_rev, _singleton_fwd, _singleton_rev).
+        gzip: smr_format_reports_gz, every non-empty stream as one gzip member (empty ones stay b"")."""
         o = opts if opts is not None else report_opts(**kw)
         if o.sam or o.blast:
             self._upload_report_refs()
@@ -527,7 +568,8 @@ class Aligner:
         cig = np.ascontiguousarray(out["cigar"], np.uint32)
         st = out.get("stats")
         txt = np.frombuffer(text, np.uint8) if text is not None else None
-        so = np.zeros(2 * G + 4, np.uint64)
+        num_out = num_out_of(o)
+        so = np.zeros(2 * G + 3 * num_out + 1, np.uint64)
         fn = self.L.smr_format_reports_gz if gzip else self.L.smr_format_reports
         fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
                        C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
@@ -542,8 +584,10 @@ class Aligner:
             rc = fn(*args, _ptr(buf), buf.size, _ptr(so))
         self._check(rc, "smr_format_reports_gz" if gzip else "smr_format_reports")
         self._report_buf = buf
-        b = [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(2 * G + 3)]
-        return dict(sam=b[:G], blast=b[G:2 * G], aligned=b[2 * G], other=b[2 * G + 1], denovo=b[2 * G + 2], groups=groups)
+        b = [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(so.size - 1)]
+        fx = [b[2 * G + j * num_out:2 * G + (j + 1) * num_out] for j in range(3)]
+        fx = [f[0] for f in fx] if num_out == 1 else [tuple(f) for f in fx]
+        return dict(sam=b[:G], blast=b[G:2 * G], aligned=fx[0], other=fx[1], denovo=fx[2], groups=groups)
 
     # ---- OTU map (smr_otu_begin / smr_otu_add / smr_otu_finish) ----
     def otu_begin(self, min_id: float = 0.97, min_cov: float = 0.97, paired_in: bool = False, paired_out: bool = False):
@@ -639,7 +683,10 @@ class ReportWriter:
     passes, as the reference) and sets total_otu and n_yid_ycov, the two OTU numbers of aligned.log.
     zip_out: the reference's -zip-out (its default for gzip input): every report file is written gzip-compressed on the device under
     its name with ".gz" appended, as members appended batch by batch (a multi-member file, as the reference's merge makes); a file
-    with no member gets one empty member.  otu_map.txt stays plain, as the reference writes it."""
+    with no member gets one empty member.  otu_map.txt stays plain, as the reference writes it.
+    out2 / sout (opts): each read file is split as the reference's -out2 / -sout split it, aligned_fwd.fq / aligned_rev.fq,
+    aligned_paired.fq / aligned_singleton.fq, or aligned_paired_fwd.fq ... aligned_singleton_rev.fq with both, and likewise other.*
+    and aligned_denovo.*; batches of stream_mates are mates without further options (mates=True for a batch passed as text)."""
 
     def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", otu_map=None, zip_out: bool = False, **opts):
         self.dir, self.al, self.header, self.zip_out = out_dir, aligner, sam_header, zip_out
@@ -667,7 +714,8 @@ class ReportWriter:
             self._append(f"sam_{g}", rows_sam)
             self._append(f"blast_{g}", rows_blast)
         for k in ("aligned", "other", "denovo"):
-            self._append(k, s[k])
+            for j, data in enumerate(s[k] if isinstance(s[k], tuple) else (s[k],)):
+                self._append(f"{k}_{j}", data)
         if self.otu_map is not None:
             self.al.otu_add(out, text)
         return s
@@ -683,7 +731,7 @@ class ReportWriter:
             files.append(("aligned.blast", [f"blast_{g}" for g in range(len(groups))], b""))
         for flag, name, key in ((o.fastx, "aligned", "aligned"), (o.other, "other", "other"), (o.denovo, "aligned_denovo", "denovo")):
             if flag:
-                files.append((f"{name}.{ext}", [key], b""))
+                files += [(f"{name}{sfx}.{ext}", [f"{key}_{j}"], b"") for j, sfx in enumerate(fx_suffixes(o))]
         paths = []
         for name, keys, head in files:
             path = os.path.join(self.dir, name + (".gz" if self.zip_out else ""))

@@ -78,20 +78,26 @@ struct Batch {
 };
 
 // What a read stream's inflate carries from one round to the next (smr_inflate.h): where to resume, the open member's CRC-32 and
-// length, the members seen so far; the last 32 KB of output are in smr_ctx::d_infwin.
-struct InfStream { InfResume at; InfCarry carry; uint32_t members = 0; bool have_window = false; };
+// length, the members seen so far, and the last 32 KB of output (win; win2 is the scratch that replaces it).
+struct InfStream { InfResume at; InfCarry carry; uint32_t members = 0; bool have_window = false; DevBuf win, win2; };
 
-// The read stream of a context (smr_stream_begin .. smr_stream_next): the compressed bytes not inflated yet (gz) and the text not
-// made into a batch yet belong to it.
-struct ReadStream {
-  bool open = false, gz = false, count_only = false, eof = false;
-  uint64_t batch_bytes = 0;
+// One file of a read stream: the compressed bytes not inflated yet (gz) and the text not made into a batch yet.
+struct StreamSide {
+  bool eof = false;
   std::vector<uint8_t> tail;   // gz: the pushed bytes from the byte of the resume point on (inf.at.bit counts from tail[0])
   InfStream inf;
   DevBuf text;                 // pending text: [off, n) is not in a batch yet
   uint64_t off = 0, n = 0, pushed = 0;
   char first = 0;              // the file's first byte: '@' = FASTQ
   bool have_first = false;
+};
+
+// The read stream of a context (smr_stream_begin .. smr_stream_next): one file, or two mate files (SMR_STREAM_MATES) whose
+// records k are paired.  Their buffers belong to it.
+struct ReadStream {
+  bool open = false, gz = false, count_only = false, mates = false;
+  uint64_t batch_bytes = 0;
+  StreamSide side[2];          // side[1]: mate 2 of a mate stream
   CountState counts;
 };
 
@@ -122,8 +128,9 @@ struct smr_ctx {
   DevBuf cub_tmp;   // cub scratch of the text layout, the report writer and the OTU map
   DevBuf seed_ctr, d_gz, d_cand, d_res, d_sym, d_win, d_ids, d_off, d_cnt64, d_moff, d_mem, d_poff, d_plen, d_pcrc;   // gz inflate (smr_inflate.cuh)
   uint64_t text_bytes = 0;          // size of the text behind the resident batch (smr_upload_fastx / _gz)
-  DevBuf d_infwin, d_infwin2, d_rc, d_cut;   // read stream: carried inflate window, count-pass partials, batch cut
+  DevBuf d_rc, d_cut, d_mflag, d_mend[2];   // read stream: count-pass partials, batch cut; mate stream: record flags, record ends per mate
   ReadStream rs;
+  bool resident_mates = false;      // the resident batch came from a mate stream: records 2k and 2k+1 are mates
   uint32_t inf_spans = 0, inf_candidates = 0; double t_inflate = 0;
   double t_decode = 0;
   uint32_t tb_threads = 0, tb_cap_w = 0, tb_cap_cig = 0; size_t tb_cap_dir = 0, tb_stride = 0;
@@ -497,7 +504,7 @@ void finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
 // host reads -> the resident batch (no text behind it)
 void upload_batch_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads) {
   Batch& b = ctx->resident;
-  b.nreads = 0; b.from_text = false; ctx->text_bytes = 0;
+  b.nreads = 0; b.from_text = false; ctx->text_bytes = 0; ctx->resident_mates = false;
   if (nreads == 0) return;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
   CK(cudaEventRecord(e0, ctx->stream));
@@ -577,6 +584,7 @@ uint32_t upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, char
   Batch& b = ctx->resident;
   b.nreads = 0; b.from_text = true;
   ctx->text_bytes = nbytes;
+  ctx->resident_mates = false;
   if (nbytes == 0) return 0;
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
   CK(cudaEventRecord(e0, ctx->stream));
@@ -725,7 +733,7 @@ uint64_t inflate_round(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t c
         (const uint64_t*)ctx->d_cnt64.p, (const uint32_t*)ctx->d_moff.p, (MemberEnd*)ctx->d_mem.p, nreal, (uint16_t*)ctx->d_sym.p, (SpanResult*)ctx->d_res.p);
     CK(cudaGetLastError());
     // WINDOW (seeded with the last 32 KB of the previous round), RESOLVE of the bytes kept
-    if (st.have_window) CK(cudaMemcpyAsync(ctx->d_win.p, ctx->d_infwin.p, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
+    if (st.have_window) CK(cudaMemcpyAsync(ctx->d_win.p, st.win.p, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
     else CK(cudaMemsetAsync(ctx->d_win.p, 0, kInfWindow, ctx->stream));
     inf_window_kernel<<<1, 1024, 0, ctx->stream>>>((const uint16_t*)ctx->d_sym.p, (const uint64_t*)ctx->d_off.p, (const uint64_t*)ctx->d_cnt64.p, nreal, (uint8_t*)ctx->d_win.p);
     CK(cudaGetLastError());
@@ -763,13 +771,13 @@ uint64_t inflate_round(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t c
     }
     // the window the next round starts from: the last 32 KB of (previous window, this round's output)
     if (!next.eos) {
-      ensure(ctx->d_infwin, kInfWindow);
-      ensure(ctx->d_infwin2, kInfWindow);
-      if (total >= kInfWindow) CK(cudaMemcpyAsync(ctx->d_infwin.p, dst + total - kInfWindow, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
+      ensure(st.win, kInfWindow);
+      ensure(st.win2, kInfWindow);
+      if (total >= kInfWindow) CK(cudaMemcpyAsync(st.win.p, dst + total - kInfWindow, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
       else if (total) {
-        CK(cudaMemcpyAsync(ctx->d_infwin2.p, (uint8_t*)ctx->d_win.p + total, kInfWindow - total, cudaMemcpyDeviceToDevice, ctx->stream));
-        CK(cudaMemcpyAsync((uint8_t*)ctx->d_infwin2.p + kInfWindow - total, dst, total, cudaMemcpyDeviceToDevice, ctx->stream));
-        std::swap(ctx->d_infwin, ctx->d_infwin2);
+        CK(cudaMemcpyAsync(st.win2.p, (uint8_t*)ctx->d_win.p + total, kInfWindow - total, cudaMemcpyDeviceToDevice, ctx->stream));
+        CK(cudaMemcpyAsync((uint8_t*)st.win2.p + kInfWindow - total, dst, total, cudaMemcpyDeviceToDevice, ctx->stream));
+        std::swap(st.win, st.win2);
       }
       if (total) st.have_window = true;
     }
@@ -821,84 +829,194 @@ void count_text(smr_ctx* ctx, const uint8_t* t, uint64_t n, CountState& s) {
 }
 
 // the pending text from [off, n) on, with room for `extra` more bytes after n
-void compact_pending(smr_ctx* ctx, ReadStream& rs, uint64_t extra) {
-  const uint64_t live = rs.n - rs.off;
-  if (rs.off == 0 && rs.text.p && rs.text.cap >= rs.n + extra + 64) return;
+void compact_pending(smr_ctx* ctx, StreamSide& sd, uint64_t extra) {
+  const uint64_t live = sd.n - sd.off;
+  if (sd.off == 0 && sd.text.p && sd.text.cap >= sd.n + extra + 64) return;
   DevBuf nb;
   const uint64_t want = live + extra + 64;
   CK(nb.alloc(want + want / 8 + 256));
-  if (live) CK(cudaMemcpyAsync(nb.p, (uint8_t*)rs.text.p + rs.off, live, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (live) CK(cudaMemcpyAsync(nb.p, (uint8_t*)sd.text.p + sd.off, live, cudaMemcpyDeviceToDevice, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  rs.text = std::move(nb);
-  rs.off = 0; rs.n = live;
+  sd.text = std::move(nb);
+  sd.off = 0; sd.n = live;
 }
 
-// new text at [from, rs.n): the file's first byte, the count pass; a count-only stream keeps none of it
-void took_text(smr_ctx* ctx, ReadStream& rs, uint64_t from) {
-  const uint8_t* t = (const uint8_t*)rs.text.p;
-  if (rs.n > from && !rs.have_first) {
-    CK(cudaMemcpyAsync(&rs.first, t + from, 1, cudaMemcpyDeviceToHost, ctx->stream));
+// new text at [from, sd.n): the file's first byte, the count pass; a count-only stream keeps none of it.  A mate stream counts
+// nothing (the reference counts the mate files one after another: SMR_STREAM_NEXT_FILE) and checks that both mates are one format.
+void took_text(smr_ctx* ctx, ReadStream& rs, StreamSide& sd, uint64_t from) {
+  const uint8_t* t = (const uint8_t*)sd.text.p;
+  if (sd.n > from && !sd.have_first) {
+    CK(cudaMemcpyAsync(&sd.first, t + from, 1, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    rs.have_first = true;
-    if (!rs.counts.period) rs.counts.period = rs.first == '@' ? 4 : 2;   // the line cycle of a run's first file holds for all
+    sd.have_first = true;
+    if (!rs.counts.period) rs.counts.period = sd.first == '@' ? 4 : 2;   // the line cycle of a run's first file holds for all
   }
-  count_text(ctx, t + from, rs.n - from, rs.counts);
-  if (rs.count_only) rs.off = rs.n = 0;
-}
-
-void stream_push_impl(smr_ctx* ctx, const uint8_t* bytes, uint64_t n, bool eof) {
-  ReadStream& rs = ctx->rs;
-  if (!rs.open) fail(SMR_ERR_ARG, "no open read stream: call smr_stream_begin");
-  if (rs.eof) fail(SMR_ERR_ARG, "read stream: the file has ended (eof was pushed)");
-  rs.eof = eof;
-  if (!rs.gz) {
-    compact_pending(ctx, rs, n);
-    if (n) CK(cudaMemcpyAsync((uint8_t*)rs.text.p + rs.n, bytes, n, cudaMemcpyHostToDevice, ctx->stream));
-    const uint64_t from = rs.n;
-    rs.n += n;
-    took_text(ctx, rs, from);
+  if (rs.mates) {
+    const StreamSide& m1 = rs.side[0];
+    const StreamSide& m2 = rs.side[1];
+    if (m1.have_first && m2.have_first && (m1.first == '@') != (m2.first == '@'))
+      fail(SMR_ERR_ARG, std::string("mate stream: mate 1 is ") + (m1.first == '@' ? "FASTQ" : "FASTA") + " and mate 2 is " + (m2.first == '@' ? "FASTQ" : "FASTA"));
     return;
   }
-  rs.tail.insert(rs.tail.end(), bytes, bytes + n);
-  if (rs.inf.at.eos) { rs.tail.clear(); return; }   // bytes after the gzip stream are ignored
-  rs.pushed += n;
-  if (eof && rs.pushed < 18) fail(SMR_ERR_ARG, "gz input: shorter than a gzip header and trailer");
-  if (rs.tail.empty() && !eof) return;
-  compact_pending(ctx, rs, 0);
-  const uint64_t nb = rs.tail.size();
-  const uint64_t chunk = std::min<uint64_t>(65536, std::max<uint64_t>(8192, nb / 8192));   // as smr_upload_fastx_gz
-  const uint64_t from = rs.n;
-  rs.n += inflate_round(ctx, rs.tail.data(), nb, chunk, eof, rs.inf, rs.text, rs.n);
-  if (rs.inf.at.eos) rs.tail.clear();
-  else {
-    const uint64_t drop = rs.inf.at.bit / 8;
-    rs.tail.erase(rs.tail.begin(), rs.tail.begin() + drop);
-    rs.inf.at.bit -= drop * 8;
-  }
-  took_text(ctx, rs, from);
+  count_text(ctx, t + from, sd.n - from, rs.counts);
+  if (rs.count_only) sd.off = sd.n = 0;
 }
 
-// where the next batch ends in the pending text (bytes from rs.off), or 0 when more text must be pushed first
+// the next piece of file `mate` (0 for a single stream, 0 / 1 for mates 1 / 2)
+void stream_push_impl(smr_ctx* ctx, uint32_t mate, const uint8_t* bytes, uint64_t n, bool eof) {
+  ReadStream& rs = ctx->rs;
+  if (!rs.open) fail(SMR_ERR_ARG, "no open read stream: call smr_stream_begin");
+  StreamSide& sd = rs.side[mate];
+  if (sd.eof) fail(SMR_ERR_ARG, rs.mates ? "mate stream: mate " + std::to_string(mate + 1) + " has ended (eof was pushed)" : "read stream: the file has ended (eof was pushed)");
+  sd.eof = eof;
+  if (!rs.gz) {
+    compact_pending(ctx, sd, n);
+    if (n) CK(cudaMemcpyAsync((uint8_t*)sd.text.p + sd.n, bytes, n, cudaMemcpyHostToDevice, ctx->stream));
+    const uint64_t from = sd.n;
+    sd.n += n;
+    took_text(ctx, rs, sd, from);
+    return;
+  }
+  sd.tail.insert(sd.tail.end(), bytes, bytes + n);
+  if (sd.inf.at.eos) { sd.tail.clear(); return; }   // bytes after the gzip stream are ignored
+  sd.pushed += n;
+  const std::string who = rs.mates ? "mate " + std::to_string(mate + 1) + ": " : "";
+  if (eof && sd.pushed < 18) fail(SMR_ERR_ARG, who + "gz input: shorter than a gzip header and trailer");
+  if (sd.tail.empty() && !eof) return;
+  compact_pending(ctx, sd, 0);
+  const uint64_t nb = sd.tail.size();
+  const uint64_t chunk = std::min<uint64_t>(65536, std::max<uint64_t>(8192, nb / 8192));   // as smr_upload_fastx_gz
+  const uint64_t from = sd.n;
+  try {
+    sd.n += inflate_round(ctx, sd.tail.data(), nb, chunk, eof, sd.inf, sd.text, sd.n);
+  } catch (Failure& f) {
+    f.msg = who + f.msg;
+    throw;
+  }
+  if (sd.inf.at.eos) sd.tail.clear();
+  else {
+    const uint64_t drop = sd.inf.at.bit / 8;
+    sd.tail.erase(sd.tail.begin(), sd.tail.begin() + drop);
+    sd.inf.at.bit -= drop * 8;
+  }
+  took_text(ctx, rs, sd, from);
+}
+
+// where the next batch ends in the pending text (bytes from sd.off), or 0 when more text must be pushed first
 uint64_t stream_cut(smr_ctx* ctx, ReadStream& rs) {
-  const uint64_t avail = rs.n - rs.off, limit = rs.batch_bytes;
+  StreamSide& sd = rs.side[0];
+  const uint64_t avail = sd.n - sd.off, limit = rs.batch_bytes;
   if (avail == 0) return 0;
-  if (avail <= limit) return rs.eof ? avail : 0;   // a batch takes whole records up to batch_bytes: wait for more text
-  const uint8_t* t = (const uint8_t*)rs.text.p + rs.off;
+  if (avail <= limit) return sd.eof ? avail : 0;   // a batch takes whole records up to batch_bytes: wait for more text
+  const uint8_t* t = (const uint8_t*)sd.text.p + sd.off;
   unsigned long long* cut = ensure<unsigned long long>(ctx->d_cut, 16);
   uint64_t w = std::min(avail, limit + 1);   // a record end at <= limit is a '\n' before it or a header line starting at it
   for (;;) {
     const uint32_t nl = newline_index(ctx, t, w);
     const unsigned long long init[2] = {0ull, ~0ull};
     CK(cudaMemcpyAsync(cut, init, 16, cudaMemcpyHostToDevice, ctx->stream));
-    stream_cut_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(t, (const uint64_t*)ctx->d_nl.p, nl, w, limit, rs.first == '@' ? kFmtFastq : kFmtFasta, cut);
+    stream_cut_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(t, (const uint64_t*)ctx->d_nl.p, nl, w, limit, sd.first == '@' ? kFmtFastq : kFmtFasta, cut);
     CK(cudaGetLastError());
     unsigned long long h[2];
     CK(cudaMemcpyAsync(h, cut, 16, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     if (h[0]) return h[0];
     if (h[1] != ~0ull) return h[1];   // the first record is longer than a batch: it is the batch
-    if (w == avail) return rs.eof ? avail : 0;
+    if (w == avail) return sd.eof ? avail : 0;
     w = std::min(avail, 2 * w);
+  }
+}
+
+// The record ends of mate m's pending text in its first w bytes, in bytes from its off, to ctx->d_mend[m]; returns their number.
+// Once the file has ended and w covers its text, its last record ends at the end of the text, one byte further when the text
+// does not end in '\n' (the interleave appends one).
+uint32_t mate_ends(smr_ctx* ctx, StreamSide& sd, uint32_t m, uint64_t w) {
+  const uint64_t avail = sd.n - sd.off;
+  if (avail == 0) return 0;
+  const uint8_t* t = (const uint8_t*)sd.text.p + sd.off;
+  const uint32_t fmt = sd.first == '@' ? kFmtFastq : kFmtFasta;
+  const uint32_t nl = newline_index(ctx, t, w);
+  uint32_t* flag = ensure<uint32_t>(ctx->d_mflag, ((size_t)nl + 1) * 4);
+  uint64_t* ends = ensure<uint64_t>(ctx->d_mend[m], ((size_t)nl + 2) * 8);
+  const int grid = ctx->sm_count * 8;
+  const uint64_t* d_nl = (const uint64_t*)ctx->d_nl.p;
+  if (nl) record_end_flags_kernel<<<grid, 256, 0, ctx->stream>>>(t, d_nl, nl, w, fmt, flag);
+  CK(cudaMemsetAsync(flag + nl, 0, 4, ctx->stream));
+  exclusive_sum(ctx, flag, flag, nl + 1);
+  uint32_t cnt = 0;
+  CK(cudaMemcpyAsync(&cnt, flag + nl, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (cnt) record_end_list_kernel<<<grid, 256, 0, ctx->stream>>>(t, d_nl, nl, w, fmt, flag, ends);
+  CK(cudaGetLastError());
+  if (sd.eof && w == avail) {
+    uint64_t last = 0;
+    uint8_t c = 0;
+    if (cnt) CK(cudaMemcpyAsync(&last, ends + cnt - 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(&c, t + avail - 1, 1, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    if (last < avail) {
+      const uint64_t e = avail + (c != '\n');
+      CK(cudaMemcpyAsync(ends + cnt, &e, 8, cudaMemcpyHostToDevice, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));
+      ++cnt;
+    }
+  }
+  return cnt;
+}
+
+// The next batch of a mate stream: the k whole pairs whose interleaved text fits in batch_bytes (or the first pair alone when it
+// does not fit), interleaved into ctx->d_text.  Returns k; 0 = push more, or (*done) both files are exhausted.  Before both files
+// have ended, pairs that fit wait for more text, so that every batch but the last is full.
+uint32_t mate_cut(smr_ctx* ctx, ReadStream& rs, uint64_t* nbytes, int* done) {
+  StreamSide* sd = rs.side;
+  const uint64_t limit = rs.batch_bytes;
+  const uint64_t avail[2] = {sd[0].n - sd[0].off, sd[1].n - sd[1].off};
+  uint64_t w[2] = {std::min(avail[0], limit + 1), std::min(avail[1], limit + 1)};
+  unsigned long long* dk = ensure<unsigned long long>(ctx->d_cut, 16);
+  for (;;) {
+    uint32_t n[2];
+    bool closed[2];   // no more record ends can join the listed ones within batch_bytes: beyond the window, or the file ended
+    for (uint32_t m = 0; m < 2; ++m) { n[m] = mate_ends(ctx, sd[m], m, w[m]); closed[m] = w[m] < avail[m] || sd[m].eof; }
+    const uint64_t* ea = (const uint64_t*)ctx->d_mend[0].p;
+    const uint64_t* eb = (const uint64_t*)ctx->d_mend[1].p;
+    const uint32_t both = std::min(n[0], n[1]);
+    if (both) {
+      CK(cudaMemsetAsync(dk, 0, 8, ctx->stream));
+      mate_fit_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(ea, eb, both, limit, dk);
+      CK(cudaGetLastError());
+      unsigned long long fit = 0;
+      CK(cudaMemcpyAsync(&fit, dk, 8, cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));
+      uint32_t k = (uint32_t)fit;
+      if (k == 0) k = 1;   // the first pair is longer than a batch: it is the batch
+      else if (k == both && !(n[0] == k && closed[0]) && !(n[1] == k && closed[1])) return 0;   // pair k + 1 may still fit
+      uint64_t end[2];
+      CK(cudaMemcpyAsync(&end[0], ea + k - 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaMemcpyAsync(&end[1], eb + k - 1, 8, cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaStreamSynchronize(ctx->stream));
+      *nbytes = end[0] + end[1];
+      if (*nbytes >= 0xF0000000ull) fail(SMR_ERR_ARG, "mate stream: one pair of 2^32 bytes or more");
+      ensure(ctx->d_text, *nbytes + 64);
+      mate_interleave_kernel<<<std::max(1u, std::min<uint32_t>(ctx->sm_count * 16, (k + 7) / 8)), 256, 0, ctx->stream>>>(
+          (const uint8_t*)sd[0].text.p + sd[0].off, avail[0], ea, (const uint8_t*)sd[1].text.p + sd[1].off, avail[1], eb, k, (uint8_t*)ctx->d_text.p);
+      CK(cudaGetLastError());
+      for (uint32_t m = 0; m < 2; ++m) sd[m].off += std::min(end[m], avail[m]);
+      return k;
+    }
+    // a mate without a whole record in its window: it has ended, waits for more text, or its first record is longer than the window
+    const bool gone[2] = {sd[0].eof && avail[0] == 0, sd[1].eof && avail[1] == 0};
+    if (gone[0] && gone[1]) { *done = 1; return 0; }
+    for (uint32_t m = 0; m < 2; ++m)
+      if (gone[m] && avail[m ^ 1])
+        fail(SMR_ERR_ARG, "mate stream: mate " + std::to_string(m + 1) + " has ended while mate " + std::to_string(2 - m) +
+                              " holds more records (the mate files differ in record count)");
+    bool grow = false, wait = false;
+    for (uint32_t m = 0; m < 2; ++m) {
+      if (n[m]) continue;
+      if (w[m] < avail[m]) { w[m] = std::min(avail[m], 2 * w[m]); grow = true; }
+      else wait = true;
+    }
+    if (wait || !grow) return 0;
   }
 }
 
@@ -906,17 +1024,27 @@ uint32_t stream_next_impl(smr_ctx* ctx, int* done) {
   ReadStream& rs = ctx->rs;
   if (!rs.open) fail(SMR_ERR_ARG, "no open read stream: call smr_stream_begin");
   if (rs.count_only) fail(SMR_ERR_ARG, "read stream opened with SMR_STREAM_COUNT_ONLY: it makes no batches");
+  if (rs.mates) {
+    uint64_t nbytes = 0;
+    const uint32_t k = mate_cut(ctx, rs, &nbytes, done);
+    if (k == 0) return 0;
+    const uint32_t nreads = upload_fastx_impl(ctx, nullptr, nbytes, rs.side[0].first);
+    if (nreads != 2 * k) fail(SMR_ERR_ARG, "mate stream: " + std::to_string(k) + " pairs decoded to " + std::to_string(nreads) + " records");
+    ctx->resident_mates = true;
+    return nreads;
+  }
+  StreamSide& sd = rs.side[0];
   for (;;) {
-    *done = rs.eof && rs.n == rs.off;
+    *done = sd.eof && sd.n == sd.off;
     const uint64_t cut = stream_cut(ctx, rs);
     if (cut == 0) return 0;
     if (cut >= 0xF0000000ull) fail(SMR_ERR_ARG, "read stream: one record of 2^32 bytes or more");
     ensure(ctx->d_text, cut + 64);
-    CK(cudaMemcpyAsync(ctx->d_text.p, (const uint8_t*)rs.text.p + rs.off, cut, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaMemcpyAsync(ctx->d_text.p, (const uint8_t*)sd.text.p + sd.off, cut, cudaMemcpyDeviceToDevice, ctx->stream));
     char c0 = 0;
-    CK(cudaMemcpyAsync(&c0, (const uint8_t*)rs.text.p + rs.off, 1, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(&c0, (const uint8_t*)sd.text.p + sd.off, 1, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    rs.off += cut;
+    sd.off += cut;
     const uint32_t nreads = upload_fastx_impl(ctx, nullptr, cut, c0);
     if (nreads) { *done = 0; return nreads; }
   }
@@ -1370,11 +1498,15 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
 void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
                          const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
                          char* out, uint64_t cap, uint64_t* so_out, bool gz) {
-  if (o->out2 || o->sout) fail(SMR_ERR_UNSUPPORTED, "-out2 / -sout: the report writer writes one aligned and one other file");
+  const bool mates = o->mates || (!text && ctx->resident_mates);   // the resident batch of a mate stream is mates
+  const bool paired = o->paired_in || o->paired_out || mates;
+  if ((o->out2 || o->sout) && !paired) fail(SMR_ERR_UNSUPPORTED, "-out2 / -sout: only a paired batch (mates, paired_in or paired_out) has mates to split");
   if (o->blast && o->blast_format != 1) fail(SMR_ERR_UNSUPPORTED, "only tabular BLAST (-blast 1) is written on the device");
   if (o->paired_in && o->paired_out) fail(SMR_ERR_ARG, "paired_in and paired_out are exclusive");
-  const bool paired = o->paired_in || o->paired_out;
+  if (o->sout && (o->paired_in || o->paired_out)) fail(SMR_ERR_ARG, "-sout cannot be used with paired_in or paired_out");
   if (paired && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
+  const uint32_t num_out = o->out2 && o->sout ? 4 : o->out2 || o->sout ? 2 : 1;   // ReportFxBase::set_num_out
+  const uint32_t nfx = 3 * num_out;                                                // aligned, other, denovo: num_out files each
   if ((o->sam || o->blast || o->denovo) && nreads && !stats) fail(SMR_ERR_ARG, "SAM, BLAST and denovo need the smr_aln_stats of the batch");
   if (nreads && (!results || !alns)) fail(SMR_ERR_ARG, ctx->err);   // a null array: no text of its own, the last one stays
   uint32_t ncols = 0, cols[4] = {0, 0, 0, 0};
@@ -1384,7 +1516,7 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
       cols[ncols] = (uint32_t)o->blast_cols[ncols];
     }
   const std::vector<const Part*> gp = report_groups(ctx);
-  const uint32_t G = (uint32_t)gp.size(), nso = 2 * G + 4;
+  const uint32_t G = (uint32_t)gp.size(), nso = 2 * G + nfx + 1;
   std::vector<RptGroup> hg(G);
   for (uint32_t g = 0; g < G; ++g) {
     const Part& pt = *gp[g];
@@ -1416,16 +1548,17 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   uint64_t* off = ensure<uint64_t>(ctx->r_off, (N + 1) * 8);
   uint64_t* bsz = ensure<uint64_t>(ctx->r_bsz, (N + 1) * 8);
   uint64_t* boff = ensure<uint64_t>(ctx->r_boff, (N + 1) * 8);
-  uint64_t* fxsz = ensure<uint64_t>(ctx->r_fxsz, 3 * fstride * 8);
-  uint64_t* fxoff = ensure<uint64_t>(ctx->r_fxoff, 3 * fstride * 8);
+  uint64_t* fxsz = ensure<uint64_t>(ctx->r_fxsz, nfx * fstride * 8);
+  uint64_t* fxoff = ensure<uint64_t>(ctx->r_fxoff, nfx * fstride * 8);
   uint64_t* so = ensure<uint64_t>(ctx->r_so, (size_t)nso * 8);
   for (int k = 0; k < 4; ++k) a.cols[k] = cols[k];
   a.ncols = ncols; a.min_id = o->min_id; a.min_cov = o->min_cov;
-  a.paired_in = o->paired_in != 0; a.paired_out = o->paired_out != 0; a.denovo = o->denovo != 0;
+  a.paired_in = o->paired_in != 0; a.paired_out = o->paired_out != 0; a.mates = mates; a.denovo = o->denovo != 0;
+  a.out2 = o->out2 != 0; a.num_out = num_out;
   a.fx_mask = (o->fastx ? kRptAligned : 0u) | (o->other ? kRptOther : 0u) | (o->denovo ? kRptDenovo : 0u);
   CK(cudaMemsetAsync(sz, 0, (N + 1) * 8, ctx->stream));
   CK(cudaMemsetAsync(bsz, 0, (N + 1) * 8, ctx->stream));
-  CK(cudaMemsetAsync(fxsz, 0, 3 * fstride * 8, ctx->stream));
+  CK(cudaMemsetAsync(fxsz, 0, nfx * fstride * 8, ctx->stream));
   CK(cudaMemsetAsync(first, 0, ((size_t)G + 1) * 8, ctx->stream));
   if (nreads) {
     rpt_route_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags);
@@ -1444,13 +1577,13 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
     }
     cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, sz, off, (int)(N + 1), ctx->stream); });
     cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, bsz, boff, (int)(N + 1), ctx->stream); });
-    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fxsz, fxoff, (int)(3 * fstride), ctx->stream); });
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fxsz, fxoff, (int)(nfx * fstride), ctx->stream); });
   } else {
     CK(cudaMemsetAsync(off, 0, 8, ctx->stream));
     CK(cudaMemsetAsync(boff, 0, 8, ctx->stream));
-    CK(cudaMemsetAsync(fxoff, 0, 3 * fstride * 8, ctx->stream));
+    CK(cudaMemsetAsync(fxoff, 0, nfx * fstride * 8, ctx->stream));
   }
-  rpt_stream_off_kernel<<<1, 32, 0, ctx->stream>>>(first, G, off, boff, fxoff, nreads, fstride, so);
+  rpt_stream_off_kernel<<<1, 32, 0, ctx->stream>>>(first, G, off, boff, fxoff, nreads, fstride, nfx, so);
   CK(cudaGetLastError());
   std::vector<uint64_t> hso(nso);
   CK(cudaMemcpyAsync(hso.data(), so, (size_t)nso * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1554,6 +1687,7 @@ uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr
   auto& U = ctx->otu;
   otu_open(ctx);
   if (nreads && (!results || !alns || !stats)) fail(SMR_ERR_ARG, "the OTU map needs the results, alignments and smr_aln_stats of the batch");
+  if (!text && ctx->resident_mates) fail(SMR_ERR_UNSUPPORTED, "the OTU map of two mate files (a mate stream's batch) is not written on the device");
   const uint32_t slots = slots_of(ctx);
   const uint64_t N = (uint64_t)nreads * slots;
   if (N >= (1ull << 31)) fail(SMR_ERR_ARG, "batch too large for the OTU map: split it");
@@ -1912,11 +2046,13 @@ int smr_stream_begin(smr_ctx* ctx, uint32_t flags, uint64_t batch_bytes) try {
   CK(cudaSetDevice(ctx->device));
   const CountState before = ctx->rs.counts;
   ctx->rs = ReadStream{};
-  if (flags & ~(uint32_t)(SMR_STREAM_GZ | SMR_STREAM_COUNT_ONLY | SMR_STREAM_NEXT_FILE)) fail(SMR_ERR_ARG, "smr_stream_begin: unknown flags");
+  if (flags & ~(uint32_t)(SMR_STREAM_GZ | SMR_STREAM_COUNT_ONLY | SMR_STREAM_NEXT_FILE | SMR_STREAM_MATES)) fail(SMR_ERR_ARG, "smr_stream_begin: unknown flags");
+  if ((flags & SMR_STREAM_MATES) && (flags & (SMR_STREAM_COUNT_ONLY | SMR_STREAM_NEXT_FILE)))
+    fail(SMR_ERR_ARG, "smr_stream_begin: a mate stream makes batches and counts nothing: count mate files one after another (SMR_STREAM_NEXT_FILE)");
   if (flags & SMR_STREAM_NEXT_FILE) ctx->rs.counts = rc_next_file(before, flags & SMR_STREAM_GZ);
   if (!(flags & SMR_STREAM_COUNT_ONLY) && (batch_bytes == 0 || batch_bytes >= 0xF0000000ull)) fail(SMR_ERR_ARG, "smr_stream_begin: batch_bytes must be in [1, 0xF0000000)");
   ReadStream& rs = ctx->rs;
-  rs.gz = flags & SMR_STREAM_GZ; rs.count_only = flags & SMR_STREAM_COUNT_ONLY; rs.batch_bytes = batch_bytes;
+  rs.gz = flags & SMR_STREAM_GZ; rs.count_only = flags & SMR_STREAM_COUNT_ONLY; rs.mates = flags & SMR_STREAM_MATES; rs.batch_bytes = batch_bytes;
   rs.open = true;
   return SMR_OK;
 } SMR_CATCH(ctx)
@@ -1925,9 +2061,24 @@ int smr_stream_push(smr_ctx* ctx, const void* bytes, uint64_t n, int eof) try {
   if (!ctx || (!bytes && n)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   try {
-    stream_push_impl(ctx, (const uint8_t*)bytes, n, eof != 0);
+    if (ctx->rs.mates) fail(SMR_ERR_ARG, "smr_stream_push on a mate stream: push each mate with smr_stream_push_mate");
+    stream_push_impl(ctx, 0, (const uint8_t*)bytes, n, eof != 0);
   } catch (...) {
     ctx->rs = ReadStream{};   // a stream that failed is closed
+    throw;
+  }
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_stream_push_mate(smr_ctx* ctx, uint32_t mate, const void* bytes, uint64_t n, int eof) try {
+  if (!ctx || (!bytes && n)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  try {
+    if (!ctx->rs.mates) fail(SMR_ERR_ARG, "smr_stream_push_mate on a stream not opened with SMR_STREAM_MATES");
+    if (mate != 1 && mate != 2) fail(SMR_ERR_ARG, "smr_stream_push_mate: mate must be 1 or 2");
+    stream_push_impl(ctx, mate - 1, (const uint8_t*)bytes, n, eof != 0);
+  } catch (...) {
+    ctx->rs = ReadStream{};
     throw;
   }
   return SMR_OK;

@@ -40,7 +40,9 @@ struct RptGroup {
   uint32_t nref, index_num, part, pad;
 };
 
-enum : uint32_t { kRptAligned = 1, kRptOther = 2, kRptDenovo = 4, kRptSkip = 8 };
+// route flags of a read: the read files it goes to, and for each of them (kind s = 0 aligned, 1 other, 2 denovo) the file among the
+// kind's num_out in 2 bits from kRptFileShift + 2 * s
+enum : uint32_t { kRptAligned = 1, kRptOther = 2, kRptDenovo = 4, kRptSkip = 8, kRptFileShift = 8 };
 enum : uint32_t { kRptErrLen = 1, kRptErrGroup = 2, kRptErrRef = 4, kRptErrQual = 8, kRptErrCigar = 16 };
 enum : uint32_t { kColCigar = 1, kColQcov = 2, kColQstrand = 3 };
 
@@ -53,6 +55,8 @@ struct RptArgs {
   uint32_t cols[4], ncols;
   double min_id, min_cov;
   uint32_t paired_in, paired_out, denovo;
+  uint32_t mates;     // records 2k and 2k+1 are mates from two files
+  uint32_t out2, num_out;   // -out2; files per kind of read file: 1, 2 (-out2 or -sout) or 4 (both)
   uint32_t fx_mask;   // the read files asked for (kRptAligned | kRptOther | kRptDenovo)
   uint32_t* err;
 };
@@ -147,27 +151,68 @@ __device__ bool rpt_is_denovo(const RptArgs& a, uint32_t r) {   // denovo_stats_
   return true;
 }
 
+// The file of mate i (0 / 1) of a pair among the num_out of its kind, -1 = not written; h / hm: this read / its mate aligned;
+// d / dm: denovo.  Restatements of the paired branches at -threads 1 (id 0); num_out 4 means -out2 and -sout, which exclude
+// paired_in / paired_out (ReportFxBase::validate_out_type).
+//   aligned  ReportFastx::append (report_fastx.cpp:71-133)
+__device__ int rpt_file_aligned(const RptArgs& a, uint32_t i, bool h, bool hm) {
+  const bool both = h && hm;
+  if (!h && !hm) return -1;
+  if (a.num_out == 1) return (a.paired_out ? both : (a.paired_in || h)) ? 0 : -1;
+  if (a.num_out == 2 && a.out2) return (a.paired_out ? both : (a.paired_in || h)) ? (int)i : -1;   // paired_out: 'break' when not both
+  if (a.num_out == 2) return both ? 0 : h ? 1 : -1;                                               // -sout: paired, singleton
+  return both ? (int)i : h ? (int)i + 2 : -1;
+}
+//   other    ReportFxOther::append (report_fx_other.cpp:52-113)
+__device__ int rpt_file_other(const RptArgs& a, uint32_t i, bool h, bool hm) {
+  const bool any = h || hm;
+  if (h && hm) return -1;
+  if (a.num_out == 1) return (a.paired_in ? !any : (a.paired_out || !h)) ? 0 : -1;
+  if (a.num_out == 2 && a.out2) return (a.paired_in ? !any : (a.paired_out || !h)) ? (int)i : -1;   // paired_in: 'break' when any
+  if (a.num_out == 2) return !any ? 0 : !h ? 1 : -1;
+  return !any ? (int)i : !h ? (int)i + 2 : -1;
+}
+//   denovo   ReportDenovo::append (report_denovo.cpp:59-124), called when d || dm (output.cpp:133-142).  Its idx is set in the for
+//   header only: under -out2 without paired_in / paired_out a mate that is not denovo falls through to the write with the idx of
+//   the previous iteration, which is 0 (the _fwd file) for both mates.  Reproduced.
+__device__ int rpt_file_denovo(const RptArgs& a, uint32_t i, bool d, bool dm) {
+  const bool both = d && dm;
+  if (a.num_out == 1) return (a.paired_in || d) ? 0 : -1;
+  if (a.num_out == 2 && a.out2) {
+    if (a.paired_out && !both) return -1;
+    return a.paired_in || d ? (int)i : 0;
+  }
+  if (a.num_out == 2) return both ? 0 : d ? 1 : -1;
+  return both ? (int)i : d ? (int)i + 2 : -1;
+}
+
 __global__ void rpt_route_kernel(RptArgs a, uint32_t* __restrict__ flags) {
-  const bool paired = a.paired_in || a.paired_out;
+  const bool paired = a.paired_in || a.paired_out || a.mates;
   for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.nreads; r += gridDim.x * blockDim.x) {
     const uint32_t m = paired ? (r ^ 1u) : r;
     const bool empty = a.rec[paired ? (r | 1u) : r].seq_len == 0;   // Readfeed pairs: only the second read is checked (output.cpp:120)
     if (empty) { flags[r] = kRptSkip; continue; }
-    const bool h = a.res[r].is_hit, hm = a.res[m].is_hit;
+    const bool h = a.res[r].is_hit;
     uint32_t f = 0;
+    int file[3] = {-1, -1, -1};
     if (!paired) {
-      f |= h ? kRptAligned : kRptOther;
+      file[h ? 0 : 1] = 0;
     } else {
-      const bool h0 = (r & 1u) ? hm : h, h1 = (r & 1u) ? h : hm;
-      if (a.paired_out ? (h0 && h1) : (h0 || h1)) f |= kRptAligned;
-      if (!(h0 && h1) && (a.paired_out || !(h0 || h1))) f |= kRptOther;
+      const bool hm = a.res[m].is_hit;
+      file[0] = rpt_file_aligned(a, r & 1u, h, hm);
+      file[1] = rpt_file_other(a, r & 1u, h, hm);
     }
     if (a.denovo) {
       const bool d = rpt_is_denovo(a, r);
-      if (!paired) { if (d) f |= kRptDenovo; }
-      else if ((d || rpt_is_denovo(a, m)) && (a.paired_in || d)) f |= kRptDenovo;
+      if (!paired) { if (d) file[2] = 0; }
+      else {
+        const bool dm = rpt_is_denovo(a, m);
+        if (d || dm) file[2] = rpt_file_denovo(a, r & 1u, d, dm);
+      }
     }
-    flags[r] = f & a.fx_mask;
+    for (uint32_t s = 0; s < 3; ++s)
+      if (file[s] >= 0 && (a.fx_mask & (1u << s))) f |= (1u << s) | ((uint32_t)file[s] << (kRptFileShift + 2 * s));
+    flags[r] = f;
   }
 }
 
@@ -341,14 +386,16 @@ __global__ void rpt_blast_kernel(RptArgs a, const uint32_t* __restrict__ rows, c
 }
 
 // ---- aligned / other / aligned_denovo reads: write_a_read (report_fx_base.cpp:176-181) ----
+// the stream of kind s of a read with route flags f: the kinds one after another, num_out files each, in the reference's file order
+__device__ __forceinline__ uint32_t rpt_fx_stream(const RptArgs& a, uint32_t f, uint32_t s) { return s * a.num_out + ((f >> (kRptFileShift + 2 * s)) & 3u); }
+
 __global__ void rpt_fx_size_kernel(RptArgs a, const uint32_t* __restrict__ flags, uint64_t* __restrict__ size, uint64_t stride) {
   for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < a.nreads; r += gridDim.x * blockDim.x) {
     const RptRec& rc = a.rec[r];
     const uint64_t len = (uint64_t)rc.hdr_len + rc.seq_len + 2 + (a.fastq ? rc.qual_len + 3 : 0);
     const uint32_t f = flags[r];
-    size[r] = f & kRptAligned ? len : 0;   // route masked the files not asked for
-    size[stride + r] = f & kRptOther ? len : 0;
-    size[2 * stride + r] = f & kRptDenovo ? len : 0;
+    for (uint32_t s = 0; s < 3; ++s)   // route masked the files not asked for; the sizes are zeroed before
+      if (f & (1u << s)) size[rpt_fx_stream(a, f, s) * stride + r] = len;
   }
 }
 
@@ -356,8 +403,8 @@ __device__ __forceinline__ void rpt_warp_copy(char* dst, const uint8_t* src, uin
   for (uint64_t k = lane; k < n; k += 32) dst[k] = (char)src[k];
 }
 
-// off: one exclusive scan over the sizes of the three files (stride nreads + 1), so off already includes the files before; *base = start of
-// the first read file in the output
+// off: one exclusive scan over the sizes of the read files (stride nreads + 1), so off already includes the files before; *base = start
+// of the first read file in the output
 __global__ void __launch_bounds__(256) rpt_fx_write_kernel(RptArgs a, const uint32_t* __restrict__ flags, const uint64_t* __restrict__ off,
                                                            uint64_t stride, const uint64_t* __restrict__ base, char* __restrict__ out) {
   const unsigned lane = lane_id();
@@ -366,7 +413,7 @@ __global__ void __launch_bounds__(256) rpt_fx_write_kernel(RptArgs a, const uint
     const RptRec rc = a.rec[r];
     for (uint32_t s = 0; s < 3; ++s) {
       if (!(f & (1u << s))) continue;
-      char* dst = out + base[0] + off[s * stride + r];
+      char* dst = out + base[0] + off[rpt_fx_stream(a, f, s) * stride + r];
       if (rc.verbatim) { rpt_warp_copy(dst, a.text + rc.hdr, (uint64_t)rc.hdr_len + rc.seq_len + rc.qual_len + 5, lane); continue; }
       rpt_warp_copy(dst, a.text + rc.hdr, rc.hdr_len, lane);
       char* seq = dst + rc.hdr_len + 1;
@@ -378,15 +425,15 @@ __global__ void __launch_bounds__(256) rpt_fx_write_kernel(RptArgs a, const uint
   }
 }
 
-// stream offsets: SAM groups, BLAST groups, aligned, other, denovo (2 * ngroups + 4 entries)
+// stream offsets: SAM groups, BLAST groups, the nfx read files (aligned, other, denovo; num_out files each): 2 * ngroups + nfx + 1 entries
 __global__ void rpt_stream_off_kernel(const uint64_t* __restrict__ first, uint32_t ngroups, const uint64_t* __restrict__ sam_off,
                                       const uint64_t* __restrict__ blast_off, const uint64_t* __restrict__ fx_off, uint32_t nreads, uint64_t stride,
-                                      uint64_t* __restrict__ so) {
+                                      uint32_t nfx, uint64_t* __restrict__ so) {
   if (threadIdx.x != 0 || blockIdx.x != 0) return;
   const uint64_t sam_total = sam_off[first[ngroups]];
   for (uint32_t g = 0; g <= ngroups; ++g) so[g] = sam_off[first[g]];
   for (uint32_t g = 0; g <= ngroups; ++g) so[ngroups + g] = sam_total + blast_off[first[g]];
-  for (uint32_t s = 0; s < 3; ++s) so[2 * ngroups + 1 + s] = so[2 * ngroups] + fx_off[s * stride + nreads];   // fx_off: one scan over the three
+  for (uint32_t s = 0; s < nfx; ++s) so[2 * ngroups + 1 + s] = so[2 * ngroups] + fx_off[s * stride + nreads];   // fx_off: one scan over them all
 }
 
 }  // namespace smr
