@@ -30,7 +30,7 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_build_index_device", "smr_debug_index_array", "smr_set_instrumentation", "smr_set_report_refs", "smr_set_report_scoring",
            "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings",
            "smr_format_reports_gz", "smr_gzip", "smr_stream_begin", "smr_stream_push", "smr_stream_next", "smr_stream_counts",
-           "smr_stream_push_mate"]
+           "smr_stream_push_mate", "smr_format_blast_pairwise", "smr_format_blast_pairwise_gz"]
 
 CNT_NAMES = ("num_aligned", "num_short", "sw_calls", "sw_cells", "windows", "trie_nodes", "buckets",
              "bucket_entries", "pos_entries", "lis_calls", "dbg_max_read_cycles", "dbg_sum_read_cycles", "dbg_lis_kernel_cycles",
@@ -77,7 +77,8 @@ class ReportOpts(C.Structure):
 
 def report_opts(sam=False, blast=None, fastx=False, other=False, denovo=None, paired_in=False, paired_out=False, out2=False, sout=False,
                 mates=False) -> ReportOpts:
-    """blast: None, or the value of the reference's -blast option ('1 cigar qcov qstrand'; '0' = pairwise, refused by the writer);
+    """blast: None, or the value of the reference's -blast option ('1 cigar qcov qstrand'; '0' = pairwise, written by
+    format_blast_pairwise and refused by format_reports);
     denovo: None, or (min_id, min_cov) = the reference's -id / -coverage; mates: records 2k and 2k+1 come from two mate files
     (implied for the resident batch of stream_mates)."""
     o = ReportOpts(sam=int(bool(sam)), fastx=int(bool(fastx)), other=int(bool(other)), paired_in=int(bool(paired_in)),
@@ -589,6 +590,36 @@ class Aligner:
         fx = [f[0] for f in fx] if num_out == 1 else [tuple(f) for f in fx]
         return dict(sam=b[:G], blast=b[G:2 * G], aligned=fx[0], other=fx[1], denovo=fx[2], groups=groups)
 
+    def format_blast_pairwise(self, out: dict, text: bytes | None = None, opts: ReportOpts | None = None, gzip: bool = False, **kw) -> list:
+        """smr_format_blast_pairwise: the pairwise BLAST rows (-blast 0) of one batch, as a list of bytes, one per report_groups() entry.
+        out / text as for format_reports; opts = report_opts(blast="0", ...) or its keyword arguments (blast defaults to "0"; only
+        paired_in / paired_out / mates matter besides).  gzip: smr_format_blast_pairwise_gz, every non-empty stream as one gzip member."""
+        if opts is None:
+            kw.setdefault("blast", "0")
+            opts = report_opts(**kw)
+        self._upload_report_refs()
+        G = len(self.report_groups())
+        res, alns = out["res"], out["alns"]
+        cig = np.ascontiguousarray(out["cigar"], np.uint32)
+        st = out.get("stats")
+        txt = np.frombuffer(text, np.uint8) if text is not None else None
+        so = np.zeros(G + 1, np.uint64)
+        fn = self.L.smr_format_blast_pairwise_gz if gzip else self.L.smr_format_blast_pairwise
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
+                       C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_void_p]
+        args = [self.h, C.cast(C.byref(opts), C.c_void_p), _ptr(txt) if txt is not None and txt.size else None, txt.size if txt is not None else 0,
+                _ptr(res), _ptr(alns), _ptr(cig) if cig.size else None, cig.size, _ptr(st) if st is not None else None, res.shape[0]]
+        buf = getattr(self, "_report_buf", None)
+        if buf is None:
+            buf = np.zeros(1 << 20, np.uint8)
+        rc = fn(*args, _ptr(buf), buf.size, _ptr(so))
+        if rc == 5 and int(so[-1]) > buf.size:   # SMR_ERR_CAPACITY: so names the size; grow and run again
+            buf = np.zeros(int(so[-1]) + (int(so[-1]) >> 3), np.uint8)
+            rc = fn(*args, _ptr(buf), buf.size, _ptr(so))
+        self._check(rc, "smr_format_blast_pairwise_gz" if gzip else "smr_format_blast_pairwise")
+        self._report_buf = buf
+        return [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(G)]
+
     # ---- OTU map (smr_otu_begin / smr_otu_add / smr_otu_finish) ----
     def otu_begin(self, min_id: float = 0.97, min_cov: float = 0.97, paired_in: bool = False, paired_out: bool = False):
         """smr_otu_begin: open (or reset) the OTU map of this context; -id / -coverage as the reference's -otu_map defaults them"""
@@ -686,7 +717,8 @@ class ReportWriter:
     with no member gets one empty member.  otu_map.txt stays plain, as the reference writes it.
     out2 / sout (opts): each read file is split as the reference's -out2 / -sout split it, aligned_fwd.fq / aligned_rev.fq,
     aligned_paired.fq / aligned_singleton.fq, or aligned_paired_fwd.fq ... aligned_singleton_rev.fq with both, and likewise other.*
-    and aligned_denovo.*; batches of stream_mates are mates without further options (mates=True for a batch passed as text)."""
+    and aligned_denovo.*; batches of stream_mates are mates without further options (mates=True for a batch passed as text).
+    blast="0": aligned.blast holds the pairwise rows (format_blast_pairwise); the other files are written as with any other blast."""
 
     def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", otu_map=None, zip_out: bool = False, **opts):
         self.dir, self.al, self.header, self.zip_out = out_dir, aligner, sam_header, zip_out
@@ -709,7 +741,16 @@ class ReportWriter:
         if self.ext is None:
             first = text[:1] if text is not None else self.al.resident_text()[:1]
             self.ext = "fq" if first == b"@" else "fa"
-        s = self.al.format_reports(out, text, opts=self.opts, gzip=self.zip_out)
+        o = self.opts
+        pairwise = bool(o.blast) and o.blast_format == 0
+        if pairwise:   # the other files without BLAST, the BLAST streams from the pairwise writer
+            rest = ReportOpts.from_buffer_copy(o)
+            rest.blast = 0
+            s = self.al.format_reports(out, text, opts=rest, gzip=self.zip_out)
+            po = report_opts(blast="0", paired_in=o.paired_in, paired_out=o.paired_out, mates=o.mates)
+            s["blast"] = self.al.format_blast_pairwise(out, text, opts=po, gzip=self.zip_out)
+        else:
+            s = self.al.format_reports(out, text, opts=o, gzip=self.zip_out)
         for g, (rows_sam, rows_blast) in enumerate(zip(s["sam"], s["blast"])):
             self._append(f"sam_{g}", rows_sam)
             self._append(f"blast_{g}", rows_blast)

@@ -1363,7 +1363,8 @@ void upload_async(smr_ctx* ctx, DevBuf& b, const T* src, size_t n) {
   fail(SMR_ERR_ARG, e & kRptErrLen ? "an alignment's readlen or read_end1 disagrees with the length of its read in the text"
                     : e & kRptErrGroup ? "an alignment names an (index, part) that is not loaded"
                     : e & kRptErrRef ? "an alignment's ref_num is beyond the reference names of its part"
-                    : e & kRptErrQual ? "reads text: a FASTQ record without its quality line" : "an alignment's CIGAR lies outside cigar_words");
+                    : e & kRptErrQual ? "reads text: a FASTQ record without its quality line"
+                    : e & kRptErrCigar ? "an alignment's CIGAR lies outside cigar_words" : "an alignment's CIGAR runs past its read or its reference");
 }
 
 // The first half of smr_format_reports and smr_otu_add: text, results and groups on the device (e1 recorded after the copies), the
@@ -1495,19 +1496,27 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
   CK(cudaStreamSynchronize(ctx->stream));
 }
 
+// pairwise: smr_format_blast_pairwise[_gz], the pairwise BLAST rows alone (-blast 0), one stream per group; otherwise the streams of
+// smr_format_reports[_gz].  Both share the routing (the skip of empty reads), the row order and the scans.
 void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
                          const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
-                         char* out, uint64_t cap, uint64_t* so_out, bool gz) {
+                         char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise) {
   const bool mates = o->mates || (!text && ctx->resident_mates);   // the resident batch of a mate stream is mates
   const bool paired = o->paired_in || o->paired_out || mates;
-  if ((o->out2 || o->sout) && !paired) fail(SMR_ERR_UNSUPPORTED, "-out2 / -sout: only a paired batch (mates, paired_in or paired_out) has mates to split");
-  if (o->blast && o->blast_format != 1) fail(SMR_ERR_UNSUPPORTED, "only tabular BLAST (-blast 1) is written on the device");
+  if (pairwise) {   // -blast '0 cigar' is refused by the reference too (options.cpp:584-588)
+    if (!o->blast || o->blast_format != 0 || o->blast_cols[0] || o->sam || o->fastx || o->other || o->denovo)
+      fail(SMR_ERR_ARG, "pairwise BLAST: opts must ask for -blast 0 alone (blast = 1, blast_format = 0, no BLAST columns, no SAM or read files)");
+  } else {
+    if ((o->out2 || o->sout) && !paired) fail(SMR_ERR_UNSUPPORTED, "-out2 / -sout: only a paired batch (mates, paired_in or paired_out) has mates to split");
+    if (o->blast && o->blast_format != 1)
+      fail(SMR_ERR_UNSUPPORTED, "smr_format_reports writes tabular BLAST (-blast 1) only: pairwise BLAST (-blast 0) is smr_format_blast_pairwise");
+  }
   if (o->paired_in && o->paired_out) fail(SMR_ERR_ARG, "paired_in and paired_out are exclusive");
-  if (o->sout && (o->paired_in || o->paired_out)) fail(SMR_ERR_ARG, "-sout cannot be used with paired_in or paired_out");
+  if (!pairwise && o->sout && (o->paired_in || o->paired_out)) fail(SMR_ERR_ARG, "-sout cannot be used with paired_in or paired_out");
   if (paired && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
-  const uint32_t num_out = o->out2 && o->sout ? 4 : o->out2 || o->sout ? 2 : 1;   // ReportFxBase::set_num_out
-  const uint32_t nfx = 3 * num_out;                                                // aligned, other, denovo: num_out files each
-  if ((o->sam || o->blast || o->denovo) && nreads && !stats) fail(SMR_ERR_ARG, "SAM, BLAST and denovo need the smr_aln_stats of the batch");
+  const uint32_t num_out = pairwise ? 1 : o->out2 && o->sout ? 4 : o->out2 || o->sout ? 2 : 1;   // ReportFxBase::set_num_out
+  const uint32_t nfx = pairwise ? 0 : 3 * num_out;                                                // aligned, other, denovo: num_out files each
+  if ((o->sam || (o->blast && !pairwise) || o->denovo) && nreads && !stats) fail(SMR_ERR_ARG, "SAM, BLAST and denovo need the smr_aln_stats of the batch");
   if (nreads && (!results || !alns)) fail(SMR_ERR_ARG, ctx->err);   // a null array: no text of its own, the last one stays
   uint32_t ncols = 0, cols[4] = {0, 0, 0, 0};
   if (o->blast)
@@ -1525,7 +1534,8 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
     const bool sc = pt.d.index_num < ctx->rpt_score.size() && ctx->rpt_score[pt.d.index_num].set;
     if (o->blast && !sc) fail(SMR_ERR_ARG, "smr_set_report_scoring was not called for index " + std::to_string(pt.d.index_num));
     hg[g] = RptGroup{pt.rnames, pt.rname_off, sc ? (const double*)ctx->rpt_score[pt.d.index_num].ev.p : nullptr,
-                     sc ? (const uint32_t*)ctx->rpt_score[pt.d.index_num].bits.p : nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0};
+                     sc ? (const uint32_t*)ctx->rpt_score[pt.d.index_num].bits.p : nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0,
+                     pt.d.refseq, pt.d.ref_off};
   }
   const uint32_t slots = slots_of(ctx);
   const uint64_t N = (uint64_t)nreads * slots;
@@ -1571,13 +1581,14 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
     });
     rpt_group_first_kernel<<<(G + 128) / 128, 128, 0, ctx->stream>>>((const uint32_t*)ctx->r_keys2.p, N, G, first);
     if (o->sam) rpt_sam_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, sz);
-    if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz, nullptr, nullptr);
+    if (o->blast && pairwise) rpt_pw_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz);
+    else if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz, nullptr, nullptr);
     if (o->fastx || o->other || o->denovo) {
       rpt_fx_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, fxsz, fstride);
     }
     cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, sz, off, (int)(N + 1), ctx->stream); });
     cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, bsz, boff, (int)(N + 1), ctx->stream); });
-    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fxsz, fxoff, (int)(nfx * fstride), ctx->stream); });
+    if (nfx) cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, fxsz, fxoff, (int)(nfx * fstride), ctx->stream); });
   } else {
     CK(cudaMemsetAsync(off, 0, 8, ctx->stream));
     CK(cudaMemsetAsync(boff, 0, 8, ctx->stream));
@@ -1590,7 +1601,8 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   if (h[4]) rpt_error(h[4]);
-  if (!gz) memcpy(so_out, hso.data(), (size_t)nso * 8);
+  const uint32_t s0 = pairwise ? G : 0;   // the first stream handed out: pairwise, the BLAST streams alone (the SAM ones are empty)
+  if (!gz) memcpy(so_out, hso.data() + s0, (size_t)(nso - s0) * 8);
   const uint64_t total = hso[nso - 1];
   if (!gz && total && (!out || cap < total)) fail(SMR_ERR_CAPACITY, "output buffer too small: stream_off holds the sizes");
   // the encoder reads up to 8 bytes past a stream's end (def_load32): the padding is part of the one allocation before the writes,
@@ -1599,12 +1611,13 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   if (total) {
     char* dout = (char*)ctx->r_out.p;
     if (o->sam) rpt_sam_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, off, dout);
-    if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, nullptr, boff, dout + hso[G]);
+    if (o->blast && pairwise) rpt_pw_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, boff, dout + hso[G]);
+    else if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, nullptr, boff, dout + hso[G]);
     if (o->fastx || o->other || o->denovo) rpt_fx_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, fxoff, fstride, so + 2 * G, dout);
     CK(cudaGetLastError());
   }
   if (gz) {   // every non-empty stream to one gzip member, before the D2H
-    std::vector<uint64_t> sb(hso.begin(), hso.end() - 1), se(hso.begin() + 1, hso.end());
+    std::vector<uint64_t> sb(hso.begin() + s0, hso.end() - 1), se(hso.begin() + s0 + 1, hso.end());
     gzip_streams(ctx, (const uint8_t*)ctx->r_out.p, sb, se, out, cap, so_out, e2, e3);
   } else {
     CK(cudaEventRecord(e2, ctx->stream));
@@ -2189,7 +2202,7 @@ int smr_format_reports(smr_ctx* ctx, const smr_report_opts* opts, const char* te
                        char* out, uint64_t cap, uint64_t* stream_off) try {
   if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, false);
+  format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, false, false);
   return SMR_OK;
 } SMR_CATCH(ctx)
 
@@ -2198,7 +2211,25 @@ int smr_format_reports_gz(smr_ctx* ctx, const smr_report_opts* opts, const char*
                           char* out, uint64_t cap, uint64_t* stream_off) try {
   if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, true);
+  format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, true, false);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_format_blast_pairwise(smr_ctx* ctx, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
+                              const smr_aln* alns, const uint32_t* cigar_pool, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                              char* out, uint64_t cap, uint64_t* stream_off) try {
+  if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, false, true);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_format_blast_pairwise_gz(smr_ctx* ctx, const smr_report_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
+                                 const smr_aln* alns, const uint32_t* cigar_pool, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                                 char* out, uint64_t cap, uint64_t* stream_off) try {
+  if (!ctx || !opts || !stream_off || (!text && nbytes)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  format_reports_impl(ctx, opts, text, nbytes, results, alns, cigar_pool, cigar_words, stats, nreads, out, cap, stream_off, true, true);
   return SMR_OK;
 } SMR_CATCH(ctx)
 

@@ -10,6 +10,8 @@ drop-in boundary so that tests and bench.py can feed the C-ABI the same bytes th
   * `parse_stats`    -- the `.stats` index file (`Refstats::load`, src/sortmerna/refstats.cpp:103-190)
   * `minimal_score`  -- the E-value -> minimal SW score formula (refstats.cpp:236-265) given lambda, K
   * `format_sam_rows`-- the SAM row layout of `ReportSam::append` (src/sortmerna/report_sam.cpp:64-152)
+  * `format_blast_rows` / `format_blast_pairwise_rows` -- tabular and pairwise BLAST rows of `ReportBlast::append`
+    (src/sortmerna/report_blast.cpp:99-365)
 """
 from __future__ import annotations
 
@@ -272,6 +274,69 @@ def format_blast_rows(batch: "ReadBatch", refs_by_index: list, results, alns, ci
                                    str(int(al["ref_begin1"]) + 1), str(int(al["ref_end1"]) + 1), _g3(evalue), str(bitscore), cs,
                                    _g3(cov * 100), "+" if bool(al["strand"]) else "-"]))
     return rows
+
+
+_NT_BYTES = np.frombuffer(NT_MAP.encode(), np.uint8)
+PAIRWISE_COLS = 60
+
+
+def format_blast_pairwise_rows(batch: "ReadBatch", refs_by_index: list, results, alns, cigar_pool, slots: int, gumbel: list,
+                               ev_params: list, paired: bool = False) -> list:
+    """Pairwise BLAST rows (-blast 0) as ReportBlast::append prints them (src/sortmerna/report_blast.cpp:136-251), one string per
+    stored alignment in the order of aligned.blast: (index, part) group, then read, then alignment slot.  Reads are skipped as the
+    report writer skips empty reads (paired: a pair whose second mate is empty).  gumbel / ev_params as for format_blast_rows.
+    A row is its header lines, then the CIGAR's columns cut into blocks of 60; the reference's three passes per block with their
+    carry-over (left, e) come down to that plain chunking."""
+    keyed = []
+    for r in range(batch.n):
+        if len(batch.seqs[(r | 1) if paired else r]) == 0:
+            continue
+        enc = batch.cat[int(batch.off[r]):int(batch.off[r + 1])]
+        for a in range(int(results["n_align"][r])):
+            al = alns[r * slots + a]
+            keyed.append(((int(al["index_num"]), int(al["part"])), _pairwise_row(batch.headers[r], enc, al, _refs_of(refs_by_index, al),
+                                                                                  cigar_pool, gumbel, ev_params)))
+    keyed.sort(key=lambda x: x[0])   # stable: read, then slot within a group
+    return [row for _, row in keyed]
+
+
+def _pairwise_row(header, enc, al, refs, cigar_pool, gumbel, ev_params) -> str:
+    idx, score, strand = int(al["index_num"]), int(al["score1"]), bool(al["strand"])
+    lam, K = gumbel[idx]
+    full_ref, full_read = ev_params[idx]
+    bits = max(0, int(np.float32(np.float32(lam * score - math.log(K)) / np.float32(math.log(2)))))   # report_blast.cpp:117-119
+    evalue = K * full_ref * full_read * math.exp(-lam * score)                                       # :121-126
+    ref_num = int(al["ref_num"])
+    ref = refs.cat[int(refs.off[ref_num]):int(refs.off[ref_num + 1])]
+    read = enc if strand else np.where(enc < 4, 3 - enc, 4)[::-1]
+    out = [f"Sequence ID: {refs.ids[ref_num]}\nQuery ID: {seq_id(header)}\n"
+           f"Score: {score} bits ({bits})\tExpect: {_g3(evalue)}\tstrand: {'+' if strand else '-'}\n\n"]
+    # every column: reference char, middle char, read char, and whether it consumes the reference / the read
+    top, mid, bot, dq, dp = [], [], [], [], []
+    q, p = int(al["ref_begin1"]), int(al["read_begin1"])
+    for c in cigar_pool[int(al["cigar_off"]):int(al["cigar_off"]) + int(al["cigar_len"])]:
+        op, n = int(c) & 0xF, int(c) >> 4
+        eq, ep = (q + n if op != 1 else q), (p + n if op <= 1 else p)
+        if q < 0 or p < 0 or eq > ref.size or ep > read.size:
+            raise ValueError(f"CIGAR runs past the read or the reference of {seq_id(header)}")
+        t = _NT_BYTES[ref[q:eq]] if op != 1 else np.full(n, ord("-"), np.uint8)
+        b = _NT_BYTES[read[p:ep]] if op <= 1 else np.full(n, ord("-"), np.uint8)
+        top.append(t)
+        bot.append(b)
+        mid.append(np.where(t == b, ord("|"), ord("*")).astype(np.uint8) if op == 0 else np.full(n, ord(" "), np.uint8))
+        dq.append(np.full(n, op != 1, np.int64))
+        dp.append(np.full(n, op <= 1, np.int64))
+        q, p = eq, ep
+    if top:
+        top, mid, bot = (np.concatenate(x).tobytes().decode() for x in (top, mid, bot))
+        cq, cp = np.cumsum(np.concatenate(dq)), np.cumsum(np.concatenate(dp))
+        q, p = int(al["ref_begin1"]), int(al["read_begin1"])
+        for b in range(0, len(top), PAIRWISE_COLS):
+            e = min(b + PAIRWISE_COLS, len(top))
+            q1, p1 = int(al["ref_begin1"]) + int(cq[e - 1]), int(al["read_begin1"]) + int(cp[e - 1])
+            out.append(f"Target: {q + 1:>8}    {top[b:e]}    {q1}\n{' ' * 20}{mid[b:e]}\nQuery: {p + 1:>9}    {bot[b:e]}    {p1}\n\n")
+            q, p = q1, p1
+    return "".join(out)
 
 
 def host_aln_stats(batch: "ReadBatch", refs_by_index: list, results, alns, cigar_pool, slots: int):

@@ -8,8 +8,10 @@ databases, aligned once on the GPU, then formatted per output kind.  Prints one 
     compressed bytes, the call wall times, the sizes Python's zlib makes of the same streams at levels 1 and 6, and the gz call's
     device span minus the plain call's (compress_span_ms: the encoder's kernels plus the host work inside the span -- chunk plan,
     the read-back of the chunk sizes, the byte-size scan, the uploads).  For "all", the encoder's kernels alone under torch.profiler
-    (one run of its own): device time per kernel, their sum and its input GB/s.
-Run on the GPU:  python tools/bench_reports.py --reads 1000000 [--gzip]"""
+    (one run of its own): device time per kernel, their sum and its input GB/s;
+  * with --pairwise, only BLAST: tabular rows (smr_format_reports, '1 cigar qcov qstrand') and pairwise rows (-blast 0,
+    smr_format_blast_pairwise) of the same results, each plain and gzip: output MB, device time, H2D / D2H and the call's wall time.
+Run on the GPU:  python tools/bench_reports.py --reads 1000000 [--gzip | --pairwise]"""
 import argparse
 import json
 import os
@@ -32,6 +34,28 @@ FORMATS = {"sam": dict(sam=True), "blast": dict(blast="1 cigar qcov qstrand"), "
            "all": dict(sam=True, blast="1 cigar qcov qstrand", fastx=True, other=True, denovo=(0.97, 0.97))}
 
 
+def pairwise_leg(al, res, n, reps):
+    """tabular and pairwise BLAST of the same results, plain and gzip (medians over reps calls after one warm-up)"""
+    calls = {"blast_tabular": lambda gz: al.format_reports(res, None, gzip=gz, **FORMATS["blast"])["blast"],
+             "blast_pairwise": lambda gz: al.format_blast_pairwise(res, None, gzip=gz)}
+    out = {}
+    for name, call in calls.items():
+        for gz in (False, True):
+            call(gz)
+            dev, wall = [], []
+            for _ in range(reps):
+                t0 = time.perf_counter()
+                s = call(gz)
+                wall.append(time.perf_counter() - t0)
+                dev.append(al.report_timings())
+            nb = sum(len(x) for x in s)
+            med = {k: float(np.median([t[k] for t in dev])) for k in ("device_ms", "h2d_ms", "d2h_ms")}
+            w = float(np.median(wall))
+            out[name + ("_gz" if gz else "")] = dict(out_mb=nb / 1e6, **med, call_wall_ms=w * 1e3, device_mb_s=nb / 1e6 / (med["device_ms"] / 1e3),
+                                                     wall_reads_s=n / w)
+    return out
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--reads", type=int, default=1_000_000)
@@ -39,6 +63,7 @@ def main():
     ap.add_argument("--host-reads", type=int, default=20_000, help="subset for the Python hostio formatters")
     ap.add_argument("--reference", type=int, default=0, help="reads of the subset the reference binary formats (0: skip)")
     ap.add_argument("--gzip", action="store_true", help="also time the gzip (-zip-out) call of every format")
+    ap.add_argument("--pairwise", action="store_true", help="only tabular and pairwise BLAST (-blast 0), each plain and gzip")
     args = ap.parse_args()
     out = dict(card=bench.card(0), reads=args.reads)
     with tempfile.TemporaryDirectory(prefix="smr_bench_rpt_") as work:
@@ -63,6 +88,11 @@ def main():
         res = al.download()
         out["aligned"] = int(res["res"]["is_hit"].sum())
         out["text_mb"] = len(text) / 1e6
+        if args.pairwise:
+            out["blast"] = pairwise_leg(al, res, n, args.reps)
+            al.close()
+            print(json.dumps(out))
+            return
         def timed(kw, gz):
             al.format_reports(res, None, gzip=gz, **kw)   # warm-up: buffers, module load
             dev, wall = [], []
