@@ -351,7 +351,7 @@ int smr_format_blast_pairwise_gz(smr_ctx*, const smr_report_opts* opts, const ch
 /* n host bytes compressed on the device into one gzip member (n == 0: an empty member).  *out_bytes = its size; if out is null or
  * cap is smaller, SMR_ERR_CAPACITY. */
 int smr_gzip(smr_ctx*, const void* in, uint64_t n, void* out, uint64_t cap, uint64_t* out_bytes);
-/* of the last smr_format_reports[_gz], smr_format_blast_pairwise[_gz] or smr_gzip, milliseconds (CUDA events): out[0] = H2D of the input (text and results), [1] =
+/* of the last smr_format_reports[_gz], smr_format_blast_pairwise[_gz], smr_denovo_stats or smr_gzip, milliseconds (CUDA events): out[0] = H2D of the input (text and results), [1] =
  * device work (layout, sizes, scans, writes, compression; includes the read-backs of the sizes), [2] = D2H of the output */
 int smr_last_report_timings(const smr_ctx*, double out[3]);
 
@@ -361,25 +361,52 @@ int smr_last_report_timings(const smr_ctx*, double out[3]);
  *    alignments passes -id and -coverage with floor(x * 1000 + 0.5) / 1000.0, processor.cpp:334-342) and the alignment itself passes
  *    them with floor(x * 1000 + 0.5) * 0.001 (otumap.cpp:160-163).  %id is taken from n_match_denovo.  Lines: one per reference id in
  *    unsigned byte order of the id, "id\tread\tread...\n"; within a line the (index, part) groups in order, reads in the order added. */
+/* Paired reads: the reference's OTU pass reads readfeed slot 0 (otumap.cpp:144), which is every record of one interleaved file but
+ * only the first file of two mate files.  In both, a pair (records 2k, 2k+1) whose second record is empty was skipped by the
+ * denovo_stats pass, so neither of its mates is an entry. */
+enum { SMR_OTU_SINGLE = 0, SMR_OTU_ONE_FILE = 1, SMR_OTU_TWO_FILES = 2 };
 typedef struct {
   double min_id, min_cov;         /* -id, -coverage (the reference's default under -otu_map: 0.97, 0.97) */
-  int32_t paired_in, paired_out;  /* a paired batch: SMR_ERR_UNSUPPORTED (DESIGN.md 5e) */
+  int32_t paired_in, paired_out;  /* with feed SMR_OTU_SINGLE, a paired batch: SMR_ERR_UNSUPPORTED (DESIGN.md 5e) */
+  int32_t feed;                   /* SMR_OTU_SINGLE: single-end reads; SMR_OTU_ONE_FILE: one interleaved paired file, every record is
+                                     looked at; SMR_OTU_TWO_FILES: two mate files (records 2k and 2k+1 of a batch), only records 2k
+                                     can be entries -- the only feed that takes a mate stream's batch.  Paired feeds need even batches. */
 } smr_otu_opts;
 /* Open (or reset) the accumulator of this context.  SMR_ERR_ARG if params.is_best == 0 (the reference refuses -otu_map with
- * -no-best) or a loaded part has no smr_set_report_refs.  Loading a part or setting report ids afterwards makes the next
- * smr_otu_add / smr_otu_finish fail with SMR_ERR_ARG. */
+ * -no-best), a loaded part has no smr_set_report_refs or feed is unknown.  Loading a part or setting report ids afterwards makes the
+ * next smr_otu_add / smr_otu_finish fail with SMR_ERR_ARG. */
 int smr_otu_begin(smr_ctx*, const smr_otu_opts* opts);
-/* Add one batch: text / nbytes / results / alns / stats as for smr_format_reports (text == nullptr: the resident text).
- * *n_added = entries it added (optional). */
+/* Add one batch: text / nbytes / results / alns / stats as for smr_format_reports (text == nullptr: the resident text; a mate stream's
+ * resident batch needs feed SMR_OTU_TWO_FILES, SMR_ERR_UNSUPPORTED otherwise).  *n_added = entries it added (optional). */
 int smr_otu_add(smr_ctx*, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
                 uint32_t nreads, uint64_t* n_added);
-/* The map: counts[0] = bytes, [1] = lines ("Total OTUs"), [2] = entries ("passing %id and %coverage" of aligned.log).  The reference
- * writes no file when counts[2] == 0.  If out is null or cap < counts[0]: SMR_ERR_CAPACITY with counts filled and the accumulator
- * kept; a successful call closes it (smr_otu_begin opens the next). */
+/* The map: counts[0] = bytes, [1] = lines ("Total OTUs"), [2] = entries.  The reference writes no file when counts[2] == 0.  The
+ * "passing %id and %coverage" figure of aligned.log is the n_yid_ycov total of smr_denovo_stats, which equals the entries for
+ * single-end reads at ordinary thresholds but counts both files of two mate files.  If out is null or cap < counts[0]:
+ * SMR_ERR_CAPACITY with counts filled and the accumulator kept; a successful call closes it (smr_otu_begin opens the next). */
 int smr_otu_finish(smr_ctx*, char* out, uint64_t cap, uint64_t counts[3]);
 /* milliseconds (CUDA events): out[0] = H2D of the smr_otu_add calls since smr_otu_begin, [1] = their device work (includes the one
  * read-back of the sizes per call), [2] = the last smr_otu_finish (sort, sizes, write, D2H) */
 int smr_last_otu_timings(const smr_ctx*, double out[3]);
+
+/* -- De novo statistics on the device (sortmerna_b200/csrc/smr_otu.cuh): the reference's denovo_stats pass (denovo_stats_run,
+ *    processor.cpp:287-438, run under -otu_map or -de_novo_otu) at -threads 1.  Every stored alignment falls in one class by %id
+ *    (from n_match_denovo) and %coverage, both rounded with floor(x * 1000 + 0.5) / 1000.0: c_yid_ycov (both pass), n_yid_ncov (%id
+ *    only), n_nid_ycov (%coverage only) or n_denovo (neither). */
+typedef struct {
+  double min_id, min_cov;   /* -id, -coverage */
+  int32_t paired;           /* records 2k and 2k+1 are mates (-paired_in / -paired_out / two mate files): a pair whose second record
+                               is empty counts for neither mate (processor.cpp:323-327).  Implied for a mate stream's resident batch.
+                               The last record of an odd batch has no mate and counts for nothing, as the reference skips the
+                               last record of an odd interleaved file. */
+} smr_denovo_opts;
+/* One batch: text / nbytes / results / alns / stats / nreads as for smr_otu_add (text == nullptr: the resident text; stats required;
+ * the record count and every alignment's readlen are checked against the text, SMR_ERR_ARG otherwise).  per_read (nullable) [nreads *
+ * 4] = {c_yid_ycov, n_yid_ncov, n_nid_ycov, n_denovo} of every read, the denovo4 of smr_pack_kvdb_blobs.  totals[4] are ADDED TO
+ * (so a run of batches sums itself): Readstats n_yid_ycov, n_yid_ncov, n_nid_ycov, num_denovo of aligned.log.  Timings through
+ * smr_last_report_timings. */
+int smr_denovo_stats(smr_ctx*, const smr_denovo_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
+                     const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4]);
 
 /* Device-side timings of the last smr_run_resident / smr_align_batch, CUDA events on the
  * library's stream, milliseconds: out[0]=total [1]=seed kernels [2]=candidate/SW kernels

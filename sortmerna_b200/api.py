@@ -30,7 +30,8 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_build_index_device", "smr_debug_index_array", "smr_set_instrumentation", "smr_set_report_refs", "smr_set_report_scoring",
            "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings",
            "smr_format_reports_gz", "smr_gzip", "smr_stream_begin", "smr_stream_push", "smr_stream_next", "smr_stream_counts",
-           "smr_stream_push_mate", "smr_format_blast_pairwise", "smr_format_blast_pairwise_gz"]
+           "smr_stream_push_mate", "smr_format_blast_pairwise", "smr_format_blast_pairwise_gz",
+           "smr_denovo_stats"]
 
 CNT_NAMES = ("num_aligned", "num_short", "sw_calls", "sw_cells", "windows", "trie_nodes", "buckets",
              "bucket_entries", "pos_entries", "lis_calls", "dbg_max_read_cycles", "dbg_sum_read_cycles", "dbg_lis_kernel_cycles",
@@ -95,7 +96,20 @@ def report_opts(sam=False, blast=None, fastx=False, other=False, denovo=None, pa
 
 class OtuOpts(C.Structure):
     """smr_otu_opts (include/smr_b200.h)"""
-    _fields_ = [("min_id", C.c_double), ("min_cov", C.c_double), ("paired_in", C.c_int32), ("paired_out", C.c_int32)]
+    _fields_ = [("min_id", C.c_double), ("min_cov", C.c_double), ("paired_in", C.c_int32), ("paired_out", C.c_int32), ("feed", C.c_int32)]
+
+
+# smr_otu_opts.feed: which records of a paired run the OTU map looks at (SMR_OTU_ONE_FILE: every record of one interleaved file;
+# SMR_OTU_TWO_FILES: the first file's records 2k of two mate files)
+OTU_FEEDS = {None: 0, "one_file": 1, "two_files": 2}
+
+
+class DenovoOpts(C.Structure):
+    """smr_denovo_opts (include/smr_b200.h)"""
+    _fields_ = [("min_id", C.c_double), ("min_cov", C.c_double), ("paired", C.c_int32)]
+
+
+DENOVO_TOTALS = ("n_yid_ycov", "n_yid_ncov", "n_nid_ycov", "num_denovo")
 
 
 def num_out_of(o: ReportOpts) -> int:
@@ -621,10 +635,12 @@ class Aligner:
         return [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(G)]
 
     # ---- OTU map (smr_otu_begin / smr_otu_add / smr_otu_finish) ----
-    def otu_begin(self, min_id: float = 0.97, min_cov: float = 0.97, paired_in: bool = False, paired_out: bool = False):
-        """smr_otu_begin: open (or reset) the OTU map of this context; -id / -coverage as the reference's -otu_map defaults them"""
+    def otu_begin(self, min_id: float = 0.97, min_cov: float = 0.97, paired_in: bool = False, paired_out: bool = False, feed=None):
+        """smr_otu_begin: open (or reset) the OTU map of this context; -id / -coverage as the reference's -otu_map defaults them.
+        feed: None (single-end; paired_in / paired_out are refused), "one_file" (one interleaved paired file: every record) or
+        "two_files" (two mate files, as stream_mates batches them: records 2k, the first file's, alone)"""
         self._upload_report_refs()
-        o = OtuOpts(float(min_id), float(min_cov), int(bool(paired_in)), int(bool(paired_out)))
+        o = OtuOpts(float(min_id), float(min_cov), int(bool(paired_in)), int(bool(paired_out)), OTU_FEEDS[feed] if feed in OTU_FEEDS else int(feed))
         self._check(self.L.smr_otu_begin(self.h, C.byref(o)), "smr_otu_begin")
 
     def otu_add(self, out: dict, text: bytes | None = None) -> int:
@@ -651,6 +667,25 @@ class Aligner:
         self._check(rc, "smr_otu_finish")
         self._otu_buf = buf
         return dict(text=bytes(buf[:int(counts[0])]), total_otu=int(counts[1]), n_yid_ycov=int(counts[2]))
+
+    def denovo_stats(self, out: dict, text: bytes | None = None, min_id: float = 0.97, min_cov: float = 0.97, paired: bool = False):
+        """smr_denovo_stats: the reference's denovo_stats pass over one batch (out and text as for format_reports; out needs "stats").
+        Returns (per_read, totals): per_read an (nreads, 4) uint32 array of {c_yid_ycov, n_yid_ncov, n_nid_ycov, n_denovo} per read
+        (pack_kvdb_blobs' denovo), totals {"n_yid_ycov", "n_yid_ncov", "n_nid_ycov", "num_denovo"} of this batch.  paired: records
+        2k and 2k+1 are mates (implied for the resident batch of stream_mates)."""
+        res, alns, st = out["res"], out["alns"], out.get("stats")
+        txt = np.frombuffer(text, np.uint8) if text is not None else None
+        n = res.shape[0]
+        per_read = np.zeros((n, 4), np.uint32)
+        tot = np.zeros(4, np.uint64)
+        o = DenovoOpts(float(min_id), float(min_cov), int(bool(paired)))
+        self.L.smr_denovo_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
+                                            C.c_void_p, C.c_void_p]
+        rc = self.L.smr_denovo_stats(self.h, C.cast(C.byref(o), C.c_void_p), _ptr(txt) if txt is not None and txt.size else None,
+                                     txt.size if txt is not None else 0, _ptr(res), _ptr(alns), _ptr(st) if st is not None else None, n,
+                                     _ptr(per_read) if n else None, _ptr(tot))
+        self._check(rc, "smr_denovo_stats")
+        return per_read, dict(zip(DENOVO_TOTALS, (int(v) for v in tot)))
 
     def otu_timings(self):
         out = np.zeros(3, np.float64)
@@ -711,7 +746,16 @@ class ReportWriter:
     group 0, then group 1, ...), so that feeding a file in several batches writes what one batch writes.
     sam_header: the text before the SAM rows (hostio.sam_header); opts: report_opts(...) keyword arguments.
     otu_map: (min_id, min_cov) = the reference's -otu_map -id -coverage: close() also writes otu_map.txt (none when no alignment
-    passes, as the reference) and sets total_otu and n_yid_ycov, the two OTU numbers of aligned.log.
+    passes, as the reference) and sets total_otu (its lines, "Total OTUs" of aligned.log) and n_yid_ycov (its entries).  For
+    single-end reads the entries are aligned.log's "passing %id and %coverage" figure too; that figure is the n_yid_ycov total of the
+    denovo_stats pass (denovo_counts), which for two mate files counts both files while the map holds the first file's reads only.
+    otu_feed: for a paired run with otu_map, "one_file" (one interleaved file, -paired_in / -paired_out: every record) or
+    "two_files" (stream_mates batches: the first file's reads); without it a paired otu_map is refused (SMR_ERR_UNSUPPORTED).
+    summary: writes aligned.log at close() (hostio.summary_log, always plain): a dict of summary_log's inputs the library does not
+    know -- cmd, refs, reads, gumbel, minimal_score, and optionally lnwin, skiplengths, threads, sq, pid, timestamp and counts
+    (Aligner.read_counts(reads); counted at close() when absent).  The writer sums num_aligned and reads_matched_per_db over the
+    batches it is given, and with denovo or otu_map on runs the denovo_stats pass (Aligner.denovo_stats) on every batch, its totals
+    in denovo_counts.
     zip_out: the reference's -zip-out (its default for gzip input): every report file is written gzip-compressed on the device under
     its name with ".gz" appended, as members appended batch by batch (a multi-member file, as the reference's merge makes); a file
     with no member gets one empty member.  otu_map.txt stays plain, as the reference writes it.
@@ -720,12 +764,19 @@ class ReportWriter:
     and aligned_denovo.*; batches of stream_mates are mates without further options (mates=True for a batch passed as text).
     blast="0": aligned.blast holds the pairwise rows (format_blast_pairwise); the other files are written as with any other blast."""
 
-    def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", otu_map=None, zip_out: bool = False, **opts):
+    def __init__(self, out_dir: str, aligner: Aligner, sam_header: str = "", otu_map=None, zip_out: bool = False, otu_feed=None,
+                 summary: dict | None = None, **opts):
         self.dir, self.al, self.header, self.zip_out = out_dir, aligner, sam_header, zip_out
         self.opts = report_opts(**opts)
         self.otu_map, self.total_otu, self.n_yid_ycov = otu_map, None, None
+        if otu_feed not in OTU_FEEDS:
+            raise ValueError(f"otu_feed: {otu_feed!r} is not one of {list(OTU_FEEDS)}")
+        self.otu_feed = otu_feed
         if otu_map is not None:
-            aligner.otu_begin(otu_map[0], otu_map[1], paired_in=self.opts.paired_in, paired_out=self.opts.paired_out)
+            aligner.otu_begin(otu_map[0], otu_map[1], paired_in=self.opts.paired_in, paired_out=self.opts.paired_out, feed=otu_feed)
+        self.summary = summary
+        self.num_aligned, self.reads_matched_per_db = 0, None
+        self.denovo_counts = dict.fromkeys(DENOVO_TOTALS, 0) if summary is not None and (otu_map is not None or self.opts.denovo) else None
         self.ext = None
         self._parts = {}
         os.makedirs(out_dir, exist_ok=True)
@@ -759,6 +810,16 @@ class ReportWriter:
                 self._append(f"{k}_{j}", data)
         if self.otu_map is not None:
             self.al.otu_add(out, text)
+        if self.summary is not None:
+            self.num_aligned += out["counters"]["num_aligned"]
+            m = np.asarray(out["matched"][:max(1, self.al.n_index_files)], np.uint64)
+            self.reads_matched_per_db = m.copy() if self.reads_matched_per_db is None else self.reads_matched_per_db + m
+        if self.denovo_counts is not None:
+            mid, mcov = self.otu_map if self.otu_map is not None else (o.min_id, o.min_cov)
+            paired = bool(o.paired_in or o.paired_out or o.mates) or self.otu_feed is not None
+            _, t = self.al.denovo_stats(out, text, mid, mcov, paired=paired)
+            for k, v in t.items():
+                self.denovo_counts[k] += v
         return s
 
     def close(self) -> list:
@@ -798,11 +859,32 @@ class ReportWriter:
                 with open(path, "wb") as f:
                     f.write(m["text"])
                 paths.append(path)
+        if self.summary is not None:
+            paths.append(self._write_summary())
         for k, fh in self._parts.items():
             fh.close()
             os.unlink(os.path.join(self.dir, f".part_{k}"))
         self._parts = {}
         return paths
+
+
+    def _write_summary(self) -> str:
+        """aligned.log from the summary inputs and what the batches gave (the reference writes it with a plain ofstream, even
+        under -zip-out)"""
+        kw = dict(self.summary)
+        counts = kw.pop("counts", None) or self.al.read_counts(kw["reads"])
+        nidx = len(kw["refs"])
+        matched = self.reads_matched_per_db if self.reads_matched_per_db is not None else np.zeros(nidx, np.uint64)
+        dn = self.denovo_counts
+        text = hostio.summary_log(
+            total_reads=counts["reads"], all_reads_len=counts["length"], min_len=counts["min_len"], max_len=counts["max_len"],
+            num_aligned=self.num_aligned, reads_matched_per_db=[int(x) for x in matched[:nidx]], params=kw.pop("params", getattr(self.al, "params", None)),
+            denovo=dn["num_denovo"] if self.opts.denovo else None,
+            otu=(dn["n_yid_ycov"], self.total_otu) if self.otu_map is not None else None, **kw)
+        path = os.path.join(self.dir, "aligned.log")
+        with open(path, "wb") as f:
+            f.write(text.encode())
+        return path
 
 
 def align_files(aligner: Aligner, batch: hostio.ReadBatch):

@@ -151,12 +151,13 @@ struct smr_ctx {
   uint64_t parts_gen = 0;   // bumped whenever a part is loaded or its report ids are set: an open OTU map refuses to go on after that
   // OTU map accumulator (smr_otu.cuh), smr_otu_begin .. smr_otu_finish
   struct Otu {
-    bool active = false; uint64_t gen = 0; double min_id = 0, min_cov = 0;
+    bool active = false; uint64_t gen = 0; double min_id = 0, min_cov = 0; uint32_t feed = 0;
     std::vector<RptGroup> groups; uint32_t gbits = 0, kbits = 0;
     DevBuf rank, rank_off, grp, key, ent, pool, flag, pos, nsz, noff, vals, skey, sidx, size, off, out, scal;
     uint64_t n = 0, pool_bytes = 0;
     double t[3] = {0, 0, 0};
   } otu;
+  DevBuf dn_read, dn_tot;   // smr_denovo_stats: per-read counters, totals
   // timings
   std::vector<cudaEvent_t> ev;
   RunTimes t_run;   // the last run, and the retries of its download
@@ -1657,9 +1658,10 @@ void otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
   if (!ctx->have_params || !ctx->prm.is_best)
     fail(SMR_ERR_ARG, "the OTU map is made from the best alignments: params.is_best must be 1 (-otu_map cannot be set with -no-best)");
   if (o->paired_in && o->paired_out) fail(SMR_ERR_ARG, "paired_in and paired_out are exclusive");
-  if (o->paired_in || o->paired_out)
-    fail(SMR_ERR_UNSUPPORTED, "paired reads: the reference's OTU pass reads only the first mate file of two, but every record of one interleaved file, "
-                              "so a paired batch does not say which map is meant");
+  if (o->feed != SMR_OTU_SINGLE && o->feed != SMR_OTU_ONE_FILE && o->feed != SMR_OTU_TWO_FILES) fail(SMR_ERR_ARG, "unknown OTU feed");
+  if (o->feed == SMR_OTU_SINGLE && (o->paired_in || o->paired_out))
+    fail(SMR_ERR_UNSUPPORTED, "paired reads: the reference's OTU pass reads only the first mate file of two, but every record of one interleaved file: "
+                              "say which with feed SMR_OTU_ONE_FILE or SMR_OTU_TWO_FILES");
   const std::vector<const Part*> gp = report_groups(ctx);
   const uint32_t G = (uint32_t)gp.size();
   for (const Part* pt : gp)
@@ -1687,7 +1689,7 @@ void otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
   upload_async(ctx, U.grp, U.groups.data(), G);
   CK(cudaStreamSynchronize(ctx->stream));
   U.gbits = gbits; U.kbits = gbits + rbits;
-  U.min_id = o->min_id; U.min_cov = o->min_cov;
+  U.min_id = o->min_id; U.min_cov = o->min_cov; U.feed = (uint32_t)o->feed;
   U.n = 0; U.pool_bytes = 0;
   for (double& t : U.t) t = 0;
   U.gen = ctx->parts_gen;
@@ -1700,14 +1702,16 @@ uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr
   auto& U = ctx->otu;
   otu_open(ctx);
   if (nreads && (!results || !alns || !stats)) fail(SMR_ERR_ARG, "the OTU map needs the results, alignments and smr_aln_stats of the batch");
-  if (!text && ctx->resident_mates) fail(SMR_ERR_UNSUPPORTED, "the OTU map of two mate files (a mate stream's batch) is not written on the device");
+  if (!text && ctx->resident_mates && U.feed != SMR_OTU_TWO_FILES)
+    fail(SMR_ERR_UNSUPPORTED, "a mate stream's batch is two mate files: open the OTU map with feed SMR_OTU_TWO_FILES");
+  if (U.feed != SMR_OTU_SINGLE && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
   const uint32_t slots = slots_of(ctx);
   const uint64_t N = (uint64_t)nreads * slots;
   if (N >= (1ull << 31)) fail(SMR_ERR_ARG, "batch too large for the OTU map: split it");
   cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
   CK(cudaEventRecord(e0, ctx->stream));
   const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e1);
-  const OtuArgs oa{(const uint32_t*)U.rank.p, (const uint32_t*)U.rank_off.p, U.gbits, U.min_id, U.min_cov};
+  const OtuArgs oa{(const uint32_t*)U.rank.p, (const uint32_t*)U.rank_off.p, U.gbits, U.min_id, U.min_cov, U.feed};
   uint32_t* flag = ensure<uint32_t>(U.flag, (N + 1) * 4);
   uint32_t* pos = ensure<uint32_t>(U.pos, (N + 1) * 4);
   uint64_t* nsz = ensure<uint64_t>(U.nsz, (N + 1) * 8);
@@ -1782,6 +1786,42 @@ void otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) 
   float ms = 0;
   cudaEventElapsedTime(&ms, e0, e1); U.t[2] = ms;
   U.active = false;
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// De novo statistics (smr_otu.cuh, denovo_stats_kernel)
+// ---------------------------------------------------------------------------------------------------------------------
+void denovo_stats_impl(smr_ctx* ctx, const smr_denovo_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
+                       const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4]) {
+  if (nreads && (!results || !alns || !stats)) fail(SMR_ERR_ARG, "the denovo statistics need the results, alignments and smr_aln_stats of the batch");
+  const bool paired = o->paired || (!text && ctx->resident_mates);   // the resident batch of a mate stream is mates
+  const uint32_t slots = slots_of(ctx);
+  const uint64_t N = (uint64_t)nreads * slots;
+  if (N >= (1ull << 31)) fail(SMR_ERR_ARG, "batch too large for the denovo statistics: split it");
+  std::vector<RptGroup> hg;   // the loaded (index, part)s: an alignment of any other is refused
+  for (const Part* pt : report_groups(ctx)) { RptGroup g{}; g.index_num = pt->d.index_num; g.part = pt->d.part; hg.push_back(g); }
+  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
+  CK(cudaEventRecord(e0, ctx->stream));
+  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, hg, e1);
+  uint32_t* dread = ensure<uint32_t>(ctx->dn_read, ((size_t)nreads + 1) * 16);
+  unsigned long long* dtot = ensure<unsigned long long>(ctx->dn_tot, 32);
+  CK(cudaMemsetAsync(dread, 0, (size_t)nreads * 16, ctx->stream));
+  CK(cudaMemsetAsync(dtot, 0, 32, ctx->stream));
+  if (nreads) denovo_stats_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(a, o->min_id, o->min_cov, paired, dread, dtot);
+  CK(cudaGetLastError());
+  uint64_t tot[4] = {0, 0, 0, 0}; uint32_t err = 0;
+  CK(cudaMemcpyAsync(&err, (uint32_t*)ctx->d_scal.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e2, ctx->stream));
+  CK(cudaMemcpyAsync(tot, dtot, 32, cudaMemcpyDeviceToHost, ctx->stream));
+  if (per_read && nreads) CK(cudaMemcpyAsync(per_read, dread, (size_t)nreads * 16, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e3, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (err) rpt_error(err);
+  for (int k = 0; k < 4; ++k) totals[k] += tot[k];
+  float ms = 0;
+  cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
+  cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
+  cudaEventElapsedTime(&ms, e2, e3); ctx->t_rpt[2] = ms;
 }
 
 }  // namespace
@@ -2388,5 +2428,13 @@ int smr_last_otu_timings(const smr_ctx* ctx, double out[3]) {
   for (int k = 0; k < 3; ++k) out[k] = ctx->otu.t[k];
   return SMR_OK;
 }
+
+int smr_denovo_stats(smr_ctx* ctx, const smr_denovo_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
+                     const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4]) try {
+  if (!ctx || !opts || !totals || (!text && nbytes)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  denovo_stats_impl(ctx, opts, text, nbytes, results, alns, stats, nreads, per_read, totals);
+  return SMR_OK;
+} SMR_CATCH(ctx)
 
 }  // extern "C"

@@ -2,7 +2,9 @@
 the 8 stand-in databases, aligned once on the GPU, then the OTU map at -id / -coverage (0.97 / 0.97 by default).  Prints one JSON line:
   * device time of smr_otu_add (CUDA events: layout, rule, compaction, append) and its H2D of text + results; device time of
     smr_otu_finish (sort, sizes, scan, write, D2H); the wall time of begin + add + finish; the map's lines, entries and bytes;
-  * with --reference N, the reference binary's OTU stage ("OTU groups processing done in" of its log) on the first N reads, at -threads 1.
+  * the denovo leg: device time of smr_denovo_stats (per-read counters and totals, CUDA events) per 1 M reads;
+  * with --reference N, the reference binary's OTU stage ("OTU groups processing done in" of its log) and its denovo_stats pass
+    ("done Denovo stats in") on the first N reads, at -threads 1.
 Run on the GPU:  python tools/bench_otu.py --reads 1000000 --reference 20000"""
 import argparse
 import json
@@ -59,6 +61,17 @@ def main():
                           add_h2d_ms=med(lambda t, w: t["add_h2d_ms"]), add_device_ms=med(lambda t, w: t["add_device_ms"]),
                           finish_ms=med(lambda t, w: t["finish_ms"]), wall_ms=med(lambda t, w: w * 1e3))
         out["otu"]["device_ms_per_1m_reads"] = (out["otu"]["add_device_ms"] + out["otu"]["finish_ms"]) * 1e6 / args.reads
+        dn = []
+        for rep in range(args.reps + 1):
+            t0 = time.perf_counter()
+            _, tot = al.denovo_stats(res, None, args.id, args.coverage)
+            wall = time.perf_counter() - t0
+            if rep:
+                dn.append((al.report_timings(), wall))
+        dmed = lambda f: float(np.median([f(t, w) for t, w in dn]))   # noqa: E731
+        out["denovo"] = dict(totals=tot, h2d_ms=dmed(lambda t, w: t["h2d_ms"]), device_ms=dmed(lambda t, w: t["device_ms"]),
+                             d2h_ms=dmed(lambda t, w: t["d2h_ms"]), wall_ms=dmed(lambda t, w: w * 1e3))
+        out["denovo"]["device_ms_per_1m_reads"] = out["denovo"]["device_ms"] * 1e6 / args.reads
         al.close()
         if args.reference:
             from oracle import ora
@@ -74,8 +87,11 @@ def main():
                 mt = re.search(r"OTU groups processing done in ([0-9.eE+-]+) sec", r["stdout"])
                 sec = float(mt.group(1)) if mt else None
                 mo = re.search(r"Total OTUs = (\d+)", r["log"])
+                md = re.search(r"done Denovo stats in ([0-9.eE+-]+) sec", r["stdout"])
+                dsec = float(md.group(1)) if md else None
                 out["reference"] = dict(reads=k, threads=1, otu_stage_s=sec, reads_s=k / sec if sec else None,
-                                        total_otu=int(mo.group(1)) if mo else None)
+                                        total_otu=int(mo.group(1)) if mo else None, denovo_stats_s=dsec,
+                                        denovo_reads_s=k / dsec if dsec else None)
     print(json.dumps(out))
 
 
