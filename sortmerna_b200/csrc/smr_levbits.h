@@ -62,6 +62,28 @@ SMR_HD bool within_one_edit(uint32_t P, uint32_t T, const LevMasks& k) {
   const uint32_t a8 = (A9 & k.m8) | k.s8, a9 = A9 | k.s9;
   return ((A9 & (A9 - 1u)) == 0u) | (B8 < (a8 & (0u - a8))) | (C9 < (a9 & (0u - a9)));
 }
+// The streaming screen of the seed kernel, about half the instructions of within_one_edit.  With h = pw/2, a text within
+// one edit of P (an edit at position j, or none) passes at least one of four exact comparisons:
+//   lo:  t_i = p_i     for i in [0, h)       no edit, or an edit at j >= h
+//   hi:  t_i = p_i     for i in [h, pw)      substitution at j < h
+//   del: t_i = p_{i+1} for i in [h, pw-1)    deletion at j < h
+//   ins: t_{i+1} = p_i for i in [h, pw)      insertion at j < h
+// each one masked XOR tested against zero, with P, P >> 2 and P << 2 (the shifted patterns are computed once per pattern).
+// It only screens: some texts that pass are not within one edit, and (classify_bits & 3) != 0 decides
+// (tests/seed_filter_check.cpp proves both on every pw the flattener accepts).
+struct HalfMasks { uint32_t lo, hi, del, ins; };
+SMR_HD uint32_t char_bits(uint32_t a, uint32_t b) {  // the bits of characters [a, b), 0 <= a <= b <= 16 (b = 16: no 32-bit shift)
+  return (uint32_t)((1ull << (2 * b)) - 1ull) & ~(uint32_t)((1ull << (2 * a)) - 1ull);
+}
+SMR_HD HalfMasks half_masks(uint32_t pw) {
+  const uint32_t h = pw / 2;
+  return HalfMasks{char_bits(0, h), char_bits(h, pw), char_bits(h, pw - 1), char_bits(h + 1, pw + 1)};
+}
+// Pd = P >> 2, Pi = P << 2
+SMR_HD bool half_screen(uint32_t P, uint32_t Pd, uint32_t Pi, uint32_t T, const HalfMasks& m) {
+  const uint32_t x = T ^ P;
+  return ((x & m.lo) == 0u) | ((x & m.hi) == 0u) | (((T ^ Pd) & m.del) == 0u) | (((T ^ Pi) & m.ins) == 0u);
+}
 // is the k-character prefix of T within one edit of SOME prefix of P (the automaton is not in its dead state)?  1 <= k <= pw-1
 SMR_HD bool viable_bits(uint32_t P, uint32_t T, uint32_t k) {
   const uint32_t Ak = neq2(T ^ P) & mk2(k);
