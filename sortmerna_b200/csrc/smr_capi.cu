@@ -93,12 +93,20 @@ struct StreamSide {
 };
 
 // The read stream of a context (smr_stream_begin .. smr_stream_next): one file, or two mate files (SMR_STREAM_MATES) whose
-// records k are paired.  Their buffers belong to it.
+// records k are paired.  Their buffers belong to it; its scratch outlives it (close_stream).
 struct ReadStream {
   bool open = false, gz = false, count_only = false, mates = false;
   uint64_t batch_bytes = 0;
   StreamSide side[2];          // side[1]: mate 2 of a mate stream
   CountState counts;
+  struct Scratch { DevBuf rc, cut, mflag, mend[2]; } scr;   // count-pass partials, batch cut; mate stream: record flags, record ends per mate
+};
+
+// The device words that the text passes hand to the host, one buffer.  Each group belongs to the function named, which zeroes it.
+struct TextWords {
+  uint32_t nrec, seq_bytes, err;   // text_layout: records, sequence bytes, decode error bits
+  uint32_t pk_words, max_len;      // upload_fastx_impl: packed words of the batch, its longest read
+  uint32_t rpt_err;                // rpt_prologue: the report side's error bits (RptArgs::err)
 };
 
 }  // namespace
@@ -117,37 +125,34 @@ struct smr_ctx {
   uint32_t all_slots = 16;       // stride of the result layout when num_alignments == 0 (smr_set_aln_slots)
   uint32_t lis_ctas_per_sm = kLisMinCtas;   // persistent CTAs of the candidate kernel per SM (matches its __launch_bounds__)
 
-  Batch resident;
-  // scratch of a run that no later call reads, sized by the scale of the run
-  DevBuf parts_dev, lis_arena, lis_epochs, lis_queue, lis_done, lis_rows, lis_dbg, final_arena, lane_hits, tb_arena, tb_jobs, fin_list;
+  // the resident batch and the text it was decoded from (smr_upload_*, smr_stream_next); clear_resident empties it
+  struct Resident {
+    Batch b;
+    DevBuf text, hdroff;      // the text (smr_upload_fastx[_gz], a stream's batch) and each record's header offset in it (smr_decode.cuh)
+    uint64_t text_bytes = 0;  // 0: no text behind the batch
+    bool mates = false;       // the batch came from a mate stream: records 2k and 2k+1 are mates
+  } res;
+  // scratch of a run that no later call reads, sized by the scale of the run (setup_arenas)
+  struct { DevBuf parts, seed_ctr, lis, lis_epochs, lis_queue, lis_done, lis_rows, lis_dbg, fin, lane_hits, tb, tb_jobs, fin_list; } run;
   smr_aln_stats* host_stats = nullptr;   // optional output of the report arithmetic
-  PinBuf h_state, h_flags, h_hitdb, h_outaln, h_stats, h_cigar, h_off32, h_pkoff;
-  std::vector<uint64_t> h_coff;
-  DevBuf d_text, d_hdroff;   // input decode (smr_decode.cuh)
-  DevBuf d_cnt, d_scal, d_nl, d_hdr, d_sb, d_rec, d_spos;   // line layout of a text (text_layout), for the decode and the report writer
+  // page-locked staging of a download (download_impl) and of the host read layout (read_layout, upload_fastx_impl)
+  struct { PinBuf state, flags, hitdb, outaln, stats, cigar, off32, pkoff; std::vector<uint64_t> coff; } h;
+  // the line layout of the last text (text_layout, newline_index), read by the decode, the read stream and the report writer; cnt
+  // holds the per-chunk newline counts, and then the decode's per-record packed-word counts; words holds the TextWords
+  struct { DevBuf cnt, words, nl, hdr, sb, rec, spos; } tx;
   DevBuf cub_tmp;   // cub scratch of the text layout, the report writer and the OTU map
-  DevBuf seed_ctr, d_gz, d_cand, d_res, d_sym, d_win, d_ids, d_off, d_cnt64, d_moff, d_mem, d_poff, d_plen, d_pcrc;   // gz inflate (smr_inflate.cuh)
-  uint64_t text_bytes = 0;          // size of the text behind the resident batch (smr_upload_fastx / _gz)
-  DevBuf d_rc, d_cut, d_mflag, d_mend[2];   // read stream: count-pass partials, batch cut; mate stream: record flags, record ends per mate
+  // gz inflate scratch (inflate_round, smr_inflate.cuh) and what the last round found
+  struct { DevBuf gz, cand, res, sym, win, ids, off, cnt, moff, mem, poff, plen, pcrc; uint32_t spans = 0, candidates = 0; } inf;
   ReadStream rs;
-  bool resident_mates = false;      // the resident batch came from a mate stream: records 2k and 2k+1 are mates
-  uint32_t inf_spans = 0, inf_candidates = 0; double t_inflate = 0;
-  double t_decode = 0;
-  uint32_t tb_threads = 0, tb_cap_w = 0, tb_cap_cig = 0; size_t tb_cap_dir = 0, tb_stride = 0;
-  uint32_t lis_warps = 0, final_warps = 0;
-  size_t lis_stride = 0, final_stride = 0;
-  uint32_t hist_cap = 0, cand_cap = 0, pair_cap = 0, row_cap = 0, pall_cap = 0, task_cap = 0, cap_w = 0, cap_cig = 0; size_t cap_dir = 0;
-  uint32_t lis_ctas = 0;
-  uint32_t lane_hits_cap = 0, lane_hits_warps = 0;
+  double t_inflate = 0, t_decode = 0;
   bool instr = false;         // smr_set_instrumentation: seed kernel counts windows / lists / entries, candidate kernel accounts its phases (clock64)
   uint64_t flag_hist[6] = {0, 0, 0, 0, 0, 0};  // overflow causes seen so far (seed lane / seed region / pairs / trace / cigar / error)
-  // report writer (smr_report.cuh)
+  // report writer (smr_report.cuh): scoring tables per index_num (smr_set_report_scoring), scratch (rpt_prologue, format_reports_impl)
   struct RptScore { bool set = false; DevBuf ev, bits; };
-  std::vector<RptScore> rpt_score;   // per index_num (smr_set_report_scoring)
-  DevBuf r_text, r_line, r_recs, r_res, r_aln, r_cig, r_st, r_flags, r_keys, r_keys2, r_vals, r_rows, r_first,
-         r_sz, r_off, r_bsz, r_boff, r_fxsz, r_fxoff, r_grp, r_so, r_out;
+  std::vector<RptScore> rpt_score;
+  struct { DevBuf text, line, recs, res, aln, cig, st, flags, keys, keys2, vals, rows, first, sz, off, bsz, boff, fxsz, fxoff, grp, so, out; } r;
   double t_rpt[3] = {0, 0, 0};
-  DevBuf z_in, z_chunk, z_m, z_freq, z_codes, z_hdr, z_info, z_scratch, z_poff, z_plen, z_crc, z_dst, z_trl, z_out;   // gzip deflate (smr_deflate.cuh)
+  struct { DevBuf in, chunk, m, freq, codes, hdr, info, scratch, poff, plen, crc, dst, trl, out; } z;   // gzip deflate (gzip_streams, smr_deflate.cuh)
   uint64_t parts_gen = 0;   // bumped whenever a part is loaded or its report ids are set: an open OTU map refuses to go on after that
   // OTU map accumulator (smr_otu.cuh), smr_otu_begin .. smr_otu_finish
   struct Otu {
@@ -157,7 +162,7 @@ struct smr_ctx {
     uint64_t n = 0, pool_bytes = 0;
     double t[3] = {0, 0, 0};
   } otu;
-  DevBuf dn_read, dn_tot;   // smr_denovo_stats: per-read counters, totals
+  struct { DevBuf read, tot; } dn;   // smr_denovo_stats: per-read counters, totals
   // timings
   std::vector<cudaEvent_t> ev;
   RunTimes t_run;   // the last run, and the retries of its download
@@ -192,6 +197,33 @@ T* ensure(Buf<kPinned>& b, size_t bytes) {
   if (bytes > b.cap || !b.p) CK(b.alloc(bytes + bytes / 8 + 256));
   return (T*)b.p;
 }
+
+// grow-only as ensure, keeping the first `keep` bytes
+void ensure_keep(smr_ctx* ctx, DevBuf& b, size_t bytes, size_t keep) {
+  if (bytes <= b.cap && b.p) return;
+  DevBuf n;
+  CK(n.alloc(bytes + bytes / 8 + 256));
+  if (keep) {
+    CK(cudaMemcpyAsync(n.p, b.p, keep, cudaMemcpyDeviceToDevice, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  b = std::move(n);   // n frees the old buffer
+}
+
+// n items from the host to b (grown as needed), queued on the context's stream
+template <class T>
+void upload_async(smr_ctx* ctx, DevBuf& b, const T* src, size_t n) {
+  ensure(b, n * sizeof(T) + 16);
+  if (n) CK(cudaMemcpyAsync(b.p, src, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
+}
+
+// the context's first n events (created on first use), for the timings of one function: none is held across a call that takes its own
+cudaEvent_t* events(smr_ctx* ctx, size_t n) {
+  for (cudaEvent_t e; ctx->ev.size() < n; ctx->ev.push_back(e)) CK(cudaEventCreate(&e));
+  return ctx->ev.data();
+}
+
+double elapsed_ms(cudaEvent_t a, cudaEvent_t b) { float ms = 0; cudaEventElapsedTime(&ms, a, b); return ms; }
 
 // a device array of the part: n items, copied from src (host) or else zero, and 64 zero bytes of slack past the end; counted in pt.bytes
 template <class T>
@@ -357,11 +389,6 @@ DevParams to_dev(const smr_params& p) {
 
 uint32_t pow2_ge(uint32_t v) { uint32_t p = 1; while (p < v) p <<= 1; return p; }
 
-cudaEvent_t get_event(smr_ctx* ctx, size_t i) {
-  while (ctx->ev.size() <= i) { cudaEvent_t e; cudaEventCreate(&e); ctx->ev.push_back(e); }
-  return ctx->ev[i];
-}
-
 // scalars block layout (u32): [0]=work_n [1]=lis work_next [2]=final work_next [3]=lis work_next of the second cursor ; cigar_used (u64) at byte 16 ;
 // finalize job count (u32) at byte 24 ; task queue cursors at 128..
 struct Scalars { uint32_t* work_n; uint32_t* lis_next; uint32_t* fin_next; uint32_t* lis_next_b; unsigned long long* cigar_used; uint32_t* fin_jobs; uint32_t* q_head; uint32_t* q_tail; uint32_t* planners_done; };
@@ -370,58 +397,73 @@ Scalars scalars_of(const Batch& b) {
   return Scalars{(uint32_t*)p, (uint32_t*)(p + 4), (uint32_t*)(p + 8), (uint32_t*)(p + 12), (unsigned long long*)(p + 16), (uint32_t*)(p + 24), (uint32_t*)(p + 128), (uint32_t*)(p + 256), (uint32_t*)(p + 384)};
 }
 
-void setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
+// the arenas of a run as the kernels see them: the chunk-independent parts of LisGlobals and FinalGlobals, and the launch sizes
+struct RunGeom {
+  LisGlobals lg{};
+  FinalGlobals fg{};
+  uint32_t lis_ctas = 0, lis_warps = 0, final_warps = 0, tb_threads = 0, seed_ctas = 0, lane_hits_cap = 0;
+};
+
+RunGeom setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
+  auto& A = ctx->run;
+  RunGeom g;
+  LisGlobals& lg = g.lg; FinalGlobals& fg = g.fg;
   uint32_t max_nref = 1;
   for (auto& pt : ctx->parts) max_nref = std::max(max_nref, pt.d.nref);
-  ctx->hist_cap = max_nref;
-  ctx->cand_cap = std::max(64u, max_nref);
-  ctx->pair_cap = pow2_ge(4096u * scale);
-  ctx->task_cap = 2 * ctx->pair_cap;
+  lg.hist_cap = max_nref;
+  lg.cand_cap = std::max(64u, max_nref);
+  lg.pair_cap = pow2_ge(4096u * scale);
+  lg.task_cap = 2 * lg.pair_cap;
   // SW windows are at most read length + 2 * edges columns (alignment.cpp:272-357; edges may be a percentage of the read)
   const uint32_t edges = ctx->prm.edges_is_percent ? (uint32_t)((ctx->prm.edges / 100.0) * (double)max_len) : (uint32_t)std::max(0, ctx->prm.edges);
-  ctx->row_cap = max_len + 2 * edges + 2 * 64 + 64;
+  lg.row_cap = max_len + 2 * edges + 2 * 64 + 64;
   // planner and scorer warps wait for each other: EVERY CTA of the grid must be resident at once
   int occ = 0;
   CK(cudaFuncSetAttribute(lis_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLisSmemBytes));
   CK(cudaFuncSetAttribute(lis_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLisSmemBytes));
   CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lis_kernel<true>, kLisWarpsPerCta * 32, kLisSmemBytes));   // (same launch bounds and shared memory for both)
   if (occ < 1) fail(SMR_ERR_CUDA, "lis_kernel does not fit on an SM");
-  ctx->lis_ctas = (uint32_t)ctx->sm_count * std::min<uint32_t>(ctx->lis_ctas_per_sm, (uint32_t)occ);
-  ctx->lis_warps = ctx->lis_ctas * kPlannerWarps;   // planner warps (each owns an arena)
-  ctx->pall_cap = 32768u * scale;
-  ctx->lis_stride = lis_arena_bytes(ctx->hist_cap, ctx->cand_cap, ctx->pair_cap, ctx->task_cap, ctx->pall_cap);
+  g.lis_ctas = (uint32_t)ctx->sm_count * std::min<uint32_t>(ctx->lis_ctas_per_sm, (uint32_t)occ);
+  g.lis_warps = g.lis_ctas * kPlannerWarps;   // planner warps (each owns an arena)
+  lg.pall_cap = 32768u * scale;
+  lg.arena_stride = lis_arena_bytes(lg.hist_cap, lg.cand_cap, lg.pair_cap, lg.task_cap, lg.pall_cap);
   // keep the arena total under ~16 GB (of the 80 GB of an H100): fewer persistent CTAs for huge reference sets
   const size_t budget = (size_t)16 << 30;
-  while (ctx->lis_ctas > 16 && ctx->lis_stride * ctx->lis_warps > budget) { ctx->lis_ctas /= 2; ctx->lis_warps = ctx->lis_ctas * kPlannerWarps; }
-  ensure(ctx->lis_arena, ctx->lis_stride * ctx->lis_warps);
-  ensure(ctx->lis_epochs, (size_t)ctx->lis_warps * 4);
-  ensure(ctx->lis_queue, (size_t)2 * kQueueCap * sizeof(QSlot) + 64);
-  ensure(ctx->lis_done, (size_t)ctx->lis_warps * 4 + 64);
+  while (g.lis_ctas > 16 && lg.arena_stride * g.lis_warps > budget) { g.lis_ctas /= 2; g.lis_warps = g.lis_ctas * kPlannerWarps; }
+  lg.arena_base = ensure<uint8_t>(A.lis, lg.arena_stride * g.lis_warps);
+  lg.epochs = ensure<uint32_t>(A.lis_epochs, (size_t)g.lis_warps * 4);
+  lg.ring = ensure<QSlot>(A.lis_queue, (size_t)2 * kQueueCap * sizeof(QSlot) + 64);
+  lg.done = ensure<uint32_t>(A.lis_done, (size_t)g.lis_warps * 4 + 64);
   const size_t dbg_bytes = (size_t)(kTlBase + kTlRows * kTlBuckets) * 8;
-  ensure(ctx->lis_dbg, dbg_bytes);
-  CK(cudaMemsetAsync(ctx->lis_dbg.p, 0, dbg_bytes, ctx->stream));
-  ensure(ctx->lis_rows, (size_t)ctx->lis_ctas * kScorerWarps * 2 * ctx->row_cap * 4);
+  ensure(A.lis_dbg, dbg_bytes);
+  CK(cudaMemsetAsync(A.lis_dbg.p, 0, dbg_bytes, ctx->stream));
+  // (the timeline costs the instrumented kernel an atomic per scored pair)
+  lg.dbg = (getenv("SMR_TIMELINE") || getenv("SMR_VERBOSE")) ? (unsigned long long*)A.lis_dbg.p : nullptr;
+  lg.score_rows = ensure<int32_t>(A.lis_rows, (size_t)g.lis_ctas * kScorerWarps * 2 * lg.row_cap * 4);
   // histogram epochs start at 0 over a zeroed histogram (every run: the arena layout depends on the scale of the run)
-  CK(cudaMemset2DAsync(ctx->lis_arena.p, ctx->lis_stride, 0, lis_arena_zero_bytes(ctx->hist_cap), ctx->lis_warps, ctx->stream));   // votes + bitmaps only
-  CK(cudaMemsetAsync(ctx->lis_epochs.p, 0, (size_t)ctx->lis_warps * 4, ctx->stream));
-  ctx->cap_w = 2 * 256 * scale + 8;          // band widths up to 256*scale
-  ctx->cap_cig = 2 * (max_len + 64) + 16;
-  ctx->cap_dir = (size_t)65536 * scale + (size_t)max_len * 9 * 3 + 64;
-  ctx->final_warps = (uint32_t)ctx->sm_count * kFinalCtasPerSm * kFinalWarpsPerCta;
-  ctx->final_stride = final_arena_bytes(ctx->cap_w, ctx->cap_cig, ctx->row_cap, ctx->cap_dir);
-  while (ctx->final_warps > 64 && ctx->final_stride * ctx->final_warps > budget) ctx->final_warps /= 2;
-  ensure(ctx->final_arena, ctx->final_stride * ctx->final_warps);
+  CK(cudaMemset2DAsync(A.lis.p, lg.arena_stride, 0, lis_arena_zero_bytes(lg.hist_cap), g.lis_warps, ctx->stream));   // votes + bitmaps only
+  CK(cudaMemsetAsync(A.lis_epochs.p, 0, (size_t)g.lis_warps * 4, ctx->stream));
+  fg.cap_w = 2 * 256 * scale + 8;          // band widths up to 256*scale
+  fg.cap_cig = 2 * (max_len + 64) + 16;
+  fg.row_cap = lg.row_cap;
+  fg.cap_dir = (size_t)65536 * scale + (size_t)max_len * 9 * 3 + 64;
+  g.final_warps = (uint32_t)ctx->sm_count * kFinalCtasPerSm * kFinalWarpsPerCta;
+  fg.arena_stride = final_arena_bytes(fg.cap_w, fg.cap_cig, fg.row_cap, fg.cap_dir);
+  while (g.final_warps > 64 && fg.arena_stride * g.final_warps > budget) g.final_warps /= 2;
+  fg.arena_base = ensure<uint8_t>(A.fin, fg.arena_stride * g.final_warps);
   // traceback stage: one thread per alignment, 1024 threads per SM
-  ctx->tb_threads = (uint32_t)ctx->sm_count * 1024u;
-  ctx->tb_cap_w = 2 * 32 * scale + 8;                       // band widths up to 32*scale
-  ctx->tb_cap_cig = 128 * scale;
-  ctx->tb_cap_dir = (size_t)32768 * scale;                  // (2*band+1) * readLen * 3 bytes: band 32 at 150 nt
-  ctx->tb_stride = ((size_t)ctx->tb_cap_w * 12 + (size_t)ctx->tb_cap_cig * 4 + ctx->tb_cap_dir + 255) & ~(size_t)255;
-  while (ctx->tb_threads > 4096 && ctx->tb_stride * ctx->tb_threads > budget) ctx->tb_threads /= 2;
-  ensure(ctx->tb_arena, ctx->tb_stride * ctx->tb_threads);
-  ctx->lane_hits_cap = kLaneHitCap * scale;
-  ctx->lane_hits_warps = scale == 1 ? (uint32_t)ctx->sm_count * kSeedCtasPerSm * kSeedWarpsPerCta : 1024u;
-  ensure(ctx->lane_hits, (size_t)ctx->lane_hits_warps * ctx->lane_hits_cap * 32 * 4);
+  g.tb_threads = (uint32_t)ctx->sm_count * 1024u;
+  fg.tb_cap_w = 2 * 32 * scale + 8;                       // band widths up to 32*scale
+  fg.tb_cap_cig = 128 * scale;
+  fg.tb_cap_dir = (size_t)32768 * scale;                  // (2*band+1) * readLen * 3 bytes: band 32 at 150 nt
+  fg.tb_stride = ((size_t)fg.tb_cap_w * 12 + (size_t)fg.tb_cap_cig * 4 + fg.tb_cap_dir + 255) & ~(size_t)255;
+  while (g.tb_threads > 4096 && fg.tb_stride * g.tb_threads > budget) g.tb_threads /= 2;
+  fg.tb_arena = ensure<uint8_t>(A.tb, fg.tb_stride * g.tb_threads);
+  g.lane_hits_cap = kLaneHitCap * scale;
+  const uint32_t lane_hits_warps = scale == 1 ? (uint32_t)ctx->sm_count * kSeedCtasPerSm * kSeedWarpsPerCta : 1024u;
+  g.seed_ctas = lane_hits_warps / kSeedWarpsPerCta;
+  ensure(A.lane_hits, (size_t)lane_hits_warps * g.lane_hits_cap * 32 * 4);
+  return g;
 }
 
 // the reads c0 .. c0 + n of a batch as the kernels see them
@@ -443,8 +485,8 @@ DevBatch make_batch(const Batch& s, uint32_t c0, uint32_t n) {
 // are staged in the context's pinned buffers: the caller synchronizes before the next layout.
 template <class Len>
 uint64_t read_layout(smr_ctx* ctx, Batch& b, uint32_t n, Len len) {
-  uint32_t* pkoff = ensure<uint32_t>(ctx->h_pkoff, (size_t)(n + 1) * 4);
-  uint32_t* off32 = ensure<uint32_t>(ctx->h_off32, (size_t)(n + 1) * 4);
+  uint32_t* pkoff = ensure<uint32_t>(ctx->h.pkoff, (size_t)(n + 1) * 4);
+  uint32_t* off32 = ensure<uint32_t>(ctx->h.off32, (size_t)(n + 1) * 4);
   uint64_t total = 0, w = 0; uint32_t max_len = 0;
   for (uint32_t r = 0; r <= n; ++r) {
     off32[r] = (uint32_t)total;
@@ -458,10 +500,8 @@ uint64_t read_layout(smr_ctx* ctx, Batch& b, uint32_t n, Len len) {
   }
   if (total >= 0xF0000000ull) fail(SMR_ERR_ARG, "batch larger than 2^32 nucleotides: split it");
   if (w >= 0xFFFFFFFFull) fail(SMR_ERR_ARG, "batch too large");
-  ensure(b.seq_off, (size_t)(n + 1) * 4);
-  ensure(b.pk_off, (size_t)(n + 1) * 4);
-  CK(cudaMemcpyAsync(b.seq_off.p, off32, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(b.pk_off.p, pkoff, (size_t)(n + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+  upload_async(ctx, b.seq_off, off32, n + 1);
+  upload_async(ctx, b.pk_off, pkoff, n + 1);
   b.off32.assign(off32, off32 + n + 1);
   b.nreads = n; b.total_nt = total; b.max_len = max_len;
   return w;
@@ -502,20 +542,26 @@ void finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
   CK(cudaGetLastError());
 }
 
+// an empty resident batch with no text behind it
+void clear_resident(smr_ctx* ctx) {
+  auto& R = ctx->res;
+  R.b.nreads = 0; R.b.from_text = false; R.text_bytes = 0; R.mates = false;
+}
+
 // host reads -> the resident batch (no text behind it)
 void upload_batch_impl(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads) {
-  Batch& b = ctx->resident;
-  b.nreads = 0; b.from_text = false; ctx->text_bytes = 0; ctx->resident_mates = false;
+  clear_resident(ctx);
   if (nreads == 0) return;
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
-  CK(cudaEventRecord(e0, ctx->stream));
+  Batch& b = ctx->res.b;
+  cudaEvent_t* e = events(ctx, 2);
+  CK(cudaEventRecord(e[0], ctx->stream));
   const uint64_t w = read_layout(ctx, b, nreads, [&](uint32_t r) { return seq_off[r + 1] - seq_off[r]; });
   ensure(b.seq04, b.total_nt + 64);
   CK(cudaMemcpyAsync(b.seq04.p, seq_cat + seq_off[0], b.total_nt, cudaMemcpyHostToDevice, ctx->stream));
   finish_upload(ctx, b, w);
-  CK(cudaEventRecord(e1, ctx->stream));
+  CK(cudaEventRecord(e[1], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_h2d = ms;
+  ctx->t_h2d = elapsed_ms(e[0], e[1]);
 }
 
 // exclusive sum of n u32 (out may equal in) in the context's cub scratch
@@ -523,111 +569,116 @@ void exclusive_sum(smr_ctx* ctx, const uint32_t* in, uint32_t* out, uint32_t n) 
   cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, in, out, n, ctx->stream); });
 }
 
-// Newline positions of a text (smr_decode.cuh (1)-(3)) in d_nl: count per 32-byte chunk, scan (the total lands at [nchunks]),
+// Newline positions of a text (smr_decode.cuh (1)-(3)) in tx.nl: count per 32-byte chunk, scan (the total lands at [nchunks]),
 // positions.  A text that does not end in '\n' gets a virtual one at nbytes.  Returns their number.
 uint32_t newline_index(smr_ctx* ctx, const uint8_t* text, uint64_t nbytes) {
+  auto& X = ctx->tx;
   const int grid = ctx->sm_count * 8;
   const uint64_t nchunks = nbytes / 32 + 1;
-  uint32_t* cnt = ensure<uint32_t>(ctx->d_cnt, (nchunks + 1) * 4);
+  uint32_t* cnt = ensure<uint32_t>(X.cnt, (nchunks + 1) * 4);
   count_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks);
   CK(cudaMemsetAsync(cnt + nchunks, 0, 4, ctx->stream));
   exclusive_sum(ctx, cnt, cnt, (uint32_t)nchunks + 1);
   uint32_t n = 0;
   CK(cudaMemcpyAsync(&n, cnt + nchunks, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  ensure(ctx->d_nl, ((size_t)n + 1) * 8);
-  if (n) write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks, (uint64_t*)ctx->d_nl.p);
+  ensure(X.nl, ((size_t)n + 1) * 8);
+  if (n) write_newlines_kernel<<<grid, 256, 0, ctx->stream>>>(text, nbytes, cnt, nchunks, (uint64_t*)X.nl.p);
   CK(cudaGetLastError());
   return n;
 }
 
+TextWords* text_words(smr_ctx* ctx) { return ensure<TextWords>(ctx->tx.words, 64); }
+
 struct TextLayout { uint32_t nlines = 0, nrec = 0, total_nt = 0; uint32_t fmt = kFmtFasta; };
 
 // The line layout of a FASTA / FASTQ text on the device (the line passes of smr_decode.cuh), for the decode and the report writer.
-// first_byte is text[0] and names the format.  Leaves, for each of the nlines lines, its newline position (d_nl), header flag
-// (d_hdr), sequence bytes (d_sb), record index (d_rec) and the offset of its sequence bytes (d_spos); the arrays hold nlines + 1
-// items, d_rec and d_spos the totals at [nlines].  d_scal is zeroed; its words from [4] on are the caller's.
+// first_byte is text[0] and names the format.  Leaves in ctx->tx, for each of the nlines lines, its newline position (nl), header
+// flag (hdr), sequence bytes (sb), record index (rec) and the offset of its sequence bytes (spos); the arrays hold nlines + 1 items,
+// rec and spos the totals at [nlines].
 TextLayout text_layout(smr_ctx* ctx, const uint8_t* text, uint64_t nbytes, char first_byte) {
+  auto& X = ctx->tx;
   TextLayout L;
   if (nbytes >= 0xF0000000ull) fail(SMR_ERR_ARG, "text batch of 2^32 bytes or more: split it (line counts and sequence offsets are 32-bit on the device)");
   if (nbytes && first_byte != '@' && first_byte != '>') fail(SMR_ERR_ARG, "reads text must start with '@' (FASTQ) or '>' (FASTA)");
   L.fmt = first_byte == '@' ? kFmtFastq : kFmtFasta;
-  uint32_t* scal = ensure<uint32_t>(ctx->d_scal, 64);   // [1] records [2] sequence bytes [3] decode error
-  CK(cudaMemsetAsync(scal, 0, 64, ctx->stream));
+  TextWords* tw = text_words(ctx);
+  CK(cudaMemsetAsync(tw, 0, offsetof(TextWords, pk_words), ctx->stream));   // nrec, seq_bytes, err
   const int grid = ctx->sm_count * 8;
   L.nlines = newline_index(ctx, text, nbytes);
   const uint32_t n = L.nlines;
-  ensure(ctx->d_hdr, ((size_t)n + 1) * 4);
-  ensure(ctx->d_sb, ((size_t)n + 1) * 4);
-  ensure(ctx->d_rec, ((size_t)n + 1) * 4);
-  ensure(ctx->d_spos, ((size_t)n + 1) * 4);
+  uint32_t* hdr = ensure<uint32_t>(X.hdr, ((size_t)n + 1) * 4);
+  uint32_t* sb = ensure<uint32_t>(X.sb, ((size_t)n + 1) * 4);
+  uint32_t* rec = ensure<uint32_t>(X.rec, ((size_t)n + 1) * 4);
+  uint32_t* spos = ensure<uint32_t>(X.spos, ((size_t)n + 1) * 4);
   if (n == 0) return L;
-  uint32_t *hdr = (uint32_t*)ctx->d_hdr.p, *sb = (uint32_t*)ctx->d_sb.p, *rec = (uint32_t*)ctx->d_rec.p, *spos = (uint32_t*)ctx->d_spos.p;
   // per line: header flag and sequence bytes; their scans give the record of every line and the offset of its bytes
-  line_info_kernel<<<grid, 256, 0, ctx->stream>>>(text, (const uint64_t*)ctx->d_nl.p, n, L.fmt, hdr, sb, scal + 3);
+  line_info_kernel<<<grid, 256, 0, ctx->stream>>>(text, (const uint64_t*)X.nl.p, n, L.fmt, hdr, sb, &tw->err);
   CK(cudaMemsetAsync(hdr + n, 0, 4, ctx->stream));
   CK(cudaMemsetAsync(sb + n, 0, 4, ctx->stream));
   exclusive_sum(ctx, hdr, rec, n + 1);
   exclusive_sum(ctx, sb, spos, n + 1);
-  CK(cudaMemcpyAsync(scal + 1, rec + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
-  CK(cudaMemcpyAsync(scal + 2, spos + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
-  uint32_t h[8];
-  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&tw->nrec, rec + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  CK(cudaMemcpyAsync(&tw->seq_bytes, spos + n, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  TextWords h;
+  CK(cudaMemcpyAsync(&h, tw, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (h[3]) fail(SMR_ERR_ARG, h[3] & kDecBadHeader ? "reads text: a record does not start with its header character" : "reads text: FASTQ separator line '+' missing");
-  L.nrec = h[1]; L.total_nt = h[2];
+  if (h.err) fail(SMR_ERR_ARG, h.err & kDecBadHeader ? "reads text: a record does not start with its header character" : "reads text: FASTQ separator line '+' missing");
+  L.nrec = h.nrec; L.total_nt = h.seq_bytes;
   return L;
 }
 
 // FASTA / FASTQ text -> resident batch (smr_decode.cuh)
-// text == nullptr: the text is already in ctx->d_text (inflated on the device), first byte given.  Returns the number of reads.
+// text == nullptr: the text is already in ctx->res.text (inflated on the device), first byte given.  Returns the number of reads.
 uint32_t upload_fastx_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, char first_byte = 0) {
-  Batch& b = ctx->resident;
-  b.nreads = 0; b.from_text = true;
-  ctx->text_bytes = nbytes;
-  ctx->resident_mates = false;
+  clear_resident(ctx);
+  auto& R = ctx->res;
+  Batch& b = R.b;
+  const auto& X = ctx->tx;
+  b.from_text = true; R.text_bytes = nbytes;
   if (nbytes == 0) return 0;
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
-  CK(cudaEventRecord(e0, ctx->stream));
+  cudaEvent_t* e = events(ctx, 3);
+  CK(cudaEventRecord(e[0], ctx->stream));
   if (text) {
-    ensure(ctx->d_text, nbytes + 64);
-    CK(cudaMemcpyAsync(ctx->d_text.p, text, nbytes, cudaMemcpyHostToDevice, ctx->stream));
+    ensure(R.text, nbytes + 64);
+    CK(cudaMemcpyAsync(R.text.p, text, nbytes, cudaMemcpyHostToDevice, ctx->stream));
   }
-  CK(cudaEventRecord(e1, ctx->stream));
-  const uint8_t* dt = (const uint8_t*)ctx->d_text.p;
+  CK(cudaEventRecord(e[1], ctx->stream));
+  const uint8_t* dt = (const uint8_t*)R.text.p;
   const TextLayout L = text_layout(ctx, dt, nbytes, text ? text[0] : first_byte);
   const uint32_t nreads = L.nrec, total = L.total_nt;
   if (total >= 0xF0000000u) fail(SMR_ERR_ARG, "batch larger than 2^32 nucleotides: split it");
   if (nreads == 0) return 0;
   const int grid = ctx->sm_count * 8;
-  uint32_t* scal = (uint32_t*)ctx->d_scal.p;   // of text_layout; here [4] packed words [5] max_len
+  TextWords* tw = text_words(ctx);
   ensure(b.seq04, (size_t)total + 64);
   ensure(b.seq_off, (size_t)(nreads + 1) * 4);
   ensure(b.pk_off, (size_t)(nreads + 1) * 4);
-  ensure(ctx->d_hdroff, (size_t)nreads * 8);
-  scatter_lines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)ctx->d_nl.p, L.nlines, (const uint32_t*)ctx->d_hdr.p, (const uint32_t*)ctx->d_rec.p,
-                                                       (const uint32_t*)ctx->d_sb.p, (const uint32_t*)ctx->d_spos.p, (uint8_t*)b.seq04.p,
-                                                       (uint32_t*)b.seq_off.p, (uint64_t*)ctx->d_hdroff.p);
-  CK(cudaMemcpyAsync((uint32_t*)b.seq_off.p + nreads, scal + 2, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  ensure(R.hdroff, (size_t)nreads * 8);
+  scatter_lines_kernel<<<grid, 256, 0, ctx->stream>>>(dt, (const uint64_t*)X.nl.p, L.nlines, (const uint32_t*)X.hdr.p, (const uint32_t*)X.rec.p,
+                                                       (const uint32_t*)X.sb.p, (const uint32_t*)X.spos.p, (uint8_t*)b.seq04.p,
+                                                       (uint32_t*)b.seq_off.p, (uint64_t*)R.hdroff.p);
+  CK(cudaMemcpyAsync((uint32_t*)b.seq_off.p + nreads, &tw->seq_bytes, 4, cudaMemcpyDeviceToDevice, ctx->stream));
   // packed-word offsets and the longest read (what read_layout computes on the host); words[nreads] = 0, so pk_off[nreads] is the total
-  uint32_t* words = ensure<uint32_t>(ctx->d_cnt, (size_t)(nreads + 1) * 4);
+  uint32_t* words = ensure<uint32_t>(ctx->tx.cnt, (size_t)(nreads + 1) * 4);
   uint32_t* pk_off = (uint32_t*)b.pk_off.p;
-  record_words_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)b.seq_off.p, nreads, words, scal + 5);
+  CK(cudaMemsetAsync(&tw->max_len, 0, 4, ctx->stream));
+  record_words_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)b.seq_off.p, nreads, words, &tw->max_len);
   exclusive_sum(ctx, words, pk_off, nreads + 1);
-  CK(cudaMemcpyAsync(scal + 4, pk_off + nreads, 4, cudaMemcpyDeviceToDevice, ctx->stream));
-  ensure(ctx->h_off32, (size_t)(nreads + 1) * 4);
-  CK(cudaMemcpyAsync(ctx->h_off32.p, b.seq_off.p, (size_t)(nreads + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  uint32_t h[8];
-  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaEventRecord(e2, ctx->stream));
+  CK(cudaMemcpyAsync(&tw->pk_words, pk_off + nreads, 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  ensure(ctx->h.off32, (size_t)(nreads + 1) * 4);
+  CK(cudaMemcpyAsync(ctx->h.off32.p, b.seq_off.p, (size_t)(nreads + 1) * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  TextWords h;
+  CK(cudaMemcpyAsync(&h, tw, sizeof h, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e[2], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  const uint32_t* off32 = (const uint32_t*)ctx->h_off32.p;
+  const uint32_t* off32 = (const uint32_t*)ctx->h.off32.p;
   b.off32.assign(off32, off32 + nreads + 1);
-  b.nreads = nreads; b.total_nt = total; b.max_len = h[5];
-  finish_upload(ctx, b, h[4]);
+  b.nreads = nreads; b.total_nt = total; b.max_len = h.max_len;
+  finish_upload(ctx, b, h.pk_words);
   CK(cudaStreamSynchronize(ctx->stream));
-  float ms = 0; cudaEventElapsedTime(&ms, e0, e1); if (text) ctx->t_h2d = ms;
-  cudaEventElapsedTime(&ms, e1, e2); ctx->t_decode = ms;
+  if (text) ctx->t_h2d = elapsed_ms(e[0], e[1]);
+  ctx->t_decode = elapsed_ms(e[1], e[2]);
   return nreads;
 }
 
@@ -645,58 +696,53 @@ const char* inf_status_text(uint32_t st) {
   }
 }
 
-// grow-only, keeping the first `keep` bytes
-void ensure_keep(smr_ctx* ctx, DevBuf& b, size_t bytes, size_t keep) {
-  if (bytes <= b.cap && b.p) return;
-  DevBuf n;
-  CK(n.alloc(bytes + bytes / 8 + 256));
-  if (keep) CK(cudaMemcpyAsync(n.p, b.p, keep, cudaMemcpyDeviceToDevice, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  b = std::move(n);
-}
+// distance of the speculative block searches for nbytes of gzip input: 64 KB for large files, down to 8 KB so that a small file
+// still makes thousands of spans
+uint64_t inflate_chunk(uint64_t nbytes) { return std::min<uint64_t>(65536, std::max<uint64_t>(8192, nbytes / 8192)); }
 
 // One round of the inflate (the five steps of smr_inflate.h) over the compressed bytes gz[0 .. nbytes) (host), from st.at on: the
 // output goes to out + at (grown as needed, its first `at` bytes kept).  eof: these bytes end the file; otherwise the round keeps
 // what it inflated up to the last block boundary it could reach and st says where the next round resumes.  Returns the bytes
 // kept.  The host only walks the list of spans (a few thousand entries) between the COUNT and the WRITE pass.
 uint64_t inflate_round(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes, bool eof, InfStream& st, DevBuf& out, uint64_t at) {
-  ctx->inf_spans = ctx->inf_candidates = 0;
+  auto& I = ctx->inf;
+  I.spans = I.candidates = 0;
   if (chunk_bytes < 1024) chunk_bytes = 1024;
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
-  CK(cudaEventRecord(e0, ctx->stream));
+  cudaEvent_t* e = events(ctx, 3);
+  CK(cudaEventRecord(e[0], ctx->stream));
   const size_t padded = (nbytes + 3) / 4 * 4 + 128;
-  ensure(ctx->d_gz, padded);
-  CK(cudaMemsetAsync((uint8_t*)ctx->d_gz.p + nbytes / 4 * 4, 0, padded - nbytes / 4 * 4, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->d_gz.p, gz, nbytes, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaEventRecord(e1, ctx->stream));
-  const uint32_t* w = (const uint32_t*)ctx->d_gz.p;
+  ensure(I.gz, padded);
+  CK(cudaMemsetAsync((uint8_t*)I.gz.p + nbytes / 4 * 4, 0, padded - nbytes / 4 * 4, ctx->stream));
+  CK(cudaMemcpyAsync(I.gz.p, gz, nbytes, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaEventRecord(e[1], ctx->stream));
+  const uint32_t* w = (const uint32_t*)I.gz.p;
   // FIND
   const uint64_t nchunks = (nbytes + chunk_bytes - 1) / chunk_bytes;
   if (nchunks > (1u << 24)) fail(SMR_ERR_ARG, "gz input: too many chunks");
   std::vector<uint64_t> cand;
   if (nchunks > 1) {
-    ensure(ctx->d_cand, nchunks * 8);
-    inf_find_kernel<<<(unsigned)(nchunks - 1), 256, 0, ctx->stream>>>(w, nbytes, chunk_bytes, (uint64_t*)ctx->d_cand.p);
+    ensure(I.cand, nchunks * 8);
+    inf_find_kernel<<<(unsigned)(nchunks - 1), 256, 0, ctx->stream>>>(w, nbytes, chunk_bytes, (uint64_t*)I.cand.p);
     CK(cudaGetLastError());
     std::vector<uint64_t> raw(nchunks - 1);
-    CK(cudaMemcpyAsync(raw.data(), ctx->d_cand.p, (nchunks - 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(raw.data(), I.cand.p, (nchunks - 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     for (uint64_t p : raw) if (p != kInfNone && p > st.at.bit) cand.push_back(p);   // chunk order = position order
-    if (!cand.empty()) CK(cudaMemcpyAsync(ctx->d_cand.p, cand.data(), cand.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
-  } else ensure(ctx->d_cand, 8);
+    if (!cand.empty()) CK(cudaMemcpyAsync(I.cand.p, cand.data(), cand.size() * 8, cudaMemcpyHostToDevice, ctx->stream));
+  } else ensure(I.cand, 8);
   const uint32_t ncand = (uint32_t)cand.size(), ns = ncand + 1;
   // COUNT
   CK(cudaFuncSetAttribute(inf_span_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kInfSpanSmem));   // per device
   CK(cudaFuncSetAttribute(inf_span_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kInfSpanSmem));
-  ensure(ctx->d_res, (size_t)ns * sizeof(SpanResult));
+  ensure(I.res, (size_t)ns * sizeof(SpanResult));
   const unsigned ctas = (ns + kInfSpanThreads - 1) / kInfSpanThreads;
   const uint64_t start = st.at.bit, prior = st.carry.len;
   const bool at_member = st.at.at_member;
-  inf_span_kernel<false><<<ctas, kInfSpanThreads, kInfSpanSmem, ctx->stream>>>(w, nbytes, start, at_member, prior, (const uint64_t*)ctx->d_cand.p, ncand, nullptr, nullptr,
-                                                                               nullptr, nullptr, nullptr, ns, nullptr, (SpanResult*)ctx->d_res.p);
+  inf_span_kernel<false><<<ctas, kInfSpanThreads, kInfSpanSmem, ctx->stream>>>(w, nbytes, start, at_member, prior, (const uint64_t*)I.cand.p, ncand, nullptr, nullptr,
+                                                                               nullptr, nullptr, nullptr, ns, nullptr, (SpanResult*)I.res.p);
   CK(cudaGetLastError());
   std::vector<SpanResult> res(ns);
-  CK(cudaMemcpyAsync(res.data(), ctx->d_res.p, (size_t)ns * sizeof(SpanResult), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(res.data(), I.res.p, (size_t)ns * sizeof(SpanResult), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   std::vector<uint32_t> real(ns); std::vector<uint64_t> off(ns), cnt(ns), keep(ns);
   uint32_t nreal = 0, why = 0;
@@ -711,43 +757,40 @@ uint64_t inflate_round(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t c
   for (uint32_t k = 0; k < nreal; ++k) { cnt[k] = res[real[k]].out_n; keep[k] = cnt[k]; moff[k + 1] = moff[k] + res[real[k]].members; }
   keep[nreal - 1] = next.keep_last;
   const uint32_t nmembers = moff[nreal];
-  ctx->inf_spans = nreal; ctx->inf_candidates = ncand;
+  I.spans = nreal; I.candidates = ncand;
   ensure_keep(ctx, out, at + total + 64, at);
   uint8_t* dst = (uint8_t*)out.p + at;
   if (total || (nmembers && st.carry.len)) {
     // WRITE
-    ensure(ctx->d_ids, (size_t)nreal * 4);
-    ensure(ctx->d_off, (size_t)nreal * 8);
-    ensure(ctx->d_cnt64, (size_t)nreal * 8);
     uint64_t nsym = 0;
     for (uint32_t k = 0; k < nreal; ++k) nsym = std::max(nsym, off[k] + cnt[k]);
-    ensure(ctx->d_sym, (nsym + 8) * 2);
-    ensure(ctx->d_win, (size_t)(nreal + 1) * kInfWindow);
-    CK(cudaMemcpyAsync(ctx->d_ids.p, real.data(), (size_t)nreal * 4, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_off.p, off.data(), (size_t)nreal * 8, cudaMemcpyHostToDevice, ctx->stream));
-    CK(cudaMemcpyAsync(ctx->d_cnt64.p, cnt.data(), (size_t)nreal * 8, cudaMemcpyHostToDevice, ctx->stream));
-    ensure(ctx->d_moff, (size_t)(nreal + 1) * 4);
-    ensure(ctx->d_mem, (size_t)(nmembers + 1) * sizeof(MemberEnd));
-    CK(cudaMemcpyAsync(ctx->d_moff.p, moff.data(), (size_t)(nreal + 1) * 4, cudaMemcpyHostToDevice, ctx->stream));
+    ensure(I.sym, (nsym + 8) * 2);
+    ensure(I.win, (size_t)(nreal + 1) * kInfWindow);
+    upload_async(ctx, I.ids, real.data(), nreal);
+    upload_async(ctx, I.off, off.data(), nreal);
+    upload_async(ctx, I.cnt, cnt.data(), nreal);
+    upload_async(ctx, I.moff, moff.data(), nreal + 1);
+    ensure(I.mem, (size_t)(nmembers + 1) * sizeof(MemberEnd));
+    const uint64_t* d_off = (const uint64_t*)I.off.p;
+    const uint64_t* d_cnt = (const uint64_t*)I.cnt.p;
     inf_span_kernel<true><<<(nreal + kInfSpanThreads - 1) / kInfSpanThreads, kInfSpanThreads, kInfSpanSmem, ctx->stream>>>(
-        w, nbytes, start, at_member, prior, (const uint64_t*)ctx->d_cand.p, ncand, (const uint32_t*)ctx->d_ids.p, (const uint64_t*)ctx->d_off.p,
-        (const uint64_t*)ctx->d_cnt64.p, (const uint32_t*)ctx->d_moff.p, (MemberEnd*)ctx->d_mem.p, nreal, (uint16_t*)ctx->d_sym.p, (SpanResult*)ctx->d_res.p);
+        w, nbytes, start, at_member, prior, (const uint64_t*)I.cand.p, ncand, (const uint32_t*)I.ids.p, d_off, d_cnt, (const uint32_t*)I.moff.p,
+        (MemberEnd*)I.mem.p, nreal, (uint16_t*)I.sym.p, (SpanResult*)I.res.p);
     CK(cudaGetLastError());
     // WINDOW (seeded with the last 32 KB of the previous round), RESOLVE of the bytes kept
-    if (st.have_window) CK(cudaMemcpyAsync(ctx->d_win.p, st.win.p, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
-    else CK(cudaMemsetAsync(ctx->d_win.p, 0, kInfWindow, ctx->stream));
-    inf_window_kernel<<<1, 1024, 0, ctx->stream>>>((const uint16_t*)ctx->d_sym.p, (const uint64_t*)ctx->d_off.p, (const uint64_t*)ctx->d_cnt64.p, nreal, (uint8_t*)ctx->d_win.p);
+    if (st.have_window) CK(cudaMemcpyAsync(I.win.p, st.win.p, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
+    else CK(cudaMemsetAsync(I.win.p, 0, kInfWindow, ctx->stream));
+    inf_window_kernel<<<1, 1024, 0, ctx->stream>>>((const uint16_t*)I.sym.p, d_off, d_cnt, nreal, (uint8_t*)I.win.p);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(ctx->d_cnt64.p, keep.data(), (size_t)nreal * 8, cudaMemcpyHostToDevice, ctx->stream));
+    upload_async(ctx, I.cnt, keep.data(), nreal);
     const uint64_t avg = total / nreal + 1;
     const unsigned pieces = (unsigned)std::min<uint64_t>(64, std::max<uint64_t>(1, avg / 8192));
-    inf_resolve_kernel<<<dim3(pieces, nreal), 256, 0, ctx->stream>>>((const uint16_t*)ctx->d_sym.p, (const uint64_t*)ctx->d_off.p, (const uint64_t*)ctx->d_cnt64.p,
-                                                                     (const uint8_t*)ctx->d_win.p, dst);
+    inf_resolve_kernel<<<dim3(pieces, nreal), 256, 0, ctx->stream>>>((const uint16_t*)I.sym.p, d_off, d_cnt, (const uint8_t*)I.win.p, dst);
     CK(cudaGetLastError());
     std::vector<SpanResult> res2(nreal);
     std::vector<MemberEnd> ends(nmembers);
-    CK(cudaMemcpyAsync(res2.data(), ctx->d_res.p, (size_t)nreal * sizeof(SpanResult), cudaMemcpyDeviceToHost, ctx->stream));
-    if (nmembers) CK(cudaMemcpyAsync(ends.data(), ctx->d_mem.p, (size_t)nmembers * sizeof(MemberEnd), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(res2.data(), I.res.p, (size_t)nreal * sizeof(SpanResult), cudaMemcpyDeviceToHost, ctx->stream));
+    if (nmembers) CK(cudaMemcpyAsync(ends.data(), I.mem.p, (size_t)nmembers * sizeof(MemberEnd), cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     for (uint32_t k = 0; k < nreal; ++k) {
       if (res2[k].status != res[real[k]].status || res2[k].out_n != cnt[k] || res2[k].end_bit != res[real[k]].end_bit || res2[k].members != res[real[k]].members)
@@ -760,15 +803,12 @@ uint64_t inflate_round(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t c
     const uint32_t npieces = (uint32_t)poff.size();
     std::vector<uint32_t> crcs(npieces);
     if (npieces) {
-      ensure(ctx->d_poff, (size_t)npieces * 8);
-      ensure(ctx->d_plen, (size_t)npieces * 4);
-      ensure(ctx->d_pcrc, (size_t)npieces * 4);
-      CK(cudaMemcpyAsync(ctx->d_poff.p, poff.data(), (size_t)npieces * 8, cudaMemcpyHostToDevice, ctx->stream));
-      CK(cudaMemcpyAsync(ctx->d_plen.p, plen.data(), (size_t)npieces * 4, cudaMemcpyHostToDevice, ctx->stream));
-      inf_crc_kernel<<<(npieces + 127) / 128, 128, 0, ctx->stream>>>(dst, (const uint64_t*)ctx->d_poff.p, (const uint32_t*)ctx->d_plen.p, npieces,
-                                                                       (uint32_t*)ctx->d_pcrc.p);
+      upload_async(ctx, I.poff, poff.data(), npieces);
+      upload_async(ctx, I.plen, plen.data(), npieces);
+      ensure(I.pcrc, (size_t)npieces * 4);
+      inf_crc_kernel<<<(npieces + 127) / 128, 128, 0, ctx->stream>>>(dst, (const uint64_t*)I.poff.p, (const uint32_t*)I.plen.p, npieces, (uint32_t*)I.pcrc.p);
       CK(cudaGetLastError());
-      CK(cudaMemcpyAsync(crcs.data(), ctx->d_pcrc.p, (size_t)npieces * 4, cudaMemcpyDeviceToHost, ctx->stream));
+      CK(cudaMemcpyAsync(crcs.data(), I.pcrc.p, (size_t)npieces * 4, cudaMemcpyDeviceToHost, ctx->stream));
     }
     // the window the next round starts from: the last 32 KB of (previous window, this round's output)
     if (!next.eos) {
@@ -776,32 +816,33 @@ uint64_t inflate_round(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t c
       ensure(st.win2, kInfWindow);
       if (total >= kInfWindow) CK(cudaMemcpyAsync(st.win.p, dst + total - kInfWindow, kInfWindow, cudaMemcpyDeviceToDevice, ctx->stream));
       else if (total) {
-        CK(cudaMemcpyAsync(st.win2.p, (uint8_t*)ctx->d_win.p + total, kInfWindow - total, cudaMemcpyDeviceToDevice, ctx->stream));
+        CK(cudaMemcpyAsync(st.win2.p, (uint8_t*)I.win.p + total, kInfWindow - total, cudaMemcpyDeviceToDevice, ctx->stream));
         CK(cudaMemcpyAsync((uint8_t*)st.win2.p + kInfWindow - total, dst, total, cudaMemcpyDeviceToDevice, ctx->stream));
         std::swap(st.win, st.win2);
       }
       if (total) st.have_window = true;
     }
-    CK(cudaEventRecord(e2, ctx->stream));
+    CK(cudaEventRecord(e[2], ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     if (const uint32_t bad = inf_crc_verify(ends, plen, first, crcs.data(), &st.carry)) fail(SMR_ERR_ARG, std::string("gz input: ") + inf_status_text(bad));
   } else {
-    CK(cudaEventRecord(e2, ctx->stream));
+    CK(cudaEventRecord(e[2], ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
   st.members += nmembers;
   st.at = next;
-  float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_h2d = ms;
-  cudaEventElapsedTime(&ms, e1, e2); ctx->t_inflate = ms;
+  ctx->t_h2d = elapsed_ms(e[0], e[1]);
+  ctx->t_inflate = elapsed_ms(e[1], e[2]);
   return total;
 }
 
-// gzip file (host bytes) -> inflated bytes in ctx->d_text; returns their number.  The whole file is one round.
+// gzip file (host bytes) -> inflated bytes in the resident text, which no batch is decoded from yet; returns their number.  The
+// whole file is one round.
 uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes) {
-  ctx->inf_spans = ctx->inf_candidates = 0;
+  clear_resident(ctx);
   if (nbytes < 18) fail(SMR_ERR_ARG, "gz input: shorter than a gzip header and trailer");
   InfStream st;
-  return inflate_round(ctx, gz, nbytes, chunk_bytes, true, st, ctx->d_text, 0);
+  return inflate_round(ctx, gz, nbytes, chunk_bytes, true, st, ctx->res.text, 0);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -809,24 +850,24 @@ uint64_t inflate_impl(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t ch
 // ---------------------------------------------------------------------------------------------------------------------
 
 // the count pass (smr_stream.h) over n bytes of new text at t (device)
-void count_text(smr_ctx* ctx, const uint8_t* t, uint64_t n, CountState& s) {
+void count_text(smr_ctx* ctx, ReadStream& rs, const uint8_t* t, uint64_t n) {
   if (n == 0) return;
   const uint32_t nlines = newline_index(ctx, t, n);
   const uint32_t parts = (uint32_t)std::max<uint64_t>(1, std::min<uint64_t>((uint64_t)ctx->sm_count * 8, (nlines + 255) / 256));
   const uint32_t per = (uint32_t)(((uint64_t)nlines + parts - 1) / parts + 255) / 256 * 256;
-  uint8_t* rc = ensure<uint8_t>(ctx->d_rc, (size_t)(parts + 1) * sizeof(ReadCounts) + 16);
+  uint8_t* rc = ensure<uint8_t>(rs.scr.rc, (size_t)(parts + 1) * sizeof(ReadCounts) + 16);
   ReadCounts* part = (ReadCounts*)rc;
   uint64_t* info = (uint64_t*)(rc + (size_t)(parts + 1) * sizeof(ReadCounts));
-  count_lines_kernel<<<parts, 256, 0, ctx->stream>>>((const uint64_t*)ctx->d_nl.p, nlines, n, s, per, part);
+  count_lines_kernel<<<parts, 256, 0, ctx->stream>>>((const uint64_t*)ctx->tx.nl.p, nlines, n, rs.counts, per, part);
   CK(cudaGetLastError());
-  count_fold_kernel<<<1, 1, 0, ctx->stream>>>(part, parts, (const uint64_t*)ctx->d_nl.p, nlines, n, part + parts, info);
+  count_fold_kernel<<<1, 1, 0, ctx->stream>>>(part, parts, (const uint64_t*)ctx->tx.nl.p, nlines, n, part + parts, info);
   CK(cudaGetLastError());
   struct { ReadCounts r; uint64_t nl[2]; } h;
   CK(cudaMemcpyAsync(&h.r, part + parts, sizeof(ReadCounts), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(h.nl, info, 16, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  rc_fold(s, h.r);
-  rc_advance(s, n, h.nl[0], h.nl[1]);
+  rc_fold(rs.counts, h.r);
+  rc_advance(rs.counts, n, h.nl[0], h.nl[1]);
 }
 
 // the pending text from [off, n) on, with room for `extra` more bytes after n
@@ -859,7 +900,7 @@ void took_text(smr_ctx* ctx, ReadStream& rs, StreamSide& sd, uint64_t from) {
       fail(SMR_ERR_ARG, std::string("mate stream: mate 1 is ") + (m1.first == '@' ? "FASTQ" : "FASTA") + " and mate 2 is " + (m2.first == '@' ? "FASTQ" : "FASTA"));
     return;
   }
-  count_text(ctx, t + from, sd.n - from, rs.counts);
+  count_text(ctx, rs, t + from, sd.n - from);
   if (rs.count_only) sd.off = sd.n = 0;
 }
 
@@ -886,10 +927,9 @@ void stream_push_impl(smr_ctx* ctx, uint32_t mate, const uint8_t* bytes, uint64_
   if (sd.tail.empty() && !eof) return;
   compact_pending(ctx, sd, 0);
   const uint64_t nb = sd.tail.size();
-  const uint64_t chunk = std::min<uint64_t>(65536, std::max<uint64_t>(8192, nb / 8192));   // as smr_upload_fastx_gz
   const uint64_t from = sd.n;
   try {
-    sd.n += inflate_round(ctx, sd.tail.data(), nb, chunk, eof, sd.inf, sd.text, sd.n);
+    sd.n += inflate_round(ctx, sd.tail.data(), nb, inflate_chunk(nb), eof, sd.inf, sd.text, sd.n);
   } catch (Failure& f) {
     f.msg = who + f.msg;
     throw;
@@ -910,13 +950,13 @@ uint64_t stream_cut(smr_ctx* ctx, ReadStream& rs) {
   if (avail == 0) return 0;
   if (avail <= limit) return sd.eof ? avail : 0;   // a batch takes whole records up to batch_bytes: wait for more text
   const uint8_t* t = (const uint8_t*)sd.text.p + sd.off;
-  unsigned long long* cut = ensure<unsigned long long>(ctx->d_cut, 16);
+  unsigned long long* cut = ensure<unsigned long long>(rs.scr.cut, 16);
   uint64_t w = std::min(avail, limit + 1);   // a record end at <= limit is a '\n' before it or a header line starting at it
   for (;;) {
     const uint32_t nl = newline_index(ctx, t, w);
     const unsigned long long init[2] = {0ull, ~0ull};
     CK(cudaMemcpyAsync(cut, init, 16, cudaMemcpyHostToDevice, ctx->stream));
-    stream_cut_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(t, (const uint64_t*)ctx->d_nl.p, nl, w, limit, sd.first == '@' ? kFmtFastq : kFmtFasta, cut);
+    stream_cut_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(t, (const uint64_t*)ctx->tx.nl.p, nl, w, limit, sd.first == '@' ? kFmtFastq : kFmtFasta, cut);
     CK(cudaGetLastError());
     unsigned long long h[2];
     CK(cudaMemcpyAsync(h, cut, 16, cudaMemcpyDeviceToHost, ctx->stream));
@@ -928,19 +968,20 @@ uint64_t stream_cut(smr_ctx* ctx, ReadStream& rs) {
   }
 }
 
-// The record ends of mate m's pending text in its first w bytes, in bytes from its off, to ctx->d_mend[m]; returns their number.
+// The record ends of mate m's pending text in its first w bytes, in bytes from its off, to rs.scr.mend[m]; returns their number.
 // Once the file has ended and w covers its text, its last record ends at the end of the text, one byte further when the text
 // does not end in '\n' (the interleave appends one).
-uint32_t mate_ends(smr_ctx* ctx, StreamSide& sd, uint32_t m, uint64_t w) {
+uint32_t mate_ends(smr_ctx* ctx, ReadStream& rs, uint32_t m, uint64_t w) {
+  const StreamSide& sd = rs.side[m];
   const uint64_t avail = sd.n - sd.off;
   if (avail == 0) return 0;
   const uint8_t* t = (const uint8_t*)sd.text.p + sd.off;
   const uint32_t fmt = sd.first == '@' ? kFmtFastq : kFmtFasta;
   const uint32_t nl = newline_index(ctx, t, w);
-  uint32_t* flag = ensure<uint32_t>(ctx->d_mflag, ((size_t)nl + 1) * 4);
-  uint64_t* ends = ensure<uint64_t>(ctx->d_mend[m], ((size_t)nl + 2) * 8);
+  uint32_t* flag = ensure<uint32_t>(rs.scr.mflag, ((size_t)nl + 1) * 4);
+  uint64_t* ends = ensure<uint64_t>(rs.scr.mend[m], ((size_t)nl + 2) * 8);
   const int grid = ctx->sm_count * 8;
-  const uint64_t* d_nl = (const uint64_t*)ctx->d_nl.p;
+  const uint64_t* d_nl = (const uint64_t*)ctx->tx.nl.p;
   if (nl) record_end_flags_kernel<<<grid, 256, 0, ctx->stream>>>(t, d_nl, nl, w, fmt, flag);
   CK(cudaMemsetAsync(flag + nl, 0, 4, ctx->stream));
   exclusive_sum(ctx, flag, flag, nl + 1);
@@ -966,20 +1007,20 @@ uint32_t mate_ends(smr_ctx* ctx, StreamSide& sd, uint32_t m, uint64_t w) {
 }
 
 // The next batch of a mate stream: the k whole pairs whose interleaved text fits in batch_bytes (or the first pair alone when it
-// does not fit), interleaved into ctx->d_text.  Returns k; 0 = push more, or (*done) both files are exhausted.  Before both files
-// have ended, pairs that fit wait for more text, so that every batch but the last is full.
+// does not fit), interleaved into the resident text.  Returns k; 0 = push more, or (*done) both files are exhausted.  Before both
+// files have ended, pairs that fit wait for more text, so that every batch but the last is full.
 uint32_t mate_cut(smr_ctx* ctx, ReadStream& rs, uint64_t* nbytes, int* done) {
   StreamSide* sd = rs.side;
   const uint64_t limit = rs.batch_bytes;
   const uint64_t avail[2] = {sd[0].n - sd[0].off, sd[1].n - sd[1].off};
   uint64_t w[2] = {std::min(avail[0], limit + 1), std::min(avail[1], limit + 1)};
-  unsigned long long* dk = ensure<unsigned long long>(ctx->d_cut, 16);
+  unsigned long long* dk = ensure<unsigned long long>(rs.scr.cut, 16);
   for (;;) {
     uint32_t n[2];
     bool closed[2];   // no more record ends can join the listed ones within batch_bytes: beyond the window, or the file ended
-    for (uint32_t m = 0; m < 2; ++m) { n[m] = mate_ends(ctx, sd[m], m, w[m]); closed[m] = w[m] < avail[m] || sd[m].eof; }
-    const uint64_t* ea = (const uint64_t*)ctx->d_mend[0].p;
-    const uint64_t* eb = (const uint64_t*)ctx->d_mend[1].p;
+    for (uint32_t m = 0; m < 2; ++m) { n[m] = mate_ends(ctx, rs, m, w[m]); closed[m] = w[m] < avail[m] || sd[m].eof; }
+    const uint64_t* ea = (const uint64_t*)rs.scr.mend[0].p;
+    const uint64_t* eb = (const uint64_t*)rs.scr.mend[1].p;
     const uint32_t both = std::min(n[0], n[1]);
     if (both) {
       CK(cudaMemsetAsync(dk, 0, 8, ctx->stream));
@@ -997,9 +1038,9 @@ uint32_t mate_cut(smr_ctx* ctx, ReadStream& rs, uint64_t* nbytes, int* done) {
       CK(cudaStreamSynchronize(ctx->stream));
       *nbytes = end[0] + end[1];
       if (*nbytes >= 0xF0000000ull) fail(SMR_ERR_ARG, "mate stream: one pair of 2^32 bytes or more");
-      ensure(ctx->d_text, *nbytes + 64);
+      ensure(ctx->res.text, *nbytes + 64);
       mate_interleave_kernel<<<std::max(1u, std::min<uint32_t>(ctx->sm_count * 16, (k + 7) / 8)), 256, 0, ctx->stream>>>(
-          (const uint8_t*)sd[0].text.p + sd[0].off, avail[0], ea, (const uint8_t*)sd[1].text.p + sd[1].off, avail[1], eb, k, (uint8_t*)ctx->d_text.p);
+          (const uint8_t*)sd[0].text.p + sd[0].off, avail[0], ea, (const uint8_t*)sd[1].text.p + sd[1].off, avail[1], eb, k, (uint8_t*)ctx->res.text.p);
       CK(cudaGetLastError());
       for (uint32_t m = 0; m < 2; ++m) sd[m].off += std::min(end[m], avail[m]);
       return k;
@@ -1031,7 +1072,7 @@ uint32_t stream_next_impl(smr_ctx* ctx, int* done) {
     if (k == 0) return 0;
     const uint32_t nreads = upload_fastx_impl(ctx, nullptr, nbytes, rs.side[0].first);
     if (nreads != 2 * k) fail(SMR_ERR_ARG, "mate stream: " + std::to_string(k) + " pairs decoded to " + std::to_string(nreads) + " records");
-    ctx->resident_mates = true;
+    ctx->res.mates = true;
     return nreads;
   }
   StreamSide& sd = rs.side[0];
@@ -1040,8 +1081,8 @@ uint32_t stream_next_impl(smr_ctx* ctx, int* done) {
     const uint64_t cut = stream_cut(ctx, rs);
     if (cut == 0) return 0;
     if (cut >= 0xF0000000ull) fail(SMR_ERR_ARG, "read stream: one record of 2^32 bytes or more");
-    ensure(ctx->d_text, cut + 64);
-    CK(cudaMemcpyAsync(ctx->d_text.p, (const uint8_t*)sd.text.p + sd.off, cut, cudaMemcpyDeviceToDevice, ctx->stream));
+    ensure(ctx->res.text, cut + 64);
+    CK(cudaMemcpyAsync(ctx->res.text.p, (const uint8_t*)sd.text.p + sd.off, cut, cudaMemcpyDeviceToDevice, ctx->stream));
     char c0 = 0;
     CK(cudaMemcpyAsync(&c0, (const uint8_t*)sd.text.p + sd.off, 1, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
@@ -1049,6 +1090,19 @@ uint32_t stream_next_impl(smr_ctx* ctx, int* done) {
     const uint32_t nreads = upload_fastx_impl(ctx, nullptr, cut, c0);
     if (nreads) { *done = 0; return nreads; }
   }
+}
+
+// closes the read stream; its scratch stays for the next one
+void close_stream(ReadStream& rs) {
+  ReadStream::Scratch scr = std::move(rs.scr);
+  rs = ReadStream{};
+  rs.scr = std::move(scr);
+}
+
+// runs f, one call on the open read stream: a stream that fails is closed
+template <class F>
+void stream_call(smr_ctx* ctx, F&& f) {
+  try { f(); } catch (...) { close_stream(ctx->rs); throw; }
 }
 
 // Several contexts may share a device (two per GPU let the copies and the host-side result packing of one batch run under the
@@ -1071,15 +1125,17 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   if (nreads == 0) return;
   const uint32_t slots = slots_of(ctx);
   std::lock_guard<std::mutex> dev_lock(device_kernel_mutex(ctx->device));   // held until the stream has drained
-  setup_arenas(ctx, bt.scale, bt.max_len);
+  auto& A = ctx->run;
+  RunGeom g = setup_arenas(ctx, bt.scale, bt.max_len);
+  LisGlobals& lg = g.lg; FinalGlobals& fg = g.fg;
   // device copy of the part table (finalize looks parts up by slot)
   std::vector<DevIndex> hp;
   for (size_t i = 0; i < ctx->parts.size(); ++i) {
     DevIndex d = ctx->parts[i].d; d.slot = (uint32_t)i; d.is_last = (i + 1 == ctx->parts.size()) ? 1u : 0u;
     hp.push_back(d);
   }
-  ensure(ctx->parts_dev, hp.size() * sizeof(DevIndex));
-  CK(cudaMemcpyAsync(ctx->parts_dev.p, hp.data(), hp.size() * sizeof(DevIndex), cudaMemcpyHostToDevice, ctx->stream));
+  ensure(A.parts, hp.size() * sizeof(DevIndex));
+  CK(cudaMemcpyAsync(A.parts.p, hp.data(), hp.size() * sizeof(DevIndex), cudaMemcpyHostToDevice, ctx->stream));
   // cigar pool on the device: generous fixed share per alignment slot
   bt.cigar_cap_dev = (uint64_t)nreads * slots * 24 * bt.scale + 4096;
   if (bt.cigar_cap_dev >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, "CIGAR pool of this batch would pass 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches");
@@ -1091,92 +1147,75 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   CK(cudaMemsetAsync(bt.flags.p, 0, (size_t)nreads * 4, ctx->stream));
   CK(cudaMemsetAsync(bt.hit_db.p, 0xFF, (size_t)nreads * 2, ctx->stream));
   const DevParams dp = to_dev(ctx->prm);
-  size_t evi = 2;
-  std::vector<std::pair<size_t, int>> spans;   // (event index of start, kind) ; end = start+1
-  cudaEvent_t eb = get_event(ctx, evi++); CK(cudaEventRecord(eb, ctx->stream));
-  for (uint32_t c0 = 0; c0 < nreads; c0 += ctx->chunk_reads) {
+  lg.aln_work = (AlnWork*)bt.aln_work.p; lg.slots = slots; lg.work_next = sc.lis_next; lg.work_next_b = sc.lis_next_b;
+  lg.parts = (const DevIndex*)A.parts.p; lg.nparts = (uint32_t)hp.size();
+  lg.q_head = sc.q_head; lg.q_tail = sc.q_tail; lg.planners_done = sc.planners_done;
+  fg.parts = (const DevIndex*)A.parts.p; fg.aln_work = (const AlnWork*)bt.aln_work.p; fg.out = (OutAln*)bt.out_aln.p;
+  fg.slots = slots; fg.cigar_pool = (uint32_t*)bt.cigar_pool.p; fg.cigar_cap = bt.cigar_cap_dev; fg.cigar_used = sc.cigar_used;
+  fg.work_next = sc.fin_next; fg.job_count = sc.fin_jobs;
+  // events: [0] start, [1] end, and per chunk k from 2 + 5k on: seed, candidate kernel, end of it; finalize, end of it
+  const uint32_t nchunks = (nreads + ctx->chunk_reads - 1) / ctx->chunk_reads;
+  cudaEvent_t* e = events(ctx, 2 + 5 * (size_t)nchunks);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  for (uint32_t c0 = 0, k = 0; c0 < nreads; c0 += ctx->chunk_reads, ++k) {
     const uint32_t n = std::min(ctx->chunk_reads, nreads - c0);
+    cudaEvent_t* ek = e + 2 + 5 * k;
     DevBatch b = make_batch(bt, c0, n);
     CK(cudaMemsetAsync(sc.work_n, 0, 16, ctx->stream));  // (unused word), the two cursors of the candidate kernel's read schedule, finalize's cursor (zeroed again before it runs)
     CK(cudaMemsetAsync(b.cost, 0, (size_t)n * 4, ctx->stream));
     CK(cudaMemsetAsync(b.bin_count, 0, (size_t)kCostBins * 4, ctx->stream));
-    cudaEvent_t s0 = get_event(ctx, evi), s1 = get_event(ctx, evi + 1), s2 = get_event(ctx, evi + 2); evi += 3;
-    CK(cudaEventRecord(s0, ctx->stream));
-    ensure(ctx->seed_ctr, hp.size() * 4);
-    CK(cudaMemsetAsync(ctx->seed_ctr.p, 0, hp.size() * 4, ctx->stream));   // one work counter per seed launch
+    CK(cudaEventRecord(ek[0], ctx->stream));
+    ensure(A.seed_ctr, hp.size() * 4);
+    CK(cudaMemsetAsync(A.seed_ctr.p, 0, hp.size() * 4, ctx->stream));   // one work counter per seed launch
     for (size_t pi = 0; pi < hp.size(); ++pi) {
-      const int ctas = (int)(ctx->lane_hits_warps / kSeedWarpsPerCta);
-      uint32_t* next_read = (uint32_t*)ctx->seed_ctr.p + pi;
-      if (ctx->instr) seed_kernel<true><<<ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[pi], b, dp, (uint32_t*)ctx->lane_hits.p, ctx->lane_hits_cap, next_read);
-      else seed_kernel<false><<<ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[pi], b, dp, (uint32_t*)ctx->lane_hits.p, ctx->lane_hits_cap, next_read);
+      uint32_t* next_read = (uint32_t*)A.seed_ctr.p + pi;
+      if (ctx->instr) seed_kernel<true><<<g.seed_ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[pi], b, dp, (uint32_t*)A.lane_hits.p, g.lane_hits_cap, next_read);
+      else seed_kernel<false><<<g.seed_ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[pi], b, dp, (uint32_t*)A.lane_hits.p, g.lane_hits_cap, next_read);
       CK(cudaGetLastError());
       t.launches += 1;
     }
     bin_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(b);
     CK(cudaGetLastError());
-    CK(cudaEventRecord(s1, ctx->stream));
-    {
-      LisGlobals lg{};
-      lg.arena_base = (uint8_t*)ctx->lis_arena.p; lg.arena_stride = ctx->lis_stride;
-      lg.hist_cap = ctx->hist_cap; lg.cand_cap = ctx->cand_cap; lg.pair_cap = ctx->pair_cap; lg.row_cap = ctx->row_cap; lg.pall_cap = ctx->pall_cap;
-      lg.task_cap = ctx->task_cap;
-      lg.epochs = (uint32_t*)ctx->lis_epochs.p; lg.aln_work = (AlnWork*)bt.aln_work.p; lg.slots = slots; lg.work_next = sc.lis_next; lg.work_next_b = sc.lis_next_b;
-      lg.parts = (const DevIndex*)ctx->parts_dev.p; lg.nparts = (uint32_t)hp.size();
-      lg.ring = (QSlot*)ctx->lis_queue.p; lg.done = (uint32_t*)ctx->lis_done.p; lg.score_rows = (int32_t*)ctx->lis_rows.p;
-      lg.dbg = (getenv("SMR_TIMELINE") || getenv("SMR_VERBOSE")) ? (unsigned long long*)ctx->lis_dbg.p : nullptr;   // (the timeline costs the instrumented kernel an atomic per scored pair)
-      lg.q_head = sc.q_head; lg.q_tail = sc.q_tail; lg.planners_done = sc.planners_done;
-      lis_reset_kernel<<<kQueueCap / 256, 256, 0, ctx->stream>>>(lg, ctx->lis_warps);
-      CK(cudaGetLastError());
-      if (ctx->instr) lis_kernel<true><<<ctx->lis_ctas, kLisWarpsPerCta * 32, kLisSmemBytes, ctx->stream>>>(b, dp, lg);
-      else lis_kernel<false><<<ctx->lis_ctas, kLisWarpsPerCta * 32, kLisSmemBytes, ctx->stream>>>(b, dp, lg);
-      CK(cudaGetLastError());
-      CK(cudaEventRecord(s2, ctx->stream));
-      spans.push_back({evi - 3, 0});
-      t.launches += 2;
-    }
+    CK(cudaEventRecord(ek[1], ctx->stream));
+    lis_reset_kernel<<<kQueueCap / 256, 256, 0, ctx->stream>>>(lg, g.lis_warps);
+    CK(cudaGetLastError());
+    if (ctx->instr) lis_kernel<true><<<g.lis_ctas, kLisWarpsPerCta * 32, kLisSmemBytes, ctx->stream>>>(b, dp, lg);
+    else lis_kernel<false><<<g.lis_ctas, kLisWarpsPerCta * 32, kLisSmemBytes, ctx->stream>>>(b, dp, lg);
+    CK(cudaGetLastError());
+    CK(cudaEventRecord(ek[2], ctx->stream));
+    t.launches += 2;
     // finalize this chunk
     CK(cudaMemsetAsync(sc.fin_next, 0, 4, ctx->stream));
     CK(cudaMemsetAsync(sc.fin_jobs, 0, 4, ctx->stream));
-    cudaEvent_t f0 = get_event(ctx, evi), f1 = get_event(ctx, evi + 1); evi += 2;
-    CK(cudaEventRecord(f0, ctx->stream));
-    FinalGlobals fg{};
-    fg.arena_base = (uint8_t*)ctx->final_arena.p; fg.arena_stride = ctx->final_stride;
-    fg.cap_w = ctx->cap_w; fg.cap_cig = ctx->cap_cig; fg.row_cap = ctx->row_cap; fg.cap_dir = ctx->cap_dir;
-    fg.parts = (const DevIndex*)ctx->parts_dev.p; fg.aln_work = (const AlnWork*)bt.aln_work.p; fg.out = (OutAln*)bt.out_aln.p;
-    fg.slots = slots; fg.cigar_pool = (uint32_t*)bt.cigar_pool.p; fg.cigar_cap = bt.cigar_cap_dev; fg.cigar_used = sc.cigar_used;
-    fg.work_next = sc.fin_next;
-    ensure(ctx->tb_jobs, (size_t)n * slots * sizeof(TraceJob));
-    ensure(ctx->fin_list, (size_t)n * slots * 4);
-    fg.job_list = (uint32_t*)ctx->fin_list.p; fg.job_count = sc.fin_jobs;
-    fg.jobs = (TraceJob*)ctx->tb_jobs.p; fg.tb_arena = (uint8_t*)ctx->tb_arena.p; fg.tb_stride = ctx->tb_stride;
-    fg.tb_cap_w = ctx->tb_cap_w; fg.tb_cap_cig = ctx->tb_cap_cig; fg.tb_cap_dir = ctx->tb_cap_dir;
-    fg.stats = nullptr;
-    if (ctx->host_stats) {
-      ensure(bt.aln_stats, (size_t)nreads * slots * sizeof(AlnStats));
-      fg.stats = (AlnStats*)bt.aln_stats.p;
-    }
+    CK(cudaEventRecord(ek[3], ctx->stream));
+    fg.jobs = ensure<TraceJob>(A.tb_jobs, (size_t)n * slots * sizeof(TraceJob));
+    fg.job_list = ensure<uint32_t>(A.fin_list, (size_t)n * slots * 4);
+    fg.stats = ctx->host_stats ? ensure<AlnStats>(bt.aln_stats, (size_t)nreads * slots * sizeof(AlnStats)) : nullptr;
     final_jobs_kernel<<<std::min<uint32_t>((n * slots + 255) / 256, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(b, fg);
     CK(cudaGetLastError());
-    finalize_kernel<<<ctx->final_warps / kFinalWarpsPerCta, kFinalWarpsPerCta * 32, 0, ctx->stream>>>(b, dp, fg);
+    finalize_kernel<<<g.final_warps / kFinalWarpsPerCta, kFinalWarpsPerCta * 32, 0, ctx->stream>>>(b, dp, fg);
     CK(cudaGetLastError());
-    traceback_kernel<<<ctx->tb_threads / 128, 128, 0, ctx->stream>>>(b, dp, fg);
+    traceback_kernel<<<g.tb_threads / 128, 128, 0, ctx->stream>>>(b, dp, fg);
     CK(cudaGetLastError());
-    t.launches += 2;
-    CK(cudaEventRecord(f1, ctx->stream));
-    spans.push_back({evi - 2, 1});
-    t.launches += 1;
+    CK(cudaEventRecord(ek[4], ctx->stream));
+    t.launches += 3;
   }
-  cudaEvent_t ee = get_event(ctx, evi++); CK(cudaEventRecord(ee, ctx->stream));
+  CK(cudaEventRecord(e[1], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, eb, ee); t.total = ms;
+  t.total = elapsed_ms(e[0], e[1]);
+  for (uint32_t k = 0; k < nchunks; ++k) {
+    const cudaEvent_t* ek = e + 2 + 5 * k;
+    t.seed += elapsed_ms(ek[0], ek[1]);
+    t.lis += elapsed_ms(ek[1], ek[2]);
+    t.final += elapsed_ms(ek[3], ek[4]);
+  }
   if (getenv("SMR_VERBOSE")) {
-    unsigned long long d[16]; cudaMemcpy(d, ctx->lis_dbg.p, 128, cudaMemcpyDeviceToHost);
+    unsigned long long d[16]; cudaMemcpy(d, A.lis_dbg.p, 128, cudaMemcpyDeviceToHost);
     fprintf(stderr, "[smr] slowest read %llu: %.2f ms; cycles vote %llu order %llu group %llu plan %llu wait %llu replay %llu; sw calls %llu, tasks scored %llu, rounds %llu\n", d[10], d[0] / 1.965e6, d[1], d[2], d[3], d[4], d[5], d[6], d[7], d[8], d[9]);
   }
   if (ctx->instr && getenv("SMR_TIMELINE")) {   // ns per role and state in 1 ms buckets since the kernel's start (this run's candidate launches summed)
     std::vector<unsigned long long> tl((size_t)kTlRows * kTlBuckets);
-    cudaMemcpy(tl.data(), (const unsigned long long*)ctx->lis_dbg.p + kTlBase, tl.size() * 8, cudaMemcpyDeviceToHost);
+    cudaMemcpy(tl.data(), (const unsigned long long*)A.lis_dbg.p + kTlBase, tl.size() * 8, cudaMemcpyDeviceToHost);
     static const char* names[kTlRows] = {"scorer_wait_ns", "scorer_busy_ns", "planner_wait_ns", "planner_vote_group_ns", "reads_done", "planner_alive_ns"};
     for (int r = 0; r < kTlRows; ++r) {
       int last = 0; for (int k = 0; k < kTlBuckets; ++k) if (tl[(size_t)r * kTlBuckets + k]) last = k + 1;
@@ -1185,13 +1224,14 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
       fprintf(stderr, "\n");
     }
   }
-  for (auto& s : spans) {
-    if (s.second == 0) {
-      cudaEventElapsedTime(&ms, ctx->ev[s.first], ctx->ev[s.first + 1]); t.seed += ms;
-      cudaEventElapsedTime(&ms, ctx->ev[s.first + 1], ctx->ev[s.first + 2]); t.lis += ms;
-    } else { cudaEventElapsedTime(&ms, ctx->ev[s.first], ctx->ev[s.first + 1]); t.final += ms; }
-  }
 }
+
+// the device counters 1 .. dcCount - 1 are copied to the caller's counters of the same index (download_impl)
+static_assert(+dcNumShort == +SMR_CNT_NUM_SHORT && +dcSwCalls == +SMR_CNT_SW_CALLS && +dcSwCells == +SMR_CNT_SW_CELLS &&
+                  +dcWindows == +SMR_CNT_WINDOWS && +dcNodes == +SMR_CNT_TRIE_NODES && +dcBuckets == +SMR_CNT_BUCKETS &&
+                  +dcEntries == +SMR_CNT_BUCKET_ENTRIES && +dcPosEntries == +SMR_CNT_POS_ENTRIES && +dcLisCalls == +SMR_CNT_LIS_CALLS,
+              "DevCnt and the SMR_CNT_* indices disagree");
+static_assert(+dcCount <= +SMR_CNT_FIXED, "device counters overlap reads_matched_per_db");
 
 struct HostOut {
   smr_read_result* results; smr_aln* alns; uint32_t* cigar_pool; uint64_t cigar_cap; uint64_t cigar_used;
@@ -1205,37 +1245,37 @@ void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint3
   flagged.clear();
   if (n == 0) return;
   const uint32_t slots = slots_of(ctx);
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
-  CK(cudaEventRecord(e0, ctx->stream));
-  const ReadState* st = ensure<ReadState>(ctx->h_state, (size_t)n * sizeof(ReadState));
-  const uint32_t* fl = ensure<uint32_t>(ctx->h_flags, (size_t)n * 4);
-  const uint16_t* hdb = ensure<uint16_t>(ctx->h_hitdb, (size_t)n * 2);
-  const OutAln* oa = ensure<OutAln>(ctx->h_outaln, (size_t)n * slots * sizeof(OutAln));
+  cudaEvent_t* e = events(ctx, 2);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  const ReadState* st = ensure<ReadState>(ctx->h.state, (size_t)n * sizeof(ReadState));
+  const uint32_t* fl = ensure<uint32_t>(ctx->h.flags, (size_t)n * 4);
+  const uint16_t* hdb = ensure<uint16_t>(ctx->h.hitdb, (size_t)n * 2);
+  const OutAln* oa = ensure<OutAln>(ctx->h.outaln, (size_t)n * slots * sizeof(OutAln));
   const AlnStats* ast = nullptr;
   if (ctx->host_stats) {
-    ast = ensure<AlnStats>(ctx->h_stats, (size_t)n * slots * sizeof(AlnStats));
-    CK(cudaMemcpyAsync(ctx->h_stats.p, b.aln_stats.p, (size_t)n * slots * sizeof(AlnStats), cudaMemcpyDeviceToHost, ctx->stream));
+    ast = ensure<AlnStats>(ctx->h.stats, (size_t)n * slots * sizeof(AlnStats));
+    CK(cudaMemcpyAsync(ctx->h.stats.p, b.aln_stats.p, (size_t)n * slots * sizeof(AlnStats), cudaMemcpyDeviceToHost, ctx->stream));
   }
   unsigned long long used = 0;
   std::vector<unsigned long long> cnt(dcCount + 64);
-  CK(cudaMemcpyAsync(ctx->h_state.p, b.state.p, (size_t)n * sizeof(ReadState), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->h_flags.p, b.flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->h_hitdb.p, b.hit_db.p, (size_t)n * 2, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->h_outaln.p, b.out_aln.p, (size_t)n * slots * sizeof(OutAln), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h.state.p, b.state.p, (size_t)n * sizeof(ReadState), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h.flags.p, b.flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h.hitdb.p, b.hit_db.p, (size_t)n * 2, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->h.outaln.p, b.out_aln.p, (size_t)n * slots * sizeof(OutAln), cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(&used, scalars_of(b).cigar_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(cnt.data(), b.counters.p, cnt.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   used = std::min<unsigned long long>(used, b.cigar_cap_dev);
-  const uint32_t* cig = ensure<uint32_t>(ctx->h_cigar, (size_t)used * 4 + 16);
-  if (used) CK(cudaMemcpyAsync(ctx->h_cigar.p, b.cigar_pool.p, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaEventRecord(e1, ctx->stream));
+  const uint32_t* cig = ensure<uint32_t>(ctx->h.cigar, (size_t)used * 4 + 16);
+  if (used) CK(cudaMemcpyAsync(ctx->h.cigar.p, b.cigar_pool.p, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e[1], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  float ms = 0; cudaEventElapsedTime(&ms, e0, e1); ctx->t_d2h = ms;
+  ctx->t_d2h = elapsed_ms(e[0], e[1]);
   // a trace back error fails the call after what it can still write; the capacity errors below take precedence
   bool trace_error = false;
   auto fail_on_trace_error = [&] { if (trace_error) fail(SMR_ERR_INDEX, "trace back error (ssw.c:707 is fatal in the reference too)"); };
   // pass 1 (sequential, cheap): flagged reads, cigar offsets in the caller's pool (running sum in read order), counters
-  std::vector<uint64_t>& coff = ctx->h_coff; coff.resize((size_t)n + 1);
+  std::vector<uint64_t>& coff = ctx->h.coff; coff.resize((size_t)n + 1);
   uint64_t run = out.cigar_used;
   uint32_t need_slots = 0;
   for (uint32_t r = 0; r < n; ++r) {
@@ -1293,15 +1333,9 @@ void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint3
     for (uint32_t t = 0; t < nthr; ++t) pool.emplace_back(pack, (uint32_t)((uint64_t)n * t / nthr), (uint32_t)((uint64_t)n * (t + 1) / nthr));
     for (auto& th : pool) th.join();
   }
-  if (out.counters) {
-    static const int mapc[][2] = {{SMR_CNT_NUM_SHORT, dcNumShort}, {SMR_CNT_SW_CALLS, dcSwCalls}, {SMR_CNT_SW_CELLS, dcSwCells},
-                                  {SMR_CNT_WINDOWS, dcWindows}, {SMR_CNT_TRIE_NODES, dcNodes}, {SMR_CNT_BUCKETS, dcBuckets},
-                                  {SMR_CNT_BUCKET_ENTRIES, dcEntries}, {SMR_CNT_POS_ENTRIES, dcPosEntries}, {SMR_CNT_LIS_CALLS, dcLisCalls},
-                                  {10, dcMaxReadCycles}, {11, dcSumReadCycles}, {12, dcLisKernelCycles},
-                                  {13, dcCycVote}, {14, dcCycOrder}, {15, dcCycGroup}, {16, dcCycPlan}, {17, dcCycWait}, {18, dcCycReplay}, {19, dcSpecCalls},
-                                  {20, dcSpecCells}, {21, dcSpecPairs}, {22, dcSlowPairs}, {23, dcScWait}, {24, dcScLoad}, {25, dcScSw}, {26, dcScPub}, {27, dcRoundsA}, {28, dcRoundsB}, {29, dcW1Cyc}, {30, dcW1Cnt}, {31, dcMaxReadBusy}};
-    for (auto& m : mapc) if ((uint32_t)m[0] < out.n_counters) out.counters[m[0]] += cnt[m[1]];
-  }
+  // device counter k is the caller's counter k (pinned by the static_asserts at HostOut); dcNumAligned is counted in pass 1
+  if (out.counters)
+    for (uint32_t k = dcNumShort; k < dcCount && k < out.n_counters; ++k) out.counters[k] += cnt[k];
   fail_on_trace_error();
 }
 
@@ -1319,8 +1353,7 @@ void retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t
   b.scale = failed.scale * 8;
   const uint64_t w = read_layout(ctx, b, n, [&](uint32_t k) { return failed.off32[flagged[k] + 1] - src[k]; });
   DevBuf d_src;
-  CK(d_src.alloc((size_t)n * 4));
-  CK(cudaMemcpyAsync(d_src.p, src.data(), (size_t)n * 4, cudaMemcpyHostToDevice, ctx->stream));
+  upload_async(ctx, d_src, src.data(), n);
   ensure(b.seq04, b.total_nt + 64);
   gather_reads_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
       (const uint8_t*)failed.seq04.p, (const uint32_t*)d_src.p, n, (const uint32_t*)b.seq_off.p, (uint8_t*)b.seq04.p);
@@ -1337,14 +1370,14 @@ void retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t
 // the results of the resident batch's last run into the caller's arrays, its flagged reads retried; the resident batch and its
 // device results stay as they are
 void download_resident(smr_ctx* ctx, HostOut& out) {
-  ctx->t_run = ctx->resident.run;
+  ctx->t_run = ctx->res.b.run;
   std::vector<uint32_t> flagged;
-  download_impl(ctx, ctx->resident, out, flagged, nullptr);
+  download_impl(ctx, ctx->res.b, out, flagged, nullptr);
   if (!flagged.empty()) {
     // the arenas grow with the retry's scale (after 64x, tens of GB): the next run allocates them again at its own, whether the
     // retry succeeds or not
-    const auto release = on_exit([ctx] { for (DevBuf* s : {&ctx->lis_arena, &ctx->final_arena, &ctx->tb_arena, &ctx->lane_hits}) s->reset(); });
-    retry_flagged(ctx, ctx->resident, flagged, nullptr, out, 0);
+    const auto release = on_exit([ctx] { for (DevBuf* s : {&ctx->run.lis, &ctx->run.fin, &ctx->run.tb, &ctx->run.lane_hits}) s->reset(); });
+    retry_flagged(ctx, ctx->res.b, flagged, nullptr, out, 0);
   }
   // the caller's CIGAR pool was too small: *cigar_used names the words the batch needs
   if (out.pool_short)
@@ -1354,13 +1387,9 @@ void download_resident(smr_ctx* ctx, HostOut& out) {
 // ---------------------------------------------------------------------------------------------------------------------
 // report writer (smr_report.cuh)
 // ---------------------------------------------------------------------------------------------------------------------
-template <class T>
-void upload_async(smr_ctx* ctx, DevBuf& b, const T* src, size_t n) {
-  ensure(b, n * sizeof(T) + 16);
-  if (n) CK(cudaMemcpyAsync(b.p, src, n * sizeof(T), cudaMemcpyHostToDevice, ctx->stream));
-}
-
-[[noreturn]] void rpt_error(uint32_t e) {
+// fails with the text of the report error bits e (RptArgs::err), if any
+void rpt_check(uint32_t e) {
+  if (!e) return;
   fail(SMR_ERR_ARG, e & kRptErrLen ? "an alignment's readlen or read_end1 disagrees with the length of its read in the text"
                     : e & kRptErrGroup ? "an alignment names an (index, part) that is not loaded"
                     : e & kRptErrRef ? "an alignment's ref_num is beyond the reference names of its part"
@@ -1368,50 +1397,14 @@ void upload_async(smr_ctx* ctx, DevBuf& b, const T* src, size_t n) {
                     : e & kRptErrCigar ? "an alignment's CIGAR lies outside cigar_words" : "an alignment's CIGAR runs past its read or its reference");
 }
 
-// The first half of smr_format_reports and smr_otu_add: text, results and groups on the device (e1 recorded after the copies), the
-// record layout of the text (text_layout, then rpt_records_kernel); returns the report arguments that describe them.
-// The report error word is [4] of ctx->d_scal.
-RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar,
-                     uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads, const std::vector<RptGroup>& hg, cudaEvent_t e1) {
-  const uint32_t slots = slots_of(ctx), G = (uint32_t)hg.size();
-  const uint64_t N = (uint64_t)nreads * slots;
-  // the text
-  const uint8_t* dt;
-  if (text) {
-    upload_async(ctx, ctx->r_text, (const uint8_t*)text, nbytes);
-    dt = (const uint8_t*)ctx->r_text.p;
-  } else {
-    if (!ctx->text_bytes) fail(SMR_ERR_ARG, "no resident text: smr_upload_fastx[_gz] was not called, or pass the text");
-    nbytes = ctx->text_bytes;
-    dt = (const uint8_t*)ctx->d_text.p;
-  }
-  char c0 = 0;
-  if (nbytes) { if (text) c0 = text[0]; else CK(cudaMemcpy(&c0, dt, 1, cudaMemcpyDeviceToHost)); }
-  // results
-  upload_async(ctx, ctx->r_res, results, nreads);
-  upload_async(ctx, ctx->r_aln, alns, N);
-  upload_async(ctx, ctx->r_cig, cigar, cigar ? cigar_words : 0);
-  upload_async(ctx, ctx->r_st, stats, stats ? N : 0);
-  upload_async(ctx, ctx->r_grp, hg.data(), G);
-  CK(cudaEventRecord(e1, ctx->stream));
-  const TextLayout L = text_layout(ctx, dt, nbytes, c0);
-  if (L.nrec != nreads) fail(SMR_ERR_ARG, "the text holds " + std::to_string(L.nrec) + " records, the results " + std::to_string(nreads) + " reads");
-  // per record
-  const uint64_t fstride = (uint64_t)nreads + 1;
-  ensure(ctx->r_line, fstride * 4);
-  ensure(ctx->r_recs, fstride * sizeof(RptRec));
-  RptArgs a{};
-  a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)ctx->d_nl.p; a.spos = (const uint32_t*)ctx->d_spos.p; a.nlines = L.nlines; a.fastq = L.fmt == kFmtFastq;
-  a.rec = (const RptRec*)ctx->r_recs.p; a.nreads = nreads; a.slots = slots;
-  a.res = (const smr_read_result*)ctx->r_res.p; a.aln = (const smr_aln*)ctx->r_aln.p; a.cigar = (const uint32_t*)ctx->r_cig.p;
-  a.cigar_words = cigar ? cigar_words : 0; a.st = (const smr_aln_stats*)ctx->r_st.p;
-  a.grp = (const RptGroup*)ctx->r_grp.p; a.ngroups = G; a.err = (uint32_t*)ctx->d_scal.p + 4;
-  if (nreads) {
-    const int grid = ctx->sm_count * 8;
-    rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)ctx->d_hdr.p, (const uint32_t*)ctx->d_rec.p, L.nlines, (uint32_t*)ctx->r_line.p);
-    rpt_records_kernel<<<grid, 256, 0, ctx->stream>>>(a, (const uint32_t*)ctx->r_line.p, (RptRec*)ctx->r_recs.p);
-  }
-  return a;
+// A report-side call's checks of its batch: the arrays (stats_msg: stats are read, the text if missing; arrays_msg: the text of
+// missing results or alns, stats_msg if null), an even read count when paired (mates 2k, 2k+1), fewer than 2^31 result slots.
+void rpt_check_batch(const smr_ctx* ctx, const char* what, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
+                     uint32_t nreads, bool paired, const char* stats_msg, const char* arrays_msg = nullptr) {
+  if (nreads && stats_msg && !stats) fail(SMR_ERR_ARG, stats_msg);
+  if (nreads && (!results || !alns)) fail(SMR_ERR_ARG, arrays_msg ? arrays_msg : stats_msg);
+  if (paired && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
+  if ((uint64_t)nreads * slots_of(ctx) >= (1ull << 31)) fail(SMR_ERR_ARG, std::string("batch too large for ") + what + ": split it");
 }
 
 // the loaded (index, part)s in the reference's report order (index, then part)
@@ -1422,6 +1415,75 @@ std::vector<const Part*> report_groups(const smr_ctx* ctx) {
   return gp;
 }
 
+// The RptGroup table of the loaded (index, part)s in report order.  names / scoring: the caller prints reference ids
+// (smr_set_report_refs) / E-values and bit scores (smr_set_report_scoring), which every group must then have.
+std::vector<RptGroup> rpt_groups(const smr_ctx* ctx, bool names, bool scoring) {
+  std::vector<RptGroup> hg;
+  for (const Part* pt : report_groups(ctx)) {
+    const uint32_t ix = pt->d.index_num;
+    if (names && !pt->has_rnames)
+      fail(SMR_ERR_ARG, "smr_set_report_refs was not called for index " + std::to_string(ix) + " part " + std::to_string(pt->d.part));
+    const smr_ctx::RptScore* sc = ix < ctx->rpt_score.size() && ctx->rpt_score[ix].set ? &ctx->rpt_score[ix] : nullptr;
+    if (scoring && !sc) fail(SMR_ERR_ARG, "smr_set_report_scoring was not called for index " + std::to_string(ix));
+    hg.push_back(RptGroup{pt->rnames, pt->rname_off, sc ? (const double*)sc->ev.p : nullptr, sc ? (const uint32_t*)sc->bits.p : nullptr, pt->n_rnames,
+                          ix, pt->d.part, 0, pt->d.refseq, pt->d.ref_off});
+  }
+  return hg;
+}
+
+// The first half of a report-side call, after rpt_check_batch: text, results and groups on the device (e[0] recorded before the
+// copies, e[1] after them), the record layout of the text (text_layout, then rpt_records_kernel); returns the report arguments.
+// Their error word (err) is zeroed here; the caller reads it back with its results and passes it to rpt_check.
+RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar,
+                     uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads, const std::vector<RptGroup>& hg, const cudaEvent_t* e) {
+  auto& S = ctx->r;
+  CK(cudaEventRecord(e[0], ctx->stream));
+  const uint32_t slots = slots_of(ctx), G = (uint32_t)hg.size();
+  const uint64_t N = (uint64_t)nreads * slots;
+  // the text
+  const uint8_t* dt;
+  if (text) {
+    upload_async(ctx, S.text, (const uint8_t*)text, nbytes);
+    dt = (const uint8_t*)S.text.p;
+  } else {
+    if (!ctx->res.text_bytes) fail(SMR_ERR_ARG, "no resident text: smr_upload_fastx[_gz] was not called, or pass the text");
+    nbytes = ctx->res.text_bytes;
+    dt = (const uint8_t*)ctx->res.text.p;
+  }
+  char c0 = 0;
+  if (nbytes) { if (text) c0 = text[0]; else CK(cudaMemcpy(&c0, dt, 1, cudaMemcpyDeviceToHost)); }
+  // results
+  upload_async(ctx, S.res, results, nreads);
+  upload_async(ctx, S.aln, alns, N);
+  upload_async(ctx, S.cig, cigar, cigar ? cigar_words : 0);
+  upload_async(ctx, S.st, stats, stats ? N : 0);
+  upload_async(ctx, S.grp, hg.data(), G);
+  CK(cudaEventRecord(e[1], ctx->stream));
+  const TextLayout L = text_layout(ctx, dt, nbytes, c0);
+  if (L.nrec != nreads) fail(SMR_ERR_ARG, "the text holds " + std::to_string(L.nrec) + " records, the results " + std::to_string(nreads) + " reads");
+  // per record
+  const uint64_t fstride = (uint64_t)nreads + 1;
+  ensure(S.line, fstride * 4);
+  ensure(S.recs, fstride * sizeof(RptRec));
+  const auto& X = ctx->tx;
+  RptArgs a{};
+  a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)X.nl.p; a.spos = (const uint32_t*)X.spos.p; a.nlines = L.nlines; a.fastq = L.fmt == kFmtFastq;
+  a.rec = (const RptRec*)S.recs.p; a.nreads = nreads; a.slots = slots;
+  a.res = (const smr_read_result*)S.res.p; a.aln = (const smr_aln*)S.aln.p; a.cigar = (const uint32_t*)S.cig.p;
+  a.cigar_words = cigar ? cigar_words : 0; a.st = (const smr_aln_stats*)S.st.p;
+  a.grp = (const RptGroup*)S.grp.p; a.ngroups = G; a.err = &text_words(ctx)->rpt_err;
+  CK(cudaMemsetAsync(a.err, 0, 4, ctx->stream));
+  if (nreads) {
+    const int grid = ctx->sm_count * 8;
+    rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)X.hdr.p, (const uint32_t*)X.rec.p, L.nlines, (uint32_t*)S.line.p);
+    rpt_records_kernel<<<grid, 256, 0, ctx->stream>>>(a, (const uint32_t*)S.line.p, (RptRec*)S.recs.p);
+  }
+  return a;
+}
+
+// the report timings (smr_last_report_timings) from the four events of a call: the upload, the device work, the download
+void set_rpt_times(smr_ctx* ctx, const cudaEvent_t* e) { for (int k = 0; k < 3; ++k) ctx->t_rpt[k] = elapsed_ms(e[k], e[k + 1]); }
+
 // ---------------------------------------------------------------------------------------------------------------------
 // gzip deflate (smr_deflate.cuh)
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1430,6 +1492,7 @@ std::vector<const Part*> report_groups(const smr_ctx* ctx) {
 // SMR_ERR_CAPACITY with so filled (a retry gives the same bytes).  e_dev is recorded before the D2H, e_end after it.
 void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& sb, const std::vector<uint64_t>& se, char* out, uint64_t cap,
                   uint64_t* so, cudaEvent_t e_dev, cudaEvent_t e_end) {
+  auto& Z = ctx->z;
   const uint32_t ns = (uint32_t)sb.size();
   std::vector<DefChunk> ch;
   def_plan(sb.data(), se.data(), ns, ch);
@@ -1440,31 +1503,31 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
     const uint64_t end = se[ns - 1];
     std::vector<uint64_t> poff(nch); std::vector<uint32_t> plen(nch);
     for (uint32_t c = 0; c < nch; ++c) { poff[c] = ch[c].b; plen[c] = (uint32_t)(ch[c].e - ch[c].b); }
-    upload_async(ctx, ctx->z_chunk, ch.data(), nch);
-    upload_async(ctx, ctx->z_poff, poff.data(), nch);
-    upload_async(ctx, ctx->z_plen, plen.data(), nch);
-    ensure(ctx->z_m, (end + 1) * 4);
-    ensure(ctx->z_freq, (size_t)nch * kDefFreqStride * 4);
-    ensure(ctx->z_codes, (size_t)nch * sizeof(DefCodes));
-    ensure(ctx->z_hdr, (size_t)nch * kDefHdrWords * 4);
-    ensure(ctx->z_info, (size_t)nch * sizeof(DefInfo));
-    ensure(ctx->z_scratch, (size_t)nch * kDefScratch);
-    ensure(ctx->z_crc, (size_t)nch * 4);
-    CK(cudaMemsetAsync(ctx->z_freq.p, 0, (size_t)nch * kDefFreqStride * 4, ctx->stream));
-    CK(cudaMemsetAsync(ctx->z_hdr.p, 0, (size_t)nch * kDefHdrWords * 4, ctx->stream));
-    CK(cudaMemsetAsync(ctx->z_scratch.p, 0, (size_t)nch * kDefScratch, ctx->stream));
-    const DefChunk* dch = (const DefChunk*)ctx->z_chunk.p;
-    uint32_t* m = (uint32_t*)ctx->z_m.p;
-    DefInfo* dinfo = (DefInfo*)ctx->z_info.p;
+    upload_async(ctx, Z.chunk, ch.data(), nch);
+    upload_async(ctx, Z.poff, poff.data(), nch);
+    upload_async(ctx, Z.plen, plen.data(), nch);
+    ensure(Z.m, (end + 1) * 4);
+    ensure(Z.freq, (size_t)nch * kDefFreqStride * 4);
+    ensure(Z.codes, (size_t)nch * sizeof(DefCodes));
+    ensure(Z.hdr, (size_t)nch * kDefHdrWords * 4);
+    ensure(Z.info, (size_t)nch * sizeof(DefInfo));
+    ensure(Z.scratch, (size_t)nch * kDefScratch);
+    ensure(Z.crc, (size_t)nch * 4);
+    CK(cudaMemsetAsync(Z.freq.p, 0, (size_t)nch * kDefFreqStride * 4, ctx->stream));
+    CK(cudaMemsetAsync(Z.hdr.p, 0, (size_t)nch * kDefHdrWords * 4, ctx->stream));
+    CK(cudaMemsetAsync(Z.scratch.p, 0, (size_t)nch * kDefScratch, ctx->stream));
+    const DefChunk* dch = (const DefChunk*)Z.chunk.p;
+    uint32_t* m = (uint32_t*)Z.m.p;
+    DefInfo* dinfo = (DefInfo*)Z.info.p;
     def_match_kernel<<<nch, 32, 0, ctx->stream>>>(in, dch, m);
-    def_parse_kernel<<<(nch + 127) / 128, 128, 0, ctx->stream>>>(in, dch, nch, m, (uint32_t*)ctx->z_freq.p, dinfo);
-    def_code_kernel<<<(nch + 1) / 2, 64, 0, ctx->stream>>>(dch, nch, (const uint32_t*)ctx->z_freq.p, (DefCodes*)ctx->z_codes.p, (uint32_t*)ctx->z_hdr.p, dinfo);
-    def_write_kernel<<<(nch + 3) / 4, 128, 0, ctx->stream>>>(in, dch, nch, m, (const DefCodes*)ctx->z_codes.p, (const uint32_t*)ctx->z_hdr.p, dinfo,
-                                                             (uint8_t*)ctx->z_scratch.p);
-    inf_crc_kernel<<<(nch + 127) / 128, 128, 0, ctx->stream>>>(in, (const uint64_t*)ctx->z_poff.p, (const uint32_t*)ctx->z_plen.p, nch, (uint32_t*)ctx->z_crc.p);
+    def_parse_kernel<<<(nch + 127) / 128, 128, 0, ctx->stream>>>(in, dch, nch, m, (uint32_t*)Z.freq.p, dinfo);
+    def_code_kernel<<<(nch + 1) / 2, 64, 0, ctx->stream>>>(dch, nch, (const uint32_t*)Z.freq.p, (DefCodes*)Z.codes.p, (uint32_t*)Z.hdr.p, dinfo);
+    def_write_kernel<<<(nch + 3) / 4, 128, 0, ctx->stream>>>(in, dch, nch, m, (const DefCodes*)Z.codes.p, (const uint32_t*)Z.hdr.p, dinfo,
+                                                             (uint8_t*)Z.scratch.p);
+    inf_crc_kernel<<<(nch + 127) / 128, 128, 0, ctx->stream>>>(in, (const uint64_t*)Z.poff.p, (const uint32_t*)Z.plen.p, nch, (uint32_t*)Z.crc.p);
     CK(cudaGetLastError());
-    CK(cudaMemcpyAsync(info.data(), ctx->z_info.p, (size_t)nch * sizeof(DefInfo), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(crcs.data(), ctx->z_crc.p, (size_t)nch * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(info.data(), Z.info.p, (size_t)nch * sizeof(DefInfo), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(crcs.data(), Z.crc.p, (size_t)nch * 4, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
   // the byte-size scan: chunk c goes to dst[c]; every member is header, its chunks, trailer
@@ -1484,15 +1547,15 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
   so[ns] = at;
   if (at && (!out || cap < at)) fail(SMR_ERR_CAPACITY, "output buffer too small: stream_off holds the compressed sizes");
   if (nch) {
-    upload_async(ctx, ctx->z_dst, dst.data(), nch);
-    upload_async(ctx, ctx->z_trl, trl.data(), trl.size());
-    ensure(ctx->z_out, at);
-    def_place_kernel<<<nch, 256, 0, ctx->stream>>>((const DefChunk*)ctx->z_chunk.p, (const DefInfo*)ctx->z_info.p, (const uint8_t*)ctx->z_scratch.p,
-                                                   (const uint64_t*)ctx->z_dst.p, (const uint32_t*)ctx->z_trl.p, (uint8_t*)ctx->z_out.p);
+    upload_async(ctx, Z.dst, dst.data(), nch);
+    upload_async(ctx, Z.trl, trl.data(), trl.size());
+    ensure(Z.out, at);
+    def_place_kernel<<<nch, 256, 0, ctx->stream>>>((const DefChunk*)Z.chunk.p, (const DefInfo*)Z.info.p, (const uint8_t*)Z.scratch.p,
+                                                   (const uint64_t*)Z.dst.p, (const uint32_t*)Z.trl.p, (uint8_t*)Z.out.p);
     CK(cudaGetLastError());
   }
   CK(cudaEventRecord(e_dev, ctx->stream));
-  if (at) CK(cudaMemcpyAsync(out, ctx->z_out.p, at, cudaMemcpyDeviceToHost, ctx->stream));
+  if (at) CK(cudaMemcpyAsync(out, Z.out.p, at, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(e_end, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
 }
@@ -1502,7 +1565,7 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
 void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
                          const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
                          char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise) {
-  const bool mates = o->mates || (!text && ctx->resident_mates);   // the resident batch of a mate stream is mates
+  const bool mates = o->mates || (!text && ctx->res.mates);   // the resident batch of a mate stream is mates
   const bool paired = o->paired_in || o->paired_out || mates;
   if (pairwise) {   // -blast '0 cigar' is refused by the reference too (options.cpp:584-588)
     if (!o->blast || o->blast_format != 0 || o->blast_cols[0] || o->sam || o->fastx || o->other || o->denovo)
@@ -1514,54 +1577,39 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   }
   if (o->paired_in && o->paired_out) fail(SMR_ERR_ARG, "paired_in and paired_out are exclusive");
   if (!pairwise && o->sout && (o->paired_in || o->paired_out)) fail(SMR_ERR_ARG, "-sout cannot be used with paired_in or paired_out");
-  if (paired && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
   const uint32_t num_out = pairwise ? 1 : o->out2 && o->sout ? 4 : o->out2 || o->sout ? 2 : 1;   // ReportFxBase::set_num_out
   const uint32_t nfx = pairwise ? 0 : 3 * num_out;                                                // aligned, other, denovo: num_out files each
-  if ((o->sam || (o->blast && !pairwise) || o->denovo) && nreads && !stats) fail(SMR_ERR_ARG, "SAM, BLAST and denovo need the smr_aln_stats of the batch");
-  if (nreads && (!results || !alns)) fail(SMR_ERR_ARG, ctx->err);   // a null array: no text of its own, the last one stays
+  // a null results or alns array: no text of its own, the last one stays
+  rpt_check_batch(ctx, "the report writer", results, alns, stats, nreads, paired,
+                  o->sam || (o->blast && !pairwise) || o->denovo ? "SAM, BLAST and denovo need the smr_aln_stats of the batch" : nullptr, ctx->err.c_str());
   uint32_t ncols = 0, cols[4] = {0, 0, 0, 0};
   if (o->blast)
     for (; ncols < 4 && o->blast_cols[ncols]; ++ncols) {
       if (o->blast_cols[ncols] < SMR_BLAST_COL_CIGAR || o->blast_cols[ncols] > SMR_BLAST_COL_QSTRAND) fail(SMR_ERR_ARG, "unknown BLAST column");
       cols[ncols] = (uint32_t)o->blast_cols[ncols];
     }
-  const std::vector<const Part*> gp = report_groups(ctx);
-  const uint32_t G = (uint32_t)gp.size(), nso = 2 * G + nfx + 1;
-  std::vector<RptGroup> hg(G);
-  for (uint32_t g = 0; g < G; ++g) {
-    const Part& pt = *gp[g];
-    if ((o->sam || o->blast) && !pt.has_rnames)
-      fail(SMR_ERR_ARG, "smr_set_report_refs was not called for index " + std::to_string(pt.d.index_num) + " part " + std::to_string(pt.d.part));
-    const bool sc = pt.d.index_num < ctx->rpt_score.size() && ctx->rpt_score[pt.d.index_num].set;
-    if (o->blast && !sc) fail(SMR_ERR_ARG, "smr_set_report_scoring was not called for index " + std::to_string(pt.d.index_num));
-    hg[g] = RptGroup{pt.rnames, pt.rname_off, sc ? (const double*)ctx->rpt_score[pt.d.index_num].ev.p : nullptr,
-                     sc ? (const uint32_t*)ctx->rpt_score[pt.d.index_num].bits.p : nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0,
-                     pt.d.refseq, pt.d.ref_off};
-  }
-  const uint32_t slots = slots_of(ctx);
-  const uint64_t N = (uint64_t)nreads * slots;
-  if (N >= (1ull << 31)) fail(SMR_ERR_ARG, "batch too large for the report writer: split it");
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
-  CK(cudaEventRecord(e0, ctx->stream));
-  RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e1);
+  const std::vector<RptGroup> hg = rpt_groups(ctx, o->sam || o->blast, o->blast);
+  const uint32_t G = (uint32_t)hg.size(), nso = 2 * G + nfx + 1;
+  const uint64_t N = (uint64_t)nreads * slots_of(ctx);
+  cudaEvent_t* e = events(ctx, 4);
+  RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e);
   const int grid = ctx->sm_count * 8;
-  uint32_t* scal = (uint32_t*)ctx->d_scal.p;
-  uint32_t h[8];
+  auto& S = ctx->r;
   // per record, routing, row order
   const uint64_t fstride = (uint64_t)nreads + 1;
-  uint32_t* flags = ensure<uint32_t>(ctx->r_flags, fstride * 4);
-  ensure(ctx->r_keys, (N + 1) * 4);
-  ensure(ctx->r_keys2, (N + 1) * 4);
-  ensure(ctx->r_vals, (N + 1) * 4);
-  const uint32_t* rows = ensure<uint32_t>(ctx->r_rows, (N + 1) * 4);
-  uint64_t* first = ensure<uint64_t>(ctx->r_first, ((size_t)G + 1) * 8);
-  uint64_t* sz = ensure<uint64_t>(ctx->r_sz, (N + 1) * 8);
-  uint64_t* off = ensure<uint64_t>(ctx->r_off, (N + 1) * 8);
-  uint64_t* bsz = ensure<uint64_t>(ctx->r_bsz, (N + 1) * 8);
-  uint64_t* boff = ensure<uint64_t>(ctx->r_boff, (N + 1) * 8);
-  uint64_t* fxsz = ensure<uint64_t>(ctx->r_fxsz, nfx * fstride * 8);
-  uint64_t* fxoff = ensure<uint64_t>(ctx->r_fxoff, nfx * fstride * 8);
-  uint64_t* so = ensure<uint64_t>(ctx->r_so, (size_t)nso * 8);
+  uint32_t* flags = ensure<uint32_t>(S.flags, fstride * 4);
+  const uint32_t* keys = ensure<uint32_t>(S.keys, (N + 1) * 4);
+  uint32_t* keys2 = ensure<uint32_t>(S.keys2, (N + 1) * 4);
+  const uint32_t* vals = ensure<uint32_t>(S.vals, (N + 1) * 4);
+  uint32_t* rows = ensure<uint32_t>(S.rows, (N + 1) * 4);
+  uint64_t* first = ensure<uint64_t>(S.first, ((size_t)G + 1) * 8);
+  uint64_t* sz = ensure<uint64_t>(S.sz, (N + 1) * 8);
+  uint64_t* off = ensure<uint64_t>(S.off, (N + 1) * 8);
+  uint64_t* bsz = ensure<uint64_t>(S.bsz, (N + 1) * 8);
+  uint64_t* boff = ensure<uint64_t>(S.boff, (N + 1) * 8);
+  uint64_t* fxsz = ensure<uint64_t>(S.fxsz, nfx * fstride * 8);
+  uint64_t* fxoff = ensure<uint64_t>(S.fxoff, nfx * fstride * 8);
+  uint64_t* so = ensure<uint64_t>(S.so, (size_t)nso * 8);
   for (int k = 0; k < 4; ++k) a.cols[k] = cols[k];
   a.ncols = ncols; a.min_id = o->min_id; a.min_cov = o->min_cov;
   a.paired_in = o->paired_in != 0; a.paired_out = o->paired_out != 0; a.mates = mates; a.denovo = o->denovo != 0;
@@ -1573,14 +1621,11 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   CK(cudaMemsetAsync(first, 0, ((size_t)G + 1) * 8, ctx->stream));
   if (nreads) {
     rpt_route_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags);
-    rpt_row_keys_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, (uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_vals.p);
+    rpt_row_keys_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, (uint32_t*)keys, (uint32_t*)vals);
     int nbits = 1;
     while ((1u << nbits) <= G) ++nbits;
-    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) {
-      return cub::DeviceRadixSort::SortPairs(t, b, (const uint32_t*)ctx->r_keys.p, (uint32_t*)ctx->r_keys2.p, (const uint32_t*)ctx->r_vals.p,
-                                             (uint32_t*)ctx->r_rows.p, (int)N, 0, nbits, ctx->stream);
-    });
-    rpt_group_first_kernel<<<(G + 128) / 128, 128, 0, ctx->stream>>>((const uint32_t*)ctx->r_keys2.p, N, G, first);
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, keys, keys2, vals, rows, (int)N, 0, nbits, ctx->stream); });
+    rpt_group_first_kernel<<<(G + 128) / 128, 128, 0, ctx->stream>>>(keys2, N, G, first);
     if (o->sam) rpt_sam_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, sz);
     if (o->blast && pairwise) rpt_pw_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz);
     else if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz, nullptr, nullptr);
@@ -1598,19 +1643,20 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   rpt_stream_off_kernel<<<1, 32, 0, ctx->stream>>>(first, G, off, boff, fxoff, nreads, fstride, nfx, so);
   CK(cudaGetLastError());
   std::vector<uint64_t> hso(nso);
+  uint32_t err = 0;
   CK(cudaMemcpyAsync(hso.data(), so, (size_t)nso * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(h, scal, 32, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&err, a.err, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (h[4]) rpt_error(h[4]);
+  rpt_check(err);
   const uint32_t s0 = pairwise ? G : 0;   // the first stream handed out: pairwise, the BLAST streams alone (the SAM ones are empty)
   if (!gz) memcpy(so_out, hso.data() + s0, (size_t)(nso - s0) * 8);
   const uint64_t total = hso[nso - 1];
   if (!gz && total && (!out || cap < total)) fail(SMR_ERR_CAPACITY, "output buffer too small: stream_off holds the sizes");
   // the encoder reads up to 8 bytes past a stream's end (def_load32): the padding is part of the one allocation before the writes,
   // since ensure() does not keep what a buffer held
-  if (total || gz) ensure(ctx->r_out, total + (gz ? 8 : 0));
+  if (total || gz) ensure(S.out, total + (gz ? 8 : 0));
   if (total) {
-    char* dout = (char*)ctx->r_out.p;
+    char* dout = (char*)S.out.p;
     if (o->sam) rpt_sam_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, off, dout);
     if (o->blast && pairwise) rpt_pw_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, boff, dout + hso[G]);
     else if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, nullptr, boff, dout + hso[G]);
@@ -1619,33 +1665,19 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   }
   if (gz) {   // every non-empty stream to one gzip member, before the D2H
     std::vector<uint64_t> sb(hso.begin() + s0, hso.end() - 1), se(hso.begin() + s0 + 1, hso.end());
-    gzip_streams(ctx, (const uint8_t*)ctx->r_out.p, sb, se, out, cap, so_out, e2, e3);
+    gzip_streams(ctx, (const uint8_t*)S.out.p, sb, se, out, cap, so_out, e[2], e[3]);
   } else {
-    CK(cudaEventRecord(e2, ctx->stream));
-    if (total) CK(cudaMemcpyAsync(out, ctx->r_out.p, total, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaEventRecord(e3, ctx->stream));
+    CK(cudaEventRecord(e[2], ctx->stream));
+    if (total) CK(cudaMemcpyAsync(out, S.out.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaEventRecord(e[3], ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
   }
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
-  cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
-  cudaEventElapsedTime(&ms, e2, e3); ctx->t_rpt[2] = ms;
+  set_rpt_times(ctx, e);
 }
+
 // ---------------------------------------------------------------------------------------------------------------------
 // OTU map (smr_otu.cuh)
 // ---------------------------------------------------------------------------------------------------------------------
-// device buffer grown to at least `need` bytes by doubling, keeping its first `used` bytes
-void grow_keep(smr_ctx* ctx, DevBuf& b, size_t used, size_t need) {
-  if (need <= b.cap && b.p) return;
-  DevBuf nb;
-  CK(nb.alloc(std::max<size_t>({need, 2 * b.cap, 4096})));
-  if (used) {
-    CK(cudaMemcpyAsync(nb.p, b.p, used, cudaMemcpyDeviceToDevice, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-  }
-  b = std::move(nb);   // nb frees the old buffer
-}
-
 void otu_open(smr_ctx* ctx) {
   if (!ctx->otu.active) fail(SMR_ERR_ARG, "no open OTU map: call smr_otu_begin first");
   if (ctx->otu.gen != ctx->parts_gen)
@@ -1662,24 +1694,19 @@ void otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
   if (o->feed == SMR_OTU_SINGLE && (o->paired_in || o->paired_out))
     fail(SMR_ERR_UNSUPPORTED, "paired reads: the reference's OTU pass reads only the first mate file of two, but every record of one interleaved file: "
                               "say which with feed SMR_OTU_ONE_FILE or SMR_OTU_TWO_FILES");
+  U.groups = rpt_groups(ctx, true, false);
   const std::vector<const Part*> gp = report_groups(ctx);
   const uint32_t G = (uint32_t)gp.size();
-  for (const Part* pt : gp)
-    if (!pt->has_rnames)
-      fail(SMR_ERR_ARG, "smr_set_report_refs was not called for index " + std::to_string(pt->d.index_num) + " part " + std::to_string(pt->d.part));
   // ranks of the reference ids in unsigned byte order (std::string compares as unsigned char)
   std::vector<const std::string*> ids;
   for (const Part* pt : gp) for (const std::string& s : pt->h_rnames) ids.push_back(&s);
   std::sort(ids.begin(), ids.end(), [](const std::string* a, const std::string* b) { return *a < *b; });
   ids.erase(std::unique(ids.begin(), ids.end(), [](const std::string* a, const std::string* b) { return *a == *b; }), ids.end());
   std::vector<uint32_t> rank, rank_off(std::max(G, 1u), 0);
-  U.groups.assign(G, RptGroup{});
   for (uint32_t g = 0; g < G; ++g) {
-    const Part& pt = *gp[g];
     rank_off[g] = (uint32_t)rank.size();
-    for (const std::string& s : pt.h_rnames)
+    for (const std::string& s : gp[g]->h_rnames)
       rank.push_back((uint32_t)(std::lower_bound(ids.begin(), ids.end(), &s, [](const std::string* a, const std::string* b) { return *a < *b; }) - ids.begin()));
-    U.groups[g] = RptGroup{pt.rnames, pt.rname_off, nullptr, nullptr, pt.n_rnames, pt.d.index_num, pt.d.part, 0};
   }
   uint32_t gbits = 1, rbits = 1;
   while ((1ull << gbits) <= G) ++gbits;
@@ -1701,16 +1728,13 @@ uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr
                       uint32_t nreads) {
   auto& U = ctx->otu;
   otu_open(ctx);
-  if (nreads && (!results || !alns || !stats)) fail(SMR_ERR_ARG, "the OTU map needs the results, alignments and smr_aln_stats of the batch");
-  if (!text && ctx->resident_mates && U.feed != SMR_OTU_TWO_FILES)
+  if (!text && ctx->res.mates && U.feed != SMR_OTU_TWO_FILES)
     fail(SMR_ERR_UNSUPPORTED, "a mate stream's batch is two mate files: open the OTU map with feed SMR_OTU_TWO_FILES");
-  if (U.feed != SMR_OTU_SINGLE && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
-  const uint32_t slots = slots_of(ctx);
-  const uint64_t N = (uint64_t)nreads * slots;
-  if (N >= (1ull << 31)) fail(SMR_ERR_ARG, "batch too large for the OTU map: split it");
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2);
-  CK(cudaEventRecord(e0, ctx->stream));
-  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e1);
+  rpt_check_batch(ctx, "the OTU map", results, alns, stats, nreads, U.feed != SMR_OTU_SINGLE,
+                  "the OTU map needs the results, alignments and smr_aln_stats of the batch");
+  const uint64_t N = (uint64_t)nreads * slots_of(ctx);
+  cudaEvent_t* e = events(ctx, 3);
+  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e);
   const OtuArgs oa{(const uint32_t*)U.rank.p, (const uint32_t*)U.rank_off.p, U.gbits, U.min_id, U.min_cov, U.feed};
   uint32_t* flag = ensure<uint32_t>(U.flag, (N + 1) * 4);
   uint32_t* pos = ensure<uint32_t>(U.pos, (N + 1) * 4);
@@ -1726,21 +1750,20 @@ uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr
   uint32_t m = 0, err = 0; uint64_t bytes = 0;
   CK(cudaMemcpyAsync(&m, pos + N, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(&bytes, noff + N, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(&err, (uint32_t*)ctx->d_scal.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&err, a.err, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (err) rpt_error(err);
+  rpt_check(err);
   if (U.n + m >= (1ull << 31)) fail(SMR_ERR_CAPACITY, "OTU map of 2^31 entries or more");
-  grow_keep(ctx, U.key, U.n * 8, (U.n + m) * 8);
-  grow_keep(ctx, U.ent, U.n * sizeof(OtuEnt), (U.n + m) * sizeof(OtuEnt));
-  grow_keep(ctx, U.pool, U.pool_bytes, U.pool_bytes + bytes);
+  ensure_keep(ctx, U.key, (U.n + m) * 8, U.n * 8);
+  ensure_keep(ctx, U.ent, (U.n + m) * sizeof(OtuEnt), U.n * sizeof(OtuEnt));
+  ensure_keep(ctx, U.pool, U.pool_bytes + bytes, U.pool_bytes);
   if (m) otu_append_kernel<<<grid, 256, 0, ctx->stream>>>(a, oa, flag, pos, noff, U.n, U.pool_bytes, (uint64_t*)U.key.p, (OtuEnt*)U.ent.p, (char*)U.pool.p);
   CK(cudaGetLastError());
-  CK(cudaEventRecord(e2, ctx->stream));
+  CK(cudaEventRecord(e[2], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   U.n += m; U.pool_bytes += bytes;
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1); U.t[0] += ms;
-  cudaEventElapsedTime(&ms, e1, e2); U.t[1] += ms;
+  U.t[0] += elapsed_ms(e[0], e[1]);
+  U.t[1] += elapsed_ms(e[1], e[2]);
   return m;
 }
 
@@ -1748,8 +1771,8 @@ void otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) 
   auto& U = ctx->otu;
   otu_open(ctx);
   const uint64_t m = U.n;
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
-  CK(cudaEventRecord(e0, ctx->stream));
+  cudaEvent_t* e = events(ctx, 2);
+  CK(cudaEventRecord(e[0], ctx->stream));
   uint64_t bytes = 0; uint32_t runs = 0;
   const int grid = ctx->sm_count * 8;
   if (m) {
@@ -1781,10 +1804,9 @@ void otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) 
     CK(cudaGetLastError());
     CK(cudaMemcpyAsync(out, U.out.p, bytes, cudaMemcpyDeviceToHost, ctx->stream));
   }
-  CK(cudaEventRecord(e1, ctx->stream));
+  CK(cudaEventRecord(e[1], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1); U.t[2] = ms;
+  U.t[2] = elapsed_ms(e[0], e[1]);
   U.active = false;
 }
 
@@ -1793,35 +1815,28 @@ void otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) 
 // ---------------------------------------------------------------------------------------------------------------------
 void denovo_stats_impl(smr_ctx* ctx, const smr_denovo_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
                        const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4]) {
-  if (nreads && (!results || !alns || !stats)) fail(SMR_ERR_ARG, "the denovo statistics need the results, alignments and smr_aln_stats of the batch");
-  const bool paired = o->paired || (!text && ctx->resident_mates);   // the resident batch of a mate stream is mates
-  const uint32_t slots = slots_of(ctx);
-  const uint64_t N = (uint64_t)nreads * slots;
-  if (N >= (1ull << 31)) fail(SMR_ERR_ARG, "batch too large for the denovo statistics: split it");
-  std::vector<RptGroup> hg;   // the loaded (index, part)s: an alignment of any other is refused
-  for (const Part* pt : report_groups(ctx)) { RptGroup g{}; g.index_num = pt->d.index_num; g.part = pt->d.part; hg.push_back(g); }
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
-  CK(cudaEventRecord(e0, ctx->stream));
-  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, hg, e1);
-  uint32_t* dread = ensure<uint32_t>(ctx->dn_read, ((size_t)nreads + 1) * 16);
-  unsigned long long* dtot = ensure<unsigned long long>(ctx->dn_tot, 32);
+  rpt_check_batch(ctx, "the denovo statistics", results, alns, stats, nreads, false,
+                  "the denovo statistics need the results, alignments and smr_aln_stats of the batch");
+  const bool paired = o->paired || (!text && ctx->res.mates);   // the resident batch of a mate stream is mates
+  cudaEvent_t* e = events(ctx, 4);
+  // the loaded (index, part)s: an alignment of any other is refused
+  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, rpt_groups(ctx, false, false), e);
+  uint32_t* dread = ensure<uint32_t>(ctx->dn.read, ((size_t)nreads + 1) * 16);
+  unsigned long long* dtot = ensure<unsigned long long>(ctx->dn.tot, 32);
   CK(cudaMemsetAsync(dread, 0, (size_t)nreads * 16, ctx->stream));
   CK(cudaMemsetAsync(dtot, 0, 32, ctx->stream));
   if (nreads) denovo_stats_kernel<<<ctx->sm_count * 8, 256, 0, ctx->stream>>>(a, o->min_id, o->min_cov, paired, dread, dtot);
   CK(cudaGetLastError());
   uint64_t tot[4] = {0, 0, 0, 0}; uint32_t err = 0;
-  CK(cudaMemcpyAsync(&err, (uint32_t*)ctx->d_scal.p + 4, 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaEventRecord(e2, ctx->stream));
+  CK(cudaMemcpyAsync(&err, a.err, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e[2], ctx->stream));
   CK(cudaMemcpyAsync(tot, dtot, 32, cudaMemcpyDeviceToHost, ctx->stream));
   if (per_read && nreads) CK(cudaMemcpyAsync(per_read, dread, (size_t)nreads * 16, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaEventRecord(e3, ctx->stream));
+  CK(cudaEventRecord(e[3], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  if (err) rpt_error(err);
+  rpt_check(err);
   for (int k = 0; k < 4; ++k) totals[k] += tot[k];
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
-  cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
-  cudaEventElapsedTime(&ms, e2, e3); ctx->t_rpt[2] = ms;
+  set_rpt_times(ctx, e);
 }
 
 }  // namespace
@@ -2022,7 +2037,7 @@ int smr_align_batch(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_of
   HostOut out{results, alns, cigar_pool, cigar_cap, 0, counters, n_counters};
   const auto put_used = on_exit([&] { if (cigar_used) *cigar_used = out.cigar_used; });   // a pool too small fails, and names the words needed
   upload_batch_impl(ctx, seq_cat, seq_off, nreads);
-  run_impl(ctx, ctx->resident);
+  run_impl(ctx, ctx->res.b);
   download_resident(ctx, out);
   return SMR_OK;
 } SMR_CATCH(ctx)
@@ -2057,14 +2072,12 @@ int smr_upload_fastx(smr_ctx* ctx, const char* text, uint64_t nbytes, uint32_t* 
 int smr_upload_fastx_gz(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint32_t* nreads) try {
   if (!ctx || !gz || !nreads) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  *nreads = 0; ctx->resident.nreads = 0; ctx->text_bytes = 0;
+  *nreads = 0;
   const char* e = getenv("SMR_INFLATE_CHUNK");
-  // distance of the speculative block searches: 64 KB for large files, down to 8 KB so that a small file still makes thousands of spans
-  const uint64_t chunk = e ? strtoull(e, nullptr, 10) : std::min<uint64_t>(65536, std::max<uint64_t>(8192, nbytes / 8192));
-  const uint64_t total = inflate_impl(ctx, gz, nbytes, chunk);
+  const uint64_t total = inflate_impl(ctx, gz, nbytes, e ? strtoull(e, nullptr, 10) : inflate_chunk(nbytes));
   if (total == 0) return SMR_OK;
   char c0 = 0;
-  CK(cudaMemcpy(&c0, ctx->d_text.p, 1, cudaMemcpyDeviceToHost));
+  CK(cudaMemcpy(&c0, ctx->res.text.p, 1, cudaMemcpyDeviceToHost));
   *nreads = upload_fastx_impl(ctx, nullptr, total, c0);
   return SMR_OK;
 } SMR_CATCH(ctx)
@@ -2072,24 +2085,24 @@ int smr_upload_fastx_gz(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint32_t*
 int smr_resident_text(smr_ctx* ctx, char* text, uint64_t cap, uint64_t* nbytes) try {
   if (!ctx || !nbytes) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  *nbytes = ctx->text_bytes;
-  if (!text || ctx->text_bytes == 0) return SMR_OK;
-  if (cap < ctx->text_bytes) { ctx->err = "text buffer too small"; return SMR_ERR_CAPACITY; }
-  CK(cudaMemcpy(text, ctx->d_text.p, ctx->text_bytes, cudaMemcpyDeviceToHost));
+  const auto& R = ctx->res;
+  *nbytes = R.text_bytes;
+  if (!text || R.text_bytes == 0) return SMR_OK;
+  if (cap < R.text_bytes) { ctx->err = "text buffer too small"; return SMR_ERR_CAPACITY; }
+  CK(cudaMemcpy(text, R.text.p, R.text_bytes, cudaMemcpyDeviceToHost));
   return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_debug_inflate(smr_ctx* ctx, const void* gz, uint64_t nbytes, uint64_t chunk_bytes, uint8_t* out, uint64_t out_cap, uint64_t* out_bytes, uint32_t info[4]) try {
   if (!ctx || !gz || !out_bytes) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  ctx->resident.nreads = 0; ctx->text_bytes = 0;
-  if (chunk_bytes == 0) chunk_bytes = std::min<uint64_t>(65536, std::max<uint64_t>(8192, nbytes / 8192));   // as smr_upload_fastx_gz
+  if (chunk_bytes == 0) chunk_bytes = inflate_chunk(nbytes);
   *out_bytes = 0;   // as it stays if the inflate fails
   *out_bytes = inflate_impl(ctx, gz, nbytes, chunk_bytes);
-  if (info) { info[0] = ctx->inf_spans; info[1] = ctx->inf_candidates; info[2] = (uint32_t)(ctx->t_inflate * 1000.0); info[3] = (uint32_t)(ctx->t_h2d * 1000.0); }
+  if (info) { info[0] = ctx->inf.spans; info[1] = ctx->inf.candidates; info[2] = (uint32_t)(ctx->t_inflate * 1000.0); info[3] = (uint32_t)(ctx->t_h2d * 1000.0); }
   if (out && *out_bytes) {
     if (out_cap < *out_bytes) { ctx->err = "output buffer too small"; return SMR_ERR_CAPACITY; }
-    CK(cudaMemcpy(out, ctx->d_text.p, *out_bytes, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(out, ctx->res.text.p, *out_bytes, cudaMemcpyDeviceToHost));
   }
   return SMR_OK;
 } SMR_CATCH(ctx)
@@ -2098,7 +2111,7 @@ int smr_stream_begin(smr_ctx* ctx, uint32_t flags, uint64_t batch_bytes) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   const CountState before = ctx->rs.counts;
-  ctx->rs = ReadStream{};
+  close_stream(ctx->rs);
   if (flags & ~(uint32_t)(SMR_STREAM_GZ | SMR_STREAM_COUNT_ONLY | SMR_STREAM_NEXT_FILE | SMR_STREAM_MATES)) fail(SMR_ERR_ARG, "smr_stream_begin: unknown flags");
   if ((flags & SMR_STREAM_MATES) && (flags & (SMR_STREAM_COUNT_ONLY | SMR_STREAM_NEXT_FILE)))
     fail(SMR_ERR_ARG, "smr_stream_begin: a mate stream makes batches and counts nothing: count mate files one after another (SMR_STREAM_NEXT_FILE)");
@@ -2113,27 +2126,21 @@ int smr_stream_begin(smr_ctx* ctx, uint32_t flags, uint64_t batch_bytes) try {
 int smr_stream_push(smr_ctx* ctx, const void* bytes, uint64_t n, int eof) try {
   if (!ctx || (!bytes && n)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  try {
+  stream_call(ctx, [&] {
     if (ctx->rs.mates) fail(SMR_ERR_ARG, "smr_stream_push on a mate stream: push each mate with smr_stream_push_mate");
     stream_push_impl(ctx, 0, (const uint8_t*)bytes, n, eof != 0);
-  } catch (...) {
-    ctx->rs = ReadStream{};   // a stream that failed is closed
-    throw;
-  }
+  });
   return SMR_OK;
 } SMR_CATCH(ctx)
 
 int smr_stream_push_mate(smr_ctx* ctx, uint32_t mate, const void* bytes, uint64_t n, int eof) try {
   if (!ctx || (!bytes && n)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  try {
+  stream_call(ctx, [&] {
     if (!ctx->rs.mates) fail(SMR_ERR_ARG, "smr_stream_push_mate on a stream not opened with SMR_STREAM_MATES");
     if (mate != 1 && mate != 2) fail(SMR_ERR_ARG, "smr_stream_push_mate: mate must be 1 or 2");
     stream_push_impl(ctx, mate - 1, (const uint8_t*)bytes, n, eof != 0);
-  } catch (...) {
-    ctx->rs = ReadStream{};
-    throw;
-  }
+  });
   return SMR_OK;
 } SMR_CATCH(ctx)
 
@@ -2141,12 +2148,7 @@ int smr_stream_next(smr_ctx* ctx, uint32_t* nreads, int* done) try {
   if (!ctx || !nreads || !done) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   *nreads = 0; *done = 0;
-  try {
-    *nreads = stream_next_impl(ctx, done);
-  } catch (...) {
-    ctx->rs = ReadStream{};
-    throw;
-  }
+  stream_call(ctx, [&] { *nreads = stream_next_impl(ctx, done); });
   return SMR_OK;
 } SMR_CATCH(ctx)
 
@@ -2160,12 +2162,12 @@ int smr_stream_counts(smr_ctx* ctx, uint64_t out[4]) {
 int smr_resident_layout(smr_ctx* ctx, uint64_t* header_text_off, uint64_t* read_off, uint8_t* seq04, uint64_t seq_cap) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  const Batch& b = ctx->resident;
+  const Batch& b = ctx->res.b;
   const uint32_t n = b.nreads;
   if (read_off) for (uint32_t r = 0; r <= n; ++r) read_off[r] = n ? b.off32[r] : 0;
   if (header_text_off && n) {
     if (!b.from_text) { ctx->err = "the resident batch was not uploaded as text"; return SMR_ERR_ARG; }
-    CK(cudaMemcpy(header_text_off, ctx->d_hdroff.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
+    CK(cudaMemcpy(header_text_off, ctx->res.hdroff.p, (size_t)n * 8, cudaMemcpyDeviceToHost));
   }
   if (seq04 && n) {
     if (seq_cap < b.total_nt) { ctx->err = "sequence buffer too small"; return SMR_ERR_CAPACITY; }
@@ -2177,8 +2179,8 @@ int smr_resident_layout(smr_ctx* ctx, uint64_t* header_text_off, uint64_t* read_
 int smr_run_resident(smr_ctx* ctx) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  run_impl(ctx, ctx->resident);
-  ctx->t_run = ctx->resident.run;
+  run_impl(ctx, ctx->res.b);
+  ctx->t_run = ctx->res.b.run;
   return SMR_OK;
 } SMR_CATCH(ctx)
 
@@ -2187,7 +2189,7 @@ int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, 
   if (!ctx || !results || !alns) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   const uint32_t slots = slots_of(ctx);
-  const uint32_t n = ctx->resident.nreads;
+  const uint32_t n = ctx->res.b.nreads;
   memset(results, 0, (size_t)n * sizeof(smr_read_result));
   memset(alns, 0, (size_t)n * slots * sizeof(smr_aln));
   HostOut out{results, alns, cigar_pool, cigar_cap, 0, counters, n_counters};
@@ -2277,8 +2279,8 @@ int smr_gzip(smr_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t cap, 
   if (!ctx || !out_bytes || (!in && n)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   *out_bytes = 0;
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1), e2 = get_event(ctx, 2), e3 = get_event(ctx, 3);
-  CK(cudaEventRecord(e0, ctx->stream));
+  cudaEvent_t* e = events(ctx, 4);
+  CK(cudaEventRecord(e[0], ctx->stream));
   if (n == 0) {   // one empty member
     *out_bytes = sizeof kGzEmpty;
     if (!out || cap < sizeof kGzEmpty) { ctx->err = "output buffer too small: out_bytes holds the size"; return SMR_ERR_CAPACITY; }
@@ -2286,19 +2288,16 @@ int smr_gzip(smr_ctx* ctx, const void* in, uint64_t n, void* out, uint64_t cap, 
     ctx->t_rpt[0] = ctx->t_rpt[1] = ctx->t_rpt[2] = 0;
     return SMR_OK;
   }
-  ensure(ctx->z_in, n + 64);
-  CK(cudaMemsetAsync((uint8_t*)ctx->z_in.p + n, 0, 64, ctx->stream));
-  CK(cudaMemcpyAsync(ctx->z_in.p, in, n, cudaMemcpyHostToDevice, ctx->stream));
-  CK(cudaEventRecord(e1, ctx->stream));
+  ensure(ctx->z.in, n + 64);
+  CK(cudaMemsetAsync((uint8_t*)ctx->z.in.p + n, 0, 64, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->z.in.p, in, n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaEventRecord(e[1], ctx->stream));
   uint64_t so[2] = {0, 0};
   {
     const auto put_size = on_exit([&] { *out_bytes = so[1]; });   // a buffer too small fails, and names the size needed
-    gzip_streams(ctx, (const uint8_t*)ctx->z_in.p, {0}, {n}, (char*)out, cap, so, e2, e3);
+    gzip_streams(ctx, (const uint8_t*)ctx->z.in.p, {0}, {n}, (char*)out, cap, so, e[2], e[3]);
   }
-  float ms = 0;
-  cudaEventElapsedTime(&ms, e0, e1); ctx->t_rpt[0] = ms;
-  cudaEventElapsedTime(&ms, e1, e2); ctx->t_rpt[1] = ms;
-  cudaEventElapsedTime(&ms, e2, e3); ctx->t_rpt[2] = ms;
+  set_rpt_times(ctx, e);
   return SMR_OK;
 } SMR_CATCH(ctx)
 
@@ -2321,15 +2320,15 @@ int smr_debug_dpx_peak(smr_ctx* ctx, double* giga_ops_per_s) try {
   DevBuf d;
   CK(d.alloc(64));
   const int iters = 1 << 14, ctas = ctx->sm_count * 8, thr = 256;
-  cudaEvent_t e0 = get_event(ctx, 0), e1 = get_event(ctx, 1);
+  cudaEvent_t* e = events(ctx, 2);
   double best = 0;
   for (int rep = 0; rep < 4; ++rep) {
-    CK(cudaEventRecord(e0, ctx->stream));
+    CK(cudaEventRecord(e[0], ctx->stream));
     dpx_peak_kernel<<<ctas, thr, 0, ctx->stream>>>((int32_t*)d.p, iters, -2, -1000000);
     CK(cudaGetLastError());
-    CK(cudaEventRecord(e1, ctx->stream));
+    CK(cudaEventRecord(e[1], ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
-    float ms = 0; cudaEventElapsedTime(&ms, e0, e1);
+    const double ms = elapsed_ms(e[0], e[1]);
     const double ops = (double)ctas * thr * iters * 8.0;
     if (rep > 0) best = std::max(best, ops / (ms * 1e-3) / 1e9);
   }
