@@ -54,7 +54,8 @@ typedef struct {
   uint8_t is_done, is_hit;
 } smr_read_result;
 
-/* One stored alignment = s_align2 (include/ssw.hpp:44-56); slot (read * max(1,num_alignments) + k) */
+/* One stored alignment = s_align2 (include/ssw.hpp:44-56); slot (read * max(1,num_alignments) + k), or in the packed layout
+ * (smr_set_aln_layout) sum_{j<read} n_align(j) + k */
 typedef struct {
   uint32_t cigar_off, cigar_len; /* into the cigar pool; BAM style len<<4|op, op 0=M 1=I 2=D (ssw.c:750-758) */
   uint32_t ref_num;
@@ -84,6 +85,10 @@ int smr_build_index(const char* fasta_path, const char* out_prefix, uint32_t lnw
 int smr_pack_kvdb_blobs(const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar_pool, uint32_t nreads,
                         uint32_t slots, int32_t num_alignments, const uint32_t* denovo4, uint8_t* out, uint64_t out_cap,
                         uint64_t* blob_off);
+/* The same blobs from packed results (SMR_ALNS_PACKED): read r's alignments at sum_{j<r} results[j].n_align.  Gives the bytes
+ * smr_pack_kvdb_blobs gives for the strided equivalent. */
+int smr_pack_kvdb_blobs_packed(const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar_pool, uint32_t nreads,
+                               int32_t num_alignments, const uint32_t* denovo4, uint8_t* out, uint64_t out_cap, uint64_t* blob_off);
 
 /* Report-side arithmetic of one stored alignment = Read::calc_miss_gap_match (src/sortmerna/read.cpp:547-589), computed on the
  * GPU from the CIGAR it has just produced (SURVEY 8(f)(1)): what %id / %cov / NM:i / BLAST columns 3,5,6 are derived from. */
@@ -180,6 +185,36 @@ int smr_set_aln_slots(smr_ctx*, uint32_t slots);
 uint32_t smr_aln_slots(const smr_ctx*);
 uint32_t smr_aln_slots_needed(const smr_ctx*);
 
+/* Result layout of a context (default SMR_ALNS_STRIDED; another value is SMR_ERR_ARG).
+ * SMR_ALNS_STRIDED: alns[] / stats hold nreads * smr_aln_slots() entries, read r's at r * smr_aln_slots() (above).
+ * SMR_ALNS_PACKED: read r's results[r].n_align alignments are contiguous, in read order, from sum_{j<r} results[j].n_align; the
+ *   counts define the layout, so no offset array crosses the ABI.  Any num_alignments: with N > 0 it drops the empty slots, with
+ *   N == 0 a read may store any number of alignments.  A run still stores at most smr_aln_slots() alignments per read; a read that
+ *   accepts more finishes its search, counts them, and the download runs it again, with the other such reads, in batches of its
+ *   own whose arenas are sized by those counts (at most 2^24 slots per batch, environment variable SMR_RETRY_SLOTS read at
+ *   smr_init; a larger read runs alone).  Results do not depend on it.  SMR_CNT_NUM_ALIGNED and reads_matched_per_db count each
+ *   read once; SW_CALLS and the other work counters count every run.
+ *   In this layout smr_align_batch, smr_download_results and smr_set_stats_buffer are SMR_ERR_ARG (use the _packed calls), and the
+ *   report-side calls (smr_format_reports[_gz], smr_format_blast_pairwise[_gz], smr_otu_add, smr_denovo_stats) read their alns
+ *   and stats packed. */
+enum { SMR_ALNS_STRIDED = 0, SMR_ALNS_PACKED = 1 };
+int smr_set_aln_layout(smr_ctx*, uint32_t layout);
+/* smr_align_batch in the packed layout.  alns[aln_cap]; stats (nullable) [aln_cap], indexed like alns (the device always computes
+ * them in this layout: the pointer decides whether they are copied).  *aln_used = the alignments stored, *cigar_used = the CIGAR
+ * words; if either array is too small the call fails with SMR_ERR_CAPACITY and both are exact.  The batch is then resident and
+ * run: smr_download_results_packed with arrays that large writes the bytes the call would have written, without running it again.
+ * The CIGARs follow read order in cigar_pool. */
+int smr_align_batch_packed(smr_ctx*, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads, smr_read_result* results,
+                           smr_aln* alns, uint64_t aln_cap, uint64_t* aln_used, smr_aln_stats* stats, uint32_t* cigar_pool,
+                           uint64_t cigar_cap, uint64_t* cigar_used, uint64_t* counters, uint32_t n_counters);
+/* smr_download_results in the packed layout, with the arguments of smr_align_batch_packed.  The batch must have been run
+ * (smr_run_resident) in this layout at the current stride; it never changes the resident batch, and may be called again.  The
+ * first download after a run runs the reads that outgrew the stride and places every read; the library keeps that result (host
+ * memory of the size of the returned arrays) until the batch is run again or replaced, so a later download copies it. */
+int smr_download_results_packed(smr_ctx*, smr_read_result* results, smr_aln* alns, uint64_t aln_cap, uint64_t* aln_used,
+                                smr_aln_stats* stats, uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used,
+                                uint64_t* counters, uint32_t n_counters);
+
 /* Instrumentation (default OFF; the environment variable SMR_INSTR=1 turns it on at smr_init).  With it, the seed kernel counts
  * SMR_CNT_WINDOWS / BUCKETS / BUCKET_ENTRIES and the candidate kernel accounts its phases with the cycle counter (the SMR_CNT_*
  * entries from DBG_MAX_READ_CYCLES on): separate instantiations of both kernels, 2-3 % slower.  Everything a caller of the
@@ -187,7 +222,8 @@ uint32_t smr_aln_slots_needed(const smr_ctx*);
 int smr_set_instrumentation(smr_ctx*, int on);
 
 /* Optional: where the next smr_align_batch / smr_download_results stores smr_aln_stats for every stored alignment (same
- * indexing as alns[]; nullptr = do not compute).  Host buffer of nreads * max(1,num_alignments) entries. */
+ * indexing as alns[]; nullptr = do not compute).  Host buffer of nreads * max(1,num_alignments) entries.  A non-null buffer is
+ * SMR_ERR_ARG in the packed layout, whose calls take the stats array as an argument (smr_set_aln_layout). */
 int smr_set_stats_buffer(smr_ctx*, smr_aln_stats* stats);
 
 /* Input decode on the device (SURVEY 8(f)(2)): `text` = the bytes of an uncompressed FASTA or FASTQ file (or a record-aligned

@@ -31,7 +31,10 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings",
            "smr_format_reports_gz", "smr_gzip", "smr_stream_begin", "smr_stream_push", "smr_stream_next", "smr_stream_counts",
            "smr_stream_push_mate", "smr_format_blast_pairwise", "smr_format_blast_pairwise_gz",
-           "smr_denovo_stats"]
+           "smr_denovo_stats", "smr_set_aln_layout", "smr_align_batch_packed", "smr_download_results_packed", "smr_pack_kvdb_blobs_packed"]
+
+# smr_set_aln_layout: strided, nreads * slots alignments; packed, read r's n_align alignments from the sum of the counts before it
+ALN_LAYOUTS = {"strided": 0, "packed": 1}
 
 CNT_NAMES = ("num_aligned", "num_short", "sw_calls", "sw_cells", "windows", "trie_nodes", "buckets",
              "bucket_entries", "pos_entries", "lis_calls", "dbg_max_read_cycles", "dbg_sum_read_cycles", "dbg_lis_kernel_cycles",
@@ -181,22 +184,60 @@ def build_index(fasta: str, out_prefix: str, lnwin: int = 18, interval: int = 1,
 
 def pack_kvdb_blobs(out: dict, num_alignments: int, denovo: np.ndarray | None = None):
     """smr_pack_kvdb_blobs: Read::toBinString() of every read of a result dict (align() / download() / the oracle's), as
-    (blob bytes, offsets[nreads+1]).  denovo: optional (nreads, 4) uint32 counters of hostio.denovo_classes."""
+    (blob bytes, offsets[nreads+1]).  denovo: optional (nreads, 4) uint32 counters of hostio.denovo_classes.  A packed result
+    (slots == 0) goes through smr_pack_kvdb_blobs_packed."""
     L = load_library()
     res, alns, cig, slots = out["res"], out["alns"], np.ascontiguousarray(out["cigar"], np.uint32), int(out["slots"])
     n = res.shape[0]
     off = np.zeros(n + 1, np.uint64)
     dn = np.ascontiguousarray(denovo, np.uint32) if denovo is not None else None
-    args = [_ptr(res), _ptr(alns), _ptr(cig) if cig.size else C.c_void_p(0), C.c_uint32(n), C.c_uint32(slots), C.c_int32(num_alignments),
-            _ptr(dn) if dn is not None else C.c_void_p(0)]
-    rc = L.smr_pack_kvdb_blobs(*args, C.c_void_p(0), C.c_uint64(0), _ptr(off))
+    fn, name = (L.smr_pack_kvdb_blobs_packed, "smr_pack_kvdb_blobs_packed") if slots == 0 else (L.smr_pack_kvdb_blobs, "smr_pack_kvdb_blobs")
+    args = [_ptr(res), _ptr(alns) if alns.size else C.c_void_p(0), _ptr(cig) if cig.size else C.c_void_p(0), C.c_uint32(n)]
+    args += ([] if slots == 0 else [C.c_uint32(slots)]) + [C.c_int32(num_alignments), _ptr(dn) if dn is not None else C.c_void_p(0)]
+    rc = fn(*args, C.c_void_p(0), C.c_uint64(0), _ptr(off))
     if rc != 0:
-        raise SmrError(f"smr_pack_kvdb_blobs: {STATUS.get(rc, rc)}")
+        raise SmrError(f"{name}: {STATUS.get(rc, rc)}")
     buf = np.zeros(int(off[n]), np.uint8)
-    rc = L.smr_pack_kvdb_blobs(*args, _ptr(buf) if buf.size else C.c_void_p(0), C.c_uint64(buf.size), _ptr(off))
+    rc = fn(*args, _ptr(buf) if buf.size else C.c_void_p(0), C.c_uint64(buf.size), _ptr(off))
     if rc != 0:
-        raise SmrError(f"smr_pack_kvdb_blobs: {STATUS.get(rc, rc)}")
+        raise SmrError(f"{name}: {STATUS.get(rc, rc)}")
     return buf, off
+
+
+def unpack_alns(out: dict, slots: int) -> dict:
+    """The strided equivalent of a packed result (slots == 0) at stride `slots` (at least its largest n_align): "alns" and "stats"
+    with read r's alignments at r * slots, "slots" = slots, "aln_off" dropped; the rest is shared with `out`."""
+    res = out["res"]
+    n, cnt = res.shape[0], res["n_align"].astype(np.int64)
+    if cnt.size and int(cnt.max()) > slots:
+        raise ValueError(f"unpack_alns: a read stores {int(cnt.max())} alignments, more than {slots} slots")
+    off = np.asarray(out["aln_off"], np.int64)
+    read = np.repeat(np.arange(n, dtype=np.int64), cnt)
+    dst = read * slots + (np.arange(int(off[-1]) if off.size else 0, dtype=np.int64) - off[:-1][read])
+    u = {k: v for k, v in out.items() if k != "aln_off"}
+    u["alns"] = np.zeros(n * slots, ALN_DTYPE)
+    u["alns"][dst] = out["alns"]
+    if out.get("stats") is not None:
+        u["stats"] = np.zeros(n * slots, STATS_DTYPE)
+        u["stats"][dst] = out["stats"]
+    u["slots"] = slots
+    return u
+
+
+def pack_alns(out: dict) -> dict:
+    """The packed equivalent of a strided result: the inverse of unpack_alns."""
+    res, slots = out["res"], int(out["slots"])
+    cnt = res["n_align"].astype(np.int64)
+    read = np.repeat(np.arange(res.shape[0], dtype=np.int64), cnt)
+    off = np.zeros(res.shape[0] + 1, np.uint64)
+    np.cumsum(cnt, out=off[1:])
+    src = read * slots + (np.arange(int(off[-1]), dtype=np.int64) - off[:-1].astype(np.int64)[read])
+    p = dict(out)
+    p["alns"] = out["alns"][src].copy()
+    if out.get("stats") is not None:
+        p["stats"] = out["stats"][src].copy()
+    p["slots"], p["aln_off"] = 0, off
+    return p
 
 
 class SmrError(RuntimeError):
@@ -218,6 +259,9 @@ class Aligner:
         self.n_index_files = 0
         self.refs_by_index = {}
         self.parts = []          # loaded (index_num, part)
+        self.layout = "strided"  # set_aln_layout
+        self._packed_sizes = (0, 0)   # packed layout: the largest alignment count and CIGAR words named so far (_packed_call)
+        self._stats_packed = False
         self._report_refs = set()
         self._keep = []
 
@@ -246,8 +290,46 @@ class Aligner:
         self._check(self.L.smr_set_instrumentation(self.h, C.c_int(1 if on else 0)), "smr_set_instrumentation")
 
     def set_aln_slots(self, slots: int):
-        """smr_set_aln_slots: stride of the result layout in the all-alignments mode (num_alignments == 0)."""
+        """smr_set_aln_slots: stride of the result layout in the all-alignments mode (num_alignments == 0); in the packed layout, the
+        stride of the first run (reads that store more run again at their own count)."""
         self._check(self.L.smr_set_aln_slots(self.h, C.c_uint32(slots)), "smr_set_aln_slots")
+
+    def set_aln_layout(self, layout: str):
+        """smr_set_aln_layout: "strided" (default) or "packed".  Packed: align() / download() return "alns" and "stats" holding each
+        read's n_align alignments one read after another, "aln_off" (uint64, nreads + 1) where each read's start, and slots = 0;
+        format_reports / otu_add / denovo_stats / pack_kvdb_blobs take such results as they are, unpack_alns turns them strided."""
+        self._check(self.L.smr_set_aln_layout(self.h, C.c_uint32(ALN_LAYOUTS[layout])), "smr_set_aln_layout")
+        self.layout = layout
+
+    def _packed_call(self, fn, name, head, n, with_stats):
+        """smr_align_batch_packed / smr_download_results_packed.  The alignment array and the CIGAR pool start at the largest sizes
+        the library named on this Aligner (grow-only, as the strided stride is kept), and after SMR_ERR_CAPACITY they grow to the
+        sizes it names and the results are downloaded again (smr_download_results_packed: the batch is resident and run, and the
+        library keeps the placed results of its run, so that call only copies)."""
+        cap, words = self._packed_sizes
+        cap, words = max(cap, n, 1), max(words, 48 * max(n, 1) + 4096)
+        while True:
+            res = np.zeros(n, RESULT_DTYPE)
+            alns = np.zeros(cap, ALN_DTYPE)
+            stats = np.zeros(cap, STATS_DTYPE) if with_stats else None
+            pool = np.zeros(words, np.uint32)
+            counters = np.zeros(CNT_FIXED + max(1, self.n_index_files), np.uint64)
+            used, wused = C.c_uint64(0), C.c_uint64(0)
+            rc = fn(*head, _ptr(res), _ptr(alns), C.c_uint64(cap), C.byref(used), _ptr(stats) if with_stats else C.c_void_p(0), _ptr(pool),
+                    C.c_uint64(words), C.byref(wused), _ptr(counters), C.c_uint32(counters.size))
+            if rc == 5 and (used.value > cap or wused.value > words):
+                cap, words = max(cap, used.value), max(words, wused.value)
+                self._packed_sizes = (cap, words)
+                fn, name, head = self.L.smr_download_results_packed, "smr_download_results_packed", [self.h]
+                continue
+            break
+        self._check(rc, name)
+        out = self._pack(res, alns[:used.value], pool, wused.value, counters, 0)
+        out["aln_off"] = np.zeros(n + 1, np.uint64)
+        np.cumsum(res["n_align"], out=out["aln_off"][1:])
+        if with_stats:
+            out["stats"] = stats[:used.value]
+        return out
 
     def load_index_part(self, index_num: int, part: int, prefix: str, refs: hostio.References, minimal_score: int,
                         skiplengths=(18, 9, 3), lnwin: int = 18):
@@ -335,6 +417,8 @@ class Aligner:
         cat = np.ascontiguousarray(cat, np.uint8)
         off = np.ascontiguousarray(off, np.uint64)
         n = off.size - 1
+        if self.layout == "packed":
+            return self._packed_call(self.L.smr_align_batch_packed, "smr_align_batch_packed", [self.h, _ptr(cat), _ptr(off), C.c_uint32(n)], n, with_stats)
         words = 0
         while True:
             slots, res, alns, pool, cap, counters = self._outputs(n, reuse_outputs, words)
@@ -504,6 +588,10 @@ class Aligner:
     def run_resident(self, with_stats: bool = False):
         """with_stats: download() also returns calc_miss_gap_match per stored alignment (out["stats"])"""
         n = self._n_resident
+        if self.layout == "packed":   # the device computes the stats in this layout; download() copies them
+            self._stats_packed = with_stats
+            self._check(self.L.smr_run_resident(self.h), "smr_run_resident")
+            return
         self._stats = np.zeros(n * int(self.L.smr_aln_slots(self.h)), STATS_DTYPE) if with_stats else None
         self._check(self.L.smr_set_stats_buffer(self.h, _ptr(self._stats) if with_stats else C.c_void_p(0)), "smr_set_stats_buffer")
         self._check(self.L.smr_run_resident(self.h), "smr_run_resident")
@@ -511,6 +599,8 @@ class Aligner:
     def download(self):
         """smr_download_results: the results of the last run_resident(); may be called again without running again"""
         n = self._n_resident
+        if self.layout == "packed":
+            return self._packed_call(self.L.smr_download_results_packed, "smr_download_results_packed", [self.h], n, self._stats_packed)
         stats = getattr(self, "_stats", None)
         stats = np.zeros_like(stats) if stats is not None else None
         self._check(self.L.smr_set_stats_buffer(self.h, _ptr(stats) if stats is not None else C.c_void_p(0)), "smr_set_stats_buffer")
@@ -891,5 +981,6 @@ def align_files(aligner: Aligner, batch: hostio.ReadBatch):
     """Convenience: align a parsed read batch and return results + SAM rows."""
     out = aligner.align(batch.cat, batch.off)
     refs = [aligner.refs_by_index[i] for i in range(aligner.n_index_files)]
-    out["sam"] = hostio.format_sam_rows(batch, refs, out["res"], out["alns"], out["cigar"], out["slots"])
+    s = out if out["slots"] else unpack_alns(out, max(1, int(out["res"]["n_align"].max(initial=0))))   # the host formatter is strided
+    out["sam"] = hostio.format_sam_rows(batch, refs, s["res"], s["alns"], s["cigar"], s["slots"])
     return out

@@ -27,14 +27,12 @@ inline uint64_t blob_bytes(const smr_read_result& r, const smr_aln* a) {
 }
 template <class T> inline void put(uint8_t*& p, T v) { memcpy(p, &v, sizeof(T)); p += sizeof(T); }
 
-}  // namespace
-
-extern "C" int smr_pack_kvdb_blobs(const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar_pool, uint32_t nreads,
-                                   uint32_t slots, int32_t num_alignments, const uint32_t* denovo4, uint8_t* out, uint64_t out_cap,
-                                   uint64_t* blob_off) {
-  if (!results || !alns || !blob_off || slots == 0) return SMR_ERR_ARG;
+// the blobs of reads 0 .. nreads, read r's alignments at alns + first(r)
+template <class First>
+int pack_blobs(const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar_pool, uint32_t nreads, First first,
+               int32_t num_alignments, const uint32_t* denovo4, uint8_t* out, uint64_t out_cap, uint64_t* blob_off) {
   blob_off[0] = 0;
-  for (uint32_t r = 0; r < nreads; ++r) blob_off[r + 1] = blob_off[r] + blob_bytes(results[r], alns + (size_t)r * slots);
+  for (uint32_t r = 0; r < nreads; ++r) blob_off[r + 1] = blob_off[r] + blob_bytes(results[r], alns + first(r));
   if (!out) return SMR_OK;                       // sizing call
   if (blob_off[nreads] > out_cap) return SMR_ERR_CAPACITY;
   if (blob_off[nreads] && !cigar_pool) return SMR_ERR_ARG;
@@ -42,7 +40,7 @@ extern "C" int smr_pack_kvdb_blobs(const smr_read_result* results, const smr_aln
     for (uint32_t r = lo; r < hi; ++r) {
       const smr_read_result& rr = results[r];
       if (rr.n_align == 0) continue;
-      const smr_aln* a = alns + (size_t)r * slots;
+      const smr_aln* a = alns + first(r);
       uint8_t* p = out + blob_off[r];
       put<uint32_t>(p, rr.lastIndex); put<uint32_t>(p, rr.lastPart);
       for (int k = 0; k < 4; ++k) put<uint32_t>(p, denovo4 ? denovo4[(size_t)r * 4 + k] : 0u);   // c_yid_ycov, n_yid_ncov, n_nid_ycov, n_denovo
@@ -76,4 +74,24 @@ extern "C" int smr_pack_kvdb_blobs(const smr_read_result* results, const smr_aln
     for (auto& th : pool) th.join();
   }
   return SMR_OK;
+}
+
+}  // namespace
+
+extern "C" int smr_pack_kvdb_blobs(const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar_pool, uint32_t nreads,
+                                   uint32_t slots, int32_t num_alignments, const uint32_t* denovo4, uint8_t* out, uint64_t out_cap,
+                                   uint64_t* blob_off) {
+  if (!results || !alns || !blob_off || slots == 0) return SMR_ERR_ARG;
+  return pack_blobs(results, alns, cigar_pool, nreads, [slots](uint32_t r) { return (size_t)r * slots; }, num_alignments, denovo4, out, out_cap, blob_off);
+}
+
+extern "C" int smr_pack_kvdb_blobs_packed(const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar_pool, uint32_t nreads,
+                                          int32_t num_alignments, const uint32_t* denovo4, uint8_t* out, uint64_t out_cap, uint64_t* blob_off) {
+  if (!results || !blob_off) return SMR_ERR_ARG;
+  std::vector<size_t> first((size_t)nreads + 1, 0);
+  for (uint32_t r = 0; r < nreads; ++r) first[r + 1] = first[r] + results[r].n_align;
+  if (first[nreads] && !alns) return SMR_ERR_ARG;
+  static const smr_aln none{};
+  return pack_blobs(results, first[nreads] ? alns : &none, cigar_pool, nreads, [&first](uint32_t r) { return first[r]; }, num_alignments, denovo4, out,
+                    out_cap, blob_off);
 }

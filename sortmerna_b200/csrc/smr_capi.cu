@@ -7,6 +7,7 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
+#include <deque>
 #include <mutex>
 #include <string>
 #include <thread>
@@ -74,6 +75,11 @@ struct Batch {
   DevBuf seq04, seq_off, pk_off, pk03, pk03alt, has_n;
   DevBuf hits, hit_cnt, cost, bins; size_t hits_stride = 0; uint32_t cnt_stride = 0;
   DevBuf state, flags, hit_db, aln_work, out_aln, aln_stats, cigar_pool, scalars, counters; uint64_t cigar_cap_dev = 0;
+  std::vector<uint32_t> base;        // packed arenas: read r stores at [base[r], base[r + 1]) (empty: r * slots_of, the strided arenas)
+  DevBuf aln_base;                   // device copy of base
+  uint32_t run_slots = 0;            // the stride of its last run (0: not run)
+  uint64_t run_id = 0;               // which run of the context its results are (0: not run)
+  bool run_stats = false;            // its last run computed the stats
   RunTimes run;
 };
 
@@ -123,6 +129,18 @@ struct smr_ctx {
   uint32_t chunk_reads = 1u << 20;
   uint32_t need_slots = 0;       // set with SMR_ERR_CAPACITY in all-alignments mode: the stride the batch needs
   uint32_t all_slots = 16;       // stride of the result layout when num_alignments == 0 (smr_set_aln_slots)
+  uint32_t layout = SMR_ALNS_STRIDED;   // smr_set_aln_layout
+  uint64_t retry_slots = 1u << 24;      // packed layout: slot budget of one sub-batch of reads run again for their alignment count
+  uint64_t runs_made = 0;               // numbers the runs (Batch::run_id)
+  // The packed results of the resident batch's last run as download_packed places them (place_packed), kept until the batch is run
+  // again or replaced: a download retried for capacity, or repeated, only copies them.
+  struct PackedResult {
+    uint64_t run_id = 0;   // Batch::run_id of the run they come from; 0 = none
+    std::vector<smr_read_result> res; std::vector<smr_aln> alns; std::vector<smr_aln_stats> st; std::vector<uint32_t> cig;
+    std::vector<uint64_t> cnt;   // what the download adds to the caller's counters, SMR_CNT_FIXED + n_index_files entries
+    bool trace_error = false;
+    RunTimes t_run; double t_d2h = 0;
+  } pk;
   uint32_t lis_ctas_per_sm = kLisMinCtas;   // persistent CTAs of the candidate kernel per SM (matches its __launch_bounds__)
 
   // the resident batch and the text it was decoded from (smr_upload_*, smr_stream_next); clear_resident empties it
@@ -150,7 +168,7 @@ struct smr_ctx {
   // report writer (smr_report.cuh): scoring tables per index_num (smr_set_report_scoring), scratch (rpt_prologue, format_reports_impl)
   struct RptScore { bool set = false; DevBuf ev, bits; };
   std::vector<RptScore> rpt_score;
-  struct { DevBuf text, line, recs, res, aln, cig, st, flags, keys, keys2, vals, rows, first, sz, off, bsz, boff, fxsz, fxoff, grp, so, out; } r;
+  struct { DevBuf text, line, recs, res, aln, cig, st, flags, keys, keys2, vals, rows, first, sz, off, bsz, boff, fxsz, fxoff, grp, so, out, aoff, sread; } r;
   double t_rpt[3] = {0, 0, 0};
   struct { DevBuf in, chunk, m, freq, codes, hdr, info, scratch, poff, plen, crc, dst, trl, out; } z;   // gzip deflate (gzip_streams, smr_deflate.cuh)
   uint64_t parts_gen = 0;   // bumped whenever a part is loaded or its report ids are set: an open OTU map refuses to go on after that
@@ -190,6 +208,21 @@ OnExit<F> on_exit(F f) { return OnExit<F>{f}; }
 
 // alignment slots per read in every flat result array: num_alignments, or the stride set for "all alignments" (0)
 uint32_t slots_of(const smr_ctx* ctx) { return ctx->prm.num_alignments > 0 ? (uint32_t)ctx->prm.num_alignments : std::max(1u, ctx->all_slots); }
+
+bool packed(const smr_ctx* ctx) { return ctx->layout == SMR_ALNS_PACKED; }
+
+// the result slots of a batch: strided, nreads * slots_of; packed, its stored alignments (the sum of n_align)
+uint64_t result_slots(const smr_ctx* ctx, const smr_read_result* results, uint32_t nreads) {
+  if (!packed(ctx)) return (uint64_t)nreads * slots_of(ctx);
+  uint64_t n = 0;
+  for (uint32_t r = 0; r < nreads; ++r) n += results[r].n_align;
+  return n;
+}
+
+// slots of the reads [c0, c1) of a run's batch
+uint64_t batch_slots(const smr_ctx* ctx, const Batch& b, uint32_t c0, uint32_t c1) {
+  return b.base.empty() ? (uint64_t)(c1 - c0) * slots_of(ctx) : b.base[c1] - b.base[c0];
+}
 
 // grow-only: at least `bytes`; what the buffer held is not kept
 template <class T = void, bool kPinned>
@@ -419,9 +452,9 @@ RunGeom setup_arenas(smr_ctx* ctx, uint32_t scale, uint32_t max_len) {
   lg.row_cap = max_len + 2 * edges + 2 * 64 + 64;
   // planner and scorer warps wait for each other: EVERY CTA of the grid must be resident at once
   int occ = 0;
-  CK(cudaFuncSetAttribute(lis_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLisSmemBytes));
-  CK(cudaFuncSetAttribute(lis_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, kLisSmemBytes));
-  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lis_kernel<true>, kLisWarpsPerCta * 32, kLisSmemBytes));   // (same launch bounds and shared memory for both)
+  for (auto k : {lis_kernel<false, false>, lis_kernel<true, false>, lis_kernel<false, true>, lis_kernel<true, true>})
+    CK(cudaFuncSetAttribute(k, cudaFuncAttributeMaxDynamicSharedMemorySize, kLisSmemBytes));
+  CK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, lis_kernel<true, false>, kLisWarpsPerCta * 32, kLisSmemBytes));   // (same launch bounds and shared memory for all)
   if (occ < 1) fail(SMR_ERR_CUDA, "lis_kernel does not fit on an SM");
   g.lis_ctas = (uint32_t)ctx->sm_count * std::min<uint32_t>(ctx->lis_ctas_per_sm, (uint32_t)occ);
   g.lis_warps = g.lis_ctas * kPlannerWarps;   // planner warps (each owns an arena)
@@ -510,15 +543,17 @@ uint64_t read_layout(smr_ctx* ctx, Batch& b, uint32_t n, Len len) {
 // The part of an upload that does not depend on where the reads came from: b's reads and offsets are on the device and b.off32 on the
 // host; sizes the batch's other buffers for its scale and 2-bit packs the reads.
 void finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
-  const uint32_t slots = slots_of(ctx), nreads = b.nreads;
+  const uint32_t nreads = b.nreads;
   ensure(b.pk03, (size_t)(w + 4) * 4);
   ensure(b.pk03alt, (size_t)(w + 4) * 4);
   ensure(b.has_n, nreads);
   ensure(b.flags, (size_t)nreads * 4);
   ensure(b.state, (size_t)nreads * sizeof(ReadState));
   ensure(b.hit_db, (size_t)nreads * 2);
-  ensure(b.aln_work, (size_t)nreads * slots * sizeof(AlnWork));
-  ensure(b.out_aln, (size_t)nreads * slots * sizeof(OutAln));
+  const uint64_t nslots = batch_slots(ctx, b, 0, nreads);
+  ensure(b.aln_work, (size_t)nslots * sizeof(AlnWork));
+  ensure(b.out_aln, (size_t)nslots * sizeof(OutAln));
+  if (!b.base.empty()) upload_async(ctx, b.aln_base, b.base.data(), b.base.size());
   ensure(b.scalars, 512);
   ensure(b.counters, (size_t)(dcCount + 64) * 8);
   CK(cudaMemsetAsync(b.pk03.p, 0, (size_t)(w + 4) * 4, ctx->stream));
@@ -545,7 +580,8 @@ void finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
 // an empty resident batch with no text behind it
 void clear_resident(smr_ctx* ctx) {
   auto& R = ctx->res;
-  R.b.nreads = 0; R.b.from_text = false; R.text_bytes = 0; R.mates = false;
+  R.b.nreads = 0; R.b.from_text = false; R.text_bytes = 0; R.mates = false; R.b.run_id = 0;
+  ctx->pk = smr_ctx::PackedResult{};
 }
 
 // host reads -> the resident batch (no text behind it)
@@ -1124,6 +1160,9 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   const uint32_t nreads = bt.nreads;
   if (nreads == 0) return;
   const uint32_t slots = slots_of(ctx);
+  const uint64_t nslots = batch_slots(ctx, bt, 0, nreads);
+  const uint32_t* aln_base = bt.base.empty() ? nullptr : (const uint32_t*)bt.aln_base.p;
+  bt.run_slots = slots; bt.run_stats = ctx->host_stats || packed(ctx); bt.run_id = ++ctx->runs_made;
   std::lock_guard<std::mutex> dev_lock(device_kernel_mutex(ctx->device));   // held until the stream has drained
   auto& A = ctx->run;
   RunGeom g = setup_arenas(ctx, bt.scale, bt.max_len);
@@ -1137,7 +1176,7 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   ensure(A.parts, hp.size() * sizeof(DevIndex));
   CK(cudaMemcpyAsync(A.parts.p, hp.data(), hp.size() * sizeof(DevIndex), cudaMemcpyHostToDevice, ctx->stream));
   // cigar pool on the device: generous fixed share per alignment slot
-  bt.cigar_cap_dev = (uint64_t)nreads * slots * 24 * bt.scale + 4096;
+  bt.cigar_cap_dev = nslots * 24 * bt.scale + 4096;
   if (bt.cigar_cap_dev >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, "CIGAR pool of this batch would pass 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches");
   ensure(bt.cigar_pool, bt.cigar_cap_dev * 4);
   const Scalars sc = scalars_of(bt);
@@ -1147,11 +1186,13 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   CK(cudaMemsetAsync(bt.flags.p, 0, (size_t)nreads * 4, ctx->stream));
   CK(cudaMemsetAsync(bt.hit_db.p, 0xFF, (size_t)nreads * 2, ctx->stream));
   const DevParams dp = to_dev(ctx->prm);
-  lg.aln_work = (AlnWork*)bt.aln_work.p; lg.slots = slots; lg.work_next = sc.lis_next; lg.work_next_b = sc.lis_next_b;
+  lg.aln_work = (AlnWork*)bt.aln_work.p; lg.work_next = sc.lis_next; lg.work_next_b = sc.lis_next_b;
   lg.parts = (const DevIndex*)A.parts.p; lg.nparts = (uint32_t)hp.size();
+  if (aln_base) lg.aln_base = aln_base; else lg.slots = slots;
   lg.q_head = sc.q_head; lg.q_tail = sc.q_tail; lg.planners_done = sc.planners_done;
   fg.parts = (const DevIndex*)A.parts.p; fg.aln_work = (const AlnWork*)bt.aln_work.p; fg.out = (OutAln*)bt.out_aln.p;
-  fg.slots = slots; fg.cigar_pool = (uint32_t*)bt.cigar_pool.p; fg.cigar_cap = bt.cigar_cap_dev; fg.cigar_used = sc.cigar_used;
+  if (aln_base) fg.aln_base = aln_base; else fg.slots = slots;
+  fg.cigar_pool = (uint32_t*)bt.cigar_pool.p; fg.cigar_cap = bt.cigar_cap_dev; fg.cigar_used = sc.cigar_used;
   fg.work_next = sc.fin_next; fg.job_count = sc.fin_jobs;
   // events: [0] start, [1] end, and per chunk k from 2 + 5k on: seed, candidate kernel, end of it; finalize, end of it
   const uint32_t nchunks = (nreads + ctx->chunk_reads - 1) / ctx->chunk_reads;
@@ -1179,8 +1220,8 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
     CK(cudaEventRecord(ek[1], ctx->stream));
     lis_reset_kernel<<<kQueueCap / 256, 256, 0, ctx->stream>>>(lg, g.lis_warps);
     CK(cudaGetLastError());
-    if (ctx->instr) lis_kernel<true><<<g.lis_ctas, kLisWarpsPerCta * 32, kLisSmemBytes, ctx->stream>>>(b, dp, lg);
-    else lis_kernel<false><<<g.lis_ctas, kLisWarpsPerCta * 32, kLisSmemBytes, ctx->stream>>>(b, dp, lg);
+    (ctx->instr ? (aln_base ? lis_kernel<true, true> : lis_kernel<true, false>) : (aln_base ? lis_kernel<false, true> : lis_kernel<false, false>))
+        <<<g.lis_ctas, kLisWarpsPerCta * 32, kLisSmemBytes, ctx->stream>>>(b, dp, lg);
     CK(cudaGetLastError());
     CK(cudaEventRecord(ek[2], ctx->stream));
     t.launches += 2;
@@ -1188,14 +1229,17 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
     CK(cudaMemsetAsync(sc.fin_next, 0, 4, ctx->stream));
     CK(cudaMemsetAsync(sc.fin_jobs, 0, 4, ctx->stream));
     CK(cudaEventRecord(ek[3], ctx->stream));
-    fg.jobs = ensure<TraceJob>(A.tb_jobs, (size_t)n * slots * sizeof(TraceJob));
-    fg.job_list = ensure<uint32_t>(A.fin_list, (size_t)n * slots * 4);
-    fg.stats = ctx->host_stats ? ensure<AlnStats>(bt.aln_stats, (size_t)nreads * slots * sizeof(AlnStats)) : nullptr;
-    final_jobs_kernel<<<std::min<uint32_t>((n * slots + 255) / 256, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(b, fg);
+    const uint64_t chunk_slots = batch_slots(ctx, bt, c0, c0 + n);
+    fg.jobs = ensure<TraceJob>(A.tb_jobs, (size_t)chunk_slots * sizeof(TraceJob));
+    fg.job_list = ensure<uint32_t>(A.fin_list, (size_t)chunk_slots * 4);
+    // the packed layout always computes the stats: the caller's pointer only decides whether they are copied
+    fg.stats = ctx->host_stats || packed(ctx) ? ensure<AlnStats>(bt.aln_stats, (size_t)nslots * sizeof(AlnStats)) : nullptr;
+    const uint32_t jobs_grid = (uint32_t)std::min<uint64_t>((std::max<uint64_t>(chunk_slots, 1) + 255) / 256, (uint64_t)ctx->sm_count * 8);
+    (aln_base ? final_jobs_kernel<true> : final_jobs_kernel<false>)<<<jobs_grid, 256, 0, ctx->stream>>>(b, fg);
     CK(cudaGetLastError());
-    finalize_kernel<<<g.final_warps / kFinalWarpsPerCta, kFinalWarpsPerCta * 32, 0, ctx->stream>>>(b, dp, fg);
+    (aln_base ? finalize_kernel<true> : finalize_kernel<false>)<<<g.final_warps / kFinalWarpsPerCta, kFinalWarpsPerCta * 32, 0, ctx->stream>>>(b, dp, fg);
     CK(cudaGetLastError());
-    traceback_kernel<<<g.tb_threads / 128, 128, 0, ctx->stream>>>(b, dp, fg);
+    (aln_base ? traceback_kernel<true> : traceback_kernel<false>)<<<g.tb_threads / 128, 128, 0, ctx->stream>>>(b, dp, fg);
     CK(cudaGetLastError());
     CK(cudaEventRecord(ek[4], ctx->stream));
     t.launches += 3;
@@ -1385,6 +1429,206 @@ void download_resident(smr_ctx* ctx, HostOut& out) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
+// packed results (SMR_ALNS_PACKED): read r's alignments at sum_{j<r} n_align(j), every read at its own count
+// ---------------------------------------------------------------------------------------------------------------------
+// One run's results on the host.  A packed download places nothing before every read's final count is known, so it keeps the
+// results of the first run and of each re-run until then.
+struct RunHost {
+  std::vector<ReadState> st; std::vector<uint32_t> fl; std::vector<uint16_t> hdb;
+  std::vector<OutAln> oa; std::vector<AlnStats> ast; std::vector<uint32_t> cig;
+  std::vector<uint64_t> base;                  // read r's first slot in oa / ast
+  std::vector<unsigned long long> cnt;         // the device counters
+};
+
+RunHost fetch_run(smr_ctx* ctx, const Batch& b) {
+  const uint32_t n = b.nreads;
+  RunHost h;
+  h.base.resize((size_t)n + 1);
+  for (uint32_t r = 0; r <= n; ++r) h.base[r] = b.base.empty() ? (uint64_t)r * b.run_slots : b.base[r];
+  const uint64_t ns = h.base[n];
+  h.st.resize(n); h.fl.resize(n); h.hdb.resize(n); h.oa.resize(ns); h.ast.resize(ns); h.cnt.resize(dcCount + 64);
+  unsigned long long used = 0;
+  CK(cudaMemcpyAsync(h.st.data(), b.state.p, (size_t)n * sizeof(ReadState), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h.fl.data(), b.flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h.hdb.data(), b.hit_db.p, (size_t)n * 2, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h.oa.data(), b.out_aln.p, (size_t)ns * sizeof(OutAln), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h.ast.data(), b.aln_stats.p, (size_t)ns * sizeof(AlnStats), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&used, scalars_of(b).cigar_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(h.cnt.data(), b.counters.p, h.cnt.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  h.cig.resize(std::min<unsigned long long>(used, b.cigar_cap_dev));
+  if (!h.cig.empty()) CK(cudaMemcpyAsync(h.cig.data(), b.cigar_pool.p, h.cig.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return h;
+}
+
+// Where every read of the resident batch has its final results: src[r] = (run, read in that run's batch).
+struct PackedRuns {
+  std::deque<RunHost> runs;
+  std::vector<std::pair<uint32_t, uint32_t>> src;
+  bool trace_error = false;
+  uint64_t slot_reads = 0, slot_batches = 0; uint32_t slot_max = 0;   // re-runs for the alignment count (SMR_VERBOSE)
+};
+
+// Reads idx[k] of batch `from` (map[k]: their index in the resident batch) run again as batches of their own at `scale`, read k
+// with room for cap[k] alignments, in sub-batches of at most ctx->retry_slots slots (a larger read alone).  Reads that store more
+// than their room run once more at their exact count; reads that overflow their scratch go on at 8x the scale, with room for
+// max(stride, the count they reached), for 3 scales at most.  Each sub-batch frees itself when its re-runs are done.
+void rerun_packed(smr_ctx* ctx, const Batch& from, const std::vector<uint32_t>& idx, const std::vector<uint32_t>& cap,
+                  const std::vector<uint32_t>& map, uint32_t scale, int depth, bool for_slots, PackedRuns& P) {
+  if (idx.empty()) return;
+  if (depth > 3) fail(SMR_ERR_CAPACITY, "scratch overflow persists after 3 retries (" + std::to_string(idx.size()) + " reads)");
+  if (getenv("SMR_VERBOSE") && !for_slots) fprintf(stderr, "[smr] %zu reads overflowed their scratch: retrying with scale %u\n", idx.size(), scale);
+  const uint32_t S = slots_of(ctx);
+  for (size_t a = 0; a < idx.size();) {
+    size_t e = a;
+    uint64_t total = 0;
+    while (e < idx.size() && (e == a || total + cap[e] <= ctx->retry_slots)) total += cap[e++];
+    if (total >= (1ull << 31)) fail(SMR_ERR_CAPACITY, "a batch run again for its alignment count would hold 2^31 slots or more (a read that stores that many, or SMR_RETRY_SLOTS too large)");
+    const uint32_t n = (uint32_t)(e - a);
+    if (for_slots) { P.slot_reads += n; P.slot_batches += 1; for (size_t k = a; k < e; ++k) P.slot_max = std::max(P.slot_max, cap[k]); }
+    std::vector<uint32_t> src(n);
+    for (uint32_t k = 0; k < n; ++k) src[k] = from.off32[idx[a + k]];
+    Batch b;
+    b.scale = scale;
+    b.base.resize((size_t)n + 1, 0);
+    for (uint32_t k = 0; k < n; ++k) b.base[k + 1] = b.base[k] + cap[a + k];
+    const uint64_t w = read_layout(ctx, b, n, [&](uint32_t k) { return from.off32[idx[a + k] + 1] - src[k]; });
+    DevBuf d_src;
+    upload_async(ctx, d_src, src.data(), n);
+    ensure(b.seq04, b.total_nt + 64);
+    gather_reads_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
+        (const uint8_t*)from.seq04.p, (const uint32_t*)d_src.p, n, (const uint32_t*)b.seq_off.p, (uint8_t*)b.seq04.p);
+    CK(cudaGetLastError());
+    finish_upload(ctx, b, w);
+    run_impl(ctx, b);
+    ctx->t_run += b.run;
+    P.runs.push_back(fetch_run(ctx, b));
+    const uint32_t id = (uint32_t)P.runs.size() - 1;
+    const RunHost& h = P.runs.back();
+    std::vector<uint32_t> s_idx, s_cap, s_map, x_idx, x_cap, x_map;
+    for (uint32_t k = 0; k < n; ++k) {
+      const uint32_t f = h.fl[k], m = map[a + k];
+      if (f & kErrTrace) P.trace_error = true;
+      if (!f) P.src[m] = {id, k};
+      else if (f == kOvfSlots) { s_idx.push_back(k); s_cap.push_back(h.st[k].n_align); s_map.push_back(m); }
+      else { x_idx.push_back(k); x_cap.push_back(std::max(S, h.st[k].n_align)); x_map.push_back(m); }
+    }
+    rerun_packed(ctx, b, s_idx, s_cap, s_map, scale, depth, true, P);          // the count is exact now
+    rerun_packed(ctx, b, x_idx, x_cap, x_map, scale * 8, depth + 1, false, P);
+    a = e;
+  }
+}
+
+// The packed results of the resident batch's last run, placed in ctx->pk: the first run's results, every read that stored more
+// alignments than the stride run again at its own count and every read that overflowed its scratch run again at a larger one, then
+// all of them placed in read order.  The resident batch and its device results stay as they are.
+void place_packed(smr_ctx* ctx) {
+  const Batch& R = ctx->res.b;
+  const uint32_t n = R.nreads, S = slots_of(ctx);
+  smr_ctx::PackedResult& K = ctx->pk;
+  K = smr_ctx::PackedResult{};   // frees what an earlier run left
+  K.cnt.assign(SMR_CNT_FIXED + std::max(1u, ctx->n_index_files), 0);
+  ctx->t_run = R.run;
+  cudaEvent_t* e = events(ctx, 2);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  PackedRuns P;
+  P.runs.push_back(fetch_run(ctx, R));
+  CK(cudaEventRecord(e[1], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->t_d2h = elapsed_ms(e[0], e[1]);
+  P.src.resize(n);
+  std::vector<uint32_t> s_idx, s_cap, x_idx, x_cap;
+  {
+    const RunHost& h = P.runs[0];
+    for (uint32_t r = 0; r < n; ++r) {
+      const uint32_t f = h.fl[r];
+      P.src[r] = {0, r};
+      if (f & kErrTrace) P.trace_error = true;
+      if (f == kOvfSlots) { s_idx.push_back(r); s_cap.push_back(h.st[r].n_align); }
+      else if (f) { x_idx.push_back(r); x_cap.push_back(std::max(S, h.st[r].n_align)); for (int bit = 0; bit < 6; ++bit) if (f & (1u << bit)) ctx->flag_hist[bit]++; }
+    }
+  }
+  if (!s_idx.empty() || !x_idx.empty()) {
+    // the arenas grow with a retry's scale: the next run allocates them again at its own
+    const auto release = on_exit([ctx] { for (DevBuf* s : {&ctx->run.lis, &ctx->run.fin, &ctx->run.tb, &ctx->run.lane_hits}) s->reset(); });
+    rerun_packed(ctx, R, s_idx, s_cap, s_idx, R.scale, 0, true, P);
+    rerun_packed(ctx, R, x_idx, x_cap, x_idx, R.scale * 8, 1, false, P);
+  }
+  if (P.slot_reads && getenv("SMR_VERBOSE"))
+    fprintf(stderr, "[smr] packed results: %llu reads stored more than %u alignments and were run again at their own count in %llu sub-batches (largest count %u)\n",
+            (unsigned long long)P.slot_reads, S, (unsigned long long)P.slot_batches, P.slot_max);
+  uint64_t nal = 0, words = 0;
+  for (uint32_t r = 0; r < n; ++r) {
+    const RunHost& h = P.runs[P.src[r].first];
+    const uint32_t k = P.src[r].second;
+    nal += h.st[k].n_align;
+    for (uint32_t j = 0; j < h.st[k].n_align; ++j) words += h.oa[h.base[k] + j].cigar_len;
+  }
+  if (words >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, "CIGAR pool offset passes 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches");
+  K.res.resize(n); K.alns.assign(nal, smr_aln{}); K.st.resize(nal); K.cig.resize(words);
+  uint64_t at = 0, cw = 0;
+  for (uint32_t r = 0; r < n; ++r) {
+    const RunHost& h = P.runs[P.src[r].first];
+    const uint32_t k = P.src[r].second;
+    const ReadState& s = h.st[k];
+    smr_read_result& o = K.res[r];
+    o.lastIndex = s.lastIndex; o.lastPart = s.lastPart; o.hit_seeds = s.hit_seeds; o.min_index = s.min_index; o.max_index = s.max_index;
+    o.n_align = s.n_align; o.max_SW_count = s.max_SW_count; o.is_done = s.is_done; o.is_hit = s.is_hit;
+    for (uint32_t j = 0; j < s.n_align; ++j, ++at) {
+      const OutAln& d = h.oa[h.base[k] + j];
+      smr_aln& a = K.alns[at];
+      memcpy(K.cig.data() + cw, h.cig.data() + d.cigar_off, (size_t)d.cigar_len * 4);
+      a.cigar_off = (uint32_t)cw; a.cigar_len = d.cigar_len; cw += d.cigar_len;
+      a.ref_num = d.ref_num; a.ref_begin1 = d.ref_begin1; a.ref_end1 = d.ref_end1; a.read_begin1 = d.read_begin1; a.read_end1 = d.read_end1;
+      a.readlen = d.readlen; a.score1 = d.score1; a.part = d.part; a.index_num = d.index_num; a.strand = d.strand;
+      const AlnStats& t = h.ast[h.base[k] + j];
+      K.st[at] = smr_aln_stats{t.n_miss, t.n_gap, t.n_match, t.n_match_denovo};
+    }
+    if (s.is_hit) {   // Readstats: once per read, from the run that stored it
+      K.cnt[SMR_CNT_NUM_ALIGNED]++;
+      if (h.hdb[k] != 0xFFFF && SMR_CNT_FIXED + h.hdb[k] < K.cnt.size()) K.cnt[SMR_CNT_FIXED + h.hdb[k]]++;
+    }
+  }
+  // the work counters count every run (pinned to SMR_CNT_* by the static_asserts at HostOut)
+  for (const RunHost& h : P.runs)
+    for (uint32_t k = dcNumShort; k < dcCount; ++k) K.cnt[k] += h.cnt[k];
+  K.trace_error = P.trace_error;
+  K.t_run = ctx->t_run; K.t_d2h = ctx->t_d2h;
+  K.run_id = R.run_id;
+}
+
+struct PackedOut {
+  smr_read_result* results; smr_aln* alns; uint64_t aln_cap; smr_aln_stats* stats; uint32_t* cigar_pool; uint64_t cigar_cap;
+  uint64_t* counters; uint32_t n_counters;
+  uint64_t aln_used = 0, cigar_used = 0;
+};
+
+// The packed download of the resident batch's last run: placed once per run (place_packed), then copied.  Both sizes are set before
+// a capacity check can fail, and a call with arrays that large writes the same bytes.
+void download_packed(smr_ctx* ctx, PackedOut& out) {
+  const Batch& R = ctx->res.b;
+  ctx->t_run = R.run;
+  if (R.nreads == 0) return;
+  if (!R.run_stats || R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, "the resident batch was not run in the packed layout at this stride: call smr_run_resident again");
+  if (ctx->pk.run_id != R.run_id) place_packed(ctx);
+  const smr_ctx::PackedResult& K = ctx->pk;
+  ctx->t_run = K.t_run; ctx->t_d2h = K.t_d2h;
+  out.aln_used = K.alns.size(); out.cigar_used = K.cig.size();
+  if (out.aln_used > out.aln_cap)
+    fail(SMR_ERR_CAPACITY, "alignment array too small: the batch stores " + std::to_string(out.aln_used) + " alignments, aln_cap is " + std::to_string(out.aln_cap));
+  if (out.cigar_used > out.cigar_cap)
+    fail(SMR_ERR_CAPACITY, "cigar pool too small: the batch needs " + std::to_string(out.cigar_used) + " words, cigar_cap is " + std::to_string(out.cigar_cap));
+  memcpy(out.results, K.res.data(), K.res.size() * sizeof(smr_read_result));
+  if (!K.alns.empty()) memcpy(out.alns, K.alns.data(), K.alns.size() * sizeof(smr_aln));
+  if (out.stats && !K.st.empty()) memcpy(out.stats, K.st.data(), K.st.size() * sizeof(smr_aln_stats));
+  if (!K.cig.empty()) memcpy(out.cigar_pool, K.cig.data(), K.cig.size() * 4);
+  if (out.counters)
+    for (uint32_t k = 0; k < out.n_counters && k < K.cnt.size(); ++k) out.counters[k] += K.cnt[k];
+  if (K.trace_error) fail(SMR_ERR_INDEX, "trace back error (ssw.c:707 is fatal in the reference too)");
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
 // report writer (smr_report.cuh)
 // ---------------------------------------------------------------------------------------------------------------------
 // fails with the text of the report error bits e (RptArgs::err), if any
@@ -1404,7 +1648,7 @@ void rpt_check_batch(const smr_ctx* ctx, const char* what, const smr_read_result
   if (nreads && stats_msg && !stats) fail(SMR_ERR_ARG, stats_msg);
   if (nreads && (!results || !alns)) fail(SMR_ERR_ARG, arrays_msg ? arrays_msg : stats_msg);
   if (paired && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
-  if ((uint64_t)nreads * slots_of(ctx) >= (1ull << 31)) fail(SMR_ERR_ARG, std::string("batch too large for ") + what + ": split it");
+  if (result_slots(ctx, results, nreads) >= (1ull << 31)) fail(SMR_ERR_ARG, std::string("batch too large for ") + what + ": split it");
 }
 
 // the loaded (index, part)s in the reference's report order (index, then part)
@@ -1439,7 +1683,7 @@ RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_
   auto& S = ctx->r;
   CK(cudaEventRecord(e[0], ctx->stream));
   const uint32_t slots = slots_of(ctx), G = (uint32_t)hg.size();
-  const uint64_t N = (uint64_t)nreads * slots;
+  const uint64_t N = result_slots(ctx, results, nreads);
   // the text
   const uint8_t* dt;
   if (text) {
@@ -1468,7 +1712,7 @@ RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_
   const auto& X = ctx->tx;
   RptArgs a{};
   a.text = dt; a.nbytes = nbytes; a.nl = (const uint64_t*)X.nl.p; a.spos = (const uint32_t*)X.spos.p; a.nlines = L.nlines; a.fastq = L.fmt == kFmtFastq;
-  a.rec = (const RptRec*)S.recs.p; a.nreads = nreads; a.slots = slots;
+  a.rec = (const RptRec*)S.recs.p; a.nreads = nreads; a.slots = slots; a.nslots = N;
   a.res = (const smr_read_result*)S.res.p; a.aln = (const smr_aln*)S.aln.p; a.cigar = (const uint32_t*)S.cig.p;
   a.cigar_words = cigar ? cigar_words : 0; a.st = (const smr_aln_stats*)S.st.p;
   a.grp = (const RptGroup*)S.grp.p; a.ngroups = G; a.err = &text_words(ctx)->rpt_err;
@@ -1477,6 +1721,15 @@ RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_
     const int grid = ctx->sm_count * 8;
     rpt_header_lines_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)X.hdr.p, (const uint32_t*)X.rec.p, L.nlines, (uint32_t*)S.line.p);
     rpt_records_kernel<<<grid, 256, 0, ctx->stream>>>(a, (const uint32_t*)S.line.p, (RptRec*)S.recs.p);
+    if (packed(ctx)) {   // where each read's alignments start, and the read of each slot
+      uint32_t* aoff = ensure<uint32_t>(S.aoff, fstride * 4);
+      rpt_counts_kernel<<<grid, 256, 0, ctx->stream>>>(a.res, nreads, aoff);
+      exclusive_sum(ctx, aoff, aoff, nreads + 1);
+      a.aln_off = aoff;
+      a.slot_read = ensure<uint32_t>(S.sread, (N + 1) * 4);
+      rpt_slot_read_kernel<<<grid, 256, 0, ctx->stream>>>(a.res, nreads, aoff, (uint32_t*)a.slot_read);
+    }
+    CK(cudaGetLastError());
   }
   return a;
 }
@@ -1590,9 +1843,9 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
     }
   const std::vector<RptGroup> hg = rpt_groups(ctx, o->sam || o->blast, o->blast);
   const uint32_t G = (uint32_t)hg.size(), nso = 2 * G + nfx + 1;
-  const uint64_t N = (uint64_t)nreads * slots_of(ctx);
   cudaEvent_t* e = events(ctx, 4);
   RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e);
+  const uint64_t N = a.nslots;
   const int grid = ctx->sm_count * 8;
   auto& S = ctx->r;
   // per record, routing, row order
@@ -1732,9 +1985,9 @@ uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr
     fail(SMR_ERR_UNSUPPORTED, "a mate stream's batch is two mate files: open the OTU map with feed SMR_OTU_TWO_FILES");
   rpt_check_batch(ctx, "the OTU map", results, alns, stats, nreads, U.feed != SMR_OTU_SINGLE,
                   "the OTU map needs the results, alignments and smr_aln_stats of the batch");
-  const uint64_t N = (uint64_t)nreads * slots_of(ctx);
   cudaEvent_t* e = events(ctx, 3);
   const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e);
+  const uint64_t N = a.nslots;
   const OtuArgs oa{(const uint32_t*)U.rank.p, (const uint32_t*)U.rank_off.p, U.gbits, U.min_id, U.min_cov, U.feed};
   uint32_t* flag = ensure<uint32_t>(U.flag, (N + 1) * 4);
   uint32_t* pos = ensure<uint32_t>(U.pos, (N + 1) * 4);
@@ -1869,6 +2122,7 @@ int smr_init(int device, smr_ctx** out) try {
   if (cudaStreamCreateWithFlags(&ctx->stream, cudaStreamNonBlocking) != cudaSuccess) { delete ctx; return SMR_ERR_CUDA; }
   if (const char* e = getenv("SMR_CHUNK_READS")) { const long v = atol(e); if (v >= 32 && v <= (1l << 22)) ctx->chunk_reads = (uint32_t)v; }   // tests: several chunks per batch
   if (const char* e = getenv("SMR_INSTR")) ctx->instr = atoi(e) != 0;   // instrumented instantiations of the seed and candidate kernels (smr_set_instrumentation)
+  if (const char* e = getenv("SMR_RETRY_SLOTS")) { const long long v = atoll(e); if (v >= 1) ctx->retry_slots = (uint64_t)v; }   // tests: many sub-batches
   if (const char* e = getenv("SMR_LIS_CTAS_PER_SM")) { const int v = atoi(e); if (v >= 1 && v <= 16) ctx->lis_ctas_per_sm = (uint32_t)v; }
   *out = ctx;
   return SMR_OK;
@@ -2027,9 +2281,21 @@ int smr_index_info(const smr_ctx* ctx, uint64_t out[6]) {
   return SMR_OK;
 }
 
+int smr_set_aln_layout(smr_ctx* ctx, uint32_t layout) {
+  if (!ctx) return SMR_ERR_ARG;
+  if (layout != SMR_ALNS_STRIDED && layout != SMR_ALNS_PACKED) { ctx->err = "smr_set_aln_layout: unknown layout " + std::to_string(layout); return SMR_ERR_ARG; }
+  ctx->layout = layout;
+  return SMR_OK;
+}
+
+// the strided entry points have no alignment capacity to size a packed result by
+#define SMR_REFUSE_PACKED(ctx, call, instead)                                                                      \
+  if (packed(ctx)) { (ctx)->err = call " writes the strided layout: in the packed layout call " instead; return SMR_ERR_ARG; }
+
 int smr_align_batch(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads, smr_read_result* results, smr_aln* alns,
                     uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used, uint64_t* counters, uint32_t n_counters) try {
   if (!ctx || !seq_cat || !seq_off || !results || !alns || (!cigar_pool && cigar_cap)) return SMR_ERR_ARG;
+  SMR_REFUSE_PACKED(ctx, "smr_align_batch", "smr_align_batch_packed")
   CK(cudaSetDevice(ctx->device));
   const uint32_t slots = slots_of(ctx);
   memset(results, 0, (size_t)nreads * sizeof(smr_read_result));
@@ -2050,6 +2316,7 @@ int smr_set_instrumentation(smr_ctx* ctx, int on) {
 
 int smr_set_stats_buffer(smr_ctx* ctx, smr_aln_stats* stats) {
   if (!ctx) return SMR_ERR_ARG;
+  if (stats) SMR_REFUSE_PACKED(ctx, "smr_set_stats_buffer", "smr_align_batch_packed / smr_download_results_packed with their stats argument")
   ctx->host_stats = stats;
   return SMR_OK;
 }
@@ -2179,6 +2446,7 @@ int smr_resident_layout(smr_ctx* ctx, uint64_t* header_text_off, uint64_t* read_
 int smr_run_resident(smr_ctx* ctx) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
+  ctx->pk = smr_ctx::PackedResult{};   // the packed results of the batch's previous run
   run_impl(ctx, ctx->res.b);
   ctx->t_run = ctx->res.b.run;
   return SMR_OK;
@@ -2187,6 +2455,7 @@ int smr_run_resident(smr_ctx* ctx) try {
 int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used,
                          uint64_t* counters, uint32_t n_counters) try {
   if (!ctx || !results || !alns) return SMR_ERR_ARG;
+  SMR_REFUSE_PACKED(ctx, "smr_download_results", "smr_download_results_packed")
   CK(cudaSetDevice(ctx->device));
   const uint32_t slots = slots_of(ctx);
   const uint32_t n = ctx->res.b.nreads;
@@ -2197,6 +2466,37 @@ int smr_download_results(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, 
   download_resident(ctx, out);
   return SMR_OK;
 } SMR_CATCH(ctx)
+
+// the packed calls' shared part: the results of the resident batch's last run, written as download_packed places them
+static int packed_call(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, uint64_t aln_cap, uint64_t* aln_used, smr_aln_stats* stats,
+                uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used, uint64_t* counters, uint32_t n_counters,
+                const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads, bool align) try {
+  if (!ctx) return SMR_ERR_ARG;
+  if (!results || (!alns && aln_cap) || (!cigar_pool && cigar_cap) || (align && (!seq_cat || !seq_off))) { ctx->err = "null result array"; return SMR_ERR_ARG; }
+  if (!packed(ctx)) { ctx->err = "the packed calls need smr_set_aln_layout(ctx, SMR_ALNS_PACKED)"; return SMR_ERR_ARG; }
+  CK(cudaSetDevice(ctx->device));
+  PackedOut out{results, alns, aln_cap, stats, cigar_pool, cigar_cap, counters, n_counters};
+  const auto put_used = on_exit([&] { if (aln_used) *aln_used = out.aln_used; if (cigar_used) *cigar_used = out.cigar_used; });
+  if (align) {
+    upload_batch_impl(ctx, seq_cat, seq_off, nreads);
+    run_impl(ctx, ctx->res.b);
+  }
+  memset(results, 0, (size_t)ctx->res.b.nreads * sizeof(smr_read_result));
+  download_packed(ctx, out);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_align_batch_packed(smr_ctx* ctx, const uint8_t* seq_cat, const uint64_t* seq_off, uint32_t nreads, smr_read_result* results,
+                           smr_aln* alns, uint64_t aln_cap, uint64_t* aln_used, smr_aln_stats* stats, uint32_t* cigar_pool, uint64_t cigar_cap,
+                           uint64_t* cigar_used, uint64_t* counters, uint32_t n_counters) {
+  return packed_call(ctx, results, alns, aln_cap, aln_used, stats, cigar_pool, cigar_cap, cigar_used, counters, n_counters, seq_cat, seq_off, nreads, true);
+}
+
+int smr_download_results_packed(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, uint64_t aln_cap, uint64_t* aln_used,
+                                smr_aln_stats* stats, uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used, uint64_t* counters,
+                                uint32_t n_counters) {
+  return packed_call(ctx, results, alns, aln_cap, aln_used, stats, cigar_pool, cigar_cap, cigar_used, counters, n_counters, nullptr, nullptr, 0, false);
+}
 
 int smr_set_report_refs(smr_ctx* ctx, uint32_t index_num, uint32_t part, const char* names_cat, const uint64_t* name_off, uint32_t nref) try {
   if (!ctx || !name_off || (!names_cat && name_off[nref])) return SMR_ERR_ARG;

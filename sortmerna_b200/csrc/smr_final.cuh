@@ -32,16 +32,41 @@ struct FinalGlobals {
   uint8_t* arena_base; size_t arena_stride;
   uint32_t cap_w, cap_cig, row_cap; size_t cap_dir;
   const DevIndex* parts;             // [nparts] device copy
-  const AlnWork* aln_work; OutAln* out; uint32_t slots;
+  const AlnWork* aln_work; OutAln* out;
+  union {                            // one or the other, as in LisGlobals (a larger FinalGlobals changes the strided kernels' code)
+    uint32_t slots;                  // <kPacked = false> kernels: read r's alignments at r * slots
+    const uint32_t* aln_base;        // <kPacked = true> kernels: [nreads + 1] packed arenas (LisGlobals::aln_base)
+  };
   uint32_t* cigar_pool; unsigned long long cigar_cap; unsigned long long* cigar_used;
   uint32_t* work_next;
-  // the stored alignments of the chunk: job_list[0 .. *job_count) = (read in chunk) * slots + slot (final_jobs_kernel)
+  // the stored alignments of the chunk: job_list[0 .. *job_count) = slots of the chunk from its first one (final_slot)
   uint32_t* job_list; uint32_t* job_count;
   // traceback stage (one THREAD per alignment)
-  struct TraceJob* jobs;             // [nreads_chunk * slots], indexed like job_list
+  struct TraceJob* jobs;             // [slots of the chunk], indexed like job_list
   uint8_t* tb_arena; size_t tb_stride; uint32_t tb_cap_w, tb_cap_cig; size_t tb_cap_dir;
-  AlnStats* stats;                   // [nreads * slots] or nullptr
+  AlnStats* stats;                   // indexed like out, or nullptr
 };
+
+// Slot wi of the chunk (counted from the chunk's first slot): its read r, its index k among r's alignments, and (packed) `at`, its
+// index in aln_work / out / stats (final_at).  Strided: wi = (read in chunk) * slots + k.  Packed: r is the last read whose first
+// slot is at or before at.
+struct FinalSlot { uint32_t r, k; size_t at; };
+__device__ __noinline__ FinalSlot final_slot_packed(const uint32_t* __restrict__ base, const uint32_t r0, const uint32_t n, const uint32_t wi) {
+  const uint32_t at = base[r0] + wi;
+  uint32_t lo = r0, hi = r0 + n - 1;
+  while (lo < hi) { const uint32_t m = (lo + hi + 1) / 2; if (base[m] <= at) lo = m; else hi = m - 1; }
+  return FinalSlot{lo, at - base[lo], at};
+}
+__device__ __forceinline__ FinalSlot final_slot_strided(const DevBatch& b, const FinalGlobals& g, const uint32_t wi) {
+  return FinalSlot{b.r0 + wi / g.slots, wi % g.slots, 0};
+}
+template <bool kPacked>
+__device__ __forceinline__ FinalSlot final_slot(const DevBatch& b, const FinalGlobals& g, const uint32_t wi) {
+  return kPacked ? final_slot_packed(g.aln_base, b.r0, b.nreads, wi) : final_slot_strided(b, g, wi);
+}
+// the index of slot s in aln_work / out / stats (strided: computed where it is used, so that the strided kernels keep their code)
+template <bool kPacked>
+__device__ __forceinline__ size_t final_at(const FinalGlobals& g, const FinalSlot& s) { return kPacked ? s.at : (size_t)s.r * g.slots + s.k; }
 __host__ __device__ inline size_t final_arena_bytes(uint32_t cap_w, uint32_t cap_cig, uint32_t row_cap, size_t cap_dir) {
   size_t b = (size_t)cap_w * 12 + (size_t)cap_cig * 4 + (size_t)row_cap * 8 + cap_dir;
   return (b + 255) & ~(size_t)255;
@@ -53,17 +78,19 @@ constexpr int kFinalWarpsPerCta = 4;
 #endif
 constexpr int kFinalCtasPerSm = SMR_FINAL_MIN_CTAS;
 
-// the dense job list: every live (read, slot) of the chunk -- slot k < n_align of a read without flags -- in any order
+// the dense job list: every live (read, slot) of the chunk -- slot k < n_align of a read without flags -- in any order.  A read
+// flagged kOvfSlots is not traced back: its alignments are stored again by a run at its own size, or the call fails.
+template <bool kPacked>
 __global__ void __launch_bounds__(256)
 final_jobs_kernel(DevBatch b, FinalGlobals g) {
-  const uint32_t total = b.nreads * g.slots;
+  const uint32_t total = kPacked ? g.aln_base[b.r0 + b.nreads] - g.aln_base[b.r0] : b.nreads * g.slots;
   const unsigned lane = lane_id();
   for (uint32_t w0 = (blockIdx.x * blockDim.x + threadIdx.x) & ~31u; w0 < total; w0 += gridDim.x * blockDim.x) {
     const uint32_t wi = w0 + lane;
     bool live = false;
     if (wi < total) {
-      const uint32_t r = b.r0 + wi / g.slots, k = wi % g.slots;
-      live = k < b.state[r].n_align && !b.flags[r];
+      const FinalSlot s = final_slot<kPacked>(b, g, wi);
+      live = s.k < b.state[s.r].n_align && !b.flags[s.r];
     }
     const unsigned m = __ballot_sync(kFull, live);
     if (!m) continue;
@@ -94,10 +121,12 @@ __device__ __forceinline__ TraceArena final_arena(const FinalGlobals& g, const u
   return A;
 }
 
-// the locate problem of stored alignment wi = (read in chunk) * slots + slot: query segment, window, score
+// the locate problem of stored alignment wi (final_slot): query segment, window, score
+template <bool kPacked>
 __device__ __forceinline__ PairLoc final_loc(const DevBatch& b, const FinalGlobals& g, const uint32_t wi) {
-  const uint32_t r = b.r0 + wi / g.slots, k = wi % g.slots;
-  const AlnWork a = g.aln_work[(size_t)r * g.slots + k];
+  const FinalSlot s = final_slot<kPacked>(b, g, wi);
+  const uint32_t r = s.r;
+  const AlnWork a = g.aln_work[final_at<kPacked>(g, s)];
   const DevIndex& ix = g.parts[a.idx_slot];
   const uint32_t seq_base = b.seq_off[r], len = b.seq_off[r + 1] - seq_base;
   PairLoc L;
@@ -117,10 +146,11 @@ __device__ __forceinline__ PairLoc reverse_loc(const PairLoc& L, const uint32_t 
 // The rest of one job after the packed passes: packed = both end points came from them (kPairNoHit: no cell held the score);
 // otherwise sw_forward runs here, forward and on the reversed prefixes ending at its end point.  Then the output row and the
 // traceback job.
+template <bool kPacked>
 __device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, const FinalGlobals& g, int32_t* rowH, int32_t* rowF,
                                           const uint32_t ji, const uint32_t wi, const bool packed, const uint32_t ef, const uint32_t er) {
   const unsigned lane = lane_id();
-  const PairLoc L = final_loc(b, g, wi);
+  const PairLoc L = final_loc<kPacked>(b, g, wi);
   SwEnd fwd{0, -1, 0}, rev{0, -1, 0};
   if (packed) {
     if (ef != kPairNoHit) fwd = SwEnd{L.target, (int32_t)(ef >> 16), (int32_t)(ef & 0xFFFFu)};
@@ -130,7 +160,8 @@ __device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, c
     if ((fwd.score & 0xFFFF) == L.target) rev = sw_forward(L.q.reversed_prefix(fwd.read), fwd.read + 1, L.t.reversed_prefix(fwd.ref), fwd.ref + 1, sc, rowH, rowF);
   }
   if (lane != 0) return;
-  const uint32_t r = b.r0 + wi / g.slots, k = wi % g.slots;
+  const FinalSlot s = final_slot<kPacked>(b, g, wi);
+  const uint32_t r = s.r;
   TraceJob j;
   if ((fwd.score & 0xFFFF) != L.target || rev.score != L.target) {
     atomicOr(&b.flags[r], kErrTrace);
@@ -138,7 +169,7 @@ __device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, c
     g.jobs[ji] = j;
     return;
   }
-  const AlnWork a = g.aln_work[(size_t)r * g.slots + k];
+  const AlnWork a = g.aln_work[final_at<kPacked>(g, s)];
   const int32_t a_ref_end = fwd.ref, a_read_end = fwd.read;
   const int32_t ref_begin = a_ref_end - rev.ref, read_begin = a_read_end - rev.read;
   const int32_t rl = a_ref_end - ref_begin + 1, ql = a_read_end - read_begin + 1;
@@ -148,7 +179,7 @@ __device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, c
   o.ref_begin1 = ref_begin + (int32_t)a.win_ref_start; o.ref_end1 = a_ref_end + (int32_t)a.win_ref_start;   // alignment.cpp:396-399
   o.read_begin1 = read_begin + (int32_t)a.q_start; o.read_end1 = a_read_end + (int32_t)a.q_start;
   o.readlen = b.seq_off[r + 1] - b.seq_off[r]; o.score1 = a.score1; o.part = a.part; o.index_num = a.index_num; o.strand = a.strand; o.pad = 0;
-  g.out[(size_t)r * g.slots + k] = o;
+  g.out[final_at<kPacked>(g, s)] = o;
   const SeqView qs = L.q.sub(read_begin);
   j.valid = 1; j.idx_slot = a.idx_slot; j.ref_num = a.ref_num; j.ref_off = a.win_ref_start + (uint32_t)ref_begin;
   j.q_start = qs.start; j.q_step = qs.step; j.rl = rl; j.ql = ql; j.score = (int32_t)a.score1; j.band = band;
@@ -157,7 +188,9 @@ __device__ __noinline__ void final_finish(const DevBatch& b, const SwScore sc, c
 
 // Forward pass again, now with the end-point tie-breaks (ssw.c:310-336), then the reverse pass over the prefixes that end at the
 // forward optimum, for the jobs job_list[2i], job_list[2i + 1] of a warp: both in one packed pass (sw_pair_run) where their
-// shapes and the scores allow it (sw_pair_ok), sw_forward otherwise; a lone last job runs with an empty second half.
+// shapes and the scores allow it (sw_pair_ok), sw_forward otherwise; a lone last job runs with an empty second half.  kPacked: as
+// traceback_kernel.
+template <bool kPacked>
 __global__ void __launch_bounds__(kFinalWarpsPerCta * 32, kFinalCtasPerSm)
 finalize_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
   __shared__ FinalSmem s_fin[kFinalWarpsPerCta];
@@ -178,23 +211,25 @@ finalize_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
     uint2 ef = make_uint2(kPairNoHit, kPairNoHit), er = ef;
     bool p0, p1;
     {
-      const PairLoc L0 = final_loc(b, g, w0), L1 = two ? final_loc(b, g, w1) : no_loc();
+      const PairLoc L0 = final_loc<kPacked>(b, g, w0), L1 = two ? final_loc<kPacked>(b, g, w1) : no_loc();
       p0 = final_packed(L0, sc); p1 = two && final_packed(L1, sc);
       if (p0 || p1) ef = sw_pair_run<true>(p0 ? L0 : no_loc(), p1 ? L1 : no_loc(), sc, S.prof, S.win[0], S.win[1]);
     }
     const bool r0 = p0 && ef.x != kPairNoHit, r1 = p1 && ef.y != kPairNoHit;
     if (r0 || r1) {
-      const PairLoc R0 = r0 ? reverse_loc(final_loc(b, g, w0), ef.x) : no_loc(), R1 = r1 ? reverse_loc(final_loc(b, g, w1), ef.y) : no_loc();
+      const PairLoc R0 = r0 ? reverse_loc(final_loc<kPacked>(b, g, w0), ef.x) : no_loc(), R1 = r1 ? reverse_loc(final_loc<kPacked>(b, g, w1), ef.y) : no_loc();
       er = sw_pair_run<true>(R0, R1, sc, S.prof, S.win[0], S.win[1]);
     }
-    final_finish(b, sc, g, rowH, rowF, j0, w0, p0, ef.x, er.x);
-    if (two) final_finish(b, sc, g, rowH, rowF, j0 + 1, w1, p1, ef.y, er.y);
+    final_finish<kPacked>(b, sc, g, rowH, rowF, j0, w0, p0, ef.x, er.x);
+    if (two) final_finish<kPacked>(b, sc, g, rowH, rowF, j0 + 1, w1, p1, ef.y, er.y);
     __syncwarp();
   }
 }
 
 // banded_sw (ssw.c:577-773) for every stored alignment, one THREAD per alignment (the DP rows are a serial chain of
-// 3..2*band+1 cells; 32 alignments per warp keep the lanes busy where one-lane-per-warp left 31 idle)
+// 3..2*band+1 cells; 32 alignments per warp keep the lanes busy where one-lane-per-warp left 31 idle).  kPacked: the run's arenas
+// are packed (g.aln_base); the strided instantiation is the code it was before packed arenas existed.
+template <bool kPacked>
 __global__ void __launch_bounds__(128)
 traceback_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
   const uint32_t tid = blockIdx.x * blockDim.x + threadIdx.x, nthreads = gridDim.x * blockDim.x;
@@ -214,7 +249,8 @@ traceback_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
     const TraceJob j = g.jobs[ji];
     if (!j.valid) continue;
     const uint32_t wi = g.job_list[ji];
-    const uint32_t r = b.r0 + wi / g.slots, k = wi % g.slots;
+    const FinalSlot s = final_slot<kPacked>(b, g, wi);
+    const uint32_t r = s.r;
     const DevIndex& ix = g.parts[j.idx_slot];
     const SeqView t{ix.refseq + ix.ref_off[j.ref_num], (int32_t)j.ref_off, 1, false};
     const SeqView q{b.seq04 + b.seq_off[r], j.q_start, j.q_step, j.q_step < 0};
@@ -224,7 +260,8 @@ traceback_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
     const unsigned long long off = atomicAdd(g.cigar_used, (unsigned long long)nc);
     if (off + (unsigned long long)nc > g.cigar_cap) { atomicOr(&b.flags[r], kOvfCigar); continue; }
     for (int32_t i = 0; i < nc; ++i) g.cigar_pool[off + i] = A.cig[(size_t)(nc - 1 - i) * 32];        // ssw.c:750-758 (reverse)
-    OutAln* o = g.out + (size_t)r * g.slots + k;
+    const size_t at = final_at<kPacked>(g, s);
+    OutAln* o = g.out + at;
     o->cigar_off = (uint32_t)off; o->cigar_len = (uint32_t)nc;
     if (g.stats) {   // Read::calc_miss_gap_match (read.cpp:547-589): walk the CIGAR over the 0-4 codes of reference and read
       // qd: the read as denovo_stats_run sees it (processor.cpp:329-333: 0-4 codes, never reverse-complemented)
@@ -243,7 +280,7 @@ traceback_kernel(DevBatch b, DevParams prm, FinalGlobals g) {
         else if (op == 1) { y += (int32_t)ln; gap += ln; }
         else { x += (int32_t)ln; gap += ln; }
       }
-      g.stats[(size_t)r * g.slots + k] = AlnStats{miss, gap, match, match_d};
+      g.stats[at] = AlnStats{miss, gap, match, match_d};
     }
   }
 }

@@ -191,8 +191,13 @@ struct LisGlobals {
   uint32_t* done;                              // [planners] tasks scored so far for each planner
   int32_t* score_rows;                         // [scorers][2 * row_cap] scratch of the s32 row-block fallback
   unsigned long long* dbg;                     // [16] phase cycles of the read that took longest (SMR_VERBOSE); [kTlBase ..) the timeline rows
-  AlnWork* aln_work;                           // [nreads * slots]
-  uint32_t slots;
+  AlnWork* aln_work;                           // [nreads * slots], or with packed arenas [aln_base[nreads]]
+  // One member or the other: a larger LisGlobals changes the code of the strided kernel (it copies its parameters to the stack)
+  // and slowed it by 2 %.
+  union {
+    uint32_t slots;                            // lis_kernel<.., false>: read r stores at r * slots, slots of them
+    const uint32_t* aln_base;                  // lis_kernel<.., true>: [nreads + 1] packed arenas, read r at [aln_base[r], aln_base[r + 1])
+  };
   uint32_t* work_next;                         // [1] persistent-loop cursor (SMR_SCHED_A: over the heaviest reads)
   uint32_t* work_next_b;                       // [1] second cursor (SMR_SCHED_A: over the rest of the schedule)
   const DevIndex* parts; uint32_t nparts;      // every loaded (index,part) in --ref order
@@ -377,7 +382,7 @@ __device__ __noinline__ void submit_and_wait(PassEnv& E, const uint32_t nsel) {
 
 }
 
-template <bool kInstr>
+template <bool kInstr, bool kPacked>
 __device__ void run_candidates(PassEnv& E, ReadCtx& rc, bool& search, const uint32_t max_SW_score, const uint32_t ncand, const bool by_level,
                                uint32_t level, const bool grouped);
 
@@ -385,7 +390,7 @@ __device__ void run_candidates(PassEnv& E, ReadCtx& rc, bool& search, const uint
 // (not inlined: the compiler otherwise clones this function -- and run_candidates inside it -- for both strands and both sides of the
 //  pass loop, four copies = 150 KB of kernel text that the planner warps walk through: a fifth of the kernel's stall samples were
 //  instruction fetches)
-template <bool kInstr>
+template <bool kInstr, bool kPacked>
 __device__ __noinline__ void compute_lis_dev(PassEnv& E, ReadCtx& rc, bool& search, const uint32_t max_SW_score) {
   const DevIndex& ix = *E.ix; const DevBatch& B = *E.b; const DevParams& o = *E.prm;
   const unsigned lane = lane_id();
@@ -569,7 +574,7 @@ __device__ __noinline__ void compute_lis_dev(PassEnv& E, ReadCtx& rc, bool& sear
   { const long long t2 = lis_clock<kInstr>(); E.cyc[2] += (unsigned long long)(t2 - tph); tph = t2; }
   if (kInstr && E.g->dbg) tl_add(E.g->dbg + kTlBase + 3 * kTlBuckets, E.tl0, tlv, tl_now());
   if (SMR_EXP_PLANNER_DELAY) exp_delay(t_call0, SMR_EXP_PLANNER_DELAY);
-  run_candidates<kInstr>(E, rc, search, max_SW_score, ncand, by_level, level, grouped);
+  run_candidates<kInstr, kPacked>(E, rc, search, max_SW_score, ncand, by_level, level, grouped);
   __syncwarp();
   if (grouped) {   // the cursors must not survive the call: histogram words are epoch-tagged votes otherwise
     const unsigned long long* list = E.ar.cand;
@@ -727,7 +732,7 @@ __device__ __noinline__ bool plan_candidate_warp(PassEnv& E, ReadCtx& rc, const 
 
 // candidates in order (alignment.cpp:150-508), in batches: plan -> score (by the scorer warps) -> replay.
 // Returns through rc.flags on scratch overflow.
-template <bool kInstr>
+template <bool kInstr, bool kPacked>
 __device__ void run_candidates(PassEnv& E, ReadCtx& rc, bool& search, const uint32_t max_SW_score, const uint32_t ncand, const bool by_level,
                                uint32_t level, const bool grouped) {
   const DevIndex& ix = *E.ix; const DevBatch& B = *E.b; const DevParams& o = *E.prm;
@@ -736,7 +741,7 @@ __device__ void run_candidates(PassEnv& E, ReadCtx& rc, bool& search, const uint
   bool is_aligned = false, first_cand = true, stop_all = false, searching = true;
   uint32_t prev_occur = 0;
   const uint32_t N = (uint32_t)o.num_alignments;
-  AlnWork* slots = E.g->aln_work + (size_t)rc.r * E.g->slots;
+  AlnWork* slots = E.g->aln_work + (kPacked ? (size_t)E.g->aln_base[rc.r] : (size_t)rc.r * E.g->slots);
   uint32_t cap = SMR_BATCH_CAP0;   // candidates per batch; doubles per batch (a perfect-score stop wastes at most what was useful)
   uint32_t* cfirst = E.ar.cfirst; uint32_t* ccnt = cfirst + kBatchCandCap; uint32_t* cumask = ccnt + kBatchCandCap;
 
@@ -990,7 +995,8 @@ __device__ void run_candidates(PassEnv& E, ReadCtx& rc, bool& search, const uint
                 }
                 if (N == 0 || !o.is_best || (o.is_best && rc.n_align < N)) {                    // :420-424
                   // (N == 0, "all alignments": the count runs on past the caller's stride so that the host can name the stride needed)
-                  if (rc.n_align < E.g->slots) { if (lane == 0) slots[rc.n_align] = a; } else rc.ovf_slots = true;
+                  const uint32_t room = kPacked ? E.g->aln_base[rc.r + 1] - E.g->aln_base[rc.r] : E.g->slots;
+                  if (rc.n_align < room) { if (lane == 0) slots[rc.n_align] = a; } else rc.ovf_slots = true;
                   rc.n_align++; rc.is_new_hit = true;
                 } else if (o.is_best && rc.n_align == N && slots[rc.min_index].score1 < score1) {  // :425-459
                   if (N > 1 && rc.max_index == 0 && rc.min_index == 0) {
@@ -1035,7 +1041,7 @@ __device__ void run_candidates(PassEnv& E, ReadCtx& rc, bool& search, const uint
 }
 
 // traverse() pass loop for one strand (paralleltraversal.cpp:92-297)
-template <bool kInstr>
+template <bool kInstr, bool kPacked>
 __device__ void traverse_dev(PassEnv& E, ReadCtx& rc, const bool is_last_strand) {
   const DevIndex& ix = *E.ix; const DevBatch& B = *E.b; const DevParams& o = *E.prm;
   const unsigned lane = lane_id();
@@ -1066,7 +1072,7 @@ __device__ void traverse_dev(PassEnv& E, ReadCtx& rc, const bool is_last_strand)
       newly += __popc(__ballot_sync(kFull, cnt));
     }
     rc.hit_seeds += newly;
-    if (rc.hit_seeds >= (uint32_t)o.num_seeds) compute_lis_dev<kInstr>(E, rc, search, max_SW_score);  // :256-258
+    if (rc.hit_seeds >= (uint32_t)o.num_seeds) compute_lis_dev<kInstr, kPacked>(E, rc, search, max_SW_score);  // :256-258
     if (rc.flags) return;
     if (search) {                                                                              // :262-277
       if (pass_n == 2) search = false;
@@ -1237,8 +1243,8 @@ __device__ void scorer_loop(const DevBatch& b, const DevParams& prm, const LisGl
 // through every loaded (index, part) in --ref order -- the reference's index-major loop
 // (processor.cpp:219-277) run read-major, with the KVDB carry-over of read.cpp:429-539 kept in
 // DevBatch::state between parts (equivalent because reads are independent, SURVEY 8(b)).  Scorer warps
-// run scorer_loop until the last planner has published the shutdown entries.
-template <bool kInstr>
+// run scorer_loop until the last planner has published the shutdown entries.  kPacked: the run's arenas are packed (g.aln_base).
+template <bool kInstr, bool kPacked>
 __global__ void __launch_bounds__(kLisWarpsPerCta * 32, kLisMinCtas)
 lis_kernel(DevBatch b, DevParams prm, LisGlobals g) {
   extern __shared__ __align__(16) uint8_t lis_smem[];     // kLisSmemBytes: scorer warps first, then planner warps
@@ -1322,7 +1328,7 @@ lis_kernel(DevBatch b, DevParams prm, LisGlobals g) {
       const int num_strands = single ? 1 : 2;                                                 // processor.cpp:130-146
       for (int count = 0; count < num_strands && !rc.is_done && !rc.flags; ++count) {
         if ((single && prm.is_reverse) || count == 1) rc.reversed = true;
-        traverse_dev<kInstr>(E, rc, single || count == 1);
+        traverse_dev<kInstr, kPacked>(E, rc, single || count == 1);
       }
       if (rc.flags) break;
       if (rc.is_new_hit && rc.n_align > 0 && lane == 0) {                                     // kvdb.put (processor.cpp:150-155)

@@ -38,7 +38,7 @@ __device__ bool otu_read_counts(const RptArgs& a, const OtuArgs& o, uint32_t r) 
   if (o.feed && a.rec[r | 1u].seq_len == 0) return false;
   const uint32_t n = a.res[r].n_align;
   for (uint32_t k = 0; k < n; ++k)
-    if (denovo_class(a.aln[(size_t)r * a.slots + k], a.st[(size_t)r * a.slots + k], o.min_id, o.min_cov) == kDnYidYcov) return true;
+    if (denovo_class(a.aln[rpt_slot(a, r, k)], a.st[rpt_slot(a, r, k)], o.min_id, o.min_cov) == kDnYidYcov) return true;
   return false;
 }
 
@@ -55,9 +55,9 @@ __device__ __forceinline__ bool otu_passes(const smr_aln& al, const smr_aln_stat
 
 // per (read, slot): flag = 1 for an entry of the map; nsz = length of its QNAME (0 otherwise)
 __global__ void otu_flag_kernel(RptArgs a, OtuArgs o, uint32_t* __restrict__ flag, uint64_t* __restrict__ nsz) {
-  const uint64_t n = (uint64_t)a.nreads * a.slots;
+  const uint64_t n = a.nslots;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t r = (uint32_t)(i / a.slots), k = (uint32_t)(i % a.slots);
+    const uint32_t r = rpt_read_of(a, i), k = (uint32_t)(i - rpt_slot(a, r, 0));
     bool pass = false;
     if (k < a.res[r].n_align) {
       const smr_aln& al = a.aln[i];
@@ -77,11 +77,11 @@ __global__ void otu_flag_kernel(RptArgs a, OtuArgs o, uint32_t* __restrict__ fla
 __global__ void __launch_bounds__(256) otu_append_kernel(RptArgs a, OtuArgs o, const uint32_t* __restrict__ flag, const uint32_t* __restrict__ pos,
                                                          const uint64_t* __restrict__ noff, uint64_t base, uint64_t pool_base, uint64_t* __restrict__ key,
                                                          OtuEnt* __restrict__ ent, char* __restrict__ pool) {
-  const uint64_t n = (uint64_t)a.nreads * a.slots;
+  const uint64_t n = a.nslots;
   const unsigned lane = lane_id();
   for (uint64_t i = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; i < n; i += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
     if (!flag[i]) continue;
-    const uint32_t r = (uint32_t)(i / a.slots);
+    const uint32_t r = rpt_read_of(a, i);
     const RptRec& rc = a.rec[r];
     const uint64_t dst = pool_base + noff[i];
     for (uint32_t k = lane; k < rc.name_len; k += 32) pool[dst + k] = (char)a.text[rc.hdr + rc.name_beg + k];
@@ -144,7 +144,7 @@ __global__ void __launch_bounds__(256) denovo_stats_kernel(RptArgs a, double min
   __shared__ unsigned long long s_tot[4];
   if (threadIdx.x < 4) s_tot[threadIdx.x] = 0;
   __syncthreads();
-  const uint64_t n = (uint64_t)a.nreads * a.slots;
+  const uint64_t n = a.nslots;
   const unsigned lane = lane_id();
   uint32_t t[4] = {0, 0, 0, 0};
   // warp-uniform loop: every lane takes part in the match of every round
@@ -152,7 +152,7 @@ __global__ void __launch_bounds__(256) denovo_stats_kernel(RptArgs a, double min
     const uint64_t i = base + lane;
     uint64_t key = ~0ull;
     if (i < n) {
-      const uint32_t r = (uint32_t)(i / a.slots), k = (uint32_t)(i % a.slots);
+      const uint32_t r = rpt_read_of(a, i), k = (uint32_t)(i - rpt_slot(a, r, 0));
       if (k < a.res[r].n_align) {
         const smr_aln& al = a.aln[i];
         if (rpt_group_of(a, al) == a.ngroups) atomicOr(a.err, kRptErrGroup);

@@ -54,6 +54,9 @@ struct RptArgs {
   const uint8_t* text; uint64_t nbytes;
   const uint64_t* nl; const uint32_t* spos; uint32_t nlines, fastq;
   const RptRec* rec; uint32_t nreads, slots;
+  // the alignment slots: strided (aln_off null), read r's alignment k at r * slots + k, nslots = nreads * slots; packed, at
+  // aln_off[r] + k, nslots = the sum of n_align, slot_read[i] = the read of slot i
+  uint64_t nslots; const uint32_t* aln_off; const uint32_t* slot_read;
   const smr_read_result* res; const smr_aln* aln; const uint32_t* cigar; uint64_t cigar_words; const smr_aln_stats* st;
   const RptGroup* grp; uint32_t ngroups;
   uint32_t cols[4], ncols;
@@ -64,6 +67,20 @@ struct RptArgs {
   uint32_t fx_mask;   // the read files asked for (kRptAligned | kRptOther | kRptDenovo)
   uint32_t* err;
 };
+
+__device__ __forceinline__ uint64_t rpt_slot(const RptArgs& a, uint32_t r, uint32_t k) { return a.aln_off ? (uint64_t)a.aln_off[r] + k : (uint64_t)r * a.slots + k; }
+__device__ __forceinline__ uint32_t rpt_read_of(const RptArgs& a, uint64_t i) { return a.aln_off ? a.slot_read[i] : (uint32_t)(i / a.slots); }
+
+// packed results: slot_read[aln_off[r] + k] = r for every stored alignment k of read r
+__global__ void rpt_slot_read_kernel(const smr_read_result* __restrict__ res, uint32_t nreads, const uint32_t* __restrict__ aln_off,
+                                     uint32_t* __restrict__ slot_read) {
+  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < nreads; r += gridDim.x * blockDim.x)
+    for (uint32_t k = 0, n = res[r].n_align; k < n; ++k) slot_read[aln_off[r] + k] = r;
+}
+// n_align of every read, and a 0 at [nreads]: scanned into aln_off
+__global__ void rpt_counts_kernel(const smr_read_result* __restrict__ res, uint32_t nreads, uint32_t* __restrict__ cnt) {
+  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r <= nreads; r += gridDim.x * blockDim.x) cnt[r] = r < nreads ? res[r].n_align : 0;
+}
 
 __device__ __forceinline__ uint64_t rpt_line_beg(const uint64_t* nl, uint32_t i) { return i ? nl[i - 1] + 1 : 0; }
 __device__ __forceinline__ bool rpt_space(uint8_t c) { return c == ' ' || (c >= '\t' && c <= '\r'); }
@@ -155,7 +172,7 @@ __device__ bool rpt_is_denovo(const RptArgs& a, uint32_t r) {   // n_denovo > 0 
   const uint32_t n = a.res[r].n_align;
   if (n == 0) return false;
   for (uint32_t k = 0; k < n; ++k)
-    if (denovo_class(a.aln[(size_t)r * a.slots + k], a.st[(size_t)r * a.slots + k], a.min_id, a.min_cov) != kDnDenovo) return false;
+    if (denovo_class(a.aln[rpt_slot(a, r, k)], a.st[rpt_slot(a, r, k)], a.min_id, a.min_cov) != kDnDenovo) return false;
   return true;
 }
 
@@ -226,9 +243,9 @@ __global__ void rpt_route_kernel(RptArgs a, uint32_t* __restrict__ flags) {
 
 // live alignment slots: key = group (ngroups = not written), value = slot
 __global__ void rpt_row_keys_kernel(RptArgs a, const uint32_t* __restrict__ flags, uint32_t* __restrict__ keys, uint32_t* __restrict__ vals) {
-  const uint64_t n = (uint64_t)a.nreads * a.slots;
+  const uint64_t n = a.nslots;
   for (uint64_t i = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t r = (uint32_t)(i / a.slots), k = (uint32_t)(i % a.slots);
+    const uint32_t r = rpt_read_of(a, i), k = (uint32_t)(i - rpt_slot(a, r, 0));
     uint32_t key = a.ngroups;
     if (k < a.res[r].n_align && !(flags[r] & kRptSkip)) {
       const smr_aln& al = a.aln[i];
@@ -254,10 +271,10 @@ __global__ void rpt_group_first_kernel(const uint32_t* __restrict__ keys, uint64
 // read object lives for one (index, part) pass: the quality is printed reversed iff an odd number of this read's minus-strand
 // alignments of the same (index, part), up to this one, came before in alignv order.
 __device__ bool rpt_qual_reversed(const RptArgs& a, uint32_t r, uint32_t k) {
-  const smr_aln& al = a.aln[(size_t)r * a.slots + k];
+  const smr_aln& al = a.aln[rpt_slot(a, r, k)];
   uint32_t flips = 0;
   for (uint32_t j = 0; j <= k; ++j) {
-    const smr_aln& b = a.aln[(size_t)r * a.slots + j];
+    const smr_aln& b = a.aln[rpt_slot(a, r, j)];
     flips += b.index_num == al.index_num && b.part == al.part && !b.strand;
   }
   return flips & 1u;
@@ -281,7 +298,7 @@ __device__ void rpt_sam_suffix(RptSink& o, const RptArgs& a, const smr_aln& al, 
 __global__ void rpt_sam_size_kernel(RptArgs a, const uint32_t* __restrict__ rows, const uint64_t* __restrict__ first, uint64_t* __restrict__ size) {
   const uint64_t n = first[a.ngroups];
   for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
-    const uint32_t i = rows[j], r = i / a.slots;
+    const uint32_t i = rows[j], r = rpt_read_of(a, i);
     const smr_aln& al = a.aln[i];
     const RptRec& rc = a.rec[r];
     RptSink o{nullptr, 0};
@@ -314,7 +331,7 @@ __global__ void __launch_bounds__(256) rpt_sam_write_kernel(RptArgs a, const uin
   const uint64_t n = first[a.ngroups];
   const unsigned lane = lane_id();
   for (uint64_t j = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n; j += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
-    const uint32_t i = rows[j], r = i / a.slots;
+    const uint32_t i = rows[j], r = rpt_read_of(a, i);
     const smr_aln al = a.aln[i];
     const RptRec rc = a.rec[r];
     char* dst = out + off[j];
@@ -340,7 +357,7 @@ __global__ void __launch_bounds__(256) rpt_sam_write_kernel(RptArgs a, const uin
     uint32_t qlen = 1;
     if (a.fastq) {
       qlen = rc.qual_len;
-      const bool rev = rpt_qual_reversed(a, r, i % a.slots);
+      const bool rev = rpt_qual_reversed(a, r, (uint32_t)(i - rpt_slot(a, r, 0)));
       for (uint32_t k = lane; k < qlen; k += 32) q[rev ? qlen - 1 - k : k] = (char)a.text[rc.qual + k];
     } else if (lane == 0) {
       q[0] = '*';
@@ -388,7 +405,7 @@ __global__ void rpt_blast_kernel(RptArgs a, const uint32_t* __restrict__ rows, c
     const uint32_t i = rows[j];
     const smr_aln& al = a.aln[i];
     RptSink o{out ? out + off[j] : nullptr, 0};
-    rpt_blast_row(o, a, a.rec[i / a.slots], al, a.st[i], rpt_group_of(a, al));
+    rpt_blast_row(o, a, a.rec[rpt_read_of(a, i)], al, a.st[i], rpt_group_of(a, al));
     if (size) size[j] = o.n;
   }
 }
@@ -436,7 +453,7 @@ __global__ void rpt_pw_size_kernel(RptArgs a, const uint32_t* __restrict__ rows,
   for (uint64_t j = (uint64_t)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (uint64_t)gridDim.x * blockDim.x) {
     const uint32_t i = rows[j];
     const smr_aln& al = a.aln[i];
-    const RptRec& rc = a.rec[i / a.slots];
+    const RptRec& rc = a.rec[rpt_read_of(a, i)];
     const RptGroup& G = a.grp[rpt_group_of(a, al)];
     RptSink o{nullptr, 0};
     rpt_pw_header(o, a, rc, al, G);
@@ -482,7 +499,7 @@ __global__ void __launch_bounds__(256) rpt_pw_write_kernel(RptArgs a, const uint
   for (uint64_t j = ((uint64_t)blockIdx.x * blockDim.x + threadIdx.x) >> 5; j < n; j += ((uint64_t)gridDim.x * blockDim.x) >> 5) {
     const uint32_t i = rows[j];
     const smr_aln& al = a.aln[i];
-    const RptRec& rc = a.rec[i / a.slots];
+    const RptRec& rc = a.rec[rpt_read_of(a, i)];
     const RptGroup& G = a.grp[rpt_group_of(a, al)];
     char* dst = out + off[j];
     uint64_t at = 0;
