@@ -31,7 +31,8 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_format_reports", "smr_last_report_timings", "smr_otu_begin", "smr_otu_add", "smr_otu_finish", "smr_last_otu_timings",
            "smr_format_reports_gz", "smr_gzip", "smr_stream_begin", "smr_stream_push", "smr_stream_next", "smr_stream_counts",
            "smr_stream_push_mate", "smr_format_blast_pairwise", "smr_format_blast_pairwise_gz",
-           "smr_denovo_stats", "smr_set_aln_layout", "smr_align_batch_packed", "smr_download_results_packed", "smr_pack_kvdb_blobs_packed"]
+           "smr_denovo_stats", "smr_set_aln_layout", "smr_align_batch_packed", "smr_download_results_packed", "smr_pack_kvdb_blobs_packed",
+           "smr_set_index_budget", "smr_index_residency"]
 
 # smr_set_aln_layout: strided, nreads * slots alignments; packed, read r's n_align alignments from the sum of the counts before it
 ALN_LAYOUTS = {"strided": 0, "packed": 1}
@@ -157,6 +158,8 @@ def load_library():
         L.smr_stream_next.argtypes = [C.c_void_p, C.POINTER(C.c_uint32), C.POINTER(C.c_int)]
         L.smr_stream_counts.argtypes = [C.c_void_p, C.POINTER(C.c_uint64)]
         L.smr_stream_push_mate.argtypes = [C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint64, C.c_int]
+        L.smr_set_index_budget.argtypes = [C.c_void_p, C.c_uint64]
+        L.smr_index_residency.argtypes = [C.c_void_p, C.c_void_p]
         for name in SYMBOLS:
             getattr(L, name)  # AttributeError if the build is stale
         _lib = L
@@ -386,6 +389,19 @@ class Aligner:
         out = np.zeros(6, np.uint64)
         self._check(self.L.smr_index_info(self.h, _ptr(out)), "smr_index_info")
         return dict(zip(("parts", "hbm_bytes", "nodes", "entries", "ids", "positions"), map(int, out)))
+
+    def set_index_budget(self, nbytes: int):
+        """smr_set_index_budget: at most `nbytes` of the parts' search arrays on the device (0: no limit).  Parts beyond it are
+        held in pinned host memory and each run uploads them group by group; results are those of a run without a budget."""
+        self._check(self.L.smr_set_index_budget(self.h, int(nbytes)), "smr_set_index_budget")
+
+    def index_residency(self) -> dict:
+        """smr_index_residency: the groups of the next run, the bytes of the largest, the search-array bytes on the device and in
+        pinned host memory, the group uploads and their bytes since the context was made, and the last run's upload time (us)."""
+        out = np.zeros(7, np.uint64)
+        self._check(self.L.smr_index_residency(self.h, _ptr(out)), "smr_index_residency")
+        return dict(zip(("groups", "largest_group_bytes", "device_search_bytes", "host_bytes", "uploads", "upload_bytes", "last_upload_us"),
+                        map(int, out)))
 
     def _outputs(self, n, reuse=False, cigar_words=0):
         """result buffers of n reads; the CIGAR pool holds 48 words per alignment slot, or cigar_words if that is more"""

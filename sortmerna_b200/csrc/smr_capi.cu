@@ -51,9 +51,17 @@ struct Buf {
 using DevBuf = Buf<false>;
 using PinBuf = Buf<true>;   // host staging (page-locked once; pageable vectors cost a page-fault pass + a bounce copy per batch)
 
+// The search arrays of a part -- flookup, ftext, fid, pos_off, pos, what the seed and candidate kernels read -- lie one after the
+// other in one buffer, each at a multiple of 256 bytes: the part's own device buffer, its pinned host copy and its place in the
+// index arena of a budgeted run (smr_set_index_budget) have the same layout, so that moving a part is one copy.
+constexpr int kSearchArrays = 5;
+
 struct Part {
   DevIndex d{};
-  std::vector<DevBuf> owned;   // the device arrays behind d and rnames (part_array)
+  std::vector<DevBuf> owned;   // the device arrays behind refseq, ref_off and rnames (part_array)
+  size_t search_len[kSearchArrays] = {};   // bytes of each search array, 64 bytes of zero slack included
+  DevBuf search;               // the part's own device copy of its search arrays (alloc_search); empty while the host holds them
+  PinBuf host;                 // the pinned host copy of its search arrays, while an index budget runs the batch over several groups
   size_t bytes = 0, n_nodes = 0, n_entries = 0, n_ids = 0, n_pos = 0, n_refseq = 0;
   const char* rnames = nullptr; const uint64_t* rname_off = nullptr; uint32_t n_rnames = 0; bool has_rnames = false;   // smr_set_report_refs
   std::vector<std::string> h_rnames;   // host copy of the same ids: the OTU map ranks them (smr_otu_begin)
@@ -124,6 +132,13 @@ struct smr_ctx {
   smr_params prm{};
   bool have_params = false;
   std::vector<Part> parts;
+  // the index budget (smr_set_index_budget): what the parts' search arrays may take on the device; 0 = no limit
+  struct {
+    uint64_t budget = 0;
+    DevBuf arena;                              // the resident group of a run over several groups (at most `budget` bytes)
+    uint64_t uploads = 0, upload_bytes = 0;    // group uploads into the arena since smr_init, and their bytes
+    double t_upload = 0;                       // ms of group uploads in the resident batch's last run and the retries of its download
+  } ib;
   uint32_t n_index_files = 0;
   int sm_count = 132;
   uint32_t chunk_reads = 1u << 20;
@@ -151,7 +166,8 @@ struct smr_ctx {
     bool mates = false;       // the batch came from a mate stream: records 2k and 2k+1 are mates
   } res;
   // scratch of a run that no later call reads, sized by the scale of the run (setup_arenas)
-  struct { DevBuf parts, seed_ctr, lis, lis_epochs, lis_queue, lis_done, lis_rows, lis_dbg, fin, lane_hits, tb, tb_jobs, fin_list; } run;
+  // (kept: a run over several groups of parts, the kOvfSlots bits held back between groups, group_flags_kernel)
+  struct { DevBuf parts, seed_ctr, lis, lis_epochs, lis_queue, lis_done, lis_rows, lis_dbg, fin, lane_hits, tb, tb_jobs, fin_list, kept; } run;
   smr_aln_stats* host_stats = nullptr;   // optional output of the report arithmetic
   // page-locked staging of a download (download_impl) and of the host read layout (read_layout, upload_fastx_impl)
   struct { PinBuf state, flags, hitdb, outaln, stats, cigar, off32, pkoff; std::vector<uint64_t> coff; } h;
@@ -272,6 +288,116 @@ T* part_array(smr_ctx* ctx, Part& pt, size_t n, const void* src) {
   return out;
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// search arrays and the index budget
+// ---------------------------------------------------------------------------------------------------------------------
+// where search array k starts in the part's search buffer; search_at(pt, kSearchArrays) is the buffer's size
+size_t search_at(const Part& pt, int k) {
+  size_t at = 0;
+  for (int j = 0; j < k; ++j) at += (pt.search_len[j] + 255) & ~(size_t)255;
+  return at;
+}
+size_t search_bytes(const Part& pt) { return search_at(pt, kSearchArrays); }
+
+// points d's search arrays into a buffer of the part's layout (null: none)
+void set_search_ptrs(DevIndex& d, const Part& pt, const uint8_t* base) {
+  auto at = [&](int k) { return base ? (const void*)(base + search_at(pt, k)) : nullptr; };
+  d.flookup = (const uint4*)at(0); d.ftext = (const uint32_t*)at(1); d.fid = (const uint32_t*)at(2);
+  d.pos_off = (const uint32_t*)at(3); d.pos = (const uint2*)at(4);
+}
+
+std::string part_name(const Part& pt) { return "index " + std::to_string(pt.d.index_num) + " part " + std::to_string(pt.d.part); }
+
+// fails if the part's search arrays alone pass the index budget
+void check_budget(const smr_ctx* ctx, const Part& pt, uint64_t budget) {
+  if (budget && search_bytes(pt) > budget)
+    fail(SMR_ERR_CAPACITY, part_name(pt) + ": its search arrays take " + std::to_string(search_bytes(pt)) + " bytes, more than the index budget of " +
+                               std::to_string(budget) + " bytes");
+}
+
+// The part's own device buffer for search arrays of len[k] bytes each (64 bytes of zero slack are added), zeroed; points pt.d at it.
+// pt.bytes counts len[k] + 64 for each.  A part larger than the index budget fails first.  Returns the buffer.
+uint8_t* alloc_search(smr_ctx* ctx, Part& pt, const size_t (&len)[kSearchArrays]) {
+  for (int k = 0; k < kSearchArrays; ++k) { pt.search_len[k] = len[k] + 64; pt.bytes += len[k] + 64; }
+  check_budget(ctx, pt, ctx->ib.budget);
+  CK(pt.search.alloc(search_bytes(pt)));
+  CK(cudaMemsetAsync(pt.search.p, 0, search_bytes(pt), ctx->stream));
+  set_search_ptrs(pt.d, pt, (const uint8_t*)pt.search.p);
+  return (uint8_t*)pt.search.p;
+}
+
+// the search arrays of the part to its pinned host copy; its device copy is freed
+void search_to_host(smr_ctx* ctx, Part& pt) {
+  if (!pt.search.p) return;
+  CK(pt.host.alloc(search_bytes(pt)));   // a failed pinned allocation is SMR_ERR_CUDA: the part stays on the device
+  CK(cudaMemcpyAsync(pt.host.p, pt.search.p, search_bytes(pt), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  pt.search.reset();
+  set_search_ptrs(pt.d, pt, nullptr);
+}
+
+// the search arrays of the part back to its own device buffer; its host copy is freed
+void search_to_device(smr_ctx* ctx, Part& pt) {
+  if (pt.search.p) return;
+  CK(pt.search.alloc(search_bytes(pt)));
+  CK(cudaMemcpyAsync(pt.search.p, pt.host.p, search_bytes(pt), cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  pt.host.reset();
+  set_search_ptrs(pt.d, pt, (const uint8_t*)pt.search.p);
+}
+
+// consecutive parts [first, first + n) run together; `bytes` of search arrays
+struct IndexGroup { uint32_t first, n; uint64_t bytes; };
+
+// The groups of the next run: consecutive parts in load order, each group within the budget (no budget: one group).
+std::vector<IndexGroup> index_groups(const smr_ctx* ctx) {
+  std::vector<IndexGroup> gs;
+  for (uint32_t i = 0; i < ctx->parts.size(); ++i) {
+    const uint64_t b = search_bytes(ctx->parts[i]);
+    if (gs.empty() || (ctx->ib.budget && gs.back().bytes + b > ctx->ib.budget)) gs.push_back(IndexGroup{i, 0, 0});
+    gs.back().n += 1; gs.back().bytes += b;
+  }
+  return gs;
+}
+
+// where part i of group gr lies in the index arena: after the group's parts before it
+size_t arena_at(const smr_ctx* ctx, const IndexGroup& gr, uint32_t i) {
+  size_t at = 0;
+  for (uint32_t j = gr.first; j < i; ++j) at += search_bytes(ctx->parts[j]);
+  return at;
+}
+
+uint32_t max_group_parts(const smr_ctx* ctx) {
+  uint32_t m = 1;
+  for (const IndexGroup& g : index_groups(ctx)) m = std::max(m, g.n);
+  return m;
+}
+
+// Puts the search arrays where the budget wants them: one group, every part on the device in its own buffer and no arena; several
+// groups, every part on the host (the arena is sized by the run).  Returns the groups.
+std::vector<IndexGroup> apply_budget(smr_ctx* ctx) {
+  for (const Part& pt : ctx->parts) check_budget(ctx, pt, ctx->ib.budget);
+  const std::vector<IndexGroup> gs = index_groups(ctx);
+  if (gs.size() <= 1) {
+    ctx->ib.arena.reset();
+    for (Part& pt : ctx->parts) search_to_device(ctx, pt);
+  } else {
+    for (Part& pt : ctx->parts) search_to_host(ctx, pt);
+  }
+  return gs;
+}
+
+// a loaded part joins the context's part list; under an index budget that now needs several groups, every part's search arrays go
+// to the host, so that loading too stays within the budget plus the part being loaded
+void add_part(smr_ctx* ctx, Part&& pt) {
+  if (ctx->parts.size() >= 0xFFFF) fail(SMR_ERR_UNSUPPORTED, "more than 65535 index parts in one context");   // (DevIndex::gslot, AlnWork::idx_slot)
+  const uint32_t index_num = pt.d.index_num;
+  ctx->parts.push_back(std::move(pt));
+  ctx->n_index_files = std::max(ctx->n_index_files, index_num + 1);
+  ++ctx->parts_gen;
+  if (ctx->ib.budget) apply_budget(ctx);
+}
+
 // device scratch of one call: n items of T (at least one) in a new buffer of `pool`, freed with it
 template <class T>
 T* scratch(std::vector<DevBuf>& pool, size_t n) {
@@ -293,7 +419,8 @@ void cub_run(DevBuf& tmp, F&& call) {
 // index build on the device (smr_build_dev.cuh): orchestration of one part
 // ---------------------------------------------------------------------------------------------------------------------
 
-Part build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const std::vector<size_t>& members, const BuildOptions& opt) {
+Part build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const std::vector<size_t>& members, const BuildOptions& opt,
+                       uint32_t index_num, uint32_t part) {
   BuildGeom g{};
   g.L = opt.lnwin; g.half = g.L / 2; g.pread = g.L + 1; g.interval = opt.interval; g.max_pos = opt.max_pos; g.burst_depth = g.pread - g.half - 3;
   g.nseq = (uint32_t)members.size();
@@ -374,8 +501,12 @@ Part build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const s
   CK(cudaMemcpyAsync(&npos, u3 + (n - 1), 4, cudaMemcpyDeviceToHost, st));
   CK(cudaStreamSynchronize(st));
   Part pt;
-  uint32_t* p_posoff = part_array<uint32_t>(ctx, pt, (size_t)nids + 1, nullptr);
-  uint2* p_pos = part_array<uint2>(ctx, pt, npos, nullptr);
+  pt.d.index_num = index_num; pt.d.part = part;
+  const size_t nk = (size_t)1 << (2 * g.half);
+  const size_t len[kSearchArrays] = {nk * 16, ftext_words(E) * 4, (size_t)E * 4, ((size_t)nids + 1) * 4, (size_t)npos * 8};
+  alloc_search(ctx, pt, len);
+  uint4* p_flookup = (uint4*)pt.d.flookup; uint32_t* p_ftext = (uint32_t*)pt.d.ftext; uint32_t* p_fid = (uint32_t*)pt.d.fid;
+  uint32_t* p_posoff = (uint32_t*)pt.d.pos_off; uint2* p_pos = (uint2*)pt.d.pos;
   bld_poswrite_kernel<<<gw, tb, 0, st>>>(keyB, u1, u2, u3, d_wstart, g, nids, p_posoff, p_pos);
   CK(cudaGetLastError());
   // 4. burst-trie order of the entries: first occurrence order, then one stable sort + one decision pass per level
@@ -392,10 +523,6 @@ Part build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const s
     if (d < g.burst_depth) { bld_level_kernel<<<ge, tb, 0, st>>>(ekB, pB, E, d, e_arr, e_tpar, e_leaf); CK(cudaGetLastError()); }
   }
   // 5. the lists and their lookup rows
-  const size_t nk = (size_t)1 << (2 * g.half);
-  uint32_t* p_ftext = part_array<uint32_t>(ctx, pt, ftext_words(E), nullptr);
-  uint32_t* p_fid = part_array<uint32_t>(ctx, pt, E, nullptr);
-  uint4* p_flookup = part_array<uint4>(ctx, pt, nk, nullptr);
   bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, p_ftext, p_fid, (uint32_t*)p_flookup, 0);
   bld_flist_kernel<<<ge, tb, 0, st>>>(pB, e_list, e_text, e_id, E, p_ftext, p_fid, (uint32_t*)p_flookup, 1);
   CK(cudaGetLastError());
@@ -404,7 +531,6 @@ Part build_part_device(smr_ctx* ctx, const std::vector<RefRecord>& recs, const s
   uint32_t* p_roff = part_array<uint32_t>(ctx, pt, roff.size(), roff.data());
   CK(cudaStreamSynchronize(st));
   pt.d.lnwin = g.L; pt.d.partialwin = g.half; pt.d.nref = g.nseq; pt.d.nids = nids;
-  pt.d.flookup = p_flookup; pt.d.ftext = p_ftext; pt.d.fid = p_fid; pt.d.pos_off = p_posoff; pt.d.pos = p_pos;
   pt.d.refseq = p_ref; pt.d.ref_off = p_roff;
   pt.n_entries = E; pt.n_ids = nids; pt.n_pos = npos; pt.n_refseq = c04.size();
   return pt;
@@ -540,6 +666,12 @@ uint64_t read_layout(smr_ctx* ctx, Batch& b, uint32_t n, Len len) {
   return w;
 }
 
+// the hit regions of a batch for groups of `nparts` parts
+void ensure_hit_regions(Batch& b, uint32_t nparts) {
+  ensure(b.hits, b.hits_stride * nparts * 8);
+  ensure(b.hit_cnt, (size_t)b.cnt_stride * nparts * 4);
+}
+
 // The part of an upload that does not depend on where the reads came from: b's reads and offsets are on the device and b.off32 on the
 // host; sizes the batch's other buffers for its scale and 2-bit packs the reads.
 void finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
@@ -564,12 +696,11 @@ void finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
     const uint32_t c1 = std::min(nreads, c0 + ctx->chunk_reads);
     max_chunk_nt = std::max<uint64_t>(max_chunk_nt, b.off32[c1] - b.off32[c0]);
   }
-  // one hit-region set per loaded (index,part): all parts are seeded before the candidate kernel runs read-major
-  const uint32_t nparts = (uint32_t)std::max<size_t>(1, ctx->parts.size());
+  // one hit-region set per (index,part) of a resident group: the group's parts are seeded before the candidate kernel runs read-major
+  // (run_impl grows them if the groups have changed since)
   b.cnt_stride = std::min(nreads, ctx->chunk_reads);
   b.hits_stride = (size_t)((uint64_t)b.scale * (2 * max_chunk_nt + 32ull * b.cnt_stride) + 64);
-  ensure(b.hits, b.hits_stride * nparts * 8);
-  ensure(b.hit_cnt, (size_t)b.cnt_stride * nparts * 4);
+  ensure_hit_regions(b, max_group_parts(ctx));
   ensure(b.cost, (size_t)b.cnt_stride * 4);
   ensure(b.bins, (size_t)b.cnt_stride * kCostBins * 4 + (size_t)kCostBins * 4);
   // 2-bit packing + N detection
@@ -1149,7 +1280,11 @@ std::mutex& device_kernel_mutex(int device) {
   return m[device & 63];
 }
 
-// all kernels of one pass over a batch; its results and times stay in the batch
+// All kernels of one pass over a batch; its results and times stay in the batch.  With one group of parts (no index budget, or every
+// part within it) each chunk is seeded, searched and finalized in turn.  With several, the run is group-major: each group is uploaded
+// into the index arena once, every chunk is seeded and searched over its parts, and every chunk is finalized after the last group.
+// The read state carries from group to group as it does from part to part.  Retries and packed re-runs come through here too, and
+// upload the groups again.
 void run_impl(smr_ctx* ctx, Batch& bt) {
   if (!ctx->have_params) fail(SMR_ERR_ARG, "smr_set_params not called");
   if (ctx->parts.empty()) fail(SMR_ERR_ARG, "no index loaded");
@@ -1157,6 +1292,7 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   if (ctx->prm.minoccur != 0) fail(SMR_ERR_UNSUPPORTED, "minoccur != 0 is not supported");
   RunTimes& t = bt.run;
   t = RunTimes{};
+  if (&bt == &ctx->res.b) ctx->ib.t_upload = 0;   // a new run of the resident batch; the retries of its download add theirs
   const uint32_t nreads = bt.nreads;
   if (nreads == 0) return;
   const uint32_t slots = slots_of(ctx);
@@ -1165,14 +1301,28 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   bt.run_slots = slots; bt.run_stats = ctx->host_stats || packed(ctx); bt.run_id = ++ctx->runs_made;
   std::lock_guard<std::mutex> dev_lock(device_kernel_mutex(ctx->device));   // held until the stream has drained
   auto& A = ctx->run;
+  const std::vector<IndexGroup> groups = apply_budget(ctx);
+  const uint32_t np = (uint32_t)ctx->parts.size(), ng = (uint32_t)groups.size();
+  uint64_t arena_bytes = 0;
+  for (const IndexGroup& gr : groups) arena_bytes = std::max(arena_bytes, gr.bytes);
+  if (ng > 1 && (ctx->ib.arena.cap < arena_bytes || ctx->ib.arena.cap > ctx->ib.budget)) CK(ctx->ib.arena.alloc(arena_bytes));
+  ensure_hit_regions(bt, max_group_parts(ctx));
   RunGeom g = setup_arenas(ctx, bt.scale, bt.max_len);
   LisGlobals& lg = g.lg; FinalGlobals& fg = g.fg;
-  // device copy of the part table (finalize looks parts up by slot)
+  // device copy of the part tables: [0, np) every part by its ordinal in the context (finalize looks parts up by gslot); with several
+  // groups, group k's parts follow from np + first(k), with their ordinals in the group and their search arrays in the arena
   std::vector<DevIndex> hp;
-  for (size_t i = 0; i < ctx->parts.size(); ++i) {
-    DevIndex d = ctx->parts[i].d; d.slot = (uint32_t)i; d.is_last = (i + 1 == ctx->parts.size()) ? 1u : 0u;
+  for (uint32_t i = 0; i < np; ++i) {
+    DevIndex d = ctx->parts[i].d; d.slot = d.gslot = (uint16_t)i; d.is_last = (i + 1 == np) ? 1u : 0u;
     hp.push_back(d);
   }
+  if (ng > 1)
+    for (const IndexGroup& gr : groups)
+      for (uint32_t i = gr.first; i < gr.first + gr.n; ++i) {
+        DevIndex d = hp[i]; d.slot = (uint16_t)(i - gr.first);
+        set_search_ptrs(d, ctx->parts[i], (const uint8_t*)ctx->ib.arena.p + arena_at(ctx, gr, i));
+        hp.push_back(d);
+      }
   ensure(A.parts, hp.size() * sizeof(DevIndex));
   CK(cudaMemcpyAsync(A.parts.p, hp.data(), hp.size() * sizeof(DevIndex), cudaMemcpyHostToDevice, ctx->stream));
   // cigar pool on the device: generous fixed share per alignment slot
@@ -1185,39 +1335,41 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   CK(cudaMemsetAsync(bt.state.p, 0, (size_t)nreads * sizeof(ReadState), ctx->stream));
   CK(cudaMemsetAsync(bt.flags.p, 0, (size_t)nreads * 4, ctx->stream));
   CK(cudaMemsetAsync(bt.hit_db.p, 0xFF, (size_t)nreads * 2, ctx->stream));
+  if (ng > 1) CK(cudaMemsetAsync(ensure(A.kept, (size_t)nreads * 4), 0, (size_t)nreads * 4, ctx->stream));
   const DevParams dp = to_dev(ctx->prm);
   lg.aln_work = (AlnWork*)bt.aln_work.p; lg.work_next = sc.lis_next; lg.work_next_b = sc.lis_next_b;
-  lg.parts = (const DevIndex*)A.parts.p; lg.nparts = (uint32_t)hp.size();
   if (aln_base) lg.aln_base = aln_base; else lg.slots = slots;
   lg.q_head = sc.q_head; lg.q_tail = sc.q_tail; lg.planners_done = sc.planners_done;
   fg.parts = (const DevIndex*)A.parts.p; fg.aln_work = (const AlnWork*)bt.aln_work.p; fg.out = (OutAln*)bt.out_aln.p;
   if (aln_base) fg.aln_base = aln_base; else fg.slots = slots;
   fg.cigar_pool = (uint32_t*)bt.cigar_pool.p; fg.cigar_cap = bt.cigar_cap_dev; fg.cigar_used = sc.cigar_used;
   fg.work_next = sc.fin_next; fg.job_count = sc.fin_jobs;
-  // events: [0] start, [1] end, and per chunk k from 2 + 5k on: seed, candidate kernel, end of it; finalize, end of it
+  // events: [0] start, [1] end; per group k and chunk c from 2 + 5 (k nchunks + c) on: seed, candidate kernel, end of it, and (group 0
+  // only) finalize, end of it; then two per group around its upload
   const uint32_t nchunks = (nreads + ctx->chunk_reads - 1) / ctx->chunk_reads;
-  cudaEvent_t* e = events(ctx, 2 + 5 * (size_t)nchunks);
-  CK(cudaEventRecord(e[0], ctx->stream));
-  for (uint32_t c0 = 0, k = 0; c0 < nreads; c0 += ctx->chunk_reads, ++k) {
+  cudaEvent_t* e = events(ctx, 2 + 5 * (size_t)nchunks * ng + 2 * (size_t)ng);
+  cudaEvent_t* eu = e + 2 + 5 * (size_t)nchunks * ng;
+  // seed kernels, bins and the candidate kernel of the parts hp[t0, t0 + tn) over the chunk at c0
+  auto candidates = [&](uint32_t t0, uint32_t tn, uint32_t c0, cudaEvent_t* ek) {
     const uint32_t n = std::min(ctx->chunk_reads, nreads - c0);
-    cudaEvent_t* ek = e + 2 + 5 * k;
     DevBatch b = make_batch(bt, c0, n);
     CK(cudaMemsetAsync(sc.work_n, 0, 16, ctx->stream));  // (unused word), the two cursors of the candidate kernel's read schedule, finalize's cursor (zeroed again before it runs)
     CK(cudaMemsetAsync(b.cost, 0, (size_t)n * 4, ctx->stream));
     CK(cudaMemsetAsync(b.bin_count, 0, (size_t)kCostBins * 4, ctx->stream));
     CK(cudaEventRecord(ek[0], ctx->stream));
-    ensure(A.seed_ctr, hp.size() * 4);
-    CK(cudaMemsetAsync(A.seed_ctr.p, 0, hp.size() * 4, ctx->stream));   // one work counter per seed launch
-    for (size_t pi = 0; pi < hp.size(); ++pi) {
+    ensure(A.seed_ctr, (size_t)tn * 4);
+    CK(cudaMemsetAsync(A.seed_ctr.p, 0, (size_t)tn * 4, ctx->stream));   // one work counter per seed launch
+    for (uint32_t pi = 0; pi < tn; ++pi) {
       uint32_t* next_read = (uint32_t*)A.seed_ctr.p + pi;
-      if (ctx->instr) seed_kernel<true><<<g.seed_ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[pi], b, dp, (uint32_t*)A.lane_hits.p, g.lane_hits_cap, next_read);
-      else seed_kernel<false><<<g.seed_ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[pi], b, dp, (uint32_t*)A.lane_hits.p, g.lane_hits_cap, next_read);
+      if (ctx->instr) seed_kernel<true><<<g.seed_ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[t0 + pi], b, dp, (uint32_t*)A.lane_hits.p, g.lane_hits_cap, next_read);
+      else seed_kernel<false><<<g.seed_ctas, kSeedWarpsPerCta * 32, 0, ctx->stream>>>(hp[t0 + pi], b, dp, (uint32_t*)A.lane_hits.p, g.lane_hits_cap, next_read);
       CK(cudaGetLastError());
       t.launches += 1;
     }
     bin_kernel<<<(n + 255) / 256, 256, 0, ctx->stream>>>(b);
     CK(cudaGetLastError());
     CK(cudaEventRecord(ek[1], ctx->stream));
+    lg.parts = (const DevIndex*)A.parts.p + t0; lg.nparts = tn;
     lis_reset_kernel<<<kQueueCap / 256, 256, 0, ctx->stream>>>(lg, g.lis_warps);
     CK(cudaGetLastError());
     (ctx->instr ? (aln_base ? lis_kernel<true, true> : lis_kernel<true, false>) : (aln_base ? lis_kernel<false, true> : lis_kernel<false, false>))
@@ -1225,7 +1377,11 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
     CK(cudaGetLastError());
     CK(cudaEventRecord(ek[2], ctx->stream));
     t.launches += 2;
-    // finalize this chunk
+  };
+  // finalize the chunk at c0
+  auto finalize = [&](uint32_t c0, cudaEvent_t* ek) {
+    const uint32_t n = std::min(ctx->chunk_reads, nreads - c0);
+    DevBatch b = make_batch(bt, c0, n);
     CK(cudaMemsetAsync(sc.fin_next, 0, 4, ctx->stream));
     CK(cudaMemsetAsync(sc.fin_jobs, 0, 4, ctx->stream));
     CK(cudaEventRecord(ek[3], ctx->stream));
@@ -1243,16 +1399,42 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
     CK(cudaGetLastError());
     CK(cudaEventRecord(ek[4], ctx->stream));
     t.launches += 3;
+  };
+  const uint32_t flag_grid = std::min<uint32_t>((nreads + 255) / 256, (uint32_t)ctx->sm_count * 8);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  if (ng == 1) {
+    for (uint32_t c0 = 0, k = 0; c0 < nreads; c0 += ctx->chunk_reads, ++k) {
+      candidates(0, np, c0, e + 2 + 5 * k);
+      finalize(c0, e + 2 + 5 * k);
+    }
+  } else {
+    for (uint32_t gi = 0; gi < ng; ++gi) {
+      const IndexGroup& gr = groups[gi];
+      CK(cudaEventRecord(eu[2 * gi], ctx->stream));
+      for (uint32_t i = gr.first; i < gr.first + gr.n; ++i) {
+        const Part& pt = ctx->parts[i];
+        CK(cudaMemcpyAsync((uint8_t*)ctx->ib.arena.p + arena_at(ctx, gr, i), pt.host.p, search_bytes(pt), cudaMemcpyHostToDevice, ctx->stream));
+      }
+      CK(cudaEventRecord(eu[2 * gi + 1], ctx->stream));
+      ctx->ib.uploads += 1; ctx->ib.upload_bytes += gr.bytes;
+      for (uint32_t c0 = 0, k = 0; c0 < nreads; c0 += ctx->chunk_reads, ++k) candidates(np + gr.first, gr.n, c0, e + 2 + 5 * ((size_t)gi * nchunks + k));
+      group_flags_kernel<<<flag_grid, 256, 0, ctx->stream>>>((uint32_t*)bt.flags.p, (uint32_t*)A.kept.p, nreads, gi + 1 == ng ? 1 : 0);
+      CK(cudaGetLastError());
+      t.launches += 1;
+    }
+    for (uint32_t c0 = 0, k = 0; c0 < nreads; c0 += ctx->chunk_reads, ++k) finalize(c0, e + 2 + 5 * k);
   }
   CK(cudaEventRecord(e[1], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   t.total = elapsed_ms(e[0], e[1]);
-  for (uint32_t k = 0; k < nchunks; ++k) {
+  for (uint32_t k = 0; k < nchunks * ng; ++k) {
     const cudaEvent_t* ek = e + 2 + 5 * k;
     t.seed += elapsed_ms(ek[0], ek[1]);
     t.lis += elapsed_ms(ek[1], ek[2]);
-    t.final += elapsed_ms(ek[3], ek[4]);
+    if (k < nchunks) t.final += elapsed_ms(ek[3], ek[4]);
   }
+  if (ng > 1)
+    for (uint32_t gi = 0; gi < ng; ++gi) ctx->ib.t_upload += elapsed_ms(eu[2 * gi], eu[2 * gi + 1]);
   if (getenv("SMR_VERBOSE")) {
     unsigned long long d[16]; cudaMemcpy(d, A.lis_dbg.p, 128, cudaMemcpyDeviceToHost);
     fprintf(stderr, "[smr] slowest read %llu: %.2f ms; cycles vote %llu order %llu group %llu plan %llu wait %llu replay %llu; sw calls %llu, tasks scored %llu, rounds %llu\n", d[10], d[0] / 1.965e6, d[1], d[2], d[3], d[4], d[5], d[6], d[7], d[8], d[9]);
@@ -2164,19 +2346,18 @@ int smr_load_index_part(smr_ctx* ctx, uint32_t index_num, uint32_t part, const v
   rseq.resize(rseq.size() + 64, 4);
   std::vector<uint32_t> ftext(ftext_words(fx.flist.size()), 0), fid(fx.flist.size());
   for (size_t i = 0; i < fx.flist.size(); ++i) { ftext[i] = fx.flist[i].tail; fid[i] = fx.flist[i].id; }   // an flist item's tail holds the full text
-  pt.d.flookup = (const uint4*)part_array<uint32_t>(ctx, pt, fx.flookup.size(), fx.flookup.data());
-  pt.d.ftext = part_array<uint32_t>(ctx, pt, ftext.size(), ftext.data());
-  pt.d.fid = part_array<uint32_t>(ctx, pt, fid.size(), fid.data());
-  pt.d.pos_off = part_array<uint32_t>(ctx, pt, fx.pos_off.size(), fx.pos_off.data());
-  pt.d.pos = (const uint2*)part_array<SeqPos>(ctx, pt, fx.pos.size(), fx.pos.data());
+  const size_t len[kSearchArrays] = {fx.flookup.size() * 4, ftext.size() * 4, fid.size() * 4, fx.pos_off.size() * 4, fx.pos.size() * sizeof(SeqPos)};
+  const void* src[kSearchArrays] = {fx.flookup.data(), ftext.data(), fid.data(), fx.pos_off.data(), fx.pos.data()};
+  pt.d.index_num = index_num; pt.d.part = part;
+  uint8_t* sb = alloc_search(ctx, pt, len);
+  for (int k = 0; k < kSearchArrays; ++k)
+    if (len[k]) CK(cudaMemcpyAsync(sb + search_at(pt, k), src[k], len[k], cudaMemcpyHostToDevice, ctx->stream));
   pt.d.refseq = part_array<uint8_t>(ctx, pt, rseq.size(), rseq.data());
   pt.d.ref_off = part_array<uint32_t>(ctx, pt, roff.size(), roff.data());
   CK(cudaStreamSynchronize(ctx->stream));
   pt.n_refseq = rseq.size();
   pt.n_nodes = fx.nodes.size(); pt.n_entries = fx.entries.size(); pt.n_ids = pt.d.nids; pt.n_pos = fx.pos.size();
-  ctx->parts.push_back(std::move(pt));
-  ctx->n_index_files = std::max(ctx->n_index_files, index_num + 1);
-  ++ctx->parts_gen;
+  add_part(ctx, std::move(pt));
   return SMR_OK;
 } SMR_CATCH(ctx)
 
@@ -2204,13 +2385,11 @@ int smr_build_index_device(smr_ctx* ctx, uint32_t index_num, const char* fasta_p
     e = next_index_part(recs, first, lnwin + 1, max_mb, members, next, start_part, seq_part_size);
     if (!e.empty()) { ctx->err = e; return SMR_ERR_INDEX; }
     if (members.empty()) break;
-    Part pt = build_part_device(ctx, recs, members, opt);
-    pt.d.index_num = index_num; pt.d.part = part; pt.d.minimal_score = minimal_score;
+    Part pt = build_part_device(ctx, recs, members, opt, index_num, part);
+    pt.d.minimal_score = minimal_score;
     for (int i = 0; i < 3; ++i) pt.d.skip[i] = skiplengths[i];
     rep[3] += pt.n_ids; rep[5] += pt.bytes;
-    ctx->parts.push_back(std::move(pt));
-    ctx->n_index_files = std::max(ctx->n_index_files, index_num + 1);
-    ++ctx->parts_gen;
+    add_part(ctx, std::move(pt));
     ++part; first = next;
   }
   if (part == 0) { ctx->err = "no index was created"; return SMR_ERR_INDEX; }
@@ -2225,6 +2404,11 @@ int smr_debug_index_array(smr_ctx* ctx, uint32_t slot, uint32_t which, void* out
   CK(cudaSetDevice(ctx->device));
   const Part& pt = ctx->parts[slot];
   const void* src = nullptr; uint64_t n = 0;
+  // the search arrays of a part whose device copy an index budget has freed are read from its host copy
+  auto copy = [&](void* dst, const void* dev, int k, uint64_t bytes) {
+    if (pt.search.p) CK(cudaMemcpy(dst, dev, bytes, cudaMemcpyDeviceToHost));
+    else memcpy(dst, (const uint8_t*)pt.host.p + search_at(pt, k), bytes);
+  };
   switch (which) {
     case 0: src = pt.d.flookup; n = ((uint64_t)16) << (2 * pt.d.partialwin); break;
     case 1: n = (uint64_t)pt.n_entries * 8; break;   // {text, id} pairs, interleaved below
@@ -2239,13 +2423,14 @@ int smr_debug_index_array(smr_ctx* ctx, uint32_t slot, uint32_t which, void* out
   if (cap_bytes < n) { ctx->err = "buffer too small"; return SMR_ERR_CAPACITY; }
   if (which == 1) {
     std::vector<uint32_t> text(pt.n_entries), id(pt.n_entries), pairs(2 * pt.n_entries);
-    if (n) CK(cudaMemcpy(text.data(), pt.d.ftext, n / 2, cudaMemcpyDeviceToHost));
-    if (n) CK(cudaMemcpy(id.data(), pt.d.fid, n / 2, cudaMemcpyDeviceToHost));
+    if (n) copy(text.data(), pt.d.ftext, 1, n / 2);
+    if (n) copy(id.data(), pt.d.fid, 2, n / 2);
     for (size_t i = 0; i < pt.n_entries; ++i) { pairs[2 * i] = text[i]; pairs[2 * i + 1] = id[i]; }
     if (n) memcpy(out, pairs.data(), n);
     return SMR_OK;
   }
-  if (n) CK(cudaMemcpy(out, src, n, cudaMemcpyDeviceToHost));
+  if (n && which < 4) copy(out, src, which == 0 ? 0 : which + 1, n);   // flookup, pos_off, pos: search arrays 0, 3, 4
+  else if (n) CK(cudaMemcpy(out, src, n, cudaMemcpyDeviceToHost));
   return SMR_OK;
 } SMR_CATCH(ctx)
 
@@ -2277,7 +2462,31 @@ int smr_index_info(const smr_ctx* ctx, uint64_t out[6]) {
   if (!ctx || !out) return SMR_ERR_ARG;
   memset(out, 0, 6 * sizeof(uint64_t));
   out[0] = ctx->parts.size();
-  for (auto& pt : ctx->parts) { out[1] += pt.bytes; out[2] += pt.n_nodes; out[3] += pt.n_entries; out[4] += pt.n_ids; out[5] += pt.n_pos; }
+  for (auto& pt : ctx->parts) {
+    out[1] += pt.bytes; out[2] += pt.n_nodes; out[3] += pt.n_entries; out[4] += pt.n_ids; out[5] += pt.n_pos;
+    if (!pt.search.p) for (size_t b : pt.search_len) out[1] -= b;   // its search arrays are held on the host
+  }
+  out[1] += ctx->ib.arena.cap;
+  return SMR_OK;
+}
+
+int smr_set_index_budget(smr_ctx* ctx, uint64_t bytes) try {
+  if (!ctx) return SMR_ERR_ARG;
+  for (const Part& pt : ctx->parts) check_budget(ctx, pt, bytes);
+  ctx->ib.budget = bytes;
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_index_residency(const smr_ctx* ctx, uint64_t out[7]) {
+  if (!ctx || !out) return SMR_ERR_ARG;
+  memset(out, 0, 7 * sizeof(uint64_t));
+  const std::vector<IndexGroup> gs = index_groups(ctx);
+  out[0] = gs.size();
+  for (const IndexGroup& g : gs) out[1] = std::max<uint64_t>(out[1], g.bytes);
+  for (const Part& pt : ctx->parts) { out[2] += pt.search.cap; out[3] += pt.host.cap; }
+  out[2] += ctx->ib.arena.cap;
+  out[4] = ctx->ib.uploads; out[5] = ctx->ib.upload_bytes;
+  out[6] = (uint64_t)std::llround(ctx->ib.t_upload * 1000.0);
   return SMR_OK;
 }
 
@@ -2656,7 +2865,13 @@ int smr_debug_seed_windows(smr_ctx* ctx, uint32_t part_slot, const uint8_t* seq_
   CK(cudaMemcpy(d_wr, win_read, (size_t)nwin * 4, cudaMemcpyHostToDevice));
   CK(cudaMemcpy(d_wp, win_pos, (size_t)nwin * 4, cudaMemcpyHostToDevice));
   CK(cudaMemset(d_ids, 0, (size_t)nwin * cap * 4));
-  DevIndex d = ctx->parts[part_slot].d;
+  const Part& pt = ctx->parts[part_slot];
+  DevIndex d = pt.d;
+  if (!pt.search.p) {   // an index budget holds the part's search arrays on the host: a device copy for this call
+    uint8_t* sb = scratch<uint8_t>(tmp, search_bytes(pt));
+    CK(cudaMemcpy(sb, pt.host.p, search_bytes(pt), cudaMemcpyHostToDevice));
+    set_search_ptrs(d, pt, sb);
+  }
   const int mode = cap_arg >= 0x80000000u ? 1 : 0;   // high bit of cap selects the per-lane fallback path (tests exercise both)
   seed_debug_kernel<<<(nwin + kSeedWarpsPerCta * 32 - 1) / (kSeedWarpsPerCta * 32), kSeedWarpsPerCta * 32, 0, ctx->stream>>>(
       d, d_seq, d_off, d_wr, d_wp, nwin, d_ids, cap, d_cnt, d_zero, ctx->have_params ? ctx->prm.is_full_search : 0, mode);

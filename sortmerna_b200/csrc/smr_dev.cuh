@@ -9,14 +9,17 @@ constexpr int kWarp = 32;
 constexpr unsigned kFull = 0xFFFFFFFFu;
 constexpr uint32_t kNoneDev = 0xFFFFFFFFu;
 
-// One loaded (index, part); every pointer is HBM-resident (see smr_index.h for the layout).
+// One loaded (index, part); every pointer is HBM-resident (see smr_index.h for the layout).  The search arrays (flookup .. pos) are
+// those of the part's resident group (an index budget runs a batch over groups of parts, smr_set_index_budget); refseq and ref_off
+// are always resident.
 struct DevIndex {
   uint32_t index_num, part, lnwin, partialwin;
   uint32_t minimal_score;
   uint32_t skip[3];
   uint32_t nref, nids;
   uint32_t is_last;          // last (index,part) in --ref order (paralleltraversal.cpp:294)
-  uint32_t slot;             // ordinal of this part in the context
+  uint16_t slot;             // ordinal of this part in its resident group: its hit regions and the group's part table (LisGlobals::parts)
+  uint16_t gslot;            // ordinal of this part in the context: AlnWork::idx_slot, the full part table (FinalGlobals::parts)
   const uint4* flookup;      // [4^partialwin] {offF, cntF, offR, cntR}: entry indices into ftext and fid
   const uint32_t* ftext;     // entry texts (path + tail, partialwin+1 chars, first char lowest), DFS order per (9-mer, direction);
                              // zero-padded to a multiple of 8 entries (the seed kernel reads whole aligned 32-byte chunks)

@@ -31,7 +31,7 @@ struct AlnStats { uint32_t n_miss, n_gap, n_match, n_match_denovo; };   // layou
 struct FinalGlobals {
   uint8_t* arena_base; size_t arena_stride;
   uint32_t cap_w, cap_cig, row_cap; size_t cap_dir;
-  const DevIndex* parts;             // [nparts] device copy
+  const DevIndex* parts;             // [nparts] device copy of every loaded part, by DevIndex::gslot (refseq / ref_off only are read)
   const AlnWork* aln_work; OutAln* out;
   union {                            // one or the other, as in LisGlobals (a larger FinalGlobals changes the strided kernels' code)
     uint32_t slots;                  // <kPacked = false> kernels: read r's alignments at r * slots

@@ -200,7 +200,7 @@ struct LisGlobals {
   };
   uint32_t* work_next;                         // [1] persistent-loop cursor (SMR_SCHED_A: over the heaviest reads)
   uint32_t* work_next_b;                       // [1] second cursor (SMR_SCHED_A: over the rest of the schedule)
-  const DevIndex* parts; uint32_t nparts;      // every loaded (index,part) in --ref order
+  const DevIndex* parts; uint32_t nparts;      // the resident group's (index,part)s in --ref order (every loaded one without an index budget)
 };
 
 __device__ __forceinline__ LisArena carve_arena(const LisGlobals& g, uint32_t warp) {
@@ -988,7 +988,7 @@ __device__ void run_candidates(PassEnv& E, ReadCtx& rc, bool& search, const uint
                 AlnWork a;
                 a.ref_num = pt.max_ref; a.win_ref_start = pt.win_start; a.win_len = alen; a.q_start = pt.aqs; a.q_len = qlen;
                 a.score1 = (uint16_t)score1; a.part = (uint16_t)ix.part; a.index_num = (uint16_t)ix.index_num;
-                a.strand = rc.reversed ? 0 : 1; a.idx_slot = (uint16_t)ix.slot; a.pad0 = 0;
+                a.strand = rc.reversed ? 0 : 1; a.idx_slot = ix.gslot; a.pad0 = 0;
                 if (!rc.is_hit) {                                                               // :411-416
                   rc.is_hit = true;   // readstats.num_aligned / reads_matched_per_db are summed from hit_db at download time
                   if (lane == 0) B.hit_db[rc.r] = (uint16_t)ix.index_num;

@@ -441,6 +441,18 @@ __global__ void bin_kernel(DevBatch b) {
   b.bins[(size_t)bin * b.cnt_stride + slot] = b.r0 + i;
 }
 
+// A batch run over several resident groups of parts (index budget): kOvfSlots only says that a read stored more alignments than its
+// room, and the read goes on searching, as it does through the parts of one group.  The seed kernel and bin_kernel skip every flagged
+// read, so between groups the bit is moved to `kept` (restore = 0) and put back before finalize (restore = 1).  Scratch-overflow
+// flags stay, and stop the read as they do within a group.
+__global__ void group_flags_kernel(uint32_t* flags, uint32_t* kept, uint32_t n, int restore) {
+  for (uint32_t i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) {
+    if (restore) { flags[i] |= kept[i]; continue; }
+    const uint32_t f = flags[i];
+    if (f & kOvfSlots) { kept[i] = kOvfSlots; flags[i] = f & ~kOvfSlots; }
+  }
+}
+
 // unit-test kernel: explicit windows through the SAME cooperative path as seed_kernel (mode 0), or by one
 // lane scanning its own list sequentially (mode 1) (smr_debug_seed_windows)
 __global__ void __launch_bounds__(kSeedWarpsPerCta * 32)
