@@ -466,6 +466,41 @@ typedef struct {
 int smr_denovo_stats(smr_ctx*, const smr_denovo_opts* opts, const char* text, uint64_t nbytes, const smr_read_result* results,
                      const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4]);
 
+/* -- results placed on the device (sortmerna_b200/csrc/smr_place.cuh, DESIGN.md 5g): the last smr_run_resident of the resident
+ *    batch turned into the strided layout of smr_download_results in device memory, where the report-side _placed calls read it:
+ *    nothing goes down to the host and comes back between the alignment and the report writers.  Strided layout only: in the packed
+ *    layout (smr_set_aln_layout) every call below but smr_set_place_stats is SMR_ERR_UNSUPPORTED. */
+/* Whether every later run computes the smr_aln_stats a placement keeps (default 0).  The _placed calls that read stats (SAM,
+ * tabular BLAST, aligned_denovo, the OTU map, the denovo statistics) need a placement of a run made with it on; a run made with a
+ * host stats buffer (smr_set_stats_buffer) computes them too.  The scratch-overflow retries of a placement compute the stats when
+ * the run being placed did. */
+int smr_set_place_stats(smr_ctx*, int on);
+/* Place the results of the resident batch's last smr_run_resident on the device: smr_read_result[n], smr_aln[n * smr_aln_slots()]
+ * zeroed past n_align, the stats alike, the CIGARs compacted in read order -- the bytes smr_download_results would write, with the
+ * same retries of reads that overflowed their scratch (8x, 64x, 512x; each retry batch is placed through its read map before it
+ * frees itself; their CIGARs follow those of the others) and the same errors: a read that stores more alignments than the stride
+ * gives SMR_ERR_CAPACITY and smr_aln_slots_needed(), a trace back error SMR_ERR_INDEX; an index budget runs the retries as
+ * smr_download_results does.  counters[SMR_CNT_FIXED + n_index_files] are ADDED to as by smr_download_results (nullable).
+ * *n_alns = the alignment rows (n * stride), *cigar_words = the CIGAR words placed (both nullable, 0 on failure).  The context keeps
+ * the placed arrays until the batch is run again or replaced (keyed by the run); a second call for the same run places nothing
+ * again and adds the same counters.  SMR_ERR_ARG if the batch was not run, or was run at another stride. */
+int smr_place_results(smr_ctx*, uint64_t* counters, uint32_t n_counters, uint64_t* n_alns, uint64_t* cigar_words);
+/* The placed arrays copied to the host (a caller that also wants smr_pack_kvdb_blobs): results[n], alns[n * stride], stats
+ * (nullable; SMR_ERR_ARG if the placed run computed none) and cigar_pool[cigar_cap] (SMR_ERR_CAPACITY below *cigar_words). */
+int smr_download_placed(smr_ctx*, smr_read_result* results, smr_aln* alns, smr_aln_stats* stats, uint32_t* cigar_pool, uint64_t cigar_cap);
+/* milliseconds (CUDA events) of the last placement's count, scan and scatter passes over the resident batch (retries excluded) */
+int smr_last_place_timing(const smr_ctx*, double* ms);
+/* The report-side calls on the placed results of the resident batch's last run and its resident text: smr_format_reports[_gz],
+ * smr_format_blast_pairwise[_gz], smr_otu_add and smr_denovo_stats without text, results, alns, cigar_pool or stats; everything else
+ * (opts, out, cap, stream_off, SMR_ERR_CAPACITY, n_added, per_read, totals) as there.  SMR_ERR_ARG without a placement of the
+ * resident batch's last run (none yet, or one of an earlier run or batch), or when the call reads stats the placement lacks. */
+int smr_format_reports_placed(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
+int smr_format_reports_placed_gz(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
+int smr_format_blast_pairwise_placed(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
+int smr_format_blast_pairwise_placed_gz(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
+int smr_otu_add_placed(smr_ctx*, uint64_t* n_added);
+int smr_denovo_stats_placed(smr_ctx*, const smr_denovo_opts* opts, uint32_t* per_read, uint64_t totals[4]);
+
 /* Device-side timings of the last smr_run_resident / smr_align_batch, CUDA events on the
  * library's stream, milliseconds: out[0]=total [1]=seed kernels [2]=candidate/SW kernels
  * [3]=finalize (reverse SW + traceback) [4]=h2d [5]=d2h; out[6]=number of kernel launches [7]=decode of the last text upload

@@ -32,7 +32,9 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_format_reports_gz", "smr_gzip", "smr_stream_begin", "smr_stream_push", "smr_stream_next", "smr_stream_counts",
            "smr_stream_push_mate", "smr_format_blast_pairwise", "smr_format_blast_pairwise_gz",
            "smr_denovo_stats", "smr_set_aln_layout", "smr_align_batch_packed", "smr_download_results_packed", "smr_pack_kvdb_blobs_packed",
-           "smr_set_index_budget", "smr_index_residency"]
+           "smr_set_index_budget", "smr_index_residency", "smr_set_place_stats", "smr_place_results", "smr_download_placed",
+           "smr_last_place_timing", "smr_format_reports_placed", "smr_format_reports_placed_gz", "smr_format_blast_pairwise_placed",
+           "smr_format_blast_pairwise_placed_gz", "smr_otu_add_placed", "smr_denovo_stats_placed"]
 
 # smr_set_aln_layout: strided, nreads * slots alignments; packed, read r's n_align alignments from the sum of the counts before it
 ALN_LAYOUTS = {"strided": 0, "packed": 1}
@@ -617,8 +619,8 @@ class Aligner:
         n = self._n_resident
         if self.layout == "packed":
             return self._packed_call(self.L.smr_download_results_packed, "smr_download_results_packed", [self.h], n, self._stats_packed)
-        stats = getattr(self, "_stats", None)
-        stats = np.zeros_like(stats) if stats is not None else None
+        stats = getattr(self, "_stats", None)   # sized at the stride in effect, which the library writes them at
+        stats = np.zeros(n * int(self.L.smr_aln_slots(self.h)), STATS_DTYPE) if stats is not None else None
         self._check(self.L.smr_set_stats_buffer(self.h, _ptr(stats) if stats is not None else C.c_void_p(0)), "smr_set_stats_buffer")
         words = 0
         while True:
@@ -636,6 +638,74 @@ class Aligner:
         if stats is not None:
             out["stats"] = stats
         return out
+
+    # ---- results placed on the device (smr_place_results; the report calls with out=None read them) ----
+    def set_place_stats(self, on: bool):
+        """smr_set_place_stats: later runs compute the smr_aln_stats a placement keeps (SAM, tabular BLAST, aligned_denovo, the OTU
+        map and the denovo statistics read them); default off."""
+        self._check(self.L.smr_set_place_stats(self.h, C.c_int(1 if on else 0)), "smr_set_place_stats")
+
+    def place(self) -> dict:
+        """smr_place_results: the results of the last run_resident() placed on the device in the strided layout, its scratch-overflow
+        retries included; format_reports / format_blast_pairwise / otu_add / denovo_stats / ReportWriter.write with out=None read
+        them there.  In the all-alignments mode (num_alignments 0) a read that stores more alignments than the stride makes the
+        stride grow to what the library names and the batch run again, as align() does.  Returns {"nreads", "slots", "n_alns",
+        "cigar_words", "counters" (by name, as download()), "matched" (reads_matched_per_db), "place_ms" (device time of the
+        placement passes)}."""
+        self.L.smr_place_results.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+        self.L.smr_last_place_timing.argtypes = [C.c_void_p, C.c_void_p]
+        while True:
+            counters = np.zeros(CNT_FIXED + max(1, self.n_index_files), np.uint64)
+            n_alns, words = C.c_uint64(0), C.c_uint64(0)
+            rc = self.L.smr_place_results(self.h, _ptr(counters), counters.size, C.cast(C.byref(n_alns), C.c_void_p), C.cast(C.byref(words), C.c_void_p))
+            slots = int(self.L.smr_aln_slots(self.h))
+            need = int(self.L.smr_aln_slots_needed(self.h)) if rc == 5 and self.params.num_alignments == 0 else 0
+            if need > slots:   # run again as run_resident() does, with a host stats buffer at the new stride if it had one
+                self.set_aln_slots(need)
+                self.run_resident(with_stats=getattr(self, "_stats", None) is not None)
+                continue
+            break
+        self._check(rc, "smr_place_results")
+        ms = C.c_double(0)
+        self.L.smr_last_place_timing(self.h, C.cast(C.byref(ms), C.c_void_p))
+        self.placed_info = dict(nreads=self._n_resident, slots=slots, n_alns=int(n_alns.value), cigar_words=int(words.value),
+                    counters={k: int(counters[i]) for i, k in enumerate(CNT_NAMES)}, matched=counters[CNT_FIXED:].copy(), place_ms=ms.value)
+        return self.placed_info
+
+    def download_placed(self, with_stats: bool = False) -> dict:
+        """smr_download_placed: the placed arrays on the host, in the form download() returns ("res", "alns", "cigar", "slots", and
+        "stats" with with_stats); the counters are those place() returned."""
+        n, slots = self._n_resident, int(self.L.smr_aln_slots(self.h))
+        words = C.c_uint64(0)
+        self.L.smr_place_results.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+        self._check(self.L.smr_place_results(self.h, None, 0, None, C.cast(C.byref(words), C.c_void_p)), "smr_place_results")
+        res, alns = np.zeros(n, RESULT_DTYPE), np.zeros(n * slots, ALN_DTYPE)
+        stats = np.zeros(n * slots, STATS_DTYPE) if with_stats else None
+        pool = np.zeros(max(1, words.value), np.uint32)
+        self.L.smr_download_placed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
+        self._check(self.L.smr_download_placed(self.h, _ptr(res), _ptr(alns), _ptr(stats) if with_stats else None, _ptr(pool), pool.size),
+                    "smr_download_placed")
+        out = dict(res=res, alns=alns, cigar=pool[:words.value], slots=slots)
+        if with_stats:
+            out["stats"] = stats
+        return out
+
+    def format_placed_into(self, opts: ReportOpts, buf: np.ndarray, gzip: bool = False, pairwise: bool = False):
+        """smr_format_reports_placed[_gz] (pairwise: smr_format_blast_pairwise_placed[_gz]) into `buf` (a uint8 array, grown when the
+        streams do not fit): returns (buf, stream offsets).  The streams stay in buf, for a caller that writes them out as they are."""
+        if opts.sam or opts.blast:
+            self._upload_report_refs()
+        G = len(self.report_groups())
+        so = np.zeros(G + 1 if pairwise else 2 * G + 3 * num_out_of(opts) + 1, np.uint64)
+        name = ("smr_format_blast_pairwise_placed" if pairwise else "smr_format_reports_placed") + ("_gz" if gzip else "")
+        fn = getattr(self.L, name)
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        rc = fn(self.h, C.cast(C.byref(opts), C.c_void_p), _ptr(buf), buf.size, _ptr(so))
+        if rc == 5 and int(so[-1]) > buf.size:   # SMR_ERR_CAPACITY: so names the size; grow and run again
+            buf = np.empty(int(so[-1]) + (int(so[-1]) >> 3), np.uint8)
+            rc = fn(self.h, C.cast(C.byref(opts), C.c_void_p), _ptr(buf), buf.size, _ptr(so))
+        self._check(rc, name)
+        return buf, so
 
     # ---- report writer (smr_format_reports) ----
     def report_groups(self) -> list:
@@ -679,17 +749,24 @@ class Aligner:
         or its keyword arguments.  Returns {"sam": [bytes per group], "blast": [...], "aligned": bytes, "other": bytes, "denovo": bytes,
         "groups": report_groups()}; with out2 or sout, "aligned" / "other" / "denovo" are tuples of the num_out files (2, or 4 with
         both) in the reference's order (_fwd, _rev | _paired, _singleton | _paired_fwd, _paired_rev, _singleton_fwd, _singleton_rev).
-        gzip: smr_format_reports_gz, every non-empty stream as one gzip member (empty ones stay b"")."""
+        gzip: smr_format_reports_gz, every non-empty stream as one gzip member (empty ones stay b"").
+        out=None: the results place() placed on the device and the resident text (smr_format_reports_placed[_gz]); text must be None."""
         o = opts if opts is not None else report_opts(**kw)
         if o.sam or o.blast:
             self._upload_report_refs()
         groups = self.report_groups()
         G = len(groups)
+        num_out = num_out_of(o)
+        if out is None:
+            if text is not None:
+                raise ValueError("format_reports: the placed results go with the resident text (text=None)")
+            buf, so = self.format_placed_into(o, self._report_buffer(), gzip)
+            self._report_buf = buf
+            return self._report_streams(buf, so, G, num_out, groups)
         res, alns = out["res"], out["alns"]
         cig = np.ascontiguousarray(out["cigar"], np.uint32)
         st = out.get("stats")
         txt = np.frombuffer(text, np.uint8) if text is not None else None
-        num_out = num_out_of(o)
         so = np.zeros(2 * G + 3 * num_out + 1, np.uint64)
         fn = self.L.smr_format_reports_gz if gzip else self.L.smr_format_reports
         fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64,
@@ -705,6 +782,14 @@ class Aligner:
             rc = fn(*args, _ptr(buf), buf.size, _ptr(so))
         self._check(rc, "smr_format_reports_gz" if gzip else "smr_format_reports")
         self._report_buf = buf
+        return self._report_streams(buf, so, G, num_out, groups)
+
+    def _report_buffer(self) -> np.ndarray:
+        buf = getattr(self, "_report_buf", None)
+        return buf if buf is not None else np.zeros(1 << 20, np.uint8)
+
+    @staticmethod
+    def _report_streams(buf, so, G, num_out, groups) -> dict:
         b = [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(so.size - 1)]
         fx = [b[2 * G + j * num_out:2 * G + (j + 1) * num_out] for j in range(3)]
         fx = [f[0] for f in fx] if num_out == 1 else [tuple(f) for f in fx]
@@ -713,12 +798,19 @@ class Aligner:
     def format_blast_pairwise(self, out: dict, text: bytes | None = None, opts: ReportOpts | None = None, gzip: bool = False, **kw) -> list:
         """smr_format_blast_pairwise: the pairwise BLAST rows (-blast 0) of one batch, as a list of bytes, one per report_groups() entry.
         out / text as for format_reports; opts = report_opts(blast="0", ...) or its keyword arguments (blast defaults to "0"; only
-        paired_in / paired_out / mates matter besides).  gzip: smr_format_blast_pairwise_gz, every non-empty stream as one gzip member."""
+        paired_in / paired_out / mates matter besides).  gzip: smr_format_blast_pairwise_gz, every non-empty stream as one gzip member.
+        out=None: the placed results and the resident text (smr_format_blast_pairwise_placed[_gz]), as format_reports."""
         if opts is None:
             kw.setdefault("blast", "0")
             opts = report_opts(**kw)
         self._upload_report_refs()
         G = len(self.report_groups())
+        if out is None:
+            if text is not None:
+                raise ValueError("format_blast_pairwise: the placed results go with the resident text (text=None)")
+            buf, so = self.format_placed_into(opts, self._report_buffer(), gzip, pairwise=True)
+            self._report_buf = buf
+            return [bytes(buf[int(so[k]):int(so[k + 1])]) for k in range(G)]
         res, alns = out["res"], out["alns"]
         cig = np.ascontiguousarray(out["cigar"], np.uint32)
         st = out.get("stats")
@@ -750,10 +842,17 @@ class Aligner:
         self._check(self.L.smr_otu_begin(self.h, C.byref(o)), "smr_otu_begin")
 
     def otu_add(self, out: dict, text: bytes | None = None) -> int:
-        """smr_otu_add: one batch (out and text as for format_reports; out needs "stats"); returns the entries it added"""
+        """smr_otu_add: one batch (out and text as for format_reports; out needs "stats"); returns the entries it added.
+        out=None: the placed results and the resident text (smr_otu_add_placed)."""
+        n = C.c_uint64(0)
+        if out is None:
+            if text is not None:
+                raise ValueError("otu_add: the placed results go with the resident text (text=None)")
+            self.L.smr_otu_add_placed.argtypes = [C.c_void_p, C.c_void_p]
+            self._check(self.L.smr_otu_add_placed(self.h, C.cast(C.byref(n), C.c_void_p)), "smr_otu_add_placed")
+            return int(n.value)
         res, alns, st = out["res"], out["alns"], out.get("stats")
         txt = np.frombuffer(text, np.uint8) if text is not None else None
-        n = C.c_uint64(0)
         self.L.smr_otu_add.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
         rc = self.L.smr_otu_add(self.h, _ptr(txt) if txt is not None and txt.size else None, txt.size if txt is not None else 0, _ptr(res), _ptr(alns),
                                 _ptr(st) if st is not None else None, res.shape[0], C.cast(C.byref(n), C.c_void_p))
@@ -774,24 +873,34 @@ class Aligner:
         self._otu_buf = buf
         return dict(text=bytes(buf[:int(counts[0])]), total_otu=int(counts[1]), n_yid_ycov=int(counts[2]))
 
-    def denovo_stats(self, out: dict, text: bytes | None = None, min_id: float = 0.97, min_cov: float = 0.97, paired: bool = False):
+    def denovo_stats(self, out: dict, text: bytes | None = None, min_id: float = 0.97, min_cov: float = 0.97, paired: bool = False,
+                     per_read: bool = True):
         """smr_denovo_stats: the reference's denovo_stats pass over one batch (out and text as for format_reports; out needs "stats").
         Returns (per_read, totals): per_read an (nreads, 4) uint32 array of {c_yid_ycov, n_yid_ncov, n_nid_ycov, n_denovo} per read
         (pack_kvdb_blobs' denovo), totals {"n_yid_ycov", "n_yid_ncov", "n_nid_ycov", "num_denovo"} of this batch.  paired: records
-        2k and 2k+1 are mates (implied for the resident batch of stream_mates)."""
+        2k and 2k+1 are mates (implied for the resident batch of stream_mates).  out=None: the placed results and the resident text
+        (smr_denovo_stats_placed).  per_read=False: the totals alone (per_read is returned as None)."""
+        tot = np.zeros(4, np.uint64)
+        o = DenovoOpts(float(min_id), float(min_cov), int(bool(paired)))
+        if out is None:
+            if text is not None:
+                raise ValueError("denovo_stats: the placed results go with the resident text (text=None)")
+            pr = np.zeros((self._n_resident, 4), np.uint32) if per_read else None
+            self.L.smr_denovo_stats_placed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+            self._check(self.L.smr_denovo_stats_placed(self.h, C.cast(C.byref(o), C.c_void_p), _ptr(pr) if pr is not None and pr.size else None,
+                                                       _ptr(tot)), "smr_denovo_stats_placed")
+            return pr, dict(zip(DENOVO_TOTALS, (int(v) for v in tot)))
         res, alns, st = out["res"], out["alns"], out.get("stats")
         txt = np.frombuffer(text, np.uint8) if text is not None else None
         n = res.shape[0]
-        per_read = np.zeros((n, 4), np.uint32)
-        tot = np.zeros(4, np.uint64)
-        o = DenovoOpts(float(min_id), float(min_cov), int(bool(paired)))
+        pr = np.zeros((n, 4), np.uint32) if per_read else None
         self.L.smr_denovo_stats.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32,
                                             C.c_void_p, C.c_void_p]
         rc = self.L.smr_denovo_stats(self.h, C.cast(C.byref(o), C.c_void_p), _ptr(txt) if txt is not None and txt.size else None,
                                      txt.size if txt is not None else 0, _ptr(res), _ptr(alns), _ptr(st) if st is not None else None, n,
-                                     _ptr(per_read) if n else None, _ptr(tot))
+                                     _ptr(pr) if pr is not None and n else None, _ptr(tot))
         self._check(rc, "smr_denovo_stats")
-        return per_read, dict(zip(DENOVO_TOTALS, (int(v) for v in tot)))
+        return pr, dict(zip(DENOVO_TOTALS, (int(v) for v in tot)))
 
     def otu_timings(self):
         out = np.zeros(3, np.float64)
@@ -893,8 +1002,11 @@ class ReportWriter:
             fh = self._parts[key] = open(os.path.join(self.dir, f".part_{key}"), "w+b")
         fh.write(data)
 
-    def write(self, out: dict, text: bytes | None = None) -> dict:
-        """format one batch (see Aligner.format_reports) and append its streams; returns them"""
+    def write(self, out: dict | None = None, text: bytes | None = None) -> dict:
+        """format one batch (see Aligner.format_reports) and append its streams; returns them.  out=None: the results the last
+        Aligner.place() placed on the device, with the resident text (their counters are the ones place() returned)."""
+        if out is None and text is not None:
+            raise ValueError("ReportWriter.write: the placed results go with the resident text (text=None)")
         if self.ext is None:
             first = text[:1] if text is not None else self.al.resident_text()[:1]
             self.ext = "fq" if first == b"@" else "fa"
@@ -917,8 +1029,9 @@ class ReportWriter:
         if self.otu_map is not None:
             self.al.otu_add(out, text)
         if self.summary is not None:
-            self.num_aligned += out["counters"]["num_aligned"]
-            m = np.asarray(out["matched"][:max(1, self.al.n_index_files)], np.uint64)
+            c = out if out is not None else self.al.placed_info
+            self.num_aligned += c["counters"]["num_aligned"]
+            m = np.asarray(c["matched"][:max(1, self.al.n_index_files)], np.uint64)
             self.reads_matched_per_db = m.copy() if self.reads_matched_per_db is None else self.reads_matched_per_db + m
         if self.denovo_counts is not None:
             mid, mcov = self.otu_map if self.otu_map is not None else (o.min_id, o.min_cov)
@@ -1000,3 +1113,273 @@ def align_files(aligner: Aligner, batch: hostio.ReadBatch):
     s = out if out["slots"] else unpack_alns(out, max(1, int(out["res"]["n_align"].max(initial=0))))   # the host formatter is strided
     out["sam"] = hostio.format_sam_rows(batch, refs, s["res"], s["alns"], s["cigar"], s["slots"])
     return out
+
+
+def _reads_ext(path: str) -> str:
+    """the read files' extension: fq for FASTQ input, fa for FASTA (report_fx_base.cpp:94), from the first byte of the reads"""
+    import gzip
+    with open(path, "rb") as f:
+        gz = f.read(2) == b"\x1f\x8b"
+    with (gzip.open(path, "rb") if gz else open(path, "rb")) as f:
+        return "fq" if f.read(1) == b"@" else "fa"
+
+
+class _FileWriter:
+    """The writer thread of run_files: appends the streams of one batch to their files while the caller makes the next batch.
+    Jobs are (buf, so, [(stream index, file handle)], release); release() hands buf back to the caller's pool once written."""
+
+    def __init__(self):
+        import queue
+        import threading
+        self.q = queue.Queue()
+        self.wait_s = self.write_s = 0.0
+        self.error = None
+        self.th = threading.Thread(target=self._loop, daemon=True)
+        self.th.start()
+
+    def _loop(self):
+        import time
+        while True:
+            t0 = time.perf_counter()
+            job = self.q.get()
+            t1 = time.perf_counter()
+            self.wait_s += t1 - t0
+            if job is None:
+                return
+            buf, so, dest, release = job
+            try:
+                if self.error is None:
+                    mv = memoryview(buf)
+                    for k, fh in dest:
+                        a, b = int(so[k]), int(so[k + 1])
+                        if b > a:
+                            fh.write(mv[a:b])
+            except BaseException as e:   # re-raised by the caller at the next put() or close()
+                self.error = e
+            finally:
+                release()
+            self.write_s += time.perf_counter() - t1
+
+    def put(self, job):
+        if self.error is not None:
+            raise self.error
+        self.q.put(job)
+
+    def close(self):
+        self.q.put(None)
+        self.th.join()
+        if self.error is not None:
+            raise self.error
+
+
+def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, minimal_score=None, evalue: float = 1.0, sam: bool = False,
+              sq: bool = False, blast=None, fastx: bool = False, other: bool = False, denovo=None, otu_map=None, paired_in: bool = False,
+              paired_out: bool = False, out2: bool = False, sout: bool = False, zip_out: bool = False, lnwin: int = 18, interval: int = 1,
+              max_pos: int = 10000, max_mb: float = 3072.0, skiplengths=None, index_budget: int = 0, batch_bytes: int = 256 << 20,
+              piece_bytes: int = 256 << 20, cmd: str = "", threads: int = 1, device: int = 0) -> dict:
+    """The reference's run from read files to its out/ directory, in one call: refs = the -ref FASTA files, reads = one reads file
+    or two mate files (plain or gzip), out_dir = where the report files go, under the reference's names.
+      1. the count pass over the reads (Aligner.read_counts);
+      2. per reference: the index statistics from the FASTA (hostio.fasta_index_stats), the minimal score (hostio.minimal_score at
+         E-value `evalue`, unless minimal_score[k] is given) and the E-value sizes, and the index built on the device
+         (Aligner.build_index_device: lnwin, interval, max_pos, max_mb, skiplengths[k] = -passes); index_budget > 0 bounds its device
+         memory (Aligner.set_index_budget);
+      3. the reads streamed through the device (stream_fastx, or stream_mates for two files) in batches of batch_bytes of text, each
+         run, placed on the device (Aligner.place) and formatted from there (the _placed calls), with the OTU map and the denovo
+         statistics added from the placed results too;
+      4. otu_map.txt and aligned.log (hostio.summary_log; cmd / threads / sq are what it prints).
+    gumbel[k] = (lambda, K) of refs[k]: the library does not compute them (the reference's ALP).  params: an api.Params (default
+    default_params()).  Report options as report_opts / ReportWriter take them: sam, sq (-SQ), blast ("1 cigar qcov qstrand", "0"),
+    fastx, other, denovo = (min_id, min_cov) for aligned_denovo.*, otu_map = (min_id, min_cov), paired_in / paired_out / out2 / sout,
+    zip_out (every report file gzip-compressed on the device, ".gz" appended; otu_map.txt and aligned.log stay plain).
+    Files are written by a writer thread while the caller's thread makes, runs and formats the next batch (the library calls release
+    the GIL); two output buffers alternate between them, and the streams go from those buffers to the files without a copy.  The
+    read files and the SAM / BLAST rows of the first (index, part) group are appended to their final files as they come.  With
+    several groups the rows of the other groups go to part files first and are appended at the end, as the reference's order (every
+    row of group 0, then of group 1, ...) requires: those bytes are written twice.
+    Returns {"reads", "batches", "num_aligned", "minimal_score", "paths", "seconds": per stage}: count, index, stream (the whole
+    streamed pass: from the first batch until every report file is complete and closed, the part files appended), produce (batch
+    production: push, inflate, cut, decode), run, place, format (the report calls, the OTU map and the denovo statistics), writer
+    (the writer thread's busy time), writer_wait (its idle time), caller_wait (the caller waiting for a free output buffer), parts
+    (appending the part files of the groups after the first, and closing the files), finish (otu_map.txt and aligned.log)."""
+    import shutil
+    import threading
+    import time
+    refs, reads = [os.fspath(r) for r in refs], [os.fspath(r) for r in ([reads] if isinstance(reads, (str, os.PathLike)) else reads)]
+    if len(reads) not in (1, 2):
+        raise ValueError("run_files: one reads file, or two mate files")
+    if len(gumbel) != len(refs) or (minimal_score is not None and len(minimal_score) != len(refs)):
+        raise ValueError("run_files: gumbel (and minimal_score) take one entry per reference")
+    params = params if params is not None else default_params()
+    mates = len(reads) == 2
+    o = report_opts(sam=sam, blast=blast, fastx=fastx, other=other, denovo=denovo, paired_in=paired_in, paired_out=paired_out,
+                    out2=out2, sout=sout)
+    pairwise = bool(o.blast) and o.blast_format == 0
+    rest = ReportOpts.from_buffer_copy(o)
+    if pairwise:
+        rest.blast = 0
+    pw_opts = report_opts(blast="0", paired_in=paired_in, paired_out=paired_out)
+    feed = "two_files" if mates else "one_file" if (paired_in or paired_out) else None
+    with_denovo = otu_map is not None or o.denovo
+    sec = dict.fromkeys(("count", "index", "stream", "produce", "run", "place", "format", "writer", "writer_wait", "caller_wait", "parts",
+                         "finish"), 0.0)
+    os.makedirs(out_dir, exist_ok=True)
+    al = Aligner(device)
+    files, parts = {}, {}
+    writer = None
+    try:
+        al.set_params(params)
+        t0 = time.perf_counter()
+        counts = al.read_counts(reads if mates else reads[0], piece_bytes)
+        sec["count"] = time.perf_counter() - t0
+        t0 = time.perf_counter()
+        stats, seqs = zip(*[hostio.fasta_index_stats(f, lnwin, max_mb) for f in refs])
+        ms = list(minimal_score) if minimal_score is not None else \
+            [hostio.minimal_score(st, lam, K, counts["length"], counts["reads"], evalue) for st, (lam, K) in zip(stats, gumbel)]
+        sk = list(skiplengths) if skiplengths is not None else [(lnwin, lnwin // 2, 3)] * len(refs)
+        if index_budget:
+            al.set_index_budget(index_budget)
+        for k, f in enumerate(refs):
+            al.build_index_device(k, f, hostio.split_by_parts(hostio.load_references(f), stats[k]), int(ms[k]), tuple(sk[k]), lnwin, interval,
+                                  max_pos, max_mb)
+            if o.blast:
+                lam, K = gumbel[k]
+                al.set_report_scoring(k, lam, K, *hostio.evalue_params(stats[k], K, counts["length"], counts["reads"]))
+        al.set_place_stats(bool(o.sam or o.blast or o.denovo or otu_map is not None))
+        if otu_map is not None:
+            al.otu_begin(otu_map[0], otu_map[1], paired_in=paired_in, paired_out=paired_out, feed=feed)
+        sec["index"] = time.perf_counter() - t0
+        # the files: every stream of a batch -> (file, or a part file for the SAM / BLAST rows of groups after the first)
+        G = len(al.report_groups())
+        ext, gz = _reads_ext(reads[0]), ".gz" if zip_out else ""
+
+        def open_file(name):
+            files[name] = open(os.path.join(out_dir, name + gz), "wb")
+            return files[name]
+
+        def part_file(key):
+            parts[key] = open(os.path.join(out_dir, f".part_{key}"), "w+b")
+            return parts[key]
+
+        dest, pw_dest = [], []
+        if o.sam:
+            fh = open_file("aligned.sam")
+            head = hostio.sam_header_of([x for s in seqs for x in s], cmd, sq).encode()
+            fh.write(al.gzip(head) if zip_out else head)
+            dest += [(g, fh if g == 0 else part_file(f"sam_{g}")) for g in range(G)]
+        if o.blast:
+            fh = open_file("aligned.blast")
+            (pw_dest if pairwise else dest).extend((g + (0 if pairwise else G), fh if g == 0 else part_file(f"blast_{g}")) for g in range(G))
+        num_out = num_out_of(o)
+        for j, (flag, name) in enumerate(((o.fastx, "aligned"), (o.other, "other"), (o.denovo, "aligned_denovo"))):
+            if flag:
+                dest += [(2 * G + j * num_out + i, open_file(f"{name}{sfx}.{ext}")) for i, sfx in enumerate(fx_suffixes(o))]
+        # two output buffers (one for each report call of a batch) alternate between this thread and the writer
+        free = [[np.zeros(1 << 20, np.uint8), np.zeros(1 << 16, np.uint8)] for _ in range(2)]
+        cv = threading.Condition()
+
+        def release(slot):
+            def f():
+                with cv:
+                    free.append(slot)
+                    cv.notify()
+            return f
+
+        writer = _FileWriter()
+        n_reads, num_aligned, n_batches = 0, 0, 0
+        matched = np.zeros(max(1, len(refs)), np.uint64)
+        dn = dict.fromkeys(DENOVO_TOTALS, 0)
+        dn_min, dn_paired = otu_map or denovo or (0, 0), bool(paired_in or paired_out) or feed is not None
+        gen = al.stream_mates(reads[0], reads[1], batch_bytes, piece_bytes) if mates else al.stream_fastx(reads[0], batch_bytes, piece_bytes)
+        t_stream = t0 = time.perf_counter()
+        for n in gen:
+            t1 = time.perf_counter()
+            sec["produce"] += t1 - t0
+            al.run_resident()
+            t2 = time.perf_counter()
+            info = al.place()
+            t3 = time.perf_counter()
+            n_reads += n
+            n_batches += 1
+            num_aligned += info["counters"]["num_aligned"]
+            matched += np.asarray(info["matched"][:matched.size], np.uint64)
+            with cv:
+                while not free:
+                    cv.wait()
+                slot = free.pop()
+            t4 = time.perf_counter()
+            jobs = []
+            if dest:
+                slot[0], so = al.format_placed_into(rest, slot[0], zip_out)
+                jobs.append((slot[0], so, dest))
+            if pw_dest:
+                slot[1], so = al.format_placed_into(pw_opts, slot[1], zip_out, pairwise=True)
+                jobs.append((slot[1], so, pw_dest))
+            if otu_map is not None:
+                al.otu_add(None)
+            if with_denovo:
+                for k, v in al.denovo_stats(None, None, dn_min[0], dn_min[1], dn_paired, per_read=False)[1].items():
+                    dn[k] += v
+            done = release(slot)
+            if not jobs:
+                done()
+            for i, (buf, so, d) in enumerate(jobs):
+                writer.put((buf, so, d, done if i + 1 == len(jobs) else (lambda: None)))
+            t0 = time.perf_counter()
+            sec["run"] += t2 - t1
+            sec["place"] += t3 - t2
+            sec["caller_wait"] += t4 - t3
+            sec["format"] += t0 - t4
+        sec["produce"] += time.perf_counter() - t0
+        writer.close()
+        sec["writer"], sec["writer_wait"] = writer.write_s, writer.wait_s
+        writer = None
+        t1 = time.perf_counter()
+        for key in [f"sam_{g}" for g in range(1, G)] + [f"blast_{g}" for g in range(1, G)]:
+            fh = parts.get(key)
+            if fh is not None:
+                fh.seek(0)
+                shutil.copyfileobj(fh, files["aligned.sam" if key.startswith("sam") else "aligned.blast"], 1 << 24)
+        paths = []
+        for name, fh in files.items():
+            if zip_out and fh.tell() == 0:
+                fh.write(al.gzip(b""))
+            fh.close()
+            paths.append(fh.name)
+        t0 = time.perf_counter()
+        sec["parts"] = t0 - t1
+        sec["stream"] = t0 - t_stream
+        total_otu = None
+        if otu_map is not None:
+            m = al.otu_finish()
+            total_otu = m["total_otu"]
+            if m["n_yid_ycov"] > 0:
+                path = os.path.join(out_dir, "otu_map.txt")
+                with open(path, "wb") as f:
+                    f.write(m["text"])
+                paths.append(path)
+        log = hostio.summary_log(cmd=cmd, refs=refs, reads=reads, total_reads=counts["reads"], num_aligned=num_aligned,
+                                 min_len=counts["min_len"], max_len=counts["max_len"], all_reads_len=counts["length"],
+                                 reads_matched_per_db=[int(x) for x in matched[:len(refs)]], gumbel=list(gumbel), minimal_score=[int(x) for x in ms],
+                                 lnwin=lnwin, skiplengths=sk, params=params, threads=threads, sq=sq,
+                                 denovo=dn["num_denovo"] if o.denovo else None, otu=(dn["n_yid_ycov"], total_otu) if otu_map is not None else None)
+        path = os.path.join(out_dir, "aligned.log")
+        with open(path, "wb") as f:
+            f.write(log.encode())
+        paths.append(path)
+        sec["finish"] = time.perf_counter() - t0
+        return dict(reads=n_reads, batches=n_batches, num_aligned=num_aligned, paths=paths, seconds=sec, minimal_score=[int(x) for x in ms])
+    finally:
+        if writer is not None:
+            try:
+                writer.close()
+            except BaseException:
+                pass
+        for fh in list(files.values()) + list(parts.values()):
+            fh.close()
+        for key in parts:
+            try:
+                os.unlink(os.path.join(out_dir, f".part_{key}"))
+            except OSError:
+                pass
+        al.close()

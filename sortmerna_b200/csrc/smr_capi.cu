@@ -22,6 +22,7 @@
 #include "smr_build.h"
 #include "smr_build_dev.cuh"
 #include "smr_final.cuh"
+#include "smr_place.cuh"
 #include "smr_index.h"
 
 using namespace smr;
@@ -156,6 +157,17 @@ struct smr_ctx {
     bool trace_error = false;
     RunTimes t_run; double t_d2h = 0;
   } pk;
+  // The results of the resident batch's last run placed on the device in the strided layout (smr_place_results, place_resident),
+  // kept until the batch is run again or replaced; the report-side _placed calls read them there.
+  struct Placed {
+    uint64_t run_id = 0;   // Batch::run_id of the run they come from; 0 = none
+    uint32_t nreads = 0, slots = 0; bool stats = false;
+    uint64_t cig_words = 0;
+    DevBuf res, aln, st, cig, cnt, words, off, scal;   // the placed arrays, the counters (ncnt u64), count-pass scratch
+    std::vector<uint64_t> cnt_host;                    // what smr_place_results adds to the caller's counters
+    double t_place = 0;                                // ms of the placement passes (CUDA events), retries excluded
+  } pl;
+  bool place_stats = false;   // smr_set_place_stats: every run computes the smr_aln_stats a placement keeps
   uint32_t lis_ctas_per_sm = kLisMinCtas;   // persistent CTAs of the candidate kernel per SM (matches its __launch_bounds__)
 
   // the resident batch and the text it was decoded from (smr_upload_*, smr_stream_next); clear_resident empties it
@@ -1298,7 +1310,7 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   const uint32_t slots = slots_of(ctx);
   const uint64_t nslots = batch_slots(ctx, bt, 0, nreads);
   const uint32_t* aln_base = bt.base.empty() ? nullptr : (const uint32_t*)bt.aln_base.p;
-  bt.run_slots = slots; bt.run_stats = ctx->host_stats || packed(ctx); bt.run_id = ++ctx->runs_made;
+  bt.run_slots = slots; bt.run_stats = ctx->host_stats || packed(ctx) || ctx->place_stats; bt.run_id = ++ctx->runs_made;
   std::lock_guard<std::mutex> dev_lock(device_kernel_mutex(ctx->device));   // held until the stream has drained
   auto& A = ctx->run;
   const std::vector<IndexGroup> groups = apply_budget(ctx);
@@ -1307,6 +1319,9 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
   for (const IndexGroup& gr : groups) arena_bytes = std::max(arena_bytes, gr.bytes);
   if (ng > 1 && (ctx->ib.arena.cap < arena_bytes || ctx->ib.arena.cap > ctx->ib.budget)) CK(ctx->ib.arena.alloc(arena_bytes));
   ensure_hit_regions(bt, max_group_parts(ctx));
+  // the stride may have grown since the upload sized these (smr_set_aln_slots, then smr_run_resident of the same batch)
+  ensure(bt.aln_work, (size_t)nslots * sizeof(AlnWork));
+  ensure(bt.out_aln, (size_t)nslots * sizeof(OutAln));
   RunGeom g = setup_arenas(ctx, bt.scale, bt.max_len);
   LisGlobals& lg = g.lg; FinalGlobals& fg = g.fg;
   // device copy of the part tables: [0, np) every part by its ordinal in the context (finalize looks parts up by gslot); with several
@@ -1389,7 +1404,7 @@ void run_impl(smr_ctx* ctx, Batch& bt) {
     fg.jobs = ensure<TraceJob>(A.tb_jobs, (size_t)chunk_slots * sizeof(TraceJob));
     fg.job_list = ensure<uint32_t>(A.fin_list, (size_t)chunk_slots * 4);
     // the packed layout always computes the stats: the caller's pointer only decides whether they are copied
-    fg.stats = ctx->host_stats || packed(ctx) ? ensure<AlnStats>(bt.aln_stats, (size_t)nslots * sizeof(AlnStats)) : nullptr;
+    fg.stats = bt.run_stats ? ensure<AlnStats>(bt.aln_stats, (size_t)nslots * sizeof(AlnStats)) : nullptr;
     const uint32_t jobs_grid = (uint32_t)std::min<uint64_t>((std::max<uint64_t>(chunk_slots, 1) + 255) / 256, (uint64_t)ctx->sm_count * 8);
     (aln_base ? final_jobs_kernel<true> : final_jobs_kernel<false>)<<<jobs_grid, 256, 0, ctx->stream>>>(b, fg);
     CK(cudaGetLastError());
@@ -1465,6 +1480,15 @@ struct HostOut {
   bool pool_short = false;   // cigar_cap was exceeded: nothing more is written, cigar_used goes on counting the words the batch needs
 };
 
+// a read stored more alignments than the stride (kOvfSlots): the batch needs smr_set_aln_slots(need) (smr_aln_slots_needed)
+[[noreturn]] void fail_need_slots(smr_ctx* ctx, uint32_t need, uint32_t slots) {
+  ctx->need_slots = need;
+  fail(SMR_ERR_CAPACITY, "all-alignments mode: a read stored " + std::to_string(need) + " alignments, the result stride is " +
+                             std::to_string(slots) + " (smr_set_aln_slots(" + std::to_string(need) + ") or more, then call again)");
+}
+const char* const kCigarOffsetMsg = "CIGAR pool offset passes 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches";
+const char* const kTraceErrorMsg = "trace back error (ssw.c:707 is fatal in the reference too)";
+
 // copies the results of a batch's run to the host; returns the indices of reads whose scratch overflowed
 void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint32_t>& flagged, const uint32_t* map /*local->caller index or null*/) {
   const uint32_t n = b.nreads;
@@ -1518,12 +1542,8 @@ void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint3
     }
   }
   coff[n] = run;
-  if (need_slots) {
-    ctx->need_slots = need_slots;
-    fail(SMR_ERR_CAPACITY, "all-alignments mode: a read stored " + std::to_string(need_slots) + " alignments, the result stride is " +
-                               std::to_string(slots) + " (smr_set_aln_slots(" + std::to_string(need_slots) + ") or more, then call again)");
-  }
-  if (run >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, "CIGAR pool offset passes 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches");
+  if (need_slots) fail_need_slots(ctx, need_slots, slots);
+  if (run >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, kCigarOffsetMsg);
   out.cigar_used = run;
   // a pool too small fails the call only at its end (download_resident): the flagged reads are still retried, so that
   // cigar_used names every word the batch needs and one larger pool is enough
@@ -1566,9 +1586,11 @@ void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint3
 }
 
 // Runs the flagged reads of a failed batch again as a batch of their own with 8x its scratch, gathered from its reads on the device,
-// and downloads them into the caller's arrays after what is there (map: index in `failed` -> the caller's index; null = the same).
-// Reads that overflow again go on to 64x and 512x.  The batch frees itself on return.
-void retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t>& flagged, const uint32_t* map, HostOut& out, int depth) {
+// and hands it to take(batch, map, again), which writes its results after what is there (map: index in the batch -> the caller's
+// index; `again`: the reads to retry once more): download_impl into the caller's arrays, or place_run into the placed arrays.
+// Reads that overflow again go on to 64x and 512x.  The batch frees itself on return, after take.
+template <class Take>
+void retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t>& flagged, const uint32_t* map, Take& take, int depth) {
   if (getenv("SMR_VERBOSE")) fprintf(stderr, "[smr] %zu reads overflowed their scratch at scale %u: retrying with scale %u (causes so far: lane %llu region %llu pairs %llu trace %llu cigar %llu err %llu)\n", flagged.size(), failed.scale, failed.scale * 8,
       (unsigned long long)ctx->flag_hist[0], (unsigned long long)ctx->flag_hist[1], (unsigned long long)ctx->flag_hist[2], (unsigned long long)ctx->flag_hist[3], (unsigned long long)ctx->flag_hist[4], (unsigned long long)ctx->flag_hist[5]);
   if (depth >= 3) fail(SMR_ERR_CAPACITY, "scratch overflow persists after 3 retries (" + std::to_string(flagged.size()) + " reads)");
@@ -1588,10 +1610,14 @@ void retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t
   run_impl(ctx, b);
   const double d2h = ctx->t_d2h;
   std::vector<uint32_t> again;
-  download_impl(ctx, b, out, again, smap.data());
+  take(b, smap.data(), again);
   ctx->t_run += b.run; ctx->t_d2h += d2h;
-  if (!again.empty()) retry_flagged(ctx, b, again, smap.data(), out, depth + 1);
+  if (!again.empty()) retry_flagged(ctx, b, again, smap.data(), take, depth + 1);
 }
+
+// the arenas grow with a retry's scale (after 64x, tens of GB): the next run allocates them again at its own, whether the retry
+// succeeds or not
+void release_retry_arenas(smr_ctx* ctx) { for (DevBuf* s : {&ctx->run.lis, &ctx->run.fin, &ctx->run.tb, &ctx->run.lane_hits}) s->reset(); }
 
 // the results of the resident batch's last run into the caller's arrays, its flagged reads retried; the resident batch and its
 // device results stay as they are
@@ -1600,14 +1626,130 @@ void download_resident(smr_ctx* ctx, HostOut& out) {
   std::vector<uint32_t> flagged;
   download_impl(ctx, ctx->res.b, out, flagged, nullptr);
   if (!flagged.empty()) {
-    // the arenas grow with the retry's scale (after 64x, tens of GB): the next run allocates them again at its own, whether the
-    // retry succeeds or not
-    const auto release = on_exit([ctx] { for (DevBuf* s : {&ctx->run.lis, &ctx->run.fin, &ctx->run.tb, &ctx->run.lane_hits}) s->reset(); });
-    retry_flagged(ctx, ctx->res.b, flagged, nullptr, out, 0);
+    const auto release = on_exit([ctx] { release_retry_arenas(ctx); });
+    auto take = [&](const Batch& b, const uint32_t* map, std::vector<uint32_t>& again) { download_impl(ctx, b, out, again, map); };
+    retry_flagged(ctx, ctx->res.b, flagged, nullptr, take, 0);
   }
   // the caller's CIGAR pool was too small: *cigar_used names the words the batch needs
   if (out.pool_short)
     fail(SMR_ERR_CAPACITY, "cigar pool too small: the batch needs " + std::to_string(out.cigar_used) + " words, cigar_cap is " + std::to_string(out.cigar_cap));
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// device placement (smr_place_results, smr_place.cuh): the strided results of the resident batch's last run kept on the device,
+// in the bytes download_resident writes to the host
+// ---------------------------------------------------------------------------------------------------------------------
+// the counters a placement keeps: SMR_CNT_FIXED + one reads_matched_per_db entry per index
+uint32_t place_counters(const smr_ctx* ctx) { return SMR_CNT_FIXED + std::max(1u, ctx->n_index_files); }
+
+// Places one run of a batch after what is placed: the resident batch's (map null), or a retry batch's through map (device array:
+// its read -> the resident batch's read).  As download_impl: a read flagged kOvfSlots fails the call with SMR_ERR_CAPACITY
+// (smr_aln_slots_needed), a trace back error with SMR_ERR_INDEX; `flagged` = the reads to retry.
+void place_run(smr_ctx* ctx, const Batch& b, const uint32_t* map, std::vector<uint32_t>& flagged) {
+  auto& P = ctx->pl;
+  flagged.clear();
+  const uint32_t n = b.nreads;
+  if (n == 0) return;
+  if (P.stats && !b.run_stats) fail(SMR_ERR_ARG, "a retry of the placed run computed no stats");
+  const uint32_t slots = slots_of(ctx), ncnt = place_counters(ctx);
+  uint64_t* words = ensure<uint64_t>(P.words, ((size_t)n + 1) * 8);
+  uint64_t* off = ensure<uint64_t>(P.off, ((size_t)n + 1) * 8);
+  PlaceWords* w = ensure<PlaceWords>(P.scal, sizeof(PlaceWords));
+  const PlaceIn in{(const ReadState*)b.state.p, (const uint32_t*)b.flags.p, (const uint16_t*)b.hit_db.p, (const OutAln*)b.out_aln.p,
+                   P.stats ? (const AlnStats*)b.aln_stats.p : nullptr, (const uint32_t*)b.cigar_pool.p, n, slots};
+  const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sm_count * 8);
+  CK(cudaMemsetAsync(w, 0, sizeof(PlaceWords), ctx->stream));
+  place_count_kernel<<<grid, 256, (size_t)ncnt * 8, ctx->stream>>>(in, (const unsigned long long*)b.counters.p, words, (unsigned long long*)P.cnt.p, ncnt, w);
+  CK(cudaGetLastError());
+  cub_run(ctx->cub_tmp, [&](void* t, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, words, off, (int)(n + 1), ctx->stream); });
+  PlaceWords hw{};
+  uint64_t total = 0;
+  CK(cudaMemcpyAsync(&hw, w, sizeof(hw), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&total, off + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (hw.need_slots) fail_need_slots(ctx, hw.need_slots, slots);
+  const uint64_t run = P.cig_words + total;
+  if (run >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, kCigarOffsetMsg);
+  if (hw.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
+  ensure_keep(ctx, P.cig, run * 4 + 16, P.cig_words * 4);
+  const PlaceOut o{(smr_read_result*)P.res.p, (smr_aln*)P.aln.p, P.stats ? (smr_aln_stats*)P.st.p : nullptr, (uint32_t*)P.cig.p, map, P.cig_words};
+  place_scatter_kernel<<<grid, 256, 0, ctx->stream>>>(in, off, o);
+  CK(cudaGetLastError());
+  P.cig_words = run;
+  if (hw.flagged) {   // rare: the flags come down only then
+    std::vector<uint32_t> fl(n);
+    CK(cudaMemcpyAsync(fl.data(), b.flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    for (uint32_t r = 0; r < n; ++r) {
+      if (!fl[r]) continue;
+      flagged.push_back(r);
+      for (int bit = 0; bit < 6; ++bit) if (fl[r] & (1u << bit)) ctx->flag_hist[bit]++;
+    }
+  }
+}
+
+// Places the resident batch's last run and its retries (once per run: a later call finds them placed).  The retries compute the
+// stats when the run did, whatever smr_set_place_stats says now.
+void place_resident(smr_ctx* ctx) {
+  auto& P = ctx->pl;
+  const Batch& R = ctx->res.b;
+  if (R.run_id == 0) fail(SMR_ERR_ARG, "smr_place_results: the resident batch has not been run (smr_run_resident)");
+  if (R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, "smr_place_results: the resident batch was run at another stride: call smr_run_resident again");
+  if (P.run_id == R.run_id) return;
+  P.run_id = 0;
+  const uint32_t n = R.nreads, slots = slots_of(ctx), ncnt = place_counters(ctx);
+  P.nreads = n; P.slots = slots; P.stats = R.run_stats; P.cig_words = 0; P.t_place = 0;
+  ensure(P.res, (size_t)n * sizeof(smr_read_result) + 16);
+  ensure(P.aln, (size_t)n * slots * sizeof(smr_aln) + 16);
+  if (P.stats) ensure(P.st, (size_t)n * slots * sizeof(smr_aln_stats) + 16);
+  ensure(P.cig, 16);
+  ensure(P.cnt, (size_t)ncnt * 8);
+  CK(cudaMemsetAsync(P.cnt.p, 0, (size_t)ncnt * 8, ctx->stream));
+  ctx->t_run = R.run; ctx->t_d2h = 0;
+  const bool keep = ctx->place_stats;
+  const auto restore = on_exit([ctx, keep] { ctx->place_stats = keep; });
+  ctx->place_stats = P.stats;
+  cudaEvent_t* e = events(ctx, 2);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  std::vector<uint32_t> flagged;
+  place_run(ctx, R, nullptr, flagged);
+  CK(cudaEventRecord(e[1], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  P.t_place = elapsed_ms(e[0], e[1]);
+  if (!flagged.empty()) {
+    const auto release = on_exit([ctx] { release_retry_arenas(ctx); });
+    auto take = [&](const Batch& b, const uint32_t* map, std::vector<uint32_t>& again) {
+      DevBuf dmap;
+      upload_async(ctx, dmap, map, b.nreads);
+      place_run(ctx, b, (const uint32_t*)dmap.p, again);
+      CK(cudaStreamSynchronize(ctx->stream));   // before dmap and the batch free themselves
+    };
+    retry_flagged(ctx, R, flagged, nullptr, take, 0);
+  }
+  P.cnt_host.assign(ncnt, 0);
+  CK(cudaMemcpyAsync(P.cnt_host.data(), P.cnt.p, (size_t)ncnt * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  P.run_id = R.run_id;
+}
+
+// the placed arrays, as the report-side calls take them
+struct PlacedArrays {
+  const smr_read_result* res; const smr_aln* aln; const uint32_t* cig; uint64_t cig_words; const smr_aln_stats* st; uint32_t n;
+};
+
+// The placed results of the resident batch's last run for the _placed call `call`; need_stats: the call reads the stats.
+PlacedArrays placed_of(const smr_ctx* ctx, const char* call, bool need_stats) {
+  if (packed(ctx))
+    fail(SMR_ERR_UNSUPPORTED, std::string(call) + ": results are placed on the device in the strided layout only; in the packed layout "
+                              "download them (smr_download_results_packed) and pass them to the call that takes result arrays");
+  const auto& P = ctx->pl;
+  if (P.run_id == 0 || P.run_id != ctx->res.b.run_id)
+    fail(SMR_ERR_ARG, std::string(call) + ": no placed results of the resident batch's last run: call smr_place_results after smr_run_resident");
+  if (P.slots != slots_of(ctx)) fail(SMR_ERR_ARG, std::string(call) + ": the results were placed at another stride");
+  if (need_stats && !P.stats)
+    fail(SMR_ERR_ARG, std::string(call) + ": the placed run computed no smr_aln_stats: call smr_set_place_stats(ctx, 1) before smr_run_resident");
+  return PlacedArrays{(const smr_read_result*)P.res.p, (const smr_aln*)P.aln.p, (const uint32_t*)P.cig.p, P.cig_words,
+                      P.stats ? (const smr_aln_stats*)P.st.p : nullptr, P.nreads};
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1859,9 +2001,11 @@ std::vector<RptGroup> rpt_groups(const smr_ctx* ctx, bool names, bool scoring) {
 
 // The first half of a report-side call, after rpt_check_batch: text, results and groups on the device (e[0] recorded before the
 // copies, e[1] after them), the record layout of the text (text_layout, then rpt_records_kernel); returns the report arguments.
-// Their error word (err) is zeroed here; the caller reads it back with its results and passes it to rpt_check.
+// Their error word (err) is zeroed here; the caller reads it back with its results and passes it to rpt_check.  dev: results,
+// alns, cigar and stats are the placed device arrays (placed_of), read where they are instead of uploaded.
 RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const uint32_t* cigar,
-                     uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads, const std::vector<RptGroup>& hg, const cudaEvent_t* e) {
+                     uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads, const std::vector<RptGroup>& hg, const cudaEvent_t* e,
+                     bool dev = false) {
   auto& S = ctx->r;
   CK(cudaEventRecord(e[0], ctx->stream));
   const uint32_t slots = slots_of(ctx), G = (uint32_t)hg.size();
@@ -1879,10 +2023,12 @@ RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_
   char c0 = 0;
   if (nbytes) { if (text) c0 = text[0]; else CK(cudaMemcpy(&c0, dt, 1, cudaMemcpyDeviceToHost)); }
   // results
-  upload_async(ctx, S.res, results, nreads);
-  upload_async(ctx, S.aln, alns, N);
-  upload_async(ctx, S.cig, cigar, cigar ? cigar_words : 0);
-  upload_async(ctx, S.st, stats, stats ? N : 0);
+  if (!dev) {
+    upload_async(ctx, S.res, results, nreads);
+    upload_async(ctx, S.aln, alns, N);
+    upload_async(ctx, S.cig, cigar, cigar ? cigar_words : 0);
+    upload_async(ctx, S.st, stats, stats ? N : 0);
+  }
   upload_async(ctx, S.grp, hg.data(), G);
   CK(cudaEventRecord(e[1], ctx->stream));
   const TextLayout L = text_layout(ctx, dt, nbytes, c0);
@@ -1897,6 +2043,10 @@ RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_
   a.rec = (const RptRec*)S.recs.p; a.nreads = nreads; a.slots = slots; a.nslots = N;
   a.res = (const smr_read_result*)S.res.p; a.aln = (const smr_aln*)S.aln.p; a.cigar = (const uint32_t*)S.cig.p;
   a.cigar_words = cigar ? cigar_words : 0; a.st = (const smr_aln_stats*)S.st.p;
+  if (dev) {   // a call without stats still gets a readable array, as an upload of none leaves one
+    a.res = results; a.aln = alns; a.cigar = cigar;
+    a.st = stats ? stats : ensure<smr_aln_stats>(S.st, 16);
+  }
   a.grp = (const RptGroup*)S.grp.p; a.ngroups = G; a.err = &text_words(ctx)->rpt_err;
   CK(cudaMemsetAsync(a.err, 0, 4, ctx->stream));
   if (nreads) {
@@ -1999,7 +2149,7 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
 // smr_format_reports[_gz].  Both share the routing (the skip of empty reads), the row order and the scans.
 void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
                          const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
-                         char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise) {
+                         char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise, bool dev = false) {
   const bool mates = o->mates || (!text && ctx->res.mates);   // the resident batch of a mate stream is mates
   const bool paired = o->paired_in || o->paired_out || mates;
   if (pairwise) {   // -blast '0 cigar' is refused by the reference too (options.cpp:584-588)
@@ -2026,7 +2176,7 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   const std::vector<RptGroup> hg = rpt_groups(ctx, o->sam || o->blast, o->blast);
   const uint32_t G = (uint32_t)hg.size(), nso = 2 * G + nfx + 1;
   cudaEvent_t* e = events(ctx, 4);
-  RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e);
+  RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e, dev);
   const uint64_t N = a.nslots;
   const int grid = ctx->sm_count * 8;
   auto& S = ctx->r;
@@ -2160,7 +2310,7 @@ void otu_begin_impl(smr_ctx* ctx, const smr_otu_opts* o) {
 
 // returns the number of entries added
 uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
-                      uint32_t nreads) {
+                      uint32_t nreads, bool dev = false) {
   auto& U = ctx->otu;
   otu_open(ctx);
   if (!text && ctx->res.mates && U.feed != SMR_OTU_TWO_FILES)
@@ -2168,7 +2318,7 @@ uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr
   rpt_check_batch(ctx, "the OTU map", results, alns, stats, nreads, U.feed != SMR_OTU_SINGLE,
                   "the OTU map needs the results, alignments and smr_aln_stats of the batch");
   cudaEvent_t* e = events(ctx, 3);
-  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e);
+  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e, dev);
   const uint64_t N = a.nslots;
   const OtuArgs oa{(const uint32_t*)U.rank.p, (const uint32_t*)U.rank_off.p, U.gbits, U.min_id, U.min_cov, U.feed};
   uint32_t* flag = ensure<uint32_t>(U.flag, (N + 1) * 4);
@@ -2249,13 +2399,13 @@ void otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) 
 // De novo statistics (smr_otu.cuh, denovo_stats_kernel)
 // ---------------------------------------------------------------------------------------------------------------------
 void denovo_stats_impl(smr_ctx* ctx, const smr_denovo_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
-                       const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4]) {
+                       const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4], bool dev = false) {
   rpt_check_batch(ctx, "the denovo statistics", results, alns, stats, nreads, false,
                   "the denovo statistics need the results, alignments and smr_aln_stats of the batch");
   const bool paired = o->paired || (!text && ctx->res.mates);   // the resident batch of a mate stream is mates
   cudaEvent_t* e = events(ctx, 4);
   // the loaded (index, part)s: an alignment of any other is refused
-  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, rpt_groups(ctx, false, false), e);
+  const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, rpt_groups(ctx, false, false), e, dev);
   uint32_t* dread = ensure<uint32_t>(ctx->dn.read, ((size_t)nreads + 1) * 16);
   unsigned long long* dtot = ensure<unsigned long long>(ctx->dn.tot, 32);
   CK(cudaMemsetAsync(dread, 0, (size_t)nreads * 16, ctx->stream));
@@ -2948,6 +3098,96 @@ int smr_denovo_stats(smr_ctx* ctx, const smr_denovo_opts* opts, const char* text
   if (!ctx || !opts || !totals || (!text && nbytes)) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   denovo_stats_impl(ctx, opts, text, nbytes, results, alns, stats, nreads, per_read, totals);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+// -- results placed on the device (smr_place.cuh) --
+int smr_set_place_stats(smr_ctx* ctx, int on) {
+  if (!ctx) return SMR_ERR_ARG;
+  ctx->place_stats = on != 0;
+  return SMR_OK;
+}
+
+int smr_place_results(smr_ctx* ctx, uint64_t* counters, uint32_t n_counters, uint64_t* n_alns, uint64_t* cigar_words) try {
+  if (!ctx) return SMR_ERR_ARG;
+  if (n_alns) *n_alns = 0;
+  if (cigar_words) *cigar_words = 0;
+  if (packed(ctx)) {
+    ctx->err = "smr_place_results places the strided layout only: in the packed layout call smr_download_results_packed";
+    return SMR_ERR_UNSUPPORTED;
+  }
+  CK(cudaSetDevice(ctx->device));
+  place_resident(ctx);
+  const auto& P = ctx->pl;
+  if (n_alns) *n_alns = (uint64_t)P.nreads * P.slots;
+  if (cigar_words) *cigar_words = P.cig_words;
+  if (counters)
+    for (uint32_t k = 0; k < n_counters && k < P.cnt_host.size(); ++k) counters[k] += P.cnt_host[k];
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_download_placed(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, smr_aln_stats* stats, uint32_t* cigar_pool, uint64_t cigar_cap) try {
+  if (!ctx) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  const PlacedArrays p = placed_of(ctx, "smr_download_placed", stats != nullptr);
+  const uint64_t N = (uint64_t)p.n * ctx->pl.slots;
+  if (p.n && (!results || !alns)) fail(SMR_ERR_ARG, "smr_download_placed: null result array");
+  if (p.cig_words > cigar_cap || (p.cig_words && !cigar_pool))
+    fail(SMR_ERR_CAPACITY, "cigar pool too small: the batch needs " + std::to_string(p.cig_words) + " words, cigar_cap is " + std::to_string(cigar_cap));
+  if (p.n) {
+    CK(cudaMemcpyAsync(results, p.res, (size_t)p.n * sizeof(smr_read_result), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(alns, p.aln, N * sizeof(smr_aln), cudaMemcpyDeviceToHost, ctx->stream));
+    if (stats) CK(cudaMemcpyAsync(stats, p.st, N * sizeof(smr_aln_stats), cudaMemcpyDeviceToHost, ctx->stream));
+  }
+  if (p.cig_words) CK(cudaMemcpyAsync(cigar_pool, p.cig, p.cig_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_last_place_timing(const smr_ctx* ctx, double* ms) {
+  if (!ctx || !ms) return SMR_ERR_ARG;
+  *ms = ctx->pl.t_place;
+  return SMR_OK;
+}
+
+// the report-side calls on the placed results: format_reports_impl and the rest with dev = true
+static int format_placed(smr_ctx* ctx, const char* call, const smr_report_opts* o, char* out, uint64_t cap, uint64_t* stream_off, bool gz,
+                         bool pairwise) try {
+  if (!ctx || !o || !stream_off) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  const PlacedArrays p = placed_of(ctx, call, o->sam || (o->blast && !pairwise) || o->denovo);
+  format_reports_impl(ctx, o, nullptr, 0, p.res, p.aln, p.cig, p.cig_words, p.st, p.n, out, cap, stream_off, gz, pairwise, true);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_format_reports_placed(smr_ctx* ctx, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off) {
+  return format_placed(ctx, "smr_format_reports_placed", opts, out, cap, stream_off, false, false);
+}
+int smr_format_reports_placed_gz(smr_ctx* ctx, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off) {
+  return format_placed(ctx, "smr_format_reports_placed_gz", opts, out, cap, stream_off, true, false);
+}
+int smr_format_blast_pairwise_placed(smr_ctx* ctx, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off) {
+  return format_placed(ctx, "smr_format_blast_pairwise_placed", opts, out, cap, stream_off, false, true);
+}
+int smr_format_blast_pairwise_placed_gz(smr_ctx* ctx, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off) {
+  return format_placed(ctx, "smr_format_blast_pairwise_placed_gz", opts, out, cap, stream_off, true, true);
+}
+
+int smr_otu_add_placed(smr_ctx* ctx, uint64_t* n_added) try {
+  if (!ctx) return SMR_ERR_ARG;
+  if (n_added) *n_added = 0;
+  CK(cudaSetDevice(ctx->device));
+  const PlacedArrays p = placed_of(ctx, "smr_otu_add_placed", true);
+  const uint64_t m = otu_add_impl(ctx, nullptr, 0, p.res, p.aln, p.st, p.n, true);
+  if (n_added) *n_added = m;
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_denovo_stats_placed(smr_ctx* ctx, const smr_denovo_opts* opts, uint32_t* per_read, uint64_t totals[4]) try {
+  if (!ctx || !opts || !totals) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  const PlacedArrays p = placed_of(ctx, "smr_denovo_stats_placed", true);
+  denovo_stats_impl(ctx, opts, nullptr, 0, p.res, p.aln, p.st, p.n, per_read, totals, true);
   return SMR_OK;
 } SMR_CATCH(ctx)
 

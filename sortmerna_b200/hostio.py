@@ -185,7 +185,7 @@ def sam_header(prefixes: list, cmdline: str, sq: bool = False) -> str:
     """The header of aligned.sam (ReportSam::write_header, report_sam.cpp:154-205): @HD, with sq (-SQ) one @SQ line per reference
     sequence of every index in --ref order (read from the sequence table after the part table of <prefix>.stats), and @PG with the
     command line."""
-    out = ["@HD\tVN:1.0\tSO:unsorted\n"]
+    seqs = []
     for prefix in prefixes:
         with open(prefix + ".stats", "rb") as fh:
             b = fh.read()
@@ -197,10 +197,86 @@ def sam_header(prefixes: list, cmdline: str, sq: bool = False) -> str:
             (lid,) = struct.unpack_from("<I", b, o); o += 4
             sid = b[o:o + lid].decode(); o += lid
             (lseq,) = struct.unpack_from("<I", b, o); o += 4
-            if sq:
-                out.append(f"@SQ\tSN:{sid}\tLN:{lseq}\n")
+            seqs.append((sid, lseq))
+    return sam_header_of(seqs, cmdline, sq)
+
+
+def sam_header_of(seqs: list, cmdline: str, sq: bool = False) -> str:
+    """sam_header from the (id, length) of every reference sequence of every index in --ref order"""
+    out = ["@HD\tVN:1.0\tSO:unsorted\n"]
+    if sq:
+        out += [f"@SQ\tSN:{sid}\tLN:{lseq}\n" for sid, lseq in seqs]
     out.append(f"@PG\tID:sortmerna\tVN:1.0\tCL:{cmdline}\n")
     return "".join(out)
+
+
+# the index builder's 2-bit code of a letter (map_nt, indexdb.cpp:83-109): what the background frequencies count
+_BUILD_NT = np.zeros(256, np.uint8)
+for _c in b"BCDWYbcwy":
+    _BUILD_NT[_c] = 1
+for _c in b"GKSXgksx":
+    _BUILD_NT[_c] = 2
+for _c in b"TUtu":
+    _BUILD_NT[_c] = 3
+
+
+def fasta_index_stats(fasta: str, lnwin: int = 18, max_mb: float = 3072.0):
+    """What <prefix>.stats of the index of `fasta` holds (build_index STEP 1 and the part split, indexdb.cpp:1188-1271 and
+    1381-1431, as smr_build_index writes it), computed from the FASTA alone: (IndexStats with prefix "", [(id, length) of every
+    sequence]).  A caller that builds the index on the device (Aligner.build_index_device) takes the minimal score, the E-value
+    sizes, the per-part references (split_by_parts) and the -SQ lines of the SAM header from it."""
+    with open(fasta, "rb") as fh:
+        b = fh.read()
+    if not b:
+        raise ValueError(f"{fasta}: empty reference file")
+    a = np.frombuffer(b, np.uint8)
+    pread = lnwin + 1
+    starts = np.flatnonzero(a == ord(">"))
+    if starts.size == 0 or starts[0] != 0:
+        raise ValueError(f"{fasta}: each header of a database FASTA file must begin with '>'")
+    ends = np.append(starts[1:], a.size)
+    nl = np.flatnonzero(a == ord("\n"))
+    seqs, lens, rec = [], [], []
+    body = np.zeros(a.size + 1, np.int64)   # body[i]: sequence letters before byte i
+    seq_mask = np.zeros(a.size, bool)
+    for s0, e0 in zip(starts.tolist(), ends.tolist()):
+        k = np.searchsorted(nl, s0)
+        h1 = int(nl[k]) if k < nl.size and nl[k] < e0 else e0
+        name = b[s0 + 1:h1]
+        cut = min((i for i in (name.find(b" "), name.find(b"\t")) if i >= 0), default=len(name))
+        seqs.append(name[:cut].decode(errors="replace"))
+        rec.append((s0, e0, min(h1 + 1, e0)))
+        seq_mask[min(h1 + 1, e0):e0] = True
+    seq_mask &= (a != ord("\n")) & (a != ord(" "))
+    np.cumsum(seq_mask, out=body[1:])
+    lens = [int(body[e0] - body[q0]) for (_, e0, q0) in rec]
+    short = [n for n in lens if n < pread]
+    if short:
+        raise ValueError(f"{fasta}: at least one sequence is shorter than the seed length {pread}")
+    freq = np.bincount(_BUILD_NT[a[seq_mask & (a != ord("N"))]], minlength=4).astype(np.float64)
+    tot = float(freq.sum())
+    parts, first = [], 0
+    while first < len(rec):
+        size, members, nxt, part_size = 0.0, 0, first, 0
+        while nxt < len(rec):
+            est = float(lens[nxt] - pread + 1) * 9.5e-6
+            if est > max_mb:
+                nxt += 1
+                continue
+            if size + est > max_mb:
+                break
+            size += est
+            part_size = rec[nxt][1] - rec[first][0]
+            members += 1
+            nxt += 1
+        if members == 0:
+            if nxt < len(rec):
+                raise ValueError(f"{fasta}: every sequence is too large to be indexed with the current memory limit")
+            break
+        parts.append((rec[first][0], part_size, members))
+        first = nxt
+    st = IndexStats("", a.size, fasta, tuple(float(f / tot) for f in freq), int(sum(lens)), lnwin, len(rec), len(parts), parts)
+    return st, list(zip(seqs, lens))
 
 
 def find_index_prefixes(idx_dir: str) -> dict:
