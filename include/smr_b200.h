@@ -231,8 +231,9 @@ int smr_align_batch_packed(smr_ctx*, const uint8_t* seq_cat, const uint64_t* seq
                            uint64_t cigar_cap, uint64_t* cigar_used, uint64_t* counters, uint32_t n_counters);
 /* smr_download_results in the packed layout, with the arguments of smr_align_batch_packed.  The batch must have been run
  * (smr_run_resident) in this layout at the current stride; it never changes the resident batch, and may be called again.  The
- * first download after a run runs the reads that outgrew the stride and places every read; the library keeps that result (host
- * memory of the size of the returned arrays) until the batch is run again or replaced, so a later download copies it. */
+ * first download after a run runs the reads that outgrew the stride and places every read on the device (smr_place_results_packed);
+ * the library keeps that placement (device memory of the size of the returned arrays) until the batch is run again or replaced,
+ * so a later download copies it. */
 int smr_download_results_packed(smr_ctx*, smr_read_result* results, smr_aln* alns, uint64_t aln_cap, uint64_t* aln_used,
                                 smr_aln_stats* stats, uint32_t* cigar_pool, uint64_t cigar_cap, uint64_t* cigar_used,
                                 uint64_t* counters, uint32_t n_counters);
@@ -467,9 +468,10 @@ int smr_denovo_stats(smr_ctx*, const smr_denovo_opts* opts, const char* text, ui
                      const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4]);
 
 /* -- results placed on the device (sortmerna_b200/csrc/smr_place.cuh, DESIGN.md 5g): the last smr_run_resident of the resident
- *    batch turned into the strided layout of smr_download_results in device memory, where the report-side _placed calls read it:
- *    nothing goes down to the host and comes back between the alignment and the report writers.  Strided layout only: in the packed
- *    layout (smr_set_aln_layout) every call below but smr_set_place_stats is SMR_ERR_UNSUPPORTED. */
+ *    batch turned into the layout of smr_download_results (strided, smr_place_results) or of smr_download_results_packed (packed,
+ *    smr_place_results_packed) in device memory, where the report-side _placed calls read it: nothing goes down to the host and
+ *    comes back between the alignment and the report writers.  In the packed layout (smr_set_aln_layout) smr_place_results is
+ *    SMR_ERR_UNSUPPORTED, and the _placed calls read the packed placement of the resident batch's last run. */
 /* Whether every later run computes the smr_aln_stats a placement keeps (default 0).  The _placed calls that read stats (SAM,
  * tabular BLAST, aligned_denovo, the OTU map, the denovo statistics) need a placement of a run made with it on; a run made with a
  * host stats buffer (smr_set_stats_buffer) computes them too.  The scratch-overflow retries of a placement compute the stats when
@@ -485,15 +487,30 @@ int smr_set_place_stats(smr_ctx*, int on);
  * the placed arrays until the batch is run again or replaced (keyed by the run); a second call for the same run places nothing
  * again and adds the same counters.  SMR_ERR_ARG if the batch was not run, or was run at another stride. */
 int smr_place_results(smr_ctx*, uint64_t* counters, uint32_t n_counters, uint64_t* n_alns, uint64_t* cigar_words);
-/* The placed arrays copied to the host (a caller that also wants smr_pack_kvdb_blobs): results[n], alns[n * stride], stats
- * (nullable; SMR_ERR_ARG if the placed run computed none) and cigar_pool[cigar_cap] (SMR_ERR_CAPACITY below *cigar_words). */
+/* The packed layout's placement: the bytes smr_download_results_packed writes -- smr_read_result[n], smr_aln[sum n_align] and
+ * the stats alike in read order, the CIGARs compacted in read order, with the same re-runs of reads that stored more alignments
+ * than the stride or overflowed their scratch -- placed in device memory.  The first run stays on the device; only the flagged reads'
+ * index, flags and n_align come to the host, which forms the re-runs; each re-run's results stay on the device until one count
+ * pass, two scans and one scatter place every read from the run that stored it.  counters as smr_download_results_packed adds them
+ * (nullable); *n_alns = the alignments placed (sum n_align), *cigar_words = the CIGAR words (both nullable).  A packed download
+ * places the same way and keeps its placement here, so either serves the other and the _placed calls; a second call for the same
+ * run places nothing and adds the same counters.  A trace back error gives SMR_ERR_INDEX after the results are placed (sizes set),
+ * as the packed download does.  SMR_ERR_ARG in the strided layout (use smr_place_results), before a run, or after a run at
+ * another stride. */
+int smr_place_results_packed(smr_ctx*, uint64_t* counters, uint32_t n_counters, uint64_t* n_alns, uint64_t* cigar_words);
+/* The placed arrays copied to the host (a caller that also wants smr_pack_kvdb_blobs): results[n], alns[n * stride] (packed:
+ * alns[n_alns] of smr_place_results_packed), stats (nullable; SMR_ERR_ARG if the placed run computed none) and
+ * cigar_pool[cigar_cap] (SMR_ERR_CAPACITY below *cigar_words). */
 int smr_download_placed(smr_ctx*, smr_read_result* results, smr_aln* alns, smr_aln_stats* stats, uint32_t* cigar_pool, uint64_t cigar_cap);
-/* milliseconds (CUDA events) of the last placement's count, scan and scatter passes over the resident batch (retries excluded) */
+/* milliseconds (CUDA events) of the last placement's count, scan and scatter passes over the resident batch (retries and packed
+ * re-runs excluded) */
 int smr_last_place_timing(const smr_ctx*, double* ms);
 /* The report-side calls on the placed results of the resident batch's last run and its resident text: smr_format_reports[_gz],
  * smr_format_blast_pairwise[_gz], smr_otu_add and smr_denovo_stats without text, results, alns, cigar_pool or stats; everything else
  * (opts, out, cap, stream_off, SMR_ERR_CAPACITY, n_added, per_read, totals) as there.  SMR_ERR_ARG without a placement of the
- * resident batch's last run (none yet, or one of an earlier run or batch), or when the call reads stats the placement lacks. */
+ * resident batch's last run (none yet, or one of an earlier run or batch), or when the call reads stats the placement lacks.  In
+ * the packed layout they read the packed placement (which always has the stats) and are SMR_ERR_UNSUPPORTED without one of the
+ * resident batch's last run; SMR_ERR_INDEX if that placement met a trace back error. */
 int smr_format_reports_placed(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
 int smr_format_reports_placed_gz(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
 int smr_format_blast_pairwise_placed(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);

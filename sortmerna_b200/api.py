@@ -34,7 +34,8 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_denovo_stats", "smr_set_aln_layout", "smr_align_batch_packed", "smr_download_results_packed", "smr_pack_kvdb_blobs_packed",
            "smr_set_index_budget", "smr_index_residency", "smr_set_place_stats", "smr_place_results", "smr_download_placed",
            "smr_last_place_timing", "smr_format_reports_placed", "smr_format_reports_placed_gz", "smr_format_blast_pairwise_placed",
-           "smr_format_blast_pairwise_placed_gz", "smr_otu_add_placed", "smr_denovo_stats_placed"]
+           "smr_format_blast_pairwise_placed_gz", "smr_otu_add_placed", "smr_denovo_stats_placed",
+           "smr_place_results_packed"]
 
 # smr_set_aln_layout: strided, nreads * slots alignments; packed, read r's n_align alignments from the sum of the counts before it
 ALN_LAYOUTS = {"strided": 0, "packed": 1}
@@ -646,7 +647,8 @@ class Aligner:
         self._check(self.L.smr_set_place_stats(self.h, C.c_int(1 if on else 0)), "smr_set_place_stats")
 
     def place(self) -> dict:
-        """smr_place_results: the results of the last run_resident() placed on the device in the strided layout, its scratch-overflow
+        """smr_place_results: the results of the last run_resident() placed on the device in the strided layout (the packed layout
+        is place_packed()), its scratch-overflow
         retries included; format_reports / format_blast_pairwise / otu_add / denovo_stats / ReportWriter.write with out=None read
         them there.  In the all-alignments mode (num_alignments 0) a read that stores more alignments than the stride makes the
         stride grow to what the library names and the batch run again, as align() does.  Returns {"nreads", "slots", "n_alns",
@@ -672,15 +674,38 @@ class Aligner:
                     counters={k: int(counters[i]) for i, k in enumerate(CNT_NAMES)}, matched=counters[CNT_FIXED:].copy(), place_ms=ms.value)
         return self.placed_info
 
+    def place_packed(self) -> dict:
+        """smr_place_results_packed: the results of the last run_resident() in the packed layout placed on the device, as download()
+        returns them there: the reads that stored more alignments than the first run's stride run again at their own count, and
+        the reads that overflowed their scratch at a larger scale, then every read placed in read order.  format_reports /
+        format_blast_pairwise / format_placed_into / otu_add / denovo_stats / ReportWriter.write with out=None read them there, and
+        a later download() copies them.  Returns the dict place() returns, with "slots" = 0 and "n_alns" = the sum of n_align."""
+        self.L.smr_place_results_packed.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+        self.L.smr_last_place_timing.argtypes = [C.c_void_p, C.c_void_p]
+        counters = np.zeros(CNT_FIXED + max(1, self.n_index_files), np.uint64)
+        n_alns, words = C.c_uint64(0), C.c_uint64(0)
+        rc = self.L.smr_place_results_packed(self.h, _ptr(counters), counters.size, C.cast(C.byref(n_alns), C.c_void_p),
+                                             C.cast(C.byref(words), C.c_void_p))
+        self._check(rc, "smr_place_results_packed")
+        ms = C.c_double(0)
+        self.L.smr_last_place_timing(self.h, C.cast(C.byref(ms), C.c_void_p))
+        self.placed_info = dict(nreads=self._n_resident, slots=0, n_alns=int(n_alns.value), cigar_words=int(words.value),
+                    counters={k: int(counters[i]) for i, k in enumerate(CNT_NAMES)}, matched=counters[CNT_FIXED:].copy(), place_ms=ms.value)
+        return self.placed_info
+
     def download_placed(self, with_stats: bool = False) -> dict:
         """smr_download_placed: the placed arrays on the host, in the form download() returns ("res", "alns", "cigar", "slots", and
-        "stats" with with_stats); the counters are those place() returned."""
-        n, slots = self._n_resident, int(self.L.smr_aln_slots(self.h))
-        words = C.c_uint64(0)
-        self.L.smr_place_results.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
-        self._check(self.L.smr_place_results(self.h, None, 0, None, C.cast(C.byref(words), C.c_void_p)), "smr_place_results")
-        res, alns = np.zeros(n, RESULT_DTYPE), np.zeros(n * slots, ALN_DTYPE)
-        stats = np.zeros(n * slots, STATS_DTYPE) if with_stats else None
+        "stats" with with_stats; packed, "alns" / "stats" of sum n_align entries, "aln_off" and slots = 0); the counters are those
+        place() / place_packed() returned."""
+        n = self._n_resident
+        n_alns, words = C.c_uint64(0), C.c_uint64(0)
+        fn = self.L.smr_place_results_packed if self.layout == "packed" else self.L.smr_place_results
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+        self._check(fn(self.h, None, 0, C.cast(C.byref(n_alns), C.c_void_p), C.cast(C.byref(words), C.c_void_p)),
+                    "smr_place_results_packed" if self.layout == "packed" else "smr_place_results")
+        slots = 0 if self.layout == "packed" else int(self.L.smr_aln_slots(self.h))
+        res, alns = np.zeros(n, RESULT_DTYPE), np.zeros(int(n_alns.value), ALN_DTYPE)
+        stats = np.zeros(int(n_alns.value), STATS_DTYPE) if with_stats else None
         pool = np.zeros(max(1, words.value), np.uint32)
         self.L.smr_download_placed.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64]
         self._check(self.L.smr_download_placed(self.h, _ptr(res), _ptr(alns), _ptr(stats) if with_stats else None, _ptr(pool), pool.size),
@@ -688,6 +713,9 @@ class Aligner:
         out = dict(res=res, alns=alns, cigar=pool[:words.value], slots=slots)
         if with_stats:
             out["stats"] = stats
+        if self.layout == "packed":
+            out["aln_off"] = np.zeros(n + 1, np.uint64)
+            np.cumsum(res["n_align"], out=out["aln_off"][1:])
         return out
 
     def format_placed_into(self, opts: ReportOpts, buf: np.ndarray, gzip: bool = False, pairwise: bool = False):
@@ -750,7 +778,8 @@ class Aligner:
         "groups": report_groups()}; with out2 or sout, "aligned" / "other" / "denovo" are tuples of the num_out files (2, or 4 with
         both) in the reference's order (_fwd, _rev | _paired, _singleton | _paired_fwd, _paired_rev, _singleton_fwd, _singleton_rev).
         gzip: smr_format_reports_gz, every non-empty stream as one gzip member (empty ones stay b"").
-        out=None: the results place() placed on the device and the resident text (smr_format_reports_placed[_gz]); text must be None."""
+        out=None: the results place() or place_packed() placed on the device and the resident text (smr_format_reports_placed[_gz]);
+        text must be None."""
         o = opts if opts is not None else report_opts(**kw)
         if o.sam or o.blast:
             self._upload_report_refs()
@@ -1004,7 +1033,8 @@ class ReportWriter:
 
     def write(self, out: dict | None = None, text: bytes | None = None) -> dict:
         """format one batch (see Aligner.format_reports) and append its streams; returns them.  out=None: the results the last
-        Aligner.place() placed on the device, with the resident text (their counters are the ones place() returned)."""
+        Aligner.place() or Aligner.place_packed() placed on the device, with the resident text (their counters are the ones it
+        returned)."""
         if out is None and text is not None:
             raise ValueError("ReportWriter.write: the placed results go with the resident text (text=None)")
         if self.ext is None:
@@ -1186,7 +1216,10 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
          memory (Aligner.set_index_budget);
       3. the reads streamed through the device (stream_fastx, or stream_mates for two files) in batches of batch_bytes of text, each
          run, placed on the device (Aligner.place) and formatted from there (the _placed calls), with the OTU map and the denovo
-         statistics added from the placed results too;
+         statistics added from the placed results too.  With params.num_alignments == 0 (all alignments) the batches run in the
+         packed layout and are placed with Aligner.place_packed: device memory follows the alignments stored, and only the reads
+         that store more than the first run's stride run again, where the strided layout would size every read by the largest
+         count of the batch;
       4. otu_map.txt and aligned.log (hostio.summary_log; cmd / threads / sq are what it prints).
     gumbel[k] = (lambda, K) of refs[k]: the library does not compute them (the reference's ALP).  params: an api.Params (default
     default_params()).  Report options as report_opts / ReportWriter take them: sam, sq (-SQ), blast ("1 cigar qcov qstrand", "0"),
@@ -1197,7 +1230,7 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
     read files and the SAM / BLAST rows of the first (index, part) group are appended to their final files as they come.  With
     several groups the rows of the other groups go to part files first and are appended at the end, as the reference's order (every
     row of group 0, then of group 1, ...) requires: those bytes are written twice.
-    Returns {"reads", "batches", "num_aligned", "minimal_score", "paths", "seconds": per stage}: count, index, stream (the whole
+    Returns {"reads", "batches", "num_aligned", "minimal_score", "paths", "layout" ("strided" or "packed"), "seconds": per stage}: count, index, stream (the whole
     streamed pass: from the first batch until every report file is complete and closed, the part files appended), produce (batch
     production: push, inflate, cut, decode), run, place, format (the report calls, the OTU map and the denovo statistics), writer
     (the writer thread's busy time), writer_wait (its idle time), caller_wait (the caller waiting for a free output buffer), parts
@@ -1246,6 +1279,9 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
                 lam, K = gumbel[k]
                 al.set_report_scoring(k, lam, K, *hostio.evalue_params(stats[k], K, counts["length"], counts["reads"]))
         al.set_place_stats(bool(o.sam or o.blast or o.denovo or otu_map is not None))
+        layout = "packed" if params.num_alignments == 0 else "strided"
+        al.set_aln_layout(layout)
+        place = al.place_packed if layout == "packed" else al.place
         if otu_map is not None:
             al.otu_begin(otu_map[0], otu_map[1], paired_in=paired_in, paired_out=paired_out, feed=feed)
         sec["index"] = time.perf_counter() - t0
@@ -1297,7 +1333,7 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
             sec["produce"] += t1 - t0
             al.run_resident()
             t2 = time.perf_counter()
-            info = al.place()
+            info = place()
             t3 = time.perf_counter()
             n_reads += n
             n_batches += 1
@@ -1368,7 +1404,8 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
             f.write(log.encode())
         paths.append(path)
         sec["finish"] = time.perf_counter() - t0
-        return dict(reads=n_reads, batches=n_batches, num_aligned=num_aligned, paths=paths, seconds=sec, minimal_score=[int(x) for x in ms])
+        return dict(reads=n_reads, batches=n_batches, num_aligned=num_aligned, paths=paths, seconds=sec, minimal_score=[int(x) for x in ms],
+                    layout=layout)
     finally:
         if writer is not None:
             try:

@@ -148,24 +148,20 @@ struct smr_ctx {
   uint32_t layout = SMR_ALNS_STRIDED;   // smr_set_aln_layout
   uint64_t retry_slots = 1u << 24;      // packed layout: slot budget of one sub-batch of reads run again for their alignment count
   uint64_t runs_made = 0;               // numbers the runs (Batch::run_id)
-  // The packed results of the resident batch's last run as download_packed places them (place_packed), kept until the batch is run
-  // again or replaced: a download retried for capacity, or repeated, only copies them.
-  struct PackedResult {
-    uint64_t run_id = 0;   // Batch::run_id of the run they come from; 0 = none
-    std::vector<smr_read_result> res; std::vector<smr_aln> alns; std::vector<smr_aln_stats> st; std::vector<uint32_t> cig;
-    std::vector<uint64_t> cnt;   // what the download adds to the caller's counters, SMR_CNT_FIXED + n_index_files entries
-    bool trace_error = false;
-    RunTimes t_run; double t_d2h = 0;
-  } pk;
-  // The results of the resident batch's last run placed on the device in the strided layout (smr_place_results, place_resident),
-  // kept until the batch is run again or replaced; the report-side _placed calls read them there.
+  // The results of the resident batch's last run placed on the device (smr_place_results, place_resident, in the strided layout;
+  // smr_place_results_packed and the packed downloads, place_packed, in the packed one), kept until the batch is run again or
+  // replaced; the report-side _placed calls read them there, and a packed download retried for capacity, or repeated, copies them.
   struct Placed {
     uint64_t run_id = 0;   // Batch::run_id of the run they come from; 0 = none
     uint32_t nreads = 0, slots = 0; bool stats = false;
-    uint64_t cig_words = 0;
+    bool packed = false;   // placed in the packed layout: n_alns alignments, read r's from aln_off[r]; slots = the first run's stride
+    bool trace = false;    // packed: a run met a trace back error (each call that reads the placement fails with SMR_ERR_INDEX)
+    uint64_t cig_words = 0, n_alns = 0;
     DevBuf res, aln, st, cig, cnt, words, off, scal;   // the placed arrays, the counters (ncnt u64), count-pass scratch
-    std::vector<uint64_t> cnt_host;                    // what smr_place_results adds to the caller's counters
-    double t_place = 0;                                // ms of the placement passes (CUDA events), retries excluded
+    DevBuf aoff, nal, src, runs, fsel, fout;           // packed: aln_off, n_align per read, each read's source run, the run table, flagged reads (bits, list)
+    std::vector<uint64_t> cnt_host;                    // what smr_place_results[_packed] adds to the caller's counters
+    double t_place = 0;                                // ms of the placement passes (CUDA events), retries and re-runs excluded
+    RunTimes t_run;                                    // packed: the first run and its re-runs
   } pl;
   bool place_stats = false;   // smr_set_place_stats: every run computes the smr_aln_stats a placement keeps
   uint32_t lis_ctas_per_sm = kLisMinCtas;   // persistent CTAs of the candidate kernel per SM (matches its __launch_bounds__)
@@ -239,9 +235,11 @@ uint32_t slots_of(const smr_ctx* ctx) { return ctx->prm.num_alignments > 0 ? (ui
 
 bool packed(const smr_ctx* ctx) { return ctx->layout == SMR_ALNS_PACKED; }
 
-// the result slots of a batch: strided, nreads * slots_of; packed, its stored alignments (the sum of n_align)
-uint64_t result_slots(const smr_ctx* ctx, const smr_read_result* results, uint32_t nreads) {
+// the result slots of a batch: strided, nreads * slots_of; packed, its stored alignments (the sum of n_align).  dev: results
+// is the placement's device array, whose count the placement keeps.
+uint64_t result_slots(const smr_ctx* ctx, const smr_read_result* results, uint32_t nreads, bool dev = false) {
   if (!packed(ctx)) return (uint64_t)nreads * slots_of(ctx);
+  if (dev) return ctx->pl.n_alns;
   uint64_t n = 0;
   for (uint32_t r = 0; r < nreads; ++r) n += results[r].n_align;
   return n;
@@ -724,7 +722,6 @@ void finish_upload(smr_ctx* ctx, Batch& b, uint64_t w) {
 void clear_resident(smr_ctx* ctx) {
   auto& R = ctx->res;
   R.b.nreads = 0; R.b.from_text = false; R.text_bytes = 0; R.mates = false; R.b.run_id = 0;
-  ctx->pk = smr_ctx::PackedResult{};
 }
 
 // host reads -> the resident batch (no text behind it)
@@ -1695,10 +1692,10 @@ void place_resident(smr_ctx* ctx) {
   const Batch& R = ctx->res.b;
   if (R.run_id == 0) fail(SMR_ERR_ARG, "smr_place_results: the resident batch has not been run (smr_run_resident)");
   if (R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, "smr_place_results: the resident batch was run at another stride: call smr_run_resident again");
-  if (P.run_id == R.run_id) return;
+  if (P.run_id == R.run_id && !P.packed) return;
   P.run_id = 0;
   const uint32_t n = R.nreads, slots = slots_of(ctx), ncnt = place_counters(ctx);
-  P.nreads = n; P.slots = slots; P.stats = R.run_stats; P.cig_words = 0; P.t_place = 0;
+  P.nreads = n; P.slots = slots; P.stats = R.run_stats; P.packed = false; P.trace = false; P.cig_words = 0; P.n_alns = 0; P.t_place = 0;
   ensure(P.res, (size_t)n * sizeof(smr_read_result) + 16);
   ensure(P.aln, (size_t)n * slots * sizeof(smr_aln) + 16);
   if (P.stats) ensure(P.st, (size_t)n * slots * sizeof(smr_aln_stats) + 16);
@@ -1735,69 +1732,86 @@ void place_resident(smr_ctx* ctx) {
 // the placed arrays, as the report-side calls take them
 struct PlacedArrays {
   const smr_read_result* res; const smr_aln* aln; const uint32_t* cig; uint64_t cig_words; const smr_aln_stats* st; uint32_t n;
+  uint64_t nslots;   // the alignment rows: n * stride, or packed the sum of n_align
 };
 
-// The placed results of the resident batch's last run for the _placed call `call`; need_stats: the call reads the stats.
+// The placed results of the resident batch's last run for the _placed call `call`; need_stats: the call reads the stats.  In the
+// packed layout they are the packed placement of that run (smr_place_results_packed, or a packed download).
 PlacedArrays placed_of(const smr_ctx* ctx, const char* call, bool need_stats) {
-  if (packed(ctx))
-    fail(SMR_ERR_UNSUPPORTED, std::string(call) + ": results are placed on the device in the strided layout only; in the packed layout "
-                              "download them (smr_download_results_packed) and pass them to the call that takes result arrays");
   const auto& P = ctx->pl;
-  if (P.run_id == 0 || P.run_id != ctx->res.b.run_id)
+  const bool current = P.run_id != 0 && P.run_id == ctx->res.b.run_id;
+  if (packed(ctx)) {
+    if (!current || !P.packed)
+      fail(SMR_ERR_UNSUPPORTED, std::string(call) + ": no placed results of the resident batch's last run in the packed layout "
+                                "(smr_place_results places the strided layout only): call smr_place_results_packed after smr_run_resident, "
+                                "or download them (smr_download_results_packed) and pass them to the call that takes result arrays");
+    if (P.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
+    return PlacedArrays{(const smr_read_result*)P.res.p, (const smr_aln*)P.aln.p, (const uint32_t*)P.cig.p, P.cig_words,
+                        (const smr_aln_stats*)P.st.p, P.nreads, P.n_alns};
+  }
+  if (!current || P.packed)
     fail(SMR_ERR_ARG, std::string(call) + ": no placed results of the resident batch's last run: call smr_place_results after smr_run_resident");
   if (P.slots != slots_of(ctx)) fail(SMR_ERR_ARG, std::string(call) + ": the results were placed at another stride");
   if (need_stats && !P.stats)
     fail(SMR_ERR_ARG, std::string(call) + ": the placed run computed no smr_aln_stats: call smr_set_place_stats(ctx, 1) before smr_run_resident");
   return PlacedArrays{(const smr_read_result*)P.res.p, (const smr_aln*)P.aln.p, (const uint32_t*)P.cig.p, P.cig_words,
-                      P.stats ? (const smr_aln_stats*)P.st.p : nullptr, P.nreads};
+                      P.stats ? (const smr_aln_stats*)P.st.p : nullptr, P.nreads, (uint64_t)P.nreads * P.slots};
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
 // packed results (SMR_ALNS_PACKED): read r's alignments at sum_{j<r} n_align(j), every read at its own count
 // ---------------------------------------------------------------------------------------------------------------------
-// One run's results on the host.  A packed download places nothing before every read's final count is known, so it keeps the
-// results of the first run and of each re-run until then.
-struct RunHost {
-  std::vector<ReadState> st; std::vector<uint32_t> fl; std::vector<uint16_t> hdb;
-  std::vector<OutAln> oa; std::vector<AlnStats> ast; std::vector<uint32_t> cig;
-  std::vector<uint64_t> base;                  // read r's first slot in oa / ast
-  std::vector<unsigned long long> cnt;         // the device counters
-};
+// The result buffers of a re-run sub-batch, kept on the device until the scatter; the rest of its batch (reads, seed scratch,
+// candidate work) frees itself when its re-runs are done, and the context's arenas are released after the last one.
+struct KeptRun { DevBuf state, hit_db, out_aln, aln_stats, cigar_pool, counters, aln_base; };
 
-RunHost fetch_run(smr_ctx* ctx, const Batch& b) {
-  const uint32_t n = b.nreads;
-  RunHost h;
-  h.base.resize((size_t)n + 1);
-  for (uint32_t r = 0; r <= n; ++r) h.base[r] = b.base.empty() ? (uint64_t)r * b.run_slots : b.base[r];
-  const uint64_t ns = h.base[n];
-  h.st.resize(n); h.fl.resize(n); h.hdb.resize(n); h.oa.resize(ns); h.ast.resize(ns); h.cnt.resize(dcCount + 64);
-  unsigned long long used = 0;
-  CK(cudaMemcpyAsync(h.st.data(), b.state.p, (size_t)n * sizeof(ReadState), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(h.fl.data(), b.flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(h.hdb.data(), b.hit_db.p, (size_t)n * 2, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(h.oa.data(), b.out_aln.p, (size_t)ns * sizeof(OutAln), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(h.ast.data(), b.aln_stats.p, (size_t)ns * sizeof(AlnStats), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(&used, scalars_of(b).cigar_used, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(h.cnt.data(), b.counters.p, h.cnt.size() * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  h.cig.resize(std::min<unsigned long long>(used, b.cigar_cap_dev));
-  if (!h.cig.empty()) CK(cudaMemcpyAsync(h.cig.data(), b.cigar_pool.p, h.cig.size() * 4, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  return h;
-}
-
-// Where every read of the resident batch has its final results: src[r] = (run, read in that run's batch).
+// The runs of a packed placement: runs[0] is the resident batch's first run, runs[k] the re-run whose buffers are kept[k - 1].
+// ctx->pl.src names, per read of the resident batch, the run and the read in it that hold its final results.
 struct PackedRuns {
-  std::deque<RunHost> runs;
-  std::vector<std::pair<uint32_t, uint32_t>> src;
+  std::deque<KeptRun> kept;
+  std::vector<PackRun> runs;
   bool trace_error = false;
   uint64_t slot_reads = 0, slot_batches = 0; uint32_t slot_max = 0;   // re-runs for the alignment count (SMR_VERBOSE)
 };
 
+// a run as the placement reads it (its buffers stay where the run left them)
+PackRun pack_run_of(const Batch& b) {
+  return PackRun{(const ReadState*)b.state.p, (const uint16_t*)b.hit_db.p, (const OutAln*)b.out_aln.p, (const AlnStats*)b.aln_stats.p,
+                 (const uint32_t*)b.cigar_pool.p, b.base.empty() ? nullptr : (const uint32_t*)b.aln_base.p,
+                 (const unsigned long long*)b.counters.p, b.run_slots, 0};
+}
+
+// the reads of a run that carry a flag, in read order: a compaction of its flags on the device (a scan of one bit per read), of
+// which only the read index, the flags and n_align come to the host
+std::vector<PackFlag> flagged_reads(smr_ctx* ctx, const Batch& b) {
+  auto& P = ctx->pl;
+  const uint32_t n = b.nreads;
+  const uint32_t* flags = (const uint32_t*)b.flags.p;
+  uint32_t* bit = ensure<uint32_t>(P.fsel, ((size_t)n + 1) * 4);
+  uint32_t* pos = ensure<uint32_t>(P.scal, ((size_t)n + 1) * 4);
+  PackFlag* out = ensure<PackFlag>(P.fout, (size_t)n * sizeof(PackFlag) + 16);
+  const uint32_t grid = std::min<uint32_t>((n + 256) / 256, (uint32_t)ctx->sm_count * 8);
+  pack_flag_bits_kernel<<<grid, 256, 0, ctx->stream>>>(flags, n, bit);
+  CK(cudaGetLastError());
+  exclusive_sum(ctx, bit, pos, n + 1);
+  pack_flagged_kernel<<<grid, 256, 0, ctx->stream>>>(flags, (const ReadState*)b.state.p, n, pos, out);
+  CK(cudaGetLastError());
+  uint32_t m = 0;
+  CK(cudaMemcpyAsync(&m, pos + n, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  std::vector<PackFlag> h(m);
+  if (m) {
+    CK(cudaMemcpyAsync(h.data(), out, (size_t)m * sizeof(PackFlag), cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  return h;
+}
+
 // Reads idx[k] of batch `from` (map[k]: their index in the resident batch) run again as batches of their own at `scale`, read k
 // with room for cap[k] alignments, in sub-batches of at most ctx->retry_slots slots (a larger read alone).  Reads that store more
 // than their room run once more at their exact count; reads that overflow their scratch go on at 8x the scale, with room for
-// max(stride, the count they reached), for 3 scales at most.  Each sub-batch frees itself when its re-runs are done.
+// max(stride, the count they reached), for 3 scales at most.  Each sub-batch's unflagged reads become the source of their reads
+// (ctx->pl.src), and its result buffers are kept for the scatter; the rest of it frees itself when its re-runs are done.
 void rerun_packed(smr_ctx* ctx, const Batch& from, const std::vector<uint32_t>& idx, const std::vector<uint32_t>& cap,
                   const std::vector<uint32_t>& map, uint32_t scale, int depth, bool for_slots, PackedRuns& P) {
   if (idx.empty()) return;
@@ -1827,16 +1841,23 @@ void rerun_packed(smr_ctx* ctx, const Batch& from, const std::vector<uint32_t>& 
     finish_upload(ctx, b, w);
     run_impl(ctx, b);
     ctx->t_run += b.run;
-    P.runs.push_back(fetch_run(ctx, b));
-    const uint32_t id = (uint32_t)P.runs.size() - 1;
-    const RunHost& h = P.runs.back();
+    const uint32_t id = (uint32_t)P.runs.size();
+    DevBuf d_map;
+    upload_async(ctx, d_map, map.data() + a, n);
+    pack_src_kernel<<<std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
+        (const uint32_t*)b.flags.p, (const uint32_t*)d_map.p, n, id, (uint2*)ctx->pl.src.p);
+    CK(cudaGetLastError());
+    const std::vector<PackFlag> fl = flagged_reads(ctx, b);   // synchronises: d_map may free
+    P.runs.push_back(pack_run_of(b));
+    KeptRun& K = P.kept.emplace_back();
+    K.state = std::move(b.state); K.hit_db = std::move(b.hit_db); K.out_aln = std::move(b.out_aln); K.aln_stats = std::move(b.aln_stats);
+    K.cigar_pool = std::move(b.cigar_pool); K.counters = std::move(b.counters); K.aln_base = std::move(b.aln_base);
     std::vector<uint32_t> s_idx, s_cap, s_map, x_idx, x_cap, x_map;
-    for (uint32_t k = 0; k < n; ++k) {
-      const uint32_t f = h.fl[k], m = map[a + k];
-      if (f & kErrTrace) P.trace_error = true;
-      if (!f) P.src[m] = {id, k};
-      else if (f == kOvfSlots) { s_idx.push_back(k); s_cap.push_back(h.st[k].n_align); s_map.push_back(m); }
-      else { x_idx.push_back(k); x_cap.push_back(std::max(S, h.st[k].n_align)); x_map.push_back(m); }
+    for (const PackFlag& f : fl) {
+      const uint32_t k = f.read, m = map[a + k];
+      if (f.flags & kErrTrace) P.trace_error = true;
+      if (f.flags == kOvfSlots) { s_idx.push_back(k); s_cap.push_back(f.n_align); s_map.push_back(m); }
+      else { x_idx.push_back(k); x_cap.push_back(std::max(S, f.n_align)); x_map.push_back(m); }
     }
     rerun_packed(ctx, b, s_idx, s_cap, s_map, scale, depth, true, P);          // the count is exact now
     rerun_packed(ctx, b, x_idx, x_cap, x_map, scale * 8, depth + 1, false, P);
@@ -1844,82 +1865,83 @@ void rerun_packed(smr_ctx* ctx, const Batch& from, const std::vector<uint32_t>& 
   }
 }
 
-// The packed results of the resident batch's last run, placed in ctx->pk: the first run's results, every read that stored more
-// alignments than the stride run again at its own count and every read that overflowed its scratch run again at a larger one, then
-// all of them placed in read order.  The resident batch and its device results stay as they are.
+// The packed results of the resident batch's last run, placed on the device in ctx->pl: the first run's results, every read that
+// stored more alignments than the stride run again at its own count and every read that overflowed its scratch run again at a
+// larger one, then all of them placed in read order (smr_place.cuh: a count pass over each read's source run, two scans, a warp
+// per read to scatter).  The resident batch and its device results stay as they are.
 void place_packed(smr_ctx* ctx) {
+  auto& P = ctx->pl;
   const Batch& R = ctx->res.b;
-  const uint32_t n = R.nreads, S = slots_of(ctx);
-  smr_ctx::PackedResult& K = ctx->pk;
-  K = smr_ctx::PackedResult{};   // frees what an earlier run left
-  K.cnt.assign(SMR_CNT_FIXED + std::max(1u, ctx->n_index_files), 0);
-  ctx->t_run = R.run;
-  cudaEvent_t* e = events(ctx, 2);
-  CK(cudaEventRecord(e[0], ctx->stream));
-  PackedRuns P;
-  P.runs.push_back(fetch_run(ctx, R));
-  CK(cudaEventRecord(e[1], ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  ctx->t_d2h = elapsed_ms(e[0], e[1]);
-  P.src.resize(n);
+  const uint32_t n = R.nreads, S = slots_of(ctx), ncnt = place_counters(ctx);
+  P.run_id = 0;
+  P.nreads = n; P.slots = S; P.stats = true; P.packed = true; P.trace = false; P.cig_words = 0; P.n_alns = 0; P.t_place = 0;
+  P.cnt_host.assign(ncnt, 0);
+  ctx->t_run = R.run; ctx->t_d2h = 0;
+  if (n == 0) { P.t_run = ctx->t_run; P.run_id = R.run_id; return; }
+  const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sm_count * 8);
+  uint2* src = ensure<uint2>(P.src, (size_t)n * sizeof(uint2) + 16);
+  pack_src_init_kernel<<<grid, 256, 0, ctx->stream>>>(src, n);
+  CK(cudaGetLastError());
+  PackedRuns K;
+  K.runs.push_back(pack_run_of(R));
   std::vector<uint32_t> s_idx, s_cap, x_idx, x_cap;
-  {
-    const RunHost& h = P.runs[0];
-    for (uint32_t r = 0; r < n; ++r) {
-      const uint32_t f = h.fl[r];
-      P.src[r] = {0, r};
-      if (f & kErrTrace) P.trace_error = true;
-      if (f == kOvfSlots) { s_idx.push_back(r); s_cap.push_back(h.st[r].n_align); }
-      else if (f) { x_idx.push_back(r); x_cap.push_back(std::max(S, h.st[r].n_align)); for (int bit = 0; bit < 6; ++bit) if (f & (1u << bit)) ctx->flag_hist[bit]++; }
-    }
+  for (const PackFlag& f : flagged_reads(ctx, R)) {
+    if (f.flags & kErrTrace) K.trace_error = true;
+    if (f.flags == kOvfSlots) { s_idx.push_back(f.read); s_cap.push_back(f.n_align); }
+    else { x_idx.push_back(f.read); x_cap.push_back(std::max(S, f.n_align)); for (int bit = 0; bit < 6; ++bit) if (f.flags & (1u << bit)) ctx->flag_hist[bit]++; }
   }
   if (!s_idx.empty() || !x_idx.empty()) {
-    // the arenas grow with a retry's scale: the next run allocates them again at its own
-    const auto release = on_exit([ctx] { for (DevBuf* s : {&ctx->run.lis, &ctx->run.fin, &ctx->run.tb, &ctx->run.lane_hits}) s->reset(); });
-    rerun_packed(ctx, R, s_idx, s_cap, s_idx, R.scale, 0, true, P);
-    rerun_packed(ctx, R, x_idx, x_cap, x_idx, R.scale * 8, 1, false, P);
+    const auto release = on_exit([ctx] { release_retry_arenas(ctx); });
+    rerun_packed(ctx, R, s_idx, s_cap, s_idx, R.scale, 0, true, K);
+    rerun_packed(ctx, R, x_idx, x_cap, x_idx, R.scale * 8, 1, false, K);
   }
-  if (P.slot_reads && getenv("SMR_VERBOSE"))
+  if (K.slot_reads && getenv("SMR_VERBOSE"))
     fprintf(stderr, "[smr] packed results: %llu reads stored more than %u alignments and were run again at their own count in %llu sub-batches (largest count %u)\n",
-            (unsigned long long)P.slot_reads, S, (unsigned long long)P.slot_batches, P.slot_max);
-  uint64_t nal = 0, words = 0;
-  for (uint32_t r = 0; r < n; ++r) {
-    const RunHost& h = P.runs[P.src[r].first];
-    const uint32_t k = P.src[r].second;
-    nal += h.st[k].n_align;
-    for (uint32_t j = 0; j < h.st[k].n_align; ++j) words += h.oa[h.base[k] + j].cigar_len;
-  }
-  if (words >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, "CIGAR pool offset passes 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches");
-  K.res.resize(n); K.alns.assign(nal, smr_aln{}); K.st.resize(nal); K.cig.resize(words);
-  uint64_t at = 0, cw = 0;
-  for (uint32_t r = 0; r < n; ++r) {
-    const RunHost& h = P.runs[P.src[r].first];
-    const uint32_t k = P.src[r].second;
-    const ReadState& s = h.st[k];
-    smr_read_result& o = K.res[r];
-    o.lastIndex = s.lastIndex; o.lastPart = s.lastPart; o.hit_seeds = s.hit_seeds; o.min_index = s.min_index; o.max_index = s.max_index;
-    o.n_align = s.n_align; o.max_SW_count = s.max_SW_count; o.is_done = s.is_done; o.is_hit = s.is_hit;
-    for (uint32_t j = 0; j < s.n_align; ++j, ++at) {
-      const OutAln& d = h.oa[h.base[k] + j];
-      smr_aln& a = K.alns[at];
-      memcpy(K.cig.data() + cw, h.cig.data() + d.cigar_off, (size_t)d.cigar_len * 4);
-      a.cigar_off = (uint32_t)cw; a.cigar_len = d.cigar_len; cw += d.cigar_len;
-      a.ref_num = d.ref_num; a.ref_begin1 = d.ref_begin1; a.ref_end1 = d.ref_end1; a.read_begin1 = d.read_begin1; a.read_end1 = d.read_end1;
-      a.readlen = d.readlen; a.score1 = d.score1; a.part = d.part; a.index_num = d.index_num; a.strand = d.strand;
-      const AlnStats& t = h.ast[h.base[k] + j];
-      K.st[at] = smr_aln_stats{t.n_miss, t.n_gap, t.n_match, t.n_match_denovo};
-    }
-    if (s.is_hit) {   // Readstats: once per read, from the run that stored it
-      K.cnt[SMR_CNT_NUM_ALIGNED]++;
-      if (h.hdb[k] != 0xFFFF && SMR_CNT_FIXED + h.hdb[k] < K.cnt.size()) K.cnt[SMR_CNT_FIXED + h.hdb[k]]++;
-    }
-  }
-  // the work counters count every run (pinned to SMR_CNT_* by the static_asserts at HostOut)
-  for (const RunHost& h : P.runs)
-    for (uint32_t k = dcNumShort; k < dcCount; ++k) K.cnt[k] += h.cnt[k];
-  K.trace_error = P.trace_error;
-  K.t_run = ctx->t_run; K.t_d2h = ctx->t_d2h;
-  K.run_id = R.run_id;
+            (unsigned long long)K.slot_reads, S, (unsigned long long)K.slot_batches, K.slot_max);
+  // count, scan, scatter
+  const uint32_t nruns = (uint32_t)K.runs.size();
+  upload_async(ctx, P.runs, K.runs.data(), nruns);
+  uint64_t* nal = ensure<uint64_t>(P.nal, ((size_t)n + 1) * 8);
+  uint64_t* words = ensure<uint64_t>(P.words, ((size_t)n + 1) * 8);
+  uint64_t* aoff = ensure<uint64_t>(P.aoff, ((size_t)n + 1) * 8);
+  uint64_t* off = ensure<uint64_t>(P.off, ((size_t)n + 1) * 8);
+  ensure(P.cnt, (size_t)ncnt * 8);
+  cudaEvent_t* e = events(ctx, 2);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  CK(cudaMemsetAsync(P.cnt.p, 0, (size_t)ncnt * 8, ctx->stream));
+  pack_count_kernel<<<grid, 256, (size_t)ncnt * 8, ctx->stream>>>((const PackRun*)P.runs.p, nruns, src, n, nal, words, (unsigned long long*)P.cnt.p, ncnt);
+  CK(cudaGetLastError());
+  cub_run(ctx->cub_tmp, [&](void* t, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, nal, aoff, (int)(n + 1), ctx->stream); });
+  cub_run(ctx->cub_tmp, [&](void* t, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, words, off, (int)(n + 1), ctx->stream); });
+  uint64_t tot[2] = {0, 0};
+  CK(cudaMemcpyAsync(&tot[0], aoff + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&tot[1], off + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (tot[1] >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, kCigarOffsetMsg);
+  ensure(P.res, (size_t)n * sizeof(smr_read_result) + 16);
+  ensure(P.aln, tot[0] * sizeof(smr_aln) + 16);
+  ensure(P.st, tot[0] * sizeof(smr_aln_stats) + 16);
+  ensure(P.cig, tot[1] * 4 + 16);
+  const PackOut o{(smr_read_result*)P.res.p, (smr_aln*)P.aln.p, (smr_aln_stats*)P.st.p, (uint32_t*)P.cig.p, aoff, off};
+  pack_scatter_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 16), 256, 0, ctx->stream>>>((const PackRun*)P.runs.p, src, n, o);
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e[1], ctx->stream));
+  CK(cudaMemcpyAsync(P.cnt_host.data(), P.cnt.p, (size_t)ncnt * 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));   // before the kept runs free themselves
+  P.t_place = elapsed_ms(e[0], e[1]);
+  P.n_alns = tot[0]; P.cig_words = tot[1]; P.trace = K.trace_error; P.t_run = ctx->t_run;
+  P.run_id = R.run_id;
+}
+
+// The packed placement of the resident batch's last run (once per run: a later call finds it placed).  `call` names the entry
+// point in its refusals.
+void place_packed_resident(smr_ctx* ctx, const char* call) {
+  const Batch& R = ctx->res.b;
+  if (R.run_id == 0) fail(SMR_ERR_ARG, std::string(call) + ": the resident batch has not been run (smr_run_resident)");
+  if (!R.run_stats || R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, "the resident batch was not run in the packed layout at this stride: call smr_run_resident again");
+  const auto& P = ctx->pl;
+  if (P.packed && P.run_id == R.run_id) { ctx->t_run = P.t_run; return; }
+  place_packed(ctx);
 }
 
 struct PackedOut {
@@ -1928,28 +1950,32 @@ struct PackedOut {
   uint64_t aln_used = 0, cigar_used = 0;
 };
 
-// The packed download of the resident batch's last run: placed once per run (place_packed), then copied.  Both sizes are set before
-// a capacity check can fail, and a call with arrays that large writes the same bytes.
+// The packed download of the resident batch's last run: placed on the device once per run (place_packed), then copied.  Both sizes
+// are set before a capacity check can fail, and a call with arrays that large writes the same bytes.
 void download_packed(smr_ctx* ctx, PackedOut& out) {
   const Batch& R = ctx->res.b;
   ctx->t_run = R.run;
   if (R.nreads == 0) return;
   if (!R.run_stats || R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, "the resident batch was not run in the packed layout at this stride: call smr_run_resident again");
-  if (ctx->pk.run_id != R.run_id) place_packed(ctx);
-  const smr_ctx::PackedResult& K = ctx->pk;
-  ctx->t_run = K.t_run; ctx->t_d2h = K.t_d2h;
-  out.aln_used = K.alns.size(); out.cigar_used = K.cig.size();
+  place_packed_resident(ctx, "smr_download_results_packed");
+  const auto& P = ctx->pl;
+  out.aln_used = P.n_alns; out.cigar_used = P.cig_words;
   if (out.aln_used > out.aln_cap)
     fail(SMR_ERR_CAPACITY, "alignment array too small: the batch stores " + std::to_string(out.aln_used) + " alignments, aln_cap is " + std::to_string(out.aln_cap));
   if (out.cigar_used > out.cigar_cap)
     fail(SMR_ERR_CAPACITY, "cigar pool too small: the batch needs " + std::to_string(out.cigar_used) + " words, cigar_cap is " + std::to_string(out.cigar_cap));
-  memcpy(out.results, K.res.data(), K.res.size() * sizeof(smr_read_result));
-  if (!K.alns.empty()) memcpy(out.alns, K.alns.data(), K.alns.size() * sizeof(smr_aln));
-  if (out.stats && !K.st.empty()) memcpy(out.stats, K.st.data(), K.st.size() * sizeof(smr_aln_stats));
-  if (!K.cig.empty()) memcpy(out.cigar_pool, K.cig.data(), K.cig.size() * 4);
+  cudaEvent_t* e = events(ctx, 2);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  CK(cudaMemcpyAsync(out.results, P.res.p, (size_t)P.nreads * sizeof(smr_read_result), cudaMemcpyDeviceToHost, ctx->stream));
+  if (P.n_alns) CK(cudaMemcpyAsync(out.alns, P.aln.p, P.n_alns * sizeof(smr_aln), cudaMemcpyDeviceToHost, ctx->stream));
+  if (out.stats && P.n_alns) CK(cudaMemcpyAsync(out.stats, P.st.p, P.n_alns * sizeof(smr_aln_stats), cudaMemcpyDeviceToHost, ctx->stream));
+  if (P.cig_words) CK(cudaMemcpyAsync(out.cigar_pool, P.cig.p, P.cig_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e[1], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  ctx->t_d2h = elapsed_ms(e[0], e[1]);
   if (out.counters)
-    for (uint32_t k = 0; k < out.n_counters && k < K.cnt.size(); ++k) out.counters[k] += K.cnt[k];
-  if (K.trace_error) fail(SMR_ERR_INDEX, "trace back error (ssw.c:707 is fatal in the reference too)");
+    for (uint32_t k = 0; k < out.n_counters && k < P.cnt_host.size(); ++k) out.counters[k] += P.cnt_host[k];
+  if (P.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -1968,11 +1994,11 @@ void rpt_check(uint32_t e) {
 // A report-side call's checks of its batch: the arrays (stats_msg: stats are read, the text if missing; arrays_msg: the text of
 // missing results or alns, stats_msg if null), an even read count when paired (mates 2k, 2k+1), fewer than 2^31 result slots.
 void rpt_check_batch(const smr_ctx* ctx, const char* what, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
-                     uint32_t nreads, bool paired, const char* stats_msg, const char* arrays_msg = nullptr) {
+                     uint32_t nreads, bool paired, const char* stats_msg, const char* arrays_msg = nullptr, bool dev = false) {
   if (nreads && stats_msg && !stats) fail(SMR_ERR_ARG, stats_msg);
   if (nreads && (!results || !alns)) fail(SMR_ERR_ARG, arrays_msg ? arrays_msg : stats_msg);
   if (paired && (nreads & 1u)) fail(SMR_ERR_ARG, "a paired batch holds mates 2k and 2k+1: the number of reads must be even");
-  if (result_slots(ctx, results, nreads) >= (1ull << 31)) fail(SMR_ERR_ARG, std::string("batch too large for ") + what + ": split it");
+  if (result_slots(ctx, results, nreads, dev) >= (1ull << 31)) fail(SMR_ERR_ARG, std::string("batch too large for ") + what + ": split it");
 }
 
 // the loaded (index, part)s in the reference's report order (index, then part)
@@ -2009,7 +2035,7 @@ RptArgs rpt_prologue(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr_
   auto& S = ctx->r;
   CK(cudaEventRecord(e[0], ctx->stream));
   const uint32_t slots = slots_of(ctx), G = (uint32_t)hg.size();
-  const uint64_t N = result_slots(ctx, results, nreads);
+  const uint64_t N = result_slots(ctx, results, nreads, dev);
   // the text
   const uint8_t* dt;
   if (text) {
@@ -2166,7 +2192,7 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   const uint32_t nfx = pairwise ? 0 : 3 * num_out;                                                // aligned, other, denovo: num_out files each
   // a null results or alns array: no text of its own, the last one stays
   rpt_check_batch(ctx, "the report writer", results, alns, stats, nreads, paired,
-                  o->sam || (o->blast && !pairwise) || o->denovo ? "SAM, BLAST and denovo need the smr_aln_stats of the batch" : nullptr, ctx->err.c_str());
+                  o->sam || (o->blast && !pairwise) || o->denovo ? "SAM, BLAST and denovo need the smr_aln_stats of the batch" : nullptr, ctx->err.c_str(), dev);
   uint32_t ncols = 0, cols[4] = {0, 0, 0, 0};
   if (o->blast)
     for (; ncols < 4 && o->blast_cols[ncols]; ++ncols) {
@@ -2316,7 +2342,7 @@ uint64_t otu_add_impl(smr_ctx* ctx, const char* text, uint64_t nbytes, const smr
   if (!text && ctx->res.mates && U.feed != SMR_OTU_TWO_FILES)
     fail(SMR_ERR_UNSUPPORTED, "a mate stream's batch is two mate files: open the OTU map with feed SMR_OTU_TWO_FILES");
   rpt_check_batch(ctx, "the OTU map", results, alns, stats, nreads, U.feed != SMR_OTU_SINGLE,
-                  "the OTU map needs the results, alignments and smr_aln_stats of the batch");
+                  "the OTU map needs the results, alignments and smr_aln_stats of the batch", nullptr, dev);
   cudaEvent_t* e = events(ctx, 3);
   const RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, nullptr, 0, stats, nreads, U.groups, e, dev);
   const uint64_t N = a.nslots;
@@ -2401,7 +2427,7 @@ void otu_finish_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t counts[3]) 
 void denovo_stats_impl(smr_ctx* ctx, const smr_denovo_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
                        const smr_aln* alns, const smr_aln_stats* stats, uint32_t nreads, uint32_t* per_read, uint64_t totals[4], bool dev = false) {
   rpt_check_batch(ctx, "the denovo statistics", results, alns, stats, nreads, false,
-                  "the denovo statistics need the results, alignments and smr_aln_stats of the batch");
+                  "the denovo statistics need the results, alignments and smr_aln_stats of the batch", nullptr, dev);
   const bool paired = o->paired || (!text && ctx->res.mates);   // the resident batch of a mate stream is mates
   cudaEvent_t* e = events(ctx, 4);
   // the loaded (index, part)s: an alignment of any other is refused
@@ -2805,7 +2831,6 @@ int smr_resident_layout(smr_ctx* ctx, uint64_t* header_text_off, uint64_t* read_
 int smr_run_resident(smr_ctx* ctx) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
-  ctx->pk = smr_ctx::PackedResult{};   // the packed results of the batch's previous run
   run_impl(ctx, ctx->res.b);
   ctx->t_run = ctx->res.b.run;
   return SMR_OK;
@@ -3126,18 +3151,37 @@ int smr_place_results(smr_ctx* ctx, uint64_t* counters, uint32_t n_counters, uin
   return SMR_OK;
 } SMR_CATCH(ctx)
 
+int smr_place_results_packed(smr_ctx* ctx, uint64_t* counters, uint32_t n_counters, uint64_t* n_alns, uint64_t* cigar_words) try {
+  if (!ctx) return SMR_ERR_ARG;
+  if (n_alns) *n_alns = 0;
+  if (cigar_words) *cigar_words = 0;
+  if (!packed(ctx)) {
+    ctx->err = "smr_place_results_packed places the packed layout only: in the strided layout call smr_place_results";
+    return SMR_ERR_ARG;
+  }
+  CK(cudaSetDevice(ctx->device));
+  place_packed_resident(ctx, "smr_place_results_packed");
+  const auto& P = ctx->pl;
+  if (n_alns) *n_alns = P.n_alns;
+  if (cigar_words) *cigar_words = P.cig_words;
+  if (counters)
+    for (uint32_t k = 0; k < n_counters && k < P.cnt_host.size(); ++k) counters[k] += P.cnt_host[k];
+  if (P.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
 int smr_download_placed(smr_ctx* ctx, smr_read_result* results, smr_aln* alns, smr_aln_stats* stats, uint32_t* cigar_pool, uint64_t cigar_cap) try {
   if (!ctx) return SMR_ERR_ARG;
   CK(cudaSetDevice(ctx->device));
   const PlacedArrays p = placed_of(ctx, "smr_download_placed", stats != nullptr);
-  const uint64_t N = (uint64_t)p.n * ctx->pl.slots;
+  const uint64_t N = p.nslots;
   if (p.n && (!results || !alns)) fail(SMR_ERR_ARG, "smr_download_placed: null result array");
   if (p.cig_words > cigar_cap || (p.cig_words && !cigar_pool))
     fail(SMR_ERR_CAPACITY, "cigar pool too small: the batch needs " + std::to_string(p.cig_words) + " words, cigar_cap is " + std::to_string(cigar_cap));
   if (p.n) {
     CK(cudaMemcpyAsync(results, p.res, (size_t)p.n * sizeof(smr_read_result), cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaMemcpyAsync(alns, p.aln, N * sizeof(smr_aln), cudaMemcpyDeviceToHost, ctx->stream));
-    if (stats) CK(cudaMemcpyAsync(stats, p.st, N * sizeof(smr_aln_stats), cudaMemcpyDeviceToHost, ctx->stream));
+    if (N) CK(cudaMemcpyAsync(alns, p.aln, N * sizeof(smr_aln), cudaMemcpyDeviceToHost, ctx->stream));
+    if (stats && N) CK(cudaMemcpyAsync(stats, p.st, N * sizeof(smr_aln_stats), cudaMemcpyDeviceToHost, ctx->stream));
   }
   if (p.cig_words) CK(cudaMemcpyAsync(cigar_pool, p.cig, p.cig_words * 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));

@@ -7,8 +7,9 @@ store more run again at their own count; N when N > 0) and the strided layout at
 stride the library names).  Per leg: the kernel time (CUDA events inside the C ABI, re-runs included) and the end-to-end rate (upload,
 run, download, host clock), the bytes of the result arrays on the device (computed from the struct sizes, see DEV_SLOT_BYTES; for
 packed, the first run's plus the largest re-run sub-batch's, which are allocated at the same time) and on
-the host (the arrays the call returns; the library keeps a packed copy of the same size for repeated downloads), the host staging of
-the download (computed, HOST_STAGE_SLOT_BYTES), the n_align distribution, and the reads run again and their sub-batches (from the
+the host (the arrays the call returns; the library keeps the packed placement, of the same size, on the device for repeated
+downloads), the host staging of the download (computed, HOST_STAGE_SLOT_BYTES; the packed download no longer stages since its
+placement moved to the device), the n_align distribution, and the reads run again and their sub-batches (from the
 library's SMR_VERBOSE line, in one untimed extra run).  Every leg also checks that both layouts return the same alignments.
 Prints one JSON line with the card name and power limit.
 Run on the GPU:  python tools/bench_all_alignments.py --reads 200000 --steps 3"""
