@@ -515,6 +515,24 @@ int smr_format_reports_placed(smr_ctx*, const smr_report_opts* opts, char* out, 
 int smr_format_reports_placed_gz(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
 int smr_format_blast_pairwise_placed(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
 int smr_format_blast_pairwise_placed_gz(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
+/* aligned.bam (SAMv1 4; not a reference output): the SAM rows of smr_format_reports_placed as BAM records, in the same order,
+ * compressed on the device into BGZF blocks -- gzip members with the BC subfield, each of at most 65,280 input bytes and compressed
+ * with no history before it.  One stream per loaded (index, part) group in (index, part) order, cut into blocks of exactly 65,280
+ * bytes and the rest; stream_off has groups + 1 entries.  A record: refID = the references of the groups before plus ref_num (the
+ * dictionary of smr_bam_header), pos = SAM POS - 1, mapq 255, flag 0 or 16, next_refID -1, next_pos -1, tlen 0, the bin of the
+ * reference span, the CIGAR with its soft clips, SEQ as SAM prints it in 4-bit codes, QUAL as SAM prints it - 33 (0xFF for FASTA),
+ * and AS and NM in the smallest of the types C, S, I.  opts must hold sam = 1 and blast, fastx, other and denovo off (SMR_ERR_ARG
+ * otherwise); of the rest only paired_in, paired_out and mates count, through the skip of empty reads.  SMR_ERR_ARG, naming the read,
+ * for a QNAME longer than 254 bytes, or a FASTQ quality line whose length differs from its sequence's or with a byte outside
+ * '!'..'~'.  Placement and stats as for the other _placed calls; stream_off, SMR_ERR_CAPACITY and the retry as for
+ * smr_format_reports_gz.  The file is smr_bam_header's blocks, each batch's streams, then the 28-byte BGZF EOF block.  Timings
+ * through smr_last_report_timings. */
+int smr_format_bam_placed(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off);
+/* The BAM header of the loaded indexes as BGZF blocks (as smr_format_bam_placed cuts them): magic "BAM\1", l_text and `text` (the
+ * SAM header, nbytes bytes, no NUL), n_ref and (l_name, name NUL, l_ref) of every reference of every loaded part in (index, part,
+ * ref_num) order, the refIDs of smr_format_bam_placed.  Names from smr_set_report_refs (SMR_ERR_ARG for a part without them),
+ * lengths from the resident reference offsets.  *out_bytes = the size; if out is null or cap is smaller, SMR_ERR_CAPACITY. */
+int smr_bam_header(smr_ctx*, const char* text, uint64_t nbytes, char* out, uint64_t cap, uint64_t* out_bytes);
 int smr_otu_add_placed(smr_ctx*, uint64_t* n_added);
 int smr_denovo_stats_placed(smr_ctx*, const smr_denovo_opts* opts, uint32_t* per_read, uint64_t totals[4]);
 

@@ -35,7 +35,10 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_set_index_budget", "smr_index_residency", "smr_set_place_stats", "smr_place_results", "smr_download_placed",
            "smr_last_place_timing", "smr_format_reports_placed", "smr_format_reports_placed_gz", "smr_format_blast_pairwise_placed",
            "smr_format_blast_pairwise_placed_gz", "smr_otu_add_placed", "smr_denovo_stats_placed",
-           "smr_place_results_packed"]
+           "smr_place_results_packed", "smr_format_bam_placed", "smr_bam_header"]
+
+# the BGZF end-of-file marker (SAMv1 4.1.2): an empty BGZF block, written once at the end of a BAM file
+BGZF_EOF = bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000000")
 
 # smr_set_aln_layout: strided, nreads * slots alignments; packed, read r's n_align alignments from the sum of the counts before it
 ALN_LAYOUTS = {"strided": 0, "packed": 1}
@@ -718,14 +721,16 @@ class Aligner:
             np.cumsum(res["n_align"], out=out["aln_off"][1:])
         return out
 
-    def format_placed_into(self, opts: ReportOpts, buf: np.ndarray, gzip: bool = False, pairwise: bool = False):
-        """smr_format_reports_placed[_gz] (pairwise: smr_format_blast_pairwise_placed[_gz]) into `buf` (a uint8 array, grown when the
+    def format_placed_into(self, opts: ReportOpts, buf: np.ndarray, gzip: bool = False, pairwise: bool = False, bam: bool = False):
+        """smr_format_reports_placed[_gz] (pairwise: smr_format_blast_pairwise_placed[_gz]; bam: smr_format_bam_placed, one BGZF
+        stream of BAM records per report_groups() entry, opts = report_opts(sam=True, ...)) into `buf` (a uint8 array, grown when the
         streams do not fit): returns (buf, stream offsets).  The streams stay in buf, for a caller that writes them out as they are."""
         if opts.sam or opts.blast:
             self._upload_report_refs()
         G = len(self.report_groups())
-        so = np.zeros(G + 1 if pairwise else 2 * G + 3 * num_out_of(opts) + 1, np.uint64)
-        name = ("smr_format_blast_pairwise_placed" if pairwise else "smr_format_reports_placed") + ("_gz" if gzip else "")
+        so = np.zeros(G + 1 if pairwise or bam else 2 * G + 3 * num_out_of(opts) + 1, np.uint64)
+        name = "smr_format_bam_placed" if bam else \
+            ("smr_format_blast_pairwise_placed" if pairwise else "smr_format_reports_placed") + ("_gz" if gzip else "")
         fn = getattr(self.L, name)
         fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
         rc = fn(self.h, C.cast(C.byref(opts), C.c_void_p), _ptr(buf), buf.size, _ptr(so))
@@ -769,6 +774,20 @@ class Aligner:
         nb = C.c_uint64(0)
         self.L.smr_gzip.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
         self._check(self.L.smr_gzip(self.h, _ptr(buf) if buf.size else None, buf.size, _ptr(o), o.size, C.cast(C.byref(nb), C.c_void_p)), "smr_gzip")
+        return o[:nb.value].tobytes()
+
+    def bam_header(self, text: bytes) -> bytes:
+        """smr_bam_header: the BAM header of the loaded indexes, with `text` (the SAM header) as its text, as BGZF blocks"""
+        self._upload_report_refs()
+        buf = np.frombuffer(text, np.uint8)
+        nb = C.c_uint64(0)
+        self.L.smr_bam_header.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
+        o = np.zeros(buf.size + (buf.size >> 6) + 4096, np.uint8)
+        rc = self.L.smr_bam_header(self.h, _ptr(buf) if buf.size else None, buf.size, _ptr(o), o.size, C.cast(C.byref(nb), C.c_void_p))
+        if rc == 5 and nb.value > o.size:   # SMR_ERR_CAPACITY: nb names the size (the reference names make it grow)
+            o = np.zeros(nb.value, np.uint8)
+            rc = self.L.smr_bam_header(self.h, _ptr(buf) if buf.size else None, buf.size, _ptr(o), o.size, C.cast(C.byref(nb), C.c_void_p))
+        self._check(rc, "smr_bam_header")
         return o[:nb.value].tobytes()
 
     def format_reports(self, out: dict, text: bytes | None = None, opts: ReportOpts | None = None, gzip: bool = False, **kw) -> dict:
@@ -1204,7 +1223,7 @@ class _FileWriter:
 
 def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, minimal_score=None, evalue: float = 1.0, sam: bool = False,
               sq: bool = False, blast=None, fastx: bool = False, other: bool = False, denovo=None, otu_map=None, paired_in: bool = False,
-              paired_out: bool = False, out2: bool = False, sout: bool = False, zip_out: bool = False, lnwin: int = 18, interval: int = 1,
+              paired_out: bool = False, out2: bool = False, sout: bool = False, zip_out: bool = False, bam: bool = False, lnwin: int = 18, interval: int = 1,
               max_pos: int = 10000, max_mb: float = 3072.0, skiplengths=None, index_budget: int = 0, batch_bytes: int = 256 << 20,
               piece_bytes: int = 256 << 20, cmd: str = "", threads: int = 1, device: int = 0) -> dict:
     """The reference's run from read files to its out/ directory, in one call: refs = the -ref FASTA files, reads = one reads file
@@ -1224,7 +1243,9 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
     gumbel[k] = (lambda, K) of refs[k]: the library does not compute them (the reference's ALP).  params: an api.Params (default
     default_params()).  Report options as report_opts / ReportWriter take them: sam, sq (-SQ), blast ("1 cigar qcov qstrand", "0"),
     fastx, other, denovo = (min_id, min_cov) for aligned_denovo.*, otu_map = (min_id, min_cov), paired_in / paired_out / out2 / sout,
-    zip_out (every report file gzip-compressed on the device, ".gz" appended; otu_map.txt and aligned.log stay plain).
+    zip_out (every report file gzip-compressed on the device, ".gz" appended; otu_map.txt and aligned.log stay plain).  bam: also
+    aligned.bam, the rows of aligned.sam (with or without sam) as BAM records in BGZF blocks written on the device
+    (Aligner.bam_header, format_placed_into(bam=True)) and the BGZF EOF block; it is BGZF whatever zip_out says.
     Files are written by a writer thread while the caller's thread makes, runs and formats the next batch (the library calls release
     the GIL); two output buffers alternate between them, and the streams go from those buffers to the files without a copy.  The
     read files and the SAM / BLAST rows of the first (index, part) group are appended to their final files as they come.  With
@@ -1252,6 +1273,7 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
     if pairwise:
         rest.blast = 0
     pw_opts = report_opts(blast="0", paired_in=paired_in, paired_out=paired_out)
+    bam_opts = report_opts(sam=True, paired_in=paired_in, paired_out=paired_out)
     feed = "two_files" if mates else "one_file" if (paired_in or paired_out) else None
     with_denovo = otu_map is not None or o.denovo
     sec = dict.fromkeys(("count", "index", "stream", "produce", "run", "place", "format", "writer", "writer_wait", "caller_wait", "parts",
@@ -1278,7 +1300,7 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
             if o.blast:
                 lam, K = gumbel[k]
                 al.set_report_scoring(k, lam, K, *hostio.evalue_params(stats[k], K, counts["length"], counts["reads"]))
-        al.set_place_stats(bool(o.sam or o.blast or o.denovo or otu_map is not None))
+        al.set_place_stats(bool(o.sam or bam or o.blast or o.denovo or otu_map is not None))
         layout = "packed" if params.num_alignments == 0 else "strided"
         al.set_aln_layout(layout)
         place = al.place_packed if layout == "packed" else al.place
@@ -1297,12 +1319,16 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
             parts[key] = open(os.path.join(out_dir, f".part_{key}"), "w+b")
             return parts[key]
 
-        dest, pw_dest = [], []
+        dest, pw_dest, bam_dest = [], [], []
+        head = hostio.sam_header_of([x for s in seqs for x in s], cmd, sq).encode()
         if o.sam:
             fh = open_file("aligned.sam")
-            head = hostio.sam_header_of([x for s in seqs for x in s], cmd, sq).encode()
             fh.write(al.gzip(head) if zip_out else head)
             dest += [(g, fh if g == 0 else part_file(f"sam_{g}")) for g in range(G)]
+        if bam:
+            fh = files["aligned.bam"] = open(os.path.join(out_dir, "aligned.bam"), "wb")
+            fh.write(al.bam_header(head))
+            bam_dest = [(g, fh if g == 0 else part_file(f"bam_{g}")) for g in range(G)]
         if o.blast:
             fh = open_file("aligned.blast")
             (pw_dest if pairwise else dest).extend((g + (0 if pairwise else G), fh if g == 0 else part_file(f"blast_{g}")) for g in range(G))
@@ -1310,8 +1336,8 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
         for j, (flag, name) in enumerate(((o.fastx, "aligned"), (o.other, "other"), (o.denovo, "aligned_denovo"))):
             if flag:
                 dest += [(2 * G + j * num_out + i, open_file(f"{name}{sfx}.{ext}")) for i, sfx in enumerate(fx_suffixes(o))]
-        # two output buffers (one for each report call of a batch) alternate between this thread and the writer
-        free = [[np.zeros(1 << 20, np.uint8), np.zeros(1 << 16, np.uint8)] for _ in range(2)]
+        # two sets of output buffers (one buffer for each report call of a batch) alternate between this thread and the writer
+        free = [[np.zeros(1 << 20, np.uint8), np.zeros(1 << 16, np.uint8), np.zeros(1 << 16, np.uint8)] for _ in range(2)]
         cv = threading.Condition()
 
         def release(slot):
@@ -1351,6 +1377,9 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
             if pw_dest:
                 slot[1], so = al.format_placed_into(pw_opts, slot[1], zip_out, pairwise=True)
                 jobs.append((slot[1], so, pw_dest))
+            if bam_dest:
+                slot[2], so = al.format_placed_into(bam_opts, slot[2], bam=True)
+                jobs.append((slot[2], so, bam_dest))
             if otu_map is not None:
                 al.otu_add(None)
             if with_denovo:
@@ -1371,14 +1400,17 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
         sec["writer"], sec["writer_wait"] = writer.write_s, writer.wait_s
         writer = None
         t1 = time.perf_counter()
-        for key in [f"sam_{g}" for g in range(1, G)] + [f"blast_{g}" for g in range(1, G)]:
-            fh = parts.get(key)
-            if fh is not None:
-                fh.seek(0)
-                shutil.copyfileobj(fh, files["aligned.sam" if key.startswith("sam") else "aligned.blast"], 1 << 24)
+        for kind, name in (("sam", "aligned.sam"), ("blast", "aligned.blast"), ("bam", "aligned.bam")):
+            for g in range(1, G):
+                fh = parts.get(f"{kind}_{g}")
+                if fh is not None:
+                    fh.seek(0)
+                    shutil.copyfileobj(fh, files[name], 1 << 24)
+        if bam:
+            files["aligned.bam"].write(BGZF_EOF)
         paths = []
         for name, fh in files.items():
-            if zip_out and fh.tell() == 0:
+            if zip_out and fh.tell() == 0:   # never aligned.bam: it holds its header
                 fh.write(al.gzip(b""))
             fh.close()
             paths.append(fh.name)

@@ -122,6 +122,7 @@ struct TextWords {
   uint32_t nrec, seq_bytes, err;   // text_layout: records, sequence bytes, decode error bits
   uint32_t pk_words, max_len;      // upload_fastx_impl: packed words of the batch, its longest read
   uint32_t rpt_err;                // rpt_prologue: the report side's error bits (RptArgs::err)
+  uint32_t rpt_bad;                // format_reports_impl, BAM: the first read BAM cannot hold
 };
 
 }  // namespace
@@ -194,7 +195,7 @@ struct smr_ctx {
   std::vector<RptScore> rpt_score;
   struct { DevBuf text, line, recs, res, aln, cig, st, flags, keys, keys2, vals, rows, first, sz, off, bsz, boff, fxsz, fxoff, grp, so, out, aoff, sread; } r;
   double t_rpt[3] = {0, 0, 0};
-  struct { DevBuf in, chunk, m, freq, codes, hdr, info, scratch, poff, plen, crc, dst, trl, out; } z;   // gzip deflate (gzip_streams, smr_deflate.cuh)
+  struct { DevBuf in, chunk, m, freq, codes, hdr, info, scratch, poff, plen, crc, dst, trl, ghdr, out; } z;   // gzip deflate (gzip_streams, smr_deflate.cuh)
   uint64_t parts_gen = 0;   // bumped whenever a part is loaded or its report ids are set: an open OTU map refuses to go on after that
   // OTU map accumulator (smr_otu.cuh), smr_otu_begin .. smr_otu_finish
   struct Otu {
@@ -1991,6 +1992,16 @@ void rpt_check(uint32_t e) {
                     : e & kRptErrCigar ? "an alignment's CIGAR lies outside cigar_words" : "an alignment's CIGAR runs past its read or its reference");
 }
 
+// fails with the text of the BAM error bits of e, naming the batch's read `bad`, if any
+void rpt_check_bam(uint32_t e, uint32_t bad) {
+  const uint32_t b = e & (kRptErrBamName | kRptErrBamQualLen | kRptErrBamQualByte);
+  if (b)
+    fail(SMR_ERR_ARG, "BAM: read " + std::to_string(bad) + " of the batch " +
+                      (b & kRptErrBamName ? "has a QNAME longer than 254 bytes"
+                       : b & kRptErrBamQualLen ? "has a quality line whose length differs from its sequence's"
+                                               : "has a quality byte outside '!'..'~'"));
+}
+
 // A report-side call's checks of its batch: the arrays (stats_msg: stats are read, the text if missing; arrays_msg: the text of
 // missing results or alns, stats_msg if null), an even read count when paired (mates 2k, 2k+1), fewer than 2^31 result slots.
 void rpt_check_batch(const smr_ctx* ctx, const char* what, const smr_read_result* results, const smr_aln* alns, const smr_aln_stats* stats,
@@ -2013,6 +2024,7 @@ std::vector<const Part*> report_groups(const smr_ctx* ctx) {
 // (smr_set_report_refs) / E-values and bit scores (smr_set_report_scoring), which every group must then have.
 std::vector<RptGroup> rpt_groups(const smr_ctx* ctx, bool names, bool scoring) {
   std::vector<RptGroup> hg;
+  uint32_t ref_base = 0;   // the refIDs of BAM: the references of every group in this order, one after another (smr_bam_header)
   for (const Part* pt : report_groups(ctx)) {
     const uint32_t ix = pt->d.index_num;
     if (names && !pt->has_rnames)
@@ -2020,7 +2032,8 @@ std::vector<RptGroup> rpt_groups(const smr_ctx* ctx, bool names, bool scoring) {
     const smr_ctx::RptScore* sc = ix < ctx->rpt_score.size() && ctx->rpt_score[ix].set ? &ctx->rpt_score[ix] : nullptr;
     if (scoring && !sc) fail(SMR_ERR_ARG, "smr_set_report_scoring was not called for index " + std::to_string(ix));
     hg.push_back(RptGroup{pt->rnames, pt->rname_off, sc ? (const double*)sc->ev.p : nullptr, sc ? (const uint32_t*)sc->bits.p : nullptr, pt->n_rnames,
-                          ix, pt->d.part, 0, pt->d.refseq, pt->d.ref_off});
+                          ix, pt->d.part, ref_base, pt->d.refseq, pt->d.ref_off});
+    ref_base += pt->d.nref;
   }
   return hg;
 }
@@ -2100,9 +2113,10 @@ void set_rpt_times(smr_ctx* ctx, const cudaEvent_t* e) { for (int k = 0; k < 3; 
 // ---------------------------------------------------------------------------------------------------------------------
 // The streams [sb[k], se[k]) of the device bytes `in` (padded by >= 8 readable bytes), each non-empty one compressed to one gzip
 // member, into the host buffer `out` one after another; so[0 .. ns] = their offsets.  If the members do not fit in cap, fails with
-// SMR_ERR_CAPACITY with so filled (a retry gives the same bytes).  e_dev is recorded before the D2H, e_end after it.
+// SMR_ERR_CAPACITY with so filled (a retry gives the same bytes).  e_dev is recorded before the D2H, e_end after it.  hlen:
+// kGzHeader, zlib's gzip header; kBgzfHeader, the BGZF header with each member's BSIZE (the caller cuts the BGZF blocks).
 void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& sb, const std::vector<uint64_t>& se, char* out, uint64_t cap,
-                  uint64_t* so, cudaEvent_t e_dev, cudaEvent_t e_end) {
+                  uint64_t* so, cudaEvent_t e_dev, cudaEvent_t e_end, uint32_t hlen = kGzHeader) {
   auto& Z = ctx->z;
   const uint32_t ns = (uint32_t)sb.size();
   std::vector<DefChunk> ch;
@@ -2144,25 +2158,29 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
   // the byte-size scan: chunk c goes to dst[c]; every member is header, its chunks, trailer
   std::vector<uint64_t> dst(nch);
   std::vector<uint32_t> trl(2 * (size_t)ns + 2, 0);
+  std::vector<uint8_t> hdr((size_t)ns * hlen + 1);
   uint64_t at = 0;
   uint32_t c = 0;
   for (uint32_t k = 0; k < ns; ++k) {
     so[k] = at;
     if (se[k] == sb[k]) continue;
-    at += 10;
+    at += hlen;
     uint32_t crc = 0;
     for (; c < nch && ch[c].stream == k; ++c) { dst[c] = at; at += info[c].bytes; crc = crc_concat(crc, crcs[c], ch[c].e - ch[c].b); }
     trl[2 * k] = crc; trl[2 * k + 1] = (uint32_t)(se[k] - sb[k]);
     at += 8;
+    if (hlen == kBgzfHeader) bgzf_header(&hdr[(size_t)k * hlen], (uint32_t)(at - so[k]));
+    else for (uint32_t i = 0; i < hlen; ++i) hdr[(size_t)k * hlen + i] = gz_header_byte(i);
   }
   so[ns] = at;
   if (at && (!out || cap < at)) fail(SMR_ERR_CAPACITY, "output buffer too small: stream_off holds the compressed sizes");
   if (nch) {
     upload_async(ctx, Z.dst, dst.data(), nch);
     upload_async(ctx, Z.trl, trl.data(), trl.size());
+    upload_async(ctx, Z.ghdr, hdr.data(), hdr.size());
     ensure(Z.out, at);
     def_place_kernel<<<nch, 256, 0, ctx->stream>>>((const DefChunk*)Z.chunk.p, (const DefInfo*)Z.info.p, (const uint8_t*)Z.scratch.p,
-                                                   (const uint64_t*)Z.dst.p, (const uint32_t*)Z.trl.p, (uint8_t*)Z.out.p);
+                                                   (const uint64_t*)Z.dst.p, (const uint32_t*)Z.trl.p, (const uint8_t*)Z.ghdr.p, hlen, (uint8_t*)Z.out.p);
     CK(cudaGetLastError());
   }
   CK(cudaEventRecord(e_dev, ctx->stream));
@@ -2171,16 +2189,20 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
   CK(cudaStreamSynchronize(ctx->stream));
 }
 
-// pairwise: smr_format_blast_pairwise[_gz], the pairwise BLAST rows alone (-blast 0), one stream per group; otherwise the streams of
-// smr_format_reports[_gz].  Both share the routing (the skip of empty reads), the row order and the scans.
+// pairwise: smr_format_blast_pairwise[_gz], the pairwise BLAST rows alone (-blast 0), one stream per group; bam:
+// smr_format_bam_placed, the SAM rows as BAM records in BGZF blocks, one stream per group; otherwise the streams of
+// smr_format_reports[_gz].  All share the routing (the skip of empty reads), the row order and the scans.
 void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
                          const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
-                         char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise, bool dev = false) {
+                         char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise, bool dev = false, bool bam = false) {
   const bool mates = o->mates || (!text && ctx->res.mates);   // the resident batch of a mate stream is mates
   const bool paired = o->paired_in || o->paired_out || mates;
   if (pairwise) {   // -blast '0 cigar' is refused by the reference too (options.cpp:584-588)
     if (!o->blast || o->blast_format != 0 || o->blast_cols[0] || o->sam || o->fastx || o->other || o->denovo)
       fail(SMR_ERR_ARG, "pairwise BLAST: opts must ask for -blast 0 alone (blast = 1, blast_format = 0, no BLAST columns, no SAM or read files)");
+  } else if (bam) {
+    if (!o->sam || o->blast || o->fastx || o->other || o->denovo)
+      fail(SMR_ERR_ARG, "BAM: opts must ask for SAM alone (sam = 1, no BLAST, no read files)");
   } else {
     if ((o->out2 || o->sout) && !paired) fail(SMR_ERR_UNSUPPORTED, "-out2 / -sout: only a paired batch (mates, paired_in or paired_out) has mates to split");
     if (o->blast && o->blast_format != 1)
@@ -2188,8 +2210,8 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   }
   if (o->paired_in && o->paired_out) fail(SMR_ERR_ARG, "paired_in and paired_out are exclusive");
   if (!pairwise && o->sout && (o->paired_in || o->paired_out)) fail(SMR_ERR_ARG, "-sout cannot be used with paired_in or paired_out");
-  const uint32_t num_out = pairwise ? 1 : o->out2 && o->sout ? 4 : o->out2 || o->sout ? 2 : 1;   // ReportFxBase::set_num_out
-  const uint32_t nfx = pairwise ? 0 : 3 * num_out;                                                // aligned, other, denovo: num_out files each
+  const uint32_t num_out = pairwise || bam ? 1 : o->out2 && o->sout ? 4 : o->out2 || o->sout ? 2 : 1;   // ReportFxBase::set_num_out
+  const uint32_t nfx = pairwise || bam ? 0 : 3 * num_out;                                                // aligned, other, denovo: num_out files each
   // a null results or alns array: no text of its own, the last one stays
   rpt_check_batch(ctx, "the report writer", results, alns, stats, nreads, paired,
                   o->sam || (o->blast && !pairwise) || o->denovo ? "SAM, BLAST and denovo need the smr_aln_stats of the batch" : nullptr, ctx->err.c_str(), dev);
@@ -2221,6 +2243,8 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   uint64_t* fxsz = ensure<uint64_t>(S.fxsz, nfx * fstride * 8);
   uint64_t* fxoff = ensure<uint64_t>(S.fxoff, nfx * fstride * 8);
   uint64_t* so = ensure<uint64_t>(S.so, (size_t)nso * 8);
+  uint32_t* bad = &text_words(ctx)->rpt_bad;
+  if (bam) CK(cudaMemsetAsync(bad, 0xFF, 4, ctx->stream));
   for (int k = 0; k < 4; ++k) a.cols[k] = cols[k];
   a.ncols = ncols; a.min_id = o->min_id; a.min_cov = o->min_cov;
   a.paired_in = o->paired_in != 0; a.paired_out = o->paired_out != 0; a.mates = mates; a.denovo = o->denovo != 0;
@@ -2237,7 +2261,8 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
     while ((1u << nbits) <= G) ++nbits;
     cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, keys, keys2, vals, rows, (int)N, 0, nbits, ctx->stream); });
     rpt_group_first_kernel<<<(G + 128) / 128, 128, 0, ctx->stream>>>(keys2, N, G, first);
-    if (o->sam) rpt_sam_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, sz);
+    if (bam) rpt_bam_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, sz, bad);
+    else if (o->sam) rpt_sam_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, sz);
     if (o->blast && pairwise) rpt_pw_size_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz);
     else if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, bsz, nullptr, nullptr);
     if (o->fastx || o->other || o->denovo) {
@@ -2254,27 +2279,42 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
   rpt_stream_off_kernel<<<1, 32, 0, ctx->stream>>>(first, G, off, boff, fxoff, nreads, fstride, nfx, so);
   CK(cudaGetLastError());
   std::vector<uint64_t> hso(nso);
-  uint32_t err = 0;
+  uint32_t err = 0, hbad = 0;
   CK(cudaMemcpyAsync(hso.data(), so, (size_t)nso * 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaMemcpyAsync(&err, a.err, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  if (bam) CK(cudaMemcpyAsync(&hbad, bad, 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
+  if (bam) rpt_check_bam(err, hbad);
   rpt_check(err);
   const uint32_t s0 = pairwise ? G : 0;   // the first stream handed out: pairwise, the BLAST streams alone (the SAM ones are empty)
-  if (!gz) memcpy(so_out, hso.data() + s0, (size_t)(nso - s0) * 8);
+  if (!gz && !bam) memcpy(so_out, hso.data() + s0, (size_t)(nso - s0) * 8);
   const uint64_t total = hso[nso - 1];
-  if (!gz && total && (!out || cap < total)) fail(SMR_ERR_CAPACITY, "output buffer too small: stream_off holds the sizes");
+  if (!gz && !bam && total && (!out || cap < total)) fail(SMR_ERR_CAPACITY, "output buffer too small: stream_off holds the sizes");
   // the encoder reads up to 8 bytes past a stream's end (def_load32): the padding is part of the one allocation before the writes,
   // since ensure() does not keep what a buffer held
-  if (total || gz) ensure(S.out, total + (gz ? 8 : 0));
+  if (total || gz || bam) ensure(S.out, total + (gz || bam ? 8 : 0));
   if (total) {
     char* dout = (char*)S.out.p;
-    if (o->sam) rpt_sam_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, off, dout);
+    if (bam) rpt_bam_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, off, dout, bad);
+    else if (o->sam) rpt_sam_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, off, dout);
     if (o->blast && pairwise) rpt_pw_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, boff, dout + hso[G]);
     else if (o->blast) rpt_blast_kernel<<<grid, 256, 0, ctx->stream>>>(a, rows, first, nullptr, boff, dout + hso[G]);
     if (o->fastx || o->other || o->denovo) rpt_fx_write_kernel<<<grid, 256, 0, ctx->stream>>>(a, flags, fxoff, fstride, so + 2 * G, dout);
     CK(cudaGetLastError());
   }
-  if (gz) {   // every non-empty stream to one gzip member, before the D2H
+  if (bam) {   // the quality bytes the write pass checked, then each group's records cut into BGZF blocks
+    CK(cudaMemcpyAsync(&err, a.err, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(&hbad, bad, 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+    rpt_check_bam(err, hbad);
+    std::vector<uint64_t> sb, se;
+    std::vector<size_t> gb(G + 1);   // the first block of each group
+    for (uint32_t g = 0; g < G; ++g) { gb[g] = sb.size(); bgzf_blocks(hso[g], hso[g + 1], sb, se); }
+    gb[G] = sb.size();
+    std::vector<uint64_t> bso(sb.size() + 1, 0);
+    const auto put_offsets = on_exit([&] { for (uint32_t g = 0; g <= G; ++g) so_out[g] = bso[gb[g]]; });   // a buffer too small names the sizes
+    gzip_streams(ctx, (const uint8_t*)S.out.p, sb, se, out, cap, bso.data(), e[2], e[3], kBgzfHeader);
+  } else if (gz) {   // every non-empty stream to one gzip member, before the D2H
     std::vector<uint64_t> sb(hso.begin() + s0, hso.end() - 1), se(hso.begin() + s0 + 1, hso.end());
     gzip_streams(ctx, (const uint8_t*)S.out.p, sb, se, out, cap, so_out, e[2], e[3]);
   } else {
@@ -3216,6 +3256,57 @@ int smr_format_blast_pairwise_placed(smr_ctx* ctx, const smr_report_opts* opts, 
 int smr_format_blast_pairwise_placed_gz(smr_ctx* ctx, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off) {
   return format_placed(ctx, "smr_format_blast_pairwise_placed_gz", opts, out, cap, stream_off, true, true);
 }
+
+int smr_format_bam_placed(smr_ctx* ctx, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* stream_off) try {
+  if (!ctx || !opts || !stream_off) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  const PlacedArrays p = placed_of(ctx, "smr_format_bam_placed", true);
+  format_reports_impl(ctx, opts, nullptr, 0, p.res, p.aln, p.cig, p.cig_words, p.st, p.n, out, cap, stream_off, false, false, true, true);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_bam_header(smr_ctx* ctx, const char* text, uint64_t nbytes, char* out, uint64_t cap, uint64_t* out_bytes) try {
+  if (!ctx || !out_bytes || (!text && nbytes)) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  *out_bytes = 0;
+  if (nbytes > 0x7FFFFFFFull) fail(SMR_ERR_ARG, "BAM header: a text of 2^31 bytes or more");
+  cudaEvent_t* e = events(ctx, 4);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  // magic, l_text, text, n_ref, then (l_name, name NUL, l_ref) of every reference in the refID order of rpt_groups
+  std::vector<uint8_t> h;
+  auto le32 = [&](uint32_t v) { for (int k = 0; k < 4; ++k) h.push_back((uint8_t)(v >> (8 * k))); };
+  h.insert(h.end(), {'B', 'A', 'M', 1});
+  le32((uint32_t)nbytes);
+  h.insert(h.end(), text, text + nbytes);
+  const std::vector<RptGroup> hg = rpt_groups(ctx, true, false);
+  const std::vector<const Part*> gp = report_groups(ctx);
+  le32(hg.empty() ? 0 : hg.back().ref_base + hg.back().nref);
+  for (size_t g = 0; g < gp.size(); ++g) {
+    std::vector<uint32_t> roff((size_t)hg[g].nref + 1);
+    CK(cudaMemcpy(roff.data(), hg[g].ref_off, roff.size() * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t k = 0; k < hg[g].nref; ++k) {
+      const std::string& name = gp[g]->h_rnames[k];
+      le32((uint32_t)name.size() + 1);
+      h.insert(h.end(), name.begin(), name.end());
+      h.push_back(0);
+      le32(roff[k + 1] - roff[k]);
+    }
+  }
+  const uint64_t n = h.size();
+  ensure(ctx->z.in, n + 64);
+  CK(cudaMemsetAsync((uint8_t*)ctx->z.in.p + n, 0, 64, ctx->stream));
+  CK(cudaMemcpyAsync(ctx->z.in.p, h.data(), n, cudaMemcpyHostToDevice, ctx->stream));
+  CK(cudaEventRecord(e[1], ctx->stream));
+  std::vector<uint64_t> sb, se;
+  bgzf_blocks(0, n, sb, se);
+  std::vector<uint64_t> so(sb.size() + 1, 0);
+  {
+    const auto put_size = on_exit([&] { *out_bytes = so.back(); });   // a buffer too small fails, and names the size needed
+    gzip_streams(ctx, (const uint8_t*)ctx->z.in.p, sb, se, out, cap, so.data(), e[2], e[3], kBgzfHeader);
+  }
+  set_rpt_times(ctx, e);
+  return SMR_OK;
+} SMR_CATCH(ctx)
 
 int smr_otu_add_placed(smr_ctx* ctx, uint64_t* n_added) try {
   if (!ctx) return SMR_ERR_ARG;

@@ -1,4 +1,5 @@
-// gzip deflate on the device: the kernels around smr_deflate.h (MATCH / PARSE / CODE / WRITE / PLACE, described there).  The CRC-32
+// gzip deflate on the device: the kernels around smr_deflate.h (MATCH / PARSE / CODE / WRITE / PLACE, described there), for gzip
+// members and for the BGZF blocks of BAM, which differ in the header PLACE writes and in how the caller cuts the streams.  The CRC-32
 // of every chunk is inf_crc_kernel of smr_inflate.cuh (a chunk is at most one 32 KB piece); the host joins them with crc_concat.
 //
 // GPU mapping: MATCH is one warp per chunk with the chunk's hash table (16 KB) in shared memory, 32 positions per step; PARSE is
@@ -95,17 +96,18 @@ __global__ void __launch_bounds__(128) def_write_kernel(const uint8_t* __restric
   def_write_tail(o, t + k.b, k.e - k.b, in, fin, lane, 32);
 }
 
-// PLACE: CTA c copies chunk c to out + dst[c]; the stream's first chunk writes the gzip header before it, its last the trailer
-// (trl[2 * stream], trl[2 * stream + 1] = CRC-32, ISIZE) after it.
+// PLACE: CTA c copies chunk c to out + dst[c]; the stream's first chunk writes the member's header (hlen bytes at hdr[stream *
+// hlen], gzip or BGZF) before it, its last the trailer (trl[2 * stream], trl[2 * stream + 1] = CRC-32, ISIZE) after it.
 __global__ void __launch_bounds__(256) def_place_kernel(const DefChunk* __restrict__ ch, const DefInfo* __restrict__ info, const uint8_t* __restrict__ scratch,
-                                                         const uint64_t* __restrict__ dst, const uint32_t* __restrict__ trl, uint8_t* out) {
+                                                         const uint64_t* __restrict__ dst, const uint32_t* __restrict__ trl, const uint8_t* __restrict__ hdr,
+                                                         uint32_t hlen, uint8_t* out) {
   const uint32_t c = blockIdx.x;
   const uint64_t d = dst[c];
   const uint32_t n = info[c].bytes;
   const uint8_t* s = scratch + (size_t)c * kDefScratch;
   for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) out[d + i] = s[i];
   const DefChunk k = ch[c];
-  if ((k.flags & kDefFirst) && threadIdx.x < 10) out[d - 10 + threadIdx.x] = gz_header_byte(threadIdx.x);
+  if ((k.flags & kDefFirst) && threadIdx.x < hlen) out[d - hlen + threadIdx.x] = hdr[(size_t)k.stream * hlen + threadIdx.x];
   if ((k.flags & kDefLast) && threadIdx.x < 8) out[d + n + threadIdx.x] = (uint8_t)(trl[2 * k.stream + threadIdx.x / 4] >> (8 * (threadIdx.x & 3)));
 }
 

@@ -49,6 +49,25 @@ struct DefCodes { uint16_t code[316]; uint8_t len[316]; };
 
 // byte i of zlib's gzip header: no name, mtime 0, XFL 0, OS 3 (1f 8b 08 00 00000000 00 03)
 SMR_HD uint8_t gz_header_byte(uint32_t i) { return i == 0 ? 0x1f : i == 1 ? 0x8b : i == 2 ? 8 : i == 9 ? 3 : 0; }
+constexpr uint32_t kGzHeader = 10;
+
+// BGZF (SAMv1 4.1): gzip members of at most 64 KiB, each a stream of its own (no history before its first byte), whose header
+// carries FLG.FEXTRA and the subfield BC with BSIZE = member bytes - 1.  A block takes kBgzfBlock input bytes, two chunks; with
+// both chunks stored (5 + kDefChunk + 5, then 5 + the rest, final) a member is at most kBgzfMaxMember bytes.
+constexpr uint32_t kBgzfBlock = 65280;
+constexpr uint32_t kBgzfHeader = 18;
+constexpr uint32_t kBgzfMaxMember = kBgzfHeader + (5 + kDefChunk + 5) + (5 + kBgzfBlock - kDefChunk) + 8;
+static_assert(kBgzfBlock > kDefChunk && kBgzfBlock <= 2 * kDefChunk && kBgzfMaxMember <= 65536, "a BGZF member must fit in 64 KiB");
+// the 18 header bytes of a member of `bytes` bytes: 1f 8b 08 04, MTIME 0, XFL 0, OS 255, XLEN 6, 'B' 'C', SLEN 2, BSIZE
+inline void bgzf_header(uint8_t* p, uint32_t bytes) {
+  static const uint8_t h[16] = {0x1f, 0x8b, 8, 4, 0, 0, 0, 0, 0, 0xff, 6, 0, 'B', 'C', 2, 0};
+  memcpy(p, h, 16);
+  p[16] = (uint8_t)(bytes - 1); p[17] = (uint8_t)((bytes - 1) >> 8);
+}
+// [b, e) cut into BGZF blocks of kBgzfBlock bytes, the last holding the rest (none when empty), appended to sb / se
+inline void bgzf_blocks(uint64_t b, uint64_t e, std::vector<uint64_t>& sb, std::vector<uint64_t>& se) {
+  for (; b < e; b += kBgzfBlock) { sb.push_back(b); se.push_back(std::min<uint64_t>(e, b + kBgzfBlock)); }
+}
 
 SMR_HD uint32_t def_load32(const uint8_t* t, uint64_t p) {   // 4 bytes at p, little-endian (the buffer is padded)
 #if defined(__CUDA_ARCH__)

@@ -163,5 +163,22 @@ __host__ __device__ inline int fmt_g3(double x, char* o) {
   return len;
 }
 
+// BAM's fields of a SAM row (the BAM writer of smr_report.cuh; tests/bgzf_check.cpp prints them for the host test)
+// the BAI bin of the 0-based region [beg, end) (SAMv1 5.3, reg2bin)
+__host__ __device__ inline uint32_t bam_reg2bin(int64_t beg, int64_t end) {
+  --end;
+  if (beg >> 14 == end >> 14) return ((1u << 15) - 1) / 7 + (uint32_t)(beg >> 14);
+  if (beg >> 17 == end >> 17) return ((1u << 12) - 1) / 7 + (uint32_t)(beg >> 17);
+  if (beg >> 20 == end >> 20) return ((1u << 9) - 1) / 7 + (uint32_t)(beg >> 20);
+  if (beg >> 23 == end >> 23) return ((1u << 6) - 1) / 7 + (uint32_t)(beg >> 23);
+  if (beg >> 26 == end >> 26) return ((1u << 3) - 1) / 7 + (uint32_t)(beg >> 26);
+  return 0;
+}
+// the 4-bit code ("=ACMGRSVTWYHKDBN") of a letter SAM's SEQ prints (A, C, G, T, N)
+__host__ __device__ inline uint32_t bam_nt4(char c) { return c == 'A' ? 1 : c == 'C' ? 2 : c == 'G' ? 4 : c == 'T' ? 8 : 15; }
+// the bytes and the type htslib gives a SAM ":i:" value v >= 0: 'C' up to 255, 'S' up to 65535, 'I' above
+__host__ __device__ inline uint32_t bam_int_bytes(uint64_t v) { return v <= 0xFF ? 1 : v <= 0xFFFF ? 2 : 4; }
+__host__ __device__ inline char bam_int_type(uint32_t bytes) { return bytes == 1 ? 'C' : bytes == 2 ? 'S' : 'I'; }
+
 }  // namespace fmt
 }  // namespace smr
