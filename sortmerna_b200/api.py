@@ -657,12 +657,8 @@ class Aligner:
         stride grow to what the library names and the batch run again, as align() does.  Returns {"nreads", "slots", "n_alns",
         "cigar_words", "counters" (by name, as download()), "matched" (reads_matched_per_db), "place_ms" (device time of the
         placement passes)}."""
-        self.L.smr_place_results.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
-        self.L.smr_last_place_timing.argtypes = [C.c_void_p, C.c_void_p]
         while True:
-            counters = np.zeros(CNT_FIXED + max(1, self.n_index_files), np.uint64)
-            n_alns, words = C.c_uint64(0), C.c_uint64(0)
-            rc = self.L.smr_place_results(self.h, _ptr(counters), counters.size, C.cast(C.byref(n_alns), C.c_void_p), C.cast(C.byref(words), C.c_void_p))
+            rc, info = self._place("smr_place_results")
             slots = int(self.L.smr_aln_slots(self.h))
             need = int(self.L.smr_aln_slots_needed(self.h)) if rc == 5 and self.params.num_alignments == 0 else 0
             if need > slots:   # run again as run_resident() does, with a host stats buffer at the new stride if it had one
@@ -671,11 +667,9 @@ class Aligner:
                 continue
             break
         self._check(rc, "smr_place_results")
-        ms = C.c_double(0)
-        self.L.smr_last_place_timing(self.h, C.cast(C.byref(ms), C.c_void_p))
-        self.placed_info = dict(nreads=self._n_resident, slots=slots, n_alns=int(n_alns.value), cigar_words=int(words.value),
-                    counters={k: int(counters[i]) for i, k in enumerate(CNT_NAMES)}, matched=counters[CNT_FIXED:].copy(), place_ms=ms.value)
-        return self.placed_info
+        info["slots"] = slots
+        self.placed_info = info
+        return info
 
     def place_packed(self) -> dict:
         """smr_place_results_packed: the results of the last run_resident() in the packed layout placed on the device, as download()
@@ -683,18 +677,22 @@ class Aligner:
         the reads that overflowed their scratch at a larger scale, then every read placed in read order.  format_reports /
         format_blast_pairwise / format_placed_into / otu_add / denovo_stats / ReportWriter.write with out=None read them there, and
         a later download() copies them.  Returns the dict place() returns, with "slots" = 0 and "n_alns" = the sum of n_align."""
-        self.L.smr_place_results_packed.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
+        rc, info = self._place("smr_place_results_packed")
+        self._check(rc, "smr_place_results_packed")
+        self.placed_info = info
+        return info
+
+    def _place(self, fn: str):
+        """smr_place_results[_packed] (`fn`): its status and the dict place() returns, with "slots" = 0"""
+        f = getattr(self.L, fn)
+        f.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_void_p]
         self.L.smr_last_place_timing.argtypes = [C.c_void_p, C.c_void_p]
         counters = np.zeros(CNT_FIXED + max(1, self.n_index_files), np.uint64)
-        n_alns, words = C.c_uint64(0), C.c_uint64(0)
-        rc = self.L.smr_place_results_packed(self.h, _ptr(counters), counters.size, C.cast(C.byref(n_alns), C.c_void_p),
-                                             C.cast(C.byref(words), C.c_void_p))
-        self._check(rc, "smr_place_results_packed")
-        ms = C.c_double(0)
+        n_alns, words, ms = C.c_uint64(0), C.c_uint64(0), C.c_double(0)
+        rc = f(self.h, _ptr(counters), counters.size, C.cast(C.byref(n_alns), C.c_void_p), C.cast(C.byref(words), C.c_void_p))
         self.L.smr_last_place_timing(self.h, C.cast(C.byref(ms), C.c_void_p))
-        self.placed_info = dict(nreads=self._n_resident, slots=0, n_alns=int(n_alns.value), cigar_words=int(words.value),
-                    counters={k: int(counters[i]) for i, k in enumerate(CNT_NAMES)}, matched=counters[CNT_FIXED:].copy(), place_ms=ms.value)
-        return self.placed_info
+        return rc, dict(nreads=self._n_resident, slots=0, n_alns=int(n_alns.value), cigar_words=int(words.value),
+                        counters={k: int(counters[i]) for i, k in enumerate(CNT_NAMES)}, matched=counters[CNT_FIXED:].copy(), place_ms=ms.value)
 
     def download_placed(self, with_stats: bool = False) -> dict:
         """smr_download_placed: the placed arrays on the host, in the form download() returns ("res", "alns", "cigar", "slots", and

@@ -147,22 +147,23 @@ struct smr_ctx {
   uint32_t need_slots = 0;       // set with SMR_ERR_CAPACITY in all-alignments mode: the stride the batch needs
   uint32_t all_slots = 16;       // stride of the result layout when num_alignments == 0 (smr_set_aln_slots)
   uint32_t layout = SMR_ALNS_STRIDED;   // smr_set_aln_layout
-  uint64_t retry_slots = 1u << 24;      // packed layout: slot budget of one sub-batch of reads run again for their alignment count
+  uint64_t retry_slots = 1u << 24;      // slot budget of one sub-batch of reads run again (rerun_flagged)
   uint64_t runs_made = 0;               // numbers the runs (Batch::run_id)
-  // The results of the resident batch's last run placed on the device (smr_place_results, place_resident, in the strided layout;
-  // smr_place_results_packed and the packed downloads, place_packed, in the packed one), kept until the batch is run again or
-  // replaced; the report-side _placed calls read them there, and a packed download retried for capacity, or repeated, copies them.
+  // The results of the resident batch's last run placed on the device (place: smr_place_results in the strided layout,
+  // smr_place_results_packed and the packed downloads in the packed one), kept until the batch is run again or replaced; the
+  // report-side _placed calls read them there, and a packed download retried for capacity, or repeated, copies them.
   struct Placed {
     uint64_t run_id = 0;   // Batch::run_id of the run they come from; 0 = none
     uint32_t nreads = 0, slots = 0; bool stats = false;
     bool packed = false;   // placed in the packed layout: n_alns alignments, read r's from aln_off[r]; slots = the first run's stride
     bool trace = false;    // packed: a run met a trace back error (each call that reads the placement fails with SMR_ERR_INDEX)
     uint64_t cig_words = 0, n_alns = 0;
-    DevBuf res, aln, st, cig, cnt, words, off, scal;   // the placed arrays, the counters (ncnt u64), count-pass scratch
-    DevBuf aoff, nal, src, runs, fsel, fout;           // packed: aln_off, n_align per read, each read's source run, the run table, flagged reads (bits, list)
+    DevBuf res, aln, st, cig, cnt;                     // the placed arrays, the counters (ncnt u64)
+    DevBuf words, off, nal, aoff, src, runs, scal, fsel, fout;   // scratch: CIGAR words and offsets, rows and aln_off per read, each read's
+                                                                 // source run, the run table, flagged reads (scan, bits, list)
     std::vector<uint64_t> cnt_host;                    // what smr_place_results[_packed] adds to the caller's counters
     double t_place = 0;                                // ms of the placement passes (CUDA events), retries and re-runs excluded
-    RunTimes t_run;                                    // packed: the first run and its re-runs
+    RunTimes t_run;                                    // the first run and its re-runs
   } pl;
   bool place_stats = false;   // smr_set_place_stats: every run computes the smr_aln_stats a placement keeps
   uint32_t lis_ctas_per_sm = kLisMinCtas;   // persistent CTAs of the candidate kernel per SM (matches its __launch_bounds__)
@@ -1487,11 +1488,11 @@ struct HostOut {
 const char* const kCigarOffsetMsg = "CIGAR pool offset passes 2^32 words (smr_aln.cigar_off is 32-bit): use smaller batches";
 const char* const kTraceErrorMsg = "trace back error (ssw.c:707 is fatal in the reference too)";
 
-// copies the results of a batch's run to the host; returns the indices of reads whose scratch overflowed
-void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint32_t>& flagged, const uint32_t* map /*local->caller index or null*/) {
+// copies the results of a batch's run to the host; returns the reads whose scratch overflowed (rerun_flagged runs them again)
+std::vector<PackFlag> download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, const uint32_t* map /*local->caller index or null*/) {
   const uint32_t n = b.nreads;
-  flagged.clear();
-  if (n == 0) return;
+  std::vector<PackFlag> flagged;
+  if (n == 0) return flagged;
   const uint32_t slots = slots_of(ctx);
   cudaEvent_t* e = events(ctx, 2);
   CK(cudaEventRecord(e[0], ctx->stream));
@@ -1518,7 +1519,7 @@ void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint3
   if (used) CK(cudaMemcpyAsync(ctx->h.cigar.p, b.cigar_pool.p, used * 4, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaEventRecord(e[1], ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
-  ctx->t_d2h = elapsed_ms(e[0], e[1]);
+  ctx->t_d2h += elapsed_ms(e[0], e[1]);
   // a trace back error fails the call after what it can still write; the capacity errors below take precedence
   bool trace_error = false;
   auto fail_on_trace_error = [&] { if (trace_error) fail(SMR_ERR_INDEX, "trace back error (ssw.c:707 is fatal in the reference too)"); };
@@ -1530,7 +1531,7 @@ void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint3
     coff[r] = run;
     if (fl[r] & kErrTrace) trace_error = true;
     if (fl[r] & kOvfSlots) { need_slots = std::max(need_slots, st[r].n_align); continue; }   // not retried: the stride is the caller's
-    if (fl[r]) { flagged.push_back(r); for (int bit = 0; bit < 6; ++bit) if (fl[r] & (1u << bit)) ctx->flag_hist[bit]++; continue; }
+    if (fl[r]) { flagged.push_back(PackFlag{r, fl[r], st[r].n_align}); continue; }
     const ReadState& s = st[r];
     for (uint32_t k = 0; k < slots && k < s.n_align; ++k) run += oa[(size_t)r * slots + k].cigar_len;
     if (s.is_hit && out.counters) {
@@ -1546,7 +1547,7 @@ void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint3
   // a pool too small fails the call only at its end (download_resident): the flagged reads are still retried, so that
   // cigar_used names every word the batch needs and one larger pool is enough
   if (run > out.cigar_cap) out.pool_short = true;
-  if (out.pool_short) { fail_on_trace_error(); return; }
+  if (out.pool_short) { fail_on_trace_error(); return flagged; }
   // pass 2: results, alignments and cigars of disjoint read ranges, by a few host threads for large batches
   auto pack = [&](uint32_t lo, uint32_t hi) {
     for (uint32_t r = lo; r < hi; ++r) {
@@ -1581,36 +1582,63 @@ void download_impl(smr_ctx* ctx, const Batch& b, HostOut& out, std::vector<uint3
   if (out.counters)
     for (uint32_t k = dcNumShort; k < dcCount && k < out.n_counters; ++k) out.counters[k] += cnt[k];
   fail_on_trace_error();
+  return flagged;
 }
 
-// Runs the flagged reads of a failed batch again as a batch of their own with 8x its scratch, gathered from its reads on the device,
-// and hands it to take(batch, map, again), which writes its results after what is there (map: index in the batch -> the caller's
-// index; `again`: the reads to retry once more): download_impl into the caller's arrays, or place_run into the placed arrays.
-// Reads that overflow again go on to 64x and 512x.  The batch frees itself on return, after take.
-template <class Take>
-void retry_flagged(smr_ctx* ctx, const Batch& failed, const std::vector<uint32_t>& flagged, const uint32_t* map, Take& take, int depth) {
-  if (getenv("SMR_VERBOSE")) fprintf(stderr, "[smr] %zu reads overflowed their scratch at scale %u: retrying with scale %u (causes so far: lane %llu region %llu pairs %llu trace %llu cigar %llu err %llu)\n", flagged.size(), failed.scale, failed.scale * 8,
-      (unsigned long long)ctx->flag_hist[0], (unsigned long long)ctx->flag_hist[1], (unsigned long long)ctx->flag_hist[2], (unsigned long long)ctx->flag_hist[3], (unsigned long long)ctx->flag_hist[4], (unsigned long long)ctx->flag_hist[5]);
-  if (depth >= 3) fail(SMR_ERR_CAPACITY, "scratch overflow persists after 3 retries (" + std::to_string(flagged.size()) + " reads)");
-  const uint32_t n = (uint32_t)flagged.size();
-  std::vector<uint32_t> src(n), smap(n);
-  for (uint32_t k = 0; k < n; ++k) { src[k] = failed.off32[flagged[k]]; smap[k] = map ? map[flagged[k]] : flagged[k]; }
-  Batch b;
-  b.scale = failed.scale * 8;
-  const uint64_t w = read_layout(ctx, b, n, [&](uint32_t k) { return failed.off32[flagged[k] + 1] - src[k]; });
-  DevBuf d_src;
-  upload_async(ctx, d_src, src.data(), n);
-  ensure(b.seq04, b.total_nt + 64);
-  gather_reads_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
-      (const uint8_t*)failed.seq04.p, (const uint32_t*)d_src.p, n, (const uint32_t*)b.seq_off.p, (uint8_t*)b.seq04.p);
-  CK(cudaGetLastError());
-  finish_upload(ctx, b, w);
-  run_impl(ctx, b);
-  const double d2h = ctx->t_d2h;
-  std::vector<uint32_t> again;
-  take(b, smap.data(), again);
-  ctx->t_run += b.run; ctx->t_d2h += d2h;
-  if (!again.empty()) retry_flagged(ctx, b, again, smap.data(), take, depth + 1);
+// The re-run planner.  The reads `fl` that a run of batch `from` flagged (map[k]: the resident batch's index of its read k; null: k)
+// run again as batches of their own, gathered from `from` on the device.  Each is handed to consume(batch, its map, exact) once it
+// has run, which takes its results and returns the reads it flagged; those are planned the same way.  Reads flagged kOvfSlots alone
+// stored more alignments than their room: they run again at their exact count (exact) and the same scale.  Every other flagged read
+// overflowed its scratch: it runs again at 8x the scale with room for max(stride, the count it reached), for 3 scales at most.  The
+// reads are cut into sub-batches of at most ctx->retry_slots slots (a larger read alone), each run with its own re-runs before the
+// next: the order in which the host download writes them and the strided placement scans their CIGARs.  A sub-batch whose reads
+// all have room for the stride runs on the strided arenas.  The batch frees itself after its re-runs, but for what consume moves out.
+template <class Consume>
+void rerun_flagged(smr_ctx* ctx, const Batch& from, const std::vector<PackFlag>& fl, const uint32_t* map, int depth, Consume& consume) {
+  const uint32_t S = slots_of(ctx);
+  std::vector<uint32_t> idx[2], cap[2];   // [0]: run again for their count, [1]: for their scratch
+  for (const PackFlag& f : fl) {
+    const int x = f.flags != kOvfSlots;
+    idx[x].push_back(f.read); cap[x].push_back(x ? std::max(S, f.n_align) : f.n_align);
+    if (x) for (int bit = 0; bit < 6; ++bit) if (f.flags & (1u << bit)) ctx->flag_hist[bit]++;
+  }
+  if (depth >= 3 && !idx[1].empty()) fail(SMR_ERR_CAPACITY, "scratch overflow persists after 3 retries (" + std::to_string(idx[1].size()) + " reads)");
+  for (int x = 0; x < 2; ++x) {
+    const std::vector<uint32_t>& I = idx[x];
+    const std::vector<uint32_t>& C = cap[x];
+    const uint32_t scale = x ? from.scale * 8 : from.scale;
+    for (size_t a = 0; a < I.size();) {
+      size_t e = a;
+      uint64_t total = 0;
+      bool strided = true;
+      while (e < I.size() && (e == a || total + C[e] <= ctx->retry_slots)) { strided &= C[e] == S; total += C[e++]; }
+      if (total >= (1ull << 31)) fail(SMR_ERR_CAPACITY, "a batch run again for its alignment count would hold 2^31 slots or more (a read that stores that many, or SMR_RETRY_SLOTS too large)");
+      const uint32_t n = (uint32_t)(e - a);
+      if (x && getenv("SMR_VERBOSE")) fprintf(stderr, "[smr] %u reads overflowed their scratch at scale %u: retrying with scale %u (causes so far: lane %llu region %llu pairs %llu trace %llu cigar %llu err %llu)\n", n, from.scale, scale,
+          (unsigned long long)ctx->flag_hist[0], (unsigned long long)ctx->flag_hist[1], (unsigned long long)ctx->flag_hist[2], (unsigned long long)ctx->flag_hist[3], (unsigned long long)ctx->flag_hist[4], (unsigned long long)ctx->flag_hist[5]);
+      std::vector<uint32_t> src(n), bmap(n);
+      for (uint32_t k = 0; k < n; ++k) { src[k] = from.off32[I[a + k]]; bmap[k] = map ? map[I[a + k]] : I[a + k]; }
+      Batch b;
+      b.scale = scale;
+      if (!strided) {
+        b.base.resize((size_t)n + 1, 0);
+        for (uint32_t k = 0; k < n; ++k) b.base[k + 1] = b.base[k] + C[a + k];
+      }
+      const uint64_t w = read_layout(ctx, b, n, [&](uint32_t k) { return from.off32[I[a + k] + 1] - src[k]; });
+      DevBuf d_src;
+      upload_async(ctx, d_src, src.data(), n);
+      ensure(b.seq04, b.total_nt + 64);
+      gather_reads_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
+          (const uint8_t*)from.seq04.p, (const uint32_t*)d_src.p, n, (const uint32_t*)b.seq_off.p, (uint8_t*)b.seq04.p);
+      CK(cudaGetLastError());
+      finish_upload(ctx, b, w);
+      run_impl(ctx, b);
+      ctx->t_run += b.run;
+      const std::vector<PackFlag> again = consume(b, bmap.data(), x == 0);
+      rerun_flagged(ctx, b, again, bmap.data(), depth + x, consume);
+      a = e;
+    }
+  }
 }
 
 // the arenas grow with a retry's scale (after 64x, tens of GB): the next run allocates them again at its own, whether the retry
@@ -1620,13 +1648,12 @@ void release_retry_arenas(smr_ctx* ctx) { for (DevBuf* s : {&ctx->run.lis, &ctx-
 // the results of the resident batch's last run into the caller's arrays, its flagged reads retried; the resident batch and its
 // device results stay as they are
 void download_resident(smr_ctx* ctx, HostOut& out) {
-  ctx->t_run = ctx->res.b.run;
-  std::vector<uint32_t> flagged;
-  download_impl(ctx, ctx->res.b, out, flagged, nullptr);
+  ctx->t_run = ctx->res.b.run; ctx->t_d2h = 0;
+  const std::vector<PackFlag> flagged = download_impl(ctx, ctx->res.b, out, nullptr);
   if (!flagged.empty()) {
     const auto release = on_exit([ctx] { release_retry_arenas(ctx); });
-    auto take = [&](const Batch& b, const uint32_t* map, std::vector<uint32_t>& again) { download_impl(ctx, b, out, again, map); };
-    retry_flagged(ctx, ctx->res.b, flagged, nullptr, take, 0);
+    auto consume = [&](const Batch& b, const uint32_t* map, bool) { return download_impl(ctx, b, out, map); };
+    rerun_flagged(ctx, ctx->res.b, flagged, nullptr, 0, consume);
   }
   // the caller's CIGAR pool was too small: *cigar_used names the words the batch needs
   if (out.pool_short)
@@ -1634,101 +1661,12 @@ void download_resident(smr_ctx* ctx, HostOut& out) {
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
-// device placement (smr_place_results, smr_place.cuh): the strided results of the resident batch's last run kept on the device,
-// in the bytes download_resident writes to the host
+// device placement (smr_place_results, smr_place_results_packed, smr_place.cuh): the final results of the resident batch's last
+// run kept on the device, in the bytes the host download of its layout writes (smr_download_results,
+// smr_download_results_packed)
 // ---------------------------------------------------------------------------------------------------------------------
 // the counters a placement keeps: SMR_CNT_FIXED + one reads_matched_per_db entry per index
 uint32_t place_counters(const smr_ctx* ctx) { return SMR_CNT_FIXED + std::max(1u, ctx->n_index_files); }
-
-// Places one run of a batch after what is placed: the resident batch's (map null), or a retry batch's through map (device array:
-// its read -> the resident batch's read).  As download_impl: a read flagged kOvfSlots fails the call with SMR_ERR_CAPACITY
-// (smr_aln_slots_needed), a trace back error with SMR_ERR_INDEX; `flagged` = the reads to retry.
-void place_run(smr_ctx* ctx, const Batch& b, const uint32_t* map, std::vector<uint32_t>& flagged) {
-  auto& P = ctx->pl;
-  flagged.clear();
-  const uint32_t n = b.nreads;
-  if (n == 0) return;
-  if (P.stats && !b.run_stats) fail(SMR_ERR_ARG, "a retry of the placed run computed no stats");
-  const uint32_t slots = slots_of(ctx), ncnt = place_counters(ctx);
-  uint64_t* words = ensure<uint64_t>(P.words, ((size_t)n + 1) * 8);
-  uint64_t* off = ensure<uint64_t>(P.off, ((size_t)n + 1) * 8);
-  PlaceWords* w = ensure<PlaceWords>(P.scal, sizeof(PlaceWords));
-  const PlaceIn in{(const ReadState*)b.state.p, (const uint32_t*)b.flags.p, (const uint16_t*)b.hit_db.p, (const OutAln*)b.out_aln.p,
-                   P.stats ? (const AlnStats*)b.aln_stats.p : nullptr, (const uint32_t*)b.cigar_pool.p, n, slots};
-  const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sm_count * 8);
-  CK(cudaMemsetAsync(w, 0, sizeof(PlaceWords), ctx->stream));
-  place_count_kernel<<<grid, 256, (size_t)ncnt * 8, ctx->stream>>>(in, (const unsigned long long*)b.counters.p, words, (unsigned long long*)P.cnt.p, ncnt, w);
-  CK(cudaGetLastError());
-  cub_run(ctx->cub_tmp, [&](void* t, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, words, off, (int)(n + 1), ctx->stream); });
-  PlaceWords hw{};
-  uint64_t total = 0;
-  CK(cudaMemcpyAsync(&hw, w, sizeof(hw), cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(&total, off + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  if (hw.need_slots) fail_need_slots(ctx, hw.need_slots, slots);
-  const uint64_t run = P.cig_words + total;
-  if (run >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, kCigarOffsetMsg);
-  if (hw.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
-  ensure_keep(ctx, P.cig, run * 4 + 16, P.cig_words * 4);
-  const PlaceOut o{(smr_read_result*)P.res.p, (smr_aln*)P.aln.p, P.stats ? (smr_aln_stats*)P.st.p : nullptr, (uint32_t*)P.cig.p, map, P.cig_words};
-  place_scatter_kernel<<<grid, 256, 0, ctx->stream>>>(in, off, o);
-  CK(cudaGetLastError());
-  P.cig_words = run;
-  if (hw.flagged) {   // rare: the flags come down only then
-    std::vector<uint32_t> fl(n);
-    CK(cudaMemcpyAsync(fl.data(), b.flags.p, (size_t)n * 4, cudaMemcpyDeviceToHost, ctx->stream));
-    CK(cudaStreamSynchronize(ctx->stream));
-    for (uint32_t r = 0; r < n; ++r) {
-      if (!fl[r]) continue;
-      flagged.push_back(r);
-      for (int bit = 0; bit < 6; ++bit) if (fl[r] & (1u << bit)) ctx->flag_hist[bit]++;
-    }
-  }
-}
-
-// Places the resident batch's last run and its retries (once per run: a later call finds them placed).  The retries compute the
-// stats when the run did, whatever smr_set_place_stats says now.
-void place_resident(smr_ctx* ctx) {
-  auto& P = ctx->pl;
-  const Batch& R = ctx->res.b;
-  if (R.run_id == 0) fail(SMR_ERR_ARG, "smr_place_results: the resident batch has not been run (smr_run_resident)");
-  if (R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, "smr_place_results: the resident batch was run at another stride: call smr_run_resident again");
-  if (P.run_id == R.run_id && !P.packed) return;
-  P.run_id = 0;
-  const uint32_t n = R.nreads, slots = slots_of(ctx), ncnt = place_counters(ctx);
-  P.nreads = n; P.slots = slots; P.stats = R.run_stats; P.packed = false; P.trace = false; P.cig_words = 0; P.n_alns = 0; P.t_place = 0;
-  ensure(P.res, (size_t)n * sizeof(smr_read_result) + 16);
-  ensure(P.aln, (size_t)n * slots * sizeof(smr_aln) + 16);
-  if (P.stats) ensure(P.st, (size_t)n * slots * sizeof(smr_aln_stats) + 16);
-  ensure(P.cig, 16);
-  ensure(P.cnt, (size_t)ncnt * 8);
-  CK(cudaMemsetAsync(P.cnt.p, 0, (size_t)ncnt * 8, ctx->stream));
-  ctx->t_run = R.run; ctx->t_d2h = 0;
-  const bool keep = ctx->place_stats;
-  const auto restore = on_exit([ctx, keep] { ctx->place_stats = keep; });
-  ctx->place_stats = P.stats;
-  cudaEvent_t* e = events(ctx, 2);
-  CK(cudaEventRecord(e[0], ctx->stream));
-  std::vector<uint32_t> flagged;
-  place_run(ctx, R, nullptr, flagged);
-  CK(cudaEventRecord(e[1], ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  P.t_place = elapsed_ms(e[0], e[1]);
-  if (!flagged.empty()) {
-    const auto release = on_exit([ctx] { release_retry_arenas(ctx); });
-    auto take = [&](const Batch& b, const uint32_t* map, std::vector<uint32_t>& again) {
-      DevBuf dmap;
-      upload_async(ctx, dmap, map, b.nreads);
-      place_run(ctx, b, (const uint32_t*)dmap.p, again);
-      CK(cudaStreamSynchronize(ctx->stream));   // before dmap and the batch free themselves
-    };
-    retry_flagged(ctx, R, flagged, nullptr, take, 0);
-  }
-  P.cnt_host.assign(ncnt, 0);
-  CK(cudaMemcpyAsync(P.cnt_host.data(), P.cnt.p, (size_t)ncnt * 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaStreamSynchronize(ctx->stream));
-  P.run_id = R.run_id;
-}
 
 // the placed arrays, as the report-side calls take them
 struct PlacedArrays {
@@ -1736,50 +1674,43 @@ struct PlacedArrays {
   uint64_t nslots;   // the alignment rows: n * stride, or packed the sum of n_align
 };
 
-// The placed results of the resident batch's last run for the _placed call `call`; need_stats: the call reads the stats.  In the
-// packed layout they are the packed placement of that run (smr_place_results_packed, or a packed download).
+// The placed results of the resident batch's last run for the _placed call `call`; need_stats: the call reads the stats.
 PlacedArrays placed_of(const smr_ctx* ctx, const char* call, bool need_stats) {
   const auto& P = ctx->pl;
-  const bool current = P.run_id != 0 && P.run_id == ctx->res.b.run_id;
-  if (packed(ctx)) {
-    if (!current || !P.packed)
+  if (P.run_id == 0 || P.run_id != ctx->res.b.run_id || P.packed != packed(ctx)) {
+    if (packed(ctx))
       fail(SMR_ERR_UNSUPPORTED, std::string(call) + ": no placed results of the resident batch's last run in the packed layout "
                                 "(smr_place_results places the strided layout only): call smr_place_results_packed after smr_run_resident, "
                                 "or download them (smr_download_results_packed) and pass them to the call that takes result arrays");
-    if (P.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
-    return PlacedArrays{(const smr_read_result*)P.res.p, (const smr_aln*)P.aln.p, (const uint32_t*)P.cig.p, P.cig_words,
-                        (const smr_aln_stats*)P.st.p, P.nreads, P.n_alns};
-  }
-  if (!current || P.packed)
     fail(SMR_ERR_ARG, std::string(call) + ": no placed results of the resident batch's last run: call smr_place_results after smr_run_resident");
-  if (P.slots != slots_of(ctx)) fail(SMR_ERR_ARG, std::string(call) + ": the results were placed at another stride");
+  }
+  if (P.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
+  if (!P.packed && P.slots != slots_of(ctx)) fail(SMR_ERR_ARG, std::string(call) + ": the results were placed at another stride");
   if (need_stats && !P.stats)
     fail(SMR_ERR_ARG, std::string(call) + ": the placed run computed no smr_aln_stats: call smr_set_place_stats(ctx, 1) before smr_run_resident");
   return PlacedArrays{(const smr_read_result*)P.res.p, (const smr_aln*)P.aln.p, (const uint32_t*)P.cig.p, P.cig_words,
-                      P.stats ? (const smr_aln_stats*)P.st.p : nullptr, P.nreads, (uint64_t)P.nreads * P.slots};
+                      P.stats ? (const smr_aln_stats*)P.st.p : nullptr, P.nreads, P.n_alns};
 }
 
-// ---------------------------------------------------------------------------------------------------------------------
-// packed results (SMR_ALNS_PACKED): read r's alignments at sum_{j<r} n_align(j), every read at its own count
-// ---------------------------------------------------------------------------------------------------------------------
 // The result buffers of a re-run sub-batch, kept on the device until the scatter; the rest of its batch (reads, seed scratch,
 // candidate work) frees itself when its re-runs are done, and the context's arenas are released after the last one.
 struct KeptRun { DevBuf state, hit_db, out_aln, aln_stats, cigar_pool, counters, aln_base; };
 
-// The runs of a packed placement: runs[0] is the resident batch's first run, runs[k] the re-run whose buffers are kept[k - 1].
+// The runs of a placement: runs[0] is the resident batch's first run, runs[k] the re-run whose buffers are kept[k - 1].
 // ctx->pl.src names, per read of the resident batch, the run and the read in it that hold its final results.
-struct PackedRuns {
+struct PlaceRuns {
   std::deque<KeptRun> kept;
   std::vector<PackRun> runs;
+  uint32_t reads = 0;          // the reads of all runs (the run-order CIGAR scan has one entry per read of each run)
   bool trace_error = false;
   uint64_t slot_reads = 0, slot_batches = 0; uint32_t slot_max = 0;   // re-runs for the alignment count (SMR_VERBOSE)
 };
 
-// a run as the placement reads it (its buffers stay where the run left them)
-PackRun pack_run_of(const Batch& b) {
+// a run as the placement reads it (its buffers stay where the run left them); first: its read 0's entry in the run-order scan
+PackRun pack_run_of(const Batch& b, uint32_t first) {
   return PackRun{(const ReadState*)b.state.p, (const uint16_t*)b.hit_db.p, (const OutAln*)b.out_aln.p, (const AlnStats*)b.aln_stats.p,
                  (const uint32_t*)b.cigar_pool.p, b.base.empty() ? nullptr : (const uint32_t*)b.aln_base.p,
-                 (const unsigned long long*)b.counters.p, b.run_slots, 0};
+                 (const unsigned long long*)b.counters.p, b.run_slots, first};
 }
 
 // the reads of a run that carry a flag, in read order: a compaction of its flags on the device (a scan of one bit per read), of
@@ -1808,123 +1739,100 @@ std::vector<PackFlag> flagged_reads(smr_ctx* ctx, const Batch& b) {
   return h;
 }
 
-// Reads idx[k] of batch `from` (map[k]: their index in the resident batch) run again as batches of their own at `scale`, read k
-// with room for cap[k] alignments, in sub-batches of at most ctx->retry_slots slots (a larger read alone).  Reads that store more
-// than their room run once more at their exact count; reads that overflow their scratch go on at 8x the scale, with room for
-// max(stride, the count they reached), for 3 scales at most.  Each sub-batch's unflagged reads become the source of their reads
-// (ctx->pl.src), and its result buffers are kept for the scatter; the rest of it frees itself when its re-runs are done.
-void rerun_packed(smr_ctx* ctx, const Batch& from, const std::vector<uint32_t>& idx, const std::vector<uint32_t>& cap,
-                  const std::vector<uint32_t>& map, uint32_t scale, int depth, bool for_slots, PackedRuns& P) {
-  if (idx.empty()) return;
-  if (depth > 3) fail(SMR_ERR_CAPACITY, "scratch overflow persists after 3 retries (" + std::to_string(idx.size()) + " reads)");
-  if (getenv("SMR_VERBOSE") && !for_slots) fprintf(stderr, "[smr] %zu reads overflowed their scratch: retrying with scale %u\n", idx.size(), scale);
-  const uint32_t S = slots_of(ctx);
-  for (size_t a = 0; a < idx.size();) {
-    size_t e = a;
-    uint64_t total = 0;
-    while (e < idx.size() && (e == a || total + cap[e] <= ctx->retry_slots)) total += cap[e++];
-    if (total >= (1ull << 31)) fail(SMR_ERR_CAPACITY, "a batch run again for its alignment count would hold 2^31 slots or more (a read that stores that many, or SMR_RETRY_SLOTS too large)");
-    const uint32_t n = (uint32_t)(e - a);
-    if (for_slots) { P.slot_reads += n; P.slot_batches += 1; for (size_t k = a; k < e; ++k) P.slot_max = std::max(P.slot_max, cap[k]); }
-    std::vector<uint32_t> src(n);
-    for (uint32_t k = 0; k < n; ++k) src[k] = from.off32[idx[a + k]];
-    Batch b;
-    b.scale = scale;
-    b.base.resize((size_t)n + 1, 0);
-    for (uint32_t k = 0; k < n; ++k) b.base[k + 1] = b.base[k] + cap[a + k];
-    const uint64_t w = read_layout(ctx, b, n, [&](uint32_t k) { return from.off32[idx[a + k] + 1] - src[k]; });
-    DevBuf d_src;
-    upload_async(ctx, d_src, src.data(), n);
-    ensure(b.seq04, b.total_nt + 64);
-    gather_reads_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
-        (const uint8_t*)from.seq04.p, (const uint32_t*)d_src.p, n, (const uint32_t*)b.seq_off.p, (uint8_t*)b.seq04.p);
-    CK(cudaGetLastError());
-    finish_upload(ctx, b, w);
-    run_impl(ctx, b);
-    ctx->t_run += b.run;
-    const uint32_t id = (uint32_t)P.runs.size();
-    DevBuf d_map;
-    upload_async(ctx, d_map, map.data() + a, n);
-    pack_src_kernel<<<std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
-        (const uint32_t*)b.flags.p, (const uint32_t*)d_map.p, n, id, (uint2*)ctx->pl.src.p);
-    CK(cudaGetLastError());
-    const std::vector<PackFlag> fl = flagged_reads(ctx, b);   // synchronises: d_map may free
-    P.runs.push_back(pack_run_of(b));
-    KeptRun& K = P.kept.emplace_back();
-    K.state = std::move(b.state); K.hit_db = std::move(b.hit_db); K.out_aln = std::move(b.out_aln); K.aln_stats = std::move(b.aln_stats);
-    K.cigar_pool = std::move(b.cigar_pool); K.counters = std::move(b.counters); K.aln_base = std::move(b.aln_base);
-    std::vector<uint32_t> s_idx, s_cap, s_map, x_idx, x_cap, x_map;
-    for (const PackFlag& f : fl) {
-      const uint32_t k = f.read, m = map[a + k];
-      if (f.flags & kErrTrace) P.trace_error = true;
-      if (f.flags == kOvfSlots) { s_idx.push_back(k); s_cap.push_back(f.n_align); s_map.push_back(m); }
-      else { x_idx.push_back(k); x_cap.push_back(std::max(S, f.n_align)); x_map.push_back(m); }
-    }
-    rerun_packed(ctx, b, s_idx, s_cap, s_map, scale, depth, true, P);          // the count is exact now
-    rerun_packed(ctx, b, x_idx, x_cap, x_map, scale * 8, depth + 1, false, P);
-    a = e;
-  }
-}
-
-// The packed results of the resident batch's last run, placed on the device in ctx->pl: the first run's results, every read that
-// stored more alignments than the stride run again at its own count and every read that overflowed its scratch run again at a
-// larger one, then all of them placed in read order (smr_place.cuh: a count pass over each read's source run, two scans, a warp
-// per read to scatter).  The resident batch and its device results stay as they are.
-void place_packed(smr_ctx* ctx) {
+// The results of the resident batch's last run, placed on the device in ctx->pl: the first run's results, and the flagged reads
+// run again by rerun_flagged, whose result buffers stay on the device; then every read placed from the run that completed it
+// (smr_place.cuh: a count pass over each read's source run, two scans, a group of lanes per read to scatter).  In the strided layout, as the
+// host download: a read flagged kOvfSlots fails the call with SMR_ERR_CAPACITY (smr_aln_slots_needed) and a trace back error with
+// SMR_ERR_INDEX, before anything is placed; in the packed layout a trace back error fails each call that reads the placement.  The
+// re-runs compute the stats when the first run did, whatever smr_set_place_stats says now.  The resident batch and its device
+// results stay as they are.
+void place(smr_ctx* ctx) {
   auto& P = ctx->pl;
   const Batch& R = ctx->res.b;
-  const uint32_t n = R.nreads, S = slots_of(ctx), ncnt = place_counters(ctx);
+  const bool pk = packed(ctx);
+  const uint32_t n = R.nreads, S = slots_of(ctx), ncnt = place_counters(ctx), stride = pk ? 0 : S;
   P.run_id = 0;
-  P.nreads = n; P.slots = S; P.stats = true; P.packed = true; P.trace = false; P.cig_words = 0; P.n_alns = 0; P.t_place = 0;
+  P.nreads = n; P.slots = S; P.stats = R.run_stats; P.packed = pk; P.trace = false; P.cig_words = 0; P.n_alns = 0; P.t_place = 0;
   P.cnt_host.assign(ncnt, 0);
   ctx->t_run = R.run; ctx->t_d2h = 0;
   if (n == 0) { P.t_run = ctx->t_run; P.run_id = R.run_id; return; }
+  const bool keep = ctx->place_stats;
+  const auto restore = on_exit([ctx, keep] { ctx->place_stats = keep; });
+  ctx->place_stats = P.stats;
   const uint32_t grid = std::min<uint32_t>((n + 255) / 256, (uint32_t)ctx->sm_count * 8);
   uint2* src = ensure<uint2>(P.src, (size_t)n * sizeof(uint2) + 16);
   pack_src_init_kernel<<<grid, 256, 0, ctx->stream>>>(src, n);
   CK(cudaGetLastError());
-  PackedRuns K;
-  K.runs.push_back(pack_run_of(R));
-  std::vector<uint32_t> s_idx, s_cap, x_idx, x_cap;
-  for (const PackFlag& f : flagged_reads(ctx, R)) {
-    if (f.flags & kErrTrace) K.trace_error = true;
-    if (f.flags == kOvfSlots) { s_idx.push_back(f.read); s_cap.push_back(f.n_align); }
-    else { x_idx.push_back(f.read); x_cap.push_back(std::max(S, f.n_align)); for (int bit = 0; bit < 6; ++bit) if (f.flags & (1u << bit)) ctx->flag_hist[bit]++; }
-  }
-  if (!s_idx.empty() || !x_idx.empty()) {
+  PlaceRuns K;
+  auto take = [&](const Batch& b, const std::vector<PackFlag>& fl) {   // b is run K.runs.size()
+    uint32_t need = 0;
+    for (const PackFlag& f : fl) {
+      if (f.flags & kErrTrace) K.trace_error = true;
+      if (!pk && (f.flags & kOvfSlots)) need = std::max(need, f.n_align);
+    }
+    if (need) fail_need_slots(ctx, need, S);
+    if (!pk && K.trace_error) fail(SMR_ERR_INDEX, kTraceErrorMsg);
+    K.runs.push_back(pack_run_of(b, K.reads));
+    K.reads += b.nreads;
+  };
+  const std::vector<PackFlag> flagged = flagged_reads(ctx, R);
+  take(R, flagged);
+  auto consume = [&](Batch& b, const uint32_t* map, bool exact) {
+    const uint32_t m = b.nreads;
+    DevBuf d_map;
+    upload_async(ctx, d_map, map, m);
+    pack_src_kernel<<<std::min<uint32_t>((m + 255) / 256, (uint32_t)ctx->sm_count * 8), 256, 0, ctx->stream>>>(
+        (const uint32_t*)b.flags.p, (const uint32_t*)d_map.p, m, (uint32_t)K.runs.size(), src);
+    CK(cudaGetLastError());
+    std::vector<PackFlag> fl = flagged_reads(ctx, b);   // synchronises: d_map may free
+    take(b, fl);
+    if (exact) {
+      K.slot_reads += m; K.slot_batches += 1;
+      for (uint32_t k = 0; k < m; ++k) K.slot_max = std::max(K.slot_max, b.base[k + 1] - b.base[k]);
+    }
+    KeptRun& k = K.kept.emplace_back();
+    k.state = std::move(b.state); k.hit_db = std::move(b.hit_db); k.out_aln = std::move(b.out_aln); k.aln_stats = std::move(b.aln_stats);
+    k.cigar_pool = std::move(b.cigar_pool); k.counters = std::move(b.counters); k.aln_base = std::move(b.aln_base);
+    return fl;
+  };
+  if (!flagged.empty()) {
     const auto release = on_exit([ctx] { release_retry_arenas(ctx); });
-    rerun_packed(ctx, R, s_idx, s_cap, s_idx, R.scale, 0, true, K);
-    rerun_packed(ctx, R, x_idx, x_cap, x_idx, R.scale * 8, 1, false, K);
+    rerun_flagged(ctx, R, flagged, nullptr, 0, consume);
   }
   if (K.slot_reads && getenv("SMR_VERBOSE"))
     fprintf(stderr, "[smr] packed results: %llu reads stored more than %u alignments and were run again at their own count in %llu sub-batches (largest count %u)\n",
             (unsigned long long)K.slot_reads, S, (unsigned long long)K.slot_batches, K.slot_max);
-  // count, scan, scatter
-  const uint32_t nruns = (uint32_t)K.runs.size();
+  // count, scan, scatter; the CIGAR words in read order (packed) or in run order (strided: one entry per read of each run)
+  const uint32_t nruns = (uint32_t)K.runs.size(), nw = pk ? n : K.reads;
   upload_async(ctx, P.runs, K.runs.data(), nruns);
   uint64_t* nal = ensure<uint64_t>(P.nal, ((size_t)n + 1) * 8);
-  uint64_t* words = ensure<uint64_t>(P.words, ((size_t)n + 1) * 8);
+  uint64_t* words = ensure<uint64_t>(P.words, ((size_t)nw + 1) * 8);
   uint64_t* aoff = ensure<uint64_t>(P.aoff, ((size_t)n + 1) * 8);
-  uint64_t* off = ensure<uint64_t>(P.off, ((size_t)n + 1) * 8);
+  uint64_t* off = ensure<uint64_t>(P.off, ((size_t)nw + 1) * 8);
   ensure(P.cnt, (size_t)ncnt * 8);
   cudaEvent_t* e = events(ctx, 2);
   CK(cudaEventRecord(e[0], ctx->stream));
   CK(cudaMemsetAsync(P.cnt.p, 0, (size_t)ncnt * 8, ctx->stream));
-  pack_count_kernel<<<grid, 256, (size_t)ncnt * 8, ctx->stream>>>((const PackRun*)P.runs.p, nruns, src, n, nal, words, (unsigned long long*)P.cnt.p, ncnt);
+  if (!pk) CK(cudaMemsetAsync(words, 0, ((size_t)nw + 1) * 8, ctx->stream));
+  pack_count_kernel<<<grid, 256, (size_t)ncnt * 8, ctx->stream>>>((const PackRun*)P.runs.p, nruns, src, n, stride, nal, words, (unsigned long long*)P.cnt.p, ncnt);
   CK(cudaGetLastError());
   cub_run(ctx->cub_tmp, [&](void* t, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, nal, aoff, (int)(n + 1), ctx->stream); });
-  cub_run(ctx->cub_tmp, [&](void* t, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, words, off, (int)(n + 1), ctx->stream); });
+  cub_run(ctx->cub_tmp, [&](void* t, size_t& bytes) { return cub::DeviceScan::ExclusiveSum(t, bytes, words, off, (int)(nw + 1), ctx->stream); });
   uint64_t tot[2] = {0, 0};
   CK(cudaMemcpyAsync(&tot[0], aoff + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
-  CK(cudaMemcpyAsync(&tot[1], off + n, 8, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaMemcpyAsync(&tot[1], off + nw, 8, cudaMemcpyDeviceToHost, ctx->stream));
   CK(cudaStreamSynchronize(ctx->stream));
   if (tot[1] >= 0xFFFFFFFFull) fail(SMR_ERR_CAPACITY, kCigarOffsetMsg);
   ensure(P.res, (size_t)n * sizeof(smr_read_result) + 16);
   ensure(P.aln, tot[0] * sizeof(smr_aln) + 16);
-  ensure(P.st, tot[0] * sizeof(smr_aln_stats) + 16);
+  if (P.stats) ensure(P.st, tot[0] * sizeof(smr_aln_stats) + 16);
   ensure(P.cig, tot[1] * 4 + 16);
-  const PackOut o{(smr_read_result*)P.res.p, (smr_aln*)P.aln.p, (smr_aln_stats*)P.st.p, (uint32_t*)P.cig.p, aoff, off};
-  pack_scatter_kernel<<<std::min<uint32_t>((n + 7) / 8, (uint32_t)ctx->sm_count * 16), 256, 0, ctx->stream>>>((const PackRun*)P.runs.p, src, n, o);
+  const PackOut o{(smr_read_result*)P.res.p, (smr_aln*)P.aln.p, P.stats ? (smr_aln_stats*)P.st.p : nullptr, (uint32_t*)P.cig.p, aoff, off};
+  uint32_t lg = 5;   // 2^lg lanes per read: a warp when packed, the stride rounded up to a power of two when strided
+  if (stride) for (lg = 0; (1u << lg) < stride && lg < 5; ++lg) {}
+  const uint32_t per_block = 8u << (5 - lg);
+  pack_scatter_kernel<<<std::min<uint32_t>((n + per_block - 1) / per_block, (uint32_t)ctx->sm_count * 16), 256, 0, ctx->stream>>>(
+      (const PackRun*)P.runs.p, src, n, stride, lg, o);
   CK(cudaGetLastError());
   CK(cudaEventRecord(e[1], ctx->stream));
   CK(cudaMemcpyAsync(P.cnt_host.data(), P.cnt.p, (size_t)ncnt * 8, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1934,15 +1842,17 @@ void place_packed(smr_ctx* ctx) {
   P.run_id = R.run_id;
 }
 
-// The packed placement of the resident batch's last run (once per run: a later call finds it placed).  `call` names the entry
-// point in its refusals.
-void place_packed_resident(smr_ctx* ctx, const char* call) {
+// The placement of the resident batch's last run in the context's layout (once per run: a later call finds it placed).  `call`
+// names the entry point in its refusals.
+void place_once(smr_ctx* ctx, const char* call) {
   const Batch& R = ctx->res.b;
   if (R.run_id == 0) fail(SMR_ERR_ARG, std::string(call) + ": the resident batch has not been run (smr_run_resident)");
-  if (!R.run_stats || R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, "the resident batch was not run in the packed layout at this stride: call smr_run_resident again");
+  if (packed(ctx) && (!R.run_stats || R.run_slots != slots_of(ctx)))
+    fail(SMR_ERR_ARG, "the resident batch was not run in the packed layout at this stride: call smr_run_resident again");
+  if (R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, std::string(call) + ": the resident batch was run at another stride: call smr_run_resident again");
   const auto& P = ctx->pl;
-  if (P.packed && P.run_id == R.run_id) { ctx->t_run = P.t_run; return; }
-  place_packed(ctx);
+  if (P.run_id == R.run_id && P.packed == packed(ctx)) { ctx->t_run = P.t_run; return; }
+  place(ctx);
 }
 
 struct PackedOut {
@@ -1951,14 +1861,13 @@ struct PackedOut {
   uint64_t aln_used = 0, cigar_used = 0;
 };
 
-// The packed download of the resident batch's last run: placed on the device once per run (place_packed), then copied.  Both sizes
+// The packed download of the resident batch's last run: placed on the device once per run (place_once), then copied.  Both sizes
 // are set before a capacity check can fail, and a call with arrays that large writes the same bytes.
 void download_packed(smr_ctx* ctx, PackedOut& out) {
   const Batch& R = ctx->res.b;
   ctx->t_run = R.run;
   if (R.nreads == 0) return;
-  if (!R.run_stats || R.run_slots != slots_of(ctx)) fail(SMR_ERR_ARG, "the resident batch was not run in the packed layout at this stride: call smr_run_resident again");
-  place_packed_resident(ctx, "smr_download_results_packed");
+  place_once(ctx, "smr_download_results_packed");
   const auto& P = ctx->pl;
   out.aln_used = P.n_alns; out.cigar_used = P.cig_words;
   if (out.aln_used > out.aln_cap)
@@ -3173,6 +3082,18 @@ int smr_set_place_stats(smr_ctx* ctx, int on) {
   return SMR_OK;
 }
 
+// smr_place_results[_packed] past their layout refusals
+static void place_results_impl(smr_ctx* ctx, const char* call, uint64_t* counters, uint32_t n_counters, uint64_t* n_alns, uint64_t* cigar_words) {
+  CK(cudaSetDevice(ctx->device));
+  place_once(ctx, call);
+  const auto& P = ctx->pl;
+  if (n_alns) *n_alns = P.n_alns;
+  if (cigar_words) *cigar_words = P.cig_words;
+  if (counters)
+    for (uint32_t k = 0; k < n_counters && k < P.cnt_host.size(); ++k) counters[k] += P.cnt_host[k];
+  if (P.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
+}
+
 int smr_place_results(smr_ctx* ctx, uint64_t* counters, uint32_t n_counters, uint64_t* n_alns, uint64_t* cigar_words) try {
   if (!ctx) return SMR_ERR_ARG;
   if (n_alns) *n_alns = 0;
@@ -3181,13 +3102,7 @@ int smr_place_results(smr_ctx* ctx, uint64_t* counters, uint32_t n_counters, uin
     ctx->err = "smr_place_results places the strided layout only: in the packed layout call smr_download_results_packed";
     return SMR_ERR_UNSUPPORTED;
   }
-  CK(cudaSetDevice(ctx->device));
-  place_resident(ctx);
-  const auto& P = ctx->pl;
-  if (n_alns) *n_alns = (uint64_t)P.nreads * P.slots;
-  if (cigar_words) *cigar_words = P.cig_words;
-  if (counters)
-    for (uint32_t k = 0; k < n_counters && k < P.cnt_host.size(); ++k) counters[k] += P.cnt_host[k];
+  place_results_impl(ctx, "smr_place_results", counters, n_counters, n_alns, cigar_words);
   return SMR_OK;
 } SMR_CATCH(ctx)
 
@@ -3199,14 +3114,7 @@ int smr_place_results_packed(smr_ctx* ctx, uint64_t* counters, uint32_t n_counte
     ctx->err = "smr_place_results_packed places the packed layout only: in the strided layout call smr_place_results";
     return SMR_ERR_ARG;
   }
-  CK(cudaSetDevice(ctx->device));
-  place_packed_resident(ctx, "smr_place_results_packed");
-  const auto& P = ctx->pl;
-  if (n_alns) *n_alns = P.n_alns;
-  if (cigar_words) *cigar_words = P.cig_words;
-  if (counters)
-    for (uint32_t k = 0; k < n_counters && k < P.cnt_host.size(); ++k) counters[k] += P.cnt_host[k];
-  if (P.trace) fail(SMR_ERR_INDEX, kTraceErrorMsg);
+  place_results_impl(ctx, "smr_place_results_packed", counters, n_counters, n_alns, cigar_words);
   return SMR_OK;
 } SMR_CATCH(ctx)
 

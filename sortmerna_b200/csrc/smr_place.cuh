@@ -1,114 +1,24 @@
-// Device placement of a run's results (smr_place_results): the strided run of a batch -> the caller's strided layout of
-// smr_download_results, written into device arrays the report-side calls read in place.  The bytes are those the host download
-// writes: smr_read_result[n], smr_aln[n * slots] zeroed past n_align, smr_aln_stats alike, and the CIGARs compacted in read order
-// from `base` (a scratch-overflow retry appends after the reads placed before it).  One count pass (CIGAR words per read and the
-// counters), one exclusive scan of the words, one scatter pass.  Reads flagged by the run (scratch overflow, kOvfSlots, trace
-// error) are skipped: their rows are written by the retry that runs them, or the placement fails.
+// Device placement of a run's results (smr_place_results, smr_place_results_packed, smr_download_results_packed): every read's
+// final results, from the resident batch's first run or from the re-run that completed it, placed on the device in the bytes the
+// caller's layout holds, for the report-side calls to read in place.  src[r] names the run and the read in it that hold read r's
+// results; the runs stay on the device until the scatter.  One count pass (rows and CIGAR words per read, the counters), two
+// exclusive scans (alignment offsets, CIGAR offsets), one scatter pass with a group of lanes per read (a warp when packed).
+// - packed layout (stride 0): read r's n_align alignments at sum_{j<r} n_align(j), the CIGARs compacted in read order.
+// - strided layout (stride S): read r's S rows at r * S, zeroed past n_align (stats alike), the CIGARs compacted in run order --
+//   the first run's reads, then each re-run's in the order they were made -- which is the order the host download writes them.
 #pragma once
 #include "smr_final.cuh"
 #include "../../include/smr_b200.h"
 
 namespace smr {
 
-// what the count pass hands to the host
-struct PlaceWords {
-  uint32_t trace;       // a read carries kErrTrace
-  uint32_t need_slots;  // the largest n_align of a read flagged kOvfSlots (0: none)
-  uint32_t flagged;     // reads flagged for a retry
-  uint32_t pad;
-};
-
-// one run of a batch, as the run left it on the device
-struct PlaceIn {
-  const ReadState* st; const uint32_t* flags; const uint16_t* hit_db; const OutAln* oa; const AlnStats* ast;   // ast: null = no stats
-  const uint32_t* cigar;   // the run's device CIGAR pool (OutAln::cigar_off indexes it)
-  uint32_t n, slots;
-};
-
-// words[r] = CIGAR words of read r (0 for a flagged read), words[n] = 0; counters into cnt[0 .. ncnt): SMR_CNT_NUM_ALIGNED and
-// reads_matched_per_db per read placed, and the run's device counters 1 .. dcCount - 1 (block 0).  Dynamic shared memory: ncnt u64.
-__global__ void __launch_bounds__(256) place_count_kernel(PlaceIn in, const unsigned long long* __restrict__ dev_cnt, uint64_t* __restrict__ words,
-                                                          unsigned long long* __restrict__ cnt, uint32_t ncnt, PlaceWords* __restrict__ w) {
-  extern __shared__ unsigned long long s_cnt[];
-  for (uint32_t k = threadIdx.x; k < ncnt; k += blockDim.x) s_cnt[k] = 0;
-  __syncthreads();
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < in.n; r += gridDim.x * blockDim.x) {
-    const uint32_t f = in.flags[r];
-    uint64_t sum = 0;
-    if (f) {
-      if (f & kErrTrace) atomicOr(&w->trace, 1u);
-      if (f & kOvfSlots) atomicMax(&w->need_slots, in.st[r].n_align);
-      else atomicAdd(&w->flagged, 1u);
-    } else {
-      const ReadState s = in.st[r];
-      const uint32_t na = min(s.n_align, in.slots);
-      for (uint32_t k = 0; k < na; ++k) sum += in.oa[(size_t)r * in.slots + k].cigar_len;
-      if (s.is_hit) {
-        atomicAdd(&s_cnt[SMR_CNT_NUM_ALIGNED], 1ull);
-        const uint16_t db = in.hit_db[r];
-        if (db != 0xFFFF && SMR_CNT_FIXED + (uint32_t)db < ncnt) atomicAdd(&s_cnt[SMR_CNT_FIXED + db], 1ull);
-      }
-    }
-    words[r] = sum;
-  }
-  if (blockIdx.x == 0 && threadIdx.x == 0) words[in.n] = 0;
-  __syncthreads();
-  for (uint32_t k = threadIdx.x; k < ncnt; k += blockDim.x) {
-    unsigned long long v = s_cnt[k];
-    if (blockIdx.x == 0 && k >= dcNumShort && k < dcCount) v += dev_cnt[k];
-    if (v) atomicAdd(&cnt[k], v);
-  }
-}
-
-// where the placed results go
-struct PlaceOut {
-  smr_read_result* res; smr_aln* aln; smr_aln_stats* st;   // st: null = no stats
-  uint32_t* cigar;
-  const uint32_t* map;     // read r of the run -> its row (null: r)
-  uint64_t base;           // the CIGAR words placed before this run
-};
-
-// one thread per read: its result, its `slots` alignment rows and its CIGARs at base + off[r]
-__global__ void __launch_bounds__(256) place_scatter_kernel(PlaceIn in, const uint64_t* __restrict__ off, PlaceOut o) {
-  for (uint32_t r = blockIdx.x * blockDim.x + threadIdx.x; r < in.n; r += gridDim.x * blockDim.x) {
-    if (in.flags[r]) continue;
-    const uint32_t dst = o.map ? o.map[r] : r;
-    const ReadState s = in.st[r];
-    smr_read_result x;
-    x.lastIndex = s.lastIndex; x.lastPart = s.lastPart; x.hit_seeds = s.hit_seeds; x.min_index = s.min_index; x.max_index = s.max_index;
-    x.n_align = s.n_align; x.max_SW_count = s.max_SW_count; x.is_done = s.is_done; x.is_hit = s.is_hit;
-    o.res[dst] = x;
-    uint64_t at = o.base + off[r];
-    for (uint32_t k = 0; k < in.slots; ++k) {
-      const size_t src = (size_t)r * in.slots + k, to = (size_t)dst * in.slots + k;
-      smr_aln a = {};
-      smr_aln_stats t = {};
-      if (k < s.n_align) {
-        const OutAln d = in.oa[src];
-        for (uint32_t j = 0; j < d.cigar_len; ++j) o.cigar[at + j] = in.cigar[d.cigar_off + j];
-        a.cigar_off = (uint32_t)at; a.cigar_len = d.cigar_len; at += d.cigar_len;
-        a.ref_num = d.ref_num; a.ref_begin1 = d.ref_begin1; a.ref_end1 = d.ref_end1; a.read_begin1 = d.read_begin1; a.read_end1 = d.read_end1;
-        a.readlen = d.readlen; a.score1 = d.score1; a.part = d.part; a.index_num = d.index_num; a.strand = d.strand;
-        if (o.st) { const AlnStats q = in.ast[src]; t = smr_aln_stats{q.n_miss, q.n_gap, q.n_match, q.n_match_denovo}; }
-      }
-      o.aln[to] = a;
-      if (o.st) o.st[to] = t;
-    }
-  }
-}
-
-// ---------------------------------------------------------------------------------------------------------------------
-// Packed placement (smr_place_results_packed, smr_download_results_packed): every read's final results, from the first run
-// (strided at the first stride) or from the re-run that stored it at its own count, placed in read order with no stride:
-// smr_aln[sum n_align] and smr_aln_stats alike, aln_off[n + 1], the CIGARs compacted in read order.  The runs stay on the device
-// until the scatter; src[r] names the run and the read in it that hold read r's results.
-// ---------------------------------------------------------------------------------------------------------------------
-// one run of a packed placement, as the run left it on the device
+// one run of a placement, as the run left it on the device
 struct PackRun {
   const ReadState* st; const uint16_t* hit_db; const OutAln* oa; const AlnStats* ast; const uint32_t* cigar;
   const uint32_t* base;        // read k's first slot (a re-run's packed arenas); null: k * slots
   const unsigned long long* cnt;   // the run's device counters
-  uint32_t slots, pad;
+  uint32_t slots;
+  uint32_t first;              // strided layout: the entry of its read 0 in the run-order CIGAR scan
 };
 
 // a read flagged by a run, as the host forms the re-runs from it
@@ -140,11 +50,12 @@ __global__ void __launch_bounds__(256) pack_src_kernel(const uint32_t* __restric
     if (!flags[k]) src[map[k]] = make_uint2(run, k);
 }
 
-// nal[r] = n_align and words[r] = CIGAR words of read r from its source run, nal[n] = words[n] = 0; counters into cnt[0 .. ncnt):
-// SMR_CNT_NUM_ALIGNED and reads_matched_per_db once per read, and the device counters 1 .. dcCount - 1 of every run (block 0).
-// Dynamic shared memory: ncnt u64.
+// nal[r] = the rows of read r (stride 0: its n_align; else the stride), nal[n] = 0; the CIGAR words of read r from its source run
+// into words[r] (stride 0; words[n] = 0) or words[first + read in its run] (strided: words is zeroed, of sum of run sizes + 1
+// entries); counters into cnt[0 .. ncnt): SMR_CNT_NUM_ALIGNED and reads_matched_per_db once per read, and the device counters
+// 1 .. dcCount - 1 of every run (block 0).  Dynamic shared memory: ncnt u64.
 __global__ void __launch_bounds__(256) pack_count_kernel(const PackRun* __restrict__ runs, uint32_t nruns, const uint2* __restrict__ src,
-                                                         uint32_t n, uint64_t* __restrict__ nal, uint64_t* __restrict__ words,
+                                                         uint32_t n, uint32_t stride, uint64_t* __restrict__ nal, uint64_t* __restrict__ words,
                                                          unsigned long long* __restrict__ cnt, uint32_t ncnt) {
   extern __shared__ unsigned long long s_cnt[];
   for (uint32_t k = threadIdx.x; k < ncnt; k += blockDim.x) s_cnt[k] = 0;
@@ -154,17 +65,18 @@ __global__ void __launch_bounds__(256) pack_count_kernel(const PackRun* __restri
     const PackRun& d = runs[s.x];
     const ReadState st = d.st[s.y];
     const size_t b = d.base ? (size_t)d.base[s.y] : (size_t)s.y * d.slots;
+    const uint32_t na = stride ? min(st.n_align, stride) : st.n_align;
     uint64_t sum = 0;
-    for (uint32_t j = 0; j < st.n_align; ++j) sum += d.oa[b + j].cigar_len;
-    nal[r] = st.n_align;
-    words[r] = sum;
+    for (uint32_t j = 0; j < na; ++j) sum += d.oa[b + j].cigar_len;
+    nal[r] = stride ? stride : st.n_align;
+    words[stride ? (size_t)d.first + s.y : r] = sum;
     if (st.is_hit) {
       atomicAdd(&s_cnt[SMR_CNT_NUM_ALIGNED], 1ull);
       const uint16_t db = d.hit_db[s.y];
       if (db != 0xFFFF && SMR_CNT_FIXED + (uint32_t)db < ncnt) atomicAdd(&s_cnt[SMR_CNT_FIXED + db], 1ull);
     }
   }
-  if (blockIdx.x == 0 && threadIdx.x == 0) { nal[n] = 0; words[n] = 0; }
+  if (blockIdx.x == 0 && threadIdx.x == 0) { nal[n] = 0; if (!stride) words[n] = 0; }
   __syncthreads();
   if (blockIdx.x == 0) {
     constexpr uint32_t kw = dcCount - dcNumShort;
@@ -178,40 +90,46 @@ __global__ void __launch_bounds__(256) pack_count_kernel(const PackRun* __restri
     if (s_cnt[k]) atomicAdd(&cnt[k], s_cnt[k]);
 }
 
-// where the packed results go
+// where the placed results go
 struct PackOut {
-  smr_read_result* res; smr_aln* aln; smr_aln_stats* st; uint32_t* cigar;
-  const uint64_t* aln_off;   // read r's first alignment (the scan of n_align)
-  const uint64_t* cig_off;   // read r's first CIGAR word (the scan of its words)
+  smr_read_result* res; smr_aln* aln; smr_aln_stats* st; uint32_t* cigar;   // st: null = no stats
+  const uint64_t* aln_off;   // read r's first row (the scan of nal)
+  const uint64_t* cig_off;   // read r's first CIGAR word (the scan of words, indexed as pack_count_kernel wrote it)
 };
 
-// One warp per read: lane 0 writes its result; the lanes take its alignments 32 at a time, each placing one alignment, its stats
-// and its CIGAR words after those of the lanes before it (a warp scan of cigar_len).  A read may hold thousands of alignments.
+// A group of G = 2^lg lanes per read (32 in the packed layout, where a read may hold thousands of alignments; in the
+// strided layout the smallest power of two >= the stride, up to 32), 32 / G reads per warp pass.  The group's first lane writes
+// its result; the lanes take its rows G at a time, each placing one alignment, its stats and its CIGAR words after those of the
+// lanes before it (a scan of cigar_len over the group), or zeros past n_align (strided).  stride: as pack_count_kernel.
 __global__ void __launch_bounds__(256) pack_scatter_kernel(const PackRun* __restrict__ runs, const uint2* __restrict__ src, uint32_t n,
-                                                           PackOut o) {
-  const uint32_t lane = threadIdx.x & 31, warps = gridDim.x * (blockDim.x >> 5);
-  for (uint32_t r = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5); r < n; r += warps) {
+                                                           uint32_t stride, uint32_t lg, PackOut o) {
+  const uint32_t G = 1u << lg, lane = threadIdx.x & 31, q = lane & (G - 1), per = 32u >> lg;
+  const uint32_t warps = gridDim.x * (blockDim.x >> 5);
+  for (uint32_t r0 = (blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5)) * per; r0 < n; r0 += warps * per) {   // warp-uniform
+    const bool live = r0 + (lane >> lg) < n;   // a group past the last read takes part in the shuffles with no rows to write
+    const uint32_t r = min(r0 + (lane >> lg), n - 1);
     const uint2 s = src[r];
     const PackRun& d = runs[s.x];
     const ReadState st = d.st[s.y];
-    if (lane == 0) {
+    if (live && q == 0) {
       smr_read_result x;
       x.lastIndex = st.lastIndex; x.lastPart = st.lastPart; x.hit_seeds = st.hit_seeds; x.min_index = st.min_index; x.max_index = st.max_index;
       x.n_align = st.n_align; x.max_SW_count = st.max_SW_count; x.is_done = st.is_done; x.is_hit = st.is_hit;
       o.res[r] = x;
     }
     const size_t b = d.base ? (size_t)d.base[s.y] : (size_t)s.y * d.slots;
+    const uint32_t na = !live ? 0 : stride ? min(st.n_align, stride) : st.n_align, rows = stride ? stride : st.n_align;   // rows: uniform over the warp
     const uint64_t to = o.aln_off[r];
-    uint64_t at = o.cig_off[r];
-    for (uint32_t j0 = 0; j0 < st.n_align; j0 += 32) {
-      const uint32_t j = j0 + lane;
-      const uint32_t len = j < st.n_align ? d.oa[b + j].cigar_len : 0;
+    uint64_t at = o.cig_off[stride ? (size_t)d.first + s.y : r];
+    for (uint32_t j0 = 0; j0 < rows; j0 += G) {
+      const uint32_t j = j0 + q;
+      const uint32_t len = j < na ? d.oa[b + j].cigar_len : 0;
       uint32_t incl = len;
-      for (uint32_t k = 1; k < 32; k <<= 1) {
-        const uint32_t v = __shfl_up_sync(0xffffffffu, incl, k);
-        if (lane >= k) incl += v;
+      for (uint32_t k = 1; k < G; k <<= 1) {
+        const uint32_t v = __shfl_up_sync(0xffffffffu, incl, k, G);
+        if (q >= k) incl += v;
       }
-      if (j < st.n_align) {
+      if (j < na) {
         const OutAln a = d.oa[b + j];
         const uint64_t c = at + incl - len;
         for (uint32_t w = 0; w < a.cigar_len; ++w) o.cigar[c + w] = d.cigar[a.cigar_off + w];
@@ -220,9 +138,12 @@ __global__ void __launch_bounds__(256) pack_scatter_kernel(const PackRun* __rest
         x.ref_num = a.ref_num; x.ref_begin1 = a.ref_begin1; x.ref_end1 = a.ref_end1; x.read_begin1 = a.read_begin1; x.read_end1 = a.read_end1;
         x.readlen = a.readlen; x.score1 = a.score1; x.part = a.part; x.index_num = a.index_num; x.strand = a.strand;
         o.aln[to + j] = x;
-        if (o.st) { const AlnStats q = d.ast[b + j]; o.st[to + j] = smr_aln_stats{q.n_miss, q.n_gap, q.n_match, q.n_match_denovo}; }
+        if (o.st) { const AlnStats q2 = d.ast[b + j]; o.st[to + j] = smr_aln_stats{q2.n_miss, q2.n_gap, q2.n_match, q2.n_match_denovo}; }
+      } else if (live && j < rows) {
+        o.aln[to + j] = smr_aln{};
+        if (o.st) o.st[to + j] = smr_aln_stats{};
       }
-      at += __shfl_sync(0xffffffffu, incl, 31);
+      at += __shfl_sync(0xffffffffu, incl, G - 1, G);
     }
   }
 }

@@ -138,7 +138,7 @@ def test_golden_cases(golden, case, layout, capfd, monkeypatch):
         assert ng == (2 if per == 1 else 1)
         capfd.readouterr()
         got = a.align(b.cat, b.off, with_stats=True)
-        seed_ovf = ng > 1 and re.search(r"causes so far: lane [1-9]|region [1-9]|overflowed their scratch: retrying", capfd.readouterr().err) is not None
+        seed_ovf = ng > 1 and re.search(r"causes so far: lane [1-9]|region [1-9]|overflowed their scratch at scale", capfd.readouterr().err) is not None
         assert_same(got, want, (case, layout, per), seed_ovf)
         if layout == "strided":
             rows = hostio.format_sam_rows(b, golden["refs"], got["res"], got["alns"], got["cigar"], got["slots"])

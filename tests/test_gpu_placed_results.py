@@ -176,6 +176,33 @@ def test_placed_with_scratch_overflow_retries(capfd):
         shutil.rmtree(d, ignore_errors=True)
 
 
+def test_placed_with_scratch_overflow_retries_in_sub_batches(monkeypatch, capfd):
+    """the same reads with sub-batches of 2 slots: the retries run as several batches, and the placement writes their CIGARs in the
+    order the download does"""
+    d = tempfile.mkdtemp(prefix="smr_place_ovf_")
+    monkeypatch.setenv("SMR_RETRY_SLOTS", "2")   # read when the context is made
+    al = api.Aligner(0)
+    try:
+        fasta, fq = _overflow_inputs(d)
+        al.set_params(api.default_params())
+        al.build_index_device(0, fasta, hostio.load_references(fasta), 60)
+        al.upload_fastx(open(fq, "rb").read())
+        monkeypatch.setenv("SMR_VERBOSE", "1")
+        _run(al)
+        capfd.readouterr()
+        al.place()
+        placed = capfd.readouterr().err
+        got = _assert_placed_equals_download(al)   # place() finds the placement made; download() retries the same reads
+        downloaded = capfd.readouterr().err
+        monkeypatch.delenv("SMR_VERBOSE")
+        line = "reads overflowed their scratch at scale 1: retrying"
+        assert placed.count(line) > 1 and downloaded.count(line) == placed.count(line), placed[-2000:]
+        assert int(got["res"]["is_hit"].sum()) > 0
+    finally:
+        al.close()
+        shutil.rmtree(d, ignore_errors=True)
+
+
 # -- the report side: each _placed call against its host-array twin
 GUMBEL = [(0.594908, 0.326193), (0.600371, 0.328947)]
 
