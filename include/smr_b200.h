@@ -533,6 +533,32 @@ int smr_format_bam_placed(smr_ctx*, const smr_report_opts* opts, char* out, uint
  * ref_num) order, the refIDs of smr_format_bam_placed.  Names from smr_set_report_refs (SMR_ERR_ARG for a part without them),
  * lengths from the resident reference offsets.  *out_bytes = the size; if out is null or cap is smaller, SMR_ERR_CAPACITY. */
 int smr_bam_header(smr_ctx*, const char* text, uint64_t nbytes, char* out, uint64_t cap, uint64_t* out_bytes);
+/* Coordinate-sorted aligned.bam and aligned.bam.bai (SAMv1 4, 5.2; not a reference output).  The records of smr_format_bam_placed,
+ * stably sorted by samtools' coordinate key refID << 32 | (pos + 1) << 1 | reverse strand, so equal keys keep the order of the
+ * unsorted file (batch, then the writer's row order).  The file: smr_bam_header's blocks with the text's SO:unsorted made
+ * SO:coordinate, the windows' blocks in order, the BGZF EOF block.
+ * begin: opens the accumulator (again: the open one is discarded).  SMR_ERR_UNSUPPORTED, naming it, for a reference of 2^29 bases
+ *   or more, which BAI cannot address; SMR_ERR_ARG for a part without smr_set_report_refs.
+ * add_placed: the placed batch's records (opts and refusals as smr_format_bam_placed) sorted into one run, uncompressed, into out;
+ *   *nbytes = its size.  The run's keys and sizes go to the accumulator on the device (12 B per record).  If out is null or cap is
+ *   smaller, SMR_ERR_CAPACITY with *nbytes set and the accumulator unchanged; a retry gives the same bytes and appends once.
+ * plan: one stable sort of every run's records; windows of whole records of at most window_bytes each (a larger record alone) cut
+ *   greedily; *n_windows = their number, and ranges[(w * runs + r) * 2 .. + 1] = [lo, hi), the bytes of run r (from the run's start)
+ *   that window w holds (lo = hi = 0 for none).  header_bytes = the size of the header blocks, the compressed offset of the first
+ *   window's.  SMR_ERR_CAPACITY if ranges is null or cap (uint64 entries) is below n_windows * runs * 2.
+ * window: w = 0, 1, ... in order; staged = window w's ranges of the runs concatenated in run order (nbytes their sum, SMR_ERR_ARG
+ *   otherwise, or when a record's block_size disagrees with the runs added).  Its records in sorted order, cut into BGZF blocks of
+ *   65,280 bytes and the rest, into out; *out_bytes = their size (SMR_ERR_CAPACITY as smr_bam_header, the window not done).
+ * index: after the last window, the BAI bytes into out (*nbytes = the size; SMR_ERR_CAPACITY as above): every reference, bins
+ *   ascending with their chunks merged when one starts in the block where the one before ends, the pseudo-bin 37450, the linear index
+ *   of 16 kb windows, n_no_coor = 0.  Closes the accumulator.
+ * SMR_ERR_ARG without an open accumulator, before plan, out of order, and after an index part was loaded or its report ids set since
+ * begin.  add_placed and window set smr_last_report_timings. */
+int smr_bam_sort_begin(smr_ctx*);
+int smr_bam_sort_add_placed(smr_ctx*, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* nbytes);
+int smr_bam_sort_plan(smr_ctx*, uint64_t window_bytes, uint64_t header_bytes, uint64_t* ranges, uint64_t cap, uint64_t* n_windows);
+int smr_bam_sort_window(smr_ctx*, uint64_t w, const void* staged, uint64_t nbytes, char* out, uint64_t cap, uint64_t* out_bytes);
+int smr_bam_sort_index(smr_ctx*, char* out, uint64_t cap, uint64_t* nbytes);
 int smr_otu_add_placed(smr_ctx*, uint64_t* n_added);
 int smr_denovo_stats_placed(smr_ctx*, const smr_denovo_opts* opts, uint32_t* per_read, uint64_t totals[4]);
 

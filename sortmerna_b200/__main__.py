@@ -19,7 +19,8 @@ aligned.log).  Options take the reference's names and meanings; any other option
   -fastx -other -sam -SQ    aligned.<fq|fa>, other.<fq|fa>, aligned.sam, its @SQ lines
   -blast 'F [cols]'     aligned.blast: 1 (tabular, optional columns cigar qcov qstrand) or 0 (pairwise)
   -zip-out [1|0|-1]     compress the report files (-1, the default: as the first reads file is)
-  -bam                  aligned.bam: the rows of aligned.sam as BAM (BGZF); not a reference option
+  -bam | -bam_sorted    aligned.bam: the rows of aligned.sam as BAM (BGZF); not a reference option
+                        with -bam_sorted: sorted by coordinate, and its index aligned.bam.bai; not a reference option either
  alignment
   -num_alignments N -no-best -min_lis N -num_seeds N -passes L1,L2,L3 -edges N[%] -full_search -F -R -e EVALUE
  scoring
@@ -37,7 +38,7 @@ aligned.log).  Options take the reference's names and meanings; any other option
   -minimal_score N      the minimal Smith-Waterman score of each -ref (once per -ref), instead of the one computed from -e
 """
 
-FLAGS = {"fastx", "other", "sam", "bam", "SQ", "no-best", "full_search", "F", "R", "paired_in", "paired_out", "out2", "sout", "otu_map",
+FLAGS = {"fastx", "other", "sam", "bam", "bam_sorted", "SQ", "no-best", "full_search", "F", "R", "paired_in", "paired_out", "out2", "sout", "otu_map",
          "de_novo_otu", "h", "help"}
 VALUES = {"ref", "reads", "workdir", "blast", "num_alignments", "min_lis", "num_seeds", "passes", "edges", "e", "match", "mismatch",
           "gap_open", "gap_ext", "N", "id", "coverage", "L", "interval", "max_pos", "m", "threads", "gumbel", "minimal_score"}
@@ -157,7 +158,7 @@ def parse_args(argv: list) -> dict:
         min_id = 0.97 if otu_map else 0.0
     if min_cov < 0:
         min_cov = 0.97 if otu_map else 0.0
-    fastx, sam, bam, blast = has("fastx") or paired_in or paired_out, has("sam"), has("bam"), one("blast")
+    fastx, sam, bam, blast = has("fastx") or paired_in or paired_out, has("sam"), has("bam") or has("bam_sorted"), one("blast")
     if not (fastx or blast is not None or sam or bam or otu_map or has("de_novo_otu")):
         blast = "1"   # the reference's default output
     if has("num_alignments") and not (blast is not None or sam or bam or fastx):
@@ -210,7 +211,7 @@ def parse_args(argv: list) -> dict:
         evalue = 1.0
     workdir = one("workdir", os.path.join(os.path.expanduser("~"), "sortmerna", "run"))
     return dict(refs=refs, reads=reads, out_dir=os.path.join(workdir, "out"), workdir=workdir, params=p, gumbel=gumbel, minimal_score=ms,
-                evalue=evalue, sam=sam, bam=bam, sq=has("SQ"), blast=blast, fastx=fastx, other=has("other"),
+                evalue=evalue, sam=sam, bam=bam, bam_sorted=has("bam_sorted"), sq=has("SQ"), blast=blast, fastx=fastx, other=has("other"),
                 denovo=(min_id, min_cov) if has("de_novo_otu") else None, otu_map=(min_id, min_cov) if otu_map else None,
                 paired_in=paired_in, paired_out=paired_out, out2=has("out2") and paired, sout=has("sout") and paired,
                 zip_out=zip_flag == 1 or (zip_flag == -1 and _is_gz(reads[0])), lnwin=lnwin,

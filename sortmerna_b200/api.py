@@ -35,10 +35,15 @@ SYMBOLS = ["smr_init", "smr_destroy", "smr_last_error", "smr_device_count", "smr
            "smr_set_index_budget", "smr_index_residency", "smr_set_place_stats", "smr_place_results", "smr_download_placed",
            "smr_last_place_timing", "smr_format_reports_placed", "smr_format_reports_placed_gz", "smr_format_blast_pairwise_placed",
            "smr_format_blast_pairwise_placed_gz", "smr_otu_add_placed", "smr_denovo_stats_placed",
-           "smr_place_results_packed", "smr_format_bam_placed", "smr_bam_header"]
+           "smr_place_results_packed", "smr_format_bam_placed", "smr_bam_header", "smr_bam_sort_begin", "smr_bam_sort_add_placed",
+           "smr_bam_sort_plan", "smr_bam_sort_window", "smr_bam_sort_index"]
 
 # the BGZF end-of-file marker (SAMv1 4.1.2): an empty BGZF block, written once at the end of a BAM file
 BGZF_EOF = bytes.fromhex("1f8b08040000000000ff0600424302001b0003000000000000000000")
+# the coordinate-sorted aligned.bam (Aligner.bam_sort_*): the bytes of records run_files compresses per window, and the BGZF bounds
+# (smr_deflate.h: kBgzfBlock input bytes per block, at most kBgzfMaxMember bytes per member)
+BAM_SORT_WINDOW = 256 << 20
+BGZF_BLOCK, BAM_MAX_MEMBER = 65280, 65321
 
 # smr_set_aln_layout: strided, nreads * slots alignments; packed, read r's n_align alignments from the sum of the counts before it
 ALN_LAYOUTS = {"strided": 0, "packed": 1}
@@ -788,6 +793,91 @@ class Aligner:
         self._check(rc, "smr_bam_header")
         return o[:nb.value].tobytes()
 
+    # ---- coordinate-sorted BAM (smr_bam_sort_*) ----
+    def bam_sort_begin(self):
+        """smr_bam_sort_begin: opens the accumulator of a coordinate-sorted aligned.bam (again: the open one is discarded)"""
+        self._upload_report_refs()
+        self._check(self.L.smr_bam_sort_begin(self.h), "smr_bam_sort_begin")
+
+    def bam_sort_add(self, opts: ReportOpts, buf: np.ndarray):
+        """smr_bam_sort_add_placed: the placed batch's BAM records (opts = report_opts(sam=True, ...)) sorted into one run,
+        uncompressed, into `buf` (a uint8 array, grown when the run does not fit) -> (buf, nbytes).  The caller keeps the runs (for
+        bam_sort_finish); the accumulator keeps their keys and sizes."""
+        nb = C.c_uint64(0)
+        fn = self.L.smr_bam_sort_add_placed
+        fn.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        rc = fn(self.h, C.cast(C.byref(opts), C.c_void_p), _ptr(buf), buf.size, C.cast(C.byref(nb), C.c_void_p))
+        if rc == 5 and nb.value > buf.size:   # SMR_ERR_CAPACITY: nb names the size; grow and run again
+            buf = np.empty(nb.value + (nb.value >> 3), np.uint8)
+            rc = fn(self.h, C.cast(C.byref(opts), C.c_void_p), _ptr(buf), buf.size, C.cast(C.byref(nb), C.c_void_p))
+        self._check(rc, "smr_bam_sort_add_placed")
+        return buf, nb.value
+
+    def bam_sort_finish(self, runs, run_starts, out, header_bytes: int, window_bytes: int = BAM_SORT_WINDOW) -> bytes:
+        """The end of a sorted aligned.bam: smr_bam_sort_plan, then every window (smr_bam_sort_window) with its ranges read from
+        `runs` (a binary file holding the runs of bam_sort_add, run r from byte run_starts[r]) and its BGZF blocks written to `out`
+        (a binary file, after the header_bytes of the header blocks), then smr_bam_sort_index.  Returns the BAI bytes; the caller
+        writes the EOF block.  self.bam_sort_seconds: plan, read (the runs file), upload, device (gather, compress, index pass),
+        d2h, write, index, and windows."""
+        import time
+        sec = dict.fromkeys(("plan", "read", "upload", "device", "d2h", "write", "index"), 0.0)
+        t0 = time.perf_counter()
+        R = len(run_starts)
+        nw, ranges = C.c_uint64(0), np.zeros(0, np.uint64)
+        plan = self.L.smr_bam_sort_plan
+        plan.argtypes = [C.c_void_p, C.c_uint64, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
+        rc = plan(self.h, window_bytes, header_bytes, None, 0, C.cast(C.byref(nw), C.c_void_p))
+        if rc == 5:   # SMR_ERR_CAPACITY: nw names the windows
+            ranges = np.zeros(nw.value * R * 2, np.uint64)
+            rc = plan(self.h, window_bytes, header_bytes, _ptr(ranges), ranges.size, C.cast(C.byref(nw), C.c_void_p))
+        self._check(rc, "smr_bam_sort_plan")
+        n_win = nw.value
+        ranges = ranges.reshape(n_win, R, 2) if n_win else np.zeros((0, R, 2), np.uint64)
+        sec["plan"] = time.perf_counter() - t0
+        win = self.L.smr_bam_sort_window
+        win.argtypes = [C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p, C.c_uint64, C.c_void_p]
+        staged, ob = np.empty(0, np.uint8), np.empty(0, np.uint8)
+        for w in range(n_win):
+            t0 = time.perf_counter()
+            n = int((ranges[w, :, 1] - ranges[w, :, 0]).sum())
+            if staged.size < n:
+                staged = np.empty(n, np.uint8)
+            mv, at = memoryview(staged), 0
+            for r in range(R):
+                lo, hi = int(ranges[w, r, 0]), int(ranges[w, r, 1])
+                if hi > lo:
+                    runs.seek(int(run_starts[r]) + lo)
+                    if runs.readinto(mv[at:at + hi - lo]) != hi - lo:
+                        raise SmrError(f"bam_sort_finish: the runs file ends inside run {r}")
+                    at += hi - lo
+            t1 = time.perf_counter()
+            cap = -(-n // BGZF_BLOCK) * BAM_MAX_MEMBER + 64   # the stored fallback bounds every member
+            if ob.size < cap:
+                ob = np.empty(cap, np.uint8)
+            nb = C.c_uint64(0)
+            self._check(win(self.h, w, _ptr(staged), n, _ptr(ob), ob.size, C.cast(C.byref(nb), C.c_void_p)), "smr_bam_sort_window")
+            tm = self.report_timings()
+            t2 = time.perf_counter()
+            out.write(memoryview(ob)[:nb.value])
+            sec["read"] += t1 - t0
+            sec["upload"] += tm["h2d_ms"] / 1e3
+            sec["device"] += tm["device_ms"] / 1e3
+            sec["d2h"] += tm["d2h_ms"] / 1e3
+            sec["write"] += time.perf_counter() - t2
+        t0 = time.perf_counter()
+        idx = self.L.smr_bam_sort_index
+        idx.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, C.c_void_p]
+        nb, bai = C.c_uint64(0), np.zeros(0, np.uint8)
+        rc = idx(self.h, None, 0, C.cast(C.byref(nb), C.c_void_p))
+        if rc == 5:   # SMR_ERR_CAPACITY: nb names the size
+            bai = np.zeros(nb.value, np.uint8)
+            rc = idx(self.h, _ptr(bai), bai.size, C.cast(C.byref(nb), C.c_void_p))
+        self._check(rc, "smr_bam_sort_index")
+        sec["index"] = time.perf_counter() - t0
+        sec["windows"] = n_win
+        self.bam_sort_seconds = sec
+        return bai[:nb.value].tobytes()
+
     def format_reports(self, out: dict, text: bytes | None = None, opts: ReportOpts | None = None, gzip: bool = False, **kw) -> dict:
         """smr_format_reports: the report streams of one batch as bytes.  out = what align(with_stats=True) / download(with_stats=True)
         returned for it; text = the batch's FASTA / FASTQ bytes (None: the resident text of upload_fastx[_gz]); opts = report_opts(...)
@@ -1221,7 +1311,8 @@ class _FileWriter:
 
 def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, minimal_score=None, evalue: float = 1.0, sam: bool = False,
               sq: bool = False, blast=None, fastx: bool = False, other: bool = False, denovo=None, otu_map=None, paired_in: bool = False,
-              paired_out: bool = False, out2: bool = False, sout: bool = False, zip_out: bool = False, bam: bool = False, lnwin: int = 18, interval: int = 1,
+              paired_out: bool = False, out2: bool = False, sout: bool = False, zip_out: bool = False, bam: bool = False, bam_sorted: bool = False,
+              lnwin: int = 18, interval: int = 1,
               max_pos: int = 10000, max_mb: float = 3072.0, skiplengths=None, index_budget: int = 0, batch_bytes: int = 256 << 20,
               piece_bytes: int = 256 << 20, cmd: str = "", threads: int = 1, device: int = 0) -> dict:
     """The reference's run from read files to its out/ directory, in one call: refs = the -ref FASTA files, reads = one reads file
@@ -1243,7 +1334,10 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
     fastx, other, denovo = (min_id, min_cov) for aligned_denovo.*, otu_map = (min_id, min_cov), paired_in / paired_out / out2 / sout,
     zip_out (every report file gzip-compressed on the device, ".gz" appended; otu_map.txt and aligned.log stay plain).  bam: also
     aligned.bam, the rows of aligned.sam (with or without sam) as BAM records in BGZF blocks written on the device
-    (Aligner.bam_header, format_placed_into(bam=True)) and the BGZF EOF block; it is BGZF whatever zip_out says.
+    (Aligner.bam_header, format_placed_into(bam=True)) and the BGZF EOF block; it is BGZF whatever zip_out says.  bam_sorted (implies
+    bam): aligned.bam sorted by coordinate, with SO:coordinate in its header, and its index aligned.bam.bai: each batch's records go
+    as one sorted run (Aligner.bam_sort_add) to the part file .part_bamsort, and after the stream Aligner.bam_sort_finish writes the
+    sorted records in windows of BAM_SORT_WINDOW bytes (seconds["bam_sort"]).
     Files are written by a writer thread while the caller's thread makes, runs and formats the next batch (the library calls release
     the GIL); two output buffers alternate between them, and the streams go from those buffers to the files without a copy.  The
     read files and the SAM / BLAST rows of the first (index, part) group are appended to their final files as they come.  With
@@ -1272,10 +1366,13 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
         rest.blast = 0
     pw_opts = report_opts(blast="0", paired_in=paired_in, paired_out=paired_out)
     bam_opts = report_opts(sam=True, paired_in=paired_in, paired_out=paired_out)
+    bam = bam or bam_sorted
     feed = "two_files" if mates else "one_file" if (paired_in or paired_out) else None
     with_denovo = otu_map is not None or o.denovo
     sec = dict.fromkeys(("count", "index", "stream", "produce", "run", "place", "format", "writer", "writer_wait", "caller_wait", "parts",
                          "finish"), 0.0)
+    if bam_sorted:
+        sec["bam_sort"] = 0.0
     os.makedirs(out_dir, exist_ok=True)
     al = Aligner(device)
     files, parts = {}, {}
@@ -1323,7 +1420,16 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
             fh = open_file("aligned.sam")
             fh.write(al.gzip(head) if zip_out else head)
             dest += [(g, fh if g == 0 else part_file(f"sam_{g}")) for g in range(G)]
-        if bam:
+        run_starts, bam_header_bytes = [], 0
+        if bam_sorted:   # the batches' sorted runs go to a part file; the windows are written after the stream
+            fh = files["aligned.bam"] = open(os.path.join(out_dir, "aligned.bam"), "wb")
+            hb = al.bam_header(head.replace(b"\tSO:unsorted\n", b"\tSO:coordinate\n", 1))
+            fh.write(hb)
+            bam_header_bytes = len(hb)
+            files["aligned.bam.bai"] = open(os.path.join(out_dir, "aligned.bam.bai"), "wb")
+            bam_dest = [(0, part_file("bamsort"))]
+            al.bam_sort_begin()
+        elif bam:
             fh = files["aligned.bam"] = open(os.path.join(out_dir, "aligned.bam"), "wb")
             fh.write(al.bam_header(head))
             bam_dest = [(g, fh if g == 0 else part_file(f"bam_{g}")) for g in range(G)]
@@ -1347,6 +1453,7 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
 
         writer = _FileWriter()
         n_reads, num_aligned, n_batches = 0, 0, 0
+        run_end = 0   # bytes of the runs in .part_bamsort so far
         matched = np.zeros(max(1, len(refs)), np.uint64)
         dn = dict.fromkeys(DENOVO_TOTALS, 0)
         dn_min, dn_paired = otu_map or denovo or (0, 0), bool(paired_in or paired_out) or feed is not None
@@ -1375,7 +1482,12 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
             if pw_dest:
                 slot[1], so = al.format_placed_into(pw_opts, slot[1], zip_out, pairwise=True)
                 jobs.append((slot[1], so, pw_dest))
-            if bam_dest:
+            if bam_sorted:
+                slot[2], nb = al.bam_sort_add(bam_opts, slot[2])
+                run_starts.append(run_end)
+                run_end += nb
+                jobs.append((slot[2], np.array([0, nb], np.uint64), bam_dest))
+            elif bam_dest:
                 slot[2], so = al.format_placed_into(bam_opts, slot[2], bam=True)
                 jobs.append((slot[2], so, bam_dest))
             if otu_map is not None:
@@ -1404,6 +1516,13 @@ def run_files(refs, reads, out_dir, params: Params | None = None, *, gumbel, min
                 if fh is not None:
                     fh.seek(0)
                     shutil.copyfileobj(fh, files[name], 1 << 24)
+        if bam_sorted:
+            t2 = time.perf_counter()
+            runs = parts["bamsort"]
+            runs.flush()
+            bai = al.bam_sort_finish(runs, run_starts, files["aligned.bam"], bam_header_bytes)
+            files["aligned.bam.bai"].write(bai)
+            sec["bam_sort"] = time.perf_counter() - t2
         if bam:
             files["aligned.bam"].write(BGZF_EOF)
         paths = []

@@ -16,6 +16,7 @@
 #include "smr_decode.cuh"
 #include "smr_report.cuh"
 #include "smr_otu.cuh"
+#include "smr_bamsort.cuh"
 #include "smr_inflate.cuh"
 #include "smr_stream.cuh"
 #include "smr_deflate.cuh"
@@ -207,6 +208,21 @@ struct smr_ctx {
     double t[3] = {0, 0, 0};
   } otu;
   struct { DevBuf read, tot; } dn;   // smr_denovo_stats: per-read counters, totals
+  // coordinate-sorted BAM (smr_bamsort.cuh), smr_bam_sort_begin .. smr_bam_sort_index
+  struct BamSort {
+    bool active = false, planned = false; uint64_t gen = 0;
+    std::vector<uint64_t> lin_off;                 // the linear index table: reference k's 16 kb windows at [lin_off[k], lin_off[k + 1])
+    std::vector<uint64_t> run_rec, run_bytes;      // each run's first record (accumulator order) and first byte, and the totals
+    DevBuf key, size;                              // the accumulator: each record's key and size, run after run (12 B per record)
+    DevBuf ord, bkey, sbkey, bperm, ssz, soff, doff, gat;   // scratch of add
+    DevBuf pperm, pkey, psz, pdoff, csz, coff;                // plan: the sorted order and the offsets of both orders
+    DevBuf runs, adj, stage, win, wsoff, vb, ve, rb, head, pid, piece, bso, lin, linoff, err;   // window
+    std::vector<uint64_t> pdoff_h;                 // plan: the byte offset of each record in sorted order, and the total
+    std::vector<uint64_t> win_rec;                 // plan: each window's first record in sorted order, and the total
+    std::vector<uint64_t> ranges_h;                // plan: each window's [lo, hi) of each run, as smr_bam_sort_plan returns them
+    uint64_t header_bytes = 0, next = 0, coffset = 0;   // window: the next one, and the compressed offset of its first block
+    std::vector<BamPiece> pieces;                  // window: the chunk pieces of the windows so far, in file order
+  } bs;
   // timings
   std::vector<cudaEvent_t> ev;
   RunTimes t_run;   // the last run, and the retries of its download
@@ -2098,12 +2114,13 @@ void gzip_streams(smr_ctx* ctx, const uint8_t* in, const std::vector<uint64_t>& 
   CK(cudaStreamSynchronize(ctx->stream));
 }
 
-// pairwise: smr_format_blast_pairwise[_gz], the pairwise BLAST rows alone (-blast 0), one stream per group; bam:
-// smr_format_bam_placed, the SAM rows as BAM records in BGZF blocks, one stream per group; otherwise the streams of
-// smr_format_reports[_gz].  All share the routing (the skip of empty reads), the row order and the scans.
-void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
-                         const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
-                         char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise, bool dev = false, bool bam = false) {
+// The rows of a report-side format call written uncompressed into ctx->r.out (the first half of format_reports_impl): checks,
+// prologue, routing (the skip of empty reads), row order, the size passes, scans and write passes, and the BAM refusals.  Returns the
+// stream offsets (nso = 2 * groups + read files + 1 of them); e[0], e[1] are recorded by the prologue.  Without gz or bam, so_out gets
+// the offsets and a buffer smaller than the rows fails with SMR_ERR_CAPACITY before the writes.
+std::vector<uint64_t> rpt_write_rows(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
+                                     const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                                     char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise, bool dev, bool bam, cudaEvent_t* e) {
   const bool mates = o->mates || (!text && ctx->res.mates);   // the resident batch of a mate stream is mates
   const bool paired = o->paired_in || o->paired_out || mates;
   if (pairwise) {   // -blast '0 cigar' is refused by the reference too (options.cpp:584-588)
@@ -2132,7 +2149,6 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
     }
   const std::vector<RptGroup> hg = rpt_groups(ctx, o->sam || o->blast, o->blast);
   const uint32_t G = (uint32_t)hg.size(), nso = 2 * G + nfx + 1;
-  cudaEvent_t* e = events(ctx, 4);
   RptArgs a = rpt_prologue(ctx, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, hg, e, dev);
   const uint64_t N = a.nslots;
   const int grid = ctx->sm_count * 8;
@@ -2216,6 +2232,24 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
     CK(cudaMemcpyAsync(&hbad, bad, 4, cudaMemcpyDeviceToHost, ctx->stream));
     CK(cudaStreamSynchronize(ctx->stream));
     rpt_check_bam(err, hbad);
+  }
+  return hso;
+}
+
+// pairwise: smr_format_blast_pairwise[_gz], the pairwise BLAST rows alone (-blast 0), one stream per group; bam:
+// smr_format_bam_placed, the SAM rows as BAM records in BGZF blocks, one stream per group; otherwise the streams of
+// smr_format_reports[_gz].  All share the routing (the skip of empty reads), the row order and the scans (rpt_write_rows).
+void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* text, uint64_t nbytes, const smr_read_result* results,
+                         const smr_aln* alns, const uint32_t* cigar, uint64_t cigar_words, const smr_aln_stats* stats, uint32_t nreads,
+                         char* out, uint64_t cap, uint64_t* so_out, bool gz, bool pairwise, bool dev = false, bool bam = false) {
+  cudaEvent_t* e = events(ctx, 4);
+  const std::vector<uint64_t> hso = rpt_write_rows(ctx, o, text, nbytes, results, alns, cigar, cigar_words, stats, nreads, out, cap, so_out, gz,
+                                                   pairwise, dev, bam, e);
+  auto& S = ctx->r;
+  const uint32_t nso = (uint32_t)hso.size(), G = bam || pairwise ? (nso - 1) / 2 : 0;
+  const uint32_t s0 = pairwise ? G : 0;
+  const uint64_t total = hso[nso - 1];
+  if (bam) {   // each group's records cut into BGZF blocks
     std::vector<uint64_t> sb, se;
     std::vector<size_t> gb(G + 1);   // the first block of each group
     for (uint32_t g = 0; g < G; ++g) { gb[g] = sb.size(); bgzf_blocks(hso[g], hso[g + 1], sb, se); }
@@ -2233,6 +2267,309 @@ void format_reports_impl(smr_ctx* ctx, const smr_report_opts* o, const char* tex
     CK(cudaStreamSynchronize(ctx->stream));
   }
   set_rpt_times(ctx, e);
+}
+
+// ---------------------------------------------------------------------------------------------------------------------
+// Coordinate-sorted BAM and its BAI index (smr_bamsort.cuh)
+// ---------------------------------------------------------------------------------------------------------------------
+void bam_sort_open(smr_ctx* ctx) {
+  if (!ctx->bs.active) fail(SMR_ERR_ARG, "no open sorted BAM: call smr_bam_sort_begin first");
+  if (ctx->bs.gen != ctx->parts_gen)
+    fail(SMR_ERR_ARG, "an index part was loaded or its report ids were set after smr_bam_sort_begin: begin the sorted BAM again");
+}
+
+// the bits of a sort key: pos + 1 and the strand in the low 32, the refID above
+int bam_sort_bits(const smr_ctx* ctx) {
+  int b = 32;
+  while ((1ull << (b - 32)) < ctx->bs.lin_off.size()) ++b;
+  return b;
+}
+
+void bam_sort_begin_impl(smr_ctx* ctx) {
+  auto& B = ctx->bs;
+  B.active = false;
+  const std::vector<RptGroup> hg = rpt_groups(ctx, true, false);
+  const std::vector<const Part*> gp = report_groups(ctx);
+  B.lin_off.assign(1, 0);
+  for (size_t g = 0; g < gp.size(); ++g) {
+    std::vector<uint32_t> roff((size_t)hg[g].nref + 1);
+    CK(cudaMemcpy(roff.data(), hg[g].ref_off, roff.size() * 4, cudaMemcpyDeviceToHost));
+    for (uint32_t k = 0; k < hg[g].nref; ++k) {
+      const uint64_t len = roff[k + 1] - roff[k];
+      if (len >= (1ull << 29))
+        fail(SMR_ERR_UNSUPPORTED, "sorted BAM: reference " + gp[g]->h_rnames[k] + " (refID " + std::to_string(hg[g].ref_base + k) + ") has " +
+                                      std::to_string(len) + " bases, and a BAI index addresses fewer than 2^29");
+      B.lin_off.push_back(B.lin_off.back() + (len + 16383) / 16384);
+    }
+  }
+  B.run_rec.assign(1, 0);
+  B.run_bytes.assign(1, 0);
+  B.planned = false;
+  B.pieces.clear();
+  B.gen = ctx->parts_gen;
+  B.active = true;
+}
+
+// the placed batch's BAM records sorted into a run, into out; the run's keys and sizes appended to the accumulator
+void bam_sort_add_impl(smr_ctx* ctx, const smr_report_opts* o, char* out, uint64_t cap, uint64_t* nbytes) {
+  auto& B = ctx->bs;
+  bam_sort_open(ctx);
+  const PlacedArrays p = placed_of(ctx, "smr_bam_sort_add_placed", true);
+  cudaEvent_t* e = events(ctx, 4);
+  const std::vector<uint64_t> hso = rpt_write_rows(ctx, o, nullptr, 0, p.res, p.aln, p.cig, p.cig_words, p.st, p.n, nullptr, 0, nullptr, false,
+                                                   false, true, true, e);
+  const uint64_t total = hso.back();
+  const uint32_t G = (uint32_t)(hso.size() - 1) / 2;
+  *nbytes = total;
+  if (total && (!out || cap < total)) fail(SMR_ERR_CAPACITY, "output buffer too small: *nbytes holds the size of the run");
+  uint64_t n = 0;
+  CK(cudaMemcpy(&n, (const uint64_t*)ctx->r.first.p + G, 8, cudaMemcpyDeviceToHost));
+  const uint64_t at = B.run_rec.back();
+  if (at + n >= (1ull << 31)) fail(SMR_ERR_CAPACITY, "sorted BAM of 2^31 records or more");
+  ensure_keep(ctx, B.key, (at + n) * 8, at * 8);
+  ensure_keep(ctx, B.size, (at + n) * 4, at * 4);
+  const int grid = ctx->sm_count * 8;
+  if (n) {
+    const uint8_t* rec = (const uint8_t*)ctx->r.out.p;
+    const uint64_t* off = (const uint64_t*)ctx->r.off.p;
+    uint64_t* bkey = ensure<uint64_t>(B.bkey, n * 8);
+    uint64_t* sbkey = ensure<uint64_t>(B.sbkey, n * 8);
+    uint32_t* ord = ensure<uint32_t>(B.ord, n * 4);
+    uint32_t* perm = ensure<uint32_t>(B.bperm, n * 4);
+    uint64_t* ssz = ensure<uint64_t>(B.ssz, (n + 1) * 8);
+    uint64_t* soff = ensure<uint64_t>(B.soff, n * 8);
+    uint64_t* doff = ensure<uint64_t>(B.doff, (n + 1) * 8);
+    uint8_t* gat = ensure<uint8_t>(B.gat, total);
+    bsort_key_kernel<<<grid, 256, 0, ctx->stream>>>(rec, off, n, bkey, ord);
+    const int bits = bam_sort_bits(ctx);
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)bkey, sbkey, (const uint32_t*)ord, perm, (int)n, 0, bits, ctx->stream); });
+    bsort_run_order_kernel<<<grid, 256, 0, ctx->stream>>>(perm, sbkey, off, n, ssz, soff, (uint64_t*)B.key.p, (uint32_t*)B.size.p, at);
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, (const uint64_t*)ssz, doff, (int)(n + 1), ctx->stream); });
+    bsort_gather_kernel<<<grid, 256, 0, ctx->stream>>>(rec, total, soff, doff, n, gat, false, nullptr);
+    CK(cudaGetLastError());
+  }
+  CK(cudaEventRecord(e[2], ctx->stream));
+  if (total) CK(cudaMemcpyAsync(out, B.gat.p, total, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e[3], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  B.run_rec.push_back(at + n);
+  B.run_bytes.push_back(B.run_bytes.back() + total);
+  B.planned = false;
+  set_rpt_times(ctx, e);
+}
+
+// one stable sort of every run's records, the windows cut from it and each window's byte range of each run
+void bam_sort_plan_impl(smr_ctx* ctx, uint64_t window_bytes, uint64_t header_bytes, uint64_t* ranges, uint64_t cap, uint64_t* n_windows) {
+  auto& B = ctx->bs;
+  bam_sort_open(ctx);
+  if (!window_bytes) fail(SMR_ERR_ARG, "sorted BAM: window_bytes must be at least 1");
+  B.planned = false;
+  const uint64_t M = B.run_rec.back();
+  const uint32_t R = (uint32_t)B.run_rec.size() - 1;
+  const int grid = ctx->sm_count * 8;
+  B.pdoff_h.assign(M + 1, 0);
+  std::vector<uint32_t> perm(M);
+  std::vector<uint64_t> coff(M + 1, 0);
+  if (M) {
+    uint32_t* ord = ensure<uint32_t>(B.ord, M * 4);
+    uint32_t* pperm = ensure<uint32_t>(B.pperm, M * 4);
+    uint64_t* pkey = ensure<uint64_t>(B.pkey, M * 8);
+    uint64_t* psz = ensure<uint64_t>(B.psz, (M + 1) * 8);
+    uint64_t* csz = ensure<uint64_t>(B.csz, (M + 1) * 8);
+    uint64_t* pdoff = ensure<uint64_t>(B.pdoff, (M + 1) * 8);
+    uint64_t* dcoff = ensure<uint64_t>(B.coff, (M + 1) * 8);
+    bsort_iota_kernel<<<grid, 256, 0, ctx->stream>>>(ord, M);
+    const int bits = bam_sort_bits(ctx);
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceRadixSort::SortPairs(t, b, (const uint64_t*)B.key.p, pkey, (const uint32_t*)ord, pperm, (int)M, 0, bits, ctx->stream); });
+    bsort_plan_sizes_kernel<<<grid, 256, 0, ctx->stream>>>(pperm, (const uint32_t*)B.size.p, M, psz, csz);
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, (const uint64_t*)psz, pdoff, (int)(M + 1), ctx->stream); });
+    cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, (const uint64_t*)csz, dcoff, (int)(M + 1), ctx->stream); });
+    CK(cudaGetLastError());
+    CK(cudaMemcpyAsync(B.pdoff_h.data(), pdoff, (M + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(perm.data(), pperm, M * 4, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaMemcpyAsync(coff.data(), dcoff, (M + 1) * 8, cudaMemcpyDeviceToHost, ctx->stream));
+    CK(cudaStreamSynchronize(ctx->stream));
+  }
+  // greedy windows of whole records, each at most window_bytes unless one record is larger
+  B.win_rec.assign(1, 0);
+  for (uint64_t t = 0; t < M;) {
+    uint64_t t1 = (uint64_t)(std::upper_bound(B.pdoff_h.begin() + t + 1, B.pdoff_h.end(), B.pdoff_h[t] + window_bytes) - B.pdoff_h.begin()) - 1;
+    if (t1 <= t) t1 = t + 1;
+    B.win_rec.push_back(t1);
+    t = t1;
+  }
+  const uint64_t nw = B.win_rec.size() - 1;
+  *n_windows = nw;
+  const uint64_t need = nw * R * 2;
+  if (need && (!ranges || cap < need)) fail(SMR_ERR_CAPACITY, "ranges too small: it takes n_windows * runs * 2 entries (*n_windows is set)");
+  // a run's records in a window are one range of it, since the run is sorted and the sort stable
+  std::vector<uint32_t> run_of(M);
+  for (uint32_t r = 0; r < R; ++r) std::fill(run_of.begin() + B.run_rec[r], run_of.begin() + B.run_rec[r + 1], r);
+  for (uint64_t w = 0; w < nw; ++w) {
+    uint64_t* rg = ranges + w * R * 2;
+    for (uint32_t r = 0; r < R; ++r) { rg[2 * r] = ~0ull; rg[2 * r + 1] = 0; }
+    for (uint64_t t = B.win_rec[w]; t < B.win_rec[w + 1]; ++t) {
+      const uint32_t o = perm[t], r = run_of[o];
+      const uint64_t b = coff[o] - B.run_bytes[r];
+      rg[2 * r] = std::min(rg[2 * r], b);
+      rg[2 * r + 1] = std::max(rg[2 * r + 1], b + coff[o + 1] - coff[o]);
+    }
+    for (uint32_t r = 0; r < R; ++r) if (rg[2 * r] == ~0ull) rg[2 * r] = 0;
+  }
+  B.ranges_h.assign(ranges, ranges + need);
+  // the window pass's tables: the run starts, the linear index minima (all ones: no record yet)
+  upload_async(ctx, B.runs, B.run_rec.data(), B.run_rec.size());
+  upload_async(ctx, B.linoff, B.lin_off.data(), B.lin_off.size());
+  ensure(B.lin, B.lin_off.back() * 8 + 8);
+  CK(cudaMemsetAsync(B.lin.p, 0xFF, B.lin_off.back() * 8 + 8, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  B.header_bytes = header_bytes;
+  B.coffset = header_bytes;
+  B.next = 0;
+  B.pieces.clear();
+  B.planned = true;
+}
+
+void bam_sort_planned(smr_ctx* ctx) {
+  bam_sort_open(ctx);
+  if (!ctx->bs.planned) fail(SMR_ERR_ARG, "sorted BAM: no plan of the runs added: call smr_bam_sort_plan first");
+}
+
+// window w: the staged ranges gathered into sorted order, compressed into BGZF blocks, and its index pieces and minima
+void bam_sort_window_impl(smr_ctx* ctx, uint64_t w, const void* staged, uint64_t nbytes, char* out, uint64_t cap, uint64_t* out_bytes) {
+  auto& B = ctx->bs;
+  bam_sort_planned(ctx);
+  const uint64_t nw = B.win_rec.size() - 1;
+  if (w != B.next || w >= nw)
+    fail(SMR_ERR_ARG, "sorted BAM: window " + std::to_string(w) + " out of order: the windows come in order, and the next is " + std::to_string(B.next) +
+                          " of " + std::to_string(nw));
+  const uint64_t t0 = B.win_rec[w], n = B.win_rec[w + 1] - t0;
+  const uint64_t wbytes = B.pdoff_h[t0 + n] - B.pdoff_h[t0];
+  if (nbytes != wbytes)
+    fail(SMR_ERR_ARG, "sorted BAM: window " + std::to_string(w) + " is " + std::to_string(wbytes) + " bytes, and " + std::to_string(nbytes) + " were staged");
+  if (!staged) fail(SMR_ERR_ARG, "sorted BAM: no staged bytes");
+  const uint32_t R = (uint32_t)B.run_rec.size() - 1;
+  std::vector<int64_t> adj(R);
+  for (uint64_t r = 0, base = 0; r < R; ++r) {   // run r's range sits at `base` in the staged bytes
+    const uint64_t lo = B.ranges_h[(w * R + r) * 2], hi = B.ranges_h[(w * R + r) * 2 + 1];
+    adj[r] = (int64_t)base - (int64_t)B.run_bytes[r] - (int64_t)lo;
+    base += hi - lo;
+  }
+  cudaEvent_t* e = events(ctx, 5);
+  CK(cudaEventRecord(e[0], ctx->stream));
+  upload_async(ctx, B.stage, (const uint8_t*)staged, nbytes);
+  upload_async(ctx, B.adj, adj.data(), R);
+  CK(cudaEventRecord(e[1], ctx->stream));
+  const int grid = ctx->sm_count * 8;
+  const uint64_t* doff = (const uint64_t*)B.pdoff.p + t0;
+  uint64_t* soff = ensure<uint64_t>(B.wsoff, n * 8);
+  uint8_t* win = ensure<uint8_t>(B.win, wbytes + 8);
+  uint32_t* err = ensure<uint32_t>(B.err, 4);
+  CK(cudaMemsetAsync(err, 0, 4, ctx->stream));
+  CK(cudaMemsetAsync(win + wbytes, 0, 8, ctx->stream));
+  bsort_window_src_kernel<<<grid, 256, 0, ctx->stream>>>((const uint32_t*)B.pperm.p, (const uint64_t*)B.coff.p, (const uint64_t*)B.runs.p, R,
+                                                         (const int64_t*)B.adj.p, t0, n, soff);
+  bsort_gather_kernel<<<grid, 256, 0, ctx->stream>>>((const uint8_t*)B.stage.p, nbytes, soff, doff, n, win, true, err);
+  CK(cudaGetLastError());
+  uint32_t herr = 0;
+  CK(cudaMemcpyAsync(&herr, err, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  if (herr) fail(SMR_ERR_ARG, "sorted BAM: a staged record's block_size disagrees with the runs added (stage window " + std::to_string(w) + "'s ranges of the runs, in run order)");
+  std::vector<uint64_t> sb, se;
+  bgzf_blocks(0, wbytes, sb, se);
+  const uint32_t ns = (uint32_t)sb.size();
+  std::vector<uint64_t> so(ns + 1, 0);
+  {
+    const auto put_size = on_exit([&] { *out_bytes = so.back(); });   // a buffer too small fails, and names the size needed
+    gzip_streams(ctx, win, sb, se, out, cap, so.data(), e[2], e[3], kBgzfHeader);
+  }
+  // the index pass over the compressed window
+  upload_async(ctx, B.bso, so.data(), so.size());
+  uint64_t* vb = ensure<uint64_t>(B.vb, n * 8);
+  uint64_t* ve = ensure<uint64_t>(B.ve, n * 8);
+  uint64_t* rb = ensure<uint64_t>(B.rb, n * 8);
+  uint32_t* head = ensure<uint32_t>(B.head, (n + 1) * 4);
+  uint32_t* pid = ensure<uint32_t>(B.pid, (n + 1) * 4);
+  bsort_index_kernel<kBgzfBlock><<<grid, 256, 0, ctx->stream>>>(win, doff, n, (const uint64_t*)B.bso.p, ns, B.coffset, (const uint64_t*)B.linoff.p,
+                                                                (unsigned long long*)B.lin.p, vb, ve, rb, head);
+  cub_run(ctx->cub_tmp, [&](void* t, size_t& b) { return cub::DeviceScan::ExclusiveSum(t, b, (const uint32_t*)head, pid, (int)(n + 1), ctx->stream); });
+  uint32_t np = 0;
+  CK(cudaMemcpyAsync(&np, pid + n, 4, cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  BamPiece* pc = ensure<BamPiece>(B.piece, (size_t)np * sizeof(BamPiece));
+  bsort_pieces_kernel<<<grid, 256, 0, ctx->stream>>>(vb, ve, rb, head, pid, n, pc);
+  CK(cudaGetLastError());
+  const size_t at = B.pieces.size();
+  B.pieces.resize(at + np);
+  CK(cudaMemcpyAsync(B.pieces.data() + at, pc, (size_t)np * sizeof(BamPiece), cudaMemcpyDeviceToHost, ctx->stream));
+  CK(cudaEventRecord(e[4], ctx->stream));
+  CK(cudaStreamSynchronize(ctx->stream));
+  B.coffset += so[ns];
+  ++B.next;
+  ctx->t_rpt[0] = elapsed_ms(e[0], e[1]);
+  ctx->t_rpt[1] = elapsed_ms(e[1], e[2]) + elapsed_ms(e[3], e[4]);
+  ctx->t_rpt[2] = elapsed_ms(e[2], e[3]);
+}
+
+// the BAI bytes (SAMv1 5.2) from the pieces and the linear minima of every window; closes the sorted BAM
+void bam_sort_index_impl(smr_ctx* ctx, char* out, uint64_t cap, uint64_t* nbytes) {
+  auto& B = ctx->bs;
+  bam_sort_planned(ctx);
+  const uint64_t nw = B.win_rec.size() - 1;
+  if (B.next != nw)
+    fail(SMR_ERR_ARG, "sorted BAM: the index comes after the last window: " + std::to_string(B.next) + " of " + std::to_string(nw) + " windows done");
+  const uint32_t nref = (uint32_t)B.lin_off.size() - 1;
+  std::vector<uint64_t> lin(B.lin_off.back());
+  if (!lin.empty()) CK(cudaMemcpy(lin.data(), B.lin.p, lin.size() * 8, cudaMemcpyDeviceToHost));
+  std::vector<uint8_t> h;
+  auto le32 = [&](uint32_t v) { for (int k = 0; k < 4; ++k) h.push_back((uint8_t)(v >> (8 * k))); };
+  auto le64 = [&](uint64_t v) { for (int k = 0; k < 8; ++k) h.push_back((uint8_t)(v >> (8 * k))); };
+  h.insert(h.end(), {'B', 'A', 'I', 1});
+  le32(nref);
+  size_t p = 0;   // the pieces are in file order, so in refID order
+  for (uint32_t k = 0; k < nref; ++k) {
+    std::vector<std::pair<uint32_t, std::vector<std::pair<uint64_t, uint64_t>>>> bins;   // bin -> merged chunks in ascending vbeg
+    std::vector<std::pair<uint32_t, size_t>> order;
+    uint64_t n_mapped = 0, first = ~0ull, last = 0;
+    const size_t p0 = p;
+    for (; p < B.pieces.size() && (B.pieces[p].refbin >> 32) == k; ++p) {
+      const BamPiece& pc = B.pieces[p];
+      order.emplace_back((uint32_t)pc.refbin, p);
+      n_mapped += pc.last - pc.first + 1;
+      first = std::min(first, pc.vbeg);
+      last = std::max(last, pc.vend);
+    }
+    std::stable_sort(order.begin(), order.end(), [](const auto& a, const auto& b) { return a.first < b.first; });
+    for (const auto& [bin, i] : order) {
+      const BamPiece& pc = B.pieces[i];
+      if (bins.empty() || bins.back().first != bin) bins.push_back({bin, {}});
+      auto& ch = bins.back().second;
+      if (!ch.empty() && fmt::bam_chunks_merge(ch.back().second, pc.vbeg)) ch.back().second = pc.vend;
+      else ch.emplace_back(pc.vbeg, pc.vend);
+    }
+    const bool any = p > p0;
+    le32((uint32_t)bins.size() + (any ? 1 : 0));
+    for (const auto& [bin, ch] : bins) {
+      le32(bin);
+      le32((uint32_t)ch.size());
+      for (const auto& c : ch) { le64(c.first); le64(c.second); }
+    }
+    if (any) { le32(37450); le32(2); le64(first); le64(last); le64(n_mapped); le64(0); }
+    // the linear index: the last window a record overlaps bounds it; an empty window takes the one before, or the first that is set
+    const uint64_t l0 = B.lin_off[k], l1 = B.lin_off[k + 1];
+    uint64_t n_intv = 0, lead = ~0ull;
+    for (uint64_t i = l0; i < l1; ++i) if (lin[i] != ~0ull) { n_intv = i - l0 + 1; if (lead == ~0ull) lead = lin[i]; }
+    le32((uint32_t)n_intv);
+    for (uint64_t i = 0, cur = lead; i < n_intv; ++i) {
+      if (lin[l0 + i] != ~0ull) cur = lin[l0 + i];
+      le64(cur);
+    }
+  }
+  le64(0);   // n_no_coor
+  *nbytes = h.size();
+  if (!out || cap < h.size()) fail(SMR_ERR_CAPACITY, "output buffer too small: *nbytes holds the size of the index");
+  memcpy(out, h.data(), h.size());
+  B.active = false;
 }
 
 // ---------------------------------------------------------------------------------------------------------------------
@@ -3213,6 +3550,45 @@ int smr_bam_header(smr_ctx* ctx, const char* text, uint64_t nbytes, char* out, u
     gzip_streams(ctx, (const uint8_t*)ctx->z.in.p, sb, se, out, cap, so.data(), e[2], e[3], kBgzfHeader);
   }
   set_rpt_times(ctx, e);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_bam_sort_begin(smr_ctx* ctx) try {
+  if (!ctx) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  bam_sort_begin_impl(ctx);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_bam_sort_add_placed(smr_ctx* ctx, const smr_report_opts* opts, char* out, uint64_t cap, uint64_t* nbytes) try {
+  if (!ctx || !opts || !nbytes) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  *nbytes = 0;
+  bam_sort_add_impl(ctx, opts, out, cap, nbytes);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_bam_sort_plan(smr_ctx* ctx, uint64_t window_bytes, uint64_t header_bytes, uint64_t* ranges, uint64_t cap, uint64_t* n_windows) try {
+  if (!ctx || !n_windows) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  *n_windows = 0;
+  bam_sort_plan_impl(ctx, window_bytes, header_bytes, ranges, cap, n_windows);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_bam_sort_window(smr_ctx* ctx, uint64_t w, const void* staged, uint64_t nbytes, char* out, uint64_t cap, uint64_t* out_bytes) try {
+  if (!ctx || !out_bytes) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  *out_bytes = 0;
+  bam_sort_window_impl(ctx, w, staged, nbytes, out, cap, out_bytes);
+  return SMR_OK;
+} SMR_CATCH(ctx)
+
+int smr_bam_sort_index(smr_ctx* ctx, char* out, uint64_t cap, uint64_t* nbytes) try {
+  if (!ctx || !nbytes) return SMR_ERR_ARG;
+  CK(cudaSetDevice(ctx->device));
+  *nbytes = 0;
+  bam_sort_index_impl(ctx, out, cap, nbytes);
   return SMR_OK;
 } SMR_CATCH(ctx)
 

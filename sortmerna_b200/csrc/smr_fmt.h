@@ -180,5 +180,15 @@ __host__ __device__ inline uint32_t bam_nt4(char c) { return c == 'A' ? 1 : c ==
 __host__ __device__ inline uint32_t bam_int_bytes(uint64_t v) { return v <= 0xFF ? 1 : v <= 0xFFFF ? 2 : 4; }
 __host__ __device__ inline char bam_int_type(uint32_t bytes) { return bytes == 1 ? 'C' : bytes == 2 ? 'S' : 'I'; }
 
+// The coordinate-sorted BAM (smr_bamsort.cuh; tests/bamsort_check.cpp prints these for the host test)
+// samtools' coordinate key of a record: refID, then pos + 1, then the reverse-strand bit
+__host__ __device__ inline uint64_t bam_sort_key(int32_t ref_id, int32_t pos, uint32_t flag) {
+  return (uint64_t)(uint32_t)ref_id << 32 | (uint64_t)(uint32_t)(pos + 1) << 1 | ((flag & 16) ? 1u : 0u);
+}
+// BGZF's virtual offset: the compressed offset of a block, and the offset inside its uncompressed bytes
+__host__ __device__ inline uint64_t bam_voffset(uint64_t coffset, uint32_t in_block) { return coffset << 16 | in_block; }
+// htslib's merge_chunks rule: a chunk that starts in the block where the previous one (in ascending vbeg) ends joins it
+__host__ __device__ inline bool bam_chunks_merge(uint64_t prev_vend, uint64_t vbeg) { return prev_vend >> 16 == vbeg >> 16; }
+
 }  // namespace fmt
 }  // namespace smr
